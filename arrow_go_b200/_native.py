@@ -44,6 +44,22 @@ def span_table(spans):
     return arr
 
 
+class PqPage(C.Structure):
+    """ag_pq_page: one Parquet page of a batched decode (byte offset, byte length, output slots, first output slot)."""
+    _fields_ = [("data", C.c_int64), ("len", C.c_int64), ("num_values", C.c_int64), ("out", C.c_int64)]
+
+
+PQ_LEVELS_V2_RLE, PQ_LEVELS_V1_RLE, PQ_LEVELS_BIT_PACKED = 0, 1, 2
+
+
+def page_table(pages):
+    """[(data, len, num_values, out), ...] -> ctypes array of ag_pq_page."""
+    arr = (PqPage * max(len(pages), 1))()
+    for k, (d, ln, nv, o) in enumerate(pages):
+        arr[k].data, arr[k].len, arr[k].num_values, arr[k].out = d, ln, nv, o
+    return arr
+
+
 class NativeError(RuntimeError):
     """A C-ABI call returned a non-zero ag_status."""
 
@@ -179,6 +195,12 @@ _SIGS = {
     "ag_parquet_bytes_to_bools_dev": [_p, _i64, _p, _i64, _p],
     "ag_parquet_def_levels_to_bitmap": [_p, _i64, _i, _i, _p, _i64, _i64, _pi64, _pi64],
     "ag_parquet_def_levels_to_bitmap_dev": [_p, _i64, _i, _i, _p, _i64, _i64, _p, _p],
+    "ag_parquet_levels_decode": [_i, _i, _p, _p, _i64, _p, _p],
+    "ag_parquet_levels_decode_dev": [_i, _i, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_dict_decode": [_i, _p, _i64, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_dict_decode_dev": [_i, _p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p],
+    "ag_parquet_plain_decode_spaced": [_i, _p, _p, _i64, _p, _p],
+    "ag_parquet_plain_decode_spaced_dev": [_i, _p, _p, _i64, _p, _p, _p],
     # parity helpers
     "ag_checksum64_dev": [_p, _sz, _p, _p],
     "ag_generate_dev": [_i, _u64, _i64, _i64, _p, _sz, _p],

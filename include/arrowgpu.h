@@ -569,6 +569,67 @@ ag_status ag_parquet_def_levels_to_bitmap_dev(const int16_t* d_def_levels, int64
                                               int64_t* d_counts, ag_stream_t s);
 
 /* ================================================================================= *
+ * Parquet page decode — a batch of pages in one call.  The page payloads (decompressed) sit in one buffer `data`;
+ *   `pages` is a HOST array of descriptors in both flavours (like ag_span3):
+ *     data        byte offset of the page's stream in `data`
+ *     len         bytes available to the stream
+ *     num_values  output slots of the page (valid + null slots for a spaced decode)
+ *     out         element offset of the page's first slot in `out`; also its bit offset in `valid`
+ *   Pages may come in any order and their outputs need not be contiguous.  Runs follow RleDecoder.Next / GetBatch
+ *   (parquet/internal/utils/rle.go:123-169,203-239).  A stream that ends cleanly before num_values is not an
+ *   error: decoded[i] says how many slots page i wrote (GetBatch's `read`); slots past it are left untouched.
+ *   Differences from the reference (DESIGN §2):
+ *     - bit widths 0..32 for indices, 0..16 for levels; anything else is AG_ERR_INVALID (the reference rejects
+ *       only widths >= 64 and truncates a repeated value wider than 32 bits);
+ *     - a truncated literal run, a run count of 0, a varint that runs past the stream / 5 bytes / int32 counts
+ *       and a repeated value cut off by the end of the stream are AG_ERR_INVALID naming the page (the reference's
+ *       Next() returns false on all but the first).  A truncated literal run still delivers its whole 32-value
+ *       groups that are present (bit_reader_test.go:513-566);
+ *     - a dictionary index >= dict_len is AG_ERR_INVALID "invalid index values found for dictionary converter"
+ *       with the lowest offending output slot in *bad_pos, dense and spaced alike (the reference's dense path
+ *       returns a short count instead); the slot holds 0.
+ *   The device flavours synchronise `s` once, to read the per-page error codes back; d_decoded (may be NULL) is a
+ *   device array of n_pages counts, *d_bad_pos (may be NULL) is overwritten (AG_NO_ERROR_POS when every index
+ *   is in range).  Host flavours: decoded (may be NULL) and bad_pos (may be NULL) are host memory.
+ *
+ *   ag_parquet_levels_decode: LevelDecoder.SetData / SetDataV2 / Decode (parquet/internal/encoding/levels.go:188-297).
+ *     Bit width = bits.Len(max_level).  AG_PQ_LEVELS_V1_RLE: a data page v1's level section, a 4-byte
+ *     little-endian length then the stream ("received invalid levels / invalid number of bytes (corrupt data
+ *     page?)" when it does not fit); AG_PQ_LEVELS_V2_RLE: the stream alone (len = the v2 header's byte length).
+ *     AG_PQ_LEVELS_BIT_PACKED (deprecated) is AG_ERR_NOT_IMPLEMENTED.  Output int16 levels.
+ *   ag_parquet_dict_decode: dictDecoder.SetData / decode / decodeSpaced (parquet/internal/encoding/decoder.go:125-160)
+ *     over TypedRleDecoder.GetBatchWithDict[Spaced] (utils/typed_rle_dict.go:143-236).  The first byte of a page is
+ *     its bit width; an empty page has bit width 0.  value_width 4 or 8 (int32/float, int64/double); `dict` is
+ *     aligned to it.  valid == NULL: dense output; otherwise slots whose bit is clear get 0 and the others take the
+ *     page's values in order; decoded counts slots.
+ *   ag_parquet_plain_decode_spaced: PlainDecoder.DecodeSpaced (plain_encoding_types.go:98) -> spacedExpand
+ *     (decoder.go:209) for the PLAIN pages of optional columns (what a writer falls back to once the dictionary
+ *     is full).  A page needs value_width bytes per valid slot ("eof exception decode plain" otherwise).  A
+ *     required PLAIN page is a plain copy and needs no entry point.
+ * ================================================================================= */
+typedef struct ag_pq_page {
+  int64_t data;
+  int64_t len;
+  int64_t num_values;
+  int64_t out;
+} ag_pq_page;
+#define AG_PQ_LEVELS_V2_RLE     0
+#define AG_PQ_LEVELS_V1_RLE     1
+#define AG_PQ_LEVELS_BIT_PACKED 2
+ag_status ag_parquet_levels_decode(int max_level, int encoding, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                   int16_t* out, int64_t* decoded);
+ag_status ag_parquet_levels_decode_dev(int max_level, int encoding, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                       int16_t* d_out, int64_t* d_decoded, ag_stream_t s);
+ag_status ag_parquet_dict_decode(int value_width, const void* dict, int64_t dict_len, const uint8_t* data, const ag_pq_page* pages,
+                                 int64_t n_pages, const uint8_t* valid, void* out, int64_t* decoded, int64_t* bad_pos);
+ag_status ag_parquet_dict_decode_dev(int value_width, const void* d_dict, int64_t dict_len, const uint8_t* d_data, const ag_pq_page* pages,
+                                     int64_t n_pages, const uint8_t* d_valid, void* d_out, int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s);
+ag_status ag_parquet_plain_decode_spaced(int value_width, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                         const uint8_t* valid, void* out);
+ag_status ag_parquet_plain_decode_spaced_dev(int value_width, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                             const uint8_t* d_valid, void* d_out, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

@@ -1,0 +1,141 @@
+#!/usr/bin/env python
+"""Parquet page decode on the device (include/arrowgpu.h, csrc/rle.cu) at ~100M values over 2^19-value (~1 MB) pages.
+
+  python scripts/parquet_pages_bench.py [--values N] [--steps K] [--warmup W]
+
+Prints one JSON line: for each case the time per call (CUDA events around K device-resident calls after W warm-up
+calls), the algorithmic bytes (encoded bytes read + values written + validity bits read: what a single pass has to
+move) and their share of the HBM peak, with the card's name and power limit.  Each call ends in one stream
+synchronisation (per-page error codes), which the times include.  Four distinct page bodies are reused round-robin;
+every page writes its own output range.  Writes nothing to disk.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def rle_literal_page(idx, bw):
+    """canonical literal-only hybrid stream of `idx` (a multiple of 8 values): runs of 63 groups, header byte 127"""
+    bits = ((idx[:, None] >> np.arange(bw)) & 1).astype(np.uint8).ravel()
+    payload = np.packbits(bits, bitorder="little").tobytes()
+    out = bytearray()
+    for r in range(0, idx.size, 504):
+        groups = min(504, idx.size - r) // 8
+        out.append(groups << 1 | 1)
+        out += payload[r * bw // 8:r * bw // 8 + groups * bw]
+    return bytes(out)
+
+
+def rle_repeated_page(rng, n, bw, hi):
+    """repeated runs only (clustered indices): run lengths 8..200, values uniform in [0, hi)"""
+    out, left = bytearray(), n
+    while left:
+        k = min(left, int(rng.integers(8, 201)))
+        v = int(rng.integers(0, hi))
+        h = k << 1
+        while h >= 0x80:
+            out.append(h & 0x7F | 0x80)
+            h >>= 7
+        out.append(h)
+        out += v.to_bytes((bw + 7) // 8, "little")
+        left -= k
+    return bytes(out)
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=20).stdout.strip().split(", ")
+        return {"card": out[0], "power_limit": out[1]}
+    except Exception:
+        return {"card": None, "power_limit": None}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--values", type=int, default=100_000_000)
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+
+    from arrow_go_b200 import _native as N
+    from arrow_go_b200.device import DeviceBuffer, Event
+    from bench import peaks
+
+    N.call("ag_init", 0)
+    peak, peak_kind = peaks()
+    rng = np.random.default_rng(0xDEC0DE)
+    per_page = 1 << 19
+    n_pages = max(1, args.values // per_page)
+    n = n_pages * per_page
+    res = {"values": n, "pages": n_pages, "values_per_page": per_page, "peak_gbs": peak, "peak_kind": peak_kind, **card(),
+           "timing": f"CUDA events around {args.steps} calls after {args.warmup} warm-up calls, one stream synchronisation per call included"}
+
+    def timed(fn):
+        for _ in range(args.warmup):
+            fn()
+        N.call("ag_stream_sync", None)
+        e0, e1 = Event(), Event()
+        e0.record()
+        for _ in range(args.steps):
+            fn()
+        e1.record()
+        e1.sync()
+        return e0.elapsed_ms(e1) / args.steps
+
+    def upload(arr):
+        arr = np.ascontiguousarray(arr)
+        b = DeviceBuffer(arr.nbytes + 64)
+        N.call("ag_upload", b.ptr, arr.ctypes.data, arr.nbytes, None)
+        return b
+
+    def page_set(bodies):
+        blob = b"".join(bodies) + bytes(16)
+        offs = np.cumsum([0] + [len(x) for x in bodies])
+        pages = [(int(offs[p % 4]), len(bodies[p % 4]), per_page, p * per_page) for p in range(n_pages)]
+        enc = sum(len(bodies[p % 4]) for p in range(n_pages))
+        return upload(np.frombuffer(blob, np.uint8)), N.page_table(pages), enc
+
+    def line(ms, ab, enc, note):
+        return {"ms": ms, "values_per_s": n / ms * 1e3, "algorithmic_bytes": ab, "encoded_bytes": enc,
+                "gbs": ab / ms / 1e6, "frac": ab / ms / 1e6 / peak, "note": note}
+
+    dout = DeviceBuffer(8 * n + 64)
+    dictionary = rng.integers(-(1 << 62), 1 << 62, 100_000)
+    ddict = upload(dictionary)
+    valid = rng.random(n) >= 0.1
+    dvalid = upload(np.packbits(valid, bitorder="little"))
+    dec, bad = DeviceBuffer(8 * n_pages + 64), DeviceBuffer(64)
+
+    # dictionary indices, bit width 17, literal runs
+    lit = [bytes([17]) + rle_literal_page(rng.integers(0, 100_000, per_page), 17) for _ in range(4)]
+    dblob, tbl, enc = page_set(lit)
+    for label, vp, nbits in (("required", None, 0), ("10pct_nulls", dvalid.ptr, n)):
+        ms = timed(lambda: N.call("ag_parquet_dict_decode_dev", 8, ddict.ptr, 100_000, dblob.ptr, tbl, n_pages, vp, dout.ptr, dec.ptr, bad.ptr, None))
+        res[f"parquet_dict_decode_i64_{label}"] = line(ms, enc + 8.0 * n + nbits / 8.0, enc,
+                                                       "100K-entry int64 dictionary, 17-bit indices in literal runs of 504; dictionary gather from L2")
+    dblob.free()
+    # clustered indices: repeated runs of 8..200 values
+    rep = [bytes([17]) + rle_repeated_page(rng, per_page, 17, 100_000) for _ in range(4)]
+    dblob, tbl, enc = page_set(rep)
+    ms = timed(lambda: N.call("ag_parquet_dict_decode_dev", 8, ddict.ptr, 100_000, dblob.ptr, tbl, n_pages, None, dout.ptr, dec.ptr, bad.ptr, None))
+    res["parquet_dict_decode_i64_runs"] = line(ms, enc + 8.0 * n, enc, "required column, repeated runs only (mean ~104 values)")
+    dblob.free()
+    # definition levels, bit width 1, 10 % nulls (literal runs: 1 bit per level)
+    lv = [rle_literal_page((rng.random(per_page) >= 0.1).astype(np.int64), 1) for _ in range(4)]
+    dblob, tbl, enc = page_set(lv)
+    ms = timed(lambda: N.call("ag_parquet_levels_decode_dev", 1, N.PQ_LEVELS_V2_RLE, dblob.ptr, tbl, n_pages, dout.ptr, dec.ptr, None))
+    res["parquet_levels_decode"] = line(ms, enc + 2.0 * n, enc, "max_level 1 (bit width 1), 10 % nulls, literal runs; int16 levels out")
+    dblob.free(); ddict.free(); dvalid.free(); dec.free(); bad.free(); dout.free()
+    print(json.dumps(res), flush=True)
+
+
+if __name__ == "__main__":
+    main()

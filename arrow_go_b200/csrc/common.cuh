@@ -85,6 +85,52 @@ struct CallStream {
 ag_status dev_alloc_async(void** p, size_t nbytes, cudaStream_t s);
 ag_status dev_free_async(void* p, cudaStream_t s);
 
+// ---------------------------------------------------------------- device flavours used across files ----
+// The stream-ordered implementations behind the *_dev entry points that the host flavours (host_api.cu) and other
+// device code (parquet.cu, hash.cu) call.
+// elementwise.cu
+ag_status arith_binary_dev(int type, int8_t op, int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st);
+ag_status arith_unary_same_dev(int type, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st);
+ag_status arith_unary_diff_dev(int itype, int otype, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st);
+ag_status arith_checked_dev(int type, int8_t op, int shape, const void* l, const uint8_t* lvalid, int64_t loff,
+                            const void* r, const uint8_t* rvalid, int64_t roff, void* out, int64_t n, int64_t* d_first_bad, cudaStream_t st);
+ag_status error_word_reset(int64_t* d_word, cudaStream_t st);
+ag_status arith_unary_checked_dev(int type, int8_t op, const void* in, void* out, int64_t n, int64_t* d_first_bad, cudaStream_t st);
+// cast.cu
+ag_status cast_numeric_dev(int itype, int otype, const void* in, const uint8_t* valid, int64_t voff, void* out, int64_t n,
+                           int allow_int_overflow, int allow_float_truncate, int64_t* first_bad, int64_t row_base, cudaStream_t st);
+// scan.cu
+ag_status cumulative_sum_dev(int type, const void* in, const uint8_t* valid, int64_t voff, int64_t n, int skip_nulls, int checked,
+                             void* out, uint8_t* out_valid, int64_t ooff, void* d_state, int64_t* d_first_bad, cudaStream_t st);
+ag_status cumulative_sum_state_init(void* d_state, int type, const void* start_host, cudaStream_t st);
+// compare.cu
+ag_status compare_dev(int type, int cmp, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st);
+// bitmap.cu
+ag_status bitmap_op_dev(int bitop, const uint8_t* l, int64_t loff, const uint8_t* r, int64_t roff, uint8_t* out, int64_t ooff, int64_t n, cudaStream_t st);
+ag_status bitmap_copy_dev(const uint8_t* src, int64_t soff, int64_t n, uint8_t* dst, int64_t doff, bool invert, cudaStream_t st);
+ag_status bitmap_set_dev(uint8_t* bits, int64_t off, int64_t n, int value, cudaStream_t st);
+ag_status bitmap_popcount_dev(const uint8_t* bits, int64_t off, int64_t n, int64_t* d_count, cudaStream_t st);
+ag_status kleene_dev(int kop, const uint8_t* lvalid, const uint8_t* ldata, int64_t loff, const uint8_t* rvalid, const uint8_t* rdata,
+                     int64_t roff, uint8_t* out_valid, uint8_t* out_data, int64_t ooff, int64_t n, cudaStream_t st);
+// filter.cu
+ag_status filter_output_size_dev(const uint8_t* mask, const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection, int64_t* d_out_len, cudaStream_t st);
+ag_status filter_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, const uint8_t* mask, const uint8_t* mvalid,
+                               int64_t moff, int64_t n, int null_selection, void* out, uint8_t* out_valid, int64_t capacity, int64_t* d_out_len, cudaStream_t st);
+ag_status take_indices_dev(int index_width, const uint8_t* mask, const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection,
+                           void* out_idx, uint8_t* out_valid, int64_t capacity, int64_t* d_out_len, cudaStream_t st);
+// hash.cu
+ag_status is_in_dev(int bit_width, const void* vals, const uint8_t* valid, int64_t off, int64_t n, const void* set, const uint8_t* set_valid,
+                    int64_t set_off, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid, int64_t* d_null_count, cudaStream_t st);
+ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int64_t off, int64_t n, void* out, uint8_t* out_valid, int64_t capacity,
+                     int64_t* d_out_len, cudaStream_t st);
+// sort.cu
+ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int64_t voff, int64_t n, int order, int null_placement,
+                           uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);
+// take.cu
+ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, int64_t vlen, int idx_width, int idx_signed,
+                             const void* idx, const uint8_t* ivalid, int64_t ioff, int64_t n, int bounds_check, void* out, uint8_t* out_valid,
+                             int64_t* d_bad_pos, cudaStream_t st);
+
 // ---------------------------------------------------------------- cross-GPU exchange (comm.cu, reduce.cu) ----
 struct alignas(32) MailSlot { unsigned long long flag; unsigned long long pad; unsigned long long s; unsigned long long c; };
 struct SumExchange {

@@ -27,10 +27,6 @@
 
 namespace ag {
 
-ag_status filter_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, const uint8_t* mask,
-                               const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection, void* out, uint8_t* out_valid,
-                               int64_t capacity, int64_t* d_out_len, cudaStream_t st);
-
 constexpr int kHThreads = 256;
 constexpr int kHWarps = kHThreads / 32;
 constexpr int kHUnroll = 4;                 // 32-row groups a warp has in flight

@@ -5,95 +5,50 @@
 // (arrow/compute/internal/kernels/base_arithmetic_avx2_amd64.go:35-39) and returns when the
 // output bytes are in host memory.  Each call owns pooled streams for its duration, stages its
 // operands into stream-ordered device temporaries and runs the SAME kernels as the *_dev
-// flavour (so results are bit-identical between the two).
+// flavour (so results are bit-identical between the two).  The staging helpers (Temps, h2d /
+// d2h / sync, upload_bitmap, OutBitmap) live in host_stage.cuh, shared with the host flavours
+// of the other files.
 //
 // Elementwise arithmetic and comparisons are pipelined in row chunks over three streams so
 // that H2D of chunk k+1, the kernel of chunk k and D2H of chunk k-1 overlap (PCIe is full
 // duplex; the kernels are ~100x faster than the link).  Buffers obtained from ag_host_alloc /
 // ag_host_register are DMA'd directly; pageable memory still works but the driver bounces it
 // through its own pinned staging area.
-#include "common.cuh"
+#include "host_stage.cuh"
 
-#include <stdlib.h>
 #include <string.h>
 #include <vector>
 
 namespace ag {
 
-// forward declarations of the device-flavour implementations
-ag_status arith_binary_dev(int type, int8_t op, int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st);
-ag_status arith_unary_same_dev(int type, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st);
-ag_status arith_unary_diff_dev(int itype, int otype, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st);
-ag_status arith_checked_dev(int type, int8_t op, int shape, const void* l, const uint8_t* lvalid, int64_t loff,
-                            const void* r, const uint8_t* rvalid, int64_t roff, void* out, int64_t n, int64_t* d_first_bad, cudaStream_t st);
-ag_status error_word_reset(int64_t* d_word, cudaStream_t st);
-ag_status arith_unary_checked_dev(int type, int8_t op, const void* in, void* out, int64_t n, int64_t* d_first_bad, cudaStream_t st);
-ag_status cast_numeric_dev(int itype, int otype, const void* in, const uint8_t* valid, int64_t voff, void* out, int64_t n,
-                           int allow_int_overflow, int allow_float_truncate, int64_t* first_bad, int64_t row_base, cudaStream_t st);
-ag_status cumulative_sum_dev(int type, const void* in, const uint8_t* valid, int64_t voff, int64_t n, int skip_nulls, int checked,
-                             void* out, uint8_t* out_valid, int64_t ooff, void* d_state, int64_t* d_first_bad, cudaStream_t st);
-ag_status cumulative_sum_state_init(void* d_state, int type, const void* start_host, cudaStream_t st);
-ag_status compare_dev(int type, int cmp, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st);
-ag_status bitmap_op_dev(int bitop, const uint8_t* l, int64_t loff, const uint8_t* r, int64_t roff, uint8_t* out, int64_t ooff, int64_t n, cudaStream_t st);
-ag_status bitmap_copy_dev(const uint8_t* src, int64_t soff, int64_t n, uint8_t* dst, int64_t doff, bool invert, cudaStream_t st);
-ag_status bitmap_set_dev(uint8_t* bits, int64_t off, int64_t n, int value, cudaStream_t st);
-ag_status bitmap_popcount_dev(const uint8_t* bits, int64_t off, int64_t n, int64_t* d_count, cudaStream_t st);
-ag_status kleene_dev(int kop, const uint8_t* lvalid, const uint8_t* ldata, int64_t loff, const uint8_t* rvalid, const uint8_t* rdata,
-                     int64_t roff, uint8_t* out_valid, uint8_t* out_data, int64_t ooff, int64_t n, cudaStream_t st);
-ag_status filter_output_size_dev(const uint8_t* mask, const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection, int64_t* d_out_len, cudaStream_t st);
-ag_status filter_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, const uint8_t* mask, const uint8_t* mvalid,
-                               int64_t moff, int64_t n, int null_selection, void* out, uint8_t* out_valid, int64_t capacity, int64_t* d_out_len, cudaStream_t st);
-ag_status take_indices_dev(int index_width, const uint8_t* mask, const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection,
-                           void* out_idx, uint8_t* out_valid, int64_t capacity, int64_t* d_out_len, cudaStream_t st);
-ag_status is_in_dev(int bit_width, const void* vals, const uint8_t* valid, int64_t off, int64_t n, const void* set, const uint8_t* set_valid,
-                    int64_t set_off, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid, int64_t* d_null_count, cudaStream_t st);
-ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int64_t off, int64_t n, void* out, uint8_t* out_valid, int64_t capacity,
-                     int64_t* d_out_len, cudaStream_t st);
-ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int64_t voff, int64_t n, int order, int null_placement,
-                           uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);
-ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, int64_t vlen, int idx_width, int idx_signed,
-                             const void* idx, const uint8_t* ivalid, int64_t ioff, int64_t n, int bounds_check, void* out, uint8_t* out_valid,
-                             int64_t* d_bad_pos, cudaStream_t st);
-
-// Stream-ordered temporaries of one host call; freed (async) when the call returns.
-struct Temps {
-  cudaStream_t st;
-  std::vector<void*> ptrs;
-  explicit Temps(cudaStream_t s) : st(s) {}
-  ag_status alloc(void** p, size_t nbytes) {
-    AG_TRY(dev_alloc_async(p, nbytes + 64, st));  // +64: kernels may read/write whole aligned words at the edges
-    ptrs.push_back(*p);
-    return AG_OK;
-  }
-  template <typename T> ag_status alloc_t(T** p, size_t nbytes) { return alloc(reinterpret_cast<void**>(p), nbytes); }
-  ~Temps() {
-    // An early (error) return may leave H2D / D2H copies of CALLER memory in flight on this pooled stream: wait for
-    // them before the function returns and before the stream goes back to the pool.  On the success paths the
-    // stream is already idle and this costs a few microseconds.
-    cudaStreamSynchronize(st);
-    for (void* p : ptrs) cudaFreeAsync(p, st);
-  }
-};
-
-static inline ag_status h2d(void* d, const void* h, size_t nbytes, cudaStream_t st) {
-  if (nbytes) AG_CUDA_TRY(cudaMemcpyAsync(d, h, nbytes, cudaMemcpyHostToDevice, st));
+// Upload rows [off, off+n) of a column of w-byte values and their validity bits (validity may be NULL).  The device
+// copy of the values starts at row `off`; the copy of the validity keeps the bit phase off & 7 (upload_bitmap).  The
+// kernels index a value and its validity bit with the same row number, so *d_vals comes back rebased by -phase rows:
+// value i of the slice is row i + *phase of *d_vals, next to validity bit i + *phase of *d_valid.
+static ag_status upload_column(Temps& t, const void* vals, const uint8_t* valid, int64_t off, int64_t n, int w,
+                               const void** d_vals, uint8_t** d_valid, int64_t* phase) {
+  void* dv;
+  AG_TRY(t.alloc(&dv, (size_t)n * w));
+  AG_TRY(h2d(dv, (const char*)vals + off * w, (size_t)n * w, t.st));
+  AG_TRY(upload_bitmap(t, valid, off, n, d_valid, phase));
+  *d_vals = (const char*)dv - *phase * w;
   return AG_OK;
 }
-static inline ag_status d2h(void* h, const void* d, size_t nbytes, cudaStream_t st) {
-  if (nbytes) AG_CUDA_TRY(cudaMemcpyAsync(h, d, nbytes, cudaMemcpyDeviceToHost, st));
-  return AG_OK;
-}
-static inline ag_status sync(cudaStream_t st) { AG_CUDA_TRY(cudaStreamSynchronize(st)); return AG_OK; }
 
-// Upload the bytes of a bitmap range [off, off+n) to a device temp; the device copy keeps the
-// same bit phase (off % 8) so kernels address it with bit offset (off & 7).
-static ag_status upload_bitmap(Temps& t, const uint8_t* h, int64_t off, int64_t n, uint8_t** d, int64_t* doff) {
-  *d = nullptr; *doff = 0;
-  if (!h) return AG_OK;
-  const int64_t b0 = off >> 3, b1 = (off + n + 7) >> 3;
-  AG_TRY(t.alloc_t(d, (size_t)(b1 - b0)));
-  AG_TRY(h2d(*d, h + b0, (size_t)(b1 - b0), t.st));
-  *doff = off & 7;
+// Finish a call whose output has `len` rows: copy the output validity back when the caller passed a bitmap, set *nulls
+// to its clear bits when asked (d_count: one device int64 of scratch), and synchronise the stream.
+static ag_status fetch_validity(uint8_t* out_valid, const uint8_t* d_valid, int64_t len, int64_t* nulls, int64_t* d_count,
+                                cudaStream_t st) {
+  int64_t valid = 0;
+  if (out_valid) {
+    AG_TRY(d2h(out_valid, d_valid, (size_t)((len + 7) / 8), st));
+    if (nulls) {
+      AG_TRY(bitmap_popcount_dev(d_valid, 0, len, d_count, st));
+      AG_TRY(d2h(&valid, d_count, sizeof(int64_t), st));
+    }
+  }
+  AG_TRY(sync(st));
+  if (out_valid && nulls) *nulls = len - valid;
   return AG_OK;
 }
 
@@ -371,17 +326,12 @@ ag_status ag_cast_numeric_checked(int itype, int otype, const void* in, const ui
   if (!in || !out) AG_FAIL(AG_ERR_INVALID, "cast: NULL operand");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *din, *dout; int64_t* d_bad; uint8_t* dvalid = nullptr;
+  void *din, *dout; int64_t* d_bad; uint8_t* dvalid; int64_t dvoff;
   AG_TRY(t.alloc(&din, (size_t)n * wi)); AG_TRY(t.alloc(&dout, (size_t)n * wo)); AG_TRY(t.alloc_t(&d_bad, sizeof(int64_t)));
   AG_TRY(h2d(din, in, (size_t)n * wi, cs));
-  const int64_t vbyte0 = valid_offset >> 3;
-  if (valid) {
-    const size_t vbytes = (size_t)(bytes_for_bits(valid_offset + n) - vbyte0);
-    AG_TRY(t.alloc_t(&dvalid, vbytes));
-    AG_TRY(h2d(dvalid, valid + vbyte0, vbytes, cs));
-  }
+  AG_TRY(upload_bitmap(t, valid, valid_offset, n, &dvalid, &dvoff));
   AG_TRY(error_word_reset(d_bad, cs));
-  AG_TRY(cast_numeric_dev(itype, otype, din, dvalid, valid_offset & 7, dout, n, allow_int_overflow, allow_float_truncate, d_bad, 0, cs));
+  AG_TRY(cast_numeric_dev(itype, otype, din, dvalid, dvoff, dout, n, allow_int_overflow, allow_float_truncate, d_bad, 0, cs));
   int64_t bad = AG_NO_ERROR_POS;
   AG_TRY(d2h(&bad, d_bad, sizeof(bad), cs));
   AG_TRY(d2h(out, dout, (size_t)n * wo, cs));
@@ -413,24 +363,19 @@ ag_status ag_cumulative_sum(int type, const void* in, const uint8_t* valid, int6
   if (valid && !out_valid) AG_FAIL(AG_ERR_INVALID, "cumulative_sum: an input with a validity bitmap needs an output validity bitmap");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *din, *dout; int64_t* d_bad; uint8_t *dvalid = nullptr, *dovalid = nullptr; ag_cumsum_state* dstate;
+  void *din, *dout; int64_t* d_bad; uint8_t *dvalid, *dovalid = nullptr; int64_t dvoff; ag_cumsum_state* dstate;
   AG_TRY(t.alloc(&din, (size_t)n * w)); AG_TRY(t.alloc(&dout, (size_t)n * w)); AG_TRY(t.alloc_t(&d_bad, sizeof(int64_t)));
   AG_TRY(t.alloc_t(&dstate, sizeof(ag_cumsum_state)));
   AG_TRY(h2d(din, in, (size_t)n * w, cs));
-  const int64_t vbyte0 = valid_offset >> 3;
   const size_t obytes = (size_t)bytes_for_bits(n);
-  if (valid) {
-    const size_t vbytes = (size_t)(bytes_for_bits(valid_offset + n) - vbyte0);
-    AG_TRY(t.alloc_t(&dvalid, vbytes));
-    AG_TRY(h2d(dvalid, valid + vbyte0, vbytes, cs));
-  }
+  AG_TRY(upload_bitmap(t, valid, valid_offset, n, &dvalid, &dvoff));
   if (out_valid) {
     AG_TRY(t.alloc_t(&dovalid, obytes + 4));
     AG_CUDA_TRY(cudaMemsetAsync(dovalid, 0, obytes + 4, cs));
   }
   AG_TRY(error_word_reset(d_bad, cs));
   AG_TRY(cumulative_sum_state_init(dstate, type, start, cs));
-  AG_TRY(cumulative_sum_dev(type, din, dvalid, valid_offset & 7, n, skip_nulls, checked, dout, dovalid, 0, dstate, d_bad, cs));
+  AG_TRY(cumulative_sum_dev(type, din, dvalid, dvoff, n, skip_nulls, checked, dout, dovalid, 0, dstate, d_bad, cs));
   int64_t bad = AG_NO_ERROR_POS;
   ag_cumsum_state hs;
   AG_TRY(d2h(&bad, d_bad, sizeof(bad), cs));
@@ -462,17 +407,14 @@ ag_status ag_compare(int type, int cmp, int shape, const void* l, const void* r,
   if (n == 0) return AG_OK;
   if (!l || !r || !out_bits) AG_FAIL(AG_ERR_INVALID, "compare: NULL operand");
   const int phase = bit_offset & 7;  // the reference uses offset % 8 relative to `out` (scalar_comparison.cc:72)
-  const int64_t out_bytes = (phase + n + 7) >> 3;
   Pipe pipe;
   AG_TRY(pipe.acquire());
   cudaStream_t s0 = pipe.s[0];
-  uint8_t* d_bits = nullptr;
-  AG_TRY(dev_alloc_async((void**)&d_bits, (size_t)out_bytes + 64, s0));
+  Temps t(s0);
+  OutBitmap ob;
+  AG_TRY(ob.stage(t, out_bits, phase, n));
+  AG_TRY(sync(s0));  // the edge bytes are on the device before the kernels of the other streams write next to them
   ag_status rc = AG_OK;
-  // the first and last bytes may hold neighbours' bits that must survive
-  rc = h2d(d_bits, out_bits, 1, s0);
-  if (rc == AG_OK && out_bytes > 1) rc = h2d(d_bits + out_bytes - 1, out_bits + out_bytes - 1, 1, s0);
-  if (rc == AG_OK) rc = sync(s0);
   // chunk boundaries fall on multiples of 1024 output bits, so chunks never share an output word
   int64_t chunk = (kChunkBytes / w) & ~(int64_t)1023;
   const bool la = shape != AG_SHAPE_SA, ra = shape != AG_SHAPE_AS;
@@ -491,19 +433,18 @@ ag_status ag_compare(int type, int cmp, int shape, const void* l, const void* r,
     if (la) rc = h2d(d_l[sl], (const char*)l + r0 * w, (size_t)len * w, st);
     if (rc == AG_OK && ra) rc = h2d(d_r[sl], (const char*)r + r0 * w, (size_t)len * w, st);
     const int64_t obit = phase + r0;
-    if (rc == AG_OK) rc = compare_dev(type, cmp, shape, la ? d_l[sl] : l, ra ? d_r[sl] : r, d_bits + (obit >> 3), len, (int)(obit & 7), st);
+    if (rc == AG_OK) rc = compare_dev(type, cmp, shape, la ? d_l[sl] : l, ra ? d_r[sl] : r, ob.d + (obit >> 3), len, (int)(obit & 7), st);
     r0 += len; ++ci;
   }
   for (int sl = 0; sl < kPipe; ++sl) {
     if (d_l[sl]) cudaFreeAsync(d_l[sl], pipe.s[sl]);
     if (d_r[sl]) cudaFreeAsync(d_r[sl], pipe.s[sl]);
   }
-  ag_status rs = pipe.sync_all();
-  if (rc == AG_OK) rc = rs;
-  if (rc == AG_OK) rc = d2h(out_bits, d_bits, (size_t)out_bytes, s0);
-  cudaFreeAsync(d_bits, s0);
-  rs = sync(s0);
-  return rc != AG_OK ? rc : rs;
+  const ag_status rs = pipe.sync_all();
+  AG_TRY(rc);
+  AG_TRY(rs);
+  AG_TRY(ob.fetch(s0));
+  return sync(s0);
 }
 
 #define AG_CMP_NAMED(NAME, CMP, SHAPE)                                                                        \
@@ -517,20 +458,6 @@ AG_CMP_NAMED(ag_cmp_ge_aa, AG_CMP_GE, AG_SHAPE_AA) AG_CMP_NAMED(ag_cmp_ge_as, AG
 #undef AG_CMP_NAMED
 
 // ---- bitmaps -----------------------------------------------------------------------
-// An output bitmap range is staged with its existing first/last bytes so that bits outside
-// [off, off+n) survive the round trip; only the bytes of the range are written back.
-struct OutBitmap {
-  uint8_t* h = nullptr; uint8_t* d = nullptr; int64_t b0 = 0, nbytes = 0, doff = 0;
-  ag_status stage(Temps& t, uint8_t* host, int64_t off, int64_t n) {
-    h = host; b0 = off >> 3; nbytes = ((off + n + 7) >> 3) - b0; doff = off & 7;
-    AG_TRY(t.alloc_t(&d, (size_t)nbytes));
-    AG_TRY(h2d(d, h + b0, 1, t.st));
-    if (nbytes > 1) AG_TRY(h2d(d + nbytes - 1, h + b0 + nbytes - 1, 1, t.st));
-    return AG_OK;
-  }
-  ag_status fetch(cudaStream_t st) { return d2h(h + b0, d, (size_t)nbytes, st); }
-};
-
 ag_status ag_bitmap_op(int bitop, const uint8_t* l, int64_t loff, const uint8_t* r, int64_t roff, uint8_t* out, int64_t ooff, int64_t n) {
   AG_TRY(ensure_init());
   if (n < 0 || loff < 0 || roff < 0 || ooff < 0) AG_FAIL(AG_ERR_INVALID, "bitmap_op: negative length or offset");
@@ -661,15 +588,8 @@ ag_status ag_filter_primitive(int bit_width, const void* vals, const uint8_t* vv
     // values bitmap and its validity share the row numbering: both copies keep phase voff & 7
     AG_TRY(filter_primitive_dev(1, dvd, dvv, ovd, dm, dmv, om, n, null_selection, dout, dov, len, d_len + 1, cs));
     AG_TRY(d2h(out, dout, (size_t)((len + 7) / 8), cs));
-    if (out_valid) AG_TRY(d2h(out_valid, dov, (size_t)((len + 7) / 8), cs));
-    int64_t valid = 0;
-    if (out_valid && out_nulls) {
-      AG_TRY(bitmap_popcount_dev(dov, 0, len, d_len, cs));
-      AG_TRY(d2h(&valid, d_len, sizeof(int64_t), cs));
-    }
-    AG_TRY(sync(cs));
+    AG_TRY(fetch_validity(out_valid, dov, len, out_nulls, d_len, cs));
     *out_len = len;
-    if (out_valid && out_nulls) *out_nulls = len - valid;
     return AG_OK;
   }
   const int w = bit_width / 8;
@@ -683,27 +603,16 @@ ag_status ag_filter_primitive(int bit_width, const void* vals, const uint8_t* vv
   AG_TRY(filter_output_size_dev(dm, dmv, om, n, null_selection, d_len, cs));
   int64_t len = 0;
   AG_TRY(d2h(&len, d_len, sizeof(int64_t), cs));
-  void* dv; AG_TRY(t.alloc(&dv, (size_t)n * w));
-  AG_TRY(h2d(dv, (const char*)vals + voff * w, (size_t)n * w, cs));
-  AG_TRY(upload_bitmap(t, vvalid, voff, n, &dvv, &ovv));
+  const void* dv;
+  AG_TRY(upload_column(t, vals, vvalid, voff, n, w, &dv, &dvv, &ovv));
   AG_TRY(sync(cs));
   void* dout; AG_TRY(t.alloc(&dout, (size_t)len * w));
   uint8_t* dov = nullptr;
   if (out_valid) AG_TRY(t.alloc_t(&dov, (size_t)((len + 31) / 32) * 4));
-  // the device copy of the values starts at the slice: element offset 0, validity phase ovv
-  // (the kernel indexes values and their validity with the same row number, so shift the
-  // validity pointer/offset instead of the values)
-  AG_TRY(filter_primitive_dev(bit_width, (const char*)dv - ovv * w, dvv, ovv, dm, dmv, om, n, null_selection, dout, dov, len, d_len + 1, cs));
+  AG_TRY(filter_primitive_dev(bit_width, dv, dvv, ovv, dm, dmv, om, n, null_selection, dout, dov, len, d_len + 1, cs));
   AG_TRY(d2h(out, dout, (size_t)len * w, cs));
-  if (out_valid) AG_TRY(d2h(out_valid, dov, (size_t)((len + 7) / 8), cs));
-  int64_t nulls = 0;
-  if (out_valid && out_nulls) {
-    AG_TRY(bitmap_popcount_dev(dov, 0, len, d_len, cs));
-    AG_TRY(d2h(&nulls, d_len, sizeof(int64_t), cs));
-  }
-  AG_TRY(sync(cs));
+  AG_TRY(fetch_validity(out_valid, dov, len, out_nulls, d_len, cs));
   *out_len = len;
-  if (out_valid && out_nulls) *out_nulls = len - nulls;
   return AG_OK;
 }
 
@@ -754,17 +663,17 @@ ag_status ag_take_primitive(int bit_width, const void* vals, const uint8_t* vval
   const int w = is_bool ? 0 : bit_width / 8, iw = idx_width / 8;
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *dv, *di, *dout; uint8_t *dvv, *div; int64_t ovv, oiv; int64_t* d_word;
+  const void* dv; void *di, *dout; uint8_t *dvv, *div; int64_t ovv, oiv; int64_t* d_word;
   if (is_bool) {
+    // the values bitmap keeps its phase voff & 7 and is not rebased; the kernel takes that phase from ovv
     uint8_t* dvb; int64_t ovb;
     AG_TRY(upload_bitmap(t, (const uint8_t*)vals, voff, vlen, &dvb, &ovb));
+    AG_TRY(upload_bitmap(t, vvalid, voff, vlen, &dvv, &ovv));
+    if (!vvalid) ovv = voff & 7;
     dv = dvb;
   } else {
-    AG_TRY(t.alloc(&dv, (size_t)vlen * w));
-    AG_TRY(h2d(dv, (const char*)vals + voff * w, (size_t)vlen * w, cs));
+    AG_TRY(upload_column(t, vals, vvalid, voff, vlen, w, &dv, &dvv, &ovv));
   }
-  AG_TRY(upload_bitmap(t, vvalid, voff, vlen, &dvv, &ovv));
-  if (is_bool && !vvalid) ovv = voff & 7;
   AG_TRY(t.alloc(&di, (size_t)n * iw));
   AG_TRY(h2d(di, idx, (size_t)n * iw, cs));
   AG_TRY(upload_bitmap(t, ivalid, ioff, n, &div, &oiv));
@@ -773,8 +682,7 @@ ag_status ag_take_primitive(int bit_width, const void* vals, const uint8_t* vval
   if (out_valid) AG_TRY(t.alloc_t(&dov, (size_t)((n + 31) / 32) * 4));
   AG_TRY(t.alloc_t(&d_word, 2 * sizeof(int64_t)));
   AG_TRY(error_word_reset(d_word, cs));
-  // the device copies start at the slice: element offset becomes the bitmap phase (voff & 7)
-  AG_TRY(take_primitive_dev(bit_width, is_bool ? dv : (void*)((const char*)dv - ovv * w), dvv, ovv, vlen, idx_width, idx_signed, di, div, oiv, n,
+  AG_TRY(take_primitive_dev(bit_width, dv, dvv, ovv, vlen, idx_width, idx_signed, di, div, oiv, n,
                             bounds_check, dout, dov, d_word, cs));
   int64_t bad = AG_NO_ERROR_POS;
   AG_TRY(d2h(&bad, d_word, sizeof(int64_t), cs));
@@ -793,18 +701,7 @@ ag_status ag_take_primitive(int bit_width, const void* vals, const uint8_t* vval
     AG_FAIL(AG_ERR_INDEX, "%lld out of bounds", (long long)v);  // helpers.go:951
   }
   AG_TRY(d2h(out, dout, is_bool ? (size_t)((n + 7) / 8) : (size_t)n * w, cs));
-  if (out_valid) {
-    AG_TRY(d2h(out_valid, dov, (size_t)((n + 7) / 8), cs));
-    if (out_nulls) {
-      AG_TRY(bitmap_popcount_dev(dov, 0, n, d_word + 1, cs));
-      int64_t valid = 0;
-      AG_TRY(d2h(&valid, d_word + 1, sizeof(int64_t), cs));
-      AG_TRY(sync(cs));
-      *out_nulls = n - valid;
-      return AG_OK;
-    }
-  }
-  return sync(cs);
+  return fetch_validity(out_valid, dov, n, out_nulls, d_word + 1, cs);
 }
 
 ag_status ag_sort_indices(int type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, int order,
@@ -819,13 +716,10 @@ ag_status ag_sort_indices(int type, const void* vals, const uint8_t* valid, int6
   if (!vals || !out) AG_FAIL(AG_ERR_INVALID, "sort_indices: NULL values/output");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void* dv; uint8_t* dvalid; int64_t ov; uint64_t* dout;
-  AG_TRY(t.alloc(&dv, (size_t)n * w));
-  AG_TRY(h2d(dv, (const char*)vals + offset * w, (size_t)n * w, cs));
-  AG_TRY(upload_bitmap(t, valid, offset, n, &dvalid, &ov));
+  const void* dv; uint8_t* dvalid; int64_t ov; uint64_t* dout;
+  AG_TRY(upload_column(t, vals, valid, offset, n, w, &dv, &dvalid, &ov));
   AG_TRY(t.alloc_t(&dout, (size_t)n * 8));
-  // the device copy starts at the slice: the element offset becomes the bitmap phase (offset & 7)
-  AG_TRY(sort_indices_dev(type, (const char*)dv - ov * w, dvalid, ov, n, order, null_placement, dout, null_count, nan_count, cs));
+  AG_TRY(sort_indices_dev(type, dv, dvalid, ov, n, order, null_placement, dout, null_count, nan_count, cs));
   AG_TRY(d2h(out, dout, (size_t)n * 8, cs));
   return sync(cs);
 }
@@ -842,20 +736,14 @@ ag_status ag_is_in(int bit_width, const void* vals, const uint8_t* valid, int64_
   const int w = bit_width / 8;
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *dv, *ds = nullptr; uint8_t *dvv, *dsv = nullptr, *dod, *dov; int64_t ov, os = 0; int64_t* d_nulls;
-  AG_TRY(t.alloc(&dv, (size_t)n * w));
-  AG_TRY(h2d(dv, (const char*)vals + offset * w, (size_t)n * w, cs));
-  AG_TRY(upload_bitmap(t, valid, offset, n, &dvv, &ov));
-  if (set_n > 0) {
-    AG_TRY(t.alloc(&ds, (size_t)set_n * w));
-    AG_TRY(h2d(ds, (const char*)set_vals + set_offset * w, (size_t)set_n * w, cs));
-    AG_TRY(upload_bitmap(t, set_valid, set_offset, set_n, &dsv, &os));
-  }
+  const void *dv, *ds = nullptr; uint8_t *dvv, *dsv = nullptr, *dod, *dov; int64_t ov, os = 0; int64_t* d_nulls;
+  AG_TRY(upload_column(t, vals, valid, offset, n, w, &dv, &dvv, &ov));
+  if (set_n > 0) AG_TRY(upload_column(t, set_vals, set_valid, set_offset, set_n, w, &ds, &dsv, &os));
   const size_t bm = (size_t)((n + 31) / 32) * 4;
   AG_TRY(t.alloc_t(&dod, bm));
   AG_TRY(t.alloc_t(&dov, bm));
   AG_TRY(t.alloc_t(&d_nulls, 8));
-  AG_TRY(is_in_dev(bit_width, (const char*)dv - ov * w, dvv, ov, n, ds ? (const char*)ds - os * w : nullptr, dsv, os, set_n, null_behavior, dod,
+  AG_TRY(is_in_dev(bit_width, dv, dvv, ov, n, ds, dsv, os, set_n, null_behavior, dod,
                    out_valid ? dov : nullptr, d_nulls, cs));
   AG_TRY(d2h(out_data, dod, (size_t)((n + 7) / 8), cs));
   if (out_valid) AG_TRY(d2h(out_valid, dov, (size_t)((n + 7) / 8), cs));
@@ -880,29 +768,17 @@ ag_status ag_unique(int bit_width, const void* vals, const uint8_t* valid, int64
   const int w = bit_width / 8;
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *dv, *dout; uint8_t *dvv, *dov = nullptr; int64_t ov; int64_t* d_len;
-  AG_TRY(t.alloc(&dv, (size_t)n * w));
-  AG_TRY(h2d(dv, (const char*)vals + offset * w, (size_t)n * w, cs));
-  AG_TRY(upload_bitmap(t, valid, offset, n, &dvv, &ov));
+  const void* dv; void* dout; uint8_t *dvv, *dov = nullptr; int64_t ov; int64_t* d_len;
+  AG_TRY(upload_column(t, vals, valid, offset, n, w, &dv, &dvv, &ov));
   AG_TRY(t.alloc(&dout, (size_t)n * w));
   if (valid) AG_TRY(t.alloc_t(&dov, (size_t)((n + 31) / 32) * 4));
   AG_TRY(t.alloc_t(&d_len, 16));
-  AG_TRY(unique_dev(bit_width, (const char*)dv - ov * w, dvv, ov, n, dout, dov, n, d_len, cs));
+  AG_TRY(unique_dev(bit_width, dv, dvv, ov, n, dout, dov, n, d_len, cs));
   int64_t len = 0;
   AG_TRY(d2h(&len, d_len, 8, cs));
   AG_TRY(sync(cs));
   AG_TRY(d2h(out, dout, (size_t)len * w, cs));
-  if (dov && out_valid) {
-    AG_TRY(d2h(out_valid, dov, (size_t)((len + 7) / 8), cs));
-    if (out_nulls) {
-      AG_TRY(bitmap_popcount_dev(dov, 0, len, d_len + 1, cs));
-      int64_t v = 0;
-      AG_TRY(d2h(&v, d_len + 1, 8, cs));
-      AG_TRY(sync(cs));
-      *out_nulls = len - v;
-    }
-  }
-  AG_TRY(sync(cs));
+  AG_TRY(fetch_validity(dov ? out_valid : nullptr, dov, len, out_nulls, d_len + 1, cs));
   *out_len = len;
   return AG_OK;
 }

@@ -11,7 +11,7 @@
 // warp shuffle tree -> block -> partials -> last block (ticket).  Inputs that are only
 // element-aligned (Arrow slices) peel up to 15 bytes at the head; the vector body starts at the
 // first 16-byte boundary.
-#include "common.cuh"
+#include "host_stage.cuh"
 
 #include <string.h>
 #include <limits>
@@ -201,29 +201,20 @@ extern "C" ag_status ag_min_max(int type, const void* values, int64_t n, void* m
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "min_max: negative length");
   if (!min_out || !max_out) AG_FAIL(AG_ERR_INVALID, "min_max: NULL result pointer");
   if (n > 0 && !values) AG_FAIL(AG_ERR_INVALID, "min_max: NULL values");
-  CallStream cs;
-  AG_TRY(cs.acquire());
-  uint8_t* d_in = nullptr;
-  ag_status rc = AG_OK;
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const size_t nbytes = (size_t)n * w;
+  const size_t bytes = (nbytes + 15) & ~(size_t)15;   // the two results follow the values, 16-byte aligned
+  uint8_t* d_in;
+  AG_TRY(t.alloc_t(&d_in, bytes + 16));
+  const size_t chunk = (size_t)64 << 20;
+  for (size_t off = 0; off < nbytes; off += chunk)
+    AG_TRY(h2d(d_in + off, (const uint8_t*)values + off, nbytes - off < chunk ? nbytes - off : chunk, cs));
+  AG_TRY(min_max_dev(type, d_in, n, d_in + bytes, cs));
   unsigned char res[16];
-  do {
-    const size_t bytes = ((size_t)n * w + 15) & ~(size_t)15;
-    if ((rc = dev_alloc_async((void**)&d_in, bytes + 16, cs)) != AG_OK) break;
-    cudaError_t e = cudaSuccess;
-    const size_t chunk = (size_t)64 << 20;
-    for (size_t off = 0; off < (size_t)n * w && e == cudaSuccess; off += chunk) {
-      const size_t len = ((size_t)n * w - off < chunk) ? ((size_t)n * w - off) : chunk;
-      e = cudaMemcpyAsync(d_in + off, (const uint8_t*)values + off, len, cudaMemcpyHostToDevice, cs);
-    }
-    if (e != cudaSuccess) { rc = cuda_fail(e, "H2D", __FILE__, __LINE__); break; }
-    if ((rc = min_max_dev(type, d_in, n, d_in + bytes, cs)) != AG_OK) break;
-    e = cudaMemcpyAsync(res, d_in + bytes, 2 * (size_t)w, cudaMemcpyDeviceToHost, cs);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-    if (e != cudaSuccess) { rc = cuda_fail(e, "D2H", __FILE__, __LINE__); break; }
-    memcpy(min_out, res, (size_t)w);
-    memcpy(max_out, res + w, (size_t)w);
-  } while (0);
-  if (d_in) cudaFreeAsync(d_in, cs);
-  cudaStreamSynchronize(cs);
-  return rc;
+  AG_TRY(d2h(res, d_in + bytes, 2 * (size_t)w, cs));
+  AG_TRY(sync(cs));
+  memcpy(min_out, res, (size_t)w);
+  memcpy(max_out, res + w, (size_t)w);
+  return AG_OK;
 }

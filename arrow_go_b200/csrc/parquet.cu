@@ -12,16 +12,9 @@
 //                    def level reaches RepeatedAncestorDefLevel produce a bit (pext = stable compaction of bits).
 // Roofline: HBM streams.  unpack32 reads num_bits/8 bytes and writes 4 per value; the level conversion is compare.cu's
 // int16 > scalar kernel (2 B in, 1 bit out per level) plus, for nested columns, filter.cu's boolean compaction.
-#include "common.cuh"
+#include "host_stage.cuh"
 
 namespace ag {
-
-ag_status compare_dev(int type, int cmp, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st);
-ag_status bitmap_popcount_dev(const uint8_t* bits, int64_t off, int64_t n, int64_t* d_count, cudaStream_t st);
-ag_status bitmap_copy_dev(const uint8_t* src, int64_t soff, int64_t n, uint8_t* dst, int64_t doff, bool invert, cudaStream_t st);
-ag_status filter_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, const uint8_t* mask,
-                               const uint8_t* mvalid, int64_t moff, int64_t n, int null_selection, void* out, uint8_t* out_valid,
-                               int64_t capacity, int64_t* d_out_len, cudaStream_t st);
 
 constexpr int kPqThreads = 256;
 
@@ -184,7 +177,7 @@ ag_status parquet_def_levels_to_bitmap_dev(const int16_t* levels, int64_t n, int
   do {
     if ((rc = compare_dev(AG_TYPE_INT16, AG_CMP_GT, AG_SHAPE_AS, levels, &rhs, defined, n, 0, st)) != AG_OK) break;
     if ((rc = compare_dev(AG_TYPE_INT16, AG_CMP_GT, AG_SHAPE_AS, levels, &rhs2, present, n, 0, st)) != AG_OK) break;
-    if (cudaMemsetAsync(packed, 0, bm, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break; }
+    if (const cudaError_t e = cudaMemsetAsync(packed, 0, bm, st)) { rc = cuda_fail(e, "memset", __FILE__, __LINE__); break; }
     if ((rc = filter_primitive_dev(1, defined, nullptr, 0, present, nullptr, 0, n, AG_DROP_NULLS, packed, nullptr, n, d_counts, st)) != AG_OK) break;
     // the selected count is only known on the device: copy min(count, n) bits — bits past the count are zero in `packed`
     // and the caller's bitmap beyond values_read is unspecified (FirstTimeBitmapWriter), so copy all n candidate bits
@@ -226,17 +219,15 @@ ag_status ag_parquet_unpack32(const uint32_t* in, uint32_t* out, int64_t batch_s
   if (n == 0) return AG_OK;
   if (!out || (num_bits > 0 && !in)) AG_FAIL(AG_ERR_INVALID, "unpack32: NULL buffer");
   CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
   const size_t in_bytes = (size_t)n * num_bits / 8;
-  void *din = nullptr, *dout = nullptr;
-  AG_TRY(dev_alloc_async(&din, in_bytes + 64, cs));
-  ag_status rc = dev_alloc_async(&dout, (size_t)n * 4 + 64, cs);
-  if (rc == AG_OK && in_bytes && cudaMemcpyAsync(din, in, in_bytes, cudaMemcpyHostToDevice, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "H2D", __FILE__, __LINE__);
-  if (rc == AG_OK) rc = parquet_unpack32_dev((const uint32_t*)din, (uint32_t*)dout, n, num_bits, unpacked, cs);
-  if (rc == AG_OK && cudaMemcpyAsync(out, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__);
-  cudaStreamSynchronize(cs);
-  if (din) cudaFreeAsync(din, cs);
-  if (dout) cudaFreeAsync(dout, cs);
-  return rc;
+  uint32_t *din, *dout;
+  AG_TRY(t.alloc_t(&din, in_bytes));
+  AG_TRY(t.alloc_t(&dout, (size_t)n * 4));
+  AG_TRY(h2d(din, in, in_bytes, cs));
+  AG_TRY(parquet_unpack32_dev(din, dout, n, num_bits, unpacked, cs));
+  AG_TRY(d2h(out, dout, (size_t)n * 4, cs));
+  return sync(cs);
 }
 
 ag_status ag_parquet_bytes_to_bools(const uint8_t* bytes, int64_t len, uint8_t* out, int64_t outlen) {
@@ -245,17 +236,15 @@ ag_status ag_parquet_bytes_to_bools(const uint8_t* bytes, int64_t len, uint8_t* 
   if (len == 0 || outlen == 0) return AG_OK;
   if (!bytes || !out) AG_FAIL(AG_ERR_INVALID, "bytes_to_bools: NULL buffer");
   CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
   const int64_t produced = len * 8 < outlen ? len * 8 : outlen;
-  void *din = nullptr, *dout = nullptr;
-  AG_TRY(dev_alloc_async(&din, (size_t)len + 64, cs));
-  ag_status rc = dev_alloc_async(&dout, (size_t)produced + 64, cs);
-  if (rc == AG_OK && cudaMemcpyAsync(din, bytes, (size_t)len, cudaMemcpyHostToDevice, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "H2D", __FILE__, __LINE__);
-  if (rc == AG_OK) rc = parquet_bytes_to_bools_dev((const uint8_t*)din, len, (uint8_t*)dout, produced, cs);
-  if (rc == AG_OK && cudaMemcpyAsync(out, dout, (size_t)produced, cudaMemcpyDeviceToHost, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__);
-  cudaStreamSynchronize(cs);
-  if (din) cudaFreeAsync(din, cs);
-  if (dout) cudaFreeAsync(dout, cs);
-  return rc;
+  uint8_t *din, *dout;
+  AG_TRY(t.alloc_t(&din, (size_t)len));
+  AG_TRY(t.alloc_t(&dout, (size_t)produced));
+  AG_TRY(h2d(din, bytes, (size_t)len, cs));
+  AG_TRY(parquet_bytes_to_bools_dev(din, len, dout, produced, cs));
+  AG_TRY(d2h(out, dout, (size_t)produced, cs));
+  return sync(cs);
 }
 
 ag_status ag_parquet_def_levels_to_bitmap(const int16_t* def_levels, int64_t n, int def_level, int repeated_ancestor_def_level, uint8_t* valid_bits,
@@ -266,34 +255,25 @@ ag_status ag_parquet_def_levels_to_bitmap(const int16_t* def_levels, int64_t n, 
   if (n == 0) return AG_OK;
   if (!def_levels || !valid_bits) AG_FAIL(AG_ERR_INVALID, "def_levels_to_bitmap: NULL buffer");
   CallStream cs; AG_TRY(cs.acquire());
-  // the device bitmap keeps the caller's bit phase, and starts as a copy of the touched bytes so that neighbours survive
-  const int64_t b0 = valid_bits_offset >> 3, b1 = (valid_bits_offset + n + 7) >> 3;
-  void *dl = nullptr, *db = nullptr, *dc = nullptr;
-  AG_TRY(dev_alloc_async(&dl, (size_t)n * 2 + 64, cs));
-  ag_status rc = dev_alloc_async(&db, (size_t)(b1 - b0) + 64, cs);
-  if (rc == AG_OK) rc = dev_alloc_async(&dc, 64, cs);
-  if (rc == AG_OK && (cudaMemcpyAsync(dl, def_levels, (size_t)n * 2, cudaMemcpyHostToDevice, cs) != cudaSuccess ||
-                      cudaMemcpyAsync(db, valid_bits + b0, (size_t)(b1 - b0), cudaMemcpyHostToDevice, cs) != cudaSuccess))
-    rc = cuda_fail(cudaGetLastError(), "H2D", __FILE__, __LINE__);
-  if (rc == AG_OK) rc = parquet_def_levels_to_bitmap_dev((const int16_t*)dl, n, def_level, repeated_ancestor_def_level, (uint8_t*)db, valid_bits_offset & 7,
-                                                         read_upper_bound, (int64_t*)dc, cs);
+  Temps t(cs);
+  int16_t* dl; int64_t* dc;
+  AG_TRY(t.alloc_t(&dl, (size_t)n * 2));
+  AG_TRY(h2d(dl, def_levels, (size_t)n * 2, cs));
+  // both device paths write all n bits of [offset, offset + n), so only the edge bytes' neighbours need staging
+  OutBitmap ob;
+  AG_TRY(ob.stage(t, valid_bits, valid_bits_offset, n));
+  AG_TRY(t.alloc_t(&dc, 2 * sizeof(int64_t)));
+  AG_TRY(parquet_def_levels_to_bitmap_dev(dl, n, def_level, repeated_ancestor_def_level, ob.d, ob.doff, read_upper_bound, dc, cs));
   int64_t counts[2] = {0, 0};
-  if (rc == AG_OK && cudaMemcpyAsync(counts, dc, 16, cudaMemcpyDeviceToHost, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__);
-  if (rc == AG_OK && cudaStreamSynchronize(cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-  if (rc == AG_OK) {
-    if (repeated_ancestor_def_level >= 0 && counts[0] > read_upper_bound) { rc = AG_ERR_INVALID; set_error("values read exceeded upper bound"); }
-  }
-  if (rc == AG_OK) {
-    // bring back only the bytes that hold the values_read bits appended at valid_bits_offset
-    const int64_t e1 = (valid_bits_offset + counts[0] + 7) >> 3;
-    if (e1 > b0 && cudaMemcpyAsync(valid_bits + b0, db, (size_t)(e1 - b0), cudaMemcpyDeviceToHost, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__);
-    cudaStreamSynchronize(cs);
-    if (values_read) *values_read = counts[0];
-    if (null_count) *null_count += counts[0] - counts[1];
-  }
-  cudaStreamSynchronize(cs);
-  cudaFreeAsync(dl, cs); if (db) cudaFreeAsync(db, cs); if (dc) cudaFreeAsync(dc, cs);
-  return rc;
+  AG_TRY(d2h(counts, dc, sizeof(counts), cs));
+  AG_TRY(sync(cs));
+  if (repeated_ancestor_def_level >= 0 && counts[0] > read_upper_bound) AG_FAIL(AG_ERR_INVALID, "values read exceeded upper bound");
+  // bring back only the bytes that hold the values_read bits appended at valid_bits_offset
+  AG_TRY(d2h(valid_bits + ob.b0, ob.d, (size_t)(bytes_for_bits(valid_bits_offset + counts[0]) - ob.b0), cs));
+  AG_TRY(sync(cs));
+  if (values_read) *values_read = counts[0];
+  if (null_count) *null_count += counts[0] - counts[1];
+  return AG_OK;
 }
 
 }  // extern "C"

@@ -23,7 +23,7 @@
 //   * the last block to finish (ticket) reduces partials[] with the same fixed tree.
 // 16-byte aligned inputs use 128-bit ld.global.cs; 8-byte aligned ones use two 64-bit loads
 // with the SAME pair->thread mapping, so alignment never changes the result.
-#include "common.cuh"
+#include "host_stage.cuh"
 
 #include <type_traits>
 
@@ -326,27 +326,16 @@ static ag_status host_sum(const T* buf, size_t n, T* res, F&& launch) {
   if (!buf) AG_FAIL(AG_ERR_INVALID, "sum: NULL buffer");
   CallStream cs;  // a private pooled stream per call keeps concurrent host calls independent
   AG_TRY(cs.acquire());
-  T* d_in = nullptr;
-  T* d_res = nullptr;
-  ag_status rc = AG_OK;
-  do {
-    if ((rc = dev_alloc_async((void**)&d_in, n * sizeof(T) + sizeof(T), cs)) != AG_OK) break;
-    d_res = d_in + n;
-    const size_t chunk = (size_t)8 << 20;  // elements (64 MiB)
-    cudaError_t e = cudaSuccess;
-    for (size_t off = 0; off < n && e == cudaSuccess; off += chunk) {
-      const size_t len = (n - off < chunk) ? (n - off) : chunk;
-      e = cudaMemcpyAsync(d_in + off, buf + off, len * sizeof(T), cudaMemcpyHostToDevice, cs);
-    }
-    if (e != cudaSuccess) { rc = cuda_fail(e, "H2D", __FILE__, __LINE__); break; }
-    if ((rc = launch(d_in, n, d_res, cs)) != AG_OK) break;
-    e = cudaMemcpyAsync(res, d_res, sizeof(T), cudaMemcpyDeviceToHost, cs);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-    if (e != cudaSuccess) { rc = cuda_fail(e, "D2H", __FILE__, __LINE__); break; }
-  } while (0);
-  if (d_in) cudaFreeAsync(d_in, cs);
-  cudaStreamSynchronize(cs);
-  return rc;
+  Temps t(cs);
+  T* d_in;
+  AG_TRY(t.alloc_t(&d_in, n * sizeof(T) + sizeof(T)));
+  T* d_res = d_in + n;
+  const size_t chunk = (size_t)8 << 20;  // elements (64 MiB)
+  for (size_t off = 0; off < n; off += chunk)
+    AG_TRY(h2d(d_in + off, buf + off, (n - off < chunk ? n - off : chunk) * sizeof(T), cs));
+  AG_TRY(launch(d_in, n, d_res, cs));
+  AG_TRY(d2h(res, d_res, sizeof(T), cs));
+  return sync(cs);
 }
 
 static ag_status launch_reforder(const double* d_in, size_t n, double* d_res, cudaStream_t st) {

@@ -21,10 +21,11 @@
 // reads the encoded bytes up to twice (pass 2 only touches the headers' windows and the payload it expands) and
 // writes 8 B per run descriptor, so its own bound is (2 x encoded + written) bytes of HBM traffic; the dictionary
 // gather is served from L2.
-#include <stdlib.h>
 #include <string.h>
 
-#include "common.cuh"
+#include <vector>
+
+#include "host_stage.cuh"
 
 namespace ag {
 
@@ -454,30 +455,27 @@ ag_status parquet_pages_dev(int kind, int fixed_bw, int v1, int width, const voi
   // plan: pages | run_base[n+1] | tile_base[n+1]
   const size_t pb = (size_t)n_pages * sizeof(ag_pq_page);
   const size_t plan_bytes = pb + 2 * (size_t)(n_pages + 1) * 8;
-  uint8_t* h = (uint8_t*)malloc(plan_bytes);
-  if (!h) AG_FAIL(AG_ERR_OOM, "%s: host allocation failed", fn);
-  memcpy(h, pages, pb);
-  int64_t* run_base = reinterpret_cast<int64_t*>(h + pb);
+  std::vector<uint8_t> h(plan_bytes);
+  memcpy(h.data(), pages, pb);
+  int64_t* run_base = reinterpret_cast<int64_t*>(h.data() + pb);
   int64_t* tile_base = run_base + n_pages + 1;
   run_base[0] = tile_base[0] = 0;
   bool any_data = false;
   for (int64_t i = 0; i < n_pages; ++i) {
     const ag_pq_page& g = pages[i];
-    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL) {
-      free(h);
+    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL)
       AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field, more than 2^31-1 values or more than 2^32-1 bytes", fn, (long long)i);
-    }
     any_data |= g.len > 0;
     const int64_t cap = kind == kPlain ? 0 : (g.num_values < g.len ? g.num_values : g.len);
     run_base[i + 1] = run_base[i] + cap;
     tile_base[i + 1] = tile_base[i] + (g.num_values + kTile - 1) / kTile;
   }
   const int64_t n_runs = run_base[n_pages], n_tiles = tile_base[n_pages];
-  if (n_tiles > 0 && !out) { free(h); AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn); }
-  if (any_data && !data) { free(h); AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn); }
-  if (kind == kDict && dict_len > 0 && !dict) { free(h); AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn); }
-  if (kind == kDict && dict && (reinterpret_cast<uintptr_t>(dict) & (width - 1))) { free(h); AG_FAIL(AG_ERR_INVALID, "%s: dictionary not aligned to its value width", fn); }
-  if (out && (reinterpret_cast<uintptr_t>(out) & ((kind == kLevels ? 2 : width) - 1))) { free(h); AG_FAIL(AG_ERR_INVALID, "%s: output not aligned to its element width", fn); }
+  if (n_tiles > 0 && !out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  if (any_data && !data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  if (kind == kDict && dict_len > 0 && !dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
+  if (kind == kDict && dict && (reinterpret_cast<uintptr_t>(dict) & (width - 1))) AG_FAIL(AG_ERR_INVALID, "%s: dictionary not aligned to its value width", fn);
+  if (out && (reinterpret_cast<uintptr_t>(out) & ((kind == kLevels ? 2 : width) - 1))) AG_FAIL(AG_ERR_INVALID, "%s: output not aligned to its element width", fn);
 
   const size_t st_bytes = (size_t)n_pages * sizeof(PageState);
   const size_t tc_bytes = valid ? (size_t)n_tiles * 8 : 0;
@@ -487,63 +485,52 @@ ag_status parquet_pages_dev(int kind, int fixed_bw, int v1, int width, const voi
   const size_t off_bad = (off_ti + (size_t)n_tiles * 8 + 255) & ~(size_t)255;
   const size_t off_runs = off_bad + 256;
   const size_t total = off_runs + (size_t)n_runs * 8;
-  uint8_t* d = nullptr;
-  ag_status rc = dev_alloc_async((void**)&d, total, st);
-  if (rc != AG_OK) { free(h); return rc; }
-  PageState* hs = (PageState*)malloc(st_bytes);
-  do {
-    if (!hs) { rc = AG_ERR_OOM; set_error("%s: host allocation failed", fn); break; }
-    if (cudaMemcpyAsync(d, h, plan_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "H2D", __FILE__, __LINE__); break; }
-    PqArgs a;
-    a.plan.pages = reinterpret_cast<const ag_pq_page*>(d);
-    a.plan.run_base = reinterpret_cast<const int64_t*>(d + pb);
-    a.plan.tile_base = a.plan.run_base + n_pages + 1;
-    a.plan.n_pages = n_pages;
-    a.plan.n_tiles = n_tiles;
-    a.data = data;
-    a.valid = valid;
-    a.st = reinterpret_cast<PageState*>(d + off_st);
-    a.tile_cnt = valid ? reinterpret_cast<int64_t*>(d + off_tc) : nullptr;
-    a.tile_info = reinterpret_cast<int2*>(d + off_ti);
-    a.bad = reinterpret_cast<unsigned long long*>(d_bad_pos ? (void*)d_bad_pos : (void*)(d + off_bad));
-    a.runs = n_runs ? reinterpret_cast<uint2*>(d + off_runs) : nullptr;
-    a.d_decoded = d_decoded;
-    a.kind = kind; a.fixed_bw = fixed_bw; a.v1 = v1; a.width = width;
-    a.dict_len = dict_len; a.dict = dict; a.out = out;
-    if (valid && n_tiles) {
-      pq_tile_count_kernel<<<grid_for(n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(a);
-      if ((rc = check_launch("pq_tile_count_kernel")) != AG_OK) break;
-    }
-    pq_runs_kernel<<<(unsigned)n_pages, kRleThreads, 0, st>>>(a);
-    if ((rc = check_launch("pq_runs_kernel")) != AG_OK) break;
-    if (kind == kLevels) rc = launch_expand<kLevels, int16_t, false>(a, st);
-    else if (kind == kDict && width == 4) rc = valid ? launch_expand<kDict, uint32_t, true>(a, st) : launch_expand<kDict, uint32_t, false>(a, st);
-    else if (kind == kDict) rc = valid ? launch_expand<kDict, unsigned long long, true>(a, st) : launch_expand<kDict, unsigned long long, false>(a, st);
-    else if (width == 4) rc = valid ? launch_expand<kPlain, uint32_t, true>(a, st) : launch_expand<kPlain, uint32_t, false>(a, st);
-    else rc = valid ? launch_expand<kPlain, unsigned long long, true>(a, st) : launch_expand<kPlain, unsigned long long, false>(a, st);
-    if (rc != AG_OK) break;
-    int64_t bad = AG_NO_ERROR_POS;
-    if (cudaMemcpyAsync(hs, a.st, st_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        (kind == kDict && cudaMemcpyAsync(&bad, a.bad, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-        cudaStreamSynchronize(st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__); break; }
-    if (h_decoded)
-      for (int64_t i = 0; i < n_pages; ++i) h_decoded[i] = hs[i].slots;
-    for (int64_t i = 0; i < n_pages; ++i) {
-      if (hs[i].err != kErrNone) {
-        rc = AG_ERR_INVALID;
-        set_error("%s: page %lld: %s (%lld values decoded)", fn, (long long)i, err_text(hs[i].err), (long long)hs[i].slots);
-        break;
-      }
-    }
-    if (rc == AG_OK && bad != AG_NO_ERROR_POS) {
-      rc = AG_ERR_INVALID;
-      set_error("%s: invalid index values found for dictionary converter (output slot %lld)", fn, (long long)bad);
-    }
-  } while (0);
-  cudaFreeAsync(d, st);
-  free(hs);
-  free(h);
-  return rc;
+  // this call synchronises `st` anyway, so its device scratch may live in a Temps
+  Temps t(st);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, total));
+  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  PqArgs a;
+  a.plan.pages = reinterpret_cast<const ag_pq_page*>(d);
+  a.plan.run_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.plan.tile_base = a.plan.run_base + n_pages + 1;
+  a.plan.n_pages = n_pages;
+  a.plan.n_tiles = n_tiles;
+  a.data = data;
+  a.valid = valid;
+  a.st = reinterpret_cast<PageState*>(d + off_st);
+  a.tile_cnt = valid ? reinterpret_cast<int64_t*>(d + off_tc) : nullptr;
+  a.tile_info = reinterpret_cast<int2*>(d + off_ti);
+  a.bad = reinterpret_cast<unsigned long long*>(d_bad_pos ? (void*)d_bad_pos : (void*)(d + off_bad));
+  a.runs = n_runs ? reinterpret_cast<uint2*>(d + off_runs) : nullptr;
+  a.d_decoded = d_decoded;
+  a.kind = kind; a.fixed_bw = fixed_bw; a.v1 = v1; a.width = width;
+  a.dict_len = dict_len; a.dict = dict; a.out = out;
+  if (valid && n_tiles) {
+    pq_tile_count_kernel<<<grid_for(n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(a);
+    AG_TRY(check_launch("pq_tile_count_kernel"));
+  }
+  pq_runs_kernel<<<(unsigned)n_pages, kRleThreads, 0, st>>>(a);
+  AG_TRY(check_launch("pq_runs_kernel"));
+  ag_status rc;
+  if (kind == kLevels) rc = launch_expand<kLevels, int16_t, false>(a, st);
+  else if (kind == kDict && width == 4) rc = valid ? launch_expand<kDict, uint32_t, true>(a, st) : launch_expand<kDict, uint32_t, false>(a, st);
+  else if (kind == kDict) rc = valid ? launch_expand<kDict, unsigned long long, true>(a, st) : launch_expand<kDict, unsigned long long, false>(a, st);
+  else if (width == 4) rc = valid ? launch_expand<kPlain, uint32_t, true>(a, st) : launch_expand<kPlain, uint32_t, false>(a, st);
+  else rc = valid ? launch_expand<kPlain, unsigned long long, true>(a, st) : launch_expand<kPlain, unsigned long long, false>(a, st);
+  AG_TRY(rc);
+  std::vector<PageState> hs((size_t)n_pages);
+  int64_t bad = AG_NO_ERROR_POS;
+  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
+  if (kind == kDict) AG_TRY(d2h(&bad, a.bad, 8, st));
+  AG_TRY(sync(st));
+  if (h_decoded)
+    for (int64_t i = 0; i < n_pages; ++i) h_decoded[i] = hs[i].slots;
+  for (int64_t i = 0; i < n_pages; ++i)
+    if (hs[i].err != kErrNone)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: %s (%lld values decoded)", fn, (long long)i, err_text(hs[i].err), (long long)hs[i].slots);
+  if (bad != AG_NO_ERROR_POS) AG_FAIL(AG_ERR_INVALID, "%s: invalid index values found for dictionary converter (output slot %lld)", fn, (long long)bad);
+  return AG_OK;
 }
 
 static int bit_len(int v) { int n = 0; while (v) { ++n; v >>= 1; } return n; }
@@ -574,40 +561,31 @@ static ag_status pages_host(int kind, int fixed_bw, int v1, int width, const voi
   if (kind == kDict && dict_len > 0 && !dict) AG_FAIL(AG_ERR_INVALID, "NULL dictionary");
   const int esz = kind == kLevels ? 2 : width;
   CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
   const size_t vbytes = valid ? (size_t)((slot_end + 7) >> 3) : 0;
   const size_t dbytes = kind == kDict ? (size_t)dict_len * width : 0;
   const size_t o_valid = ((size_t)data_end + 255) & ~(size_t)255;
   const size_t o_dict = (o_valid + vbytes + 255) & ~(size_t)255;
   const size_t o_out = (o_dict + dbytes + 255) & ~(size_t)255;
   const size_t o_bad = (o_out + (size_t)slot_end * esz + 255) & ~(size_t)255;
-  uint8_t* d = nullptr;
-  AG_TRY(dev_alloc_async((void**)&d, o_bad + 64, cs));
-  int64_t* dec = (int64_t*)calloc((size_t)n_pages, 8);   // stays 0 when the call fails before decoding
-  ag_status rc = dec ? AG_OK : AG_ERR_OOM;
-  if (!dec) set_error("host allocation failed");
-  if (rc == AG_OK && ((data_end && cudaMemcpyAsync(d, data, (size_t)data_end, cudaMemcpyHostToDevice, cs) != cudaSuccess) ||
-                      (vbytes && cudaMemcpyAsync(d + o_valid, valid, vbytes, cudaMemcpyHostToDevice, cs) != cudaSuccess) ||
-                      (dbytes && cudaMemcpyAsync(d + o_dict, dict, dbytes, cudaMemcpyHostToDevice, cs) != cudaSuccess)))
-    rc = cuda_fail(cudaGetLastError(), "H2D", __FILE__, __LINE__);
-  if (rc == AG_OK) {
-    rc = parquet_pages_dev(kind, fixed_bw, v1, width, dbytes ? d + o_dict : nullptr, dict_len, d, pages, n_pages, vbytes ? d + o_valid : nullptr,
-                           d + o_out, nullptr, dec, reinterpret_cast<int64_t*>(d + o_bad), cs);
-    // a decode error still delivers the values decoded before it
-    if (rc == AG_OK || rc == AG_ERR_INVALID) {
-      const ag_status rc2 = rc;
-      for (int64_t i = 0; i < n_pages; ++i) {
-        const size_t off = (size_t)pages[i].out * esz, nb = (size_t)dec[i] * esz;
-        if (nb && cudaMemcpyAsync((uint8_t*)out + off, d + o_out + off, nb, cudaMemcpyDeviceToHost, cs) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__); break; }
-      }
-      if (rc == rc2 && kind == kDict && bad_pos && cudaMemcpyAsync(bad_pos, d + o_bad, 8, cudaMemcpyDeviceToHost, cs) != cudaSuccess) rc = cuda_fail(cudaGetLastError(), "D2H", __FILE__, __LINE__);
-      if (cudaStreamSynchronize(cs) != cudaSuccess && rc == AG_OK) rc = cuda_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-      if (decoded) memcpy(decoded, dec, (size_t)n_pages * 8);
-    }
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, o_bad));
+  AG_TRY(h2d(d, data, (size_t)data_end, cs));
+  AG_TRY(h2d(d + o_valid, valid, vbytes, cs));
+  AG_TRY(h2d(d + o_dict, dict, dbytes, cs));
+  std::vector<int64_t> dec((size_t)n_pages, 0);   // stays 0 when the call fails before decoding
+  const ag_status rc = parquet_pages_dev(kind, fixed_bw, v1, width, dbytes ? d + o_dict : nullptr, dict_len, d, pages, n_pages,
+                                         vbytes ? d + o_valid : nullptr, d + o_out, nullptr, dec.data(), reinterpret_cast<int64_t*>(d + o_bad), cs);
+  // a decode error still delivers the values decoded before it
+  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
+  if (decoded) memcpy(decoded, dec.data(), (size_t)n_pages * 8);
+  for (int64_t i = 0; i < n_pages; ++i) {
+    const size_t off = (size_t)pages[i].out * esz;
+    AG_TRY(d2h((uint8_t*)out + off, d + o_out + off, (size_t)dec[i] * esz, cs));
   }
-  cudaStreamSynchronize(cs);
-  cudaFreeAsync(d, cs);
-  free(dec);
-  return rc;
+  if (kind == kDict && bad_pos) AG_TRY(d2h(bad_pos, d + o_bad, 8, cs));
+  const ag_status rs = sync(cs);
+  return rc != AG_OK ? rc : rs;
 }
 
 }  // namespace ag

@@ -53,6 +53,10 @@ def test_reference_known_answers(ag):
     assert gpu_sum_f64(ag, e, "ag_sum_f64_reforder") == 0.0
     ag.call("ag_sum_i64", None, 0, C.byref(r))
     assert r.value == 0
+    # a NULL buffer with rows is an error and leaves the result untouched
+    rf = C.c_double(123.0)
+    st, _ = ag.call_status("ag_sum_f64", None, 4, C.byref(rf))
+    assert st == ag.AG_ERR_INVALID and rf.value == 123.0
 
 
 @pytest.mark.parametrize("n", [1, 2, 3, 31, 32, 33, 63, 64, 255, 256, 257, 1000, 2047, 2048, 8192, 100003, 1 << 20, (1 << 22) + 5])

@@ -141,6 +141,8 @@ def test_def_levels_random_vs_model(ag):
                 ag.call("ag_parquet_def_levels_to_bitmap", ptr(lv), n, 3, ancestor, ptr(got), off, n, C.byref(rd), C.byref(nc))
                 assert rd.value == read and nc.value == 7 + read - setc, (n, ancestor, off)
                 assert np.array_equal(unpack_bits(got, 0, off + read), unpack_bits(want, 0, off + read)), (n, ancestor, off)
+                # bytes past the one holding the last bit read keep the caller's values
+                assert np.array_equal(got[(off + read + 7) >> 3:], vb[(off + read + 7) >> 3:]), (n, ancestor, off)
                 # device flavour
                 dl, dv, dc = Dev(lv), Dev(vb.copy()), Dev(np.zeros(2, dtype=np.int64))
                 ag.call("ag_parquet_def_levels_to_bitmap_dev", dl.ptr, n, 3, ancestor, dv.ptr, off, n, dc.ptr, None)

@@ -270,24 +270,6 @@ ag_status cast_io(const void* in, void* out, int64_t n, const uint8_t* valid, in
   }
 }
 
-template <typename I>
-ag_status cast_i(int otype, const void* in, void* out, int64_t n, const uint8_t* valid, int64_t voff,
-                 int aio, int aft, int64_t* first_bad, int64_t row_base, cudaStream_t st) {
-  switch (otype) {
-    case AG_TYPE_UINT8: return cast_io<I, uint8_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT8: return cast_io<I, int8_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT16: return cast_io<I, uint16_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT16: return cast_io<I, int16_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT32: return cast_io<I, uint32_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT32: return cast_io<I, int32_t>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT64: return cast_io<I, unsigned long long>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT64: return cast_io<I, long long>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_FLOAT32: return cast_io<I, float>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_FLOAT64: return cast_io<I, double>(in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    default: AG_FAIL(AG_ERR_TYPE, "cast: unsupported output type id %d", otype);
-  }
-}
-
 }  // namespace
 
 ag_status cast_numeric_dev(int itype, int otype, const void* in, const uint8_t* valid, int64_t voff, void* out, int64_t n,
@@ -301,20 +283,12 @@ ag_status cast_numeric_dev(int itype, int otype, const void* in, const uint8_t* 
     AG_CUDA_TRY(cudaMemcpyAsync(out, in, (size_t)n * type_width(itype), cudaMemcpyDeviceToDevice, st));
     return AG_OK;
   }
-  const int aio = allow_int_overflow, aft = allow_float_truncate;
-  switch (itype) {
-    case AG_TYPE_UINT8: return cast_i<uint8_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT8: return cast_i<int8_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT16: return cast_i<uint16_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT16: return cast_i<int16_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT32: return cast_i<uint32_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT32: return cast_i<int32_t>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_UINT64: return cast_i<unsigned long long>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_INT64: return cast_i<long long>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_FLOAT32: return cast_i<float>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    case AG_TYPE_FLOAT64: return cast_i<double>(otype, in, out, n, valid, voff, aio, aft, first_bad, row_base, st);
-    default: AG_FAIL(AG_ERR_TYPE, "cast: unsupported input type id %d", itype);
-  }
+  return visit_type(itype, [&](auto itag) {
+    return visit_type(otype, [&](auto otag) {
+      return cast_io<typename decltype(itag)::type, typename decltype(otag)::type>(in, out, n, valid, voff, allow_int_overflow,
+                                                                                 allow_float_truncate, first_bad, row_base, st);
+    }, [&] { AG_FAIL(AG_ERR_TYPE, "cast: unsupported output type id %d", otype); });
+  }, [&] { AG_FAIL(AG_ERR_TYPE, "cast: unsupported input type id %d", itype); });
 }
 
 }  // namespace ag

@@ -8,6 +8,7 @@
 #include <stdio.h>
 #include <atomic>
 #include <mutex>
+#include <type_traits>
 
 #include "../../include/arrowgpu.h"
 
@@ -160,12 +161,77 @@ inline bool type_is_unsigned_int(int type) {
 }
 inline bool type_is_float(int type) { return type == AG_TYPE_FLOAT32 || type == AG_TYPE_FLOAT64; }
 
+// ---------------------------------------------------------------- kernel dispatch ----
+// How an ABI argument picks a kernel instantiation.  Each visitor calls `f` with a TypeTag<T> (visit_shape: a
+// std::integral_constant) and returns what `f` returns; a value it does not map goes to `unsupported()` instead,
+// so the caller keeps its own status and message.  A caller that takes a subset (integers only, say) checks before
+// the call or branches with `if constexpr` inside `f`; the branch also keeps kernels of the other types from
+// being instantiated.
+template <typename T> struct TypeTag { using type = T; };
+
+// Exact type: each of the 10 numeric type ids as its own C++ type.
+template <typename F, typename U>
+inline ag_status visit_type(int type, F&& f, U&& unsupported) {
+  switch (type) {
+    case AG_TYPE_UINT8: return f(TypeTag<uint8_t>{});
+    case AG_TYPE_INT8: return f(TypeTag<int8_t>{});
+    case AG_TYPE_UINT16: return f(TypeTag<uint16_t>{});
+    case AG_TYPE_INT16: return f(TypeTag<int16_t>{});
+    case AG_TYPE_UINT32: return f(TypeTag<uint32_t>{});
+    case AG_TYPE_INT32: return f(TypeTag<int32_t>{});
+    case AG_TYPE_UINT64: return f(TypeTag<unsigned long long>{});
+    case AG_TYPE_INT64: return f(TypeTag<long long>{});
+    case AG_TYPE_FLOAT32: return f(TypeTag<float>{});
+    case AG_TYPE_FLOAT64: return f(TypeTag<double>{});
+    default: return unsupported();
+  }
+}
+
+// Storage type: signed and unsigned integers of one width share the unsigned type; floats stay as they are.  For
+// ops whose result bits do not depend on signedness: two's-complement add/sub/mul (base_arithmetic.cc:121-148 makes
+// the same move for Multiply), bitwise ops, == and !=.
+template <typename F, typename U>
+inline ag_status visit_storage_type(int type, F&& f, U&& unsupported) {
+  switch (type) {
+    case AG_TYPE_UINT8: case AG_TYPE_INT8: return f(TypeTag<uint8_t>{});
+    case AG_TYPE_UINT16: case AG_TYPE_INT16: return f(TypeTag<uint16_t>{});
+    case AG_TYPE_UINT32: case AG_TYPE_INT32: return f(TypeTag<uint32_t>{});
+    case AG_TYPE_UINT64: case AG_TYPE_INT64: return f(TypeTag<unsigned long long>{});
+    case AG_TYPE_FLOAT32: return f(TypeTag<float>{});
+    case AG_TYPE_FLOAT64: return f(TypeTag<double>{});
+    default: return unsupported();
+  }
+}
+
+// Width: a value or index width of 8/16/32/64 bits as the unsigned integer of that size.
+template <typename F, typename U>
+inline ag_status visit_width(int bits, F&& f, U&& unsupported) {
+  switch (bits) {
+    case 8: return f(TypeTag<uint8_t>{});
+    case 16: return f(TypeTag<uint16_t>{});
+    case 32: return f(TypeTag<uint32_t>{});
+    case 64: return f(TypeTag<unsigned long long>{});
+    default: return unsupported();
+  }
+}
+
+// Operand shape of a binary op: AG_SHAPE_AA / AS / SA as a compile-time constant.
+template <typename F, typename U>
+inline ag_status visit_shape(int shape, F&& f, U&& unsupported) {
+  switch (shape) {
+    case AG_SHAPE_AA: return f(std::integral_constant<int, AG_SHAPE_AA>{});
+    case AG_SHAPE_AS: return f(std::integral_constant<int, AG_SHAPE_AS>{});
+    case AG_SHAPE_SA: return f(std::integral_constant<int, AG_SHAPE_SA>{});
+    default: return unsupported();
+  }
+}
+
 inline int64_t bytes_for_bits(int64_t nbits) { return (nbits + 7) >> 3; }
 
 int blocks_per_sm(const void* kernel, int threads);
 // Opt a kernel into `bytes` of dynamic shared memory on the calling thread's device, once per device
 // (`done` = the caller's per-instantiation bit set; the attribute is per function per context).
-inline ag_status ensure_dynamic_smem(const void* kernel, int bytes, std::atomic<unsigned>* done) {
+static inline ag_status ensure_dynamic_smem(const void* kernel, int bytes, std::atomic<unsigned>* done) {
   const unsigned bit = 1u << (current_device() & 31);
   if (done->load(std::memory_order_acquire) & bit) return AG_OK;
   AG_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));

@@ -103,54 +103,14 @@ static ag_status launch_cmp_shape(int shape, const void* l, const void* r, uint8
   const int shift = (int)(p & 3) * 8 + (bit_offset & 7);
   const int64_t n_words = (n + shift + 31) >> 5;
   const int64_t blocks_needed = (((n_words + 31) >> 5) + kCmpThreads / 32 - 1) / (kCmpThreads / 32);
-  int grid;
-  switch (shape) {
-    case AG_SHAPE_AA:
-      grid = grid_one_wave(compare_kernel<T, Cmp, AG_SHAPE_AA>, kCmpThreads, blocks_needed);
-      compare_kernel<T, Cmp, AG_SHAPE_AA><<<grid, kCmpThreads, 0, st>>>((const T*)l, (const T*)r, T(0), words, shift, n, n_words);
-      break;
-    case AG_SHAPE_AS:
-      grid = grid_one_wave(compare_kernel<T, Cmp, AG_SHAPE_AS>, kCmpThreads, blocks_needed);
-      compare_kernel<T, Cmp, AG_SHAPE_AS><<<grid, kCmpThreads, 0, st>>>((const T*)l, nullptr, *(const T*)r, words, shift, n, n_words);
-      break;
-    case AG_SHAPE_SA:
-      grid = grid_one_wave(compare_kernel<T, Cmp, AG_SHAPE_SA>, kCmpThreads, blocks_needed);
-      compare_kernel<T, Cmp, AG_SHAPE_SA><<<grid, kCmpThreads, 0, st>>>(nullptr, (const T*)r, *(const T*)l, words, shift, n, n_words);
-      break;
-    default: AG_FAIL(AG_ERR_INVALID, "compare: bad operand shape %d", shape);
-  }
-  return check_launch("compare_kernel");
-}
-
-template <typename Cmp>
-static ag_status launch_cmp_ordered(int type, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st) {
-  switch (type) {
-    case AG_TYPE_UINT8: return launch_cmp_shape<uint8_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_INT8: return launch_cmp_shape<int8_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT16: return launch_cmp_shape<uint16_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_INT16: return launch_cmp_shape<int16_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT32: return launch_cmp_shape<uint32_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_INT32: return launch_cmp_shape<int32_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT64: return launch_cmp_shape<unsigned long long, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_INT64: return launch_cmp_shape<long long, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_FLOAT32: return launch_cmp_shape<float, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_FLOAT64: return launch_cmp_shape<double, Cmp>(shape, l, r, out, n, off, st);
-    default: AG_FAIL(AG_ERR_TYPE, "compare: unsupported type id %d", type);
-  }
-}
-
-// ==/!= only look at the bits for integers: signed and unsigned share kernels
-template <typename Cmp>
-static ag_status launch_cmp_equality(int type, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st) {
-  switch (type) {
-    case AG_TYPE_UINT8: case AG_TYPE_INT8: return launch_cmp_shape<uint8_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT16: case AG_TYPE_INT16: return launch_cmp_shape<uint16_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT32: case AG_TYPE_INT32: return launch_cmp_shape<uint32_t, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_UINT64: case AG_TYPE_INT64: return launch_cmp_shape<unsigned long long, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_FLOAT32: return launch_cmp_shape<float, Cmp>(shape, l, r, out, n, off, st);
-    case AG_TYPE_FLOAT64: return launch_cmp_shape<double, Cmp>(shape, l, r, out, n, off, st);
-    default: AG_FAIL(AG_ERR_TYPE, "compare: unsupported type id %d", type);
-  }
+  return visit_shape(shape, [&](auto s) {
+    constexpr int kShape = decltype(s)::value;
+    const T scalar = kShape == AG_SHAPE_AS ? *(const T*)r : (kShape == AG_SHAPE_SA ? *(const T*)l : T(0));
+    const int grid = grid_one_wave(compare_kernel<T, Cmp, kShape>, kCmpThreads, blocks_needed);
+    compare_kernel<T, Cmp, kShape><<<grid, kCmpThreads, 0, st>>>(kShape == AG_SHAPE_SA ? nullptr : (const T*)l,
+                                                                  kShape == AG_SHAPE_AS ? nullptr : (const T*)r, scalar, words, shift, n, n_words);
+    return check_launch("compare_kernel");
+  }, [&] { AG_FAIL(AG_ERR_INVALID, "compare: bad operand shape %d", shape); });
 }
 
 ag_status compare_dev(int type, int cmp, int shape, const void* l, const void* r, uint8_t* out, int64_t n, int off, cudaStream_t st) {
@@ -168,11 +128,16 @@ ag_status compare_dev(int type, int cmp, int shape, const void* l, const void* r
   const uintptr_t m = (uintptr_t)(w - 1);
   if ((shape != AG_SHAPE_SA && ((uintptr_t)l & m)) || (shape != AG_SHAPE_AS && ((uintptr_t)r & m)))
     AG_FAIL(AG_ERR_INVALID, "compare: operand not aligned to its element width");
+  const auto launch = [&](auto cmp_tag) {
+    return [&, cmp_tag](auto tag) { return launch_cmp_shape<typename decltype(tag)::type, decltype(cmp_tag)>(shape, l, r, out, n, off, st); };
+  };
+  const auto bad_type = [&] { AG_FAIL(AG_ERR_TYPE, "compare: unsupported type id %d", type); };
+  // ==/!= only look at the bits: they run on the storage type
   switch (cmp) {
-    case AG_CMP_EQ: return launch_cmp_equality<CmpEq>(type, shape, l, r, out, n, off, st);
-    case AG_CMP_NE: return launch_cmp_equality<CmpNe>(type, shape, l, r, out, n, off, st);
-    case AG_CMP_GT: return launch_cmp_ordered<CmpGt>(type, shape, l, r, out, n, off, st);
-    case AG_CMP_GE: return launch_cmp_ordered<CmpGe>(type, shape, l, r, out, n, off, st);
+    case AG_CMP_EQ: return visit_storage_type(type, launch(CmpEq{}), bad_type);
+    case AG_CMP_NE: return visit_storage_type(type, launch(CmpNe{}), bad_type);
+    case AG_CMP_GT: return visit_type(type, launch(CmpGt{}), bad_type);
+    case AG_CMP_GE: return visit_type(type, launch(CmpGe{}), bad_type);
     default: AG_FAIL(AG_ERR_INVALID, "compare: bad operator %d", cmp);
   }
 }

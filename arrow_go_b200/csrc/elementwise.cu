@@ -29,9 +29,7 @@ constexpr int kEwUnroll = 4;
 constexpr int kEwBlocksPerSM = 8;
 
 // ---------------------------------------------------------------- functors ---------
-// Integers run on the unsigned type of the same width: two's-complement add/sub/mul have
-// the same low bits for signed and unsigned operands (base_arithmetic.cc:121-148 makes the
-// same move for Multiply), so int8/uint8 ... int64/uint64 share kernels.
+// Integers run on their storage type (visit_storage_type), so int8/uint8 ... int64/uint64 share kernels.
 struct OpAdd { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { return (T)(a + b); } };
 struct OpSub { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { return (T)(a - b); } };
 struct OpMul {
@@ -93,69 +91,6 @@ __device__ __forceinline__ uint4 neighbour_vector(const uint4 cur, const uint4 n
 
 // ---------------------------------------------------------------- binary -----------
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
-template <typename T, typename Op, int kShape>
-static ag_status launch_single_span(const T* l, const T* r, T* out, int64_t n, T scalar, cudaStream_t st);
-
-template <typename T, typename Op, int kShape>
-static ag_status launch_binary_t(const void* l, const void* r, void* out, int64_t n, const void* scalar_host, cudaStream_t st) {
-  T scalar = T(0);
-  if (kShape != AG_SHAPE_AA) scalar = *reinterpret_cast<const T*>(scalar_host);
-  const T* lp = reinterpret_cast<const T*>(l);
-  const T* rp = reinterpret_cast<const T*>(r);
-  T* op = reinterpret_cast<T*>(out);
-  return launch_single_span<T, Op, kShape>(lp, rp, op, n, scalar, st);   // any element alignment
-}
-
-template <typename T, typename Op>
-static ag_status launch_binary_shape(int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st) {
-  switch (shape) {
-    case AG_SHAPE_AA: return launch_binary_t<T, Op, AG_SHAPE_AA>(l, r, out, n, nullptr, st);
-    case AG_SHAPE_AS: return launch_binary_t<T, Op, AG_SHAPE_AS>(l, nullptr, out, n, r, st);
-    case AG_SHAPE_SA: return launch_binary_t<T, Op, AG_SHAPE_SA>(nullptr, r, out, n, l, st);
-    default: AG_FAIL(AG_ERR_INVALID, "arith: bad operand shape %d", shape);
-  }
-}
-
-template <typename T>
-static ag_status launch_binary_op(int8_t op, int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st) {
-  switch (op) {
-    // the *_CHECKED aliases are the plain loops here, like the reference's native code
-    // (base_arithmetic.cc:445-462); the checking variants are ag_arith_checked.
-    case AG_OP_ADD: case AG_OP_ADD_CHECKED: return launch_binary_shape<T, OpAdd>(shape, l, r, out, n, st);
-    case AG_OP_SUB: case AG_OP_SUB_CHECKED: return launch_binary_shape<T, OpSub>(shape, l, r, out, n, st);
-    case AG_OP_MUL: case AG_OP_MUL_CHECKED: return launch_binary_shape<T, OpMul>(shape, l, r, out, n, st);
-    case AG_OP_BIT_AND: case AG_OP_BIT_OR: case AG_OP_BIT_XOR:
-      if constexpr (std::is_integral<T>::value) {
-        if (op == AG_OP_BIT_AND) return launch_binary_shape<T, OpBitAnd>(shape, l, r, out, n, st);
-        if (op == AG_OP_BIT_OR) return launch_binary_shape<T, OpBitOr>(shape, l, r, out, n, st);
-        return launch_binary_shape<T, OpBitXor>(shape, l, r, out, n, st);
-      } else {
-        AG_FAIL(AG_ERR_TYPE, "arith: bitwise ops take integer types");
-      }
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: binary op %d has no native kernel (the reference has none either)", (int)op);
-  }
-}
-
-ag_status arith_binary_dev(int type, int8_t op, int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st) {
-  if (n < 0) AG_FAIL(AG_ERR_INVALID, "arith: negative length");
-  if (n == 0) return AG_OK;
-  const int w = type_width(type);
-  if (w == 0) AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type);
-  const uintptr_t m = (uintptr_t)(w - 1);
-  if (((uintptr_t)out & m) || (shape != AG_SHAPE_SA && ((uintptr_t)l & m)) || (shape != AG_SHAPE_AS && ((uintptr_t)r & m)))
-    AG_FAIL(AG_ERR_INVALID, "arith: operand not aligned to its element width");
-  switch (type) {
-    case AG_TYPE_UINT8: case AG_TYPE_INT8: return launch_binary_op<uint8_t>(op, shape, l, r, out, n, st);
-    case AG_TYPE_UINT16: case AG_TYPE_INT16: return launch_binary_op<uint16_t>(op, shape, l, r, out, n, st);
-    case AG_TYPE_UINT32: case AG_TYPE_INT32: return launch_binary_op<uint32_t>(op, shape, l, r, out, n, st);
-    case AG_TYPE_UINT64: case AG_TYPE_INT64: return launch_binary_op<unsigned long long>(op, shape, l, r, out, n, st);
-    case AG_TYPE_FLOAT32: return launch_binary_op<float>(op, shape, l, r, out, n, st);
-    case AG_TYPE_FLOAT64: return launch_binary_op<double>(op, shape, l, r, out, n, st);
-    default: AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type);
-  }
-}
-
 
 // ---------------------------------------------------------------- batched spans -----
 // One launch for ALL aligned spans of a chunked call (iterateExecSpans, executor.go:757-863,
@@ -315,60 +250,74 @@ binary_spans_kernel(const SpanDesc* __restrict__ spans, int n_spans, long long t
   }
 }
 
-// The contiguous call: one span by value through the same tile kernel (contiguous 32 KB tiles per
-// block iteration streamed faster than a grid-strided loop).
-template <typename T, typename Op, int kShape>
-static ag_status launch_single_span(const T* l, const T* r, T* out, int64_t n, T scalar, cudaStream_t st) {
-  SpanDesc sp{l, r, out, (long long)n, 0};
-  const long long tiles = span_tiles(out, (int)sizeof(T), n);
-  if (span_needs_shift(kShape, l, r, out, (int)sizeof(T), n)) {
-    const int grid = grid_one_wave(binary_spans_kernel<T, Op, kShape, true, true>, kEwThreads, tiles);
-    binary_spans_kernel<T, Op, kShape, true, true><<<grid, kEwThreads, 0, st>>>(nullptr, 1, tiles, scalar, sp);
-  } else {
-    const int grid = grid_one_wave(binary_spans_kernel<T, Op, kShape, true, false>, kEwThreads, tiles);
-    binary_spans_kernel<T, Op, kShape, true, false><<<grid, kEwThreads, 0, st>>>(nullptr, 1, tiles, scalar, sp);
-  }
-  return check_launch("binary_spans_kernel");
-}
+// One launch of binary_spans_kernel.  A chunked call passes its device table of `n_spans` spans; the contiguous call
+// passes `d_spans` = NULL and its one span by value in `single`.  `scalar_host` is the host scalar of an AS / SA call.
+struct SpanLaunch {
+  const SpanDesc* d_spans;
+  int n_spans;
+  long long tiles;
+  const void* scalar_host;
+  bool shift;  // span_needs_shift for some span
+  SpanDesc single;
+};
 
 template <typename T, typename Op, int kShape>
-static ag_status launch_spans_t(const SpanDesc* d_spans, int n_spans, long long total_tiles, const void* scalar_host, bool shift, cudaStream_t st) {
-  T scalar = T(0);
-  if (kShape != AG_SHAPE_AA) scalar = *reinterpret_cast<const T*>(scalar_host);
-  if (shift) {
-    const int grid = grid_one_wave(binary_spans_kernel<T, Op, kShape, false, true>, kEwThreads, total_tiles);
-    binary_spans_kernel<T, Op, kShape, false, true><<<grid, kEwThreads, 0, st>>>(d_spans, n_spans, total_tiles, scalar, SpanDesc{});
-  } else {
-    const int grid = grid_one_wave(binary_spans_kernel<T, Op, kShape, false, false>, kEwThreads, total_tiles);
-    binary_spans_kernel<T, Op, kShape, false, false><<<grid, kEwThreads, 0, st>>>(d_spans, n_spans, total_tiles, scalar, SpanDesc{});
-  }
-  return check_launch("binary_spans_kernel");
+static ag_status launch_spans_t(const SpanLaunch& a, cudaStream_t st) {
+  const T scalar = kShape == AG_SHAPE_AA ? T(0) : *reinterpret_cast<const T*>(a.scalar_host);
+  const auto go = [&](auto kernel) {
+    kernel<<<grid_one_wave(kernel, kEwThreads, a.tiles), kEwThreads, 0, st>>>(a.d_spans, a.n_spans, a.tiles, scalar, a.single);
+    return check_launch("binary_spans_kernel");
+  };
+  if (!a.d_spans) return a.shift ? go(binary_spans_kernel<T, Op, kShape, true, true>) : go(binary_spans_kernel<T, Op, kShape, true, false>);
+  return a.shift ? go(binary_spans_kernel<T, Op, kShape, false, true>) : go(binary_spans_kernel<T, Op, kShape, false, false>);
 }
+
 template <typename T, typename Op>
-static ag_status launch_spans_shape(int shape, const SpanDesc* d, int n, long long tiles, const void* sc, bool shift, cudaStream_t st) {
-  switch (shape) {
-    case AG_SHAPE_AA: return launch_spans_t<T, Op, AG_SHAPE_AA>(d, n, tiles, sc, shift, st);
-    case AG_SHAPE_AS: return launch_spans_t<T, Op, AG_SHAPE_AS>(d, n, tiles, sc, shift, st);
-    case AG_SHAPE_SA: return launch_spans_t<T, Op, AG_SHAPE_SA>(d, n, tiles, sc, shift, st);
-    default: AG_FAIL(AG_ERR_INVALID, "arith: bad operand shape %d", shape);
-  }
+static ag_status launch_binary_shape(int shape, const SpanLaunch& a, cudaStream_t st) {
+  return visit_shape(shape, [&](auto s) { return launch_spans_t<T, Op, decltype(s)::value>(a, st); },
+                     [&] { AG_FAIL(AG_ERR_INVALID, "arith: bad operand shape %d", shape); });
 }
-template <typename T>
-static ag_status launch_spans_op(int8_t op, int shape, const SpanDesc* d, int n, long long tiles, const void* sc, bool shift, cudaStream_t st) {
-  switch (op) {
-    case AG_OP_ADD: case AG_OP_ADD_CHECKED: return launch_spans_shape<T, OpAdd>(shape, d, n, tiles, sc, shift, st);
-    case AG_OP_SUB: case AG_OP_SUB_CHECKED: return launch_spans_shape<T, OpSub>(shape, d, n, tiles, sc, shift, st);
-    case AG_OP_MUL: case AG_OP_MUL_CHECKED: return launch_spans_shape<T, OpMul>(shape, d, n, tiles, sc, shift, st);
-    case AG_OP_BIT_AND: case AG_OP_BIT_OR: case AG_OP_BIT_XOR:
-      if constexpr (std::is_integral<T>::value) {
-        if (op == AG_OP_BIT_AND) return launch_spans_shape<T, OpBitAnd>(shape, d, n, tiles, sc, shift, st);
-        if (op == AG_OP_BIT_OR) return launch_spans_shape<T, OpBitOr>(shape, d, n, tiles, sc, shift, st);
-        return launch_spans_shape<T, OpBitXor>(shape, d, n, tiles, sc, shift, st);
-      } else {
-        AG_FAIL(AG_ERR_TYPE, "arith: bitwise ops take integer types");
-      }
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: binary op %d has no native kernel", (int)op);
-  }
+
+static ag_status launch_binary(int type, int8_t op, int shape, const SpanLaunch& a, cudaStream_t st) {
+  return visit_storage_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    switch (op) {
+      // the *_CHECKED aliases are the plain loops here, like the reference's native code
+      // (base_arithmetic.cc:445-462); the checking variants are ag_arith_checked.
+      case AG_OP_ADD: case AG_OP_ADD_CHECKED: return launch_binary_shape<T, OpAdd>(shape, a, st);
+      case AG_OP_SUB: case AG_OP_SUB_CHECKED: return launch_binary_shape<T, OpSub>(shape, a, st);
+      case AG_OP_MUL: case AG_OP_MUL_CHECKED: return launch_binary_shape<T, OpMul>(shape, a, st);
+      case AG_OP_BIT_AND: case AG_OP_BIT_OR: case AG_OP_BIT_XOR:
+        if constexpr (std::is_integral<T>::value) {
+          if (op == AG_OP_BIT_AND) return launch_binary_shape<T, OpBitAnd>(shape, a, st);
+          if (op == AG_OP_BIT_OR) return launch_binary_shape<T, OpBitOr>(shape, a, st);
+          return launch_binary_shape<T, OpBitXor>(shape, a, st);
+        } else {
+          AG_FAIL(AG_ERR_TYPE, "arith: bitwise ops take integer types");
+        }
+      default:
+        AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: binary op %d has no native kernel%s", (int)op,
+                a.d_spans ? "" : " (the reference has none either)");
+    }
+  }, [&] { AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type); });
+}
+
+// The contiguous call: one span by value through the same tile kernel (contiguous 32 KB tiles per
+// block iteration streamed faster than a grid-strided loop), any element alignment.
+ag_status arith_binary_dev(int type, int8_t op, int shape, const void* l, const void* r, void* out, int64_t n, cudaStream_t st) {
+  if (n < 0) AG_FAIL(AG_ERR_INVALID, "arith: negative length");
+  if (n == 0) return AG_OK;
+  const int w = type_width(type);
+  if (w == 0) AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type);
+  const uintptr_t m = (uintptr_t)(w - 1);
+  if (((uintptr_t)out & m) || (shape != AG_SHAPE_SA && ((uintptr_t)l & m)) || (shape != AG_SHAPE_AS && ((uintptr_t)r & m)))
+    AG_FAIL(AG_ERR_INVALID, "arith: operand not aligned to its element width");
+  const void* lp = shape == AG_SHAPE_SA ? nullptr : l;
+  const void* rp = shape == AG_SHAPE_AS ? nullptr : r;
+  const void* scalar_host = shape == AG_SHAPE_AS ? r : (shape == AG_SHAPE_SA ? l : nullptr);
+  const SpanLaunch a{nullptr, 1, span_tiles(out, w, n), scalar_host, span_needs_shift(shape, lp, rp, out, w, n),
+                     SpanDesc{lp, rp, out, (long long)n, 0}};
+  return launch_binary(type, op, shape, a, st);
 }
 
 // spans: HOST array of {l, r, out, n} with DEVICE pointers (the scalar side is a HOST pointer to
@@ -404,17 +353,7 @@ ag_status arith_binary_spans_dev(int type, int8_t op, int shape, const ag_span3*
   // pageable source: the copy is staged before the call returns, so `desc` may die afterwards
   cudaError_t e = cudaMemcpyAsync(d_spans, desc.data(), desc.size() * sizeof(SpanDesc), cudaMemcpyHostToDevice, st);
   if (e != cudaSuccess) { cudaFreeAsync(d_spans, st); return cuda_fail(e, "span table upload", __FILE__, __LINE__); }
-  ag_status rc;
-  const int n = (int)desc.size();
-  switch (type) {
-    case AG_TYPE_UINT8: case AG_TYPE_INT8: rc = launch_spans_op<uint8_t>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    case AG_TYPE_UINT16: case AG_TYPE_INT16: rc = launch_spans_op<uint16_t>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    case AG_TYPE_UINT32: case AG_TYPE_INT32: rc = launch_spans_op<uint32_t>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    case AG_TYPE_UINT64: case AG_TYPE_INT64: rc = launch_spans_op<unsigned long long>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    case AG_TYPE_FLOAT32: rc = launch_spans_op<float>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    case AG_TYPE_FLOAT64: rc = launch_spans_op<double>(op, shape, d_spans, n, tiles, scalar_host, shift, st); break;
-    default: rc = AG_ERR_TYPE; set_error("arith: unsupported type id %d", type); break;
-  }
+  const ag_status rc = launch_binary(type, op, shape, SpanLaunch{d_spans, (int)desc.size(), tiles, scalar_host, shift, SpanDesc{}}, st);
   cudaFreeAsync(d_spans, st);
   return rc;
 }
@@ -555,53 +494,30 @@ static ag_status launch_unary_same_op(int8_t op, const void* in, void* out, int6
 ag_status arith_unary_same_dev(int type, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st) {
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "arith: negative length");
   if (n == 0) return AG_OK;
-  switch (type) {
-    case AG_TYPE_UINT8: return launch_unary_same_op<uint8_t>(op, in, out, n, st);
-    case AG_TYPE_INT8: return launch_unary_same_op<int8_t>(op, in, out, n, st);
-    case AG_TYPE_UINT16: return launch_unary_same_op<uint16_t>(op, in, out, n, st);
-    case AG_TYPE_INT16: return launch_unary_same_op<int16_t>(op, in, out, n, st);
-    case AG_TYPE_UINT32: return launch_unary_same_op<uint32_t>(op, in, out, n, st);
-    case AG_TYPE_INT32: return launch_unary_same_op<int32_t>(op, in, out, n, st);
-    case AG_TYPE_UINT64: return launch_unary_same_op<unsigned long long>(op, in, out, n, st);
-    case AG_TYPE_INT64: return launch_unary_same_op<long long>(op, in, out, n, st);
-    case AG_TYPE_FLOAT32: return launch_unary_same_op<float>(op, in, out, n, st);
-    case AG_TYPE_FLOAT64: return launch_unary_same_op<double>(op, in, out, n, st);
-    default: AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type);
-  }
+  return visit_type(type, [&](auto tag) { return launch_unary_same_op<typename decltype(tag)::type>(op, in, out, n, st); },
+                    [&] { AG_FAIL(AG_ERR_TYPE, "arith: unsupported type id %d", type); });
 }
 
 template <typename TI>
 static ag_status launch_sign_diff(int otype, const void* in, void* out, int64_t n, cudaStream_t st) {
   const int grid = grid_for(n, kEwThreads * kEwUnroll, kEwBlocksPerSM);
-#define AG_SIGN_CASE(ID, TO) \
-  case ID: unary_scalar_kernel<TI, TO, USign><<<grid, kEwThreads, 0, st>>>((const TI*)in, (TO*)out, n); break;
-  switch (otype) {
-    AG_SIGN_CASE(AG_TYPE_UINT8, uint8_t) AG_SIGN_CASE(AG_TYPE_INT8, int8_t)
-    AG_SIGN_CASE(AG_TYPE_UINT16, uint16_t) AG_SIGN_CASE(AG_TYPE_INT16, int16_t)
-    AG_SIGN_CASE(AG_TYPE_UINT32, uint32_t) AG_SIGN_CASE(AG_TYPE_INT32, int32_t)
-    AG_SIGN_CASE(AG_TYPE_UINT64, unsigned long long) AG_SIGN_CASE(AG_TYPE_INT64, long long)
-    AG_SIGN_CASE(AG_TYPE_FLOAT32, float) AG_SIGN_CASE(AG_TYPE_FLOAT64, double)
-    default: AG_FAIL(AG_ERR_TYPE, "arith: unsupported output type id %d", otype);
-  }
-#undef AG_SIGN_CASE
-  return check_launch("sign_diff_kernel");
+  return visit_type(otype, [&](auto tag) {
+    using TO = typename decltype(tag)::type;
+    unary_scalar_kernel<TI, TO, USign><<<grid, kEwThreads, 0, st>>>((const TI*)in, (TO*)out, n);
+    return check_launch("sign_diff_kernel");
+  }, [&] { AG_FAIL(AG_ERR_TYPE, "arith: unsupported output type id %d", otype); });
 }
 
 ag_status arith_unary_diff_dev(int itype, int otype, int8_t op, const void* in, void* out, int64_t n, cudaStream_t st) {
   if (op != AG_OP_SIGN) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: unary_diff_type only implements SIGN (base_arithmetic.cc:427-438)");
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "arith: negative length");
   if (n == 0) return AG_OK;
-  switch (itype) {
-    case AG_TYPE_UINT8: return launch_sign_diff<uint8_t>(otype, in, out, n, st);
-    case AG_TYPE_INT8: return launch_sign_diff<int8_t>(otype, in, out, n, st);
-    case AG_TYPE_UINT16: return launch_sign_diff<uint16_t>(otype, in, out, n, st);
-    case AG_TYPE_INT16: return launch_sign_diff<int16_t>(otype, in, out, n, st);
-    case AG_TYPE_UINT32: return launch_sign_diff<uint32_t>(otype, in, out, n, st);
-    case AG_TYPE_INT32: return launch_sign_diff<int32_t>(otype, in, out, n, st);
-    case AG_TYPE_UINT64: return launch_sign_diff<unsigned long long>(otype, in, out, n, st);
-    case AG_TYPE_INT64: return launch_sign_diff<long long>(otype, in, out, n, st);
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: sign with differing types needs an integer input");
-  }
+  const auto not_int = [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith: sign with differing types needs an integer input"); };
+  return visit_type(itype, [&](auto tag) {
+    using TI = typename decltype(tag)::type;
+    if constexpr (std::is_integral<TI>::value) return launch_sign_diff<TI>(otype, in, out, n, st);
+    else return not_int();
+  }, not_int);
 }
 
 // ---------------------------------------------------------------- checked ----------
@@ -834,32 +750,26 @@ static ag_status launch_checked_shape(int shape, const void* l, const uint8_t* l
   long long* fb = reinterpret_cast<long long*>(d_first_bad);
   const bool hv = kNotNull && ((shape != AG_SHAPE_SA && lvalid) || (shape != AG_SHAPE_AS && rvalid));
   const bool vec = aligned16(out) && (shape == AG_SHAPE_SA || aligned16(l)) && (shape == AG_SHAPE_AS || aligned16(r));
-#define AG_CHK_LAUNCH(SHAPE, HV, L, LV, LO, R, RV, RO, SC)                                                                                      \
-  do {                                                                                                                                          \
-    if (vec)                                                                                                                                    \
-      checked_tile_kernel<ST, Op, SHAPE, kNotNull, HV>                                                                                          \
-          <<<grid_one_wave(checked_tile_kernel<ST, Op, SHAPE, kNotNull, HV>, kEwThreads, (n + kSpanTile - 1) / kSpanTile), kEwThreads, 0, st>>>( \
-              (const ST*)(L), LV, LO, (const ST*)(R), RV, RO, (ST*)out, n, SC, fb);                                                             \
-    else                                                                                                                                        \
-      checked_kernel<ST, Op, SHAPE, kNotNull, HV><<<grid, kEwThreads, 0, st>>>((const ST*)(L), LV, LO, (const ST*)(R), RV, RO, (ST*)out, n, SC, fb); \
-  } while (0)
-  switch (shape) {
-    case AG_SHAPE_AA:
-      if (hv) AG_CHK_LAUNCH(AG_SHAPE_AA, true, l, lvalid, loff, r, rvalid, roff, ST(0));
-      else AG_CHK_LAUNCH(AG_SHAPE_AA, false, l, nullptr, 0, r, nullptr, 0, ST(0));
-      break;
-    case AG_SHAPE_AS:
-      if (hv) AG_CHK_LAUNCH(AG_SHAPE_AS, true, l, lvalid, loff, nullptr, nullptr, 0, *(const ST*)r);
-      else AG_CHK_LAUNCH(AG_SHAPE_AS, false, l, nullptr, 0, nullptr, nullptr, 0, *(const ST*)r);
-      break;
-    case AG_SHAPE_SA:
-      if (hv) AG_CHK_LAUNCH(AG_SHAPE_SA, true, nullptr, nullptr, 0, r, rvalid, roff, *(const ST*)l);
-      else AG_CHK_LAUNCH(AG_SHAPE_SA, false, nullptr, nullptr, 0, r, nullptr, 0, *(const ST*)l);
-      break;
-    default: AG_FAIL(AG_ERR_INVALID, "arith_checked: bad operand shape %d", shape);
-  }
-#undef AG_CHK_LAUNCH
-  return check_launch("checked_kernel");
+  return visit_shape(shape, [&](auto s) {
+    constexpr int kShape = decltype(s)::value;
+    // the scalar side passes no array and no bitmap; only the kHasValid instantiation gets the bitmaps
+    const ST* lp = kShape == AG_SHAPE_SA ? nullptr : (const ST*)l;
+    const ST* rp = kShape == AG_SHAPE_AS ? nullptr : (const ST*)r;
+    const ST scalar = kShape == AG_SHAPE_AS ? *(const ST*)r : (kShape == AG_SHAPE_SA ? *(const ST*)l : ST(0));
+    const bool lbits = hv && kShape != AG_SHAPE_SA, rbits = hv && kShape != AG_SHAPE_AS;
+    const uint8_t* lv = lbits ? lvalid : nullptr;
+    const uint8_t* rv = rbits ? rvalid : nullptr;
+    const int64_t lo = lbits ? loff : 0, ro = rbits ? roff : 0;
+    const auto go = [&](auto tile_kernel, auto row_kernel) {
+      if (vec)
+        tile_kernel<<<grid_one_wave(tile_kernel, kEwThreads, (n + kSpanTile - 1) / kSpanTile), kEwThreads, 0, st>>>(lp, lv, lo, rp, rv, ro, (ST*)out, n, scalar, fb);
+      else
+        row_kernel<<<grid, kEwThreads, 0, st>>>(lp, lv, lo, rp, rv, ro, (ST*)out, n, scalar, fb);
+      return check_launch("checked_kernel");
+    };
+    if (hv) return go(checked_tile_kernel<ST, Op, kShape, kNotNull, true>, checked_kernel<ST, Op, kShape, kNotNull, true>);
+    return go(checked_tile_kernel<ST, Op, kShape, kNotNull, false>, checked_kernel<ST, Op, kShape, kNotNull, false>);
+  }, [&] { AG_FAIL(AG_ERR_INVALID, "arith_checked: bad operand shape %d", shape); });
 }
 
 template <typename ST>
@@ -897,19 +807,11 @@ ag_status arith_checked_dev(int type, int8_t op, int shape, const void* l, const
   if (n == 0) return AG_OK;
   // null scalar: "fast path if one side is entirely null" (helpers.go:287,314,341) — output untouched
   if ((shape == AG_SHAPE_SA && !l) || (shape == AG_SHAPE_AS && !r)) return AG_OK;
-  switch (type) {
-    case AG_TYPE_INT8: return launch_checked_op<int8_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_INT16: return launch_checked_op<int16_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_INT32: return launch_checked_op<int32_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_INT64: return launch_checked_op<long long>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_UINT8: return launch_checked_op<uint8_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_UINT16: return launch_checked_op<uint16_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_UINT32: return launch_checked_op<uint32_t>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_UINT64: return launch_checked_op<unsigned long long>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_FLOAT32: return launch_checked_fdiv<float>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    case AG_TYPE_FLOAT64: return launch_checked_fdiv<double>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
-    default: AG_FAIL(AG_ERR_TYPE, "arith_checked: type id %d is not a numeric type", type);
-  }
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if constexpr (std::is_floating_point<T>::value) return launch_checked_fdiv<T>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
+    else return launch_checked_op<T>(op, shape, l, lvalid, loff, r, rvalid, roff, out, n, d_first_bad, st);
+  }, [&] { AG_FAIL(AG_ERR_TYPE, "arith_checked: type id %d is not a numeric type", type); });
 }
 
 // AbsoluteValueChecked / NegateChecked on signed integers (base_arithmetic.go:295-340): ScalarUnary,
@@ -948,13 +850,13 @@ ag_status arith_unary_checked_dev(int type, int8_t op, const void* in, void* out
   if (op != AG_OP_ABS_CHECKED && op != AG_OP_NEGATE_CHECKED) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "arith_unary_checked: op %d", (int)op);
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "arith: negative length");
   if (n == 0) return AG_OK;
-  switch (type) {
-    case AG_TYPE_INT8: return launch_unary_checked<int8_t>(op, in, out, n, d_first_bad, st);
-    case AG_TYPE_INT16: return launch_unary_checked<int16_t>(op, in, out, n, d_first_bad, st);
-    case AG_TYPE_INT32: return launch_unary_checked<int32_t>(op, in, out, n, d_first_bad, st);
-    case AG_TYPE_INT64: return launch_unary_checked<long long>(op, in, out, n, d_first_bad, st);
-    default: return arith_unary_same_dev(type, op, in, out, n, st);  // unsigned / floating: cannot overflow
-  }
+  // unsigned / floating: cannot overflow; an unknown type id is refused by arith_unary_same_dev
+  const auto unchecked = [&] { return arith_unary_same_dev(type, op, in, out, n, st); };
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if constexpr (std::is_integral<T>::value && std::is_signed<T>::value) return launch_unary_checked<T>(op, in, out, n, d_first_bad, st);
+    else return unchecked();
+  }, unchecked);
 }
 
 __global__ void reset_error_word_kernel(long long* w) { *w = AG_NO_ERROR_POS; }

@@ -412,15 +412,12 @@ ag_status filter_primitive_dev(int bit_width, const void* vals, const uint8_t* v
     if ((uintptr_t)out & 3) AG_FAIL(AG_ERR_INVALID, "filter: boolean output bitmap must be 4-byte aligned");
     return launch_filter_t<uint32_t, 2>(p, st);
   }
-  if (bit_width != 8 && bit_width != 16 && bit_width != 32 && bit_width != 64) AG_FAIL(AG_ERR_TYPE, "filter: invalid values bit width %d", bit_width);
-  const uintptr_t am = (uintptr_t)(bit_width / 8 - 1);
-  if (((uintptr_t)vals & am) || ((uintptr_t)out & am)) AG_FAIL(AG_ERR_INVALID, "filter: buffers not aligned to the element width");
-  switch (bit_width) {
-    case 8: return launch_filter_t<uint8_t, 0>(p, st);
-    case 16: return launch_filter_t<uint16_t, 0>(p, st);
-    case 32: return launch_filter_t<uint32_t, 0>(p, st);
-    default: return launch_filter_t<unsigned long long, 0>(p, st);
-  }
+  return visit_width(bit_width, [&](auto tag) {
+    using V = typename decltype(tag)::type;
+    const uintptr_t am = sizeof(V) - 1;
+    if (((uintptr_t)vals & am) || ((uintptr_t)out & am)) AG_FAIL(AG_ERR_INVALID, "filter: buffers not aligned to the element width");
+    return launch_filter_t<V, 0>(p, st);
+  }, [&] { AG_FAIL(AG_ERR_TYPE, "filter: invalid values bit width %d", bit_width); });
 }
 
 ag_status take_indices_dev(int index_width, const uint8_t* mask, const uint8_t* mvalid, int64_t moff, int64_t n,
@@ -699,15 +696,14 @@ ag_status filter_compare_scalar_dev(int type, int cmp, const void* vals, const v
   if (!d_out_len || !scalar_host) AG_FAIL(AG_ERR_INVALID, "filter_compare: NULL argument");
   if (n == 0) { AG_CUDA_TRY(cudaMemsetAsync(d_out_len, 0, sizeof(int64_t), st)); return AG_OK; }
   if (!vals || (!out && capacity > 0)) AG_FAIL(AG_ERR_INVALID, "filter_compare: NULL values/output");
-  switch (type) {
-    case AG_TYPE_INT32: return launch_fused_cmp<int32_t>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    case AG_TYPE_UINT32: return launch_fused_cmp<uint32_t>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    case AG_TYPE_INT64: return launch_fused_cmp<long long>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    case AG_TYPE_UINT64: return launch_fused_cmp<unsigned long long>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    case AG_TYPE_FLOAT32: return launch_fused_cmp<float>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    case AG_TYPE_FLOAT64: return launch_fused_cmp<double>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "filter_compare: fused path covers 32/64-bit types; use compare + filter for type id %d", type);
-  }
+  const auto not_fused = [&] {
+    AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "filter_compare: fused path covers 32/64-bit types; use compare + filter for type id %d", type);
+  };
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if constexpr (sizeof(T) >= 4) return launch_fused_cmp<T>(cmp, vals, scalar_host, n, out, capacity, d_out_len, st);
+    else return not_fused();
+  }, not_fused);
 }
 
 // ---------------------------------------------------------------- output size ------

@@ -430,13 +430,10 @@ ag_status is_in_dev(int bit_width, const void* vals, const uint8_t* valid, int64
   if (!vals || !out_data || (set_n > 0 && !set)) AG_FAIL(AG_ERR_INVALID, "is_in: NULL values / value set / output");
   if ((reinterpret_cast<uintptr_t>(out_data) & 3) || (reinterpret_cast<uintptr_t>(out_valid) & 3)) AG_FAIL(AG_ERR_INVALID, "is_in: output bitmaps must be 4-byte aligned");
   if (set_n >= (1ll << 31)) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "is_in: value set too large");
-  switch (bit_width) {
-    case 8: return is_in_t<uint8_t>(vals, valid, off, n, set, set_valid, set_off, set_n, null_behavior, out_data, out_valid, d_null_count, st);
-    case 16: return is_in_t<uint16_t>(vals, valid, off, n, set, set_valid, set_off, set_n, null_behavior, out_data, out_valid, d_null_count, st);
-    case 32: return is_in_t<uint32_t>(vals, valid, off, n, set, set_valid, set_off, set_n, null_behavior, out_data, out_valid, d_null_count, st);
-    case 64: return is_in_t<unsigned long long>(vals, valid, off, n, set, set_valid, set_off, set_n, null_behavior, out_data, out_valid, d_null_count, st);
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "is_in: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width);
-  }
+  return visit_width(bit_width, [&](auto tag) {
+    return is_in_t<typename decltype(tag)::type>(vals, valid, off, n, set, set_valid, set_off, set_n, null_behavior, out_data, out_valid,
+                                                 d_null_count, st);
+  }, [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "is_in: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width); });
 }
 
 // columns above `small_rows` try a table of `small_slots` slots (2M x 16 B = 32 MB: resident in H100's 50 MB L2) first
@@ -490,13 +487,9 @@ ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int6
   if (!vals || (!out && capacity > 0)) AG_FAIL(AG_ERR_INVALID, "unique: NULL values/output");
   if (valid && !out_valid && capacity > 0) AG_FAIL(AG_ERR_INVALID, "unique: an input with a validity bitmap needs an output validity bitmap");
   if (n >= (1ll << 31)) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "unique: more than 2^31-1 rows per call");
-  switch (bit_width) {
-    case 8: return unique_t<uint8_t>(bit_width, vals, valid, off, n, out, out_valid, capacity, d_out_len, st);
-    case 16: return unique_t<uint16_t>(bit_width, vals, valid, off, n, out, out_valid, capacity, d_out_len, st);
-    case 32: return unique_t<uint32_t>(bit_width, vals, valid, off, n, out, out_valid, capacity, d_out_len, st);
-    case 64: return unique_t<unsigned long long>(bit_width, vals, valid, off, n, out, out_valid, capacity, d_out_len, st);
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "unique: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width);
-  }
+  return visit_width(bit_width, [&](auto tag) {
+    return unique_t<typename decltype(tag)::type>(bit_width, vals, valid, off, n, out, out_valid, capacity, d_out_len, st);
+  }, [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "unique: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width); });
 }
 
 }  // namespace ag

@@ -171,17 +171,14 @@ ag_status min_max_dev(int type, const void* d_in, int64_t n, void* d_out, cudaSt
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "min_max: negative length");
   if (!d_out) AG_FAIL(AG_ERR_INVALID, "min_max: NULL output");
   if (n > 0 && !d_in) AG_FAIL(AG_ERR_INVALID, "min_max: NULL values");
-  switch (type) {
-    case AG_TYPE_INT8: return launch_minmax<int8_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_UINT8: return launch_minmax<uint8_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_INT16: return launch_minmax<int16_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_UINT16: return launch_minmax<uint16_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_INT32: return launch_minmax<int32_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_UINT32: return launch_minmax<uint32_t>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_INT64: return launch_minmax<long long>(d_in, (size_t)n, d_out, st);
-    case AG_TYPE_UINT64: return launch_minmax<unsigned long long>(d_in, (size_t)n, d_out, st);
-    default: AG_FAIL(AG_ERR_TYPE, "min_max: type id %d is not an integer type (internal/utils/min_max.go covers the 8 integer types)", type);
-  }
+  const auto not_int = [&] {
+    AG_FAIL(AG_ERR_TYPE, "min_max: type id %d is not an integer type (internal/utils/min_max.go covers the 8 integer types)", type);
+  };
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if constexpr (std::is_integral<T>::value) return launch_minmax<T>(d_in, (size_t)n, d_out, st);
+    else return not_int();
+  }, not_int);
 }
 
 }  // namespace ag

@@ -1065,18 +1065,9 @@ ag_status cumulative_sum_dev(int type, const void* in, const uint8_t* valid, int
   p.out_valid = out_valid; p.ooff = ooff;
   p.in = in; p.out = out; p.valid = valid; p.voff = voff; p.n = n; p.skip_nulls = skip_nulls; p.checked = checked;
   p.first_null = nullptr; p.state = static_cast<CumsumState*>(d_state); p.first_bad = (long long*)d_first_bad;
-  switch (type) {
-    case AG_TYPE_UINT8: return launch_cumsum<uint8_t>(p, st);
-    case AG_TYPE_INT8: return launch_cumsum<int8_t>(p, st);
-    case AG_TYPE_UINT16: return launch_cumsum<uint16_t>(p, st);
-    case AG_TYPE_INT16: return launch_cumsum<int16_t>(p, st);
-    case AG_TYPE_UINT32: return launch_cumsum<uint32_t>(p, st);
-    case AG_TYPE_INT32: return launch_cumsum<int32_t>(p, st);
-    case AG_TYPE_UINT64: return launch_cumsum<unsigned long long>(p, st);
-    case AG_TYPE_INT64: return launch_cumsum<long long>(p, st);
-    case AG_TYPE_FLOAT32: return launch_cumsum<float>(p, st);
-    default: return launch_cumsum<double>(p, st);
-  }
+  // the type id was validated above; anything else would run as float64
+  return visit_type(type, [&](auto tag) { return launch_cumsum<typename decltype(tag)::type>(p, st); },
+                    [&] { return launch_cumsum<double>(p, st); });
 }
 
 ag_status cumulative_sum_state_init(void* d_state, int type, const void* start_host, cudaStream_t st) {
@@ -1086,16 +1077,17 @@ ag_status cumulative_sum_state_init(void* d_state, int type, const void* start_h
   unsigned long long lo = 0;
   long long hi = 0;
   if (start_host) {
-    if (type_is_float(type)) memcpy(&lo, start_host, (size_t)w);  // bit pattern (float in the low 32 bits)
-    else if (type_is_signed_int(type)) {
-      long long v = 0;
-      switch (w) { case 1: v = *(const int8_t*)start_host; break; case 2: v = *(const int16_t*)start_host; break;
-                   case 4: v = *(const int32_t*)start_host; break; default: v = *(const int64_t*)start_host; break; }
-      lo = (unsigned long long)v; hi = v < 0 ? -1 : 0;
-    } else {
-      switch (w) { case 1: lo = *(const uint8_t*)start_host; break; case 2: lo = *(const uint16_t*)start_host; break;
-                   case 4: lo = *(const uint32_t*)start_host; break; default: lo = *(const uint64_t*)start_host; break; }
-    }
+    visit_type(type, [&](auto tag) {
+      using T = typename decltype(tag)::type;
+      if constexpr (std::is_floating_point<T>::value) {
+        memcpy(&lo, start_host, sizeof(T));  // bit pattern (float in the low 32 bits)
+      } else {
+        const T v = *(const T*)start_host;
+        lo = (unsigned long long)v;  // sign-extends a signed start value
+        if constexpr (std::is_signed<T>::value) hi = v < 0 ? -1 : 0;
+      }
+      return AG_OK;
+    }, [] { return AG_OK; });  // the type id was validated above
   }
   cumsum_state_init_kernel<<<1, 1, 0, st>>>(static_cast<CumsumState*>(d_state), lo, hi);
   return check_launch("cumsum_state_init_kernel");

@@ -629,19 +629,11 @@ ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int
   if (n >= (1ll << 32)) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: more than 2^32-1 rows per call");
   SortSource src{vals, valid, voff, n, order, null_placement};
   unsigned long long* out = reinterpret_cast<unsigned long long*>(d_out);
-  switch (type) {
-    case AG_TYPE_INT8: return sort_indices_t<int8_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_UINT8: return sort_indices_t<uint8_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_INT16: return sort_indices_t<int16_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_UINT16: return sort_indices_t<uint16_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_INT32: return sort_indices_t<int32_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_UINT32: return sort_indices_t<uint32_t, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_FLOAT32: return sort_indices_t<float, uint32_t>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_INT64: return sort_indices_t<long long, unsigned long long>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_UINT64: return sort_indices_t<unsigned long long, unsigned long long>(src, out, nulls_out, nans_out, st);
-    case AG_TYPE_FLOAT64: return sort_indices_t<double, unsigned long long>(src, out, nulls_out, nans_out, st);
-    default: AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: unsupported type id %d (fixed-width numeric columns only)", type);
-  }
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    using K = typename std::conditional<sizeof(T) == 8, unsigned long long, uint32_t>::type;
+    return sort_indices_t<T, K>(src, out, nulls_out, nans_out, st);
+  }, [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: unsupported type id %d (fixed-width numeric columns only)", type); });
 }
 
 }  // namespace ag

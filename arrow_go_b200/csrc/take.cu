@@ -184,27 +184,21 @@ take_bool_kernel(const TakeParams p) {
 
 static ag_status launch_take_bool(int idx_width, const TakeParams& p, cudaStream_t st) {
   const int64_t need = (p.n + kTkThreads - 1) / kTkThreads;
-  switch (idx_width) {
-    case 8: take_bool_kernel<uint8_t><<<grid_one_wave(take_bool_kernel<uint8_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 16: take_bool_kernel<uint16_t><<<grid_one_wave(take_bool_kernel<uint16_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 32: take_bool_kernel<uint32_t><<<grid_one_wave(take_bool_kernel<uint32_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 64: take_bool_kernel<unsigned long long><<<grid_one_wave(take_bool_kernel<unsigned long long>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    default: AG_FAIL(AG_ERR_INDEX, "take: invalid indices byte width");
-  }
-  return check_launch("take_bool_kernel");
+  return visit_width(idx_width, [&](auto tag) {
+    const auto kernel = take_bool_kernel<typename decltype(tag)::type>;
+    kernel<<<grid_one_wave(kernel, kTkThreads, need), kTkThreads, 0, st>>>(p);
+    return check_launch("take_bool_kernel");
+  }, [&] { AG_FAIL(AG_ERR_INDEX, "take: invalid indices byte width"); });
 }
 
 template <typename V>
 static ag_status launch_take_v(int idx_width, const TakeParams& p, cudaStream_t st) {
   const int64_t need = (p.n + kTkThreads * kTkUnroll - 1) / (kTkThreads * kTkUnroll);
-  switch (idx_width) {
-    case 8: take_kernel<V, uint8_t><<<grid_one_wave(take_kernel<V, uint8_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 16: take_kernel<V, uint16_t><<<grid_one_wave(take_kernel<V, uint16_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 32: take_kernel<V, uint32_t><<<grid_one_wave(take_kernel<V, uint32_t>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    case 64: take_kernel<V, unsigned long long><<<grid_one_wave(take_kernel<V, unsigned long long>, kTkThreads, need), kTkThreads, 0, st>>>(p); break;
-    default: AG_FAIL(AG_ERR_INDEX, "take: invalid indices byte width");  // vector_selection.go:1157
-  }
-  return check_launch("take_kernel");
+  return visit_width(idx_width, [&](auto tag) {
+    const auto kernel = take_kernel<V, typename decltype(tag)::type>;
+    kernel<<<grid_one_wave(kernel, kTkThreads, need), kTkThreads, 0, st>>>(p);
+    return check_launch("take_kernel");
+  }, [&] { AG_FAIL(AG_ERR_INDEX, "take: invalid indices byte width"); });  // vector_selection.go:1157
 }
 
 
@@ -719,23 +713,16 @@ ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vva
   p.out = out; p.out_valid = reinterpret_cast<uint32_t*>(out_valid); p.bad_pos = reinterpret_cast<long long*>(d_bad_pos);
   TakeWindowPlan w;
   if (plan_windowed(bit_width, idx_width, p, &w)) {
-    switch (bit_width) {
-      case 8: return take_windowed<uint8_t>(idx_width, p, w, st);
-      case 16: return take_windowed<uint16_t>(idx_width, p, w, st);
-      case 32: return take_windowed<uint32_t>(idx_width, p, w, st);
-      default: return take_windowed<unsigned long long>(idx_width, p, w, st);
-    }
+    // plan_windowed admits 8/16/32/64-bit values only; anything else would run as 64-bit
+    return visit_width(bit_width, [&](auto tag) { return take_windowed<typename decltype(tag)::type>(idx_width, p, w, st); },
+                       [&] { return take_windowed<unsigned long long>(idx_width, p, w, st); });
   }
-  switch (bit_width) {
-    case 8: return launch_take_v<uint8_t>(idx_width, p, st);
-    case 16: return launch_take_v<uint16_t>(idx_width, p, st);
-    case 32: return launch_take_v<uint32_t>(idx_width, p, st);
-    case 64: return launch_take_v<unsigned long long>(idx_width, p, st);
-    case 1:
-      if (reinterpret_cast<uintptr_t>(out) & 3) AG_FAIL(AG_ERR_INVALID, "take: boolean output bitmap must be 4-byte aligned");
-      return launch_take_bool(idx_width, p, st);
-    default: AG_FAIL(AG_ERR_INVALID, "take: invalid values byte width for take");  // vector_selection.go:1190
+  if (bit_width == 1) {
+    if (reinterpret_cast<uintptr_t>(out) & 3) AG_FAIL(AG_ERR_INVALID, "take: boolean output bitmap must be 4-byte aligned");
+    return launch_take_bool(idx_width, p, st);
   }
+  return visit_width(bit_width, [&](auto tag) { return launch_take_v<typename decltype(tag)::type>(idx_width, p, st); },
+                     [&] { AG_FAIL(AG_ERR_INVALID, "take: invalid values byte width for take"); });  // vector_selection.go:1190
 }
 
 }  // namespace ag

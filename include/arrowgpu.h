@@ -630,6 +630,42 @@ ag_status ag_parquet_plain_decode_spaced_dev(int value_width, const uint8_t* d_d
                                              const uint8_t* d_valid, void* d_out, ag_stream_t s);
 
 /* ================================================================================= *
+ * DELTA_BINARY_PACKED INT32 / INT64 pages — the same batch-of-pages contract as ag_parquet_dict_decode (host page
+ *   table, any page order, valid == NULL for dense output, decoded[i] in slots, the device flavour synchronises `s`
+ *   once).  value_width 4 (INT32) or 8 (INT64), anything else AG_ERR_INVALID; `out` aligned to it.
+ *   deltaBitPackDecoder (parquet/internal/encoding/delta_bit_packing.go): SetData (:72-133, called with the page's
+ *   num_values, file/column_reader.go:527), initBlock (:136-160), unpackNextMini (:162-216), Decode (:264-302),
+ *   DecodeSpaced (:305-316).  Each error is AG_ERR_INVALID naming the page, with the reference's message:
+ *     - the header (block size, miniblocks per block, total values, first value) is always parsed, even when the
+ *       page needs no value: a missing, truncated or over-64-bit varint is "parquet: eof exception"; the block size,
+ *       miniblock and values-per-miniblock checks and "invalid delta value count %d for %d buffered values"
+ *       (total > 2^32-1 or > num_values) are SetData's; INT32: "initial delta value %d exceeds INT32 range";
+ *     - blocks and miniblocks are read lazily, as the reference reads them: only those holding one of the first
+ *       min(need, total) - 1 deltas are read ("touched"; need = num_values dense, the page's valid bits spaced).
+ *       A touched block: min delta ("parquet: eof exception", INT32: "minimum delta %d exceeds INT32 range"), then
+ *       all its width bytes ("failed to read byte").  A touched miniblock: width <= 32 (INT32) / 64 (INT64)
+ *       ("delta bit width %d exceeds decoder width %d") and its whole payload of vpm*width/8 bytes present, even
+ *       when only part of it is needed ("unexpected EOF").  Widths of miniblocks past the last needed delta are
+ *       never looked at, and a stream may end right after the last needed miniblock;
+ *     - dense, total < num_values: not an error, decoded = total (Decode's short count);
+ *     - spaced, total < valid slots: "parquet: number of values / definition levels read did not match", decoded =
+ *       0 and nothing is written (as for a short PLAIN page).
+ *   value[k] = value[k-1] + delta + min_delta modulo 2^(8*value_width): every sum wraps at the physical width, so the
+ *   result is bit-exact in any summation order, and INT32 is computed in uint32 (the reference accumulates in int64
+ *   and truncates, which gives the same bits).
+ *   Differences from the reference (DESIGN §2):
+ *     - an error inside the block chain still delivers the first value and every miniblock before the failing one;
+ *       decoded says how many slots were written (spaced: every slot before the first valid slot whose value was
+ *       not delivered), like a truncated literal run.  The reference's Decode returns (0, err).  A header error
+ *       delivers no value (spaced: the null slots before the first valid slot get 0);
+ *     - the page is decoded in parallel (a block walk, then a prefix sum of the deltas), not miniblock by miniblock.
+ * ================================================================================= */
+ag_status ag_parquet_delta_decode(int value_width, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                  const uint8_t* valid, void* out, int64_t* decoded);
+ag_status ag_parquet_delta_decode_dev(int value_width, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                      const uint8_t* d_valid, void* d_out, int64_t* d_decoded, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

@@ -1,17 +1,21 @@
 #!/usr/bin/env python
 """Parquet page decode on the device (include/arrowgpu.h, csrc/rle.cu) at ~100M values over 2^19-value (~1 MB) pages.
 
-  python scripts/parquet_pages_bench.py [--values N] [--steps K] [--warmup W]
+  python scripts/parquet_pages_bench.py [--values N] [--steps K] [--warmup W] [--profile]
 
 Prints one JSON line: for each case the time per call (CUDA events around K device-resident calls after W warm-up
 calls), the algorithmic bytes (encoded bytes read + values written + validity bits read: what a single pass has to
 move) and their share of the HBM peak, with the card's name and power limit.  Each call ends in one stream
 synchronisation (per-page error codes), which the times include.  Four distinct page bodies are reused round-robin;
 every page writes its own output range.  Writes nothing to disk.
+
+--profile runs only the DELTA_BINARY_PACKED cases, under torch.profiler, and reports the device time per call of each
+kernel (the block walk against the value passes) instead.
 """
 import argparse
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -19,6 +23,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))   # pq_delta_ref.delta_encode: the DELTA_BINARY_PACKED encoder, numpy per block
 
 
 def rle_literal_page(idx, bw):
@@ -63,6 +68,7 @@ def main():
     ap.add_argument("--values", type=int, default=100_000_000)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--profile", action="store_true")
     args = ap.parse_args()
 
     from arrow_go_b200 import _native as N
@@ -108,6 +114,10 @@ def main():
                 "gbs": ab / ms / 1e6, "frac": ab / ms / 1e6 / peak, "note": note}
 
     dout = DeviceBuffer(8 * n + 64)
+    if args.profile:
+        res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer, profile=True))
+        print(json.dumps(res), flush=True)
+        return
     dictionary = rng.integers(-(1 << 62), 1 << 62, 100_000)
     ddict = upload(dictionary)
     valid = rng.random(n) >= 0.1
@@ -133,8 +143,67 @@ def main():
     dblob, tbl, enc = page_set(lv)
     ms = timed(lambda: N.call("ag_parquet_levels_decode_dev", 1, N.PQ_LEVELS_V2_RLE, dblob.ptr, tbl, n_pages, dout.ptr, dec.ptr, None))
     res["parquet_levels_decode"] = line(ms, enc + 2.0 * n, enc, "max_level 1 (bit width 1), 10 % nulls, literal runs; int16 levels out")
-    dblob.free(); ddict.free(); dvalid.free(); dec.free(); bad.free(); dout.free()
+    dblob.free(); ddict.free(); dvalid.free(); dec.free(); bad.free()
+    res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer))
+    dout.free()
     print(json.dumps(res), flush=True)
+
+
+def delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer, profile=False):
+    """DELTA_BINARY_PACKED: (a) int64 timestamps (sorted, increments uniform in [0, 1000), 256/4 blocks), required;
+    (b) the same with 10 % nulls; (c) int32 uniform random values (128/4 blocks, every miniblock 32 bits wide);
+    (d) ag_parquet_plain_decode_spaced_dev writing the output of (b), the floor for writing it."""
+    import pq_delta_ref as R
+    out = {}
+    valid = rng.random(n) >= 0.1
+    dvalid = upload(np.packbits(valid, bitorder="little"))
+    dec = DeviceBuffer(8 * n_pages + 64)
+    ts = [R.delta_encode(np.cumsum(rng.integers(0, 1000, per_page)) + (k << 40), 8, 256, 4) for k in range(4)]
+    rnd = [R.delta_encode(rng.integers(-(1 << 31), 1 << 31, per_page), 4, 128, 4) for _ in range(4)]
+    plain = [rng.integers(-(1 << 62), 1 << 62, per_page).tobytes() for _ in range(4)]
+    runs = []
+    dblob, tbl, enc = page_set(ts)
+    runs.append(("parquet_delta_decode_i64_timestamps_required", 8, dblob, tbl, None, enc + 8.0 * n, enc,
+                 "int64 sorted, increments uniform in [0, 1000): 256/4 blocks, ~10-bit miniblocks; dense output"))
+    runs.append(("parquet_delta_decode_i64_timestamps_10pct_nulls", 8, dblob, tbl, dvalid.ptr, enc + 8.0 * n + n / 8.0, enc,
+                 "the same pages, 10 % nulls: each page's first ~90 % of values spaced out"))
+    rblob, rtbl, renc = page_set(rnd)
+    runs.append(("parquet_delta_decode_i32_random", 4, rblob, rtbl, None, renc + 4.0 * n, renc,
+                 "int32 uniform random: 128/4 blocks, every miniblock 32 bits wide (the most encoded bytes)"))
+    if profile:
+        import torch
+        from torch.profiler import ProfilerActivity, profile as tprofile
+        for name, w, b, t, vp, ab, e, note in runs:
+            fn = (lambda w=w, b=b, t=t, vp=vp: N.call("ag_parquet_delta_decode_dev", w, b.ptr, t, n_pages, vp, dout.ptr, dec.ptr, None))
+            for _ in range(args.warmup):
+                fn()
+            with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(args.steps):
+                    fn()
+                torch.cuda.synchronize()
+            kern = {}
+            for ev in prof.key_averages():
+                if ev.device_type == torch.autograd.DeviceType.CUDA:
+                    m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel)(<[^>]*>)?", ev.key)
+                    short = (m.group(1) + (m.group(2) or "")) if m else ev.key.strip()
+                    us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
+                    kern[short] = kern.get(short, 0.0) + us / 1e3 / args.steps
+            walk = sum(v for k, v in kern.items() if "walk" in k)
+            out[name + "_profile"] = {"kernels_ms_per_call": kern, "walk_ms": walk,
+                                      "value_passes_ms": sum(v for k, v in kern.items() if "delta_values" in k or "delta_scan" in k)}
+    else:
+        for name, w, b, t, vp, ab, e, note in runs:
+            ms = timed(lambda w=w, b=b, t=t, vp=vp: N.call("ag_parquet_delta_decode_dev", w, b.ptr, t, n_pages, vp, dout.ptr, dec.ptr, None))
+            out[name] = line(ms, ab, e, note)
+        pblob, ptbl, _ = page_set(plain)
+        penc = 8.0 * int(valid.sum())
+        ms = timed(lambda: N.call("ag_parquet_plain_decode_spaced_dev", 8, pblob.ptr, ptbl, n_pages, dvalid.ptr, dout.ptr, None))
+        out["parquet_plain_decode_spaced_i64_10pct_nulls"] = line(ms, penc + 8.0 * n + n / 8.0, penc,
+                                                                  "PLAIN int64 pages, same slots and validity as the timestamps case: the floor for its output")
+        out["delta_10pct_nulls_over_plain"] = out["parquet_delta_decode_i64_timestamps_10pct_nulls"]["ms"] / ms
+        pblob.free()
+    dblob.free(); rblob.free(); dvalid.free(); dec.free()
+    return out
 
 
 if __name__ == "__main__":

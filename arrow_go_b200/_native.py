@@ -60,6 +60,19 @@ def page_table(pages):
     return arr
 
 
+class PqCompressed(C.Structure):
+    """ag_pq_compressed: one compressed Parquet page of a batched decompression (byte offsets and lengths)."""
+    _fields_ = [("src", C.c_int64), ("src_len", C.c_int64), ("dst", C.c_int64), ("dst_len", C.c_int64)]
+
+
+def compressed_table(pages):
+    """[(src, src_len, dst, dst_len), ...] -> ctypes array of ag_pq_compressed."""
+    arr = (PqCompressed * max(len(pages), 1))()
+    for k, (s, sl, d, dl) in enumerate(pages):
+        arr[k].src, arr[k].src_len, arr[k].dst, arr[k].dst_len = s, sl, d, dl
+    return arr
+
+
 class NativeError(RuntimeError):
     """A C-ABI call returned a non-zero ag_status."""
 
@@ -203,6 +216,8 @@ _SIGS = {
     "ag_parquet_plain_decode_spaced_dev": [_i, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_delta_decode": [_i, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_delta_decode_dev": [_i, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
+    "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     # parity helpers
     "ag_checksum64_dev": [_p, _sz, _p, _p],
     "ag_generate_dev": [_i, _u64, _i64, _i64, _p, _sz, _p],

@@ -1,0 +1,477 @@
+// snappy.cu — raw Snappy decompression of Parquet SNAPPY pages on the device.
+//   serializedPageReader.decompress   parquet/file/page_reader.go:597-621 -> compress.Decode (parquet/compress/compress.go:107)
+//                                     -> snappyCodec.DecodeWithError (parquet/compress/snappy.go:43-45)
+//   element checks                    golang/snappy's decode (ErrCorrupt)
+//
+// A call decompresses a batch of pages (ag_pq_compressed descriptors, one device buffer of compressed bytes) in two
+// launches, both one block per page:
+//   1. snappy_parse_kernel: reads the preamble, then streams the compressed bytes through a 16 KB shared-memory window
+//      in spans of 1024 candidate element starts.  Every thread decodes the element that would start at each of its
+//      4 positions (length, output length, offset); the element chain through the span is found by pointer doubling
+//      over those next-positions (a reach bitmask, log2(elements) rounds), and a block scan of the chain's output
+//      lengths gives each element its output position.  Each element is validated here and written as a 9-byte
+//      descriptor {output position, literal source / copy offset, literal flag}, so a failing page knows how many
+//      bytes its valid elements produce before anything is executed.  A literal longer than the window moves the next
+//      span (and window) past it without loading it.
+//   2. snappy_exec_kernel: walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
+//      dst[pos - off + (j mod off)], so every output byte names one source byte: a compressed byte (literals), an
+//      output byte before the batch (read back from dst, which the same block wrote, L2-resident), or an earlier byte
+//      of the same batch.  Pointer jumping in shared memory resolves the last kind, so overlapping copies and copies of
+//      copies in one batch (offset 1 runs, the offset-8 copies of int64 columns) are as parallel as literals.
+// Roofline.  compressed bytes read + decompressed bytes written.  This design also writes and reads 9 B per element
+// descriptor and reads each copied byte once more (from L2).
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "host_stage.cuh"
+
+namespace ag {
+
+namespace {
+
+constexpr int kSnThreads = 256;
+constexpr int kSpan = 1024;                 // candidate element starts per parse step
+constexpr int kPer = kSpan / kSnThreads;    // 4 consecutive positions per thread
+constexpr int kWinVec = 1024;               // 16-byte vectors per shared-memory window (16 KB)
+constexpr int kWinBytes = kWinVec * 16;
+constexpr int kLook = 4;                    // bytes an element header reaches past its tag byte
+constexpr int kBatch = 2048;                // output bytes per execute step
+constexpr unsigned long long kCntOne = 1ull << 48;   // parse scan: element count in bits 48.., output bytes below
+constexpr unsigned long long kLenMask = kCntOne - 1;
+constexpr unsigned long long kLenClamp = 1ull << 33; // any longer element is corrupt (dst_len <= 2^32-1)
+constexpr unsigned long long kFromDst = 1ull << 62;  // execute: source byte is dst[low bits]
+constexpr unsigned long long kFromSrc = 1ull << 63;  // execute: source byte is the page's compressed byte [low bits]
+constexpr unsigned long long kPosMask = (1ull << 62) - 1;
+
+enum SnapErr : int { kSnOk = 0, kSnCorrupt = 1, kSnSize = 2 };
+
+struct SnapPage {           // written by snappy_parse_kernel, read by snappy_exec_kernel and the host
+  int64_t written;          // output bytes of the page's valid elements
+  int64_t nelem;            // element descriptors written
+  int64_t preamble;         // the stream's uncompressed length (kSnSize names it)
+  int32_t err;
+  int32_t pad;
+};
+
+struct SnapArgs {
+  const ag_pq_compressed* pages;
+  const int64_t* elem_base;   // [n_pages + 1]: first element descriptor of every page
+  const uint8_t* src;
+  uint8_t* dst;
+  SnapPage* st;
+  uint32_t* e_out;            // element: first output byte, within the page
+  uint32_t* e_ref;            // literal: byte offset of its bytes in the page's stream; copy: the offset
+  uint8_t* e_lit;             // 1 = literal
+  int64_t* d_written;         // may be NULL
+};
+
+// exclusive block scan of one value per thread
+__device__ __forceinline__ unsigned long long block_excl_scan(unsigned long long v, unsigned long long* warp_tot, unsigned long long* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  unsigned long long x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_tot[wid] = x;
+  __syncthreads();
+  unsigned long long off = 0, tot = 0;
+#pragma unroll
+  for (int w = 0; w < kSnThreads / 32; ++w) {
+    const unsigned long long t = warp_tot[w];
+    off += (w < wid) ? t : 0ull;
+    tot += t;
+  }
+  __syncthreads();
+  *total = tot;
+  return off + x - v;
+}
+
+__device__ __forceinline__ bool bit_on(const uint32_t* m, int q) { return (m[q >> 5] >> (q & 31)) & 1u; }
+
+// one block per page: preamble, element chain, validation, element descriptors
+__global__ void __launch_bounds__(kSnThreads)
+snappy_parse_kernel(SnapArgs a) {
+  __shared__ uint4 win[kWinVec];
+  __shared__ uint16_t jmp[2][kSpan];         // next chain position 2^r elements on (kSpan: leaves the span)
+  __shared__ uint32_t reach[kSpan / 32];     // span positions on the element chain
+  __shared__ unsigned long long warp_tot[kSnThreads / 32];
+  __shared__ int64_t s_pos, s_next, s_written, s_nelem, s_pre, s_fail_out, s_fail_idx;
+  __shared__ int s_err, s_done, s_fail;
+  const int64_t p = blockIdx.x;
+  const ag_pq_compressed pg = a.pages[p];
+  const int tid = threadIdx.x;
+  const uint8_t* in = a.src + pg.src;
+  const int64_t len = pg.src_len, dlen = pg.dst_len;
+  const int64_t eb = a.elem_base[p], cap = a.elem_base[p + 1] - eb;
+
+  if (tid == 0) {
+    int err = kSnOk;
+    int64_t pos = 0;
+    unsigned long long v = 0;
+    if (len != 0 || dlen != 0) {                                 // an empty v2 value region has no preamble
+      bool ok = false;                                           // binary.Uvarint
+      for (int i = 0; i < 10 && pos < len; ++i) {
+        const uint32_t c = __ldg(in + pos++);
+        if (c < 0x80) { ok = !(i == 9 && c > 1); v |= (unsigned long long)c << (7 * i); break; }
+        v |= (unsigned long long)(c & 0x7f) << (7 * i);
+      }
+      if (!ok || v > 0xffffffffull) err = kSnCorrupt;
+      else if ((int64_t)v != dlen) err = kSnSize;
+    }
+    s_pos = pos; s_pre = (int64_t)v; s_err = err; s_written = 0; s_nelem = 0;
+    s_done = err != kSnOk || pos >= len;
+  }
+
+  const uint8_t* wb = reinterpret_cast<const uint8_t*>(win);
+  const uintptr_t sbeg = reinterpret_cast<uintptr_t>(in), send = sbeg + len;
+  int64_t wlo = INT64_MIN / 2;                                   // stream offset of the window's first byte
+  while (true) {
+    __syncthreads();
+    if (s_done) break;
+    const int64_t cur = s_pos;
+    if ((cur + kSpan + kLook < len ? cur + kSpan + kLook : len) > wlo + kWinBytes) {
+      // window [a0, a0 + 16 KB), a0 = 16-byte aligned start of the span; only vectors holding a stream byte are loaded
+      const uintptr_t a0 = (sbeg + cur) & ~(uintptr_t)15;
+#pragma unroll 4
+      for (int v = tid; v < kWinVec; v += kSnThreads) {
+        const uintptr_t ad = a0 + (uintptr_t)v * 16;
+        if (ad < send && ad + 16 > sbeg) win[v] = __ldcs(reinterpret_cast<const uint4*>(ad));
+      }
+      wlo = (int64_t)a0 - (int64_t)sbeg;
+      __syncthreads();
+    }
+    auto byte_at = [&](int64_t i) -> uint32_t { return i < len ? (uint32_t)wb[i - wlo] : 0u; };
+
+    // ---- the element that would start at each of this thread's positions ----
+    uint32_t J[kPer], ref[kPer];
+    unsigned long long olen[kPer], elen[kPer];
+    bool lit[kPer], bad[kPer], ends[kPer];
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      const int q = tid * kPer + k;
+      const int64_t i = cur + q;
+      J[k] = kSpan; ref[k] = 0; olen[k] = 0; elen[k] = 0; lit[k] = false; bad[k] = true;
+      if (i < len) {
+        const uint32_t tag = byte_at(i);
+        unsigned long long hdr, L;
+        switch (tag & 3) {
+          case 0: {
+            const uint32_t m = tag >> 2;
+            if (m < 60) {
+              hdr = 1; L = m + 1;
+            } else {                                             // length-1 in the next 1..4 bytes, little-endian
+              const int nb = (int)m - 59;
+              unsigned long long x = 0;
+              for (int b = 0; b < nb; ++b) x |= (unsigned long long)byte_at(i + 1 + b) << (8 * b);
+              hdr = 1 + nb; L = x + 1;
+            }
+            lit[k] = true;
+            ref[k] = (uint32_t)(i + (int64_t)hdr);
+            break;
+          }
+          case 1: hdr = 2; L = 4 + ((tag >> 2) & 7); ref[k] = ((tag >> 5) << 8) | byte_at(i + 1); break;
+          case 2: hdr = 3; L = 1 + (tag >> 2); ref[k] = byte_at(i + 1) | byte_at(i + 2) << 8; break;
+          default:
+            hdr = 5; L = 1 + (tag >> 2);
+            ref[k] = byte_at(i + 1) | byte_at(i + 2) << 8 | byte_at(i + 3) << 16 | byte_at(i + 4) << 24;
+            break;
+        }
+        const unsigned long long e = hdr + (lit[k] ? L : 0ull);
+        bad[k] = (unsigned long long)(len - i) < e;              // length, literal bytes or offset cut off
+        elen[k] = e;
+        olen[k] = L < kLenClamp ? L : kLenClamp;
+        if (!bad[k] && (unsigned long long)q + e < kSpan && i + (int64_t)e < len) J[k] = (uint32_t)(q + e);
+      }
+      ends[k] = J[k] == kSpan;
+      jmp[0][q] = (uint16_t)J[k];
+    }
+    if (tid < kSpan / 32) reach[tid] = tid == 0 ? 1u : 0u;      // the span starts on an element
+    if (tid == 0) s_fail = kSpan;
+    __syncthreads();
+
+    // ---- the chain: round r adds the positions 2^r elements after every position already on it ----
+    for (int r = 0;; ++r) {
+      bool grew = false;
+#pragma unroll
+      for (int k = 0; k < kPer; ++k) {
+        const int q = tid * kPer + k;
+        const uint32_t j = J[k];
+        if (j < kSpan && bit_on(reach, q) && !bit_on(reach, (int)j)) {
+          atomicOr(&reach[j >> 5], 1u << (j & 31));
+          grew = true;
+        }
+      }
+      if (!__syncthreads_or(grew)) break;                       // closed: every chain position is on
+#pragma unroll
+      for (int k = 0; k < kPer; ++k) {
+        J[k] = J[k] < kSpan ? jmp[r & 1][J[k]] : kSpan;
+        jmp[(r + 1) & 1][tid * kPer + k] = (uint16_t)J[k];
+      }
+    }
+
+    // ---- output positions, validation, descriptors ----
+    bool on[kPer];
+    unsigned long long loc = 0;
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      on[k] = bit_on(reach, tid * kPer + k);
+      if (on[k]) loc += kCntOne | olen[k];
+    }
+    unsigned long long tot;
+    const unsigned long long ex = block_excl_scan(loc, warp_tot, &tot);
+    const int64_t w0 = s_written, n0 = s_nelem;
+    unsigned long long run = ex;
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      if (!on[k]) continue;
+      const unsigned long long o = (unsigned long long)w0 + (run & kLenMask);
+      const bool fail = bad[k] || o > (unsigned long long)dlen || olen[k] > (unsigned long long)dlen - o ||
+                        (!lit[k] && (ref[k] == 0 || ref[k] > o));
+      if (fail) atomicMin(&s_fail, tid * kPer + k);
+      run += kCntOne | olen[k];
+    }
+    __syncthreads();
+    const int fq = s_fail;
+    run = ex;
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      if (!on[k]) continue;
+      const int q = tid * kPer + k;
+      const int64_t o = w0 + (int64_t)(run & kLenMask), idx = n0 + (int64_t)(run >> 48);
+      if (q < fq) {
+        if (idx < cap) {
+          a.e_out[eb + idx] = (uint32_t)o;
+          a.e_ref[eb + idx] = ref[k];
+          a.e_lit[eb + idx] = lit[k] ? 1 : 0;
+        }
+        if (ends[k]) s_next = cur + q + (int64_t)elen[k];
+      } else if (q == fq) {
+        s_fail_out = o; s_fail_idx = idx;
+      }
+      run += kCntOne | olen[k];
+    }
+    __syncthreads();
+    if (tid == 0) {
+      if (fq < kSpan) {
+        s_err = kSnCorrupt; s_written = s_fail_out; s_nelem = s_fail_idx; s_done = 1;
+      } else {
+        s_written = w0 + (int64_t)(tot & kLenMask); s_nelem = n0 + (int64_t)(tot >> 48);
+        s_pos = s_next;
+        s_done = s_next >= len;
+      }
+    }
+  }
+
+  if (tid == 0) {
+    int err = s_err;
+    int64_t written = s_written, nelem = s_nelem;
+    if (err == kSnOk && written != dlen) err = kSnCorrupt;      // the stream ends before the output is full
+    if (err == kSnSize) written = nelem = 0;
+    SnapPage ps;
+    ps.written = written; ps.nelem = nelem < cap ? nelem : cap; ps.preamble = s_pre; ps.err = err; ps.pad = 0;
+    a.st[p] = ps;
+    if (a.d_written) a.d_written[p] = written;
+  }
+}
+
+// one block per page: the page's output in batches of kBatch bytes, in order
+__global__ void __launch_bounds__(kSnThreads)
+snappy_exec_kernel(SnapArgs a) {
+  __shared__ uint32_t s_out[kBatch + 1], s_ref[kBatch + 1];
+  __shared__ uint8_t s_lit[kBatch + 1];
+  __shared__ unsigned long long s_src[kBatch];
+  const int64_t p = blockIdx.x;
+  const SnapPage ps = a.st[p];
+  const int64_t written = ps.written, nelem = ps.nelem;
+  if (written <= 0 || nelem <= 0) return;                        // block-uniform
+  const ag_pq_compressed pg = a.pages[p];
+  const uint8_t* in = a.src + pg.src;
+  uint8_t* out = a.dst + pg.dst;
+  const int64_t eb = a.elem_base[p];
+  const int tid = threadIdx.x;
+  int64_t e0 = 0;                                                // the element holding the batch's first byte
+  for (int64_t B = 0; B < written; B += kBatch) {
+    const int nb = (int)(written - B < kBatch ? written - B : kBatch);
+    // elements e0 .. e0 + nl - 1 hold every byte of [B, B + kBatch] (each element produces at least one byte)
+    const int nl = (int)(nelem - e0 < kBatch + 1 ? nelem - e0 : kBatch + 1);
+    for (int k = tid; k < nl; k += kSnThreads) {
+      s_out[k] = a.e_out[eb + e0 + k];
+      s_ref[k] = a.e_ref[eb + e0 + k];
+      s_lit[k] = a.e_lit[eb + e0 + k];
+    }
+    __syncthreads();
+    auto holder = [&](uint32_t pos) {                            // last loaded element starting at or before pos
+      int lo = 0, hi = nl - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (s_out[mid] <= pos) lo = mid; else hi = mid - 1;
+      }
+      return lo;
+    };
+    for (int b = tid; b < nb; b += kSnThreads) {
+      const uint32_t pos = (uint32_t)(B + b);
+      const int e = holder(pos);
+      const uint32_t j = pos - s_out[e], r = s_ref[e];
+      unsigned long long s;
+      if (s_lit[e]) {
+        s = kFromSrc | (unsigned long long)(r + j);
+      } else {
+        const uint32_t q = s_out[e] - r + (r >= 64 ? j : j % r);   // a copy is at most 64 bytes long
+        s = (int64_t)q < B ? kFromDst | q : (unsigned long long)((int64_t)q - B);
+      }
+      s_src[b] = s;
+    }
+    __syncthreads();
+    while (true) {                                               // pointer jumping to a byte outside the batch
+      bool pend = false;
+      for (int b = tid; b < nb; b += kSnThreads) {
+        const unsigned long long v = s_src[b];
+        if (v < kFromDst) {
+          const unsigned long long w = s_src[v];
+          s_src[b] = w;
+          pend |= w < kFromDst;
+        }
+      }
+      if (!__syncthreads_or(pend)) break;
+    }
+    for (int b = tid; b < nb; b += kSnThreads) {
+      const unsigned long long v = s_src[b];
+      // dst bytes before the batch were written by this block before the last barrier: a plain (coherent) load
+      out[B + b] = (v & kFromSrc) ? __ldg(in + (v & kPosMask)) : out[v & kPosMask];
+    }
+    e0 += holder((uint32_t)(B + kBatch < written ? B + kBatch : written - 1));
+    __syncthreads();
+  }
+}
+
+}  // namespace
+
+// Argument checks shared by both flavours; every one is AG_ERR_INVALID before any launch.  *src_end / *dst_end: the
+// bytes of `src` / `dst` the batch spans.
+static ag_status snappy_check(const char* fn, const ag_pq_compressed* pages, int64_t n_pages, int64_t* src_end, int64_t* dst_end) {
+  *src_end = *dst_end = 0;
+  if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
+  if (n_pages == 0) return AG_OK;
+  if (!pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
+  std::vector<int64_t> order;
+  for (int64_t i = 0; i < n_pages; ++i) {
+    const ag_pq_compressed& g = pages[i];
+    if (g.src < 0 || g.src_len < 0 || g.dst < 0 || g.dst_len < 0 || g.src_len > 0xffffffffLL || g.dst_len > 0xffffffffLL)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field or more than 2^32-1 bytes", fn, (long long)i);
+    *src_end = std::max(*src_end, g.src + g.src_len);
+    *dst_end = std::max(*dst_end, g.dst + g.dst_len);
+    if (g.dst_len > 0) order.push_back(i);
+  }
+  std::sort(order.begin(), order.end(), [&](int64_t x, int64_t y) { return pages[x].dst < pages[y].dst || (pages[x].dst == pages[y].dst && x < y); });
+  for (size_t k = 1; k < order.size(); ++k) {
+    const ag_pq_compressed &u = pages[order[k - 1]], &v = pages[order[k]];
+    if (v.dst < u.dst + u.dst_len) {
+      const int64_t x = std::min(order[k - 1], order[k]), y = std::max(order[k - 1], order[k]);
+      AG_FAIL(AG_ERR_INVALID, "%s: pages %lld and %lld: overlapping dst ranges", fn, (long long)x, (long long)y);
+    }
+  }
+  return AG_OK;
+}
+
+// Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
+// `st` once to read the per-page error codes back.  h_written (host, may be NULL) receives the bytes per page.
+static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst, int64_t* d_written,
+                            int64_t* h_written, cudaStream_t st) {
+  const char* fn = "snappy_decompress";
+  int64_t src_end, dst_end;
+  AG_TRY(snappy_check(fn, pages, n_pages, &src_end, &dst_end));
+  if (n_pages == 0) return AG_OK;
+  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
+  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  // plan: pages | elem_base[n+1].  A valid element takes >= 2 compressed bytes and produces >= 1 output byte.
+  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed);
+  const size_t plan_bytes = pb + (size_t)(n_pages + 1) * 8;
+  std::vector<uint8_t> h(plan_bytes);
+  memcpy(h.data(), pages, pb);
+  int64_t* elem_base = reinterpret_cast<int64_t*>(h.data() + pb);
+  elem_base[0] = 0;
+  for (int64_t i = 0; i < n_pages; ++i) elem_base[i + 1] = elem_base[i] + std::min(pages[i].src_len / 2, pages[i].dst_len);
+  const int64_t n_elem = elem_base[n_pages];
+  const size_t st_bytes = (size_t)n_pages * sizeof(SnapPage);
+  const size_t off_st = (plan_bytes + 255) & ~(size_t)255;
+  const size_t off_out = (off_st + st_bytes + 255) & ~(size_t)255;
+  const size_t off_ref = (off_out + (size_t)n_elem * 4 + 255) & ~(size_t)255;
+  const size_t off_lit = (off_ref + (size_t)n_elem * 4 + 255) & ~(size_t)255;
+  const size_t total = off_lit + (size_t)n_elem;
+  // this call synchronises `st` anyway, so its device scratch may live in a Temps
+  Temps t(st);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, total));
+  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  SnapArgs a;
+  a.pages = reinterpret_cast<const ag_pq_compressed*>(d);
+  a.elem_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.src = src;
+  a.dst = dst;
+  a.st = reinterpret_cast<SnapPage*>(d + off_st);
+  a.e_out = reinterpret_cast<uint32_t*>(d + off_out);
+  a.e_ref = reinterpret_cast<uint32_t*>(d + off_ref);
+  a.e_lit = d + off_lit;
+  a.d_written = d_written;
+  snappy_parse_kernel<<<(unsigned)n_pages, kSnThreads, 0, st>>>(a);
+  AG_TRY(check_launch("snappy_parse_kernel"));
+  snappy_exec_kernel<<<(unsigned)n_pages, kSnThreads, 0, st>>>(a);
+  AG_TRY(check_launch("snappy_exec_kernel"));
+  std::vector<SnapPage> hs((size_t)n_pages);
+  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
+  AG_TRY(sync(st));
+  if (h_written)
+    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
+  for (int64_t i = 0; i < n_pages; ++i) {
+    if (hs[i].err == kSnSize)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: metadata said %lld bytes uncompressed data page, got %lld bytes (0 bytes written)", fn,
+              (long long)i, (long long)pages[i].dst_len, (long long)hs[i].preamble);
+    if (hs[i].err == kSnCorrupt)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: could not decompress page: snappy: corrupt input (%lld bytes written)", fn,
+              (long long)i, (long long)hs[i].written);
+  }
+  return AG_OK;
+}
+
+}  // namespace ag
+
+using namespace ag;
+
+extern "C" {
+
+ag_status ag_parquet_snappy_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                           int64_t* d_written, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  return snappy_dev(d_src, pages, n_pages, d_dst, d_written, nullptr, resolve_stream(s));
+}
+
+// host flavour: stage the compressed bytes, decompress, copy back only the bytes each page wrote
+ag_status ag_parquet_snappy_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                       int64_t* written) {
+  AG_TRY(ensure_init());
+  int64_t src_end, dst_end;
+  AG_TRY(snappy_check("snappy_decompress", pages, n_pages, &src_end, &dst_end));
+  if (n_pages == 0) return AG_OK;
+  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "snappy_decompress: NULL compressed data");
+  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "snappy_decompress: NULL output");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const size_t o_dst = ((size_t)src_end + 255) & ~(size_t)255;
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, o_dst + (size_t)dst_end));
+  AG_TRY(h2d(d, src, (size_t)src_end, cs));
+  std::vector<int64_t> w((size_t)n_pages, 0);                    // stays 0 when the call fails before decoding
+  const ag_status rc = snappy_dev(d, pages, n_pages, d + o_dst, nullptr, w.data(), cs);
+  // a corrupt page still delivers the bytes of its valid elements
+  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
+  if (written) memcpy(written, w.data(), (size_t)n_pages * 8);
+  for (int64_t i = 0; i < n_pages; ++i) AG_TRY(d2h(dst + pages[i].dst, d + o_dst + pages[i].dst, (size_t)w[i], cs));
+  const ag_status rs = sync(cs);
+  return rc != AG_OK ? rc : rs;
+}
+
+}  // extern "C"

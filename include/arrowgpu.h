@@ -666,6 +666,58 @@ ag_status ag_parquet_delta_decode_dev(int value_width, const uint8_t* d_data, co
                                       const uint8_t* d_valid, void* d_out, int64_t* d_decoded, ag_stream_t s);
 
 /* ================================================================================= *
+ * SNAPPY page decompression — a batch of pages in one call, so that a reader uploads a column chunk as it sits in the
+ *   file and decodes it in device memory.  The output is what the page decoders above take (`ag_pq_page` offsets then
+ *   point into `dst`).  serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> compress.Decode
+ *   (parquet/compress/compress.go:107) -> snappyCodec.DecodeWithError (parquet/compress/snappy.go:43-45).
+ *     src      byte offset of the page's compressed bytes in `src`
+ *     src_len  compressed bytes
+ *     dst      byte offset of the page's output in `dst` (any byte offset)
+ *     dst_len  the page header's uncompressed size (a v2 page: minus its level bytes, which are never compressed)
+ *   `pages` is a HOST array in both flavours; pages may come in any order.  written (may be NULL) receives the bytes
+ *   each page wrote.  The device flavour synchronises `s` once, to read the per-page error codes back; d_written is a
+ *   device array.  The host flavour stages `src` and `dst` through device memory and copies back only written bytes.
+ *   `src` and `dst` must not overlap (not checked).
+ *   Argument checks, AG_ERR_INVALID before any launch: a negative field, src_len or dst_len above 2^32-1, and dst
+ *   ranges that overlap each other (empty ranges overlap nothing).
+ *   Format: raw Snappy, with the checks golang/snappy's decode makes.  A preamble holds the uncompressed length as a
+ *   binary.Uvarint (missing, overflowing or above 0xffffffff is corrupt), then elements by the low two tag bits:
+ *     00 literal, length-1 = tag>>2, or for 60..63 the next 1..4 bytes little-endian;
+ *     01 copy, length 4+((tag>>2)&7), 11-bit offset (tag>>5)<<8 | next byte;
+ *     10 copy, length 1+(tag>>2), 2-byte offset;   11 copy, length 1+(tag>>2), 4-byte offset.
+ *   Copies may overlap their own output (offset < length).  Corrupt: a literal or an offset cut off by the end of the
+ *   stream; a copy with offset 0 or an offset greater than the bytes produced so far; an element that would produce
+ *   more than the preamble's length; a stream that ends before the output is full (so trailing elements after a full
+ *   output are corrupt too).
+ *   Page outcomes:
+ *     - src_len == 0 && dst_len == 0: success with 0 bytes (the empty v2 value region of a page with no values);
+ *     - preamble != dst_len: "parquet: metadata said %d bytes uncompressed data page, got %d bytes"
+ *       (page_reader.go:1094-1095); nothing of the page is written and written = 0;
+ *     - a corrupt stream: "parquet: could not decompress page: snappy: corrupt input"; written = the bytes the elements
+ *       before the failing one produce, and those bytes are correct;
+ *     - every other page of the batch is decoded in full.  The call returns AG_ERR_INVALID naming the lowest failing
+ *       page: "snappy_decompress: page %lld: <message> (%lld bytes written)".
+ *   No byte outside [dst, dst + dst_len) of any page is ever written, on error paths too.
+ *   Differences from the reference (DESIGN §2):
+ *     - the reference calls github.com/klauspost/compress/snappy, whose source is not in the reference tree; the inner
+ *       message follows golang/snappy's ErrCorrupt and is not pinned against the reference;
+ *     - S2 extensions (repeat-offset copies) are corrupt here: a SNAPPY page is plain Snappy;
+ *     - a size mismatch is reported from the preamble without decoding the body (the reference decodes first, so it
+ *       would report a corrupt body before the mismatch);
+ *     - dictionary pages get the data-page wording of the size message.
+ * ================================================================================= */
+typedef struct ag_pq_compressed {
+  int64_t src;
+  int64_t src_len;
+  int64_t dst;
+  int64_t dst_len;
+} ag_pq_compressed;
+ag_status ag_parquet_snappy_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                       int64_t* written);
+ag_status ag_parquet_snappy_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                           int64_t* d_written, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

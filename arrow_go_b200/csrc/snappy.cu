@@ -13,7 +13,7 @@
 //      descriptor {output position, literal source / copy offset, literal flag}, so a failing page knows how many
 //      bytes its valid elements produce before anything is executed.  A literal longer than the window moves the next
 //      span (and window) past it without loading it.
-//   2. snappy_exec_kernel: walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
+//   2. snappy_exec_kernel (lz_exec.cuh, shared with ZSTD): walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
 //      dst[pos - off + (j mod off)], so every output byte names one source byte: a compressed byte (literals), an
 //      output byte before the batch (read back from dst, which the same block wrote, L2-resident), or an earlier byte
 //      of the same batch.  Pointer jumping in shared memory resolves the last kind, so overlapping copies and copies of
@@ -25,7 +25,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "host_stage.cuh"
+#include "lz_exec.cuh"
 
 namespace ag {
 
@@ -37,18 +37,14 @@ constexpr int kPer = kSpan / kSnThreads;    // 4 consecutive positions per threa
 constexpr int kWinVec = 1024;               // 16-byte vectors per shared-memory window (16 KB)
 constexpr int kWinBytes = kWinVec * 16;
 constexpr int kLook = 4;                    // bytes an element header reaches past its tag byte
-constexpr int kBatch = 2048;                // output bytes per execute step
 constexpr unsigned long long kCntOne = 1ull << 48;   // parse scan: element count in bits 48.., output bytes below
 constexpr unsigned long long kLenMask = kCntOne - 1;
 constexpr unsigned long long kLenClamp = 1ull << 33; // any longer element is corrupt (dst_len <= 2^32-1)
-constexpr unsigned long long kFromDst = 1ull << 62;  // execute: source byte is dst[low bits]
-constexpr unsigned long long kFromSrc = 1ull << 63;  // execute: source byte is the page's compressed byte [low bits]
-constexpr unsigned long long kPosMask = (1ull << 62) - 1;
 
 enum SnapErr : int { kSnOk = 0, kSnCorrupt = 1, kSnSize = 2 };
 
 struct SnapPage {           // written by snappy_parse_kernel, read by snappy_exec_kernel and the host
-  int64_t written;          // output bytes of the page's valid elements
+  int64_t written;          // output bytes of the page's valid elements (LzExec::done)
   int64_t nelem;            // element descriptors written
   int64_t preamble;         // the stream's uncompressed length (kSnSize names it)
   int32_t err;
@@ -278,104 +274,13 @@ snappy_parse_kernel(SnapArgs a) {
   }
 }
 
-// one block per page: the page's output in batches of kBatch bytes, in order
-__global__ void __launch_bounds__(kSnThreads)
-snappy_exec_kernel(SnapArgs a) {
-  __shared__ uint32_t s_out[kBatch + 1], s_ref[kBatch + 1];
-  __shared__ uint8_t s_lit[kBatch + 1];
-  __shared__ unsigned long long s_src[kBatch];
-  const int64_t p = blockIdx.x;
-  const SnapPage ps = a.st[p];
-  const int64_t written = ps.written, nelem = ps.nelem;
-  if (written <= 0 || nelem <= 0) return;                        // block-uniform
-  const ag_pq_compressed pg = a.pages[p];
-  const uint8_t* in = a.src + pg.src;
-  uint8_t* out = a.dst + pg.dst;
-  const int64_t eb = a.elem_base[p];
-  const int tid = threadIdx.x;
-  int64_t e0 = 0;                                                // the element holding the batch's first byte
-  for (int64_t B = 0; B < written; B += kBatch) {
-    const int nb = (int)(written - B < kBatch ? written - B : kBatch);
-    // elements e0 .. e0 + nl - 1 hold every byte of [B, B + kBatch] (each element produces at least one byte)
-    const int nl = (int)(nelem - e0 < kBatch + 1 ? nelem - e0 : kBatch + 1);
-    for (int k = tid; k < nl; k += kSnThreads) {
-      s_out[k] = a.e_out[eb + e0 + k];
-      s_ref[k] = a.e_ref[eb + e0 + k];
-      s_lit[k] = a.e_lit[eb + e0 + k];
-    }
-    __syncthreads();
-    auto holder = [&](uint32_t pos) {                            // last loaded element starting at or before pos
-      int lo = 0, hi = nl - 1;
-      while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (s_out[mid] <= pos) lo = mid; else hi = mid - 1;
-      }
-      return lo;
-    };
-    for (int b = tid; b < nb; b += kSnThreads) {
-      const uint32_t pos = (uint32_t)(B + b);
-      const int e = holder(pos);
-      const uint32_t j = pos - s_out[e], r = s_ref[e];
-      unsigned long long s;
-      if (s_lit[e]) {
-        s = kFromSrc | (unsigned long long)(r + j);
-      } else {
-        const uint32_t q = s_out[e] - r + (r >= 64 ? j : j % r);   // a copy is at most 64 bytes long
-        s = (int64_t)q < B ? kFromDst | q : (unsigned long long)((int64_t)q - B);
-      }
-      s_src[b] = s;
-    }
-    __syncthreads();
-    while (true) {                                               // pointer jumping to a byte outside the batch
-      bool pend = false;
-      for (int b = tid; b < nb; b += kSnThreads) {
-        const unsigned long long v = s_src[b];
-        if (v < kFromDst) {
-          const unsigned long long w = s_src[v];
-          s_src[b] = w;
-          pend |= w < kFromDst;
-        }
-      }
-      if (!__syncthreads_or(pend)) break;
-    }
-    for (int b = tid; b < nb; b += kSnThreads) {
-      const unsigned long long v = s_src[b];
-      // dst bytes before the batch were written by this block before the last barrier: a plain (coherent) load
-      out[B + b] = (v & kFromSrc) ? __ldg(in + (v & kPosMask)) : out[v & kPosMask];
-    }
-    e0 += holder((uint32_t)(B + kBatch < written ? B + kBatch : written - 1));
-    __syncthreads();
-  }
+// one block per page: the page's output from its element descriptors (lz_exec.cuh)
+__global__ void __launch_bounds__(kLzThreads)
+snappy_exec_kernel(LzExec a) {
+  lz_exec_page(a, blockIdx.x);
 }
 
 }  // namespace
-
-// Argument checks shared by both flavours; every one is AG_ERR_INVALID before any launch.  *src_end / *dst_end: the
-// bytes of `src` / `dst` the batch spans.
-static ag_status snappy_check(const char* fn, const ag_pq_compressed* pages, int64_t n_pages, int64_t* src_end, int64_t* dst_end) {
-  *src_end = *dst_end = 0;
-  if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
-  if (n_pages == 0) return AG_OK;
-  if (!pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
-  std::vector<int64_t> order;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const ag_pq_compressed& g = pages[i];
-    if (g.src < 0 || g.src_len < 0 || g.dst < 0 || g.dst_len < 0 || g.src_len > 0xffffffffLL || g.dst_len > 0xffffffffLL)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field or more than 2^32-1 bytes", fn, (long long)i);
-    *src_end = std::max(*src_end, g.src + g.src_len);
-    *dst_end = std::max(*dst_end, g.dst + g.dst_len);
-    if (g.dst_len > 0) order.push_back(i);
-  }
-  std::sort(order.begin(), order.end(), [&](int64_t x, int64_t y) { return pages[x].dst < pages[y].dst || (pages[x].dst == pages[y].dst && x < y); });
-  for (size_t k = 1; k < order.size(); ++k) {
-    const ag_pq_compressed &u = pages[order[k - 1]], &v = pages[order[k]];
-    if (v.dst < u.dst + u.dst_len) {
-      const int64_t x = std::min(order[k - 1], order[k]), y = std::max(order[k - 1], order[k]);
-      AG_FAIL(AG_ERR_INVALID, "%s: pages %lld and %lld: overlapping dst ranges", fn, (long long)x, (long long)y);
-    }
-  }
-  return AG_OK;
-}
 
 // Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
 // `st` once to read the per-page error codes back.  h_written (host, may be NULL) receives the bytes per page.
@@ -383,7 +288,7 @@ static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, i
                             int64_t* h_written, cudaStream_t st) {
   const char* fn = "snappy_decompress";
   int64_t src_end, dst_end;
-  AG_TRY(snappy_check(fn, pages, n_pages, &src_end, &dst_end));
+  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
   if (n_pages == 0) return AG_OK;
   if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
   if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
@@ -419,7 +324,11 @@ static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, i
   a.d_written = d_written;
   snappy_parse_kernel<<<(unsigned)n_pages, kSnThreads, 0, st>>>(a);
   AG_TRY(check_launch("snappy_parse_kernel"));
-  snappy_exec_kernel<<<(unsigned)n_pages, kSnThreads, 0, st>>>(a);
+  LzExec x;
+  x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = nullptr; x.lit_base = nullptr; x.dst = dst;
+  x.done = reinterpret_cast<const int64_t*>(a.st); x.stride = sizeof(SnapPage) / 8;
+  x.e_out = a.e_out; x.e_ref = a.e_ref; x.e_lit = a.e_lit;
+  snappy_exec_kernel<<<(unsigned)n_pages, kLzThreads, 0, st>>>(x);
   AG_TRY(check_launch("snappy_exec_kernel"));
   std::vector<SnapPage> hs((size_t)n_pages);
   AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
@@ -453,25 +362,7 @@ ag_status ag_parquet_snappy_decompress_dev(const uint8_t* d_src, const ag_pq_com
 ag_status ag_parquet_snappy_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                        int64_t* written) {
   AG_TRY(ensure_init());
-  int64_t src_end, dst_end;
-  AG_TRY(snappy_check("snappy_decompress", pages, n_pages, &src_end, &dst_end));
-  if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "snappy_decompress: NULL compressed data");
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "snappy_decompress: NULL output");
-  CallStream cs; AG_TRY(cs.acquire());
-  Temps t(cs);
-  const size_t o_dst = ((size_t)src_end + 255) & ~(size_t)255;
-  uint8_t* d;
-  AG_TRY(t.alloc_t(&d, o_dst + (size_t)dst_end));
-  AG_TRY(h2d(d, src, (size_t)src_end, cs));
-  std::vector<int64_t> w((size_t)n_pages, 0);                    // stays 0 when the call fails before decoding
-  const ag_status rc = snappy_dev(d, pages, n_pages, d + o_dst, nullptr, w.data(), cs);
-  // a corrupt page still delivers the bytes of its valid elements
-  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
-  if (written) memcpy(written, w.data(), (size_t)n_pages * 8);
-  for (int64_t i = 0; i < n_pages; ++i) AG_TRY(d2h(dst + pages[i].dst, d + o_dst + pages[i].dst, (size_t)w[i], cs));
-  const ag_status rs = sync(cs);
-  return rc != AG_OK ? rc : rs;
+  return pq_decompress_host("snappy_decompress", snappy_dev, src, pages, n_pages, dst, written);
 }
 
 }  // extern "C"

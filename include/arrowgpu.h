@@ -718,6 +718,67 @@ ag_status ag_parquet_snappy_decompress_dev(const uint8_t* d_src, const ag_pq_com
                                            int64_t* d_written, ag_stream_t s);
 
 /* ================================================================================= *
+ * ZSTD page decompression — the same batch contract as SNAPPY above (`ag_pq_compressed` host table, pages in any
+ *   order, `written` in bytes per page, one stream synchronisation in the device flavour, the host flavour stages
+ *   `src` and `dst` and copies back only written bytes, the same argument checks before any launch).
+ *   serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> zstdCodec.DecodeWithError
+ *   (parquet/compress/zstd.go:115-118) with the decoder of getdecoder (:100-105): zstd.NewReader(nil), default options.
+ *   Format (RFC 8878), what that decoder's DecodeAll accepts for a page body:
+ *     - one or more frames back to back; skippable frames (magic 0x184D2A50..0x184D2A5F, 4-byte size) are skipped;
+ *     - the frame header in full (descriptor, window descriptor, dictionary ID, content size of 0 / 1 / 2 (+256) / 4 /
+ *       8 bytes); the reserved bit set is corrupt; a non-zero dictionary ID is refused (no dictionary is supplied);
+ *     - Raw, RLE and Compressed zstd blocks; the reserved type is corrupt; a zstd block's stored size and output are at
+ *       most min(window, 128 KiB);
+ *     - Raw, RLE, Huffman (1 stream, or 4 with the jump table) and Treeless literals (the frame's previous Huffman
+ *       table); Huffman descriptions with FSE-compressed or direct 4-bit weights, code lengths up to 11 bits;
+ *     - every sequence-count form; Predefined, RLE, FSE_Compressed and Repeat modes, accuracy logs up to 9 / 8 / 9
+ *       (LL / OF / ML); the repeat-offset rules, including the shift for a literal length of 0 and `rep0 - 1`;
+ *     - the content checksum: the low 32 bits of XXH64 (seed 0) over the frame's output.
+ *   Exactness checks: a Huffman stream decodes exactly its share of the literals; every backward bitstream has its
+ *   padding marker and is consumed exactly; sequences never consume more literals than the zstd block has; an offset
+ *   of 0, beyond the bytes the frame has produced or beyond its window is corrupt; a frame with a content size produces
+ *   exactly that many bytes.  A page's sequences may not exceed dst_len / 3 (every match is at least 3 bytes).
+ *   Page outcomes:
+ *     - src_len == 0 && dst_len == 0: success with 0 bytes;
+ *     - every frame has a content size and their sum != dst_len: "parquet: metadata said %d bytes uncompressed data
+ *       page, got %d bytes" with that sum; nothing of the page is written;
+ *     - the page decodes, but its frames (some without a content size) produce a total != dst_len: the same message
+ *       with the real total; nothing of the page is written;
+ *     - a corrupt page: "parquet: could not decompress page: zstd: <check>"; written = the bytes of the whole zstd
+ *       blocks (and earlier frames) before the first failing zstd block, and those bytes are correct.  <check> is the
+ *       first that fails, checked per page in this order: the frame / zstd-block header walk, then per zstd block its
+ *       section headers, Huffman literals, sequences bitstream, then execution:
+ *         truncated     the input ends inside a frame header, zstd block or checksum
+ *         bad magic     neither a zstd nor a skippable frame
+ *         frame header  the reserved bit of the frame header descriptor is set
+ *         dictionary    a non-zero dictionary ID
+ *         block type    the reserved zstd-block type
+ *         block size    a zstd block's stored size or output above min(window, 128 KiB)
+ *         literals      a literals section header that does not fit its zstd block
+ *         huffman       a bad Huffman description or stream, or Treeless literals with no previous table
+ *         fse           a bad FSE table description
+ *         sequences     a bad sequences header or bitstream, Repeat with no previous table, a page with more than
+ *                       dst_len / 3 sequences, sequences that consume more literals than the zstd block has
+ *         offset        an offset of 0, beyond the frame's output so far or beyond its window
+ *         content size  a frame that does not produce its content size
+ *         page size     the output passes dst_len before the failing zstd block (the output stops there instead)
+ *     - a checksum mismatch: "parquet: could not decompress page: zstd: checksum mismatch"; the frame's bytes are out
+ *       and written counts them (with every other zstd block before the first failing one);
+ *     - every other page of the batch is decoded in full.  The call returns AG_ERR_INVALID naming the lowest failing
+ *       page: "zstd_decompress: page %lld: <message> (%lld bytes written)".
+ *   No byte outside [dst, dst + dst_len) of any page is ever written, on error paths too.
+ *   Differences from the reference (DESIGN §2):
+ *     - klauspost/compress's source is not in the reference tree, so the inner messages are not pinned against it;
+ *     - dictionaries are refused;
+ *     - sizes are reported as above, from the frame headers or before anything is executed, not after a full decode;
+ *     - dictionary pages get the data-page wording of the size message.
+ * ================================================================================= */
+ag_status ag_parquet_zstd_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                     int64_t* written);
+ag_status ag_parquet_zstd_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                         int64_t* d_written, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

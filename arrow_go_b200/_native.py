@@ -50,6 +50,8 @@ class PqPage(C.Structure):
 
 
 PQ_LEVELS_V2_RLE, PQ_LEVELS_V1_RLE, PQ_LEVELS_BIT_PACKED = 0, 1, 2
+# include/arrowgpu.h AG_PQ_ENC_* (parquet.thrift Encoding values)
+PQ_ENC_PLAIN, PQ_ENC_PLAIN_DICTIONARY, PQ_ENC_DELTA_LENGTH_BYTE_ARRAY, PQ_ENC_DELTA_BYTE_ARRAY, PQ_ENC_RLE_DICTIONARY = 0, 2, 6, 7, 8
 
 
 def page_table(pages):
@@ -216,6 +218,8 @@ _SIGS = {
     "ag_parquet_plain_decode_spaced_dev": [_i, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_delta_decode": [_i, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_delta_decode_dev": [_i, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_byte_array_decode": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_byte_array_decode_dev": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p, _p],
     "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_zstd_decompress": [_p, _p, _i64, _p, _p],

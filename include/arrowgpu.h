@@ -666,6 +666,73 @@ ag_status ag_parquet_delta_decode_dev(int value_width, const uint8_t* d_data, co
                                       const uint8_t* d_valid, void* d_out, int64_t* d_decoded, ag_stream_t s);
 
 /* ================================================================================= *
+ * BYTE_ARRAY pages into an Arrow Binary / String (offset_width 4, int32 offsets) or LargeBinary / LargeString
+ *   (offset_width 8) array: `offsets` plus one data buffer, as arrow-go's byteArrayRecordReader builds with
+ *   array.BinaryBuilder (parquet/file/record_reader.go:902-1030).  The same batch-of-pages contract as
+ *   ag_parquet_dict_decode: a host page table, pages in any order, valid == NULL for dense output, pg.out is both the
+ *   slot and the bit offset, decoded[i] counts page i's slots, and the device flavour synchronises `s` once.
+ *   encoding is the parquet.thrift Encoding of the pages (AG_PQ_ENC_*); any other encoding or offset width is
+ *   AG_ERR_INVALID.  Argument checks, AG_ERR_INVALID before any launch: a negative field, a page's slots past
+ *   n_slots, and page slot ranges that overlap.
+ *   Offsets.  `offsets` holds n_slots + 1 entries of offset_width bytes; offsets[0] = offset_base, and slot i's length
+ *   is 0 when it is null, past its page's decoded count or covered by no page, so `offsets` is always a valid Arrow
+ *   offsets buffer.  *total = offsets[n_slots] - offset_base.
+ *   Data.  out_data is the array's whole data buffer: slot i's bytes go to out_data[offsets[i] .. offsets[i+1]).
+ *   offset_base lets one chunk be decoded by chained calls (the dictionary-encoded pages, then the PLAIN pages a
+ *   writer fell back to, with offset_base = the first call's total and `offsets` advanced to the second call's first
+ *   slot).  When offset_base + *total > out_cap the call returns AG_OK with the offsets and *total written and no byte
+ *   of out_data written, so out_data = NULL, out_cap = 0 is a size query.  PLAIN and DELTA_LENGTH_BYTE_ARRAY totals are
+ *   bounded by the page bytes; dictionary and DELTA_BYTE_ARRAY totals are not.  The device decides whether the bytes
+ *   fit.  With offset_width 4, offset_base + total > 2^31-1 is AG_ERR_INVALID and neither offsets nor data are written
+ *   (arrow-go only debug.Asserts this, arrow/array/binarybuilder.go:347).
+ *   Encodings (each error is AG_ERR_INVALID "byte_array_decode: page %lld: <message> (%lld values decoded)" naming the
+ *   lowest failing page; every other page is decoded in full):
+ *     AG_PQ_ENC_PLAIN: PlainByteArrayDecoder.Decode / DecodeSpaced (parquet/internal/encoding/byte_array_decoder.go:
+ *       144-189): a 4-byte little-endian length, then the bytes.  "parquet: eof reading bytearray" when a length or a
+ *       value is cut off, "parquet: invalid BYTE_ARRAY value" for a negative length.  Bytes after the last value the
+ *       page's slots need are not looked at.
+ *     AG_PQ_ENC_PLAIN_DICTIONARY / AG_PQ_ENC_RLE_DICTIONARY: dict_offsets (dict_len + 1 entries of offset_width) and
+ *       dict_data are what this call produces from the dictionary page with AG_PQ_ENC_PLAIN, dense, offset_base 0
+ *       (configureDict, parquet/file/column_reader.go:333-361).  Runs, bit widths, their messages and the
+ *       out-of-range index (message, *bad_pos, a slot of length 0) are those of ag_parquet_dict_decode.
+ *     AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY: DeltaLengthByteArrayDecoder.SetData / Decode (delta_length_byte_array.go:
+ *       113-188): every length of the DELTA_BINARY_PACKED INT32 stream is decoded and checked before any value is
+ *       delivered (header and chain errors are ag_parquet_delta_decode's messages; "parquet: negative delta byte array
+ *       length %d"; "parquet: delta byte array lengths exceed payload size").  The values start at the length
+ *       stream's bytesRead(), the end of the miniblock holding the last length.
+ *     AG_PQ_ENC_DELTA_BYTE_ARRAY: DeltaByteArrayDecoder.SetData / Decode (delta_byte_array.go:166-303): a stream of
+ *       prefix lengths, then a DELTA_LENGTH_BYTE_ARRAY stream of suffixes.  "parquet: delta prefix and suffix length
+ *       counts do not match"; "parquet: first delta byte array prefix length must be zero"; "parquet: invalid delta
+ *       byte array prefix length %d" (negative, or longer than the previous value).  The previous value resets on
+ *       every page and, spaced, is the previous valid value.
+ *     A DELTA page with fewer values than valid slots (spaced) is "parquet: number of values / definition levels read
+ *     did not match" and delivers nothing; dense, it delivers a short count.  The reference's "delta length / prefix
+ *     count exceeds value count" and "not enough ..." checks cannot fire after the stream header's own count check.
+ *   No UTF-8 validation, as in the reference.
+ *   Differences from the reference (DESIGN §2):
+ *     - a PLAIN value or a DELTA_BYTE_ARRAY prefix that fails still delivers the values before it; decoded says how
+ *       many slots were written (the reference's Decode returns (0, err) for DELTA_BYTE_ARRAY);
+ *     - the dictionary page is decoded in full up front (the reference's dictConverter reads it lazily);
+ *     - offset_base + total > 2^31-1 with int32 offsets is an error, not a debug assertion.
+ *   The device flavour: *total is host memory, d_decoded and d_bad_pos (may be NULL) device memory, *d_bad_pos is
+ *   overwritten.  The host flavour stages `data`, `valid` and the dictionary, and copies back the offsets and only
+ *   the bytes it wrote; out_data outside them is untouched.
+ * ================================================================================= */
+#define AG_PQ_ENC_PLAIN                   0
+#define AG_PQ_ENC_PLAIN_DICTIONARY        2
+#define AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY 6
+#define AG_PQ_ENC_DELTA_BYTE_ARRAY        7
+#define AG_PQ_ENC_RLE_DICTIONARY          8
+ag_status ag_parquet_byte_array_decode(int encoding, int offset_width, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                       int64_t n_slots, const uint8_t* valid, const void* dict_offsets, const uint8_t* dict_data,
+                                       int64_t dict_len, int64_t offset_base, void* offsets, uint8_t* out_data, int64_t out_cap,
+                                       int64_t* total, int64_t* decoded, int64_t* bad_pos);
+ag_status ag_parquet_byte_array_decode_dev(int encoding, int offset_width, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                           int64_t n_slots, const uint8_t* d_valid, const void* d_dict_offsets, const uint8_t* d_dict_data,
+                                           int64_t dict_len, int64_t offset_base, void* d_offsets, uint8_t* d_out_data, int64_t out_cap,
+                                           int64_t* total, int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s);
+
+/* ================================================================================= *
  * SNAPPY page decompression — a batch of pages in one call, so that a reader uploads a column chunk as it sits in the
  *   file and decodes it in device memory.  The output is what the page decoders above take (`ag_pq_page` offsets then
  *   point into `dst`).  serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> compress.Decode

@@ -9,6 +9,9 @@ move) and their share of the HBM peak, with the card's name and power limit.  Ea
 synchronisation (per-page error codes), which the times include.  Four distinct page bodies are reused round-robin;
 every page writes its own output range.  Writes nothing to disk.
 
+--bytearray runs only the BYTE_ARRAY cases (ag_parquet_byte_array_decode_dev, csrc/byte_array.cu): time, share of the HBM
+peak, and a torch.profiler split of the device time over the three stages (values, offsets, bytes).
+
 --profile runs only the DELTA_BINARY_PACKED, SNAPPY and ZSTD cases, under torch.profiler, and reports the device time
 per call of each kernel (the delta block walk against the value passes, the Snappy parse against the execute, the ZSTD
 walk / literals / sequences / resolve / execute / checksum kernels) instead.
@@ -73,6 +76,7 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--bytearray", action="store_true")
     args = ap.parse_args()
 
     from arrow_go_b200 import _native as N
@@ -117,6 +121,11 @@ def main():
         return {"ms": ms, "values_per_s": n / ms * 1e3, "algorithmic_bytes": ab, "encoded_bytes": enc,
                 "gbs": ab / ms / 1e6, "frac": ab / ms / 1e6 / peak, "note": note}
 
+    if args.bytearray:
+        res = {"peak_gbs": peak, "peak_kind": peak_kind, **card(), "timing": res["timing"]}
+        res.update(bytearray_cases(args, N, np.random.default_rng(0xB17E), timed, upload, DeviceBuffer))
+        print(json.dumps(res), flush=True)
+        return
     dout = DeviceBuffer(8 * n + 64)
     if args.profile:
         res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer, profile=True))
@@ -163,7 +172,7 @@ def kernel_ms(prof, steps):
     kern = {}
     for ev in prof.key_averages():
         if ev.device_type == torch.autograd.DeviceType.CUDA:
-            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel)(<[^>]*>)?", ev.key)
+            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|ba_\w+_kernel)(<[^>]*>)?", ev.key)
             short = (m.group(1) + (m.group(2) or "")) if m else ev.key.strip()
             us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
             kern[short] = kern.get(short, 0.0) + us / 1e3 / steps
@@ -368,6 +377,128 @@ def zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, De
         out["zstd_timestamps_over_copy"] = out["parquet_zstd_i64_timestamps"]["ms"] / ms
         cp.free()
     tsrc.free(); isrc.free(); ddst.free(); dec.free(); ddict.free(); bad.free()
+    return out
+
+
+
+def bytearray_cases(args, N, rng, timed, upload, DeviceBuffer, values=20_000_000):
+    """BYTE_ARRAY pages of ~1 MiB (pyarrow's default page size) into int64 offsets + data, dense, ~20M values:
+    (a) RLE_DICTIONARY, 14-bit indices into 10K short strings (3..20 bytes); (b) PLAIN random lengths (0..70 bytes,
+    mean ~14); (c) DELTA_LENGTH_BYTE_ARRAY of the same values; (d) DELTA_BYTE_ARRAY on sorted keys ("key_" + 9
+    digits); (e) the PLAIN pages of (b) compressed with SNAPPY: decompression, then decode.  Algorithmic bytes: encoded
+    bytes read + offsets written (8 per slot) + data written (+ the dictionary bytes read for (a)).  Four distinct page
+    bodies are reused round-robin; every page writes its own slots."""
+    import ctypes as C
+
+    import pyarrow as pa
+    import torch
+    from torch.profiler import ProfilerActivity, profile as tprofile
+
+    import pq_bytearray_files as BF
+    import pq_bytearray_ref as B
+    out = {}
+
+    def make(bodies, per_page):
+        n_pages = max(1, values // per_page)
+        blob = b"".join(bodies) + bytes(16)
+        offs = np.cumsum([0] + [len(x) for x in bodies])
+        pages = [(int(offs[p % 4]), len(bodies[p % 4]), per_page, p * per_page) for p in range(n_pages)]
+        enc = sum(len(bodies[p % 4]) for p in range(n_pages))
+        return upload(np.frombuffer(blob, np.uint8)), pages, enc, n_pages
+
+    def stages(kern):
+        s = {"values": 0.0, "offsets": 0.0, "bytes": 0.0}
+        for k, v in kern.items():
+            if "ba_gather" in k:
+                s["bytes"] += v
+            elif any(x in k for x in ("ba_slot", "ba_sum", "ba_scan", "ba_offsets")):
+                s["offsets"] += v
+            else:
+                s["values"] += v
+        return s
+
+    def run(name, enc_id, dblob, pages, enc, n_pages, per_page, data_bytes, note, dict_args=None, extra_read=0, pre=None):
+        n = n_pages * per_page
+        tbl = N.page_table(pages)
+        doffs, dout = DeviceBuffer(8 * (n + 1) + 64), DeviceBuffer(data_bytes + 64)
+        dec = DeviceBuffer(8 * n_pages + 64)
+        tot = C.c_int64(0)
+        do, dd, dl = dict_args or (None, None, 0)
+        call = lambda: N.call("ag_parquet_byte_array_decode_dev", enc_id, 8, dblob.ptr, tbl, n_pages, n, None, do, dd, dl, 0,
+                              doffs.ptr, dout.ptr, data_bytes, C.byref(tot), dec.ptr, None, None)
+        fn = (lambda: (pre(), call())) if pre else call
+        fn()
+        assert tot.value == data_bytes, (name, tot.value, data_bytes)
+        ms = timed(fn)
+        ab = enc + 8.0 * (n + 1) + data_bytes + extra_read
+        with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                fn()
+            torch.cuda.synchronize()
+        kern = kernel_ms(prof, args.steps)
+        out[name] = {"ms": ms, "values": n, "pages": n_pages, "values_per_page": per_page, "encoded_bytes": enc,
+                     "data_bytes": data_bytes, "algorithmic_bytes": ab, "gbs": ab / ms / 1e6, "frac": ab / ms / 1e6 / peak_of(),
+                     "stage_ms_per_call": stages(kern), "kernels_ms_per_call": kern, "note": note}
+        doffs.free(); dout.free(); dec.free()
+
+    from bench import peaks
+    peak_of = lambda: peaks()[0]
+
+    # (a) dictionary
+    dictionary = [bytes(rng.integers(97, 123, int(k), dtype=np.uint8)) for k in rng.integers(3, 21, 10_000)]
+    dl = np.array([len(v) for v in dictionary], np.int64)
+    ddoff, dddata = upload(np.concatenate([[0], np.cumsum(dl)]).astype(np.int64)), upload(np.frombuffer(b"".join(dictionary), np.uint8))
+    per = 1 << 19
+    idx = [rng.integers(0, 10_000, per) for _ in range(4)]
+    bodies = [bytes([14]) + rle_literal_page(i, 14) for i in idx]
+    dblob, pages, enc, n_pages = make(bodies, per)
+    data = sum(int(dl[idx[p % 4]].sum()) for p in range(n_pages))
+    run("bytearray_dict_short_strings", B.RLE_DICTIONARY, dblob, pages, enc, n_pages, per, data,
+        "RLE_DICTIONARY pages of 2^19 14-bit indices (0.9 MiB), 10K strings of 3..20 bytes", (ddoff.ptr, dddata.ptr, 10_000), extra_read=data)
+    dblob.free(); ddoff.free(); dddata.free()
+
+    # (b) PLAIN, (c) DELTA_LENGTH, (e) SNAPPY + PLAIN: ~1 MiB pages of random-length strings
+    per = 58_000
+    vals = [BF.random_strings(rng, per) for _ in range(4)]
+    vbytes = [sum(len(v) for v in vs) for vs in vals]
+    plain = [B.plain_encode(vs) for vs in vals]
+    dblob, pages, enc, n_pages = make(plain, per)
+    data = sum(vbytes[p % 4] for p in range(n_pages))
+    run("bytearray_plain_random_lengths", B.PLAIN, dblob, pages, enc, n_pages, per, data,
+        f"PLAIN pages of {per} strings of 0..70 bytes (~{len(plain[0]) >> 10} KiB)")
+    # (e) the same pages compressed: decompress into dblob's layout, then decode
+    comp = [pa.compress(b, codec="snappy", asbytes=True) for b in plain]
+    cblob = upload(np.frombuffer(b"".join(comp) + bytes(16), np.uint8))
+    coffs = np.cumsum([0] + [len(c) for c in comp])
+    dst = DeviceBuffer(enc + 64)
+    ctab, d = [], 0
+    ppages = []
+    for p in range(n_pages):
+        ctab.append((int(coffs[p % 4]), len(comp[p % 4]), d, len(plain[p % 4])))
+        ppages.append((d, len(plain[p % 4]), per, p * per))
+        d += len(plain[p % 4])
+    ctbl = N.compressed_table(ctab)
+    snap = lambda: N.call("ag_parquet_snappy_decompress_dev", cblob.ptr, ctbl, n_pages, dst.ptr, None, None)
+    csize = sum(len(comp[p % 4]) for p in range(n_pages))
+    run("bytearray_snappy_then_plain", B.PLAIN, dst, ppages, csize, n_pages, per, data,
+        "(b)'s pages compressed with SNAPPY, decompressed on the device, then decoded; algorithmic bytes count the compressed bytes",
+        pre=snap)
+    dblob.free(); cblob.free(); dst.free()
+    dlba = [B.dlba_encode(vs) for vs in vals]
+    dblob, pages, enc, n_pages = make(dlba, per)
+    run("bytearray_delta_length", B.DELTA_LENGTH_BYTE_ARRAY, dblob, pages, enc, n_pages, per, data,
+        f"DELTA_LENGTH_BYTE_ARRAY pages of the same {per} strings")
+    dblob.free()
+
+    # (d) DELTA_BYTE_ARRAY on sorted keys
+    per = 1 << 18
+    keys = [BF.random_strings(rng, per, sorted_keys=True) for _ in range(4)]
+    dba = [B.dba_encode(k) for k in keys]
+    dblob, pages, enc, n_pages = make(dba, per)
+    data = sum(sum(len(v) for v in keys[p % 4]) for p in range(n_pages))
+    run("bytearray_delta_sorted_keys", B.DELTA_BYTE_ARRAY, dblob, pages, enc, n_pages, per, data,
+        f"DELTA_BYTE_ARRAY pages of {per} sorted 13-byte keys (~{len(dba[0]) >> 10} KiB; prefix ~7 bytes)")
+    dblob.free()
     return out
 
 

@@ -52,6 +52,9 @@ class PqPage(C.Structure):
 PQ_LEVELS_V2_RLE, PQ_LEVELS_V1_RLE, PQ_LEVELS_BIT_PACKED = 0, 1, 2
 # include/arrowgpu.h AG_PQ_ENC_* (parquet.thrift Encoding values)
 PQ_ENC_PLAIN, PQ_ENC_PLAIN_DICTIONARY, PQ_ENC_DELTA_LENGTH_BYTE_ARRAY, PQ_ENC_DELTA_BYTE_ARRAY, PQ_ENC_RLE_DICTIONARY = 0, 2, 6, 7, 8
+PQ_ENC_RLE, PQ_ENC_BYTE_STREAM_SPLIT = 3, 9
+# include/arrowgpu.h AG_PQ_TYPE_* (parquet.thrift Type values)
+PQ_TYPE_INT32, PQ_TYPE_INT64, PQ_TYPE_INT96, PQ_TYPE_FLOAT, PQ_TYPE_DOUBLE, PQ_TYPE_FIXED_LEN_BYTE_ARRAY = 1, 2, 3, 4, 5, 7
 
 
 def page_table(pages):
@@ -220,6 +223,10 @@ _SIGS = {
     "ag_parquet_delta_decode_dev": [_i, _p, _p, _i64, _p, _p, _p, _p],
     "ag_parquet_byte_array_decode": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_byte_array_decode_dev": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_bool_decode": [_i, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_bool_decode_dev": [_i, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_fixed_decode": [_i, _i, _i, _p, _p, _i64, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_fixed_decode_dev": [_i, _i, _i, _p, _p, _i64, _p, _p, _i64, _p, _p, _p, _p],
     "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_zstd_decompress": [_p, _p, _i64, _p, _p],

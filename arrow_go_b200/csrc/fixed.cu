@@ -1,0 +1,532 @@
+// fixed.cu — Parquet pages of the remaining flat physical types on the device: BOOLEAN (PLAIN bit-packed, RLE) into an
+// Arrow boolean bitmap, and INT32 / INT64 / FLOAT / DOUBLE / INT96 / FIXED_LEN_BYTE_ARRAY (PLAIN, dictionary,
+// BYTE_STREAM_SPLIT) into `width` bytes per slot.
+//   PlainBooleanDecoder.DecodeToBitmap / decodeSpacedToBitmap   parquet/internal/encoding/boolean_decoder.go:264-304
+//   RleBooleanDecoder.SetData / DecodeToBitmap                   boolean_decoder.go:321-341,382-417
+//   PlainDecoder[T] (INT96 too)                                  plain_encoding_types.go:61-110
+//   PlainFixedLenByteArrayDecoder, ByteStreamSplitFixedLenByteArrayDecoder   fixed_len_byte_array_decoder.go
+//   validateByteStreamSplitPageData, ByteStreamSplitDecoder[T]   byte_stream_split.go:98-250
+//   accepted encodings per physical type                         typed_encoder.go:250-291,432-437,538-552,714-727
+//
+// Every call runs the passes of pq_decode.cuh first: pq_tile_count_kernel (spaced), then pq_runs_kernel, one block per
+// page, which scans the spaced rank bases, walks the runs of dictionary and RLE pages and checks the pages of the
+// pass-1 kinds this file adds (kBss, kBoolPlain, kBoolRle).  What runs after it:
+//   - PLAIN and dictionary pages of 4- and 8-byte values: pq_expand_kernel<kPlain / kDict>, the kernels
+//     ag_parquet_plain_decode_spaced and ag_parquet_dict_decode run.
+//   - BYTE_STREAM_SPLIT pages of 4- and 8-byte values: pq_expand_kernel<kBss>, one thread per slot assembling its value
+//     in a register from one byte of each stream; consecutive threads read consecutive bytes of every stream and store
+//     consecutive values.
+//   - other widths, and BYTE_STREAM_SPLIT of other widths: the source of a slot is its dense rank (dense: the slot
+//     itself; spaced: pq_expand_kernel<kRank>) or its dictionary index (pq_expand_kernel<kIndex>), one int32 per slot.
+//     fx_copy_kernel then writes the output in aligned 16-byte pieces, consecutive threads on consecutive pieces, each
+//     piece assembled byte by byte from its sources (PLAIN: data[rank * width + j], dictionary: dict[index * width + j],
+//     BYTE_STREAM_SPLIT: data[j * stride + rank]).  A piece at either end of a tile is stored byte by byte, so no
+//     byte outside the slots a page decoded is written.
+//   - booleans: fx_bool_kernel, one block per 1024-slot tile.  Each thread finds its slot's value bit (PLAIN: bit
+//     `rank` of the page; RLE: the run holding `rank`, found as pq_expand_kernel finds it), a ballot per warp packs 32
+//     slots into shared memory, and one thread per aligned 32-bit output word stores it.  A word shared with a
+//     neighbouring tile or page, or with slots the call does not write, is merged with atomicAnd / atomicOr.
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "pq_decode.cuh"
+
+namespace ag {
+
+namespace {
+
+constexpr int kCopyChunk = 16384;   // output bytes per fx_copy_kernel block and step
+
+enum FxSrc { kSrcPlain = 0, kSrcDict = 1, kSrcBss = 2 };
+
+// what runs after pass 1
+enum FxJob { kJobPlainT = 0, kJobDictT = 1, kJobPlainW = 2, kJobDictW = 3, kJobBss = 4, kJobBoolPlain = 5, kJobBoolRle = 6, kJobBssT = 7 };
+
+struct FxArgs {
+  PqPlan plan;
+  const PageState* st;
+  const uint8_t* data;
+  const uint8_t* valid;     // NULL = every slot valid
+  const int32_t* map;       // per slot: dense rank or dictionary index; NULL = the slot itself
+  const uint8_t* dict;
+  int64_t dict_len;
+  int64_t width;
+  uint8_t* out;
+};
+
+// grid (tiles, chunks): block (t, y) writes the output bytes [t0 + y * kCopyChunk, ...) of tile t, stepping by
+// gridDim.y chunks
+template <int SRC>
+__global__ void __launch_bounds__(kRleThreads)
+fx_copy_kernel(FxArgs a) {
+  const int64_t tile = blockIdx.x;
+  const int64_t p = find_page(a.plan.tile_base, a.plan.n_pages, tile);
+  const ag_pq_page pg = a.plan.pages[p];
+  const PageState ps = a.st[p];
+  const int64_t s0 = (tile - a.plan.tile_base[p]) * kTile;
+  const int64_t s1 = min(s0 + (int64_t)kTile, ps.slots);
+  if (s0 >= s1) return;                                          // block-uniform
+  const int64_t w = a.width;
+  const int64_t t0 = (pg.out + s0) * w, t1 = (pg.out + s1) * w;   // the tile's output bytes
+  const uint8_t* src_base = SRC == kSrcDict ? a.dict : a.data + ps.stream;
+  const int64_t step = SRC == kSrcBss ? ps.stream_len / w : 1;   // source distance of bytes j and j + 1 of a value
+  // source offset of byte 0 of slot s's value, or -1 for a slot that holds zeros
+  auto source = [&](int64_t s) -> int64_t {
+    if (a.valid && !bit_is_set(a.valid, pg.out + s)) return -1;
+    const int64_t r = a.map ? (int64_t)a.map[pg.out + s] : s;
+    if (SRC == kSrcDict) return (r >= 0 && r < a.dict_len) ? r * w : -1;
+    return SRC == kSrcBss ? r : r * w;
+  };
+  const uintptr_t ob = reinterpret_cast<uintptr_t>(a.out);
+  for (int64_t lo = t0 + (int64_t)blockIdx.y * kCopyChunk; lo < t1; lo += (int64_t)gridDim.y * kCopyChunk) {
+    const int64_t hi = min(lo + (int64_t)kCopyChunk, t1);
+    const int64_t first = (int64_t)(((ob + lo) & ~(uintptr_t)15) - ob);   // first aligned piece touching [lo, hi)
+    for (int64_t q0 = first + (int64_t)threadIdx.x * 16; q0 < hi; q0 += (int64_t)kRleThreads * 16) {
+      const int64_t b0 = q0 > lo ? q0 : lo;
+      const int64_t rel = b0 - t0;
+      int64_t s = s0 + rel / w;
+      int64_t j = rel - (s - s0) * w;
+      int64_t src = source(s);
+      uint32_t v[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        const int64_t o = q0 + k;
+        if (o >= b0 && o < hi) {
+          if (src >= 0) v[k >> 2] |= (uint32_t)__ldg(src_base + src + j * step) << (8 * (k & 3));
+          if (++j == w) {
+            j = 0;
+            ++s;
+            if (o + 1 < hi) src = source(s);
+          }
+        }
+      }
+      if (q0 >= lo && q0 + 16 <= hi) {
+        *reinterpret_cast<uint4*>(a.out + q0) = make_uint4(v[0], v[1], v[2], v[3]);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+          const int64_t o = q0 + k;
+          if (o >= lo && o < hi) a.out[o] = (uint8_t)(v[k >> 2] >> (8 * (k & 3)));
+        }
+      }
+    }
+  }
+}
+
+// one block per tile of 1024 slots of one page; a.out is the output bitmap
+template <bool RLE, bool SPACED>
+__global__ void __launch_bounds__(kRleThreads)
+fx_bool_kernel(PqArgs a) {
+  __shared__ int warp_tot[kRleThreads / 32];
+  __shared__ uint32_t tbits[kTile / 32];                         // bit i = value of the tile's slot i
+  const int64_t tile = blockIdx.x;
+  const int2 ti = a.tile_info[tile];
+  const int64_t p = ti.x;
+  const ag_pq_page pg = a.plan.pages[p];
+  const PageState ps = a.st[p];
+  const int64_t s0 = (tile - a.plan.tile_base[p]) * kTile;
+  const int64_t limit = ps.slots;
+  if (s0 >= limit) return;                                       // block-uniform
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const uint2* runs = a.runs + (RLE ? a.plan.run_base[p] : 0);
+  const uint8_t* stream = a.data + ps.stream;
+  const int64_t rlo = ti.y;
+  int64_t rhi = tile + 1 < a.plan.tile_base[p + 1] ? a.tile_info[tile + 1].y : ps.nruns - 1;
+  if (rhi < rlo) rhi = rlo;
+
+  int64_t rank_base = SPACED ? a.tile_cnt[tile] : s0;
+#pragma unroll
+  for (int q = 0; q < kTile / kRleThreads; ++q) {
+    const int64_t s = s0 + q * kRleThreads + tid;
+    bool v = s < limit;
+    int64_t rank = s;
+    if (SPACED) {
+      v = v && bit_is_set(a.valid, pg.out + s);
+      const unsigned m = __ballot_sync(0xffffffffu, v);
+      if (lane == 0) warp_tot[wid] = __popc(m);
+      __syncthreads();
+      int off = 0, tot = 0;
+#pragma unroll
+      for (int w = 0; w < kRleThreads / 32; ++w) { const int t = warp_tot[w]; off += (w < wid) ? t : 0; tot += t; }
+      __syncthreads();
+      rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
+      rank_base += tot;
+    }
+    bool bit = false;
+    if (v) {
+      if (!RLE) {
+        bit = (__ldg(stream + (rank >> 3)) >> (rank & 7)) & 1;
+      } else {
+        int64_t lo = rlo, hi = rhi;
+        while (lo < hi) {
+          const int64_t mid = (lo + hi + 1) >> 1;
+          if ((int64_t)(runs[mid].x & ~kLiteralFlag) <= rank) lo = mid; else hi = mid - 1;
+        }
+        const uint2 r = runs[lo];
+        // a repeated value is true when any bit of its byte is set (rle.go:161-165 keeps the whole byte)
+        bit = (r.x & kLiteralFlag) ? unpack_at(stream + r.y, rank - (int64_t)(r.x & ~kLiteralFlag), 1) != 0u : r.y != 0u;
+      }
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, bit);
+    if (lane == 0) tbits[q * (kRleThreads / 32) + wid] = m;
+  }
+  __syncthreads();
+
+  // output words: absolute bits [b0, b1) of the word-aligned base
+  const int64_t s1 = min(s0 + (int64_t)kTile, limit);
+  const uintptr_t ob = reinterpret_cast<uintptr_t>(a.out);
+  uint32_t* words = reinterpret_cast<uint32_t*>(ob & ~(uintptr_t)3);
+  const int64_t b0 = (int64_t)(ob & 3) * 8 + pg.out + s0, b1 = b0 + (s1 - s0);
+  const int64_t w0 = b0 >> 5, nw = ((b1 - 1) >> 5) - w0 + 1;
+  auto tw = [&](int64_t k) -> uint32_t { return (k >= 0 && k < kTile / 32) ? tbits[k] : 0u; };
+  for (int64_t i = tid; i < nw; i += kRleThreads) {
+    const int64_t wb = (w0 + i) * 32;                            // absolute bit of the word's bit 0
+    const int64_t rel = wb - b0;                                 // tile slot at the word's bit 0 (>= -31)
+    const uint32_t val = rel >= 0 ? __funnelshift_r(tw(rel >> 5), tw((rel >> 5) + 1), (int)(rel & 31)) : tw(0) << (int)(-rel);
+    uint32_t mask = 0xffffffffu;
+    if (wb < b0) mask &= 0xffffffffu << (int)(b0 - wb);
+    if (wb + 32 > b1) mask &= 0xffffffffu >> (int)(wb + 32 - b1);
+    if (mask == 0xffffffffu) {
+      words[w0 + i] = val;
+    } else {
+      atomicAnd(words + w0 + i, ~mask);
+      atomicOr(words + w0 + i, val & mask);
+    }
+  }
+}
+
+int pass1_kind(int job) {
+  switch (job) {
+    case kJobPlainT: case kJobPlainW: return kPlain;
+    case kJobDictT: return kDict;
+    case kJobDictW: return kIndex;
+    case kJobBss: case kJobBssT: return kBss;
+    case kJobBoolPlain: return kBoolPlain;
+    default: return kBoolRle;
+  }
+}
+
+void fx_err_text(const PageState& s, const ag_pq_page& pg, int ptype, int width, char* buf, size_t n) {
+  switch (s.err) {
+    case kErrPlainShort:
+      if (ptype == AG_PQ_TYPE_INT96)
+        snprintf(buf, n, "parquet: eof exception decode plain INT96, nvals: %lld, nbytes: %lld, datalen: %lld", (long long)s.need,
+                 (long long)s.need * 12, (long long)pg.len);
+      else if (ptype == AG_PQ_TYPE_FIXED_LEN_BYTE_ARRAY) snprintf(buf, n, "parquet: eof exception");
+      else snprintf(buf, n, "%s", err_text(s.err));
+      break;
+    case kErrBssSize:
+      snprintf(buf, n, "data size (%lld) is too small for the number of values in in BYTE_STREAM_SPLIT (%lld)", (long long)pg.len,
+               (long long)pg.num_values);
+      break;
+    case kErrBssAlign:
+      if (ptype == AG_PQ_TYPE_FIXED_LEN_BYTE_ARRAY)
+        snprintf(buf, n, "ByteStreamSplit data size %lld not aligned with type FIXED_LEN_BYTE_ARRAY and byte_width: %d", (long long)pg.len, width);
+      else snprintf(buf, n, "ByteStreamSplit data size %lld not aligned with byte_width: %d", (long long)pg.len, width);
+      break;
+    case kErrBssEof: snprintf(buf, n, "parquet: eof exception"); break;
+    case kErrBssShort: snprintf(buf, n, "parquet: number of values / definitions levels read did not match"); break;
+    case kErrBoolShort:
+      snprintf(buf, n, "parquet: boolean data has %lld bits available, need %lld: unexpected EOF", (long long)pg.len * 8, (long long)s.need);
+      break;
+    case kErrBoolLength: snprintf(buf, n, "invalid length - %lld (corrupt data page?)", (long long)pg.len); break;
+    case kErrBoolBytes: snprintf(buf, n, "received invalid number of bytes - %u (corrupt data page?)", (unsigned)s.pad); break;
+    case kErrBoolEof: snprintf(buf, n, "unexpected EOF"); break;
+    default: snprintf(buf, n, "%s", err_text(s.err)); break;
+  }
+}
+
+struct FxCall {
+  const char* fn;
+  int job;
+  int ptype;                // AG_PQ_TYPE_* (booleans: 0), for the error texts
+  int width;                // bytes per value (booleans: 1)
+  const uint8_t* data;
+  const ag_pq_page* pages;
+  int64_t n_pages;
+  const uint8_t* valid;
+  const void* dict;
+  int64_t dict_len;
+  void* out;
+};
+
+// The device work of every entry point of this file.  `pages` is host memory; everything else device memory on `st`.
+// Synchronises `st` once.  h_decoded (host, may be NULL) receives the per-page decoded counts.
+ag_status fx_pages_dev(const FxCall& c, int64_t* d_decoded, int64_t* h_decoded, int64_t* d_bad_pos, cudaStream_t st) {
+  const char* fn = c.fn;
+  const int64_t n_pages = c.n_pages;
+  const int kind = pass1_kind(c.job);
+  const bool has_runs = kind == kDict || kind == kIndex || kind == kBoolRle;
+  const bool dict = c.job == kJobDictT || c.job == kJobDictW;
+  if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
+  if (n_pages == 0) return AG_OK;
+  if (!c.pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
+  // plan: pages | run_base[n+1] | tile_base[n+1], as parquet_pages_dev lays it out
+  const size_t pb = (size_t)n_pages * sizeof(ag_pq_page);
+  const size_t plan_bytes = pb + 2 * (size_t)(n_pages + 1) * 8;
+  std::vector<uint8_t> h(plan_bytes);
+  memcpy(h.data(), c.pages, pb);
+  int64_t* run_base = reinterpret_cast<int64_t*>(h.data() + pb);
+  int64_t* tile_base = run_base + n_pages + 1;
+  run_base[0] = tile_base[0] = 0;
+  bool any_data = false;
+  int64_t slot_end = 0;
+  for (int64_t i = 0; i < n_pages; ++i) {
+    const ag_pq_page& g = c.pages[i];
+    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field, more than 2^31-1 values or more than 2^32-1 bytes", fn, (long long)i);
+    any_data |= g.len > 0;
+    slot_end = std::max(slot_end, g.out + g.num_values);
+    run_base[i + 1] = run_base[i] + (has_runs ? std::min(g.num_values, g.len) : 0);
+    tile_base[i + 1] = tile_base[i] + (g.num_values + kTile - 1) / kTile;
+  }
+  const int64_t n_runs = run_base[n_pages], n_tiles = tile_base[n_pages];
+  if (n_tiles > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  if (any_data && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  if (dict && c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
+  if (c.job == kJobDictT && c.dict && (reinterpret_cast<uintptr_t>(c.dict) & (c.width - 1)))
+    AG_FAIL(AG_ERR_INVALID, "%s: dictionary not aligned to its value width", fn);
+  if ((c.job == kJobPlainT || c.job == kJobDictT || c.job == kJobBssT) && c.out && (reinterpret_cast<uintptr_t>(c.out) & (c.width - 1)))
+    AG_FAIL(AG_ERR_INVALID, "%s: output not aligned to its value width", fn);
+  const bool mapped = c.job == kJobDictW || ((c.job == kJobPlainW || c.job == kJobBss) && c.valid);
+
+  const size_t st_bytes = (size_t)n_pages * sizeof(PageState);
+  const size_t off_st = (plan_bytes + 255) & ~(size_t)255;
+  const size_t off_tc = (off_st + st_bytes + 255) & ~(size_t)255;
+  const size_t off_ti = (off_tc + (c.valid ? (size_t)n_tiles * 8 : 0) + 255) & ~(size_t)255;
+  const size_t off_bad = (off_ti + (size_t)n_tiles * 8 + 255) & ~(size_t)255;
+  const size_t off_runs = off_bad + 256;
+  const size_t off_map = (off_runs + (size_t)n_runs * 8 + 255) & ~(size_t)255;
+  const size_t total = off_map + (mapped ? (size_t)slot_end * 4 : 0);
+  // this call synchronises `st` anyway, so its device scratch may live in a Temps
+  Temps t(st);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, total));
+  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  int32_t* map = mapped ? reinterpret_cast<int32_t*>(d + off_map) : nullptr;
+  PqArgs a{};
+  a.plan.pages = reinterpret_cast<const ag_pq_page*>(d);
+  a.plan.run_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.plan.tile_base = a.plan.run_base + n_pages + 1;
+  a.plan.n_pages = n_pages;
+  a.plan.n_tiles = n_tiles;
+  a.data = c.data;
+  a.valid = c.valid;
+  a.st = reinterpret_cast<PageState*>(d + off_st);
+  a.tile_cnt = c.valid ? reinterpret_cast<int64_t*>(d + off_tc) : nullptr;
+  a.tile_info = reinterpret_cast<int2*>(d + off_ti);
+  a.bad = reinterpret_cast<unsigned long long*>(d_bad_pos ? (void*)d_bad_pos : (void*)(d + off_bad));
+  a.runs = n_runs ? reinterpret_cast<uint2*>(d + off_runs) : nullptr;
+  a.d_decoded = d_decoded;
+  a.kind = kind; a.fixed_bw = kind == kBoolRle ? 1 : 0; a.v1 = 0; a.width = c.width;
+  a.dict_len = c.dict_len; a.dict = c.dict; a.out = mapped ? (void*)map : c.out;
+  if (c.valid && n_tiles) {
+    pq_tile_count_kernel<<<grid_for(n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(a);
+    AG_TRY(check_launch("pq_tile_count_kernel"));
+  }
+  pq_runs_kernel<<<(unsigned)n_pages, kRleThreads, 0, st>>>(a);
+  AG_TRY(check_launch("pq_runs_kernel"));
+  const bool sp = c.valid != nullptr;
+  switch (c.job) {
+    case kJobPlainT:
+      AG_TRY(c.width == 4 ? (sp ? launch_expand<kPlain, uint32_t, true>(a, st) : launch_expand<kPlain, uint32_t, false>(a, st))
+                          : (sp ? launch_expand<kPlain, unsigned long long, true>(a, st) : launch_expand<kPlain, unsigned long long, false>(a, st)));
+      break;
+    case kJobDictT:
+      AG_TRY(c.width == 4 ? (sp ? launch_expand<kDict, uint32_t, true>(a, st) : launch_expand<kDict, uint32_t, false>(a, st))
+                          : (sp ? launch_expand<kDict, unsigned long long, true>(a, st) : launch_expand<kDict, unsigned long long, false>(a, st)));
+      break;
+    case kJobBssT:
+      AG_TRY(c.width == 4 ? (sp ? launch_expand<kBss, uint32_t, true>(a, st) : launch_expand<kBss, uint32_t, false>(a, st))
+                          : (sp ? launch_expand<kBss, unsigned long long, true>(a, st) : launch_expand<kBss, unsigned long long, false>(a, st)));
+      break;
+    case kJobPlainW: case kJobDictW: case kJobBss: {
+      if (c.job == kJobDictW) AG_TRY((sp ? launch_expand<kIndex, int32_t, true>(a, st) : launch_expand<kIndex, int32_t, false>(a, st)));
+      else if (mapped) AG_TRY((launch_expand<kRank, int32_t, true>(a, st)));
+      if (n_tiles == 0) break;
+      FxArgs f;
+      f.plan = a.plan; f.st = a.st; f.data = c.data; f.valid = c.valid; f.map = map;
+      f.dict = static_cast<const uint8_t*>(c.dict); f.dict_len = c.dict_len; f.width = c.width;
+      f.out = static_cast<uint8_t*>(c.out);
+      const int64_t chunks = std::min<int64_t>(((int64_t)kTile * c.width + kCopyChunk - 1) / kCopyChunk, 65535);
+      const dim3 grid((unsigned)n_tiles, (unsigned)chunks);
+      if (c.job == kJobPlainW) fx_copy_kernel<kSrcPlain><<<grid, kRleThreads, 0, st>>>(f);
+      else if (c.job == kJobDictW) fx_copy_kernel<kSrcDict><<<grid, kRleThreads, 0, st>>>(f);
+      else fx_copy_kernel<kSrcBss><<<grid, kRleThreads, 0, st>>>(f);
+      AG_TRY(check_launch("fx_copy_kernel"));
+      break;
+    }
+    default:
+      if (n_tiles == 0) break;
+      if (c.job == kJobBoolPlain) {
+        if (sp) fx_bool_kernel<false, true><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
+        else fx_bool_kernel<false, false><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
+      } else {
+        if (sp) fx_bool_kernel<true, true><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
+        else fx_bool_kernel<true, false><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
+      }
+      AG_TRY(check_launch("fx_bool_kernel"));
+      break;
+  }
+  std::vector<PageState> hs((size_t)n_pages);
+  int64_t bad = AG_NO_ERROR_POS;
+  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
+  if (dict) AG_TRY(d2h(&bad, a.bad, 8, st));
+  AG_TRY(sync(st));
+  if (h_decoded)
+    for (int64_t i = 0; i < n_pages; ++i) h_decoded[i] = hs[i].slots;
+  for (int64_t i = 0; i < n_pages; ++i)
+    if (hs[i].err != kErrNone) {
+      char msg[200];
+      fx_err_text(hs[i], c.pages[i], c.ptype, c.width, msg, sizeof msg);
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: %s (%lld values decoded)", fn, (long long)i, msg, (long long)hs[i].slots);
+    }
+  if (bad != AG_NO_ERROR_POS) AG_FAIL(AG_ERR_INVALID, "%s: invalid index values found for dictionary converter (output slot %lld)", fn, (long long)bad);
+  return AG_OK;
+}
+
+// host flavours: stage the page bytes, validity and dictionary.  Values: copy back only the slots each page wrote.
+// Booleans: the output bitmap's bytes up to the last page's last slot go up and come back whole, so every bit the
+// call does not write keeps its value.
+ag_status fx_pages_host(FxCall c, int64_t* decoded, int64_t* bad_pos) {
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  const char* fn = c.fn;
+  if (c.n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
+  if (c.n_pages == 0) return AG_OK;
+  if (!c.pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
+  const bool boolean = c.job == kJobBoolPlain || c.job == kJobBoolRle;
+  const bool dict = c.job == kJobDictT || c.job == kJobDictW;
+  int64_t data_end = 0, slot_end = 0;
+  for (int64_t i = 0; i < c.n_pages; ++i) {
+    const ag_pq_page& g = c.pages[i];
+    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field", fn, (long long)i);
+    data_end = std::max(data_end, g.data + g.len);
+    slot_end = std::max(slot_end, g.out + g.num_values);
+  }
+  if (data_end > 0 && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  if (slot_end > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  if (dict && c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const size_t vbytes = c.valid ? (size_t)((slot_end + 7) >> 3) : 0;
+  const size_t dbytes = dict ? (size_t)c.dict_len * c.width : 0;
+  const size_t obytes = boolean ? (size_t)((slot_end + 7) >> 3) : (size_t)slot_end * c.width;
+  const size_t o_valid = ((size_t)data_end + 255) & ~(size_t)255;
+  const size_t o_dict = (o_valid + vbytes + 255) & ~(size_t)255;
+  const size_t o_out = (o_dict + dbytes + 255) & ~(size_t)255;
+  const size_t o_bad = (o_out + obytes + 255) & ~(size_t)255;
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, o_bad + 8));
+  AG_TRY(h2d(d, c.data, (size_t)data_end, cs));
+  AG_TRY(h2d(d + o_valid, c.valid, vbytes, cs));
+  AG_TRY(h2d(d + o_dict, c.dict, dbytes, cs));
+  // *bad_pos is copied back whatever happens: it reads AG_NO_ERROR_POS when the call fails before any kernel runs
+  static const int64_t kNone = AG_NO_ERROR_POS;
+  AG_TRY(h2d(d + o_bad, &kNone, 8, cs));
+  if (boolean) AG_TRY(h2d(d + o_out, c.out, obytes, cs));
+  FxCall dc = c;
+  dc.data = d;
+  dc.valid = vbytes ? d + o_valid : nullptr;
+  dc.dict = dbytes ? d + o_dict : nullptr;
+  dc.out = d + o_out;
+  std::vector<int64_t> dec((size_t)c.n_pages, 0);   // stays 0 when the call fails before decoding
+  const ag_status rc = fx_pages_dev(dc, nullptr, dec.data(), reinterpret_cast<int64_t*>(d + o_bad), cs);
+  // a decode error still delivers the values decoded before it
+  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
+  if (decoded) memcpy(decoded, dec.data(), (size_t)c.n_pages * 8);
+  if (boolean) {
+    AG_TRY(d2h(c.out, d + o_out, obytes, cs));
+  } else {
+    for (int64_t i = 0; i < c.n_pages; ++i) {
+      const size_t off = (size_t)c.pages[i].out * c.width;
+      AG_TRY(d2h((uint8_t*)c.out + off, d + o_out + off, (size_t)dec[i] * c.width, cs));
+    }
+  }
+  if (dict && bad_pos) AG_TRY(d2h(bad_pos, d + o_bad, 8, cs));
+  const ag_status rs = sync(cs);
+  return rc != AG_OK ? rc : rs;
+}
+
+ag_status fixed_args(int ptype, int type_length, int encoding, int64_t dict_len, FxCall* c) {
+  const char* fn = "fixed_decode";
+  int w;
+  switch (ptype) {
+    case AG_PQ_TYPE_INT32: case AG_PQ_TYPE_FLOAT: w = 4; break;
+    case AG_PQ_TYPE_INT64: case AG_PQ_TYPE_DOUBLE: w = 8; break;
+    case AG_PQ_TYPE_INT96: w = 12; break;
+    case AG_PQ_TYPE_FIXED_LEN_BYTE_ARRAY:
+      if (type_length < 1) AG_FAIL(AG_ERR_INVALID, "%s: FIXED_LEN_BYTE_ARRAY type_length must be >= 1, got %d", fn, type_length);
+      w = type_length;
+      break;
+    default: AG_FAIL(AG_ERR_INVALID, "%s: physical type %d is not INT32, INT64, INT96, FLOAT, DOUBLE or FIXED_LEN_BYTE_ARRAY", fn, ptype);
+  }
+  const bool wide = w == 4 || w == 8;
+  int job;
+  if (encoding == AG_PQ_ENC_PLAIN) job = wide ? kJobPlainT : kJobPlainW;
+  else if (encoding == AG_PQ_ENC_PLAIN_DICTIONARY || encoding == AG_PQ_ENC_RLE_DICTIONARY) job = wide ? kJobDictT : kJobDictW;
+  else if (encoding == AG_PQ_ENC_BYTE_STREAM_SPLIT && ptype != AG_PQ_TYPE_INT96) job = wide ? kJobBssT : kJobBss;
+  else AG_FAIL(AG_ERR_INVALID, "%s: encoding %d is not accepted for physical type %d", fn, encoding, ptype);
+  if ((job == kJobDictT || job == kJobDictW) && dict_len < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative dictionary length", fn);
+  *c = FxCall{};
+  c->fn = fn; c->job = job; c->ptype = ptype; c->width = w; c->dict_len = dict_len;
+  return AG_OK;
+}
+
+ag_status bool_args(int encoding, FxCall* c) {
+  if (encoding != AG_PQ_ENC_PLAIN && encoding != AG_PQ_ENC_RLE)
+    AG_FAIL(AG_ERR_INVALID, "bool_decode: encoding %d is not accepted for BOOLEAN (PLAIN or RLE)", encoding);
+  *c = FxCall{};
+  c->fn = "bool_decode"; c->job = encoding == AG_PQ_ENC_PLAIN ? kJobBoolPlain : kJobBoolRle; c->width = 1;
+  return AG_OK;
+}
+
+}  // namespace
+
+}  // namespace ag
+
+using namespace ag;
+
+extern "C" {
+
+ag_status ag_parquet_bool_decode_dev(int encoding, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* d_valid,
+                                     uint8_t* d_out_bits, int64_t* d_decoded, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  FxCall c;
+  AG_TRY(bool_args(encoding, &c));
+  c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.out = d_out_bits;
+  return fx_pages_dev(c, d_decoded, nullptr, nullptr, resolve_stream(s));
+}
+
+ag_status ag_parquet_bool_decode(int encoding, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* valid,
+                                 uint8_t* out_bits, int64_t* decoded) {
+  AG_TRY(ensure_init());
+  FxCall c;
+  AG_TRY(bool_args(encoding, &c));
+  c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.out = out_bits;
+  return fx_pages_host(c, decoded, nullptr);
+}
+
+ag_status ag_parquet_fixed_decode_dev(int physical_type, int type_length, int encoding, const uint8_t* d_data, const ag_pq_page* pages,
+                                      int64_t n_pages, const uint8_t* d_valid, const void* d_dict, int64_t dict_len, void* d_out,
+                                      int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  FxCall c;
+  AG_TRY(fixed_args(physical_type, type_length, encoding, dict_len, &c));
+  c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.dict = d_dict; c.out = d_out;
+  return fx_pages_dev(c, d_decoded, nullptr, d_bad_pos, resolve_stream(s));
+}
+
+ag_status ag_parquet_fixed_decode(int physical_type, int type_length, int encoding, const uint8_t* data, const ag_pq_page* pages,
+                                  int64_t n_pages, const uint8_t* valid, const void* dict, int64_t dict_len, void* out, int64_t* decoded,
+                                  int64_t* bad_pos) {
+  AG_TRY(ensure_init());
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  FxCall c;
+  AG_TRY(fixed_args(physical_type, type_length, encoding, dict_len, &c));
+  c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.dict = dict; c.out = out;
+  return fx_pages_host(c, decoded, bad_pos);
+}
+
+}  // extern "C"

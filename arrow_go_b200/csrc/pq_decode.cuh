@@ -18,8 +18,13 @@ constexpr int kWinBytes = kWinVec * 16;
 constexpr uint32_t kLiteralFlag = 0x80000000u;
 
 // kIndex: dictionary indices themselves (int32; an index >= dict_len becomes -1 and lowers *bad), for dictionaries the
-// expansion cannot gather from, such as byte arrays
-enum PqKind { kLevels = 0, kDict = 1, kPlain = 2, kDelta = 3, kIndex = 4 };
+// expansion cannot gather from, such as byte arrays.  fixed.cu adds an expansion kind and three pass-1 kinds:
+//   kRank      (expansion only) the dense rank of every valid slot (int32), for values of any width gathered later
+//   kBss       pass 1: BYTE_STREAM_SPLIT page geometry, stride = len / width, checked as SetData does; expansion (4- and
+//              8-byte values): each slot's value assembled in a register from its byte in every stream
+//   kBoolPlain (pass 1 only) bit-packed PLAIN booleans: need <= 8 * len
+//   kBoolRle   (pass 1 only) RLE booleans: a 4-byte length prefix on every page, then runs of bit width 1
+enum PqKind { kLevels = 0, kDict = 1, kPlain = 2, kDelta = 3, kIndex = 4, kRank = 5, kBss = 6, kBoolPlain = 7, kBoolRle = 8 };
 
 // per-page error codes (reported through the status and message of the call)
 enum PqErr : int {
@@ -32,7 +37,18 @@ enum PqErr : int {
   kErrLevelsShort = 6,     // v1 level page shorter than its 4-byte length
   kErrLevelsLength = 7,    // v1 level length negative or past the page
   kErrPlainShort = 8,      // PLAIN page holds fewer values than its valid slots
+  // fixed.cu's kinds; each but kErrBoolEof delivers nothing of the page
+  kErrBssSize = 9,         // BYTE_STREAM_SPLIT: more bytes than num_values values
+  kErrBssAlign = 10,       // BYTE_STREAM_SPLIT: bytes not a multiple of the width
+  kErrBssEof = 11,         // BYTE_STREAM_SPLIT: the values to read take more than 2^31-1 bytes
+  kErrBssShort = 12,       // BYTE_STREAM_SPLIT spaced: fewer values than valid slots
+  kErrBoolShort = 13,      // PLAIN booleans: fewer bits than values
+  kErrBoolLength = 14,     // RLE booleans: page shorter than its 4-byte length
+  kErrBoolBytes = 15,      // RLE booleans: length past the page (PageState.pad holds it)
+  kErrBoolEof = 16,        // RLE booleans: the stream ends before the values the page needs
 };
+
+__host__ __device__ __forceinline__ bool err_delivers_nothing(int e) { return e == kErrPlainShort || (e >= kErrBssSize && e <= kErrBoolBytes); }
 
 struct PageState {          // written by pq_runs_kernel, read by pq_expand_kernel and the host
   int64_t stream;           // absolute byte offset of the hybrid stream / PLAIN values in d_data
@@ -169,6 +185,7 @@ pq_runs_kernel(PqArgs a) {
   __shared__ int64_t s_pos, s_produced;
   __shared__ int s_done, s_nruns, s_err, s_bw;
   __shared__ int64_t s_stream, s_len;
+  __shared__ uint32_t s_arg;
   const int64_t p = blockIdx.x;
   const ag_pq_page pg = a.plan.pages[p];
   const int tid = threadIdx.x;
@@ -186,6 +203,7 @@ pq_runs_kernel(PqArgs a) {
   if (tid == 0) {
     int err = kErrNone, bw = a.fixed_bw;
     int64_t stream = pg.data, len = pg.len;
+    s_arg = 0;
     if (a.kind == kLevels && a.v1) {
       if (len < 4) {
         err = kErrLevelsShort; len = 0;
@@ -203,14 +221,35 @@ pq_runs_kernel(PqArgs a) {
         stream += 1; len -= 1;
         if (bw > 32) { err = kErrBitWidth; len = 0; }
       }
+    } else if (a.kind == kBoolRle) {                     // RleBooleanDecoder.SetData (boolean_decoder.go:321-341)
+      if (len < 4) {
+        err = kErrBoolLength;
+      } else {
+        const uint8_t* b = a.data + pg.data;
+        const uint32_t nb = (uint32_t)b[0] | ((uint32_t)b[1] << 8) | ((uint32_t)b[2] << 16) | ((uint32_t)b[3] << 24);
+        if ((int64_t)nb > len - 4) { err = kErrBoolBytes; s_arg = nb; }
+        else { stream += 4; len = nb; }
+      }
     }
-    s_stream = stream; s_len = len; s_bw = bw; s_err = err;
+    const bool one_pass = a.kind == kPlain || a.kind == kBss || a.kind == kBoolPlain;
+    s_stream = stream; s_len = err ? 0 : len; s_bw = bw; s_err = err;
     s_pos = 0; s_produced = 0; s_nruns = 0;
-    s_done = (err != kErrNone || a.kind == kPlain) ? 1 : 0;
+    s_done = (err != kErrNone || one_pass) ? 1 : 0;
     if (a.kind == kPlain) {
       const int64_t have = len / a.width;
       if (need > have) { s_err = kErrPlainShort; s_produced = 0; }
       else s_produced = need;
+    } else if (a.kind == kBoolPlain) {
+      if (need > len * 8) s_err = kErrBoolShort;           // ensureBitsAvailable (boolean_decoder.go:57-63)
+      else s_produced = need;
+    } else if (a.kind == kBss) {                         // validateByteStreamSplitPageData, Decode, DecodeSpaced
+      const int64_t w = a.width;
+      const int64_t to_read = need < len / w ? need : len / w;
+      if (pg.num_values * w < len) s_err = kErrBssSize;
+      else if (len % w) s_err = kErrBssAlign;
+      else if (to_read * w > 0x7fffffffLL) s_err = kErrBssEof;
+      else if (a.valid && to_read < need) s_err = kErrBssShort;
+      else s_produced = to_read;                         // dense: min(num_values, stride)
     }
   }
   __syncthreads();
@@ -305,8 +344,10 @@ pq_runs_kernel(PqArgs a) {
   if (tid == 0) {
     cover(s_nruns > 0 ? s_nruns - 1 : 0, INT64_MAX);         // tiles past the last decoded value
     const int64_t produced = s_produced;
+    // RleBooleanDecoder.DecodeToBitmap: a short stream is io.ErrUnexpectedEOF after the values delivered
+    if (a.kind == kBoolRle && s_err == kErrNone && produced < need) s_err = kErrBoolEof;
     int64_t slots = produced;
-    if (s_err == kErrPlainShort) {
+    if (err_delivers_nothing(s_err)) {
       slots = 0;                                               // DecodeSpaced delivers nothing then
     } else if (a.valid) {
       slots = produced < need ? slot_of_rank(a.valid, pg.out, a.tile_cnt, a.plan.tile_base[p], a.plan.tile_base[p + 1], produced)
@@ -314,7 +355,7 @@ pq_runs_kernel(PqArgs a) {
     }
     PageState ps;
     ps.stream = stream; ps.stream_len = len; ps.need = need; ps.produced = produced; ps.slots = slots;
-    ps.nruns = s_nruns; ps.bw = bw; ps.err = s_err; ps.pad = 0;
+    ps.nruns = s_nruns; ps.bw = bw; ps.err = s_err; ps.pad = (int32_t)s_arg;
     a.st[p] = ps;
     if (a.d_decoded) a.d_decoded[p] = slots;
   }
@@ -356,7 +397,7 @@ pq_expand_kernel(PqArgs a) {
   const int64_t limit = ps.slots;
   if (s0 >= limit) return;                                      // block-uniform
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const uint2* runs = a.runs + (KIND == kPlain ? 0 : a.plan.run_base[p]);
+  const uint2* runs = a.runs + (KIND == kPlain || KIND == kRank || KIND == kBss ? 0 : a.plan.run_base[p]);
   const uint8_t* stream = a.data + ps.stream;
   T* out = reinterpret_cast<T*>(a.out) + pg.out;
 
@@ -390,6 +431,17 @@ pq_expand_kernel(PqArgs a) {
     uint32_t idx;
     if (KIND == kPlain) {
       out[s] = load_unaligned<T>(stream + rank * (int64_t)sizeof(T));
+      continue;
+    } else if (KIND == kRank) {
+      out[s] = (T)rank;
+      continue;
+    } else if (KIND == kBss) {
+      // byte j of rank r is stream[j * stride + r]: consecutive lanes read consecutive bytes of each stream
+      const int64_t stride = ps.stream_len / (int64_t)sizeof(T);
+      T v = 0;
+#pragma unroll
+      for (int j = 0; j < (int)sizeof(T); ++j) v |= (T)__ldg(stream + j * stride + rank) << (8 * j);
+      out[s] = v;
       continue;
     } else {
       int64_t lo = rlo, hi = rhi;

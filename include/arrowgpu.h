@@ -733,6 +733,81 @@ ag_status ag_parquet_byte_array_decode_dev(int encoding, int offset_width, const
                                            int64_t* total, int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s);
 
 /* ================================================================================= *
+ * BOOLEAN, INT32 / INT64 / FLOAT / DOUBLE, INT96 and FIXED_LEN_BYTE_ARRAY pages — the same batch-of-pages contract as
+ *   ag_parquet_dict_decode: a host page table, pages in any order, valid == NULL for dense output, pg.out is both the
+ *   slot and the bit offset in `valid`, decoded[i] counts page i's slots, and the device flavour synchronises `s`
+ *   once.  Each error is AG_ERR_INVALID "<fn>: page %lld: <message> (%lld values decoded)" naming the lowest failing
+ *   page; every other page is decoded in full.  A spaced page with fewer values than valid slots cannot occur for
+ *   BOOLEAN, whose value count is the page's slot count.
+ *
+ *   ag_parquet_bool_decode: PlainBooleanDecoder / RleBooleanDecoder .DecodeToBitmap and decodeSpacedToBitmap
+ *   (parquet/internal/encoding/boolean_decoder.go:264-304,321-341,382-417), as record_reader.go:331-370 calls them:
+ *   an Arrow boolean bitmap.  encoding AG_PQ_ENC_PLAIN or AG_PQ_ENC_RLE.  pg.out is the page's first bit in `valid`
+ *   and in `out_bits`; a null slot gets 0.  Bits outside [pg.out, pg.out + decoded[i]) of every page are left
+ *   untouched, also where two pages share a byte or a 32-bit word of out_bits.  Pages sharing a byte are decoded at
+ *   the same time, so the device flavour merges a partly written word with 32-bit atomics on the aligned word: d_out_bits
+ *   must be readable and writable through every aligned 4-byte word that holds a bit of a page (a cudaMalloc buffer
+ *   rounded up to a multiple of 4 bytes is); the bytes of those words outside the pages keep their values.  The host
+ *   flavour stages the bitmap, so out_bits needs only its own bytes.
+ *     AG_PQ_ENC_PLAIN: bit-packed, LSB first.  "parquet: boolean data has %d bits available, need %d: unexpected EOF"
+ *       when the page holds fewer bits than the values it needs (valid slots); nothing of the page is delivered.
+ *     AG_PQ_ENC_RLE: a 4-byte little-endian length on every page (v1 and v2), then an RLE / bit-packed stream of bit
+ *       width 1.  "invalid length - %d (corrupt data page?)" (page shorter than 4 bytes) and "received invalid number
+ *       of bytes - %d (corrupt data page?)" (length past the page) deliver nothing.  A stream that ends before the
+ *       values the page needs is "unexpected EOF" after the values delivered (DecodeToBitmap's io.ErrUnexpectedEOF;
+ *       unlike a level stream's short count).  Bad run headers are the run-walk messages of ag_parquet_dict_decode.
+ *
+ *   ag_parquet_fixed_decode: values of width 4 (INT32, FLOAT), 8 (INT64, DOUBLE), 12 (INT96) or type_length
+ *   (FIXED_LEN_BYTE_ARRAY; type_length is ignored for the other types) bytes per slot in `out`; a null slot gets zero
+ *   bytes (record_reader.go:847-871 AppendNull).  Accepted encodings (typed_encoder.go:250-291,432-437,714-727):
+ *   INT32 / INT64 / FLOAT / DOUBLE and FIXED_LEN_BYTE_ARRAY: PLAIN, PLAIN_DICTIONARY / RLE_DICTIONARY and
+ *   BYTE_STREAM_SPLIT; INT96: PLAIN and dictionary.  Any other type, encoding or a type_length < 1 is AG_ERR_INVALID
+ *   before any launch.  For widths 4 and 8, `out` and `dict` are aligned to the width; other widths have no alignment
+ *   requirement.
+ *     AG_PQ_ENC_PLAIN (plain_encoding_types.go:61-110, fixed_len_byte_array_decoder.go): dense or spaced, so one call
+ *       replaces one copy per page.  A page with fewer values than it needs delivers nothing: widths 4 / 8 "parquet:
+ *       eof exception decode plain (fewer values than valid slots)" (ag_parquet_plain_decode_spaced's message), INT96
+ *       "parquet: eof exception decode plain INT96, nvals: %d, nbytes: %d, datalen: %d", FIXED_LEN_BYTE_ARRAY
+ *       "parquet: eof exception".
+ *     AG_PQ_ENC_PLAIN_DICTIONARY / AG_PQ_ENC_RLE_DICTIONARY: `dict` holds dict_len values of the width, which this call
+ *       produces from the dictionary page with AG_PQ_ENC_PLAIN, dense (so its length is checked too).  Runs, bit
+ *       widths, their messages and an out-of-range index (message, *bad_pos, a zeroed slot) are those of
+ *       ag_parquet_dict_decode.
+ *     AG_PQ_ENC_BYTE_STREAM_SPLIT (byte_stream_split.go:98-250, fixed_len_byte_array_decoder.go): byte j of the value
+ *       of dense rank r is data[j * stride + r], stride = len / width.  "data size (%d) is too small for the number of
+ *       values in in BYTE_STREAM_SPLIT (%d)" when the page holds more than num_values values (the reference's wording);
+ *       "ByteStreamSplit data size %d not aligned with byte_width: %d" (FIXED_LEN_BYTE_ARRAY: "... not aligned with type
+ *       FIXED_LEN_BYTE_ARRAY and byte_width: %d"); "parquet: eof exception" when the values to read take more than
+ *       2^31-1 bytes; spaced, fewer values than valid slots: "parquet: number of values / definitions levels read did
+ *       not match".  Each delivers nothing.  Dense, a page with fewer values than slots delivers stride slots.
+ *   Differences from the reference (DESIGN §2): a boolean null slot is 0 (decodeSpacedToBitmap can leave packed bits
+ *   there); an RLE boolean repeated byte other than 0 or 1 is true (value != 0, rle.go:161-165 does not mask it); a
+ *   BYTE_STREAM_SPLIT page's value count is its stride, len / width (SetData replaces nvals with it).
+ *   Device flavours: d_decoded (may be NULL) is device memory; *d_bad_pos (may be NULL) is overwritten
+ *   (AG_NO_ERROR_POS when every index is in range).  Host flavours: decoded and bad_pos (may be NULL) are host
+ *   memory; they stage `data`, `valid`, the dictionary and (booleans) the output bitmap's bytes up to the last page's
+ *   last slot, and copy back only what the call wrote, so the rest of `out` / `out_bits` is untouched.
+ * ================================================================================= */
+#define AG_PQ_ENC_RLE                     3
+#define AG_PQ_ENC_BYTE_STREAM_SPLIT       9
+#define AG_PQ_TYPE_INT32                  1
+#define AG_PQ_TYPE_INT64                  2
+#define AG_PQ_TYPE_INT96                  3
+#define AG_PQ_TYPE_FLOAT                  4
+#define AG_PQ_TYPE_DOUBLE                 5
+#define AG_PQ_TYPE_FIXED_LEN_BYTE_ARRAY   7
+ag_status ag_parquet_bool_decode(int encoding, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* valid,
+                                 uint8_t* out_bits, int64_t* decoded);
+ag_status ag_parquet_bool_decode_dev(int encoding, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* d_valid,
+                                     uint8_t* d_out_bits, int64_t* d_decoded, ag_stream_t s);
+ag_status ag_parquet_fixed_decode(int physical_type, int type_length, int encoding, const uint8_t* data, const ag_pq_page* pages,
+                                  int64_t n_pages, const uint8_t* valid, const void* dict, int64_t dict_len, void* out, int64_t* decoded,
+                                  int64_t* bad_pos);
+ag_status ag_parquet_fixed_decode_dev(int physical_type, int type_length, int encoding, const uint8_t* d_data, const ag_pq_page* pages,
+                                      int64_t n_pages, const uint8_t* d_valid, const void* d_dict, int64_t dict_len, void* d_out,
+                                      int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s);
+
+/* ================================================================================= *
  * SNAPPY page decompression — a batch of pages in one call, so that a reader uploads a column chunk as it sits in the
  *   file and decodes it in device memory.  The output is what the page decoders above take (`ag_pq_page` offsets then
  *   point into `dst`).  serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> compress.Decode

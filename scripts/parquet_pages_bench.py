@@ -12,6 +12,9 @@ every page writes its own output range.  Writes nothing to disk.
 --bytearray runs only the BYTE_ARRAY cases (ag_parquet_byte_array_decode_dev, csrc/byte_array.cu): time, share of the HBM
 peak, and a torch.profiler split of the device time over the three stages (values, offsets, bytes).
 
+--fixed runs only the BOOLEAN and fixed-width cases (ag_parquet_bool_decode_dev / ag_parquet_fixed_decode_dev,
+csrc/fixed.cu): time, share of the HBM peak and a torch.profiler split per kernel.
+
 --profile runs only the DELTA_BINARY_PACKED, SNAPPY and ZSTD cases, under torch.profiler, and reports the device time
 per call of each kernel (the delta block walk against the value passes, the Snappy parse against the execute, the ZSTD
 walk / literals / sequences / resolve / execute / checksum kernels) instead.
@@ -77,6 +80,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--bytearray", action="store_true")
+    ap.add_argument("--fixed", action="store_true")
     args = ap.parse_args()
 
     from arrow_go_b200 import _native as N
@@ -126,6 +130,11 @@ def main():
         res.update(bytearray_cases(args, N, np.random.default_rng(0xB17E), timed, upload, DeviceBuffer))
         print(json.dumps(res), flush=True)
         return
+    if args.fixed:
+        res = {"peak_gbs": peak, "peak_kind": peak_kind, **card(), "timing": res["timing"]}
+        res.update(fixed_cases(args, N, np.random.default_rng(0xF1ED), timed, upload, DeviceBuffer, peak, n_pages, per_page))
+        print(json.dumps(res), flush=True)
+        return
     dout = DeviceBuffer(8 * n + 64)
     if args.profile:
         res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer, profile=True))
@@ -172,7 +181,7 @@ def kernel_ms(prof, steps):
     kern = {}
     for ev in prof.key_averages():
         if ev.device_type == torch.autograd.DeviceType.CUDA:
-            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|ba_\w+_kernel)(<[^>]*>)?", ev.key)
+            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|ba_\w+_kernel|fx_\w+_kernel)(<[^>]*>)?", ev.key)
             short = (m.group(1) + (m.group(2) or "")) if m else ev.key.strip()
             us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
             kern[short] = kern.get(short, 0.0) + us / 1e3 / steps
@@ -499,6 +508,88 @@ def bytearray_cases(args, N, rng, timed, upload, DeviceBuffer, values=20_000_000
     run("bytearray_delta_sorted_keys", B.DELTA_BYTE_ARRAY, dblob, pages, enc, n_pages, per, data,
         f"DELTA_BYTE_ARRAY pages of {per} sorted 13-byte keys (~{len(dba[0]) >> 10} KiB; prefix ~7 bytes)")
     dblob.free()
+    return out
+
+
+def fixed_cases(args, N, rng, timed, upload, DeviceBuffer, peak, n_pages, per):
+    """BOOLEAN and fixed-width pages (ag_parquet_fixed_decode_dev / ag_parquet_bool_decode_dev), n_pages pages of `per`
+    values.  Algorithmic bytes: encoded bytes read + output written (+ 1/8 B per slot of validity when spaced, + the
+    dictionary for (d)).  Four distinct page bodies are reused round-robin; every page writes its own slots."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile as tprofile
+    out = {}
+    n = n_pages * per
+    valid = rng.random(n) >= 0.1
+    dvalid = upload(np.packbits(valid, bitorder="little"))
+    dec = DeviceBuffer(8 * n_pages + 64)
+
+    def pages_of(bodies):
+        blob = b"".join(bodies) + bytes(16)
+        offs = np.cumsum([0] + [len(x) for x in bodies])
+        pages = [(int(offs[p % 4]), len(bodies[p % 4]), per, p * per) for p in range(n_pages)]
+        return upload(np.frombuffer(blob, np.uint8)), N.page_table(pages), sum(len(bodies[p % 4]) for p in range(n_pages))
+
+    def run(name, fn, ab, note):
+        fn()
+        N.call("ag_stream_sync", None)
+        ms = timed(fn)
+        with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                fn()
+            torch.cuda.synchronize()
+        out[name] = {"ms": ms, "values": n, "pages": n_pages, "values_per_page": per, "algorithmic_bytes": ab, "gbs": ab / ms / 1e6,
+                     "frac": ab / ms / 1e6 / peak, "kernels_ms_per_call": kernel_ms(prof, args.steps), "note": note}
+
+    # (a) DOUBLE BYTE_STREAM_SPLIT, dense and 10 % nulls
+    bodies = [np.ascontiguousarray(rng.standard_normal(per).view(np.uint8).reshape(per, 8).T).tobytes() for _ in range(4)]
+    dblob, tbl, enc = pages_of(bodies)
+    dout = DeviceBuffer(8 * n + 64)
+    for label, vp, vb in (("required", None, 0.0), ("10pct_nulls", dvalid.ptr, n / 8)):
+        run(f"fixed_bss_double_{label}", lambda: N.call("ag_parquet_fixed_decode_dev", N.PQ_TYPE_DOUBLE, 0, N.PQ_ENC_BYTE_STREAM_SPLIT, dblob.ptr, tbl,
+                                                       n_pages, vp, None, 0, dout.ptr, dec.ptr, None, None),
+            enc + 8.0 * n + vb, "DOUBLE BYTE_STREAM_SPLIT pages of 2^19 values (4 MiB)")
+    dblob.free(); dout.free()
+    # (b) FLBA(16) BYTE_STREAM_SPLIT
+    bodies = [np.ascontiguousarray(rng.integers(0, 256, (per, 16), dtype=np.uint8).T).tobytes() for _ in range(4)]
+    dblob, tbl, enc = pages_of(bodies)
+    dout = DeviceBuffer(16 * n + 64)
+    run("fixed_bss_flba16", lambda: N.call("ag_parquet_fixed_decode_dev", N.PQ_TYPE_FIXED_LEN_BYTE_ARRAY, 16, N.PQ_ENC_BYTE_STREAM_SPLIT, dblob.ptr,
+                                           tbl, n_pages, None, None, 0, dout.ptr, dec.ptr, None, None),
+        enc + 16.0 * n, "FIXED_LEN_BYTE_ARRAY(16) BYTE_STREAM_SPLIT pages, dense")
+    dblob.free()
+    # (c) FLBA(16) dictionary, 64K entries, 16-bit indices in literal runs
+    ddict = upload(rng.integers(0, 256, (1 << 16, 16), dtype=np.uint8))
+    bodies = [bytes([16]) + rle_literal_page(rng.integers(0, 1 << 16, per), 16) for _ in range(4)]
+    dblob, tbl, enc = pages_of(bodies)
+    bad = DeviceBuffer(64)
+    run("fixed_dict_flba16", lambda: N.call("ag_parquet_fixed_decode_dev", N.PQ_TYPE_FIXED_LEN_BYTE_ARRAY, 16, N.PQ_ENC_RLE_DICTIONARY, dblob.ptr,
+                                            tbl, n_pages, None, ddict.ptr, 1 << 16, dout.ptr, dec.ptr, bad.ptr, None),
+        enc + 16.0 * n, "FIXED_LEN_BYTE_ARRAY(16), 64K-entry dictionary (1 MiB, L2-resident), 16-bit indices in literal runs, dense")
+    dblob.free(); ddict.free(); bad.free(); dout.free()
+    # (d) INT96 PLAIN spaced, 10 % nulls
+    bodies = [rng.integers(0, 256, 12 * per, dtype=np.uint8).tobytes() for _ in range(4)]
+    dblob, tbl, enc = pages_of(bodies)
+    dout = DeviceBuffer(12 * n + 64)
+    run("fixed_plain_int96_10pct_nulls", lambda: N.call("ag_parquet_fixed_decode_dev", N.PQ_TYPE_INT96, 0, N.PQ_ENC_PLAIN, dblob.ptr, tbl, n_pages,
+                                                        dvalid.ptr, None, 0, dout.ptr, dec.ptr, None, None),
+        12.0 * valid.sum() + 12.0 * n + n / 8, "INT96 PLAIN pages of 2^19 values, 10 % nulls (the valid slots' values are read)")
+    dblob.free(); dout.free()
+    # (e) BOOLEAN PLAIN dense and spaced, (f) BOOLEAN RLE of random bits
+    dout = DeviceBuffer(n // 8 + 64)
+    bodies = [np.packbits(rng.random(per) < 0.5, bitorder="little").tobytes() for _ in range(4)]
+    dblob, tbl, enc = pages_of(bodies)
+    for label, vp, vb in (("required", None, 0.0), ("10pct_nulls", dvalid.ptr, n / 8)):
+        run(f"bool_plain_{label}", lambda: N.call("ag_parquet_bool_decode_dev", N.PQ_ENC_PLAIN, dblob.ptr, tbl, n_pages, vp, dout.ptr, dec.ptr, None),
+            enc + n / 8 + vb, "BOOLEAN PLAIN pages of 2^19 bits")
+    dblob.free()
+    bodies = []
+    for _ in range(4):
+        s = rle_literal_page((rng.random(per) < 0.5).astype(np.int64), 1)
+        bodies.append(len(s).to_bytes(4, "little") + s)
+    dblob, tbl, enc = pages_of(bodies)
+    run("bool_rle_random", lambda: N.call("ag_parquet_bool_decode_dev", N.PQ_ENC_RLE, dblob.ptr, tbl, n_pages, None, dout.ptr, dec.ptr, None),
+        enc + n / 8, "BOOLEAN RLE pages of 2^19 random bits (literal runs of 504), dense")
+    dblob.free(); dout.free(); dvalid.free(); dec.free()
     return out
 
 

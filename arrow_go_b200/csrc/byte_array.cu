@@ -719,8 +719,6 @@ void ba_err_text(const BaPage& s, const DeltaPage& dp, const DeltaPage& dl, char
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 }  // namespace
 
 // The device flavour's work.  out_at_base = out_data + offset_base (may be NULL when cap_rel == 0).  *h_total and
@@ -744,34 +742,26 @@ static ag_status byte_array_dev(int enc, int ow, const uint8_t* data, const ag_p
   if (dict && dict_len < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative dictionary length", fn);
   if (dict && !doff) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary offsets", fn);
   if (dict && (reinterpret_cast<uintptr_t>(doff) & (ow - 1))) AG_FAIL(AG_ERR_INVALID, "%s: dictionary offsets not aligned to offset_width", fn);
-  // plan: pages | tile_base[n+1] | run_base[n+1] | delta pages (out = first dense index)
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_page);
-  const size_t plan_bytes = 2 * pb + 2 * (size_t)(n_pages + 1) * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  if (n_pages) memcpy(h.data(), pages, pb);
-  int64_t* tile_base = reinterpret_cast<int64_t*>(h.data() + pb);
-  int64_t* run_base = tile_base + n_pages + 1;
-  ag_pq_page* dpages = reinterpret_cast<ag_pq_page*>(run_base + n_pages + 1);
-  tile_base[0] = run_base[0] = 0;
-  bool any_data = false;
+  // plan: pages | run_base[n+1] | tile_base[n+1] | delta pages (out = first dense index)
+  PagePlan plan;
+  AG_TRY(plan_pages(fn, pages, n_pages, [&](const ag_pq_page& g) { return dict ? std::min(g.num_values, g.len) : (int64_t)0; }, &plan));
+  const size_t o_dpages = plan.bytes.size();
+  plan.bytes.resize(o_dpages + (size_t)n_pages * sizeof(ag_pq_page));
+  const int64_t* tile_base = plan.tile_base();
+  ag_pq_page* dpages = reinterpret_cast<ag_pq_page*>(plan.bytes.data() + o_dpages);
   std::vector<std::pair<int64_t, int64_t>> ranges;
   for (int64_t i = 0; i < n_pages; ++i) {
     const ag_pq_page& g = pages[i];
-    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field, more than 2^31-1 values or more than 2^32-1 bytes", fn, (long long)i);
     if (g.out + g.num_values > n_slots) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: slots past n_slots", fn, (long long)i);
     if (g.num_values) ranges.emplace_back(g.out, g.out + g.num_values);
-    any_data |= g.len > 0;
-    run_base[i + 1] = run_base[i] + (dict ? (g.num_values < g.len ? g.num_values : g.len) : 0);
-    tile_base[i + 1] = tile_base[i] + (g.num_values + kTile - 1) / kTile;
     dpages[i] = g;
     dpages[i].out = tile_base[i] * kTile;
   }
   std::sort(ranges.begin(), ranges.end());
   for (size_t i = 1; i < ranges.size(); ++i)
     if (ranges[i].first < ranges[i - 1].second) AG_FAIL(AG_ERR_INVALID, "%s: page slot ranges overlap", fn);
-  if (any_data && !data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
-  const int64_t n_tiles = tile_base[n_pages], n_runs = run_base[n_pages], n_dense = n_tiles * kTile;
+  if (plan.any_data && !data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  const int64_t n_tiles = plan.n_tiles, n_runs = plan.n_desc, n_dense = n_tiles * kTile;
   const int64_t n_chunks = (n_slots + kTile - 1) / kTile;
 
   // psv levels: 32^(l+1) values per entry, until one entry covers everything
@@ -780,47 +770,47 @@ static ag_status byte_array_dev(int enc, int ow, const uint8_t* data, const ag_p
   if (dba) for (int64_t m = n_dense / 32; nlev < kPsvLevels; m = (m + 31) / 32) { lev_n[nlev++] = m; if (m <= 1) break; }
 
   // scratch
-  size_t o = align256(plan_bytes);
-  auto take = [&](size_t bytes) { const size_t r = o; o = align256(o + bytes); return r; };
-  const size_t o_st = take((size_t)n_pages * sizeof(BaPage));
-  const size_t o_tc = take(valid ? (size_t)n_tiles * 8 : 0);
-  const size_t o_vlen = take(dict ? 0 : (size_t)n_dense * 8);
-  const size_t o_vsrc = take(dict ? 0 : (size_t)n_dense * 8);
-  const size_t o_slen = take((size_t)n_slots * 8);
-  const size_t o_ssrc = take((size_t)n_slots * 8);
-  const size_t o_soff = take((size_t)(n_slots + 1) * 8);
-  const size_t o_csum = take((size_t)n_chunks * 8);
-  const size_t o_ctl = take(sizeof(BaCtl));
-  const size_t o_bad = take(8);
+  Carve sc;
+  const size_t o_plan = sc.take(plan.bytes.size());
+  const size_t o_st = sc.take((size_t)n_pages * sizeof(BaPage));
+  const size_t o_tc = sc.take(valid ? (size_t)n_tiles * 8 : 0);
+  const size_t o_vlen = sc.take(dict ? 0 : (size_t)n_dense * 8);
+  const size_t o_vsrc = sc.take(dict ? 0 : (size_t)n_dense * 8);
+  const size_t o_slen = sc.take((size_t)n_slots * 8);
+  const size_t o_ssrc = sc.take((size_t)n_slots * 8);
+  const size_t o_soff = sc.take((size_t)(n_slots + 1) * 8);
+  const size_t o_csum = sc.take((size_t)n_chunks * 8);
+  const size_t o_ctl = sc.take(sizeof(BaCtl));
+  const size_t o_bad = sc.take(8);
   // dictionary
-  const size_t o_pqs = take(dict ? (size_t)n_pages * sizeof(PageState) : 0);
-  const size_t o_ti = take(dict ? (size_t)n_tiles * 8 : 0);
-  const size_t o_runs = take(dict ? (size_t)n_runs * 8 : 0);
-  const size_t o_idx = take(dict ? (size_t)n_slots * 4 : 0);
+  const size_t o_pqs = sc.take(dict ? (size_t)n_pages * sizeof(PageState) : 0);
+  const size_t o_ti = sc.take(dict ? (size_t)n_tiles * 8 : 0);
+  const size_t o_runs = sc.take(dict ? (size_t)n_runs * 8 : 0);
+  const size_t o_idx = sc.take(dict ? (size_t)n_slots * 4 : 0);
   // delta
-  const size_t o_dls = take(delta ? (size_t)n_pages * sizeof(DeltaPage) : 0);
-  const size_t o_dps = take(dba ? (size_t)n_pages * sizeof(DeltaPage) : 0);
-  const size_t o_mbl = take(delta ? (size_t)tile_base[n_pages] * (kTile / 32) * sizeof(DeltaMini) : 0);
-  const size_t o_mbp = take(dba ? (size_t)tile_base[n_pages] * (kTile / 32) * sizeof(DeltaMini) : 0);
-  const size_t o_mbb = take(delta ? (size_t)(n_pages + 1) * 8 : 0);
-  const size_t o_tsum = take(delta ? (size_t)n_tiles * 8 : 0);
-  const size_t o_suf = take(delta ? (size_t)n_dense * 4 : 0);
-  const size_t o_pre = take(dba ? (size_t)n_dense * 4 : 0);
-  const size_t o_skip = take(dba ? (size_t)n_pages * 8 : 0);
-  const size_t o_lt = take(delta ? (size_t)n_tiles * sizeof(LenTile) : 0);
-  const size_t o_tb = take(delta ? (size_t)n_tiles * 8 : 0);
-  const size_t o_psv = take(dba ? (size_t)n_dense * 8 : 0);
+  const size_t o_dls = sc.take(delta ? (size_t)n_pages * sizeof(DeltaPage) : 0);
+  const size_t o_dps = sc.take(dba ? (size_t)n_pages * sizeof(DeltaPage) : 0);
+  const size_t o_mbl = sc.take(delta ? (size_t)tile_base[n_pages] * (kTile / 32) * sizeof(DeltaMini) : 0);
+  const size_t o_mbp = sc.take(dba ? (size_t)tile_base[n_pages] * (kTile / 32) * sizeof(DeltaMini) : 0);
+  const size_t o_mbb = sc.take(delta ? (size_t)(n_pages + 1) * 8 : 0);
+  const size_t o_tsum = sc.take(delta ? (size_t)n_tiles * 8 : 0);
+  const size_t o_suf = sc.take(delta ? (size_t)n_dense * 4 : 0);
+  const size_t o_pre = sc.take(dba ? (size_t)n_dense * 4 : 0);
+  const size_t o_skip = sc.take(dba ? (size_t)n_pages * 8 : 0);
+  const size_t o_lt = sc.take(delta ? (size_t)n_tiles * sizeof(LenTile) : 0);
+  const size_t o_tb = sc.take(delta ? (size_t)n_tiles * 8 : 0);
+  const size_t o_psv = sc.take(dba ? (size_t)n_dense * 8 : 0);
   size_t o_lv[kPsvLevels];
-  for (int l = 0; l < nlev; ++l) o_lv[l] = take((size_t)lev_n[l] * 4 + 128);
-  const size_t total_bytes = o;
+  for (int l = 0; l < nlev; ++l) o_lv[l] = sc.take((size_t)lev_n[l] * 4 + 128);
 
   Temps t(st);
   uint8_t* d;
-  AG_TRY(t.alloc_t(&d, total_bytes));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  AG_TRY(t.alloc_t(&d, sc.size));
+  PqPlan pl;
+  AG_TRY(upload_plan(plan, d + o_plan, st, &pl));
   BaArgs a{};
-  a.pages = reinterpret_cast<const ag_pq_page*>(d);
-  a.tile_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.pages = pl.pages;
+  a.tile_base = pl.tile_base;
   a.n_pages = n_pages; a.n_tiles = n_tiles; a.n_slots = n_slots;
   a.data = data; a.valid = valid;
   a.tile_cnt = valid ? reinterpret_cast<int64_t*>(d + o_tc) : nullptr;
@@ -850,20 +840,13 @@ static ag_status byte_array_dev(int enc, int ow, const uint8_t* data, const ag_p
   if (n_slots) AG_CUDA_TRY(cudaMemsetAsync(a.slen, 0, (size_t)n_slots * 8, st));
 
   // ---- stage 1: values ----
-  if (valid && n_tiles) {
-    PqArgs c{};
-    c.plan.pages = a.pages; c.plan.tile_base = a.tile_base; c.plan.n_pages = n_pages; c.plan.n_tiles = n_tiles;
-    c.valid = valid; c.tile_cnt = a.tile_cnt;
-    pq_tile_count_kernel<<<grid_for(n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(c);
-    AG_TRY(check_launch("pq_tile_count_kernel"));
-  }
+  AG_TRY(launch_tile_counts(pl, valid, a.tile_cnt, st));
   if (n_pages && enc == AG_PQ_ENC_PLAIN) {
     ba_plain_parse_kernel<<<(unsigned)n_pages, kBaThreads, 0, st>>>(a);
     AG_TRY(check_launch("ba_plain_parse_kernel"));
   } else if (n_pages && dict) {
     PqArgs c{};
-    c.plan.pages = a.pages; c.plan.run_base = a.tile_base + n_pages + 1;
-    c.plan.tile_base = a.tile_base; c.plan.n_pages = n_pages; c.plan.n_tiles = n_tiles;
+    c.plan = pl;
     c.data = data; c.valid = valid;
     c.st = reinterpret_cast<PageState*>(d + o_pqs);
     c.runs = n_runs ? reinterpret_cast<uint2*>(d + o_runs) : nullptr;
@@ -884,7 +867,7 @@ static ag_status byte_array_dev(int enc, int ow, const uint8_t* data, const ag_p
     for (int64_t i = 0; i <= n_pages; ++i) hm[i] = tile_base[i] * (kTile / 32);
     AG_TRY(h2d(mbb, hm.data(), hm.size() * 8, st));
     DeltaArgs da{};
-    da.pages = reinterpret_cast<const ag_pq_page*>(d + pb + 2 * (size_t)(n_pages + 1) * 8);
+    da.pages = reinterpret_cast<const ag_pq_page*>(d + o_plan + o_dpages);
     da.mb_base = mbb; da.tile_base = a.tile_base; da.n_pages = n_pages; da.data = data; da.valid = nullptr;
     da.tile_sum = reinterpret_cast<unsigned long long*>(d + o_tsum);
     da.d_decoded = nullptr; da.width = 4;

@@ -1,6 +1,11 @@
-// fixed.cu — Parquet pages of the remaining flat physical types on the device: BOOLEAN (PLAIN bit-packed, RLE) into an
-// Arrow boolean bitmap, and INT32 / INT64 / FLOAT / DOUBLE / INT96 / FIXED_LEN_BYTE_ARRAY (PLAIN, dictionary,
-// BYTE_STREAM_SPLIT) into `width` bytes per slot.
+// fixed.cu — the fixed-width Parquet page driver: definition / repetition levels, dictionary-encoded and PLAIN spaced
+// 4- and 8-byte values, BOOLEAN (PLAIN bit-packed, RLE) into an Arrow boolean bitmap, and INT32 / INT64 / FLOAT /
+// DOUBLE / INT96 / FIXED_LEN_BYTE_ARRAY (PLAIN, dictionary, BYTE_STREAM_SPLIT) into `width` bytes per slot.
+//   RleDecoder.Next / GetBatch                                   parquet/internal/utils/rle.go:123-169,203-239
+//   LevelDecoder.SetData / SetDataV2 / Decode                    parquet/internal/encoding/levels.go:188-297
+//   dictDecoder.SetData / decode / decodeSpaced                  decoder.go:125-160 over
+//                                                                TypedRleDecoder.GetBatchWithDict[Spaced] (utils/typed_rle_dict.go:143-236)
+//   PlainDecoder.DecodeSpaced                                    plain_encoding_types.go:98 -> spacedExpand (decoder.go:209)
 //   PlainBooleanDecoder.DecodeToBitmap / decodeSpacedToBitmap   parquet/internal/encoding/boolean_decoder.go:264-304
 //   RleBooleanDecoder.SetData / DecodeToBitmap                   boolean_decoder.go:321-341,382-417
 //   PlainDecoder[T] (INT96 too)                                  plain_encoding_types.go:61-110
@@ -9,10 +14,11 @@
 //   accepted encodings per physical type                         typed_encoder.go:250-291,432-437,538-552,714-727
 //
 // Every call runs the passes of pq_decode.cuh first: pq_tile_count_kernel (spaced), then pq_runs_kernel, one block per
-// page, which scans the spaced rank bases, walks the runs of dictionary and RLE pages and checks the pages of the
-// pass-1 kinds this file adds (kBss, kBoolPlain, kBoolRle).  What runs after it:
-//   - PLAIN and dictionary pages of 4- and 8-byte values: pq_expand_kernel<kPlain / kDict>, the kernels
-//     ag_parquet_plain_decode_spaced and ag_parquet_dict_decode run.
+// page, which scans the spaced rank bases, walks the runs of level, dictionary and RLE pages and checks the pages of
+// the pass-1 kinds this file adds (kBss, kBoolPlain, kBoolRle).  What runs after it:
+//   - levels: pq_expand_kernel<kLevels> into int16.
+//   - PLAIN and dictionary pages of 4- and 8-byte values: pq_expand_kernel<kPlain / kDict>, for
+//     ag_parquet_plain_decode_spaced and ag_parquet_dict_decode as for the fixed_decode pages of those widths.
 //   - BYTE_STREAM_SPLIT pages of 4- and 8-byte values: pq_expand_kernel<kBss>, one thread per slot assembling its value
 //     in a register from one byte of each stream; consecutive threads read consecutive bytes of every stream and store
 //     consecutive values.
@@ -42,7 +48,7 @@ constexpr int kCopyChunk = 16384;   // output bytes per fx_copy_kernel block and
 enum FxSrc { kSrcPlain = 0, kSrcDict = 1, kSrcBss = 2 };
 
 // what runs after pass 1
-enum FxJob { kJobPlainT = 0, kJobDictT = 1, kJobPlainW = 2, kJobDictW = 3, kJobBss = 4, kJobBoolPlain = 5, kJobBoolRle = 6, kJobBssT = 7 };
+enum FxJob { kJobPlainT = 0, kJobDictT = 1, kJobPlainW = 2, kJobDictW = 3, kJobBss = 4, kJobBoolPlain = 5, kJobBoolRle = 6, kJobBssT = 7, kJobLevels = 8 };
 
 struct FxArgs {
   PqPlan plan;
@@ -204,6 +210,7 @@ int pass1_kind(int job) {
     case kJobDictW: return kIndex;
     case kJobBss: case kJobBssT: return kBss;
     case kJobBoolPlain: return kBoolPlain;
+    case kJobLevels: return kLevels;
     default: return kBoolRle;
   }
 }
@@ -238,110 +245,75 @@ void fx_err_text(const PageState& s, const ag_pq_page& pg, int ptype, int width,
   }
 }
 
-struct FxCall {
-  const char* fn;
-  int job;
-  int ptype;                // AG_PQ_TYPE_* (booleans: 0), for the error texts
-  int width;                // bytes per value (booleans: 1)
-  const uint8_t* data;
-  const ag_pq_page* pages;
-  int64_t n_pages;
-  const uint8_t* valid;
-  const void* dict;
-  int64_t dict_len;
-  void* out;
-};
+// pq_expand_kernel<K> over the call's 4- or 8-byte values
+template <int K>
+ag_status expand_wide(const PqArgs& a, bool spaced, cudaStream_t st) {
+  if (a.width == 4) return spaced ? launch_expand<K, uint32_t, true>(a, st) : launch_expand<K, uint32_t, false>(a, st);
+  return spaced ? launch_expand<K, unsigned long long, true>(a, st) : launch_expand<K, unsigned long long, false>(a, st);
+}
 
-// The device work of every entry point of this file.  `pages` is host memory; everything else device memory on `st`.
-// Synchronises `st` once.  h_decoded (host, may be NULL) receives the per-page decoded counts.
-ag_status fx_pages_dev(const FxCall& c, int64_t* d_decoded, int64_t* h_decoded, int64_t* d_bad_pos, cudaStream_t st) {
+// The device work of every entry point of this file.  `c.pages` is host memory; everything else device memory on
+// `st`.  Synchronises `st` once.  h_decoded (host, may be NULL) receives the per-page decoded counts.
+ag_status fx_pages_dev(const PqCall& c, int64_t* d_decoded, int64_t* h_decoded, int64_t* d_bad_pos, cudaStream_t st) {
   const char* fn = c.fn;
-  const int64_t n_pages = c.n_pages;
   const int kind = pass1_kind(c.job);
-  const bool has_runs = kind == kDict || kind == kIndex || kind == kBoolRle;
-  const bool dict = c.job == kJobDictT || c.job == kJobDictW;
-  if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
-  if (n_pages == 0) return AG_OK;
-  if (!c.pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
-  // plan: pages | run_base[n+1] | tile_base[n+1], as parquet_pages_dev lays it out
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_page);
-  const size_t plan_bytes = pb + 2 * (size_t)(n_pages + 1) * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  memcpy(h.data(), c.pages, pb);
-  int64_t* run_base = reinterpret_cast<int64_t*>(h.data() + pb);
-  int64_t* tile_base = run_base + n_pages + 1;
-  run_base[0] = tile_base[0] = 0;
-  bool any_data = false;
-  int64_t slot_end = 0;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const ag_pq_page& g = c.pages[i];
-    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field, more than 2^31-1 values or more than 2^32-1 bytes", fn, (long long)i);
-    any_data |= g.len > 0;
-    slot_end = std::max(slot_end, g.out + g.num_values);
-    run_base[i + 1] = run_base[i] + (has_runs ? std::min(g.num_values, g.len) : 0);
-    tile_base[i + 1] = tile_base[i] + (g.num_values + kTile - 1) / kTile;
+  const bool has_runs = kind == kLevels || kind == kDict || kind == kIndex || kind == kBoolRle;
+  PagePlan plan;
+  AG_TRY(plan_pages(fn, c.pages, c.n_pages, [&](const ag_pq_page& g) { return has_runs ? std::min(g.num_values, g.len) : (int64_t)0; }, &plan));
+  if (c.n_pages == 0) {
+    // no index is looked at: *d_bad_pos is still overwritten
+    if (!d_bad_pos) return AG_OK;
+    static const int64_t kNone = AG_NO_ERROR_POS;
+    AG_TRY(h2d(d_bad_pos, &kNone, 8, st));
+    return sync(st);
   }
-  const int64_t n_runs = run_base[n_pages], n_tiles = tile_base[n_pages];
+  const int64_t n_tiles = plan.n_tiles;
+  const bool dict = c.job == kJobDictT || c.job == kJobDictW;
+  // jobs whose expansion stores whole 2-, 4- or 8-byte elements
+  const bool typed = c.job == kJobLevels || c.job == kJobPlainT || c.job == kJobDictT || c.job == kJobBssT;
   if (n_tiles > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
-  if (any_data && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
-  if (dict && c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
+  if (plan.any_data && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  if (c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
   if (c.job == kJobDictT && c.dict && (reinterpret_cast<uintptr_t>(c.dict) & (c.width - 1)))
     AG_FAIL(AG_ERR_INVALID, "%s: dictionary not aligned to its value width", fn);
-  if ((c.job == kJobPlainT || c.job == kJobDictT || c.job == kJobBssT) && c.out && (reinterpret_cast<uintptr_t>(c.out) & (c.width - 1)))
-    AG_FAIL(AG_ERR_INVALID, "%s: output not aligned to its value width", fn);
+  if (typed && c.out && (reinterpret_cast<uintptr_t>(c.out) & (c.width - 1)))
+    AG_FAIL(AG_ERR_INVALID, "%s: output not aligned to its element width", fn);
   const bool mapped = c.job == kJobDictW || ((c.job == kJobPlainW || c.job == kJobBss) && c.valid);
 
-  const size_t st_bytes = (size_t)n_pages * sizeof(PageState);
-  const size_t off_st = (plan_bytes + 255) & ~(size_t)255;
-  const size_t off_tc = (off_st + st_bytes + 255) & ~(size_t)255;
-  const size_t off_ti = (off_tc + (c.valid ? (size_t)n_tiles * 8 : 0) + 255) & ~(size_t)255;
-  const size_t off_bad = (off_ti + (size_t)n_tiles * 8 + 255) & ~(size_t)255;
-  const size_t off_runs = off_bad + 256;
-  const size_t off_map = (off_runs + (size_t)n_runs * 8 + 255) & ~(size_t)255;
-  const size_t total = off_map + (mapped ? (size_t)slot_end * 4 : 0);
+  Carve sc;
+  const size_t o_plan = sc.take(plan.bytes.size());
+  const size_t o_st = sc.take((size_t)c.n_pages * sizeof(PageState));
+  const size_t o_tc = sc.take(c.valid ? (size_t)n_tiles * 8 : 0);
+  const size_t o_ti = sc.take((size_t)n_tiles * 8);
+  const size_t o_bad = sc.take(8);
+  const size_t o_runs = sc.take((size_t)plan.n_desc * 8);
+  const size_t o_map = sc.take(mapped ? (size_t)plan.slot_end * 4 : 0);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
-  AG_TRY(t.alloc_t(&d, total));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
-  int32_t* map = mapped ? reinterpret_cast<int32_t*>(d + off_map) : nullptr;
+  AG_TRY(t.alloc_t(&d, sc.size));
+  int32_t* map = mapped ? reinterpret_cast<int32_t*>(d + o_map) : nullptr;
   PqArgs a{};
-  a.plan.pages = reinterpret_cast<const ag_pq_page*>(d);
-  a.plan.run_base = reinterpret_cast<const int64_t*>(d + pb);
-  a.plan.tile_base = a.plan.run_base + n_pages + 1;
-  a.plan.n_pages = n_pages;
-  a.plan.n_tiles = n_tiles;
+  AG_TRY(upload_plan(plan, d + o_plan, st, &a.plan));
   a.data = c.data;
   a.valid = c.valid;
-  a.st = reinterpret_cast<PageState*>(d + off_st);
-  a.tile_cnt = c.valid ? reinterpret_cast<int64_t*>(d + off_tc) : nullptr;
-  a.tile_info = reinterpret_cast<int2*>(d + off_ti);
-  a.bad = reinterpret_cast<unsigned long long*>(d_bad_pos ? (void*)d_bad_pos : (void*)(d + off_bad));
-  a.runs = n_runs ? reinterpret_cast<uint2*>(d + off_runs) : nullptr;
+  a.st = reinterpret_cast<PageState*>(d + o_st);
+  a.tile_cnt = c.valid ? reinterpret_cast<int64_t*>(d + o_tc) : nullptr;
+  a.tile_info = reinterpret_cast<int2*>(d + o_ti);
+  a.bad = reinterpret_cast<unsigned long long*>(d_bad_pos ? (void*)d_bad_pos : (void*)(d + o_bad));
+  a.runs = plan.n_desc ? reinterpret_cast<uint2*>(d + o_runs) : nullptr;
   a.d_decoded = d_decoded;
-  a.kind = kind; a.fixed_bw = kind == kBoolRle ? 1 : 0; a.v1 = 0; a.width = c.width;
+  a.kind = kind; a.fixed_bw = c.fixed_bw; a.v1 = c.v1; a.width = c.width;
   a.dict_len = c.dict_len; a.dict = c.dict; a.out = mapped ? (void*)map : c.out;
-  if (c.valid && n_tiles) {
-    pq_tile_count_kernel<<<grid_for(n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(a);
-    AG_TRY(check_launch("pq_tile_count_kernel"));
-  }
-  pq_runs_kernel<<<(unsigned)n_pages, kRleThreads, 0, st>>>(a);
+  AG_TRY(launch_tile_counts(a.plan, c.valid, a.tile_cnt, st));
+  pq_runs_kernel<<<(unsigned)c.n_pages, kRleThreads, 0, st>>>(a);
   AG_TRY(check_launch("pq_runs_kernel"));
   const bool sp = c.valid != nullptr;
   switch (c.job) {
-    case kJobPlainT:
-      AG_TRY(c.width == 4 ? (sp ? launch_expand<kPlain, uint32_t, true>(a, st) : launch_expand<kPlain, uint32_t, false>(a, st))
-                          : (sp ? launch_expand<kPlain, unsigned long long, true>(a, st) : launch_expand<kPlain, unsigned long long, false>(a, st)));
-      break;
-    case kJobDictT:
-      AG_TRY(c.width == 4 ? (sp ? launch_expand<kDict, uint32_t, true>(a, st) : launch_expand<kDict, uint32_t, false>(a, st))
-                          : (sp ? launch_expand<kDict, unsigned long long, true>(a, st) : launch_expand<kDict, unsigned long long, false>(a, st)));
-      break;
-    case kJobBssT:
-      AG_TRY(c.width == 4 ? (sp ? launch_expand<kBss, uint32_t, true>(a, st) : launch_expand<kBss, uint32_t, false>(a, st))
-                          : (sp ? launch_expand<kBss, unsigned long long, true>(a, st) : launch_expand<kBss, unsigned long long, false>(a, st)));
-      break;
+    case kJobLevels: AG_TRY((launch_expand<kLevels, int16_t, false>(a, st))); break;
+    case kJobPlainT: AG_TRY(expand_wide<kPlain>(a, sp, st)); break;
+    case kJobDictT: AG_TRY(expand_wide<kDict>(a, sp, st)); break;
+    case kJobBssT: AG_TRY(expand_wide<kBss>(a, sp, st)); break;
     case kJobPlainW: case kJobDictW: case kJobBss: {
       if (c.job == kJobDictW) AG_TRY((sp ? launch_expand<kIndex, int32_t, true>(a, st) : launch_expand<kIndex, int32_t, false>(a, st)));
       else if (mapped) AG_TRY((launch_expand<kRank, int32_t, true>(a, st)));
@@ -370,86 +342,32 @@ ag_status fx_pages_dev(const FxCall& c, int64_t* d_decoded, int64_t* h_decoded, 
       AG_TRY(check_launch("fx_bool_kernel"));
       break;
   }
-  std::vector<PageState> hs((size_t)n_pages);
-  int64_t bad = AG_NO_ERROR_POS;
-  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
-  if (dict) AG_TRY(d2h(&bad, a.bad, 8, st));
-  AG_TRY(sync(st));
-  if (h_decoded)
-    for (int64_t i = 0; i < n_pages; ++i) h_decoded[i] = hs[i].slots;
-  for (int64_t i = 0; i < n_pages; ++i)
-    if (hs[i].err != kErrNone) {
-      char msg[200];
-      fx_err_text(hs[i], c.pages[i], c.ptype, c.width, msg, sizeof msg);
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: %s (%lld values decoded)", fn, (long long)i, msg, (long long)hs[i].slots);
-    }
-  if (bad != AG_NO_ERROR_POS) AG_FAIL(AG_ERR_INVALID, "%s: invalid index values found for dictionary converter (output slot %lld)", fn, (long long)bad);
+  return read_back(fn, a.st, c.n_pages, dict ? a.bad : nullptr, h_decoded, st,
+                   [&](int64_t i, const PageState& s, char* buf, size_t n) { fx_err_text(s, c.pages[i], c.ptype, c.width, buf, n); });
+}
+
+// ---- argument checks of the entry points, each giving the call's PqCall ----
+int bit_len(int v) { int n = 0; while (v) { ++n; v >>= 1; } return n; }
+
+ag_status levels_args(int max_level, int encoding, PqCall* c) {
+  if (encoding == AG_PQ_LEVELS_BIT_PACKED) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "levels_decode: deprecated BIT_PACKED levels are not implemented");
+  if (encoding != AG_PQ_LEVELS_V1_RLE && encoding != AG_PQ_LEVELS_V2_RLE) AG_FAIL(AG_ERR_INVALID, "levels_decode: unknown level encoding %d", encoding);
+  if (max_level < 0 || max_level > 0xffff) AG_FAIL(AG_ERR_INVALID, "levels_decode: max_level must be 0..65535 (bit width 0..16)");
+  *c = PqCall{};
+  c->fn = "levels_decode"; c->job = kJobLevels; c->width = 2; c->fixed_bw = bit_len(max_level); c->v1 = encoding == AG_PQ_LEVELS_V1_RLE;
   return AG_OK;
 }
 
-// host flavours: stage the page bytes, validity and dictionary.  Values: copy back only the slots each page wrote.
-// Booleans: the output bitmap's bytes up to the last page's last slot go up and come back whole, so every bit the
-// call does not write keeps its value.
-ag_status fx_pages_host(FxCall c, int64_t* decoded, int64_t* bad_pos) {
-  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
-  const char* fn = c.fn;
-  if (c.n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
-  if (c.n_pages == 0) return AG_OK;
-  if (!c.pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
-  const bool boolean = c.job == kJobBoolPlain || c.job == kJobBoolRle;
-  const bool dict = c.job == kJobDictT || c.job == kJobDictW;
-  int64_t data_end = 0, slot_end = 0;
-  for (int64_t i = 0; i < c.n_pages; ++i) {
-    const ag_pq_page& g = c.pages[i];
-    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field", fn, (long long)i);
-    data_end = std::max(data_end, g.data + g.len);
-    slot_end = std::max(slot_end, g.out + g.num_values);
-  }
-  if (data_end > 0 && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
-  if (slot_end > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
-  if (dict && c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
-  CallStream cs; AG_TRY(cs.acquire());
-  Temps t(cs);
-  const size_t vbytes = c.valid ? (size_t)((slot_end + 7) >> 3) : 0;
-  const size_t dbytes = dict ? (size_t)c.dict_len * c.width : 0;
-  const size_t obytes = boolean ? (size_t)((slot_end + 7) >> 3) : (size_t)slot_end * c.width;
-  const size_t o_valid = ((size_t)data_end + 255) & ~(size_t)255;
-  const size_t o_dict = (o_valid + vbytes + 255) & ~(size_t)255;
-  const size_t o_out = (o_dict + dbytes + 255) & ~(size_t)255;
-  const size_t o_bad = (o_out + obytes + 255) & ~(size_t)255;
-  uint8_t* d;
-  AG_TRY(t.alloc_t(&d, o_bad + 8));
-  AG_TRY(h2d(d, c.data, (size_t)data_end, cs));
-  AG_TRY(h2d(d + o_valid, c.valid, vbytes, cs));
-  AG_TRY(h2d(d + o_dict, c.dict, dbytes, cs));
-  // *bad_pos is copied back whatever happens: it reads AG_NO_ERROR_POS when the call fails before any kernel runs
-  static const int64_t kNone = AG_NO_ERROR_POS;
-  AG_TRY(h2d(d + o_bad, &kNone, 8, cs));
-  if (boolean) AG_TRY(h2d(d + o_out, c.out, obytes, cs));
-  FxCall dc = c;
-  dc.data = d;
-  dc.valid = vbytes ? d + o_valid : nullptr;
-  dc.dict = dbytes ? d + o_dict : nullptr;
-  dc.out = d + o_out;
-  std::vector<int64_t> dec((size_t)c.n_pages, 0);   // stays 0 when the call fails before decoding
-  const ag_status rc = fx_pages_dev(dc, nullptr, dec.data(), reinterpret_cast<int64_t*>(d + o_bad), cs);
-  // a decode error still delivers the values decoded before it
-  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
-  if (decoded) memcpy(decoded, dec.data(), (size_t)c.n_pages * 8);
-  if (boolean) {
-    AG_TRY(d2h(c.out, d + o_out, obytes, cs));
-  } else {
-    for (int64_t i = 0; i < c.n_pages; ++i) {
-      const size_t off = (size_t)c.pages[i].out * c.width;
-      AG_TRY(d2h((uint8_t*)c.out + off, d + o_out + off, (size_t)dec[i] * c.width, cs));
-    }
-  }
-  if (dict && bad_pos) AG_TRY(d2h(bad_pos, d + o_bad, 8, cs));
-  const ag_status rs = sync(cs);
-  return rc != AG_OK ? rc : rs;
+// dict_decode (kJobDictT) and plain_decode_spaced (kJobPlainT): 4- or 8-byte values
+ag_status wide_args(const char* fn, int job, int value_width, int64_t dict_len, PqCall* c) {
+  if (value_width != 4 && value_width != 8) AG_FAIL(AG_ERR_INVALID, "%s: value_width must be 4 or 8", fn);
+  if (job == kJobDictT && dict_len < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative dictionary length", fn);
+  *c = PqCall{};
+  c->fn = fn; c->job = job; c->width = value_width; c->dict_len = job == kJobDictT ? dict_len : 0;
+  return AG_OK;
 }
 
-ag_status fixed_args(int ptype, int type_length, int encoding, int64_t dict_len, FxCall* c) {
+ag_status fixed_args(int ptype, int type_length, int encoding, int64_t dict_len, PqCall* c) {
   const char* fn = "fixed_decode";
   int w;
   switch (ptype) {
@@ -468,19 +386,22 @@ ag_status fixed_args(int ptype, int type_length, int encoding, int64_t dict_len,
   else if (encoding == AG_PQ_ENC_PLAIN_DICTIONARY || encoding == AG_PQ_ENC_RLE_DICTIONARY) job = wide ? kJobDictT : kJobDictW;
   else if (encoding == AG_PQ_ENC_BYTE_STREAM_SPLIT && ptype != AG_PQ_TYPE_INT96) job = wide ? kJobBssT : kJobBss;
   else AG_FAIL(AG_ERR_INVALID, "%s: encoding %d is not accepted for physical type %d", fn, encoding, ptype);
-  if ((job == kJobDictT || job == kJobDictW) && dict_len < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative dictionary length", fn);
-  *c = FxCall{};
-  c->fn = fn; c->job = job; c->ptype = ptype; c->width = w; c->dict_len = dict_len;
+  const bool dict = job == kJobDictT || job == kJobDictW;
+  if (dict && dict_len < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative dictionary length", fn);
+  *c = PqCall{};
+  c->fn = fn; c->job = job; c->ptype = ptype; c->width = w; c->dict_len = dict ? dict_len : 0;
   return AG_OK;
 }
 
-ag_status bool_args(int encoding, FxCall* c) {
+ag_status bool_args(int encoding, PqCall* c) {
   if (encoding != AG_PQ_ENC_PLAIN && encoding != AG_PQ_ENC_RLE)
     AG_FAIL(AG_ERR_INVALID, "bool_decode: encoding %d is not accepted for BOOLEAN (PLAIN or RLE)", encoding);
-  *c = FxCall{};
-  c->fn = "bool_decode"; c->job = encoding == AG_PQ_ENC_PLAIN ? kJobBoolPlain : kJobBoolRle; c->width = 1;
+  *c = PqCall{};
+  c->fn = "bool_decode"; c->job = encoding == AG_PQ_ENC_PLAIN ? kJobBoolPlain : kJobBoolRle; c->width = 1; c->bitmap = true;
+  c->fixed_bw = encoding == AG_PQ_ENC_RLE ? 1 : 0;
   return AG_OK;
 }
+
 
 }  // namespace
 
@@ -490,10 +411,65 @@ using namespace ag;
 
 extern "C" {
 
+ag_status ag_parquet_levels_decode_dev(int max_level, int encoding, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                       int16_t* d_out, int64_t* d_decoded, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  PqCall c;
+  AG_TRY(levels_args(max_level, encoding, &c));
+  c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.out = d_out;
+  return fx_pages_dev(c, d_decoded, nullptr, nullptr, resolve_stream(s));
+}
+
+ag_status ag_parquet_levels_decode(int max_level, int encoding, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                   int16_t* out, int64_t* decoded) {
+  AG_TRY(ensure_init());
+  PqCall c;
+  AG_TRY(levels_args(max_level, encoding, &c));
+  c.data = data; c.pages = pages; c.n_pages = n_pages; c.out = out;
+  return pq_pages_host(fx_pages_dev, c, decoded, nullptr);
+}
+
+ag_status ag_parquet_dict_decode_dev(int value_width, const void* d_dict, int64_t dict_len, const uint8_t* d_data, const ag_pq_page* pages,
+                                     int64_t n_pages, const uint8_t* d_valid, void* d_out, int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  PqCall c;
+  AG_TRY(wide_args("dict_decode", kJobDictT, value_width, dict_len, &c));
+  c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.dict = d_dict; c.out = d_out;
+  return fx_pages_dev(c, d_decoded, nullptr, d_bad_pos, resolve_stream(s));
+}
+
+ag_status ag_parquet_dict_decode(int value_width, const void* dict, int64_t dict_len, const uint8_t* data, const ag_pq_page* pages,
+                                 int64_t n_pages, const uint8_t* valid, void* out, int64_t* decoded, int64_t* bad_pos) {
+  AG_TRY(ensure_init());
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  PqCall c;
+  AG_TRY(wide_args("dict_decode", kJobDictT, value_width, dict_len, &c));
+  c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.dict = dict; c.out = out;
+  return pq_pages_host(fx_pages_dev, c, decoded, bad_pos);
+}
+
+ag_status ag_parquet_plain_decode_spaced_dev(int value_width, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages,
+                                             const uint8_t* d_valid, void* d_out, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  PqCall c;
+  AG_TRY(wide_args("plain_decode_spaced", kJobPlainT, value_width, 0, &c));
+  c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.out = d_out;
+  return fx_pages_dev(c, nullptr, nullptr, nullptr, resolve_stream(s));
+}
+
+ag_status ag_parquet_plain_decode_spaced(int value_width, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages,
+                                         const uint8_t* valid, void* out) {
+  AG_TRY(ensure_init());
+  PqCall c;
+  AG_TRY(wide_args("plain_decode_spaced", kJobPlainT, value_width, 0, &c));
+  c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.out = out;
+  return pq_pages_host(fx_pages_dev, c, nullptr, nullptr);
+}
+
 ag_status ag_parquet_bool_decode_dev(int encoding, const uint8_t* d_data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* d_valid,
                                      uint8_t* d_out_bits, int64_t* d_decoded, ag_stream_t s) {
   AG_TRY(ensure_init());
-  FxCall c;
+  PqCall c;
   AG_TRY(bool_args(encoding, &c));
   c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.out = d_out_bits;
   return fx_pages_dev(c, d_decoded, nullptr, nullptr, resolve_stream(s));
@@ -502,17 +478,17 @@ ag_status ag_parquet_bool_decode_dev(int encoding, const uint8_t* d_data, const 
 ag_status ag_parquet_bool_decode(int encoding, const uint8_t* data, const ag_pq_page* pages, int64_t n_pages, const uint8_t* valid,
                                  uint8_t* out_bits, int64_t* decoded) {
   AG_TRY(ensure_init());
-  FxCall c;
+  PqCall c;
   AG_TRY(bool_args(encoding, &c));
   c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.out = out_bits;
-  return fx_pages_host(c, decoded, nullptr);
+  return pq_pages_host(fx_pages_dev, c, decoded, nullptr);
 }
 
 ag_status ag_parquet_fixed_decode_dev(int physical_type, int type_length, int encoding, const uint8_t* d_data, const ag_pq_page* pages,
                                       int64_t n_pages, const uint8_t* d_valid, const void* d_dict, int64_t dict_len, void* d_out,
                                       int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s) {
   AG_TRY(ensure_init());
-  FxCall c;
+  PqCall c;
   AG_TRY(fixed_args(physical_type, type_length, encoding, dict_len, &c));
   c.data = d_data; c.pages = pages; c.n_pages = n_pages; c.valid = d_valid; c.dict = d_dict; c.out = d_out;
   return fx_pages_dev(c, d_decoded, nullptr, d_bad_pos, resolve_stream(s));
@@ -523,10 +499,10 @@ ag_status ag_parquet_fixed_decode(int physical_type, int type_length, int encodi
                                   int64_t* bad_pos) {
   AG_TRY(ensure_init());
   if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
-  FxCall c;
+  PqCall c;
   AG_TRY(fixed_args(physical_type, type_length, encoding, dict_len, &c));
   c.data = data; c.pages = pages; c.n_pages = n_pages; c.valid = valid; c.dict = dict; c.out = out;
-  return fx_pages_host(c, decoded, bad_pos);
+  return pq_pages_host(fx_pages_dev, c, decoded, bad_pos);
 }
 
 }  // extern "C"

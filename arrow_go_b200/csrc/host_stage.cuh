@@ -52,6 +52,15 @@ static inline ag_status d2h(void* h, const void* d, size_t nbytes, cudaStream_t 
 }
 static inline ag_status sync(cudaStream_t st) { AG_CUDA_TRY(cudaStreamSynchronize(st)); return AG_OK; }
 
+static inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
+// Carves one scratch allocation into 256-byte aligned regions: take(n) returns the offset of the next n bytes, and
+// `size` is what to allocate once every region is taken.
+struct Carve {
+  size_t size = 0;
+  size_t take(size_t nbytes) { const size_t r = size; size = align256(size + nbytes); return r; }
+};
+
 // Upload the bytes of a bitmap range [off, off+n) to a device temp; the device copy keeps the
 // same bit phase (off % 8) so kernels address it with bit offset (off & 7).
 static inline ag_status upload_bitmap(Temps& t, const uint8_t* h, int64_t off, int64_t n, uint8_t** d, int64_t* doff) {

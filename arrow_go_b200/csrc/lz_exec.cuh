@@ -58,9 +58,11 @@ static inline ag_status pq_decompress_host(const char* fn, pq_codec_dev_fn dev, 
   if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  const size_t o_dst = ((size_t)src_end + 255) & ~(size_t)255;
+  Carve sc;
+  sc.take((size_t)src_end);
+  const size_t o_dst = sc.take((size_t)dst_end);
   uint8_t* d;
-  AG_TRY(t.alloc_t(&d, o_dst + (size_t)dst_end));
+  AG_TRY(t.alloc_t(&d, sc.size));
   AG_TRY(h2d(d, src, (size_t)src_end, cs));
   std::vector<int64_t> w((size_t)n_pages, 0);                    // stays 0 when the call fails before decoding
   const ag_status rc = dev(d, pages, n_pages, d + o_dst, nullptr, w.data(), cs);

@@ -1,9 +1,31 @@
-// pq_decode.cuh — the Parquet page-decode building blocks shared by rle.cu and byte_array.cu.  Internal, not part of
-// the ABI.  rle.cu's header comment describes the passes: tile counts, the RLE/bit-packed run walk and expansion, and
-// the DELTA_BINARY_PACKED block walk, tile sums and scan.
+// pq_decode.cuh — the Parquet page-decode building blocks shared by fixed.cu, rle.cu and byte_array.cu.  Internal, not
+// part of the ABI.  The device passes: tile counts, the RLE/bit-packed run walk and expansion, and the
+// DELTA_BINARY_PACKED block walk, tile sums and scan (rle.cu's header describes those).  The host side every page
+// driver shares: the checked page plan and its upload, the tile-count launch, the read-back of the per-page states,
+// and the host flavour's staging.
+//
+// A call decodes a batch of pages (ag_pq_page descriptors, one device buffer of page payloads) in three launches:
+//   1. pq_tile_count_kernel (spaced only): valid bits per 1024-slot tile of every page.
+//   2. pq_runs_kernel, one block per page: scans the page's tile counts into dense-rank bases, then streams the page
+//      bytes through shared memory in 16 KB windows while thread 0 walks the run headers (the chain is sequential; the
+//      parallelism comes from the pages).  Each run becomes an 8-byte descriptor {first dense value | literal flag,
+//      repeated value or payload byte offset}; the page records its run count, decoded count and an error code.
+//      Windows start at the next header, so the bytes of long literal runs between two windows are never loaded.
+//   3. pq_expand_kernel, one block per 1024-slot tile of output: finds its page and run by binary search, broadcasts
+//      repeated values, unpacks literal values with aligned 32-bit loads + funnel shift, gathers dictionary values
+//      (the dictionary stays in L2) with the bounds check fused, and maps slots to dense ranks with a ballot scan of
+//      the validity bits (null slots get 0, like FillZero).
+// Roofline.  Single pass: encoded bytes read once + values written once (+ 1 bit of validity per slot).  This design
+// reads the encoded bytes up to twice (pass 2 only touches the headers' windows and the payload it expands) and
+// writes 8 B per run descriptor, so its own bound is (2 x encoded + written) bytes of HBM traffic; the dictionary
+// gather is served from L2.
 #pragma once
 
 #include <stdio.h>
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
 
 #include "host_stage.cuh"
 
@@ -812,6 +834,159 @@ ag_status launch_expand(const PqArgs& a, cudaStream_t st) {
   if (a.plan.n_tiles == 0) return AG_OK;
   pq_expand_kernel<KIND, T, SPACED><<<(unsigned)a.plan.n_tiles, kRleThreads, 0, st>>>(a);
   return check_launch("pq_expand_kernel");
+}
+
+// ---------------------------------------------------------------- host side of every page driver ----
+// A checked page table and the plan the device reads: pages | desc_base[n+1] | tile_base[n+1], where desc_base is
+// every page's first descriptor (runs, or DELTA_BINARY_PACKED miniblocks) and tile_base its first 1024-slot tile.
+struct PagePlan {
+  std::vector<uint8_t> bytes;         // a caller may append its own page data before upload_plan
+  int64_t n_pages = 0, n_desc = 0, n_tiles = 0;
+  int64_t data_end = 0, slot_end = 0; // one past the last page byte / output slot
+  bool any_data = false;              // some page has bytes
+  int64_t* desc_base() { return reinterpret_cast<int64_t*>(bytes.data() + (size_t)n_pages * sizeof(ag_pq_page)); }
+  int64_t* tile_base() { return desc_base() + n_pages + 1; }
+};
+
+// Checks `pages` and plans them; cap(page) is the number of descriptors a page may need.  No page gives an empty plan.
+template <typename Cap>
+static inline ag_status plan_pages(const char* fn, const ag_pq_page* pages, int64_t n_pages, Cap cap, PagePlan* p) {
+  if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
+  if (n_pages > 0 && !pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
+  const size_t pb = (size_t)n_pages * sizeof(ag_pq_page);
+  p->n_pages = n_pages;
+  p->bytes.assign(pb + 2 * (size_t)(n_pages + 1) * 8, 0);
+  if (n_pages) memcpy(p->bytes.data(), pages, pb);
+  int64_t *desc_base = p->desc_base(), *tile_base = p->tile_base();
+  for (int64_t i = 0; i < n_pages; ++i) {
+    const ag_pq_page& g = pages[i];
+    if (g.data < 0 || g.len < 0 || g.num_values < 0 || g.out < 0 || g.num_values > 0x7fffffffLL || g.len > 0xffffffffLL)
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field, more than 2^31-1 values or more than 2^32-1 bytes", fn, (long long)i);
+    desc_base[i + 1] = desc_base[i] + cap(g);
+    tile_base[i + 1] = tile_base[i] + (g.num_values + kTile - 1) / kTile;
+    p->data_end = std::max(p->data_end, g.data + g.len);
+    p->slot_end = std::max(p->slot_end, g.out + g.num_values);
+    p->any_data |= g.len > 0;
+  }
+  p->n_desc = desc_base[n_pages];
+  p->n_tiles = tile_base[n_pages];
+  return AG_OK;
+}
+
+// Uploads the plan to device memory `d` (p.bytes.size() bytes) and returns its device views.
+static inline ag_status upload_plan(const PagePlan& p, uint8_t* d, cudaStream_t st, PqPlan* out) {
+  AG_TRY(h2d(d, p.bytes.data(), p.bytes.size(), st));
+  out->pages = reinterpret_cast<const ag_pq_page*>(d);
+  out->run_base = reinterpret_cast<const int64_t*>(d + (size_t)p.n_pages * sizeof(ag_pq_page));
+  out->tile_base = out->run_base + p.n_pages + 1;
+  out->n_pages = p.n_pages;
+  out->n_tiles = p.n_tiles;
+  return AG_OK;
+}
+
+// spaced calls: the valid bits of every tile into tile_cnt
+static inline ag_status launch_tile_counts(const PqPlan& plan, const uint8_t* valid, int64_t* tile_cnt, cudaStream_t st) {
+  if (!valid || plan.n_tiles == 0) return AG_OK;
+  PqArgs c{};
+  c.plan = plan; c.valid = valid; c.tile_cnt = tile_cnt;
+  pq_tile_count_kernel<<<grid_for(plan.n_tiles, kRleThreads / 32, 8), kRleThreads, 0, st>>>(c);
+  return check_launch("pq_tile_count_kernel");
+}
+
+// The end of a driver: copies the per-page states back, synchronises `st` once, fills h_decoded (host, may be NULL),
+// fails on the lowest failing page with the text text(page, state, buf, size) gives, then on the lowest out-of-range
+// dictionary index in *d_bad (NULL: the call looks up no dictionary).
+template <typename S, typename Text>
+ag_status read_back(const char* fn, const S* d_st, int64_t n_pages, const unsigned long long* d_bad, int64_t* h_decoded,
+                    cudaStream_t st, Text text) {
+  std::vector<S> hs((size_t)n_pages);
+  int64_t bad = AG_NO_ERROR_POS;
+  AG_TRY(d2h(hs.data(), d_st, (size_t)n_pages * sizeof(S), st));
+  if (d_bad) AG_TRY(d2h(&bad, d_bad, 8, st));
+  AG_TRY(sync(st));
+  if (h_decoded)
+    for (int64_t i = 0; i < n_pages; ++i) h_decoded[i] = hs[i].slots;
+  for (int64_t i = 0; i < n_pages; ++i)
+    if (hs[i].err != 0) {
+      char msg[200];
+      text(i, hs[i], msg, sizeof msg);
+      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: %s (%lld values decoded)", fn, (long long)i, msg, (long long)hs[i].slots);
+    }
+  if (bad != AG_NO_ERROR_POS) AG_FAIL(AG_ERR_INVALID, "%s: invalid index values found for dictionary converter (output slot %lld)", fn, (long long)bad);
+  return AG_OK;
+}
+
+// One call of a fixed-width or DELTA_BINARY_PACKED page entry point.  `pages` is host memory; the other pointers are
+// host memory in a host flavour and device memory in a device flavour.
+struct PqCall {
+  const char* fn;           // message prefix
+  int job;                  // fixed.cu: what runs after pass 1
+  int ptype;                // AG_PQ_TYPE_* where the error texts depend on it, else 0
+  int width;                // bytes per output slot (booleans: 1)
+  int fixed_bw;             // levels: bits.Len(max_level); RLE booleans: 1
+  int v1;                   // levels: 4-byte length prefix
+  bool bitmap;              // booleans: `out` is a bitmap
+  const uint8_t* data;
+  const ag_pq_page* pages;
+  int64_t n_pages;
+  const uint8_t* valid;     // NULL = every slot valid
+  const void* dict;
+  int64_t dict_len;         // 0 unless the pages are dictionary-encoded
+  void* out;
+};
+
+// A device flavour: decodes `c`, fills h_decoded (host, may be NULL), synchronises `st` once.
+typedef ag_status (*pq_pages_dev_fn)(const PqCall& c, int64_t* d_decoded, int64_t* h_decoded, int64_t* d_bad_pos, cudaStream_t st);
+
+// host flavour: stage the page bytes, validity and dictionary, decode, copy back only the slots each page wrote.  A
+// boolean bitmap's bytes up to the last page's last slot go up and come back whole, so every bit the call does not
+// write keeps its value.
+static inline ag_status pq_pages_host(pq_pages_dev_fn dev, const PqCall& c, int64_t* decoded, int64_t* bad_pos) {
+  const char* fn = c.fn;
+  PagePlan plan;
+  AG_TRY(plan_pages(fn, c.pages, c.n_pages, [](const ag_pq_page&) { return (int64_t)0; }, &plan));
+  if (c.n_pages == 0) return AG_OK;
+  if (plan.data_end > 0 && !c.data) AG_FAIL(AG_ERR_INVALID, "%s: NULL page data", fn);
+  if (plan.slot_end > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  if (c.dict_len > 0 && !c.dict) AG_FAIL(AG_ERR_INVALID, "%s: NULL dictionary", fn);
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const size_t vbytes = c.valid ? (size_t)((plan.slot_end + 7) >> 3) : 0;
+  const size_t dbytes = (size_t)c.dict_len * c.width;
+  const size_t obytes = c.bitmap ? (size_t)((plan.slot_end + 7) >> 3) : (size_t)plan.slot_end * c.width;
+  Carve sc;
+  const size_t o_data = sc.take((size_t)plan.data_end), o_valid = sc.take(vbytes), o_dict = sc.take(dbytes);
+  const size_t o_out = sc.take(obytes), o_bad = sc.take(8);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, sc.size));
+  AG_TRY(h2d(d + o_data, c.data, (size_t)plan.data_end, cs));
+  AG_TRY(h2d(d + o_valid, c.valid, vbytes, cs));
+  AG_TRY(h2d(d + o_dict, c.dict, dbytes, cs));
+  // *bad_pos is copied back whatever happens: it reads AG_NO_ERROR_POS when the call fails before any kernel runs
+  static const int64_t kNone = AG_NO_ERROR_POS;
+  AG_TRY(h2d(d + o_bad, &kNone, 8, cs));
+  if (c.bitmap) AG_TRY(h2d(d + o_out, c.out, obytes, cs));
+  PqCall dc = c;
+  dc.data = d + o_data;
+  dc.valid = vbytes ? d + o_valid : nullptr;
+  dc.dict = dbytes ? d + o_dict : nullptr;
+  dc.out = d + o_out;
+  std::vector<int64_t> dec((size_t)c.n_pages, 0);   // stays 0 when the call fails before decoding
+  const ag_status rc = dev(dc, nullptr, dec.data(), reinterpret_cast<int64_t*>(d + o_bad), cs);
+  // a decode error still delivers the values decoded before it
+  if (rc != AG_OK && rc != AG_ERR_INVALID) return rc;
+  if (decoded) memcpy(decoded, dec.data(), (size_t)c.n_pages * 8);
+  if (c.bitmap) {
+    AG_TRY(d2h(c.out, d + o_out, obytes, cs));
+  } else {
+    for (int64_t i = 0; i < c.n_pages; ++i) {
+      const size_t off = (size_t)c.pages[i].out * c.width;
+      AG_TRY(d2h((uint8_t*)c.out + off, d + o_out + off, (size_t)dec[i] * c.width, cs));
+    }
+  }
+  if (bad_pos) AG_TRY(d2h(bad_pos, d + o_bad, 8, cs));
+  const ag_status rs = sync(cs);
+  return rc != AG_OK ? rc : rs;
 }
 
 }  // namespace

@@ -302,15 +302,14 @@ static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, i
   for (int64_t i = 0; i < n_pages; ++i) elem_base[i + 1] = elem_base[i] + std::min(pages[i].src_len / 2, pages[i].dst_len);
   const int64_t n_elem = elem_base[n_pages];
   const size_t st_bytes = (size_t)n_pages * sizeof(SnapPage);
-  const size_t off_st = (plan_bytes + 255) & ~(size_t)255;
-  const size_t off_out = (off_st + st_bytes + 255) & ~(size_t)255;
-  const size_t off_ref = (off_out + (size_t)n_elem * 4 + 255) & ~(size_t)255;
-  const size_t off_lit = (off_ref + (size_t)n_elem * 4 + 255) & ~(size_t)255;
-  const size_t total = off_lit + (size_t)n_elem;
+  Carve sc;
+  sc.take(plan_bytes);
+  const size_t off_st = sc.take(st_bytes), off_out = sc.take((size_t)n_elem * 4), off_ref = sc.take((size_t)n_elem * 4);
+  const size_t off_lit = sc.take((size_t)n_elem);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
-  AG_TRY(t.alloc_t(&d, total));
+  AG_TRY(t.alloc_t(&d, sc.size));
   AG_TRY(h2d(d, h.data(), plan_bytes, st));
   SnapArgs a;
   a.pages = reinterpret_cast<const ag_pq_compressed*>(d);

@@ -906,16 +906,16 @@ ag_status zstd_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_
     sq[i + 1] = sq[i] + dl / 3;
     eb[i + 1] = eb[i] + std::min(dl, 2 * (dl / 3) + 2 * (sl / 3));
   }
-  auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t o_st = up(plan_bytes), o_blk = up(o_st + (size_t)n_pages * sizeof(ZPage));
-  const size_t o_fr = up(o_blk + (size_t)bb[n_pages] * sizeof(ZBlk)), o_lit = up(o_fr + (size_t)fb[n_pages] * sizeof(ZFrame));
-  const size_t o_ll = up(o_lit + (size_t)lb[n_pages]), o_ml = up(o_ll + (size_t)sq[n_pages] * 4), o_of = up(o_ml + (size_t)sq[n_pages] * 4);
-  const size_t o_eo = up(o_of + (size_t)sq[n_pages] * 4), o_er = up(o_eo + (size_t)eb[n_pages] * 4), o_ek = up(o_er + (size_t)eb[n_pages] * 4);
-  const size_t total = o_ek + (size_t)eb[n_pages];
+  Carve sc;
+  sc.take(plan_bytes);
+  const size_t o_st = sc.take((size_t)n_pages * sizeof(ZPage)), o_blk = sc.take((size_t)bb[n_pages] * sizeof(ZBlk));
+  const size_t o_fr = sc.take((size_t)fb[n_pages] * sizeof(ZFrame)), o_lit = sc.take((size_t)lb[n_pages]);
+  const size_t o_ll = sc.take((size_t)sq[n_pages] * 4), o_ml = sc.take((size_t)sq[n_pages] * 4), o_of = sc.take((size_t)sq[n_pages] * 4);
+  const size_t o_eo = sc.take((size_t)eb[n_pages] * 4), o_er = sc.take((size_t)eb[n_pages] * 4), o_ek = sc.take((size_t)eb[n_pages]);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
-  AG_TRY(t.alloc_t(&d, total));
+  AG_TRY(t.alloc_t(&d, sc.size));
   AG_TRY(h2d(d, h.data(), plan_bytes, st));
   const int64_t* dbase = reinterpret_cast<const int64_t*>(d + pb);
   ZArgs a;

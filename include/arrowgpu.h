@@ -590,7 +590,7 @@ ag_status ag_parquet_def_levels_to_bitmap_dev(const int16_t* d_def_levels, int64
  *       returns a short count instead); the slot holds 0.
  *   The device flavours synchronise `s` once, to read the per-page error codes back; d_decoded (may be NULL) is a
  *   device array of n_pages counts, *d_bad_pos (may be NULL) is overwritten (AG_NO_ERROR_POS when every index
- *   is in range).  Host flavours: decoded (may be NULL) and bad_pos (may be NULL) are host memory.
+ *   is in range, n_pages == 0 included).  Host flavours: decoded (may be NULL) and bad_pos (may be NULL) are host memory.
  *
  *   ag_parquet_levels_decode: LevelDecoder.SetData / SetDataV2 / Decode (parquet/internal/encoding/levels.go:188-297).
  *     Bit width = bits.Len(max_level).  AG_PQ_LEVELS_V1_RLE: a data page v1's level section, a 4-byte
@@ -784,7 +784,7 @@ ag_status ag_parquet_byte_array_decode_dev(int encoding, int offset_width, const
  *   there); an RLE boolean repeated byte other than 0 or 1 is true (value != 0, rle.go:161-165 does not mask it); a
  *   BYTE_STREAM_SPLIT page's value count is its stride, len / width (SetData replaces nvals with it).
  *   Device flavours: d_decoded (may be NULL) is device memory; *d_bad_pos (may be NULL) is overwritten
- *   (AG_NO_ERROR_POS when every index is in range).  Host flavours: decoded and bad_pos (may be NULL) are host
+ *   (AG_NO_ERROR_POS when every index is in range, n_pages == 0 included).  Host flavours: decoded and bad_pos (may be NULL) are host
  *   memory; they stage `data`, `valid`, the dictionary and (booleans) the output bitmap's bytes up to the last page's
  *   last slot, and copy back only what the call wrote, so the rest of `out` / `out_bits` is untouched.
  * ================================================================================= */

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Parquet page decode on the device (include/arrowgpu.h, csrc/rle.cu) at ~100M values over 2^19-value (~1 MB) pages.
+"""Parquet page decode on the device (include/arrowgpu.h, csrc/fixed.cu and csrc/rle.cu) at ~100M values over 2^19-value (~1 MB) pages.
 
   python scripts/parquet_pages_bench.py [--values N] [--steps K] [--warmup W] [--profile]
 

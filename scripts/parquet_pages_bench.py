@@ -403,8 +403,8 @@ def bytearray_cases(args, N, rng, timed, upload, DeviceBuffer, values=20_000_000
     import torch
     from torch.profiler import ProfilerActivity, profile as tprofile
 
-    import pq_bytearray_files as BF
     import pq_bytearray_ref as B
+    import pq_files as F
     out = {}
 
     def make(bodies, per_page):
@@ -468,7 +468,7 @@ def bytearray_cases(args, N, rng, timed, upload, DeviceBuffer, values=20_000_000
 
     # (b) PLAIN, (c) DELTA_LENGTH, (e) SNAPPY + PLAIN: ~1 MiB pages of random-length strings
     per = 58_000
-    vals = [BF.random_strings(rng, per) for _ in range(4)]
+    vals = [F.random_strings(rng, per) for _ in range(4)]
     vbytes = [sum(len(v) for v in vs) for vs in vals]
     plain = [B.plain_encode(vs) for vs in vals]
     dblob, pages, enc, n_pages = make(plain, per)
@@ -501,7 +501,7 @@ def bytearray_cases(args, N, rng, timed, upload, DeviceBuffer, values=20_000_000
 
     # (d) DELTA_BYTE_ARRAY on sorted keys
     per = 1 << 18
-    keys = [BF.random_strings(rng, per, sorted_keys=True) for _ in range(4)]
+    keys = [F.random_strings(rng, per, sorted_keys=True) for _ in range(4)]
     dba = [B.dba_encode(k) for k in keys]
     dblob, pages, enc, n_pages = make(dba, per)
     data = sum(sum(len(v) for v in keys[p % 4]) for p in range(n_pages))

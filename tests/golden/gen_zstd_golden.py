@@ -9,7 +9,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
-from test_zstd_oracle import golden_payload  # noqa: E402
+from zstd_ref import golden_payload  # noqa: E402
 
 ZSTD_c_compressionLevel, ZSTD_c_contentSizeFlag, ZSTD_c_checksumFlag = 100, 200, 201
 

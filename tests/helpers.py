@@ -129,5 +129,13 @@ class Dev:
         return self.buf.to_numpy(dtype, count, self.byte_offset)
 
 
+def checksum64(words):
+    """what ag_checksum64_dev gives for the uint64 `words`: sum of word i times a splitmix64 mix of i, modulo 2^64"""
+    z = np.arange(words.size, dtype=np.uint64) + np.uint64(0x9E3779B97F4A7C15)
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return int(((z ^ (z >> np.uint64(31))) * words).sum(dtype=np.uint64))
+
+
 def dev_scalar_i64(value=0):
     return Dev(np.array([value], dtype=np.int64))

@@ -1,6 +1,9 @@
 """Python restatement of raw Snappy decoding as the device decompressor (csrc/snappy.cu) does it: golang/snappy's decode
 checks, plus the page outcomes of include/arrowgpu.h.  And an encoder that can emit every element form: inline and
-1-4-byte literal lengths, copy-1/2/4, overlapping copies.  Not product code."""
+1-4-byte literal lengths, copy-1/2/4, overlapping copies; the streams of every form and the corrupt rows the tests
+share.  Not product code."""
+import numpy as np
+
 OK, CORRUPT, SIZE = 0, 1, 2
 MESSAGE = {CORRUPT: "parquet: could not decompress page: snappy: corrupt input",
            SIZE: "parquet: metadata said {} bytes uncompressed data page, got {} bytes"}
@@ -147,3 +150,54 @@ def encode(data, copy_form=None, lit_bytes=None, max_copy=64):
         lit0 = i
     flush(len(data))
     return stream(len(data), els)
+
+
+def forms():
+    """(name, stream, expected output) covering every element form"""
+    rng = np.random.default_rng(52)
+    big = rng.integers(0, 256, 70_000, dtype=np.uint8).tobytes()
+    far = big + big[:100]                                       # a copy 70 000 bytes back: copy-4
+    out = [
+        ("inline_literals", encode(b"abcdefgh" * 3 + bytes(range(40)), lit_bytes=0)),
+        ("literal_1_byte_length", stream(200, [literal(big[:200], 1)])),
+        ("literal_2_byte_length", stream(300, [literal(big[:300], 2)])),
+        ("literal_3_byte_length", stream(70_000, [literal(big, 3)])),
+        ("literal_4_byte_length", stream(61, [literal(big[:61], 4)])),
+        ("literal_1_byte_length_short", stream(5, [literal(big[:5], 1)])),
+        ("copy_1", stream(20, [literal(b"0123456789"), copy(10, 10, 1)])),
+        ("copy_2", stream(74, [literal(b"0123456789"), copy(10, 64, 2)])),
+        ("copy_4", stream(74, [literal(b"0123456789"), copy(10, 64, 4)])),
+        ("offset_1_run", stream(1 + 64 * 3, [literal(b"z"), copy(1, 64, 2), copy(1, 64, 4), copy(64, 64, 2)])),
+        ("overlap_offset_3", stream(3 + 11, [literal(b"abc"), copy(3, 11, 1)])),
+        ("copy_of_length_1", stream(2, [literal(b"q"), copy(1, 1, 2)])),
+        ("offset_beyond_64k", encode(far)),
+        ("greedy_copy_2_only", encode(b"hello hello hello world " * 40, copy_form=2)),
+        ("greedy_copy_4_only", encode(b"hello hello hello world " * 40, copy_form=4)),
+        ("greedy_literal_4_bytes", encode(big[:5000] + big[:5000], lit_bytes=4)),
+        ("empty_stream", stream(0, [])),
+    ]
+    return [(n, s, decode(s)[0]) for n, s in out]
+
+
+def corrupt_rows():
+    """(name, stream, dst_len, bytes the restatement delivers)"""
+    ok = literal(b"0123456789")
+    return [
+        ("no_preamble", b"", 5, 0),
+        ("preamble_cut", b"\x80", 5, 0),
+        ("preamble_over_10_bytes", b"\xff" * 10 + b"\x01", 5, 0),
+        ("preamble_over_32_bits", put_uvarint(1 << 32), 1 << 32, 0),
+        ("literal_length_cut", stream(20, [ok, b"\xf0"]), 20, 10),
+        ("literal_4_length_cut", stream(20, [ok, b"\xfc\x01\x00"]), 20, 10),
+        ("literal_bytes_cut", stream(20, [ok, literal(b"abcdefghij")[:-1]]), 20, 10),
+        ("literal_past_output", stream(15, [ok, literal(b"abcdefghij")]), 15, 10),
+        ("copy_1_offset_cut", stream(20, [ok, copy(10, 10, 1)[:1]]), 20, 10),
+        ("copy_2_offset_cut", stream(20, [ok, copy(10, 10, 2)[:2]]), 20, 10),
+        ("copy_4_offset_cut", stream(20, [ok, copy(10, 10, 4)[:4]]), 20, 10),
+        ("copy_offset_0", stream(20, [ok, copy(0, 10, 2)]), 20, 10),
+        ("copy_offset_past_output", stream(30, [ok, copy(11, 10, 2)]), 30, 10),
+        ("copy_past_output", stream(15, [ok, copy(10, 10, 2)]), 15, 10),
+        ("stream_ends_early", stream(30, [ok, copy(10, 10, 1)]), 30, 20),
+        ("trailing_element", stream(20, [ok, copy(10, 10, 1), literal(b"x")]), 20, 20),
+        ("preamble_only", stream(7, []), 7, 0),
+    ]

@@ -9,12 +9,14 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_bytearray_files as BF
 import pq_bytearray_ref as B
 import pq_delta_ref as D
+import pq_files as F
+import pq_pages as P
 from arrow_go_b200 import _native as N
-from helpers import Dev, ptr
-from test_gpu_parquet_pages import batch
+from helpers import Dev, checksum64, ptr
+from pq_chunk import read_chunk_dev
+from pq_pages import batch
 
 gpu = pytest.mark.gpu
 FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
@@ -96,13 +98,13 @@ def compare(ag, enc, ow, streams, rng, dev, frac=None, gap=True, dictionary=None
 def random_streams(rng, enc, long_values=False):
     streams = []
     for n in (1, 7, 1000, 5000):
-        vals = BF.random_strings(rng, n, sorted_keys=bool(rng.integers(0, 2)))
+        vals = F.random_strings(rng, n, sorted_keys=bool(rng.integers(0, 2)))
         streams.append((ENCODERS[enc](vals), n))
     streams.append((ENCODERS[enc]([b""] * 300), 300))                        # empty values only
     streams.append((ENCODERS[enc]([]), 0))
     if long_values:
         big = [bytes(rng.integers(0, 256, 20_000, dtype=np.uint8)), b"ab", bytes(rng.integers(0, 256, (1 << 20) + 77, dtype=np.uint8)), b""]
-        streams.append((ENCODERS[enc](big + BF.random_strings(rng, 50)), 54))
+        streams.append((ENCODERS[enc](big + F.random_strings(rng, 50)), 54))
     return streams
 
 
@@ -126,7 +128,7 @@ def test_random_pages(ag, enc, ow, dev):
 def test_dictionary_pages(ag, ow, dev):
     rng = np.random.default_rng(41 + ow)
     import pq_ref as R
-    dictionary = BF.random_strings(rng, 400) + [b"", b"z" * 5000]
+    dictionary = F.random_strings(rng, 400) + [b"", b"z" * 5000]
     streams = []
     for n in (1, 100, 3000, 20000):
         idx = rng.integers(0, len(dictionary), n)
@@ -169,7 +171,7 @@ def error_cases():
 def test_error_cases(ag, case, dev):
     name, enc, stream, nv, frac = case
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    good = ENCODERS[enc](BF.random_strings(rng, 500))
+    good = ENCODERS[enc](F.random_strings(rng, 500))
     for ow in (4, 8):
         st, msg, errs, _, _ = compare(ag, enc, ow, [(good, 500), (stream, nv), (stream, nv)], rng, dev, frac, gap=False)
         assert errs and errs[0][0] in (1, 2), errs                           # spaced: the validity decides what a page needs
@@ -181,7 +183,7 @@ def test_error_cases(ag, case, dev):
 @pytest.mark.parametrize("enc", [B.PLAIN, B.DELTA_BYTE_ARRAY], ids=["plain", "dba"])
 def test_capacity_and_size_query(ag, enc, dev):
     rng = np.random.default_rng(43)
-    vals = BF.random_strings(rng, 3000, sorted_keys=enc == B.DELTA_BYTE_ARRAY)
+    vals = F.random_strings(rng, 3000, sorted_keys=enc == B.DELTA_BYTE_ARRAY)
     blob, pages, n_slots = batch([(ENCODERS[enc](vals), 3000)], rng, gap=False)
     woffs, wdata, _, _, _ = expect(enc, blob, pages, n_slots, offset_base=5)
     for cap in (5 + len(wdata) - 1, 0):
@@ -219,91 +221,44 @@ def test_invalid_arguments(ag):
     assert st == N.AG_ERR_INVALID and "overlap" in msg
 
 
-def upload_plan(ag, plan, valid):
-    vbits = None if valid.all() else np.packbits(valid, bitorder="little")
-    return np.frombuffer(plan["data"], np.uint8).copy(), vbits
+def write_and_plan(path, rng, enc, nf, version, n, **kw):
+    tbl = F.write_column(path, F.make_string_column(rng, enc, n, nf), nullable=nf is not None, encoding=enc, version=version, **kw)
+    return tbl, P.chunk_plan(path)
 
 
-def device_decode_chunk(ag, plan, valid, ow, dev=True):
-    """dictionary page as PLAIN, then the dictionary pages, then the PLAIN pages chained with offset_base"""
-    blob, vbits = upload_plan(ag, plan, valid)
-    n = plan["n_slots"]
-    doff = ddata = None
-    if plan["dict"]:
-        b, ln, nv = plan["dict"]
-        st, msg, offs, out, dec, total, _ = run_ba(ag, B.PLAIN, ow, blob, [(b, ln, nv, 0)], nv, out_cap=ln, dev=dev)
-        assert st == N.AG_OK, msg
-        doff, ddata = offs.astype(np.int32 if ow == 4 else np.int64), out[:max(total, 1)].copy()
-    groups = {}
-    for enc, desc in plan["pages"]:
-        groups.setdefault(B.PLAIN_DICTIONARY if enc == B.RLE_DICTIONARY else enc, []).append(desc)
-    vals, lens, base = [b""] * n, np.zeros(n, np.int64), 0
-    for enc in sorted(groups, reverse=True):                    # dictionary pages first, then PLAIN
-        pages = groups[enc]
-        st, msg, offs, out, dec, total, _ = run_ba(ag, enc, ow, blob, pages, n, vbits,
-                                                   doff if enc != B.PLAIN else None, ddata if enc != B.PLAIN else None,
-                                                   offset_base=base, dev=dev)
-        assert st == N.AG_OK, msg
-        for (_, _, nv, o) in pages:
-            for s in range(o, o + nv):
-                vals[s] = out[offs[s]:offs[s + 1]].tobytes()
-        base += total
-    return vals
+def check_chunk(ag, tbl, plan, flavours=((4, True), (8, False))):
+    """read the chunk with each (offset width, values through the host entry point) against pyarrow"""
+    want, wvalid = F.expected(tbl, plan)
+    for ow, host in flavours:
+        values, valid = read_chunk_dev(ag, plan, offset_width=ow, host_values=host)
+        assert np.array_equal(valid, wvalid)
+        assert values == want, (ow, host)
 
 
 @gpu
-@pytest.mark.parametrize("case", BF.cases(), ids=BF.case_id)
+@pytest.mark.parametrize("case", F.ba_cases(), ids=F.case_id)
 def test_pyarrow_files_end_to_end(ag, case, tmp_path):
     enc, nf, ver, ps = case
-    rng = np.random.default_rng(zlib.crc32(BF.case_id(case).encode()))
-    path = str(tmp_path / "c.parquet")
-    tbl = BF.write_file(path, rng, enc, nf, ver, n=8000, data_page_size=ps)
-    want, valid = BF.expected(tbl)
-    for ow in (4, 8):
-        assert device_decode_chunk(ag, BF.chunk_plan(path), valid, ow, dev=ow == 8) == want
+    rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
+    check_chunk(ag, *write_and_plan(str(tmp_path / "c.parquet"), rng, enc, nf, ver, 8000, data_page_size=ps))
 
 
 @gpu
 def test_dictionary_fallback_chunk_chained(ag, tmp_path):
     rng = np.random.default_rng(44)
-    path = str(tmp_path / "c.parquet")
-    tbl = BF.write_file(path, rng, "RLE_DICTIONARY", 0.1, "1.0", n=30_000, dictionary_pagesize_limit=2048)
-    plan = BF.chunk_plan(path)
-    assert B.PLAIN in {e for e, _ in plan["pages"]}
-    want, valid = BF.expected(tbl)
-    for ow, dev in ((4, False), (8, True)):
-        assert device_decode_chunk(ag, plan, valid, ow, dev) == want
+    tbl, plan = write_and_plan(str(tmp_path / "c.parquet"), rng, "RLE_DICTIONARY", 0.1, "1.0", 30_000, dictionary_pagesize_limit=2048)
+    assert B.PLAIN in P.encodings(plan)
+    check_chunk(ag, tbl, plan)
 
 
 @gpu
 @pytest.mark.parametrize("codec", ["snappy", "zstd"])
 def test_compressed_string_chunks(ag, codec, tmp_path):
-    import pq_snappy_files as SF
     rng = np.random.default_rng(45)
-    for enc in BF.ENCODINGS:
-        path = str(tmp_path / f"{enc}.parquet")
-        tbl = BF.write_file(path, rng, enc, 0.1, "2.0", n=20_000, compression=codec.upper())
-        want, valid = BF.expected(tbl)
-        chunk, pages = SF.column_chunk(path)
-        regions, comp, n_dst = SF.decompress_table(pages)
-        dsrc, ddst = Dev(SF.as_array(chunk)), Dev(nbytes=n_dst)
-        fn = "ag_parquet_snappy_decompress_dev" if codec == "snappy" else "ag_parquet_zstd_decompress_dev"
-        tab = [regions[k] for k in comp]
-        ag.call(fn, dsrc.ptr, N.compressed_table(tab), len(tab), ddst.ptr, None, None)
-        ag.call("ag_stream_sync", None)
-        dst = ddst.get(np.uint8, n_dst).tobytes()
-        for s, d, ln in [(r[0], r[2], r[3]) for k, r in enumerate(regions) if k not in comp]:
-            dst = dst[:d] + chunk[s:s + ln] + dst[d + ln:]
-        plan = {"data": dst + bytes(16), "dict": None, "pages": [], "n_slots": 0}
-        slot = 0
-        for pg, (s, sl, d, dl) in zip(pages, regions):
-            if pg["type"] == 2:
-                plan["dict"] = (d, dl, pg["num_values"])
-                continue
-            plan["pages"].append((pg["encoding"], (d, dl, pg["num_values"], slot)))
-            slot += pg["num_values"]
-        plan["n_slots"] = slot
-        assert device_decode_chunk(ag, plan, valid, 8) == want, enc
+    for enc in F.BA_ENCODINGS:
+        tbl, plan = write_and_plan(str(tmp_path / f"{enc}.parquet"), rng, enc, 0.1, "2.0", 20_000, compression=codec.upper())
+        assert plan["codec"] == codec.upper()
+        check_chunk(ag, tbl, plan, flavours=((8, False),))
 
 
 @gpu
@@ -311,7 +266,7 @@ def test_large_batch_checksum(ag):
     """32M short strings in 2^19-value PLAIN pages, dense: the data buffer through the device checksum"""
     rng = np.random.default_rng(46)
     per_page, n_pages = 1 << 19, 64
-    bodies = [BF.random_strings(rng, per_page) for _ in range(2)]
+    bodies = [F.random_strings(rng, per_page) for _ in range(2)]
     encs = [B.plain_encode(v) for v in bodies]
     blob, offs = bytearray(), []
     for e in encs:
@@ -328,13 +283,12 @@ def test_large_batch_checksum(ag):
             do.ptr, dout.ptr, total, C.byref(t), None, None, None)
     ag.call("ag_stream_sync", None)
     assert t.value == total
-    from test_gpu_parquet_pages import _mix
     data = b"".join(b"".join(bodies[p % 2]) for p in range(n_pages))
     words = np.frombuffer(data[:total // 8 * 8], np.uint64)
     res = Dev(np.zeros(1, np.uint64))
     ag.call("ag_checksum64_dev", dout.ptr, total // 8, res.ptr, None)
     ag.call("ag_stream_sync", None)
-    assert int(res.get()[0]) == int((_mix(np.arange(words.size, dtype=np.uint64)) * words).sum(dtype=np.uint64))
+    assert int(res.get()[0]) == checksum64(words)
     got_off = do.get(np.int64, n + 1)
     assert got_off[-1] == total and got_off[per_page] == lens[0]
 
@@ -346,7 +300,7 @@ def test_reference_vectors(ag, case, dev):
     """the reference's test vectors, each page after a good one: the oracle's outcome, byte for byte"""
     rng = np.random.default_rng(zlib.crc32(case["name"].encode()))
     enc = case["encoding"]
-    good = ENCODERS[enc](BF.random_strings(rng, 300))
+    good = ENCODERS[enc](F.random_strings(rng, 300))
     for ow in (4, 8):
         st, msg, errs, _, _ = compare(ag, enc, ow, [(good, 300), (bytes(case["bytes"]), case["num_values"])], rng, dev, gap=False)
         if case["error"] is None:

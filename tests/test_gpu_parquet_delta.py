@@ -7,12 +7,13 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_delta_files as DF
 import pq_delta_ref as D
 import pq_files as F
+import pq_pages as P
 from arrow_go_b200 import _native as N
-from helpers import Dev, ptr
-from test_gpu_parquet_pages import _mix, batch
+from helpers import Dev, checksum64, ptr
+from pq_chunk import read_chunk_dev
+from pq_pages import batch
 
 gpu = pytest.mark.gpu
 SHAPES = ((128, 4), (256, 4), (128, 1), (1024, 8), (4096, 1))   # values per miniblock 32, 64, 128, 128, 4096
@@ -192,44 +193,18 @@ def test_invalid_arguments(ag):
     assert st == N.AG_ERR_INVALID and "aligned" in msg
 
 
-def device_decode_delta_chunk(ag, path, dt):
-    """levels decode -> ag_parquet_def_levels_to_bitmap_dev -> delta decode, all on the device"""
-    plan = DF.delta_chunk_plan(path)
-    data = np.frombuffer(plan["data"], np.uint8).copy()
-    n = plan["n_slots"]
-    ddata = Dev(data)
-    dvalid = None
-    if plan["max_def"]:
-        dlv = Dev(nbytes=2 * n + 64)
-        dldec = Dev(np.zeros(len(plan["levels"]), np.int64))
-        enc = N.PQ_LEVELS_V1_RLE if plan["v1"] else N.PQ_LEVELS_V2_RLE
-        ag.call("ag_parquet_levels_decode_dev", plan["max_def"], enc, ddata.ptr, N.page_table(plan["levels"]), len(plan["levels"]),
-                dlv.ptr, dldec.ptr, None)
-        dvalid = Dev(nbytes=n // 8 + 64)
-        counts = Dev(np.zeros(2, np.int64))
-        ag.call("ag_parquet_def_levels_to_bitmap_dev", dlv.ptr, n, plan["max_def"], -1, dvalid.ptr, 0, n, counts.ptr, None)
-    dout = Dev(np.zeros(n, dt))
-    ddec = Dev(np.zeros(len(plan["delta"]), np.int64))
-    ag.call("ag_parquet_delta_decode_dev", np.dtype(dt).itemsize, ddata.ptr, N.page_table(plan["delta"]), len(plan["delta"]),
-            dvalid.ptr if dvalid else None, dout.ptr, ddec.ptr, None)
-    ag.call("ag_stream_sync", None)
-    assert ddec.get().tolist() == [p[2] for p in plan["delta"]]
-    valid = np.unpackbits(dvalid.get(np.uint8, n // 8 + 1), bitorder="little")[:n].astype(bool) if dvalid else np.ones(n, bool)
-    return dout.get(), valid, plan
-
-
 @gpu
-@pytest.mark.parametrize("case", DF.delta_cases(), ids=DF.delta_case_id)
+@pytest.mark.parametrize("case", F.delta_cases(), ids=F.case_id)
 def test_pyarrow_delta_files_end_to_end(ag, case, tmp_path):
-    t, nf, v, ps = case
-    rng = np.random.default_rng(zlib.crc32(DF.delta_case_id(case).encode()))
+    rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    tbl = DF.write_delta_file(path, rng, t, nf, v, data_page_size=ps)
-    want, wvalid = F.expected(tbl)
-    out, valid, plan = device_decode_delta_chunk(ag, path, want.dtype)
-    assert plan["delta"] and plan["other"] == []
+    tbl = F.write_numeric_case(path, rng, ("delta",) + case + (None,))
+    plan = P.chunk_plan(path)
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(tbl, plan)
+    assert P.encodings(plan) == {P.DELTA_BINARY_PACKED} and plan["dict"] is None
     assert np.array_equal(valid, wvalid)
-    assert out.tobytes() == want.tobytes()
+    assert values == want
 
 
 @gpu
@@ -275,5 +250,4 @@ def test_delta_decode_100m_values_device(ag):
     res = Dev(np.zeros(1, np.uint64))
     ag.call("ag_checksum64_dev", dout.ptr, n, res.ptr, None)
     ag.call("ag_stream_sync", None)
-    want_sum = int((_mix(np.arange(n, dtype=np.uint64)) * want_all.view(np.uint64)).sum(dtype=np.uint64))
-    assert int(res.get()[0]) == want_sum
+    assert int(res.get()[0]) == checksum64(want_all.view(np.uint64))

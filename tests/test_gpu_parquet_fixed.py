@@ -8,12 +8,14 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_fixed_files as FF
+import pq_files as F
 import pq_fixed_ref as X
+import pq_pages as P
 import pq_ref as R
 from arrow_go_b200 import _native as N
 from helpers import Dev, ptr
-from test_gpu_parquet_pages import batch
+from pq_chunk import read_chunk_dev
+from pq_pages import batch
 
 gpu = pytest.mark.gpu
 FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
@@ -267,72 +269,24 @@ def test_bool_errors(ag, dev):
 
 
 # -------------------------------------------------------------------------------------------------- end to end ----
-def device_chunk(ag, plan, valid):
-    """decompress a chunk on the device, then decode its dictionary and data pages -> (bytes of the output, dst)"""
-    n = plan["n_slots"]
-    dchunk = Dev(np.frombuffer(bytes(plan["chunk"]) + bytes(16), np.uint8).copy())
-    ddst = Dev(nbytes=plan["n_dst"])
-    if plan["codec"] == "UNCOMPRESSED":
-        for s, sl, d, dl in plan["comp"]:
-            if dl:
-                ag.call("ag_copy_dev", ddst.ptr + d, dchunk.ptr + s, dl, None)
-    elif plan["comp"]:
-        fn = {"SNAPPY": "ag_parquet_snappy_decompress_dev", "ZSTD": "ag_parquet_zstd_decompress_dev"}[plan["codec"]]
-        dw = Dev(np.zeros(len(plan["comp"]), np.int64))
-        ag.call(fn, dchunk.ptr, N.compressed_table(plan["comp"]), len(plan["comp"]), ddst.ptr, dw.ptr, None)
-    for s, d, k in plan["copies"]:
-        ag.call("ag_copy_dev", ddst.ptr + d, dchunk.ptr + s, k, None)
-    ag.call("ag_stream_sync", None)
-    dst = ddst.get(np.uint8, plan["n_dst"])
-    FF.value_sections(plan, dst)
-    dvalid = Dev(np.packbits(valid, bitorder="little")) if plan["max_def"] else None
-    vp = dvalid.ptr if dvalid else None
-    ptype, tl = plan["ptype"], plan["type_length"]
-    if ptype == 0:
-        dout = Dev(np.zeros(n // 8 + 8, np.uint8))
-        for enc in sorted({e for e, _ in plan["pages"]}):
-            pages = [p for e, p in plan["pages"] if e == enc]
-            ag.call("ag_parquet_bool_decode_dev", enc, ddst.ptr, N.page_table(pages), len(pages), vp, dout.ptr, None, None)
-        ag.call("ag_stream_sync", None)
-        return np.unpackbits(dout.get(), bitorder="little")[:n].astype(np.uint8).tobytes(), dst
-    width = X.width_of(ptype, tl)
-    dout = Dev(np.full(n * width, CANARY, np.uint8))
-    ddict = None
-    if plan["dict"]:
-        b, ln, nv = plan["dict"]
-        ddict = Dev(nbytes=nv * width + 8)
-        ag.call("ag_parquet_fixed_decode_dev", ptype, tl, X.PLAIN, ddst.ptr + b, N.page_table([(0, ln, nv, 0)]), 1, None, None, 0,
-                ddict.ptr, None, None, None)
-    groups = {}
-    for e, p in plan["pages"]:
-        groups.setdefault(X.RLE_DICTIONARY if e == X.PLAIN_DICTIONARY else e, []).append(p)
-    for enc, pages in groups.items():
-        dic = ddict.ptr if enc == X.RLE_DICTIONARY else None
-        dlen = plan["dict"][2] if enc == X.RLE_DICTIONARY else 0
-        ag.call("ag_parquet_fixed_decode_dev", ptype, tl, enc, ddst.ptr, N.page_table(pages), len(pages), vp, dic, dlen, dout.ptr, None, None, None)
-    ag.call("ag_stream_sync", None)
-    return dout.get().tobytes(), dst
-
-
-E2E = [(k, nf, v, c) for k in FF.KINDS for nf in (None, 0.1, 1.0) for v in ("1.0", "2.0") for c in ("NONE", "SNAPPY", "ZSTD")
+E2E = [(k, nf, v, c) for k in F.KINDS for nf in (None, 0.1, 1.0) for v in F.PAGE_VERSIONS for c in ("NONE", "SNAPPY", "ZSTD")
        if c == "NONE" or nf == 0.1]
 
 
 @gpu
-@pytest.mark.parametrize("case", E2E, ids=lambda c: f"{c[0]}-{'req' if c[1] is None else f'null{int(c[1] * 100)}'}-v{c[2][0]}-{c[3]}")
+@pytest.mark.parametrize("case", E2E, ids=lambda c: F.case_id(c[:3]) + "-" + c[3])
 def test_pyarrow_files_end_to_end(ag, case, tmp_path):
     kind, nf, ver, codec = case
     rng = np.random.default_rng(zlib.crc32(repr(case).encode()))
     path = str(tmp_path / "c.parquet")
-    n = 3000 if kind == "fsb1000" else 20_000
-    tbl = FF.write_file(path, rng, kind, nf, ver, n=n, data_page_size=8192, compression=codec,
-                        dictionary_pagesize_limit=2048 if kind.endswith("_dict") else None)
-    plan = FF.chunk_plan(path)
-    width = X.width_of(plan["ptype"], plan["type_length"]) if plan["ptype"] else 0
-    want, valid = FF.expected(tbl, plan["ptype"], width)
-    got, dst = device_chunk(ag, plan, valid)
-    assert dst.tobytes() == FF.host_decompress(plan, plan["codec"])
-    assert got == want.tobytes()
+    arr = F.make_array(rng, kind, 3000 if kind == "fsb1000" else 20_000, nf)
+    tbl = F.write_column(path, arr, nullable=nf is not None, encoding=F.KINDS[kind], version=ver, compression=codec,
+                         data_page_size=8192, dictionary_pagesize_limit=2048 if kind.endswith("_dict") else None)
+    plan = P.chunk_plan(path)
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(tbl, plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 @gpu
@@ -343,14 +297,11 @@ def test_golden_fixtures(ag, name, column):
     import pyarrow.parquet as pq
     path = os.path.join(GOLDEN, name)
     f = pq.ParquetFile(path)
-    idx = [f.schema.column(i).name for i in range(len(f.schema))].index(column)
-    tbl = pq.read_table(path, columns=[column], coerce_int96_timestamp_unit="ns")
-    plan = FF.chunk_plan(path, column=idx)
-    width = X.width_of(plan["ptype"], plan["type_length"]) if plan["ptype"] else 0
-    want, valid = FF.expected(tbl, plan["ptype"], width)
-    got, dst = device_chunk(ag, plan, valid)
-    assert dst.tobytes() == FF.host_decompress(plan, plan["codec"])
-    assert got == want.tobytes()
+    plan = P.chunk_plan(path, column=[f.schema.column(i).name for i in range(len(f.schema))].index(column))
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(pq.read_table(path, columns=[column], coerce_int96_timestamp_unit="ns"), plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 BIG = ["bss_double", "bss_double_spaced", "bss_flba16", "dict_flba16_spaced", "plain_int96_spaced", "plain_flba1000_spaced",

@@ -7,26 +7,14 @@ import numpy as np
 import pytest
 
 import pq_files as F
+import pq_pages as P
 import pq_ref as R
 from arrow_go_b200 import _native as N
-from helpers import Dev, ptr
+from helpers import Dev, checksum64, ptr
+from pq_chunk import read_chunk_dev
+from pq_pages import batch
 
 gpu = pytest.mark.gpu
-
-
-def batch(streams, rng, gap=True):
-    """Lay `streams` [(bytes, num_values)] out in one buffer at odd byte offsets, give each page an output range
-    (with gaps, at odd element offsets), and shuffle the page order.  Returns (blob, pages, n_out)."""
-    blob, pages, slot = bytearray(), [], 3 if gap else 0
-    for s, nv in streams:
-        if gap:
-            blob += bytes(int(rng.integers(0, 7)))
-        pages.append((len(blob), len(s), nv, slot))
-        blob += s
-        slot += nv + (int(rng.integers(0, 5)) if gap else 0)
-    blob += bytes(8)
-    order = rng.permutation(len(pages)) if gap else np.arange(len(pages))
-    return np.frombuffer(bytes(blob), np.uint8).copy(), [pages[i] for i in order], slot + 8
 
 
 def run_dict(ag, width, dictionary, blob, pages, n_out, valid=None, dev=False):
@@ -230,61 +218,19 @@ def test_error_cases(ag):
     assert st == N.AG_ERR_INVALID and "eof exception decode plain" in msg
 
 
-def device_decode_chunk(ag, path, dt):
-    """levels decode -> ag_parquet_def_levels_to_bitmap_dev -> dictionary / PLAIN spaced decode, all on the device"""
-    plan = F.chunk_plan(path)
-    data = np.frombuffer(plan["data"], np.uint8).copy()
-    n = plan["n_slots"]
-    ddata = Dev(data)
-    width = np.dtype(dt).itemsize
-    dvalid = None
-    if plan["max_def"]:
-        dlv = Dev(nbytes=2 * n + 64)
-        dldec = Dev(np.zeros(len(plan["levels"]), np.int64))
-        enc = N.PQ_LEVELS_V1_RLE if plan["v1"] else N.PQ_LEVELS_V2_RLE
-        ag.call("ag_parquet_levels_decode_dev", plan["max_def"], enc, ddata.ptr, N.page_table(plan["levels"]), len(plan["levels"]),
-                dlv.ptr, dldec.ptr, None)
-        assert dldec.get().tolist() == [p[2] for p in plan["levels"]]
-        dvalid = Dev(nbytes=n // 8 + 64)
-        counts = Dev(np.zeros(2, np.int64))
-        ag.call("ag_parquet_def_levels_to_bitmap_dev", dlv.ptr, n, plan["max_def"], -1, dvalid.ptr, 0, n, counts.ptr, None)
-    dout = Dev(np.zeros(n, dt))
-    if plan["dpages"]:
-        b, nv = plan["dict"]
-        dd = Dev(data[b:b + nv * width].copy())
-        ddec = Dev(np.zeros(len(plan["dpages"]), np.int64))
-        dbad = Dev(np.zeros(1, np.int64))
-        ag.call("ag_parquet_dict_decode_dev", width, dd.ptr, nv, ddata.ptr, N.page_table(plan["dpages"]), len(plan["dpages"]),
-                dvalid.ptr if dvalid else None, dout.ptr, ddec.ptr, dbad.ptr, None)
-        assert ddec.get().tolist() == [p[2] for p in plan["dpages"]] and dbad.get()[0] == N.NO_ERROR_POS
-    if plan["ppages"]:
-        ag.call("ag_parquet_plain_decode_spaced_dev", width, ddata.ptr, N.page_table(plan["ppages"]), len(plan["ppages"]),
-                dvalid.ptr if dvalid else None, dout.ptr, None)
-    ag.call("ag_stream_sync", None)
-    valid = np.unpackbits(dvalid.get(np.uint8, n // 8 + 1), bitorder="little")[:n].astype(bool) if dvalid else np.ones(n, bool)
-    return dout.get(), valid, plan
-
-
 @gpu
 @pytest.mark.parametrize("case", F.cases(), ids=F.case_id)
 def test_pyarrow_files_end_to_end(ag, case, tmp_path):
-    t, nf, v, ps, dl = case
     rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    tbl = F.write_file(path, rng, t, nf, v, data_page_size=ps, dict_limit=dl)
-    want, wvalid = F.expected(tbl)
-    out, valid, plan = device_decode_chunk(ag, path, want.dtype)
+    tbl = F.write_numeric_case(path, rng, ("dict",) + case)
+    plan = P.chunk_plan(path)
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(tbl, plan)
     assert np.array_equal(valid, wvalid)
-    assert out.tobytes() == want.tobytes()
-    if dl:
-        assert plan["ppages"]
-
-
-def _mix(i):
-    z = (i.astype(np.uint64) + np.uint64(0x9E3779B97F4A7C15))
-    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
-    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
-    return z ^ (z >> np.uint64(31))
+    assert values == want
+    if case[4]:
+        assert P.PLAIN in P.encodings(plan)
 
 
 @gpu
@@ -330,5 +276,4 @@ def test_dict_decode_100m_values_device(ag):
     res = Dev(np.zeros(1, np.uint64))
     ag.call("ag_checksum64_dev", dout.ptr, n, res.ptr, None)
     ag.call("ag_stream_sync", None)
-    want_sum = int((_mix(np.arange(n, dtype=np.uint64)) * want_all.view(np.uint64)).sum(dtype=np.uint64))
-    assert int(res.get()[0]) == want_sum
+    assert int(res.get()[0]) == checksum64(want_all.view(np.uint64))

@@ -9,14 +9,13 @@ import pyarrow as pa
 import pyarrow.parquet as pq
 import pytest
 
-import pq_delta_files as DF
 import pq_files as F
-import pq_snappy_files as Z
+import pq_pages as P
 import snappy_ref as S
 from arrow_go_b200 import _native as N
-from helpers import Dev, ptr
-from test_gpu_parquet_pages import _mix
-from test_snappy_oracle import corrupt_rows, forms
+from helpers import Dev, checksum64, ptr
+from pq_chunk import read_chunk_dev
+from pq_pages import compressed_batch
 
 gpu = pytest.mark.gpu
 FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
@@ -24,21 +23,6 @@ CANARY = 0xA5
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 FIXTURES = ("alltypes_plain.snappy.parquet", "datapage_v2.snappy.parquet", "datapage_v2_empty_datapage.snappy.parquet",
             "datapage_v1-snappy-compressed-checksum.parquet")
-
-
-def batch(streams, rng, gap=True):
-    """Lay `streams` [(bytes, dst_len)] out in one buffer at odd byte offsets, give each page an output range at odd
-    byte offsets with gaps between them, and shuffle the page order.  Returns (src, pages, n_out)."""
-    blob, pages, out = bytearray(), [], 3 if gap else 0
-    for s, n in streams:
-        if gap:
-            blob += bytes(int(rng.integers(0, 7)))
-        pages.append((len(blob), len(s), out, n))
-        blob += s
-        out += n + (int(rng.integers(1, 6)) if gap else 0)
-    blob += bytes(8)
-    order = rng.permutation(len(pages)) if gap else np.arange(len(pages))
-    return np.frombuffer(bytes(blob), np.uint8).copy(), [pages[i] for i in order], out + 8
 
 
 def run_snappy(ag, src, pages, n_out, dev=False):
@@ -69,7 +53,7 @@ def expect(src, pages, n_out):
 
 
 def decode_and_compare(ag, streams, rng, dev, gap=True):
-    src, pages, n_out = batch(streams, rng, gap)
+    src, pages, n_out = compressed_batch(streams, rng, gap)
     st, msg, out, w = run_snappy(ag, src, pages, n_out, dev)
     want, ww, errs = expect(src, pages, n_out)
     assert w.tolist() == ww, (msg, errs)
@@ -81,7 +65,7 @@ def decode_and_compare(ag, streams, rng, dev, gap=True):
 @FLAVOURS
 def test_every_element_form(ag, dev):
     rng = np.random.default_rng(61)
-    streams = [(s, len(x)) for _, s, x in forms()]
+    streams = [(s, len(x)) for _, s, x in S.forms()]
     for name, x in (("random", rng.integers(0, 256, 50_000, dtype=np.uint8).tobytes()), ("zeros", bytes(70_000)),
                     ("timestamps", (np.cumsum(rng.integers(0, 1000, 9000)) + (1 << 40)).astype(np.int64).tobytes())):
         streams.append((pa.compress(x, codec="snappy", asbytes=True), len(x)))
@@ -108,7 +92,7 @@ def test_page_sizes(ag, dev):
     big[1 << 23:(1 << 23) + (1 << 22)] = (np.cumsum(rng.integers(0, 1000, 1 << 19)) + (1 << 40)).astype(np.int64).tobytes()
     big = bytes(big)
     lit = S.stream(300_000, [S.literal(big[:300_000], 3)])       # one literal longer than the window
-    src, pages, n_out = batch([(pa.compress(big, codec="snappy", asbytes=True), len(big)), (lit, 300_000)], rng)
+    src, pages, n_out = compressed_batch([(pa.compress(big, codec="snappy", asbytes=True), len(big)), (lit, 300_000)], rng)
     st, msg, out, w = run_snappy(ag, src, pages, n_out, dev)
     assert st == N.AG_OK, msg
     for (s, sl, d, dl), k in zip(pages, w):
@@ -119,7 +103,7 @@ def test_page_sizes(ag, dev):
 
 
 def error_rows():
-    rows = [(name, s, n) for name, s, n, _ in corrupt_rows() if n < 1 << 32]
+    rows = [(name, s, n) for name, s, n, _ in S.corrupt_rows() if n < 1 << 32]
     good = S.stream(20, [S.literal(b"0123456789"), S.copy(10, 10, 1)])
     rows += [("size_mismatch_small", good, 19), ("size_mismatch_large", good, 21),
              ("size_mismatch_corrupt_body", S.stream(20, [S.literal(b"0123456789"), b"\xf0"]), 25),
@@ -136,7 +120,7 @@ def test_error_rows(ag, row, dev):
     x = rng.integers(0, 3, 5000, dtype=np.uint8).tobytes()
     good = pa.compress(x, codec="snappy", asbytes=True)
     # the failing page twice (pages 1 and 3 in the caller's order): the message names page 1
-    src, pages, n_out = batch([(good, len(x)), (s, n), (good, len(x)), (s, n)], rng, gap=False)
+    src, pages, n_out = compressed_batch([(good, len(x)), (s, n), (good, len(x)), (s, n)], rng, gap=False)
     st, msg, out, w = run_snappy(ag, src, pages, n_out, dev)
     want, ww, errs = expect(src, pages, n_out)
     assert [e[0] for e in errs] == [1, 3]
@@ -174,83 +158,18 @@ def test_invalid_arguments(ag, dev):
     assert st == N.AG_OK and w.tolist() == [12, 0, 12] and o[:24].tobytes() == b"abcdabcdabcd" * 2, msg
 
 
-def device_decode_snappy_chunk(ag, path, dt):
-    """upload the chunk once -> decompress -> levels / def levels to validity / dictionary / PLAIN / delta, on the device"""
-    plan = Z.snappy_chunk_plan(path)
-    n, width = plan["n_slots"], np.dtype(dt).itemsize
-    dchunk = Dev(Z.as_array(plan["chunk"]))
-    ddst = Dev(nbytes=plan["n_dst"])
-    dw = Dev(np.zeros(max(len(plan["comp"]), 1), np.int64))
-    ag.call("ag_parquet_snappy_decompress_dev", dchunk.ptr, N.compressed_table(plan["comp"]), len(plan["comp"]), ddst.ptr, dw.ptr, None)
-    for s, d, k in plan["copies"]:
-        ag.call("ag_copy_dev", ddst.ptr + d, dchunk.ptr + s, k, None)
-    ag.call("ag_stream_sync", None)
-    assert dw.get()[:len(plan["comp"])].tolist() == [c[3] for c in plan["comp"]]
-    dst = ddst.get(np.uint8, plan["n_dst"])
-    assert dst.tobytes() == Z.host_decompressed(plan)
-    Z.value_sections(plan, dst)
-    dvalid = None
-    if plan["max_def"]:
-        dlv = Dev(nbytes=2 * n + 64)
-        dldec = Dev(np.zeros(len(plan["levels"]), np.int64))
-        enc = N.PQ_LEVELS_V1_RLE if plan["v1"] else N.PQ_LEVELS_V2_RLE
-        lsrc = dchunk if plan["levels_in"] == "chunk" else ddst
-        ag.call("ag_parquet_levels_decode_dev", plan["max_def"], enc, lsrc.ptr, N.page_table(plan["levels"]), len(plan["levels"]),
-                dlv.ptr, dldec.ptr, None)
-        dvalid = Dev(nbytes=n // 8 + 64)
-        counts = Dev(np.zeros(2, np.int64))
-        ag.call("ag_parquet_def_levels_to_bitmap_dev", dlv.ptr, n, plan["max_def"], -1, dvalid.ptr, 0, n, counts.ptr, None)
-    vp = dvalid.ptr if dvalid else None
-    dout = Dev(np.zeros(n, dt))
-    if plan["dpages"]:
-        b, nv = plan["dict"]
-        ddec = Dev(np.zeros(len(plan["dpages"]), np.int64))
-        dbad = Dev(np.zeros(1, np.int64))
-        ag.call("ag_parquet_dict_decode_dev", width, ddst.ptr + b, nv, ddst.ptr, N.page_table(plan["dpages"]), len(plan["dpages"]),
-                vp, dout.ptr, ddec.ptr, dbad.ptr, None)
-        ag.call("ag_stream_sync", None)
-        assert ddec.get().tolist() == [p[2] for p in plan["dpages"]] and dbad.get()[0] == N.NO_ERROR_POS
-    if plan["ppages"]:
-        ag.call("ag_parquet_plain_decode_spaced_dev", width, ddst.ptr, N.page_table(plan["ppages"]), len(plan["ppages"]), vp, dout.ptr, None)
-    if plan["delta"]:
-        ag.call("ag_parquet_delta_decode_dev", width, ddst.ptr, N.page_table(plan["delta"]), len(plan["delta"]), vp, dout.ptr, None, None)
-    ag.call("ag_stream_sync", None)
-    assert plan["other"] == []
-    valid = np.unpackbits(dvalid.get(np.uint8, n // 8 + 1), bitorder="little")[:n].astype(bool) if dvalid else np.ones(n, bool)
-    return dout.get(), valid, plan
-
-
-def snappy_cases():
-    """pq_files.cases() shapes (dictionary / PLAIN fallback) plus DELTA_BINARY_PACKED files, v1 and v2"""
-    return [("dict",) + c for c in F.cases()] + [("delta",) + c + (None,) for c in DF.delta_cases()]
-
-
-def snappy_case_id(c):
-    return c[0] + "-" + (F.case_id(c[1:]) if c[0] == "dict" else DF.delta_case_id(c[1:5]))
-
-
 @gpu
-@pytest.mark.parametrize("case", snappy_cases(), ids=snappy_case_id)
+@pytest.mark.parametrize("case", F.compressed_cases(), ids=F.compressed_case_id)
 def test_pyarrow_snappy_files_end_to_end(ag, case, tmp_path):
-    kind, t, nf, v, ps, dl = case
-    rng = np.random.default_rng(zlib.crc32(snappy_case_id(case).encode()))
+    rng = np.random.default_rng(zlib.crc32(F.compressed_case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    if kind == "dict":
-        col, at = F.make_column(rng, t, 20_000, nf, 300)
-        tbl = pa.Table.from_arrays([col], schema=pa.schema([pa.field("c", at, nullable=nf is not None)]))
-        kw = {"dictionary_pagesize_limit": dl} if dl else {}
-        pq.write_table(tbl, path, compression="SNAPPY", use_dictionary=True, data_page_version=v,
-                       **({"data_page_size": ps} if ps else {}), **kw)
-    else:
-        DF.write_delta_file(str(tmp_path / "plain.parquet"), rng, t, nf, v, data_page_size=ps)
-        tbl = pq.read_table(str(tmp_path / "plain.parquet"))
-        Z.write_snappy_file(path, tbl, v, use_dictionary=False, column_encoding={"c": "DELTA_BINARY_PACKED"}, data_page_size=ps)
-    assert pq.ParquetFile(path).metadata.row_group(0).column(0).compression == "SNAPPY"
-    want, wvalid = F.expected(pq.read_table(path))
-    out, valid, plan = device_decode_snappy_chunk(ag, path, want.dtype)
+    tbl = F.write_numeric_case(path, rng, case, compression="SNAPPY")
+    plan = P.chunk_plan(path)
+    assert plan["codec"] == "SNAPPY" and (P.DELTA_BINARY_PACKED in P.encodings(plan)) == (case[0] == "delta")
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(tbl, plan)
     assert np.array_equal(valid, wvalid)
-    assert out.tobytes() == want.tobytes()
-    assert plan["delta"] if kind == "delta" else plan["dpages"] or plan["ppages"]
+    assert values == want
 
 
 @gpu
@@ -261,10 +180,10 @@ def test_fixture_pages_against_host(ag, name, dev):
     path = os.path.join(GOLDEN, name)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
     for c in range(pq.ParquetFile(path).metadata.num_columns):
-        chunk, pages = Z.column_chunk(path, column=c)
-        regions, comp, n_dst = Z.decompress_table(pages)
+        chunk, pages = P.column_chunk(path, column=c)
+        regions, comp, n_dst = P.decompress_table(pages)
         streams = [(chunk[regions[k][0]:regions[k][0] + regions[k][1]], regions[k][3]) for k in comp]
-        src, tbl, n_out = batch(streams, rng)
+        src, tbl, n_out = compressed_batch(streams, rng)
         st, msg, out, w = run_snappy(ag, src, tbl, n_out, dev)
         assert st == N.AG_OK, (c, msg)
         for (s, sl, d, dl), k in zip(tbl, w):
@@ -302,5 +221,4 @@ def test_decompress_200mb_device(ag):
     res = Dev(np.zeros(1, np.uint64))
     ag.call("ag_checksum64_dev", dout.ptr, allw.size, res.ptr, None)
     ag.call("ag_stream_sync", None)
-    want_sum = int((_mix(np.arange(allw.size, dtype=np.uint64)) * allw).sum(dtype=np.uint64))
-    assert int(res.get()[0]) == want_sum
+    assert int(res.get()[0]) == checksum64(allw)

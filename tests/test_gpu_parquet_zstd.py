@@ -9,15 +9,13 @@ import pyarrow as pa
 import pyarrow.parquet as pq
 import pytest
 
-import pq_delta_files as DF
 import pq_files as F
-import pq_snappy_files as Z
+import pq_pages as P
 import zstd_ref as R
 from arrow_go_b200 import _native as N
-from helpers import Dev, ptr
-from test_gpu_parquet_pages import _mix
-from test_gpu_parquet_snappy import batch, snappy_case_id, snappy_cases
-from test_zstd_oracle import corrupt_rows, forms, golden_payload
+from helpers import Dev, checksum64, ptr
+from pq_chunk import read_chunk_dev
+from pq_pages import compressed_batch
 
 gpu = pytest.mark.gpu
 FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
@@ -53,7 +51,7 @@ def expect(src, pages, n_out):
 
 
 def decode_and_compare(ag, streams, rng, dev, gap=True):
-    src, pages, n_out = batch(streams, rng, gap)
+    src, pages, n_out = compressed_batch(streams, rng, gap)
     st, msg, out, w = run_zstd(ag, src, pages, n_out, dev)
     want, ww, errs = expect(src, pages, n_out)
     assert w.tolist() == ww, (msg, errs)
@@ -65,9 +63,9 @@ def decode_and_compare(ag, streams, rng, dev, gap=True):
 @FLAVOURS
 def test_every_form(ag, dev):
     rng = np.random.default_rng(81)
-    streams = [(s, len(x)) for _, s, x in forms()]
+    streams = [(s, len(x)) for _, s, x in R.forms()]
     for name in ("zstd_checksum.zst", "zstd_no_content_size.zst"):
-        streams.append((open(os.path.join(GOLDEN, name), "rb").read(), len(golden_payload())))
+        streams.append((open(os.path.join(GOLDEN, name), "rb").read(), len(R.golden_payload())))
     for gap in (True, False):
         st, msg, errs, _ = decode_and_compare(ag, streams, rng, dev, gap)
         assert st == N.AG_OK and not errs, msg
@@ -88,7 +86,7 @@ def test_page_sizes(ag, dev):
 
 
 def error_rows():
-    rows = [(name, s, n) for name, s, n, _ in corrupt_rows()]
+    rows = [(name, s, n) for name, s, n, _ in R.corrupt_rows()]
     x = b"0123456789" * 100
     good = pa.compress(x, codec="zstd", asbytes=True)
     nofcs = R.reframe(good, fcs=False)
@@ -107,7 +105,7 @@ def test_error_rows(ag, row, dev):
     x = rng.integers(0, 3, 5000, dtype=np.uint8).tobytes()
     good = pa.compress(x, codec="zstd", asbytes=True)
     # the failing page twice (pages 1 and 3 in the caller's order): the message names page 1
-    src, pages, n_out = batch([(good, len(x)), (s, n), (good, len(x)), (s, n)], rng, gap=False)
+    src, pages, n_out = compressed_batch([(good, len(x)), (s, n), (good, len(x)), (s, n)], rng, gap=False)
     st, msg, out, w = run_zstd(ag, src, pages, n_out, dev)
     want, ww, errs = expect(src, pages, n_out)
     assert [e[0] for e in errs] == [1, 3]
@@ -143,78 +141,18 @@ def test_invalid_arguments(ag, dev):
     assert st == N.AG_OK and w.tolist() == [12, 0, 12] and o[:24].tobytes() == b"abcdabcdabcd" * 2, msg
 
 
-def host_decompressed(plan):
-    out = bytearray(plan["n_dst"])
-    for s, sl, d, dl in plan["comp"]:
-        if dl:
-            out[d:d + dl] = pa.decompress(plan["chunk"][s:s + sl], decompressed_size=dl, codec="zstd", asbytes=True)
-    for s, d, n in plan["copies"]:
-        out[d:d + n] = plan["chunk"][s:s + n]
-    return bytes(out)
-
-
 @gpu
-@pytest.mark.parametrize("case", snappy_cases(), ids=snappy_case_id)
+@pytest.mark.parametrize("case", F.compressed_cases(), ids=F.compressed_case_id)
 def test_pyarrow_zstd_files_end_to_end(ag, case, tmp_path):
-    """the ZSTD chunk flow: upload once, one ag_parquet_zstd_decompress_dev call, then the unchanged page decoders"""
-    kind, t, nf, v, ps, dl = case
-    rng = np.random.default_rng(zlib.crc32(snappy_case_id(case).encode()))
+    rng = np.random.default_rng(zlib.crc32(F.compressed_case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    if kind == "dict":
-        col, at = F.make_column(rng, t, 20_000, nf, 300)
-        tbl = pa.Table.from_arrays([col], schema=pa.schema([pa.field("c", at, nullable=nf is not None)]))
-        kw = {"dictionary_pagesize_limit": dl} if dl else {}
-        pq.write_table(tbl, path, compression="ZSTD", use_dictionary=True, data_page_version=v,
-                       **({"data_page_size": ps} if ps else {}), **kw)
-    else:
-        DF.write_delta_file(str(tmp_path / "plain.parquet"), rng, t, nf, v, data_page_size=ps)
-        tbl = pq.read_table(str(tmp_path / "plain.parquet"))
-        pq.write_table(tbl, path, compression="ZSTD", use_dictionary=False, data_page_version=v,
-                       column_encoding={"c": "DELTA_BINARY_PACKED"}, **({"data_page_size": ps} if ps else {}))
-    assert pq.ParquetFile(path).metadata.row_group(0).column(0).compression == "ZSTD"
-    want, wvalid = F.expected(pq.read_table(path))
-    plan = Z.snappy_chunk_plan(path)                             # the chunk walk is codec-agnostic
-    n, width, dt = plan["n_slots"], np.dtype(want.dtype).itemsize, want.dtype
-    dchunk = Dev(Z.as_array(plan["chunk"]))
-    ddst = Dev(nbytes=plan["n_dst"])
-    dw = Dev(np.zeros(max(len(plan["comp"]), 1), np.int64))
-    ag.call("ag_parquet_zstd_decompress_dev", dchunk.ptr, N.compressed_table(plan["comp"]), len(plan["comp"]), ddst.ptr, dw.ptr, None)
-    for s, d, k in plan["copies"]:
-        ag.call("ag_copy_dev", ddst.ptr + d, dchunk.ptr + s, k, None)
-    ag.call("ag_stream_sync", None)
-    assert dw.get()[:len(plan["comp"])].tolist() == [c[3] for c in plan["comp"]]
-    dst = ddst.get(np.uint8, plan["n_dst"])
-    assert dst.tobytes() == host_decompressed(plan)
-    Z.value_sections(plan, dst)
-    dvalid = None
-    if plan["max_def"]:
-        dlv = Dev(nbytes=2 * n + 64)
-        dldec = Dev(np.zeros(len(plan["levels"]), np.int64))
-        enc = N.PQ_LEVELS_V1_RLE if plan["v1"] else N.PQ_LEVELS_V2_RLE
-        lsrc = dchunk if plan["levels_in"] == "chunk" else ddst
-        ag.call("ag_parquet_levels_decode_dev", plan["max_def"], enc, lsrc.ptr, N.page_table(plan["levels"]), len(plan["levels"]),
-                dlv.ptr, dldec.ptr, None)
-        dvalid = Dev(nbytes=n // 8 + 64)
-        counts = Dev(np.zeros(2, np.int64))
-        ag.call("ag_parquet_def_levels_to_bitmap_dev", dlv.ptr, n, plan["max_def"], -1, dvalid.ptr, 0, n, counts.ptr, None)
-    vp = dvalid.ptr if dvalid else None
-    dout = Dev(np.zeros(n, dt))
-    if plan["dpages"]:
-        b, nv = plan["dict"]
-        ddec = Dev(np.zeros(len(plan["dpages"]), np.int64))
-        dbad = Dev(np.zeros(1, np.int64))
-        ag.call("ag_parquet_dict_decode_dev", width, ddst.ptr + b, nv, ddst.ptr, N.page_table(plan["dpages"]), len(plan["dpages"]),
-                vp, dout.ptr, ddec.ptr, dbad.ptr, None)
-    if plan["ppages"]:
-        ag.call("ag_parquet_plain_decode_spaced_dev", width, ddst.ptr, N.page_table(plan["ppages"]), len(plan["ppages"]), vp, dout.ptr, None)
-    if plan["delta"]:
-        ag.call("ag_parquet_delta_decode_dev", width, ddst.ptr, N.page_table(plan["delta"]), len(plan["delta"]), vp, dout.ptr, None, None)
-    ag.call("ag_stream_sync", None)
-    assert plan["other"] == []
-    valid = np.unpackbits(dvalid.get(np.uint8, n // 8 + 1), bitorder="little")[:n].astype(bool) if dvalid else np.ones(n, bool)
+    tbl = F.write_numeric_case(path, rng, case, compression="ZSTD")
+    plan = P.chunk_plan(path)
+    assert plan["codec"] == "ZSTD" and (P.DELTA_BINARY_PACKED in P.encodings(plan)) == (case[0] == "delta")
+    values, valid = read_chunk_dev(ag, plan)
+    want, wvalid = F.expected(tbl, plan)
     assert np.array_equal(valid, wvalid)
-    assert dout.get().tobytes() == want.tobytes()
-    assert plan["delta"] if kind == "delta" else plan["dpages"] or plan["ppages"]
+    assert values == want
 
 
 @gpu
@@ -224,11 +162,11 @@ def test_fixture_pages_against_host(ag, dev):
     path = os.path.join(GOLDEN, "byte_stream_split.zstd.parquet")
     rng = np.random.default_rng(83)
     for c in range(pq.ParquetFile(path).metadata.num_columns):
-        chunk, pages = Z.column_chunk(path, column=c)
-        regions, comp, n_dst = Z.decompress_table(pages)
+        chunk, pages = P.column_chunk(path, column=c)
+        regions, comp, n_dst = P.decompress_table(pages)
         streams = [(chunk[regions[k][0]:regions[k][0] + regions[k][1]], regions[k][3]) for k in comp]
         assert streams
-        src, tbl, n_out = batch(streams, rng)
+        src, tbl, n_out = compressed_batch(streams, rng)
         st, msg, out, w = run_zstd(ag, src, tbl, n_out, dev)
         assert st == N.AG_OK, (c, msg)
         for (s, sl, d, dl), k in zip(tbl, w):
@@ -267,5 +205,4 @@ def test_decompress_200mb_device(ag):
     res = Dev(np.zeros(1, np.uint64))
     ag.call("ag_checksum64_dev", dout.ptr, allw.size, res.ptr, None)
     ag.call("ag_stream_sync", None)
-    want_sum = int((_mix(np.arange(allw.size, dtype=np.uint64)) * allw).sum(dtype=np.uint64))
-    assert int(res.get()[0]) == want_sum
+    assert int(res.get()[0]) == checksum64(allw)

@@ -7,55 +7,45 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_bytearray_files as BF
 import pq_bytearray_ref as B
+import pq_files as F
+import pq_pages as P
+from pq_chunk import read_chunk_oracle
 
 
-def oracle_chunk(plan, valid):
-    """decode every page of a chunk with the oracle -> slot values"""
-    data = plan["data"]
-    dictionary = None
-    if plan["dict"]:
-        b, ln, nv = plan["dict"]
-        dictionary, slots, msg = B.plain_decode(data[b:b + ln], nv)
-        assert msg is None and slots == nv
-    out = [b""] * plan["n_slots"]
-    for enc, (b, ln, nv, o) in plan["pages"]:
-        v = valid[o:o + nv].copy() if not valid.all() else nv
-        vals, slots, msg, bad = B.decode(enc, data[b:b + ln], v, dictionary)
-        assert msg is None and bad is None and slots == nv, (enc, msg)
-        out[o:o + nv] = vals
-    return out
+def write_and_read(path, rng, enc, nf, version, n, **kw):
+    """write one string case, read it back through the oracle -> (plan, values, validity, table)"""
+    tbl = F.write_column(path, F.make_string_column(rng, enc, n, nf), nullable=nf is not None, encoding=enc, version=version, **kw)
+    plan = P.chunk_plan(path)
+    return (plan, *read_chunk_oracle(plan, P.host_decompress(plan)), tbl)
 
 
-@pytest.mark.parametrize("case", BF.cases(), ids=BF.case_id)
+@pytest.mark.parametrize("case", F.ba_cases(), ids=F.case_id)
 def test_oracle_matches_pyarrow(case, tmp_path):
     enc, nf, ver, ps = case
-    rng = np.random.default_rng(zlib.crc32(BF.case_id(case).encode()))
-    path = str(tmp_path / "c.parquet")
-    tbl = BF.write_file(path, rng, enc, nf, ver, n=5000, data_page_size=ps)
-    plan = BF.chunk_plan(path)
-    want, valid = BF.expected(tbl)
-    encs = {e for e, _ in plan["pages"]}
-    assert encs <= {B.PLAIN, B.PLAIN_DICTIONARY, B.RLE_DICTIONARY, B.DELTA_LENGTH_BYTE_ARRAY, B.DELTA_BYTE_ARRAY}
-    assert oracle_chunk(plan, valid) == want
+    rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
+    plan, values, valid, tbl = write_and_read(str(tmp_path / "c.parquet"), rng, enc, nf, ver, 5000, data_page_size=ps)
+    assert P.encodings(plan) <= {B.PLAIN, B.PLAIN_DICTIONARY, B.RLE_DICTIONARY, B.DELTA_LENGTH_BYTE_ARRAY, B.DELTA_BYTE_ARRAY}
+    want, wvalid = F.expected(tbl, plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 def test_oracle_dictionary_fallback_chunk(tmp_path):
     rng = np.random.default_rng(5)
-    path = str(tmp_path / "c.parquet")
-    tbl = BF.write_file(path, rng, "RLE_DICTIONARY", 0.1, "1.0", n=30_000, dictionary_pagesize_limit=2048)
-    plan = BF.chunk_plan(path)
-    encs = [e for e, _ in plan["pages"]]
+    plan, values, valid, tbl = write_and_read(str(tmp_path / "c.parquet"), rng, "RLE_DICTIONARY", 0.1, "1.0", 30_000,
+                                              dictionary_pagesize_limit=2048)
+    encs = P.encodings(plan)
     assert plan["dict"] and B.PLAIN in encs and (B.RLE_DICTIONARY in encs or B.PLAIN_DICTIONARY in encs)
-    want, valid = BF.expected(tbl)
-    assert oracle_chunk(plan, valid) == want
+    want, wvalid = F.expected(tbl, plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 @pytest.mark.parametrize("enc", [B.PLAIN, B.DELTA_LENGTH_BYTE_ARRAY, B.DELTA_BYTE_ARRAY])
 def test_round_trip(enc):
     rng = np.random.default_rng(enc)
-    vals = BF.random_strings(rng, 3000) + [b"", b"x" * 20_000] + BF.random_strings(rng, 500, sorted_keys=True)
+    vals = F.random_strings(rng, 3000) + [b"", b"x" * 20_000] + F.random_strings(rng, 500, sorted_keys=True)
     page = {B.PLAIN: B.plain_encode, B.DELTA_LENGTH_BYTE_ARRAY: B.dlba_encode, B.DELTA_BYTE_ARRAY: B.dba_encode}[enc](vals)
     out, slots, msg, _ = B.decode(enc, page, len(vals))
     assert msg is None and slots == len(vals) and out == vals

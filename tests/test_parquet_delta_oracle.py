@@ -8,10 +8,10 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_delta_files as DF
 import pq_delta_ref as D
 import pq_files as F
-import pq_ref as R
+import pq_pages as P
+from pq_chunk import read_chunk_oracle
 
 GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "parquet_delta.json")))
 
@@ -111,40 +111,22 @@ def test_chain_error_keeps_earlier_miniblocks():
     assert err == D.DERR_WIDTH and slots == 2 * 65 + 1 and out[1::2].tolist() == vals[:65].tolist() and not out[0::2].any()
 
 
-def decode_chunk_oracle(path):
-    plan = DF.delta_chunk_plan(path)
-    import pyarrow.parquet as pq
-    dt = np.dtype(pq.read_schema(path).field(0).type.to_pandas_dtype())
-    data, n = plan["data"], plan["n_slots"]
-    valid = np.ones(n, bool)
-    for (b, ln, nv, o) in plan["levels"]:
-        lv, err = R.levels_decode_page(data[b:b + ln], plan["max_def"], plan["v1"], nv)
-        assert err == R.ERR_NONE and lv.size == nv
-        valid[o:o + nv] = lv >= plan["max_def"]
-    out = np.zeros(n, dt)
-    for (b, ln, nv, o) in plan["delta"]:
-        v = valid[o:o + nv].copy() if plan["max_def"] else nv
-        vals, slots, err, msg = D.delta_decode(data[b:b + ln], dt.itemsize, v)
-        assert err == D.DERR_NONE and slots == nv, msg
-        out[o:o + nv] = vals
-    return out, valid, plan
-
-
-@pytest.mark.parametrize("case", DF.delta_cases(), ids=DF.delta_case_id)
+@pytest.mark.parametrize("case", F.delta_cases(), ids=F.case_id)
 def test_oracle_decodes_pyarrow_delta_files(case, tmp_path):
     t, nf, v, ps = case
-    rng = np.random.default_rng(zlib.crc32(DF.delta_case_id(case).encode()))
+    rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    tbl = DF.write_delta_file(path, rng, t, nf, v, data_page_size=ps)
-    out, valid, plan = decode_chunk_oracle(path)
-    want, wvalid = F.expected(tbl)
-    assert plan["other"] == [] and plan["delta"]
+    tbl = F.write_numeric_case(path, rng, ("delta",) + case + (None,))
+    plan = P.chunk_plan(path)
+    dst = P.host_decompress(plan)
+    values, valid = read_chunk_oracle(plan, dst)
+    want, wvalid = F.expected(tbl, plan)
+    assert P.encodings(plan) == {P.DELTA_BINARY_PACKED} and plan["dict"] is None
     assert np.array_equal(valid, wvalid)
-    assert out.tobytes() == want.tobytes()
+    assert values == want
     if ps and nf != 1.0:
-        assert len(plan["delta"]) > 3
+        assert len(plan["pages"]) > 3
     # pyarrow's block shape: 128/4 for INT32, 256/4 for INT64
-    b, ln, nv, o = plan["delta"][0]
-    block, pos = D._uvarint(plan["data"], b)
-    assert (block, plan["data"][pos]) == ((128 if t == "int32" else 256), 4)
-
+    _, (b, ln, nv, o) = P.value_sections(plan, dst)[0]
+    block, pos = D._uvarint(dst, b)
+    assert (block, dst[pos]) == ((128 if t == "int32" else 256), 4)

@@ -7,75 +7,50 @@ import zlib
 import numpy as np
 import pytest
 
-import pq_fixed_files as FF
+import pq_files as F
 import pq_fixed_ref as X
+import pq_pages as P
 import pq_ref as R
+from pq_chunk import read_chunk_oracle
 from arrow_go_b200 import _native as N
 
 
-def oracle_chunk(plan, dst, valid):
-    """decode every page of a chunk with the oracle -> (slot values, lowest message)"""
-    width = X.width_of(plan["ptype"], plan["type_length"]) if plan["ptype"] else 0
-    dictionary = None
-    if plan["dict"]:
-        b, ln, nv = plan["dict"]
-        dictionary, slots, msg, _ = X.fixed_decode(plan["ptype"], width, X.PLAIN, dst[b:b + ln], nv)
-        assert msg is None and slots == nv
-    n = plan["n_slots"]
-    out = np.zeros(n, np.uint8) if not width else np.zeros((n, width), np.uint8)
-    for enc, (b, ln, nv, o) in plan["pages"]:
-        v = valid[o:o + nv].copy() if plan["max_def"] else nv
-        if plan["ptype"] == 0:
-            vals, slots, msg = X.bool_decode(enc, dst[b:b + ln], v)
-        else:
-            vals, slots, msg, bad = X.fixed_decode(plan["ptype"], width, enc, dst[b:b + ln], v, dictionary)
-            assert bad is None
-        assert msg is None and slots == nv, (enc, msg)
-        out[o:o + nv] = vals
-    return out
+def write_and_read(path, rng, kind, nf, version, n, **kw):
+    """write one fixed-width case, read it back through the oracle -> (plan, values, validity, table)"""
+    tbl = F.write_column(path, F.make_array(rng, kind, n, nf), nullable=nf is not None, encoding=F.KINDS[kind], version=version, **kw)
+    plan = P.chunk_plan(path)
+    return (plan, *read_chunk_oracle(plan, P.host_decompress(plan)), tbl)
 
 
-CASES = [(k, nf, v) for k, nf, v in itertools.product(FF.KINDS, FF.NULL_FRACS, ("1.0", "2.0"))]
+CASES = [(k, nf, v) for k, nf, v in itertools.product(F.KINDS, F.FIXED_NULL_FRACS, F.PAGE_VERSIONS)]
 
 
-def case_id(c):
-    k, nf, v = c
-    return f"{k}-{'req' if nf is None else f'null{int(nf * 100)}'}-v{v[0]}"
-
-
-@pytest.mark.parametrize("case", CASES, ids=case_id)
+@pytest.mark.parametrize("case", CASES, ids=F.case_id)
 def test_oracle_matches_pyarrow(case, tmp_path):
     kind, nf, ver = case
-    rng = np.random.default_rng(zlib.crc32(case_id(case).encode()))
-    path = str(tmp_path / "c.parquet")
-    n = 600 if kind == "fsb1000" else 3000
-    tbl = FF.write_file(path, rng, kind, nf, ver, n=n, data_page_size=512)
-    plan = FF.chunk_plan(path)
-    dst = FF.host_decompress(plan, plan["codec"])
-    FF.value_sections(plan, dst)
-    width = X.width_of(plan["ptype"], plan["type_length"]) if plan["ptype"] else 0
-    want, valid = FF.expected(tbl, plan["ptype"], width)
-    encs = {e for e, _ in plan["pages"]}
+    rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
+    plan, values, valid, tbl = write_and_read(str(tmp_path / "c.parquet"), rng, kind, nf, ver, 600 if kind == "fsb1000" else 3000,
+                                              data_page_size=512)
+    encs = P.encodings(plan)
     if kind == "bool":
         assert encs == ({X.PLAIN} if ver == "1.0" else {X.RLE})
-    elif FF.KINDS[kind] == "BYTE_STREAM_SPLIT":
+    elif F.KINDS[kind] == "BYTE_STREAM_SPLIT":
         assert encs == {X.BYTE_STREAM_SPLIT}
-    assert oracle_chunk(plan, dst, valid).tobytes() == want.tobytes()
+    want, wvalid = F.expected(tbl, plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 @pytest.mark.parametrize("kind", ["fsb16_dict", "int96_dict"])
 def test_oracle_dictionary_fallback_chunk(kind, tmp_path):
     rng = np.random.default_rng(7)
-    path = str(tmp_path / "c.parquet")
-    tbl = FF.write_file(path, rng, kind, 0.1, "1.0", n=20_000, data_page_size=4096, dictionary_pagesize_limit=1024)
-    plan = FF.chunk_plan(path)
-    dst = FF.host_decompress(plan, plan["codec"])
-    FF.value_sections(plan, dst)
-    encs = [e for e, _ in plan["pages"]]
+    plan, values, valid, tbl = write_and_read(str(tmp_path / "c.parquet"), rng, kind, 0.1, "1.0", 20_000, data_page_size=4096,
+                                              dictionary_pagesize_limit=1024)
+    encs = P.encodings(plan)
     assert plan["dict"] and X.PLAIN in encs and (X.RLE_DICTIONARY in encs or X.PLAIN_DICTIONARY in encs)
-    width = X.width_of(plan["ptype"], plan["type_length"])
-    want, valid = FF.expected(tbl, plan["ptype"], width)
-    assert oracle_chunk(plan, dst, valid).tobytes() == want.tobytes()
+    want, wvalid = F.expected(tbl, plan)
+    assert np.array_equal(valid, wvalid)
+    assert values == want
 
 
 def test_round_trips_and_run_forms():

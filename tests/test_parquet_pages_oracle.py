@@ -9,7 +9,9 @@ import numpy as np
 import pytest
 
 import pq_files as F
+import pq_pages as P
 import pq_ref as R
+from pq_chunk import read_chunk_oracle
 
 GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "parquet_rle.json")))
 
@@ -82,46 +84,17 @@ def test_error_cases():
     assert err == R.ERR_NONE and bad == 4 and out[4] == 0 and slots == 8
 
 
-def decode_chunk_oracle(path):
-    """Every page of the chunk through the oracle: levels -> validity -> dictionary / PLAIN values"""
-    plan = F.chunk_plan(path)
-    data = plan["data"]
-    n = plan["n_slots"]
-    dictionary = None
-    import pyarrow.parquet as pq
-    dt = np.dtype(pq.read_schema(path).field(0).type.to_pandas_dtype())
-    if plan["dict"]:
-        b, nv = plan["dict"]
-        dictionary = np.frombuffer(data[b:b + nv * dt.itemsize], dtype=dt)
-    valid = np.ones(n, bool)
-    for (b, ln, nv, o) in plan["levels"]:
-        lv, err = R.levels_decode_page(data[b:b + ln], plan["max_def"], plan["v1"], nv)
-        assert err == R.ERR_NONE and lv.size == nv
-        valid[o:o + nv] = lv >= plan["max_def"]
-    out = np.zeros(n, dt)
-    for (b, ln, nv, o) in plan["dpages"]:
-        v = valid[o:o + nv] if plan["max_def"] else nv
-        vals, slots, err, bad = R.dict_decode(data[b:b + ln], dictionary, v)
-        assert err == R.ERR_NONE and bad is None and slots == nv
-        out[o:o + nv] = vals
-    for (b, ln, nv, o) in plan["ppages"]:
-        vals, err = R.plain_decode_spaced(data[b:b + ln], dt, valid[o:o + nv])
-        assert err == R.ERR_NONE
-        out[o:o + nv] = vals
-    return out, valid, plan
-
-
 @pytest.mark.parametrize("case", F.cases(), ids=F.case_id)
 def test_oracle_decodes_pyarrow_files(case, tmp_path):
-    t, nf, v, ps, dl = case
     rng = np.random.default_rng(zlib.crc32(F.case_id(case).encode()))
     path = str(tmp_path / "c.parquet")
-    tbl = F.write_file(path, rng, t, nf, v, data_page_size=ps, dict_limit=dl)
-    out, valid, plan = decode_chunk_oracle(path)
-    want, wvalid = F.expected(tbl)
+    tbl = F.write_numeric_case(path, rng, ("dict",) + case)
+    plan = P.chunk_plan(path)
+    values, valid = read_chunk_oracle(plan, P.host_decompress(plan))
+    want, wvalid = F.expected(tbl, plan)
     assert np.array_equal(valid, wvalid)
-    assert out.tobytes() == want.tobytes()
-    if ps:
-        assert len(plan["dpages"]) + len(plan["ppages"]) > 3
-    if dl:
-        assert plan["ppages"], "no PLAIN fallback page was written"
+    assert values == want
+    if case[3]:
+        assert len(plan["pages"]) > 3
+    if case[4]:
+        assert P.PLAIN in P.encodings(plan), "no PLAIN fallback page was written"

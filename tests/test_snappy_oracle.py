@@ -33,34 +33,7 @@ def test_restatement_decodes_pyarrow(name):
     assert err == S.OK and pre == len(x) and out == x
 
 
-def forms():
-    """(name, stream, expected output) covering every element form"""
-    rng = np.random.default_rng(52)
-    big = rng.integers(0, 256, 70_000, dtype=np.uint8).tobytes()
-    far = big + big[:100]                                       # a copy 70 000 bytes back: copy-4
-    out = [
-        ("inline_literals", S.encode(b"abcdefgh" * 3 + bytes(range(40)), lit_bytes=0)),
-        ("literal_1_byte_length", S.stream(200, [S.literal(big[:200], 1)])),
-        ("literal_2_byte_length", S.stream(300, [S.literal(big[:300], 2)])),
-        ("literal_3_byte_length", S.stream(70_000, [S.literal(big, 3)])),
-        ("literal_4_byte_length", S.stream(61, [S.literal(big[:61], 4)])),
-        ("literal_1_byte_length_short", S.stream(5, [S.literal(big[:5], 1)])),
-        ("copy_1", S.stream(20, [S.literal(b"0123456789"), S.copy(10, 10, 1)])),
-        ("copy_2", S.stream(74, [S.literal(b"0123456789"), S.copy(10, 64, 2)])),
-        ("copy_4", S.stream(74, [S.literal(b"0123456789"), S.copy(10, 64, 4)])),
-        ("offset_1_run", S.stream(1 + 64 * 3, [S.literal(b"z"), S.copy(1, 64, 2), S.copy(1, 64, 4), S.copy(64, 64, 2)])),
-        ("overlap_offset_3", S.stream(3 + 11, [S.literal(b"abc"), S.copy(3, 11, 1)])),
-        ("copy_of_length_1", S.stream(2, [S.literal(b"q"), S.copy(1, 1, 2)])),
-        ("offset_beyond_64k", S.encode(far)),
-        ("greedy_copy_2_only", S.encode(b"hello hello hello world " * 40, copy_form=2)),
-        ("greedy_copy_4_only", S.encode(b"hello hello hello world " * 40, copy_form=4)),
-        ("greedy_literal_4_bytes", S.encode(big[:5000] + big[:5000], lit_bytes=4)),
-        ("empty_stream", S.stream(0, [])),
-    ]
-    return [(n, s, S.decode(s)[0]) for n, s in out]
-
-
-@pytest.mark.parametrize("case", forms(), ids=lambda c: c[0])
+@pytest.mark.parametrize("case", S.forms(), ids=lambda c: c[0])
 def test_pyarrow_decodes_every_form(case):
     name, s, x = case
     out, err, pre = S.decode(s, len(x))
@@ -87,31 +60,7 @@ def _tags(s):
     return out
 
 
-def corrupt_rows():
-    """(name, stream, dst_len, bytes the restatement delivers)"""
-    ok = S.literal(b"0123456789")
-    return [
-        ("no_preamble", b"", 5, 0),
-        ("preamble_cut", b"\x80", 5, 0),
-        ("preamble_over_10_bytes", b"\xff" * 10 + b"\x01", 5, 0),
-        ("preamble_over_32_bits", S.put_uvarint(1 << 32), 1 << 32, 0),
-        ("literal_length_cut", S.stream(20, [ok, b"\xf0"]), 20, 10),
-        ("literal_4_length_cut", S.stream(20, [ok, b"\xfc\x01\x00"]), 20, 10),
-        ("literal_bytes_cut", S.stream(20, [ok, S.literal(b"abcdefghij")[:-1]]), 20, 10),
-        ("literal_past_output", S.stream(15, [ok, S.literal(b"abcdefghij")]), 15, 10),
-        ("copy_1_offset_cut", S.stream(20, [ok, S.copy(10, 10, 1)[:1]]), 20, 10),
-        ("copy_2_offset_cut", S.stream(20, [ok, S.copy(10, 10, 2)[:2]]), 20, 10),
-        ("copy_4_offset_cut", S.stream(20, [ok, S.copy(10, 10, 4)[:4]]), 20, 10),
-        ("copy_offset_0", S.stream(20, [ok, S.copy(0, 10, 2)]), 20, 10),
-        ("copy_offset_past_output", S.stream(30, [ok, S.copy(11, 10, 2)]), 30, 10),
-        ("copy_past_output", S.stream(15, [ok, S.copy(10, 10, 2)]), 15, 10),
-        ("stream_ends_early", S.stream(30, [ok, S.copy(10, 10, 1)]), 30, 20),
-        ("trailing_element", S.stream(20, [ok, S.copy(10, 10, 1), S.literal(b"x")]), 20, 20),
-        ("preamble_only", S.stream(7, []), 7, 0),
-    ]
-
-
-@pytest.mark.parametrize("row", corrupt_rows(), ids=lambda r: r[0])
+@pytest.mark.parametrize("row", S.corrupt_rows(), ids=lambda r: r[0])
 def test_corrupt_rows_rejected_by_both(row):
     name, s, n, delivered = row
     out, err, _ = S.decode(s, n)

@@ -9,6 +9,8 @@ A page is checked in the order the device does it, so that both name the same ch
 """
 import collections
 
+import numpy as np
+
 OK, CORRUPT, SIZE, CHECKSUM = 0, 1, 2, 3
 CHECKS = ("truncated", "bad magic", "frame header", "dictionary", "block type", "block size", "literals", "huffman",
           "fse", "sequences", "offset", "content size", "page size")
@@ -812,3 +814,136 @@ def rle_seq_block(lits, nseq, ll_code, of_code, ml_code, of_bits, last, repeat=F
         nb += of_code
     stream = acc.to_bytes((nb + 8) // 8, "little")
     return block("compressed", lh + bytes(lits) + sh + stream, last)
+
+
+# ---------------------------------------------------------------------------------------------------- test streams
+LEVELS = (-5, 1, 3, 9, 19, 22)
+
+
+def datasets(rng):
+    return {
+        "timestamps": (np.cumsum(rng.integers(0, 1000, 40_000)) + (1 << 40)).astype(np.int64).tobytes(),
+        "dict_indices": (rng.integers(0, 100_000, 60_000) & 0x1FFFF).astype(np.uint32).tobytes(),
+        "zeros": bytes(300_000),
+        "random": rng.integers(0, 256, 150_000, dtype=np.uint8).tobytes(),
+        "text": b" ".join(rng.choice([b"alpha", b"beta", b"gamma", b"delta", b"parquet", b"zstd"], 40_000)),
+        "skewed": np.minimum(rng.geometric(0.03, 200_000), 255).astype(np.uint8).tobytes(),
+        "one": b"x",
+        "empty": b"",
+    }
+
+
+def corpus():
+    """[(name, compressed, raw)] written by pyarrow"""
+    rng = np.random.default_rng(71)
+    import pyarrow as pa
+    out = []
+    for name, x in datasets(rng).items():
+        for lvl in LEVELS:
+            out.append((f"{name}-{lvl}", pa.Codec("zstd", compression_level=lvl).compress(x, asbytes=True), x))
+    big = (np.cumsum(rng.integers(0, 1000, 1 << 19)) + (1 << 40)).astype(np.int64).tobytes()
+    out.append(("timestamps-4MB-3", pa.compress(big, codec="zstd", asbytes=True), big))
+    return out
+
+
+def comp(x, level=3):
+    import pyarrow as pa
+    return pa.Codec("zstd", compression_level=level).compress(x, asbytes=True)
+
+
+def surgery():
+    """[(name, stream, raw)]: the forms libzstd does not emit"""
+    import pyarrow as pa
+    rng = np.random.default_rng(72)
+    text = b" ".join(rng.choice([b"alpha", b"beta", b"gamma", b"delta"], 3000))
+    ts = (np.cumsum(rng.integers(0, 1000, 5000)) + (1 << 40)).astype(np.int64).tobytes()
+    letters = rng.integers(97, 123, 20_000, dtype=np.uint8).tobytes()
+    assert direct_weights(comp(letters))[1] > 0
+    a, b = comp(text), comp(ts, 19)
+    rows = [
+        ("concatenated", a + b, text + ts),
+        ("skippable_frames", skippable(b"meta") + a + skippable(b"", 15) + b + skippable(bytes(100), 7), text + ts),
+        ("checksum", reframe(a, checksum=True), text),
+        ("no_content_size", reframe(b, fcs=False), ts),
+        ("checksum_no_content_size", reframe(a + b, fcs=False, checksum=True), text + ts),
+        ("content_size_2_bytes", reframe(comp(text[:5000]), fcs_bytes=2), text[:5000]),
+        ("content_size_8_bytes", reframe(a, fcs_bytes=8), text),
+        ("dictionary_id_zero", frame([block("raw", b"hello", 1)], fcs=5, dict_id=(0, 2)), b"hello"),
+        ("raw_and_rle_blocks", frame([block("raw", b"hello", 0), block("rle", b"x", 1, size=1000)], fcs=1005),
+         b"hello" + b"x" * 1000),
+        ("empty_raw_block_frames", frame([block("raw", b"", 1)], fcs=0) * 3, b""),
+        ("direct_weights", direct_weights(comp(letters))[0], letters),
+        ("rle_literals", frame([block("compressed", bytes([20 << 3 | 1, ord("k"), 0]), 1)], fcs=20), b"k" * 20),
+        ("repeat_modes", frame([block("raw", b"abcdefgh", 0), rle_seq_block(b"xyz", 3, 1, 0, 2, lambda i: 0, 0),
+                                  rle_seq_block(b"uv", 2, 1, 0, 2, lambda i: 0, 1, repeat=True)], fcs=8 + 3 * 6 + 2 * 6),
+         None),
+        ("rle_modes_3_byte_count", frame([block("raw", b"abcdefgh", 0),
+                                            rle_seq_block(b"", 33_000, 0, 0, 0, lambda i: 0, 1)], fcs=8 + 99_000), None),
+        ("rep0_minus_1", frame([block("raw", bytes(range(64)), 0), rle_seq_block(b"", 4, 0, 5, 0, lambda i: 3, 0),
+                                  rle_seq_block(b"zz", 5, 0, 1, 0, lambda i: 1, 1)], fcs=64 + 12 + 15 + 2), None),
+        ("window_descriptor_1KB", frame([block("raw", b"q" * 1024, 0), block("rle", b"r", 1, size=1024)],
+                                          window_log=10), b"q" * 1024 + b"r" * 1024),
+    ]
+    out = []
+    for name, s, x in rows:
+        if x is None:                                             # hand-built: libzstd decodes it the same way
+            x, err, _ = decode(s)
+            assert err == OK and pa.decompress(s, decompressed_size=len(x), codec="zstd", asbytes=True) == x, name
+        out.append((name, s, x))
+    return out
+
+
+def forms():
+    """every stream of the corpus and the surgery rows, for the device tests: [(name, stream, raw)]"""
+    return [r for r in corpus() if len(r[2]) < 1 << 20] + surgery()
+
+
+def corrupt_rows():
+    """[(name, stream, dst_len, expected check or CHECKSUM)]: every row but the two
+    window rows (test_zstd_oracle.WINDOW_ROWS) pa.decompress rejects too"""
+    rng = np.random.default_rng(73)
+    text = b" ".join(rng.choice([b"alpha", b"beta", b"gamma", b"delta"], 3000))
+    good = comp(text)
+    n = len(text)
+    ck = reframe(good, checksum=True)
+    hdr = frame_header(fcs=None, window_log=17, single=False)
+    bad_ck = ck[:-1] + bytes([ck[-1] ^ 1])
+    rows = [
+        ("truncated_block", good[:-3], n, "truncated"),
+        ("truncated_checksum", ck[:-2], n, "truncated"),
+        ("truncated_skippable", skippable(b"abcdef")[:-2], n, "truncated"),
+        ("bad_magic", b"\x28\xb5\x2f\xfe" + good[4:], n, "bad magic"),
+        ("reserved_bit", good[:4] + bytes([good[4] | 8]) + good[5:], n, "frame header"),
+        ("dictionary", frame([block("raw", b"hello", 1)], fcs=5, dict_id=(7, 1)), 5, "dictionary"),
+        ("reserved_block_type", hdr + block("reserved", b"abc", 1), 3, "block type"),
+        ("block_over_window", frame_header(window_log=10, single=False) + block("raw", bytes(2000), 1), 2000, "block size"),
+        ("literals_past_block", hdr + block("compressed", bytes([31 << 3]) + b"ab", 1), 31, "literals"),
+        ("treeless_without_table", hdr + block("compressed", bytes([3, 0, 0, 0]), 1), 0, "huffman"),
+        ("fse_accuracy_too_high", hdr + block("raw", b"abcdefgh", 0) +
+         block("compressed", bytes([0, 1, 2 << 6, 0x0F, 0, 0]), 1), 11, "fse"),
+        ("repeat_without_table", hdr + block("raw", b"abcdefgh", 0) + block("compressed", bytes([0, 1, 0xFC, 1]), 1), 11,
+         "sequences"),
+        ("zero_sequences_trailing_bytes", hdr + block("compressed", bytes([0, 0, 7]), 1), 0, "sequences"),
+        ("no_padding_marker", hdr + block("raw", b"abcdefgh", 0) + rle_seq_block(b"", 2, 0, 0, 0, lambda i: 0, 1)[:-1] +
+         b"\x00", 14, "sequences"),
+        ("literal_overrun", hdr + block("raw", b"abcdefgh", 0) + rle_seq_block(b"ab", 1, 5, 0, 0, lambda i: 0, 1), 16,
+         "sequences"),
+        ("offset_before_output", hdr + rle_seq_block(b"", 1, 0, 0, 0, lambda i: 0, 1), 3, "offset"),
+        ("offset_zero", hdr + block("raw", b"abcdefgh", 0) + rle_seq_block(b"", 1, 0, 1, 0, lambda i: 1, 1), 11, "offset"),
+        ("offset_beyond_window", frame_header(window_log=10, single=False) + block("raw", bytes(1024), 0) +
+         block("raw", bytes(1024), 0) + rle_seq_block(b"", 1, 0, 10, 0, lambda i: 1503 - 1024, 1), 2051, "offset"),
+        ("content_size_short", frame([block("raw", b"hello", 1)], fcs=10), 10, "content size"),
+        ("content_size_long", frame([block("raw", b"hello", 0), block("raw", b"world", 1)], fcs=7), 7, "content size"),
+        ("second_frame_corrupt", good + good[:-3], 2 * n, "truncated"),
+        ("checksum_mismatch", bad_ck, n, CHECKSUM),
+        ("checksum_mismatch_then_corrupt", bad_ck + good[:-3], 2 * n, CHECKSUM),
+        ("page_size_then_corrupt", reframe(good, fcs=False) + good[:-3], n - 10, "page size"),
+    ]
+    return rows
+
+
+def golden_payload():
+    """the bytes the golden frames hold (tests/golden/gen_zstd_golden.py writes them)"""
+    rng = np.random.default_rng(2024)
+    ts = (np.cumsum(rng.integers(0, 1000, 40_000)) + (1 << 40)).astype(np.int64).tobytes()
+    return ts + b" ".join(rng.choice([b"alpha", b"beta", b"gamma"], 20_000))

@@ -8,11 +8,11 @@
 // Every value lives in a dense per-page array indexed d = tile_base[p] * 1024 + rank (so a page's values start on a
 // 1024-value boundary).  Three stages:
 //   1. Lengths per dense value (vlen, int64) and where its bytes start (vsrc):
-//      - PLAIN: ba_plain_parse_kernel, one block per page, streams the page through a 16 KB shared-memory window in
-//        spans of 1024 candidate starts.  Every candidate reads the 4-byte length it would have and its next start; the
-//        chain of real values through the span is found by pointer doubling (as snappy_parse_kernel finds Snappy
-//        elements), and a block scan of the chain ranks the values.  A value longer than the window moves the next
-//        span past it without loading it.
+//      - PLAIN: ba_plain_parse_kernel, one block per page, streams the page through the shared-memory window of
+//        pq_window.cuh in spans of 1024 candidate starts.  Every candidate reads the 4-byte length it would have and its
+//        next start; the chain of real values through the span is found by span_chain's pointer doubling (as
+//        snappy_parse_kernel finds Snappy elements), and a block scan of the chain ranks the values.  A value longer
+//        than the window moves the next span past it without loading it.
 //      - dictionary: pq_runs_kernel + pq_expand_kernel<kIndex> write one int32 index per slot; the length is
 //        dict_off[i+1] - dict_off[i].
 //      - DELTA_LENGTH / DELTA: delta_walk_kernel and delta_values_kernel (pq_decode.cuh) decode every length of the
@@ -39,9 +39,7 @@ namespace ag {
 
 namespace {
 
-constexpr int kBaThreads = kRleThreads;
-constexpr int kSpan = 1024;                 // PLAIN: candidate value starts per parse step
-constexpr int kPer = kSpan / kBaThreads;
+constexpr int kBaThreads = kPqThreads;
 constexpr int kPsvLevels = 7;               // group minima of 32^1 .. 32^7 values (pages hold < 2^31 values)
 
 enum BaErr : int {
@@ -112,12 +110,8 @@ struct BaArgs {
   const uint8_t* src_base;    // data, or dict_data
 };
 
-__device__ __forceinline__ bool bit_on(const uint32_t* m, int q) { return (m[q >> 5] >> (q & 31)) & 1u; }
-
 __device__ __forceinline__ int64_t page_slots(const BaArgs& a, int64_t p, const ag_pq_page& pg, int64_t need, int64_t produced, int err) {
-  if (err == kBaShort) return 0;                               // DecodeSpaced delivers nothing then
-  if (!a.valid) return produced;
-  return produced < need ? slot_of_rank(a.valid, pg.out, a.tile_cnt, a.tile_base[p], a.tile_base[p + 1], produced) : pg.num_values;
+  return slots_written(a.valid, pg, a.tile_cnt, a.tile_base[p], a.tile_base[p + 1], need, produced, err == kBaShort);
 }
 
 __device__ __forceinline__ void finish_page(const BaArgs& a, int64_t p, int64_t produced, int64_t slots, int err, int64_t arg) {
@@ -145,7 +139,7 @@ ba_plain_parse_kernel(BaArgs a) {
   const int64_t d0 = a.tile_base[p] * kTile;
   if (tid == 0) { s_pos = 0; s_nval = 0; s_next = len; s_err = kBaNone; s_done = need == 0; }
   const uint8_t* wb = reinterpret_cast<const uint8_t*>(win);
-  const uintptr_t sbeg = reinterpret_cast<uintptr_t>(in), send = sbeg + len;
+  const uintptr_t sbeg = reinterpret_cast<uintptr_t>(in);
   int64_t wlo = INT64_MIN / 2;
   while (true) {
     __syncthreads();
@@ -153,13 +147,8 @@ ba_plain_parse_kernel(BaArgs a) {
     const int64_t cur = s_pos;
     if ((cur + kSpan + 4 < len ? cur + kSpan + 4 : len) > wlo + kWinBytes) {
       const uintptr_t a0 = (sbeg + cur) & ~(uintptr_t)15;
-#pragma unroll 4
-      for (int v = tid; v < kWinVec; v += kBaThreads) {
-        const uintptr_t ad = a0 + (uintptr_t)v * 16;
-        if (ad < send && ad + 16 > sbeg) win[v] = __ldcs(reinterpret_cast<const uint4*>(ad));
-      }
+      load_window(win, sbeg, sbeg + len, a0);
       wlo = (int64_t)a0 - (int64_t)sbeg;
-      __syncthreads();
     }
     // ---- the value that would start at each of this thread's positions ----
     uint32_t J[kPer];
@@ -186,27 +175,8 @@ ba_plain_parse_kernel(BaArgs a) {
       last[k] = J[k] == kSpan;
       jmp[0][q] = (uint16_t)J[k];
     }
-    if (tid < kSpan / 32) reach[tid] = tid == 0 ? 1u : 0u;
     if (tid == 0) s_fail = INT64_MAX;
-    __syncthreads();
-    for (int r = 0;; ++r) {
-      bool grew = false;
-#pragma unroll
-      for (int k = 0; k < kPer; ++k) {
-        const int q = tid * kPer + k;
-        const uint32_t j = J[k];
-        if (j < kSpan && bit_on(reach, q) && !bit_on(reach, (int)j)) {
-          atomicOr(&reach[j >> 5], 1u << (j & 31));
-          grew = true;
-        }
-      }
-      if (!__syncthreads_or(grew)) break;
-#pragma unroll
-      for (int k = 0; k < kPer; ++k) {
-        J[k] = J[k] < kSpan ? jmp[r & 1][J[k]] : kSpan;
-        jmp[(r + 1) & 1][tid * kPer + k] = (uint16_t)J[k];
-      }
-    }
+    span_chain(J, jmp, reach);
     // ---- ranks, values, the first failing value, the next span ----
     int cnt = 0;
 #pragma unroll

@@ -7,8 +7,8 @@
 // A call decodes a batch of pages (ag_pq_page descriptors, one device buffer of page payloads) in three launches:
 //   1. pq_tile_count_kernel (spaced only): valid bits per 1024-slot tile of every page.
 //   2. pq_runs_kernel, one block per page: scans the page's tile counts into dense-rank bases, then streams the page
-//      bytes through shared memory in 16 KB windows while thread 0 walks the run headers (the chain is sequential; the
-//      parallelism comes from the pages).  Each run becomes an 8-byte descriptor {first dense value | literal flag,
+//      bytes through the shared-memory window of pq_window.cuh while thread 0 walks the run headers (the chain is
+//      sequential; the parallelism comes from the pages).  Each run becomes an 8-byte descriptor {first dense value | literal flag,
 //      repeated value or payload byte offset}; the page records its run count, decoded count and an error code.
 //      Windows start at the next header, so the bytes of long literal runs between two windows are never loaded.
 //   3. pq_expand_kernel, one block per 1024-slot tile of output: finds its page and run by binary search, broadcasts
@@ -28,15 +28,14 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "pq_window.cuh"
 
 namespace ag {
 
 namespace {
 
-constexpr int kRleThreads = 256;
+constexpr int kRleThreads = kPqThreads;
 constexpr int kTile = 1024;                 // output slots per expansion block (4 per thread)
-constexpr int kWinVec = 1024;               // 16-byte vectors per shared-memory window (16 KB)
-constexpr int kWinBytes = kWinVec * 16;
 constexpr uint32_t kLiteralFlag = 0x80000000u;
 
 // kIndex: dictionary indices themselves (int32; an index >= dict_len becomes -1 and lowers *bad), for dictionaries the
@@ -144,34 +143,6 @@ pq_tile_count_kernel(PqArgs a) {
   }
 }
 
-// inclusive block scan of one value per thread (int ranks, or unsigned sums that wrap at their width)
-template <typename V>
-__device__ __forceinline__ V block_incl_scan(V v, V* warp_tot, V* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  V x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const V y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_tot[wid] = x;
-  __syncthreads();
-  V off = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kRleThreads / 32; ++w) {
-    const V t = warp_tot[w];
-    off += (w < wid) ? t : (V)0;
-    tot += t;
-  }
-  __syncthreads();
-  *total = tot;
-  return off + x;
-}
-
-__device__ __forceinline__ int block_excl_scan(int v, int* warp_tot, int* total) {
-  return block_incl_scan(v, warp_tot, total) - v;
-}
-
 // spaced: turns the valid counts of a page's tiles [t0, t1) into each tile's first dense rank (one block per page);
 // returns the page's valid count
 __device__ __forceinline__ int64_t scan_tile_ranks(int64_t* tile_cnt, int64_t t0, int64_t t1, int* warp_tot) {
@@ -197,6 +168,15 @@ __device__ int64_t slot_of_rank(const uint8_t* valid, int64_t bit0, const int64_
     if (bit_is_set(valid, bit0 + s)) { if (r == rank) break; ++r; }
   }
   return s;
+}
+
+// output slots a page's first `produced` dense values fill: none when its error delivers nothing (DecodeSpaced), else
+// every slot up to the first valid slot whose value was not delivered; the page's tiles are [t0, t1)
+__device__ __forceinline__ int64_t slots_written(const uint8_t* valid, const ag_pq_page& pg, const int64_t* tile_cnt, int64_t t0, int64_t t1,
+                                                 int64_t need, int64_t produced, bool nothing) {
+  if (nothing) return 0;
+  if (!valid) return produced;
+  return produced < need ? slot_of_rank(valid, pg.out, tile_cnt, t0, t1, produced) : pg.num_values;
 }
 
 // one block per page: stream geometry, spaced rank bases, run table
@@ -293,17 +273,10 @@ pq_runs_kernel(PqArgs a) {
   while (true) {
     __syncthreads();
     if (s_done) break;
-    // window [a0, a0 + 16 KB) over absolute addresses, a0 = 16-byte aligned start of the next header; only vectors
-    // that hold at least one byte of the stream are loaded (an aligned vector never straddles a mapping boundary)
+    // the window starts at the 16-byte aligned start of the next header
     const uintptr_t sbeg = reinterpret_cast<uintptr_t>(a.data) + stream;
-    const uintptr_t send = sbeg + len;
     const uintptr_t a0 = (sbeg + s_pos) & ~(uintptr_t)15;
-#pragma unroll 4
-    for (int v = tid; v < kWinVec; v += kRleThreads) {
-      const uintptr_t ad = a0 + (uintptr_t)v * 16;
-      if (ad < send && ad + 16 > sbeg) win[v] = __ldcs(reinterpret_cast<const uint4*>(ad));
-    }
-    __syncthreads();
+    load_window(win, sbeg, sbeg + len, a0);
     if (tid == 0) {
       int64_t pos = s_pos, produced = s_produced;
       int nruns = s_nruns, err = kErrNone, done = 0;
@@ -368,13 +341,8 @@ pq_runs_kernel(PqArgs a) {
     const int64_t produced = s_produced;
     // RleBooleanDecoder.DecodeToBitmap: a short stream is io.ErrUnexpectedEOF after the values delivered
     if (a.kind == kBoolRle && s_err == kErrNone && produced < need) s_err = kErrBoolEof;
-    int64_t slots = produced;
-    if (err_delivers_nothing(s_err)) {
-      slots = 0;                                               // DecodeSpaced delivers nothing then
-    } else if (a.valid) {
-      slots = produced < need ? slot_of_rank(a.valid, pg.out, a.tile_cnt, a.plan.tile_base[p], a.plan.tile_base[p + 1], produced)
-                              : pg.num_values;
-    }
+    const int64_t slots = slots_written(a.valid, pg, a.tile_cnt, a.plan.tile_base[p], a.plan.tile_base[p + 1], need, produced,
+                                        err_delivers_nothing(s_err));
     PageState ps;
     ps.stream = stream; ps.stream_len = len; ps.need = need; ps.produced = produced; ps.slots = slots;
     ps.nruns = s_nruns; ps.bw = bw; ps.err = s_err; ps.pad = (int32_t)s_arg;
@@ -547,23 +515,6 @@ struct DeltaArgs {
   void* out;
 };
 
-// binary.ReadUvarint: at most 10 bytes, the 10th at most 1
-template <typename B>
-__device__ __forceinline__ bool read_uvarint(B byte_at, int64_t& pos, int64_t len, unsigned long long* v) {
-  unsigned long long x = 0;
-  for (int i = 0; i < 10; ++i) {
-    if (pos >= len) return false;
-    const uint32_t c = byte_at(pos++);
-    if (c < 0x80) {
-      if (i == 9 && c > 1) return false;
-      *v = x | (unsigned long long)c << (7 * i);
-      return true;
-    }
-    x |= (unsigned long long)(c & 0x7f) << (7 * i);
-  }
-  return false;
-}
-
 __device__ __forceinline__ long long unzigzag(unsigned long long u) { return (long long)(u >> 1) ^ -(long long)(u & 1); }
 
 // One block per page: parses the header (SetData) and walks the block chain (initBlock / unpackNextMini) up to the
@@ -624,16 +575,10 @@ delta_walk_kernel(DeltaArgs a) {
   while (true) {
     __syncthreads();
     if (w.done) break;
-    // window [a0, a0 + 16 KB) over absolute addresses, a0 = 16-byte aligned start of the next block header
+    // the window starts at the 16-byte aligned start of the next block header
     const uintptr_t sbeg = reinterpret_cast<uintptr_t>(page);
-    const uintptr_t send = sbeg + len;
     const uintptr_t a0 = (sbeg + w.pos) & ~(uintptr_t)15;
-#pragma unroll 4
-    for (int v = tid; v < kWinVec; v += kRleThreads) {
-      const uintptr_t ad = a0 + (uintptr_t)v * 16;
-      if (ad < send && ad + 16 > sbeg) win[v] = __ldcs(reinterpret_cast<const uint4*>(ad));
-    }
-    __syncthreads();
+    load_window(win, sbeg, sbeg + len, a0);
     if (tid == 0) {
       const int64_t wlo = (int64_t)(a0 - sbeg), wend = wlo + kWinBytes;   // page offsets the window covers
       auto byte_at = [&](int64_t i) -> uint32_t { return i < wend ? sb[i - wlo] : __ldg(page + i); };
@@ -675,9 +620,7 @@ delta_walk_kernel(DeltaArgs a) {
     const int64_t cap = s_cap;
     int64_t produced = err == kDErrNone ? cap : cap > 0 ? (int64_t)(1 + (unsigned long long)w.nmb * w.vpm) : 0;
     if (err == kDErrNone && a.valid && s_total < need) { err = kDErrShort; produced = 0; }
-    int64_t slots = produced;
-    if (err == kDErrShort) slots = 0;                            // DecodeSpaced delivers nothing then
-    else if (a.valid) slots = produced < need ? slot_of_rank(a.valid, pg.out, a.tile_cnt, t0, t1, produced) : pg.num_values;
+    const int64_t slots = slots_written(a.valid, pg, a.tile_cnt, t0, t1, need, produced, err == kDErrShort);
     DeltaPage ps;
     ps.first = s_first; ps.produced = produced; ps.slots = slots; ps.arg0 = w.arg0; ps.arg1 = w.arg1; ps.end = w.pos;
     ps.vpm = (uint32_t)w.vpm; ps.err = err;

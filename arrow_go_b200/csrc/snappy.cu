@@ -5,14 +5,14 @@
 //
 // A call decompresses a batch of pages (ag_pq_compressed descriptors, one device buffer of compressed bytes) in two
 // launches, both one block per page:
-//   1. snappy_parse_kernel: reads the preamble, then streams the compressed bytes through a 16 KB shared-memory window
-//      in spans of 1024 candidate element starts.  Every thread decodes the element that would start at each of its
-//      4 positions (length, output length, offset); the element chain through the span is found by pointer doubling
-//      over those next-positions (a reach bitmask, log2(elements) rounds), and a block scan of the chain's output
-//      lengths gives each element its output position.  Each element is validated here and written as a 9-byte
-//      descriptor {output position, literal source / copy offset, literal flag}, so a failing page knows how many
-//      bytes its valid elements produce before anything is executed.  A literal longer than the window moves the next
-//      span (and window) past it without loading it.
+//   1. snappy_parse_kernel: reads the preamble, then streams the compressed bytes through the shared-memory window of
+//      pq_window.cuh in spans of 1024 candidate element starts.  Every thread decodes the element that would start at
+//      each of its 4 positions (length, output length, offset); the element chain through the span is found by
+//      span_chain's pointer doubling over those next-positions (a reach bitmask, log2(elements) rounds), and a block
+//      scan of the chain's output lengths gives each element its output position.  Each element is validated here and
+//      written as a 9-byte descriptor {output position, literal source / copy offset, literal flag}, so a failing page
+//      knows how many bytes its valid elements produce before anything is executed.  A literal longer than the window
+//      moves the next span (and window) past it without loading it.
 //   2. snappy_exec_kernel (lz_exec.cuh, shared with ZSTD): walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
 //      dst[pos - off + (j mod off)], so every output byte names one source byte: a compressed byte (literals), an
 //      output byte before the batch (read back from dst, which the same block wrote, L2-resident), or an earlier byte
@@ -26,16 +26,12 @@
 #include <vector>
 
 #include "lz_exec.cuh"
+#include "pq_window.cuh"
 
 namespace ag {
 
 namespace {
 
-constexpr int kSnThreads = 256;
-constexpr int kSpan = 1024;                 // candidate element starts per parse step
-constexpr int kPer = kSpan / kSnThreads;    // 4 consecutive positions per thread
-constexpr int kWinVec = 1024;               // 16-byte vectors per shared-memory window (16 KB)
-constexpr int kWinBytes = kWinVec * 16;
 constexpr int kLook = 4;                    // bytes an element header reaches past its tag byte
 constexpr unsigned long long kCntOne = 1ull << 48;   // parse scan: element count in bits 48.., output bytes below
 constexpr unsigned long long kLenMask = kCntOne - 1;
@@ -63,38 +59,13 @@ struct SnapArgs {
   int64_t* d_written;         // may be NULL
 };
 
-// exclusive block scan of one value per thread
-__device__ __forceinline__ unsigned long long block_excl_scan(unsigned long long v, unsigned long long* warp_tot, unsigned long long* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  unsigned long long x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_tot[wid] = x;
-  __syncthreads();
-  unsigned long long off = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kSnThreads / 32; ++w) {
-    const unsigned long long t = warp_tot[w];
-    off += (w < wid) ? t : 0ull;
-    tot += t;
-  }
-  __syncthreads();
-  *total = tot;
-  return off + x - v;
-}
-
-__device__ __forceinline__ bool bit_on(const uint32_t* m, int q) { return (m[q >> 5] >> (q & 31)) & 1u; }
-
 // one block per page: preamble, element chain, validation, element descriptors
-__global__ void __launch_bounds__(kSnThreads)
+__global__ void __launch_bounds__(kPqThreads)
 snappy_parse_kernel(SnapArgs a) {
   __shared__ uint4 win[kWinVec];
   __shared__ uint16_t jmp[2][kSpan];         // next chain position 2^r elements on (kSpan: leaves the span)
   __shared__ uint32_t reach[kSpan / 32];     // span positions on the element chain
-  __shared__ unsigned long long warp_tot[kSnThreads / 32];
+  __shared__ unsigned long long warp_tot[kPqThreads / 32];
   __shared__ int64_t s_pos, s_next, s_written, s_nelem, s_pre, s_fail_out, s_fail_idx;
   __shared__ int s_err, s_done, s_fail;
   const int64_t p = blockIdx.x;
@@ -109,13 +80,7 @@ snappy_parse_kernel(SnapArgs a) {
     int64_t pos = 0;
     unsigned long long v = 0;
     if (len != 0 || dlen != 0) {                                 // an empty v2 value region has no preamble
-      bool ok = false;                                           // binary.Uvarint
-      for (int i = 0; i < 10 && pos < len; ++i) {
-        const uint32_t c = __ldg(in + pos++);
-        if (c < 0x80) { ok = !(i == 9 && c > 1); v |= (unsigned long long)c << (7 * i); break; }
-        v |= (unsigned long long)(c & 0x7f) << (7 * i);
-      }
-      if (!ok || v > 0xffffffffull) err = kSnCorrupt;
+      if (!read_uvarint([&](int64_t i) { return (uint32_t)__ldg(in + i); }, pos, len, &v) || v > 0xffffffffull) err = kSnCorrupt;
       else if ((int64_t)v != dlen) err = kSnSize;
     }
     s_pos = pos; s_pre = (int64_t)v; s_err = err; s_written = 0; s_nelem = 0;
@@ -123,22 +88,16 @@ snappy_parse_kernel(SnapArgs a) {
   }
 
   const uint8_t* wb = reinterpret_cast<const uint8_t*>(win);
-  const uintptr_t sbeg = reinterpret_cast<uintptr_t>(in), send = sbeg + len;
+  const uintptr_t sbeg = reinterpret_cast<uintptr_t>(in);
   int64_t wlo = INT64_MIN / 2;                                   // stream offset of the window's first byte
   while (true) {
     __syncthreads();
     if (s_done) break;
     const int64_t cur = s_pos;
     if ((cur + kSpan + kLook < len ? cur + kSpan + kLook : len) > wlo + kWinBytes) {
-      // window [a0, a0 + 16 KB), a0 = 16-byte aligned start of the span; only vectors holding a stream byte are loaded
-      const uintptr_t a0 = (sbeg + cur) & ~(uintptr_t)15;
-#pragma unroll 4
-      for (int v = tid; v < kWinVec; v += kSnThreads) {
-        const uintptr_t ad = a0 + (uintptr_t)v * 16;
-        if (ad < send && ad + 16 > sbeg) win[v] = __ldcs(reinterpret_cast<const uint4*>(ad));
-      }
+      const uintptr_t a0 = (sbeg + cur) & ~(uintptr_t)15;      // the window starts at the span's aligned start
+      load_window(win, sbeg, sbeg + len, a0);
       wlo = (int64_t)a0 - (int64_t)sbeg;
-      __syncthreads();
     }
     auto byte_at = [&](int64_t i) -> uint32_t { return i < len ? (uint32_t)wb[i - wlo] : 0u; };
 
@@ -185,29 +144,8 @@ snappy_parse_kernel(SnapArgs a) {
       ends[k] = J[k] == kSpan;
       jmp[0][q] = (uint16_t)J[k];
     }
-    if (tid < kSpan / 32) reach[tid] = tid == 0 ? 1u : 0u;      // the span starts on an element
     if (tid == 0) s_fail = kSpan;
-    __syncthreads();
-
-    // ---- the chain: round r adds the positions 2^r elements after every position already on it ----
-    for (int r = 0;; ++r) {
-      bool grew = false;
-#pragma unroll
-      for (int k = 0; k < kPer; ++k) {
-        const int q = tid * kPer + k;
-        const uint32_t j = J[k];
-        if (j < kSpan && bit_on(reach, q) && !bit_on(reach, (int)j)) {
-          atomicOr(&reach[j >> 5], 1u << (j & 31));
-          grew = true;
-        }
-      }
-      if (!__syncthreads_or(grew)) break;                       // closed: every chain position is on
-#pragma unroll
-      for (int k = 0; k < kPer; ++k) {
-        J[k] = J[k] < kSpan ? jmp[r & 1][J[k]] : kSpan;
-        jmp[(r + 1) & 1][tid * kPer + k] = (uint16_t)J[k];
-      }
-    }
+    span_chain(J, jmp, reach);
 
     // ---- output positions, validation, descriptors ----
     bool on[kPer];
@@ -321,7 +259,7 @@ static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, i
   a.e_ref = reinterpret_cast<uint32_t*>(d + off_ref);
   a.e_lit = d + off_lit;
   a.d_written = d_written;
-  snappy_parse_kernel<<<(unsigned)n_pages, kSnThreads, 0, st>>>(a);
+  snappy_parse_kernel<<<(unsigned)n_pages, kPqThreads, 0, st>>>(a);
   AG_TRY(check_launch("snappy_parse_kernel"));
   LzExec x;
   x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = nullptr; x.lit_base = nullptr; x.dst = dst;

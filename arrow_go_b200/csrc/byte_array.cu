@@ -16,10 +16,11 @@
 //      - dictionary: pq_runs_kernel + pq_expand_kernel<kIndex> write one int32 index per slot; the length is
 //        dict_off[i+1] - dict_off[i].
 //      - DELTA_LENGTH / DELTA: delta_walk_kernel and delta_values_kernel (pq_decode.cuh) decode every length of the
-//        stream (DELTA: the prefix stream, then the suffix stream from its bytesRead()); ba_len_tiles_kernel and
-//        ba_len_page_kernel check them and scan them into payload offsets, ba_len_write_kernel writes vlen / vsrc.
-//   2. Offsets: ba_slot_kernel maps slots to dense ranks (ballot scan of the validity bits, null slots get 0) and
-//      writes every slot's length and source; ba_sum_kernel / ba_scan_kernel / ba_offsets_kernel scan the lengths over
+//        stream (DELTA: the prefix stream, then the suffix stream from its bytesRead()); ba_len_tiles_kernel (tile
+//        sums) and ba_len_page_kernel check them, tile_sum_scan_kernel scans the tile sums per page, and
+//        ba_len_write_kernel scans each tile into payload offsets and writes vlen / vsrc.
+//   2. Offsets: ba_slot_kernel maps slots to dense ranks (spaced_rank, null slots get 0) and writes every slot's
+//      length and source; ba_sum_kernel / ba_scan_kernel (segment_excl_scan) / ba_offsets_kernel scan the lengths over
 //      all slots, decide on the device whether the int32 offsets overflow and whether the bytes fit `out_cap`, and
 //      write the offsets at their width.
 //   3. Bytes: ba_gather_kernel, a grid over 16-byte pieces of the output; each piece finds its slot by binary search
@@ -234,11 +235,11 @@ ba_plain_parse_kernel(BaArgs a) {
 // ---------------------------------------------------------------- DELTA_LENGTH / DELTA ----
 // One block per page: the page's stream errors, then (after the length tiles) its payload checks.  Runs twice:
 // PHASE 0 before the tiles (stream errors, counts, payload start), PHASE 1 after them (negative / exceed, delivered).
-struct LenTile { long long sum, before_neg; long long neg; };   // per dense tile: length sum, sum before its first negative, that rank
+struct LenTile { long long before_neg; long long neg; };   // per dense tile: the length sum before its first negative, that rank
 
 template <int PHASE>
 __global__ void __launch_bounds__(kBaThreads)
-ba_len_page_kernel(BaArgs a, LenTile* lt) {
+ba_len_page_kernel(BaArgs a, const LenTile* lt, const long long* tile_sum) {
   __shared__ int warp_tot[kBaThreads / 32];
   __shared__ long long warp_sum[kBaThreads / 32];
   const int64_t p = blockIdx.x;
@@ -271,15 +272,14 @@ ba_len_page_kernel(BaArgs a, LenTile* lt) {
   long long run = 0, before = -1, negrank = INT64_MAX;
   for (int64_t t = t0; t < t1; t += kBaThreads) {
     const int64_t i = t + tid;
-    const LenTile x = i < t1 ? lt[i] : LenTile{0, 0, INT64_MAX};
+    const LenTile x = i < t1 ? lt[i] : LenTile{0, INT64_MAX};
+    const long long sum = i < t1 ? tile_sum[i] : 0;
     const bool has = x.neg != INT64_MAX;
-    const unsigned m = __ballot_sync(0xffffffffu, has);
     // exclusive sum of the tile sums before each tile
     long long tot;
-    const long long incl = block_incl_scan(x.sum, warp_sum, &tot);
+    const long long incl = block_incl_scan(sum, warp_sum, &tot);
     int any;
     block_excl_scan(has ? 1 : 0, warp_tot, &any);
-    (void)m;
     if (negrank == INT64_MAX && any) {
       // the first tile (in this chunk) with a negative length
       __shared__ long long s_neg, s_before;
@@ -287,7 +287,7 @@ ba_len_page_kernel(BaArgs a, LenTile* lt) {
       __syncthreads();
       if (has) atomicMin((unsigned long long*)&s_neg, (unsigned long long)x.neg);
       __syncthreads();
-      if (has && x.neg == s_neg) s_before = run + incl - x.sum + x.before_neg;
+      if (has && x.neg == s_neg) s_before = run + incl - sum + x.before_neg;
       __syncthreads();
       negrank = s_neg; before = s_before;
     }
@@ -318,10 +318,10 @@ ba_len_page_kernel(BaArgs a, LenTile* lt) {
   }
 }
 
-// one block per dense tile: the tile's length sum, its first negative length, the sum before it; DELTA: the first
-// invalid prefix length (value k needs 0 <= prefix[k] <= length[k-1], and prefix[0] == 0)
+// one block per dense tile: the tile's length sum (into tile_sum), its first negative length, the sum before it;
+// DELTA: the first invalid prefix length (value k needs 0 <= prefix[k] <= length[k-1], and prefix[0] == 0)
 __global__ void __launch_bounds__(kBaThreads)
-ba_len_tiles_kernel(BaArgs a, LenTile* lt) {
+ba_len_tiles_kernel(BaArgs a, LenTile* lt, long long* tile_sum) {
   __shared__ long long warp_sum[kBaThreads / 32];
   __shared__ unsigned long long s_neg;
   const int64_t tile = blockIdx.x;
@@ -367,12 +367,12 @@ ba_len_tiles_kernel(BaArgs a, LenTile* lt) {
     block_incl_scan(b, warp_sum, &bt);
     before = bt;
   }
-  if (tid == 0) lt[tile] = LenTile{tot, before, (long long)neg};
+  if (tid == 0) { lt[tile] = LenTile{before, (long long)neg}; tile_sum[tile] = tot; }
 }
 
 // one block per dense tile of a delivered page: the value lengths and where each value's (suffix) bytes start
 __global__ void __launch_bounds__(kBaThreads)
-ba_len_write_kernel(BaArgs a, const LenTile* lt, const long long* tile_before) {
+ba_len_write_kernel(BaArgs a, const long long* tile_before) {
   __shared__ long long warp_sum[kBaThreads / 32];
   const int64_t tile = blockIdx.x;
   const int64_t p = find_page(a.tile_base, a.n_pages, tile);
@@ -382,7 +382,6 @@ ba_len_write_kernel(BaArgs a, const LenTile* lt, const long long* tile_before) {
   const int tid = threadIdx.x;
   const bool dba = a.kind == AG_PQ_ENC_DELTA_BYTE_ARRAY;
   long long carry = s.payload + tile_before[tile];
-  (void)lt;
 #pragma unroll
   for (int q = 0; q < kTile / kBaThreads; ++q) {
     const int64_t r = r0 + q * kBaThreads + tid;
@@ -394,22 +393,6 @@ ba_len_write_kernel(BaArgs a, const LenTile* lt, const long long* tile_before) {
       a.vlen[d0 + r] = dba ? L + a.pre[d0 + r] : L;
     }
     carry += tot;
-  }
-}
-
-// one block per page: tile sums -> the sum of the page's lengths before each tile
-__global__ void __launch_bounds__(kBaThreads)
-ba_len_tile_scan_kernel(BaArgs a, const LenTile* lt, long long* tile_before) {
-  __shared__ long long warp_sum[kBaThreads / 32];
-  const int64_t p = blockIdx.x, t0 = a.tile_base[p], t1 = a.tile_base[p + 1];
-  long long run = 0;
-  for (int64_t t = t0; t < t1; t += kBaThreads) {
-    const int64_t i = t + threadIdx.x;
-    const long long v = i < t1 ? lt[i].sum : 0;
-    long long tot;
-    const long long incl = block_incl_scan(v, warp_sum, &tot);
-    if (i < t1) tile_before[i] = run + incl - v;
-    run += tot;
   }
 }
 
@@ -494,7 +477,7 @@ ba_slot_kernel(BaArgs a) {
   const BaPage ps = a.st[p];
   const int64_t s0 = (tile - a.tile_base[p]) * kTile, d0 = a.tile_base[p] * kTile;
   if (s0 >= ps.slots) return;                                    // block-uniform
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x;
   int64_t rank_base = SPACED ? a.tile_cnt[tile] : s0;
 #pragma unroll
   for (int q = 0; q < kTile / kBaThreads; ++q) {
@@ -502,18 +485,7 @@ ba_slot_kernel(BaArgs a) {
     const bool in = s < ps.slots;
     bool v = in;
     int64_t rank = s;
-    if (SPACED) {
-      v = in && bit_is_set(a.valid, pg.out + s);
-      const unsigned m = __ballot_sync(0xffffffffu, v);
-      if (lane == 0) warp_tot[wid] = __popc(m);
-      __syncthreads();
-      int off = 0, tot = 0;
-#pragma unroll
-      for (int w = 0; w < kBaThreads / 32; ++w) { const int t = warp_tot[w]; off += (w < wid) ? t : 0; tot += t; }
-      __syncthreads();
-      rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
-      rank_base += tot;
-    }
+    if (SPACED) rank = spaced_rank(in, a.valid, pg.out + s, warp_tot, rank_base, v);
     if (!in) continue;
     int64_t L = 0, src = 0;
     if (v) {
@@ -556,15 +528,7 @@ ba_sum_kernel(BaArgs a) {
 __global__ void __launch_bounds__(kBaThreads)
 ba_scan_kernel(BaArgs a, int64_t n_chunks) {
   __shared__ long long warp_sum[kBaThreads / 32];
-  long long run = 0;
-  for (int64_t c = 0; c < n_chunks; c += kBaThreads) {
-    const int64_t i = c + threadIdx.x;
-    const long long v = i < n_chunks ? a.csum[i] : 0;
-    long long tot;
-    const long long incl = block_incl_scan(v, warp_sum, &tot);
-    if (i < n_chunks) a.csum[i] = run + incl - v;
-    run += tot;
-  }
+  const long long run = segment_excl_scan(a.csum, 0, n_chunks, warp_sum);
   if (threadIdx.x == 0) {
     BaCtl c;
     c.total = run;
@@ -857,19 +821,19 @@ static ag_status byte_array_dev(int enc, int ow, const uint8_t* data, const ag_p
     }
     AG_TRY(run_stream(const_cast<DeltaPage*>(a.dls), reinterpret_cast<DeltaMini*>(d + o_mbl), skip, d + o_suf));
     LenTile* lt = reinterpret_cast<LenTile*>(d + o_lt);
-    long long* tb = reinterpret_cast<long long*>(d + o_tb);
-    ba_len_page_kernel<0><<<(unsigned)n_pages, kBaThreads, 0, st>>>(a, lt);
+    long long* tb = reinterpret_cast<long long*>(d + o_tb);   // per tile: length sum, then the page's sum before it
+    ba_len_page_kernel<0><<<(unsigned)n_pages, kBaThreads, 0, st>>>(a, lt, tb);
     AG_TRY(check_launch("ba_len_page_kernel"));
     if (n_tiles) {
-      ba_len_tiles_kernel<<<(unsigned)n_tiles, kBaThreads, 0, st>>>(a, lt);
+      ba_len_tiles_kernel<<<(unsigned)n_tiles, kBaThreads, 0, st>>>(a, lt, tb);
       AG_TRY(check_launch("ba_len_tiles_kernel"));
     }
-    ba_len_page_kernel<1><<<(unsigned)n_pages, kBaThreads, 0, st>>>(a, lt);
+    ba_len_page_kernel<1><<<(unsigned)n_pages, kBaThreads, 0, st>>>(a, lt, tb);
     AG_TRY(check_launch("ba_len_page_kernel"));
     if (n_tiles) {
-      ba_len_tile_scan_kernel<<<(unsigned)n_pages, kBaThreads, 0, st>>>(a, lt, tb);
-      AG_TRY(check_launch("ba_len_tile_scan_kernel"));
-      ba_len_write_kernel<<<(unsigned)n_tiles, kBaThreads, 0, st>>>(a, lt, tb);
+      tile_sum_scan_kernel<<<(unsigned)n_pages, kBaThreads, 0, st>>>(a.tile_base, reinterpret_cast<unsigned long long*>(tb));
+      AG_TRY(check_launch("tile_sum_scan_kernel"));
+      ba_len_write_kernel<<<(unsigned)n_tiles, kBaThreads, 0, st>>>(a, tb);
       AG_TRY(check_launch("ba_len_write_kernel"));
     }
     if (dba && n_tiles) {

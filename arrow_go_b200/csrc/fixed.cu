@@ -29,9 +29,9 @@
 //     BYTE_STREAM_SPLIT: data[j * stride + rank]).  A piece at either end of a tile is stored byte by byte, so no
 //     byte outside the slots a page decoded is written.
 //   - booleans: fx_bool_kernel, one block per 1024-slot tile.  Each thread finds its slot's value bit (PLAIN: bit
-//     `rank` of the page; RLE: the run holding `rank`, found as pq_expand_kernel finds it), a ballot per warp packs 32
-//     slots into shared memory, and one thread per aligned 32-bit output word stores it.  A word shared with a
-//     neighbouring tile or page, or with slots the call does not write, is merged with atomicAnd / atomicOr.
+//     `rank` of the page; RLE: the run holding `rank`, found by find_run), a ballot per warp packs 32 slots into
+//     shared memory, and one thread per aligned 32-bit output word stores it.  A word shared with a neighbouring tile
+//     or page, or with slots the call does not write, is merged with atomicAnd / atomicOr.
 #include <string.h>
 
 #include <algorithm>
@@ -138,9 +138,7 @@ fx_bool_kernel(PqArgs a) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const uint2* runs = a.runs + (RLE ? a.plan.run_base[p] : 0);
   const uint8_t* stream = a.data + ps.stream;
-  const int64_t rlo = ti.y;
-  int64_t rhi = tile + 1 < a.plan.tile_base[p + 1] ? a.tile_info[tile + 1].y : ps.nruns - 1;
-  if (rhi < rlo) rhi = rlo;
+  const int64_t rhi = tile_last_run(a, tile, ti, ps.nruns);
 
   int64_t rank_base = SPACED ? a.tile_cnt[tile] : s0;
 #pragma unroll
@@ -148,29 +146,13 @@ fx_bool_kernel(PqArgs a) {
     const int64_t s = s0 + q * kRleThreads + tid;
     bool v = s < limit;
     int64_t rank = s;
-    if (SPACED) {
-      v = v && bit_is_set(a.valid, pg.out + s);
-      const unsigned m = __ballot_sync(0xffffffffu, v);
-      if (lane == 0) warp_tot[wid] = __popc(m);
-      __syncthreads();
-      int off = 0, tot = 0;
-#pragma unroll
-      for (int w = 0; w < kRleThreads / 32; ++w) { const int t = warp_tot[w]; off += (w < wid) ? t : 0; tot += t; }
-      __syncthreads();
-      rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
-      rank_base += tot;
-    }
+    if (SPACED) rank = spaced_rank(s < limit, a.valid, pg.out + s, warp_tot, rank_base, v);
     bool bit = false;
     if (v) {
       if (!RLE) {
         bit = (__ldg(stream + (rank >> 3)) >> (rank & 7)) & 1;
       } else {
-        int64_t lo = rlo, hi = rhi;
-        while (lo < hi) {
-          const int64_t mid = (lo + hi + 1) >> 1;
-          if ((int64_t)(runs[mid].x & ~kLiteralFlag) <= rank) lo = mid; else hi = mid - 1;
-        }
-        const uint2 r = runs[lo];
+        const uint2 r = find_run(runs, ti.y, rhi, rank);
         // a repeated value is true when any bit of its byte is set (rle.go:161-165 keeps the whole byte)
         bit = (r.x & kLiteralFlag) ? unpack_at(stream + r.y, rank - (int64_t)(r.x & ~kLiteralFlag), 1) != 0u : r.y != 0u;
       }

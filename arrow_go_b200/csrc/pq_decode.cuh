@@ -1,8 +1,9 @@
 // pq_decode.cuh — the Parquet page-decode building blocks shared by fixed.cu, rle.cu and byte_array.cu.  Internal, not
 // part of the ABI.  The device passes: tile counts, the RLE/bit-packed run walk and expansion, and the
-// DELTA_BINARY_PACKED block walk, tile sums and scan (rle.cu's header describes those).  The host side every page
-// driver shares: the checked page plan and its upload, the tile-count launch, the read-back of the per-page states,
-// and the host flavour's staging.
+// DELTA_BINARY_PACKED block walk, tile sums and scan (rle.cu's header describes those).  The tile helpers every page
+// kernel shares: segment_excl_scan (one block's scan of per-tile values), spaced_rank (a spaced slot's dense rank),
+// tile_last_run and find_run (the run holding a rank).  The host side every page driver shares: the checked page plan
+// and its upload, the tile-count launch, the read-back of the per-page states, and the host flavour's staging.
 //
 // A call decodes a batch of pages (ag_pq_page descriptors, one device buffer of page payloads) in three launches:
 //   1. pq_tile_count_kernel (spaced only): valid bits per 1024-slot tile of every page.
@@ -13,8 +14,8 @@
 //      Windows start at the next header, so the bytes of long literal runs between two windows are never loaded.
 //   3. pq_expand_kernel, one block per 1024-slot tile of output: finds its page and run by binary search, broadcasts
 //      repeated values, unpacks literal values with aligned 32-bit loads + funnel shift, gathers dictionary values
-//      (the dictionary stays in L2) with the bounds check fused, and maps slots to dense ranks with a ballot scan of
-//      the validity bits (null slots get 0, like FillZero).
+//      (the dictionary stays in L2) with the bounds check fused, and maps slots to dense ranks with spaced_rank (null
+//      slots get 0, like FillZero).
 // Roofline.  Single pass: encoded bytes read once + values written once (+ 1 bit of validity per slot).  This design
 // reads the encoded bytes up to twice (pass 2 only touches the headers' windows and the payload it expands) and
 // writes 8 B per run descriptor, so its own bound is (2 x encoded + written) bytes of HBM traffic; the dictionary
@@ -143,19 +144,44 @@ pq_tile_count_kernel(PqArgs a) {
   }
 }
 
-// spaced: turns the valid counts of a page's tiles [t0, t1) into each tile's first dense rank (one block per page);
-// returns the page's valid count
-__device__ __forceinline__ int64_t scan_tile_ranks(int64_t* tile_cnt, int64_t t0, int64_t t1, int* warp_tot) {
-  const int tid = threadIdx.x;
-  int64_t run = 0;
+// One block turns v[t0, t1) into its exclusive prefix sums in place, kRleThreads values per step, and returns the
+// total.  S is the block scan's element type (warp_tot holds kRleThreads / 32 of them); the running sum keeps V's width.
+template <typename S, typename V>
+__device__ __forceinline__ V segment_excl_scan(V* v, int64_t t0, int64_t t1, S* warp_tot) {
+  V run = 0;
   for (int64_t t = t0; t < t1; t += kRleThreads) {
-    const int c = (t + tid < t1) ? (int)tile_cnt[t + tid] : 0;
-    int tot;
-    const int ex = block_excl_scan(c, warp_tot, &tot);
-    if (t + tid < t1) tile_cnt[t + tid] = run + ex;   // now the tile's first dense rank
+    const int64_t i = t + threadIdx.x;
+    const S x = i < t1 ? (S)v[i] : (S)0;
+    S tot;
+    const S ex = block_excl_scan(x, warp_tot, &tot);
+    if (i < t1) v[i] = run + ex;
     run += tot;
   }
   return run;
+}
+
+// spaced: turns the valid counts of a page's tiles [t0, t1) into each tile's first dense rank (one block per page);
+// returns the page's valid count
+__device__ __forceinline__ int64_t scan_tile_ranks(int64_t* tile_cnt, int64_t t0, int64_t t1, int* warp_tot) {
+  return segment_excl_scan(tile_cnt, t0, t1, warp_tot);
+}
+
+// spaced: one slot per thread of a step of kRleThreads slots, at bit `bit` of the validity bitmap.  Sets v to its
+// validity (false when !in) and returns its dense rank, by a ballot scan of the step's validity bits from rank_base,
+// which then advances past the step.  Holds two block barriers: every thread of the block calls it.
+__device__ __forceinline__ int64_t spaced_rank(bool in, const uint8_t* valid, int64_t bit, int* warp_tot, int64_t& rank_base, bool& v) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  v = in && bit_is_set(valid, bit);
+  const unsigned m = __ballot_sync(0xffffffffu, v);
+  if (lane == 0) warp_tot[wid] = __popc(m);
+  __syncthreads();
+  int off = 0, tot = 0;
+#pragma unroll
+  for (int w = 0; w < kRleThreads / 32; ++w) { const int t = warp_tot[w]; off += (w < wid) ? t : 0; tot += t; }
+  __syncthreads();
+  const int64_t rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
+  rank_base += tot;
+  return rank;
 }
 
 // spaced: the page slot of the page's `rank`-th valid value (rank < the page's valid count); tile_cnt holds first ranks
@@ -373,6 +399,24 @@ __device__ __forceinline__ T load_unaligned(const uint8_t* p) {
   return v;
 }
 
+// The runs of tile `tile` (ti = tile_info[tile]) that hold every rank it needs are [ti.y, tile_last_run]: from the
+// run holding its first rank to the run holding the next tile's first rank, or the page's last run for its last tile.
+__device__ __forceinline__ int64_t tile_last_run(const PqArgs& a, int64_t tile, int2 ti, int32_t nruns) {
+  const int64_t p = ti.x, lo = ti.y;
+  int64_t hi = tile + 1 < a.plan.tile_base[p + 1] ? a.tile_info[tile + 1].y : nruns - 1;
+  if (hi < lo) hi = lo;
+  return hi;
+}
+
+// the run of runs[lo..hi] that holds dense rank `rank`
+__device__ __forceinline__ uint2 find_run(const uint2* runs, int64_t lo, int64_t hi, int64_t rank) {
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if ((int64_t)(runs[mid].x & ~kLiteralFlag) <= rank) lo = mid; else hi = mid - 1;
+  }
+  return runs[lo];
+}
+
 // one block per tile of 1024 output slots of one page
 template <int KIND, typename T, bool SPACED>
 __global__ void __launch_bounds__(kRleThreads)
@@ -386,36 +430,21 @@ pq_expand_kernel(PqArgs a) {
   const int64_t s0 = (tile - a.plan.tile_base[p]) * kTile;
   const int64_t limit = ps.slots;
   if (s0 >= limit) return;                                      // block-uniform
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tid = threadIdx.x;
   const uint2* runs = a.runs + (KIND == kPlain || KIND == kRank || KIND == kBss ? 0 : a.plan.run_base[p]);
   const uint8_t* stream = a.data + ps.stream;
   T* out = reinterpret_cast<T*>(a.out) + pg.out;
 
-  const int64_t r0 = SPACED ? a.tile_cnt[tile] : s0;   // the tile's first dense rank
-  // runs holding this tile's first rank and the next tile's first rank bracket every rank the tile needs
-  const int64_t rlo = ti.y;
-  int64_t rhi = tile + 1 < a.plan.tile_base[p + 1] ? a.tile_info[tile + 1].y : ps.nruns - 1;
-  if (rhi < rlo) rhi = rlo;
+  const int64_t rhi = tile_last_run(a, tile, ti, ps.nruns);
 
-  int64_t rank_base = r0;
+  int64_t rank_base = SPACED ? a.tile_cnt[tile] : s0;   // the tile's first dense rank
 #pragma unroll
   for (int q = 0; q < kTile / kRleThreads; ++q) {
     const int64_t s = s0 + q * kRleThreads + tid;
     const bool in = s < limit;
     bool v = in;
     int64_t rank = s;
-    if (SPACED) {
-      v = in && bit_is_set(a.valid, pg.out + s);
-      const unsigned m = __ballot_sync(0xffffffffu, v);
-      if (lane == 0) warp_tot[wid] = __popc(m);
-      __syncthreads();
-      int off = 0, tot = 0;
-#pragma unroll
-      for (int w = 0; w < kRleThreads / 32; ++w) { const int t = warp_tot[w]; off += (w < wid) ? t : 0; tot += t; }
-      __syncthreads();
-      rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
-      rank_base += tot;
-    }
+    if (SPACED) rank = spaced_rank(in, a.valid, pg.out + s, warp_tot, rank_base, v);
     if (!in) continue;
     if (!v) { out[s] = (T)0; continue; }
     uint32_t idx;
@@ -434,12 +463,7 @@ pq_expand_kernel(PqArgs a) {
       out[s] = v;
       continue;
     } else {
-      int64_t lo = rlo, hi = rhi;
-      while (lo < hi) {
-        const int64_t mid = (lo + hi + 1) >> 1;
-        if ((int64_t)(runs[mid].x & ~kLiteralFlag) <= rank) lo = mid; else hi = mid - 1;
-      }
-      const uint2 r = runs[lo];
+      const uint2 r = find_run(runs, ti.y, rhi, rank);
       idx = (r.x & kLiteralFlag) ? unpack_at(stream + r.y, rank - (int64_t)(r.x & ~kLiteralFlag), ps.bw) : r.y;
     }
     if (KIND == kLevels) {
@@ -509,7 +533,7 @@ struct DeltaArgs {
   DeltaPage* st;
   DeltaMini* mb;
   int64_t* tile_cnt;        // spaced only: valid bits per tile, then the tile's first dense rank
-  unsigned long long* tile_sum;   // per tile: sum of its deltas, then (after delta_scan_kernel) of the page's deltas before it
+  unsigned long long* tile_sum;   // per tile: sum of its deltas, then (after tile_sum_scan_kernel) of the page's deltas before it
   int64_t* d_decoded;       // may be NULL
   int width;                // 4 (INT32) or 8 (INT64)
   void* out;
@@ -656,7 +680,7 @@ __device__ __forceinline__ T delta_at(const uint8_t* page, const DeltaMini* mb, 
 
 // One block per tile of 1024 output slots.  WRITE = false: the sum of the tile's deltas into tile_sum.  WRITE = true:
 // a block scan of the deltas, plus the first value and the deltas of the page's earlier tiles; null slots get 0.
-// Slots map to dense ranks as in pq_expand_kernel.  T is the physical width, so every sum wraps like the reference's
+// Spaced slots map to dense ranks through spaced_rank.  T is the physical width, so every sum wraps like the reference's
 // int64 accumulate-then-truncate.
 template <typename T, bool SPACED, bool WRITE>
 __global__ void __launch_bounds__(kRleThreads)
@@ -668,7 +692,7 @@ delta_values_kernel(DeltaArgs a) {
   const ag_pq_page pg = a.pages[p];
   const DeltaPage ps = a.st[p];
   const int64_t s0 = (tile - a.tile_base[p]) * kTile;
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   if (s0 >= ps.slots) {                                          // block-uniform
     if (!WRITE && tid == 0) a.tile_sum[tile] = 0;
     return;
@@ -685,18 +709,7 @@ delta_values_kernel(DeltaArgs a) {
     const bool in = s < ps.slots;
     bool v = in;
     int64_t rank = s;
-    if (SPACED) {
-      v = in && bit_is_set(a.valid, pg.out + s);
-      const unsigned m = __ballot_sync(0xffffffffu, v);
-      if (lane == 0) warp_cnt[tid >> 5] = __popc(m);
-      __syncthreads();
-      int off = 0, tot = 0;
-#pragma unroll
-      for (int w = 0; w < kRleThreads / 32; ++w) { const int t = warp_cnt[w]; off += (w < (tid >> 5)) ? t : 0; tot += t; }
-      __syncthreads();
-      rank = rank_base + off + __popc(m & ((1u << lane) - 1u));
-      rank_base += tot;
-    }
+    if (SPACED) rank = spaced_rank(in, a.valid, pg.out + s, warp_cnt, rank_base, v);
     const T d = (v && rank >= 1) ? delta_at<T>(page, mb, ps.vpm, rank) : (T)0;
     if (!WRITE) { acc += d; continue; }
     T tot;
@@ -711,28 +724,20 @@ delta_values_kernel(DeltaArgs a) {
   }
 }
 
-// one block per page: tile sums -> the sum of the page's deltas before each tile
+// one block per page: per-tile sums (of deltas, or of BYTE_ARRAY lengths) -> the sum of the page's tiles before each
+// tile, wrapping at 64 bits
 __global__ void __launch_bounds__(kRleThreads)
-delta_scan_kernel(DeltaArgs a) {
+tile_sum_scan_kernel(const int64_t* tile_base, unsigned long long* sums) {
   __shared__ unsigned long long warp_sum[kRleThreads / 32];
-  const int64_t p = blockIdx.x, t0 = a.tile_base[p], t1 = a.tile_base[p + 1];
-  unsigned long long run = 0;
-  for (int64_t t = t0; t < t1; t += kRleThreads) {
-    const int64_t i = t + threadIdx.x;
-    const unsigned long long v = i < t1 ? a.tile_sum[i] : 0ull;
-    unsigned long long tot;
-    const unsigned long long incl = block_incl_scan(v, warp_sum, &tot);
-    if (i < t1) a.tile_sum[i] = run + incl - v;
-    run += tot;
-  }
+  segment_excl_scan(sums, tile_base[blockIdx.x], tile_base[blockIdx.x + 1], warp_sum);
 }
 
 template <typename T, bool SPACED>
 ag_status launch_delta_values(const DeltaArgs& a, int64_t n_tiles, cudaStream_t st) {
   delta_values_kernel<T, SPACED, false><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
   AG_TRY(check_launch("delta_values_kernel"));
-  delta_scan_kernel<<<(unsigned)a.n_pages, kRleThreads, 0, st>>>(a);
-  AG_TRY(check_launch("delta_scan_kernel"));
+  tile_sum_scan_kernel<<<(unsigned)a.n_pages, kRleThreads, 0, st>>>(a.tile_base, a.tile_sum);
+  AG_TRY(check_launch("tile_sum_scan_kernel"));
   delta_values_kernel<T, SPACED, true><<<(unsigned)n_tiles, kRleThreads, 0, st>>>(a);
   return check_launch("delta_values_kernel");
 }

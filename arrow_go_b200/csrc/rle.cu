@@ -4,7 +4,7 @@
 //
 // The delta passes reuse pq_decode.cuh's tile counts, window and tile layout: delta_walk_kernel (one block per page)
 // parses the header and walks the block chain into one 16-byte descriptor per miniblock the page needs;
-// delta_values_kernel sums each tile's deltas, delta_scan_kernel scans the sums per page, and delta_values_kernel
+// delta_values_kernel sums each tile's deltas, tile_sum_scan_kernel scans the sums per page, and delta_values_kernel
 // unpacks again, block-scans and writes.  Every value is the first value plus a prefix sum of the deltas, modulo the
 // physical width.
 #include "pq_decode.cuh"

@@ -23,6 +23,9 @@ FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
 WIDTHS = pytest.mark.parametrize("ow", [4, 8], ids=["off32", "off64"])
 ENCODERS = {B.PLAIN: B.plain_encode, B.DELTA_LENGTH_BYTE_ARRAY: B.dlba_encode, B.DELTA_BYTE_ARRAY: B.dba_encode}
 CANARY = 0xA7
+# 300 tiles of 1024 slots, the last one partial: the one-block scans over a page's tiles take a full 256-tile step and
+# a partial one, and two such pages take the all-slot chunk scan past its first 256 chunks
+SEAM_SLOTS = 307_195
 GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "parquet_bytearray.json")))
 
 
@@ -120,6 +123,9 @@ def test_random_pages(ag, enc, ow, dev):
         if frac is not None and enc != B.PLAIN:
             continue                                                          # spaced pages with more valid slots than values
         assert st == N.AG_OK and not errs, msg
+    seam = ENCODERS[enc](F.random_strings(rng, SEAM_SLOTS))
+    st, msg, errs, _, _ = compare(ag, enc, ow, [(seam, SEAM_SLOTS)] * 2, rng, dev, 0.1)
+    assert st == N.AG_OK and not errs, msg
 
 
 @gpu
@@ -133,8 +139,9 @@ def test_dictionary_pages(ag, ow, dev):
     for n in (1, 100, 3000, 20000):
         idx = rng.integers(0, len(dictionary), n)
         streams.append((bytes([9]) + R.rle_encode(idx, 9), n))
-    for frac in (None, 0.25):
-        st, msg, errs, bad, wbad = compare(ag, B.RLE_DICTIONARY, ow, streams, rng, dev, frac, dictionary=dictionary)
+    seam = [(bytes([9]) + R.rle_encode(rng.integers(0, len(dictionary), SEAM_SLOTS), 9), SEAM_SLOTS)] * 2
+    for frac, ss in ((None, streams), (0.25, streams), (0.1, seam)):
+        st, msg, errs, bad, wbad = compare(ag, B.RLE_DICTIONARY, ow, ss, rng, dev, frac, dictionary=dictionary)
         assert st == N.AG_OK and not errs and bad == 2 ** 63 - 1 and wbad is None, msg
     bad_stream = bytes([9]) + R.rle_encode(np.array([1, 2, len(dictionary) + 3, 4]), 9)
     st, msg, errs, bad, wbad = compare(ag, B.RLE_DICTIONARY, ow, streams[:2] + [(bad_stream, 4)], rng, dev, gap=False, dictionary=dictionary)

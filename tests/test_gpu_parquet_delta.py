@@ -19,6 +19,9 @@ gpu = pytest.mark.gpu
 SHAPES = ((128, 4), (256, 4), (128, 1), (1024, 8), (4096, 1))   # values per miniblock 32, 64, 128, 128, 4096
 FLAVOURS = pytest.mark.parametrize("dev", [False, True], ids=["host", "dev"])
 GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "parquet_delta.json")))
+# 300 tiles of 1024 slots, the last one partial: the one-block scans over a page's tiles take a full 256-tile step and
+# a partial one
+SEAM_SLOTS = 307_195
 
 
 def run_delta(ag, width, blob, pages, n_out, vbits=None, dev=False):
@@ -93,6 +96,9 @@ def test_random_streams_every_bit_width(ag, width, dev):
         for frac in (None, 0.3):
             st, msg, errs = decode_and_compare(ag, width, streams, rng, dev, frac)
             assert st == N.AG_OK and not errs, (bw, frac, msg)
+    seam = [(D.delta_encode(values_with_delta_width(rng, width, 8 * width - 3, SEAM_SLOTS), width), SEAM_SLOTS)]
+    st, msg, errs = decode_and_compare(ag, width, seam, rng, dev, 0.1)
+    assert st == N.AG_OK and not errs, msg
 
 
 @gpu

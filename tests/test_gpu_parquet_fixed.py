@@ -305,7 +305,7 @@ def test_golden_fixtures(ag, name, column):
 
 
 BIG = ["bss_double", "bss_double_spaced", "bss_flba16", "dict_flba16_spaced", "plain_int96_spaced", "plain_flba1000_spaced",
-       "bool_plain", "bool_plain_spaced", "bool_rle"]
+       "bool_plain", "bool_plain_spaced", "bool_rle", "bool_rle_spaced"]
 
 
 @gpu

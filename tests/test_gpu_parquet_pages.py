@@ -15,6 +15,9 @@ from pq_chunk import read_chunk_dev
 from pq_pages import batch
 
 gpu = pytest.mark.gpu
+# 300 tiles of 1024 slots, the last one partial: the one-block scan of a page's tile valid counts takes a full
+# 256-tile step and a partial one
+SEAM_SLOTS = 307_195
 
 
 def run_dict(ag, width, dictionary, blob, pages, n_out, valid=None, dev=False):
@@ -132,6 +135,8 @@ def test_spaced_dict_and_plain_odd_offsets(ag, dev):
     dictionary = rng.integers(-(1 << 40), 1 << 40, 5000).astype(np.int64)
     for frac in (0.0, 0.1, 0.5, 1.0):
         slots = [int(x) for x in rng.integers(0, 4000, 6)] + [0, 7]
+        if frac == 0.1:
+            slots.insert(0, SEAM_SLOTS)
         n_total = sum(slots) + 100
         valid = rng.random(n_total) >= frac
         streams, plain, o = [], [], 3

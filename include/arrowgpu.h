@@ -921,6 +921,60 @@ ag_status ag_parquet_zstd_decompress_dev(const uint8_t* d_src, const ag_pq_compr
                                          int64_t* d_written, ag_stream_t s);
 
 /* ================================================================================= *
+ * GZIP page decompression — the same batch contract as SNAPPY above (`ag_pq_compressed` host table, pages in any
+ *   order, `written` in bytes per page, one stream synchronisation in the device flavour, the host flavour stages
+ *   `src` and `dst` and copies back only written bytes, the same argument checks before any launch).
+ *   serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> compress.Decode
+ *   (parquet/compress/compress.go:107) -> gzipCodec.DecodeWithError (parquet/compress/gzip.go:51-79):
+ *   gzip.NewReader, io.ReadFull into dst_len bytes, then one more byte must read as EOF.
+ *   Format, what that reader (klauspost/compress/gzip, a fork of Go's compress/gzip and compress/flate) accepts:
+ *     - one or more gzip members (RFC 1952) back to back.  After a member: no bytes left ends the stream, 1-9 bytes
+ *       are a truncation, anything else that is not a gzip header (zero padding too) is a bad header;
+ *     - the header: 1f 8b, CM = 8, FLG, MTIME, XFL, OS; FEXTRA (2-byte length, then that many bytes); FNAME and FCOMMENT
+ *       NUL-terminated with at most 511 bytes before the NUL; FHCRC = the low 16 bits of the CRC32 of the header bytes
+ *       before it.  Reserved FLG bits are ignored.  A zlib-wrapped (RFC 1950) or raw DEFLATE body is a bad header;
+ *     - DEFLATE (RFC 1951) stored, fixed and dynamic blocks.  Stored: LEN == ~NLEN.  Dynamic: HLIT <= 286, HDIST <= 30;
+ *       a repeat code 16 with no previous length, or any repeat past HLIT + HDIST, is corrupt.  Every code is complete
+ *       except a code of one symbol of length 1; a distance code may have no symbols at all (a distance symbol is then
+ *       corrupt); a literal/length code must have end-of-block (256).  Literal/length symbols 286 and 287 and distance
+ *       symbols 30 and 31 are corrupt.  A distance reaches back at most to the member's first output byte (every
+ *       member starts a fresh window);
+ *     - the trailer: CRC32 (IEEE, reflected) and ISIZE (output mod 2^32) of the member.
+ *   Page outcomes, as events in stream order (the first one wins).  Every message starts with
+ *   "parquet: could not decompress page: ":
+ *     - src_len == 0 && dst_len == 0: success with 0 bytes;
+ *     - the input ends inside a member (a stored block cut off counts as a whole), or 1-9 bytes follow a member:
+ *       "unexpected EOF";
+ *     - every member decodes cleanly but the total is short of dst_len: "unexpected EOF", or "EOF" when the total is 0;
+ *     - output byte dst_len + 1 is produced: "codec: gzip: decoded data exceeds destination size <dst_len>";
+ *     - bad magic or CM, an FHCRC mismatch, a name or comment too long, or non-gzip bytes after a member:
+ *       "gzip: invalid header";
+ *     - a member's CRC32 or ISIZE does not match at its trailer: "gzip: invalid checksum";
+ *     - corrupt DEFLATE: "gzip: <check>", one of
+ *         block type      BTYPE 3
+ *         stored length   LEN does not match NLEN
+ *         code lengths    HLIT or HDIST out of range, a bad repeat, a bit sequence the code-length code does not have
+ *         huffman         an over-subscribed or incomplete code, or no end-of-block code
+ *         symbol          an invalid literal/length or distance symbol
+ *         distance        a distance beyond the member's output so far
+ *     - written counts the bytes of every element (literal, copy, stored block) decoded before the first decode event,
+ *       at most dst_len, and those bytes are correct.  A checksum mismatch does not stop decoding: the member's bytes
+ *       are out and counted, with those of the members after it up to the first decode event;
+ *     - every other page of the batch is decoded in full.  The call returns AG_ERR_INVALID naming the lowest failing
+ *       page: "gzip_decompress: page %lld: <message> (%lld bytes written)".
+ *   No byte outside [dst, dst + dst_len) of any page is ever written, on error paths too.
+ *   Differences from the reference (DESIGN §2):
+ *     - klauspost/compress's source is not in the reference tree, so the rules above restate Go's readers; Go reports
+ *       corrupt DEFLATE as "flate: corrupt input before offset N", with an N that depends on its bit reader, so the
+ *       <check> names are this library's own;
+ *     - src_len == 0 && dst_len == 0 is a success (the reference reports "EOF").
+ * ================================================================================= */
+ag_status ag_parquet_gzip_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                     int64_t* written);
+ag_status ag_parquet_gzip_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                         int64_t* d_written, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

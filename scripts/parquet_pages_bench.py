@@ -15,11 +15,12 @@ peak, and a torch.profiler split of the device time over the three stages (value
 --fixed runs only the BOOLEAN and fixed-width cases (ag_parquet_bool_decode_dev / ag_parquet_fixed_decode_dev,
 csrc/fixed.cu): time, share of the HBM peak and a torch.profiler split per kernel.
 
---profile runs only the DELTA_BINARY_PACKED, SNAPPY and ZSTD cases, under torch.profiler, and reports the device time
-per call of each kernel (the delta block walk against the value passes, the Snappy parse against the execute, the ZSTD
-walk / literals / sequences / resolve / execute / checksum kernels) instead.
+--profile runs only the DELTA_BINARY_PACKED, SNAPPY, ZSTD and GZIP cases, under torch.profiler, and reports the device
+time per call of each kernel (the delta block walk against the value passes, the Snappy parse against the execute, the
+ZSTD walk / literals / sequences / resolve / execute / checksum kernels, the GZIP inflate / execute / CRC32 kernels)
+instead.
 
-The SNAPPY and ZSTD cases also print pyarrow's single-thread host decompression of the same pages on this machine's CPU: a CPU
+The SNAPPY, ZSTD and GZIP cases also print pyarrow's single-thread host decompression of the same pages on this machine's CPU: a CPU
 context line, not a baseline of the kernel.
 """
 import argparse
@@ -140,6 +141,7 @@ def main():
         res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer, profile=True))
         res.update(snappy_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
         res.update(zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
+        res.update(gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
         print(json.dumps(res), flush=True)
         return
     dictionary = rng.integers(-(1 << 62), 1 << 62, 100_000)
@@ -171,6 +173,7 @@ def main():
     res.update(delta_cases(args, N, rng, n, n_pages, per_page, timed, upload, page_set, line, dout, DeviceBuffer))
     res.update(snappy_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
     res.update(zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
+    res.update(gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
     dout.free()
     print(json.dumps(res), flush=True)
 
@@ -181,7 +184,7 @@ def kernel_ms(prof, steps):
     kern = {}
     for ev in prof.key_averages():
         if ev.device_type == torch.autograd.DeviceType.CUDA:
-            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|ba_\w+_kernel|fx_\w+_kernel)(<[^>]*>)?", ev.key)
+            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|gz_\w+_kernel|ba_\w+_kernel|fx_\w+_kernel)(<[^>]*>)?", ev.key)
             short = (m.group(1) + (m.group(2) or "")) if m else ev.key.strip()
             us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
             kern[short] = kern.get(short, 0.0) + us / 1e3 / steps
@@ -317,8 +320,19 @@ def snappy_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, 
 
 
 def zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=False):
-    """ZSTD (ag_parquet_zstd_decompress_dev), the page bodies of the SNAPPY cases compressed by pyarrow at its default
-    level: (a) PLAIN int64 timestamps; (b) 17-bit dictionary indices; (c) (b) decompressed then dictionary-decoded,
+    return codec_cases("zstd", args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile)
+
+
+def gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=False):
+    return codec_cases("gzip", args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile)
+
+
+KERNEL_PREFIX = {"zstd": "zstd_", "gzip": "gz_"}
+
+
+def codec_cases(codec, args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=False):
+    """ZSTD or GZIP (ag_parquet_<codec>_decompress_dev), the page bodies of the SNAPPY cases compressed by pyarrow at its
+    default level: (a) PLAIN int64 timestamps; (b) 17-bit dictionary indices; (c) (b) decompressed then dictionary-decoded,
     against the dictionary decode alone; (d) a device-to-device copy of (a)'s decompressed bytes, the floor."""
     import time
 
@@ -328,7 +342,7 @@ def zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, De
     idx = [bytes([17]) + rle_literal_page(rng.integers(0, 100_000, per_page), 17) for _ in range(4)]
 
     def comp_set(bodies):
-        encs = [pa.compress(b, codec="zstd", asbytes=True) for b in bodies]
+        encs = [pa.compress(b, codec=codec, asbytes=True) for b in bodies]
         blob = b"".join(encs) + bytes(16)
         offs = np.cumsum([0] + [len(e) for e in encs])
         pages, d = [], 0
@@ -337,7 +351,7 @@ def zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, De
             d += len(bodies[p % 4])
         t0 = time.perf_counter()                                  # pyarrow, one thread, host memory
         for p in range(n_pages):
-            pa.decompress(encs[p % 4], decompressed_size=len(bodies[p % 4]), codec="zstd", asbytes=False)
+            pa.decompress(encs[p % 4], decompressed_size=len(bodies[p % 4]), codec=codec, asbytes=False)
         cpu_ms = (time.perf_counter() - t0) * 1e3
         comp = sum(len(encs[p % 4]) for p in range(n_pages))
         return upload(np.frombuffer(blob, np.uint8)), N.compressed_table(pages), comp, d, cpu_ms
@@ -357,33 +371,33 @@ def zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, De
     ddict, bad = upload(dictionary), DeviceBuffer(64)
     dpages = N.page_table([(p * len(idx[0]), len(idx[p % 4]), per_page, p * per_page) for p in range(n_pages)])
     assert all(len(b) == len(idx[0]) for b in idx)
-    z_t = lambda: N.call("ag_parquet_zstd_decompress_dev", tsrc.ptr, ttbl, n_pages, dout.ptr, dec.ptr, None)
-    z_i = lambda: N.call("ag_parquet_zstd_decompress_dev", isrc.ptr, itbl, n_pages, ddst.ptr, dec.ptr, None)
+    z_t = lambda: N.call(f"ag_parquet_{codec}_decompress_dev", tsrc.ptr, ttbl, n_pages, dout.ptr, dec.ptr, None)
+    z_i = lambda: N.call(f"ag_parquet_{codec}_decompress_dev", isrc.ptr, itbl, n_pages, ddst.ptr, dec.ptr, None)
     dict_i = lambda: N.call("ag_parquet_dict_decode_dev", 8, ddict.ptr, 100_000, ddst.ptr, dpages, n_pages, None, dout.ptr, dec.ptr, bad.ptr, None)
     if profile:
         import torch
         from torch.profiler import ProfilerActivity, profile as tprofile
-        for name, fn in (("parquet_zstd_i64_timestamps", z_t), ("parquet_zstd_dict_indices_17bit", z_i)):
+        for name, fn in ((f"parquet_{codec}_i64_timestamps", z_t), (f"parquet_{codec}_dict_indices_17bit", z_i)):
             for _ in range(args.warmup):
                 fn()
             with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
                 for _ in range(args.steps):
                     fn()
                 torch.cuda.synchronize()
-            out[name + "_profile"] = {"kernels_ms_per_call": {k: v for k, v in kernel_ms(prof, args.steps).items() if "zstd" in k}}
+            out[name + "_profile"] = {"kernels_ms_per_call": {k: v for k, v in kernel_ms(prof, args.steps).items() if k.startswith(KERNEL_PREFIX[codec])}}
     else:
         ms = timed(z_t)
-        out["parquet_zstd_i64_timestamps"] = z_line(ms, tcomp, tdec, tcpu, "PLAIN int64 timestamp page bodies (increments in [0, 1000)), pyarrow's default level")
+        out[f"parquet_{codec}_i64_timestamps"] = z_line(ms, tcomp, tdec, tcpu, "PLAIN int64 timestamp page bodies (increments in [0, 1000)), pyarrow's default level")
         ms = timed(z_i)
-        out["parquet_zstd_dict_indices_17bit"] = z_line(ms, icomp, idec, icpu, "17-bit dictionary-index page bodies in literal runs, pyarrow's default level")
+        out[f"parquet_{codec}_dict_indices_17bit"] = z_line(ms, icomp, idec, icpu, "17-bit dictionary-index page bodies in literal runs, pyarrow's default level")
         ms_chain = timed(lambda: (z_i(), dict_i()))
         ms_dict = timed(dict_i)
-        out["parquet_zstd_then_dict_decode"] = {"ms": ms_chain, "dict_decode_alone_ms": ms_dict, "chain_over_dict_alone": ms_chain / ms_dict,
+        out[f"parquet_{codec}_then_dict_decode"] = {"ms": ms_chain, "dict_decode_alone_ms": ms_dict, "chain_over_dict_alone": ms_chain / ms_dict,
                                                 "note": "the index pages decompressed, then ag_parquet_dict_decode_dev (required, int64) from the decompressed buffer; against the dictionary decode alone"}
         cp = DeviceBuffer(tdec + 64)
         ms = timed(lambda: N.call("ag_copy_dev", cp.ptr, dout.ptr, tdec, None))
-        out["zstd_device_copy_of_decompressed_timestamps"] = line(ms, 2.0 * tdec, tdec, "ag_copy_dev of (a)'s decompressed bytes: read + write, the floor for writing them")
-        out["zstd_timestamps_over_copy"] = out["parquet_zstd_i64_timestamps"]["ms"] / ms
+        out[f"{codec}_device_copy_of_decompressed_timestamps"] = line(ms, 2.0 * tdec, tdec, "ag_copy_dev of (a)'s decompressed bytes: read + write, the floor for writing them")
+        out[f"{codec}_timestamps_over_copy"] = out[f"parquet_{codec}_i64_timestamps"]["ms"] / ms
         cp.free()
     tsrc.free(); isrc.free(); ddst.free(); dec.free(); ddict.free(); bad.free()
     return out

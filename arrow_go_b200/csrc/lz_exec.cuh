@@ -1,4 +1,5 @@
-// lz_exec.cuh — what the Parquet page decompressors (snappy.cu, zstd.cu) share.  Internal, not part of the ABI.
+// lz_exec.cuh — what the Parquet page decompressors (snappy.cu, zstd.cu, gzip.cu, lz4.cu) share.  Internal, not part of
+// the ABI.
 //
 //   pq_compressed_check   the argument checks of an ag_pq_compressed batch, AG_ERR_INVALID before any launch
 //   pq_decompress_host    the host-pointer flavour: stage src, run the device flavour, copy back only written bytes

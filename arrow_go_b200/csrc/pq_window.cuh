@@ -1,6 +1,6 @@
 // pq_window.cuh — the device protocols the Parquet page kernels that stream a page through shared memory share
 // (pq_runs_kernel and delta_walk_kernel in pq_decode.cuh, ba_plain_parse_kernel in byte_array.cu, snappy_parse_kernel in
-// snappy.cu).  Internal, not part of the ABI; device helpers only, no kernels.
+// snappy.cu, lz4_parse_kernel in lz4.cu).  Internal, not part of the ABI; device helpers only, no kernels.
 //   load_window       one 16 KB window of a stream, 16-byte aligned to the absolute address
 //   span_chain        the chain of elements through a span of 1024 candidate starts, by pointer doubling
 //   block_incl_scan / block_excl_scan   one value per thread over a kPqThreads block

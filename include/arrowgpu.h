@@ -975,6 +975,49 @@ ag_status ag_parquet_gzip_decompress_dev(const uint8_t* d_src, const ag_pq_compr
                                          int64_t* d_written, ag_stream_t s);
 
 /* ================================================================================= *
+ * LZ4_RAW page decompression — the same batch contract as SNAPPY above (`ag_pq_compressed` host table, pages in any
+ *   order, `written` in bytes per page, one stream synchronisation in the device flavour, the host flavour stages
+ *   `src` and `dst` and copies back only written bytes, the same argument checks before any launch).
+ *   serializedPageReader.decompress (parquet/file/page_reader.go:597-621) -> compress.Decode
+ *   (parquet/compress/compress.go:107) -> lz4RawCodec.DecodeWithError (parquet/compress/lz4_raw.go:63-70):
+ *   lz4.UncompressBlock (pierrec/lz4 v4) into dst_len bytes.
+ *   Format: an LZ4 block, as pierrec/lz4 v4's block decoder accepts it.  A block is a sequence of sequences:
+ *     - a token byte; the literal length token >> 4, and if that is 15 it continues with extension bytes: each is
+ *       added, and the run ends at the first byte that is not 255;
+ *     - that many literal bytes;
+ *     - if the input ends here, the stream ends cleanly when token & 15 == 0 and is corrupt otherwise;
+ *     - a 2-byte little-endian offset;
+ *     - the match length (token & 15) + 4, continued with extension bytes as the literal length is when the nibble is 15;
+ *     - the match copies from `offset` bytes back and may overlap its own output.  After a match the end of the input
+ *       is a clean end.
+ *   Page outcomes:
+ *     - src_len == 0 && dst_len == 0: success with 0 bytes;
+ *     - a corrupt stream: "parquet: could not decompress page: lz4: invalid source or destination buffer too short"
+ *       (pierrec's ErrInvalidSourceShortBuffer).  Corrupt: an empty source with dst_len > 0; a length extension, the
+ *       literals or the offset cut off by the end of the input; a non-zero match nibble at the end of the input; offset
+ *       0; an offset beyond the bytes produced so far; an element that would write past dst_len.  written counts the
+ *       bytes of the elements before the failing one (a sequence's literal run and its match are separate elements),
+ *       and those bytes are correct;
+ *     - a stream that decodes cleanly to n != dst_len bytes: "parquet: metadata said %d bytes uncompressed data page,
+ *       got %d bytes" with n (page_reader.go:1094-1095); nothing of the page is written and written = 0;
+ *     - every other page of the batch is decoded in full.  The call returns AG_ERR_INVALID naming the lowest failing
+ *       page: "lz4_raw_decompress: page %lld: <message> (%lld bytes written)".
+ *   No byte outside [dst, dst + dst_len) of any page is ever written, on error paths too.
+ *   Differences (DESIGN §2):
+ *     - pierrec/lz4's source is not in the reference tree, so the rules above restate its block decoder;
+ *     - liblz4 (pyarrow's decoder) enforces the end-of-block rules (the last 5 bytes are literals, the last match
+ *       starts at least 12 bytes before the end); pierrec does not, and neither does this library: a stream that ends
+ *       in a match decodes here;
+ *     - liblz4 ignores a non-zero match nibble in the final literal-only sequence, and copies a match with offset 0 from
+ *       the output position itself; here both are corrupt;
+ *     - src_len == 0 && dst_len == 0 is a success (the reference and liblz4 refuse an empty block).
+ * ================================================================================= */
+ag_status ag_parquet_lz4_raw_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                        int64_t* written);
+ag_status ag_parquet_lz4_raw_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                            int64_t* d_written, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

@@ -15,12 +15,12 @@ peak, and a torch.profiler split of the device time over the three stages (value
 --fixed runs only the BOOLEAN and fixed-width cases (ag_parquet_bool_decode_dev / ag_parquet_fixed_decode_dev,
 csrc/fixed.cu): time, share of the HBM peak and a torch.profiler split per kernel.
 
---profile runs only the DELTA_BINARY_PACKED, SNAPPY, ZSTD and GZIP cases, under torch.profiler, and reports the device
-time per call of each kernel (the delta block walk against the value passes, the Snappy parse against the execute, the
-ZSTD walk / literals / sequences / resolve / execute / checksum kernels, the GZIP inflate / execute / CRC32 kernels)
-instead.
+--profile runs only the DELTA_BINARY_PACKED, SNAPPY, ZSTD, GZIP and LZ4_RAW cases, under torch.profiler, and reports the
+device time per call of each kernel (the delta block walk against the value passes, the Snappy parse against the
+execute, the ZSTD walk / literals / sequences / resolve / execute / checksum kernels, the GZIP inflate / execute / CRC32
+kernels, the LZ4 parse against the execute) instead.
 
-The SNAPPY, ZSTD and GZIP cases also print pyarrow's single-thread host decompression of the same pages on this machine's CPU: a CPU
+The SNAPPY, ZSTD, GZIP and LZ4_RAW cases also print pyarrow's single-thread host decompression of the same pages on this machine's CPU: a CPU
 context line, not a baseline of the kernel.
 """
 import argparse
@@ -142,6 +142,7 @@ def main():
         res.update(snappy_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
         res.update(zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
         res.update(gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
+        res.update(lz4_raw_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=True))
         print(json.dumps(res), flush=True)
         return
     dictionary = rng.integers(-(1 << 62), 1 << 62, 100_000)
@@ -174,6 +175,7 @@ def main():
     res.update(snappy_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
     res.update(zstd_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
     res.update(gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
+    res.update(lz4_raw_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer))
     dout.free()
     print(json.dumps(res), flush=True)
 
@@ -184,7 +186,7 @@ def kernel_ms(prof, steps):
     kern = {}
     for ev in prof.key_averages():
         if ev.device_type == torch.autograd.DeviceType.CUDA:
-            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|gz_\w+_kernel|ba_\w+_kernel|fx_\w+_kernel)(<[^>]*>)?", ev.key)
+            m = re.search(r"(delta_\w+_kernel|pq_\w+_kernel|snappy_\w+_kernel|zstd_\w+_kernel|gz_\w+_kernel|lz4_\w+_kernel|ba_\w+_kernel|fx_\w+_kernel)(<[^>]*>)?", ev.key)
             short = (m.group(1) + (m.group(2) or "")) if m else ev.key.strip()
             us = getattr(ev, "device_time_total", None) or ev.cuda_time_total
             kern[short] = kern.get(short, 0.0) + us / 1e3 / steps
@@ -327,11 +329,15 @@ def gzip_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, De
     return codec_cases("gzip", args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile)
 
 
-KERNEL_PREFIX = {"zstd": "zstd_", "gzip": "gz_"}
+def lz4_raw_cases(args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=False):
+    return codec_cases("lz4_raw", args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile)
+
+
+KERNEL_PREFIX = {"zstd": "zstd_", "gzip": "gz_", "lz4_raw": "lz4_"}
 
 
 def codec_cases(codec, args, N, rng, n, n_pages, per_page, timed, upload, line, dout, DeviceBuffer, profile=False):
-    """ZSTD or GZIP (ag_parquet_<codec>_decompress_dev), the page bodies of the SNAPPY cases compressed by pyarrow at its
+    """ZSTD, GZIP or LZ4_RAW (ag_parquet_<codec>_decompress_dev), the page bodies of the SNAPPY cases compressed by pyarrow at its
     default level: (a) PLAIN int64 timestamps; (b) 17-bit dictionary indices; (c) (b) decompressed then dictionary-decoded,
     against the dictionary decode alone; (d) a device-to-device copy of (a)'s decompressed bytes, the floor."""
     import time

@@ -7,11 +7,17 @@
 // Roofline: HBM.  8 algorithmic bytes per row, ~0.125 flop/byte.
 //
 // float64: every accumulator is a (sum, error) pair updated with Knuth's TwoSum (6 dependent-free flops per element,
-// far below what the FP64 pipe can do while the kernel waits on HBM), and partial results are merged the same way, so
-// the value returned is the correctly rounded sum of the inputs up to a relative error of ~n*eps^2 — within 1 ULP of
+// far below what the FP64 pipe can do while the kernel waits on HBM), and partial results are merged the same way.
+// With the errors summed in floating point this is Ogita, Rump and Oishi's Sum2: |res - S| <= 2 eps |S| +
+// gamma_n^2 sum|x| (eps = 2^-53, gamma_n = n eps / (1 - n eps); the 2 covers the final rounding of s + c).  So the
+// result is within 1 ULP of the exactly rounded sum while gamma_n^2 sum|x| is small against eps |S| — 0 ULP from
 // math.fsum at 100M N(0,1) rows (tests/test_gpu_sum.py), where the reference's own three association orders (AVX2 /
-// SSE4 / pure Go, SURVEY §3.4) sit tens to hundreds of ULP apart.  Whenever the exact sum is representable (the
-// reference's tests, integer-valued data) the result is bit-identical to the reference in any order;
+// SSE4 / pure Go, SURVEY §3.4) sit tens to hundreds of ULP apart — and can be many ULP off on badly conditioned data.
+// Whenever every partial sum is exact (the reference's tests, integer-valued data) the result is bit-identical to the
+// reference in any order.  Non-finite inputs: any NaN, or +inf and -inf together, give NaN; infinities or an overflow
+// of one sign give that infinity.  Unspecified, as in the reference's AVX2 order: finite inputs whose partial sums
+// overflow with both signs may give NaN, and then the class may differ from the reference's.  tests/sum_f64_ref.py
+// models this kernel's association bit for bit, so a change to the order below changes that model with it.
 // ag_sum_f64_reforder reproduces the AVX2 order bit for bit on any input.  Integers wrap (any order is exact).
 //
 // Shape of the reduction (fixed => the float64 result is a pure function of (data, n)):
@@ -99,7 +105,9 @@ template <> struct Acc<double> {
   }
   __device__ __forceinline__ void merge(const Acc& o) { add(o.s); c = __dadd_rn(c, o.c); }
   __device__ __forceinline__ Acc shfl_xor(int m) const { Acc r; r.s = shfl_xor_t(s, m); r.c = shfl_xor_t(c, m); return r; }
-  __device__ __forceinline__ double value() const { return __dadd_rn(s, c); }
+  // s is the plain IEEE sum of its chain: once it is ±inf or NaN it stays non-finite through every later add / merge,
+  // and only then can c be NaN (TwoSum's inf - inf), so a non-finite s is the result as it stands.
+  __device__ __forceinline__ double value() const { return isfinite(s) ? __dadd_rn(s, c) : s; }
   __device__ __forceinline__ ulonglong2 raw() const { return make_ulonglong2((unsigned long long)__double_as_longlong(s), (unsigned long long)__double_as_longlong(c)); }
   static __device__ __forceinline__ Acc from_raw(const ulonglong2 v) { Acc r; r.s = __longlong_as_double((long long)v.x); r.c = __longlong_as_double((long long)v.y); return r; }
 };

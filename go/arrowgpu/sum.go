@@ -15,8 +15,10 @@ import (
 // arrow/math/float64.go:25-31), so the GPU reductions are siblings with the same semantics: validity is ignored,
 // values[offset:offset+len] are summed, an empty array gives 0 (float64.go:34-39).
 
-// SumFloat64 returns the sum correctly rounded to within 1 ULP (the reference's AVX2 / SSE4 / pure-Go builds give
-// three different last bits on general data; on exactly representable sums all agree with this one).
+// SumFloat64 returns a compensated sum: |res - S| <= 2 eps |S| + gamma_n^2 sum|x|, so within 1 ULP of the correctly
+// rounded sum on well-conditioned data (the reference's AVX2 / SSE4 / pure-Go builds give three different last bits
+// on general data; when every partial sum is exact all agree with this one).  A NaN, or +inf and -inf together, give
+// NaN; infinities or an overflow of one sign give that infinity.
 func SumFloat64(a *array.Float64) float64 {
 	v := a.Float64Values()
 	if len(v) == 0 {

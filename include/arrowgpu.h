@@ -193,9 +193,15 @@ ag_status ag_flush_l2(ag_stream_t s);
  *   arrow/math/_lib/float64.c:20-26, int64.c:21-27, uint64.c; Go: float64.go:34-39.
  *   Validity is ignored (like the reference); n == 0 gives 0.
  *   Integer sums wrap (two's complement) — bit-exact for any order.
- *   Float64: default mode is a fixed-shape tree (result is a pure function of data
- *   and n, independent of grid/alignment; bit-exact with the reference whenever the
- *   sum is exactly representable, closer to the exact sum otherwise).
+ *   Float64: default mode is a fixed-shape tree of TwoSum (sum, error) pairs (result
+ *   is a pure function of data and n, independent of grid/alignment).  Error bound
+ *   (Sum2): |res - S| <= 2 eps |S| + gamma_n^2 sum|x|, eps = 2^-53, gamma_n =
+ *   n eps / (1 - n eps): within 1 ULP of the exactly rounded sum while gamma_n^2
+ *   sum|x| is small against eps |S|; bit-exact with the reference whenever every
+ *   partial sum is exact.  Any NaN, or +inf and -inf together, gives NaN; infinities
+ *   or an overflow of one sign give that infinity.  Unspecified, as in the reference's
+ *   AVX2 order: finite inputs whose partial sums overflow with both signs may give
+ *   NaN, and then the class may differ from the reference's.
  *   ag_sum_f64_reforder reproduces the reference AVX2 association order
  *   (float64_avx2_amd64.s:36-43,86-164) bit-for-bit on any input.
  * ================================================================================= */

@@ -276,6 +276,40 @@ def test_gpu_general_floats_bounded_and_deterministic(ag, cpu):
 
 
 @gpu
+@pytest.mark.parametrize("t", [N.FLOAT64, N.FLOAT32], ids=lambda t: TYPE_NAME[t])
+def test_gpu_nonfinite_prefix_classes(ag, cpu, t):
+    """±inf and NaN planted inside a tile, at tile edges and on both sides of a look-back group boundary (kScGroup =
+    128 tiles of 32 KB): every prefix has the sequential loop's class (finite, +inf, -inf or NaN) — NaN and infinity
+    bit patterns pass through the look-back's status words — and the finite prefixes before the first planted value
+    keep the bound of test_gpu_general_floats_bounded_and_deterministic.  N(0,1) data: no finite prefix overflows."""
+    dt = NP_OF[t]
+    tile = 32768 // np.dtype(dt).itemsize
+    group = 128 * tile                              # first group boundary: row 524,288 (float64), 1,048,576 (float32)
+    n = group + 3 * tile + 77
+    rng = np.random.default_rng(600 + t)
+    base = rng.standard_normal(n).astype(dt)
+    eps = np.finfo(dt).eps
+    spots = [100, tile - 1, tile, 5 * tile + 17, group - 1, group, group + tile + 3]
+    cases = [{p: v} for p in spots for v in (np.inf, -np.inf, np.nan)]
+    cases += [{group - 1: np.inf, group: -np.inf}, {tile - 1: -np.inf, group + 5: np.inf}, {tile: np.nan, group + 1: np.inf},
+              {100: np.inf, tile: np.inf, group: np.inf}]
+    for spot in cases:
+        x = base.copy()
+        for i, v in spot.items():
+            x[i] = v
+        _, want, _, _, _ = oracle_chunks(cpu, t, [x], [None], False, False)
+        st, got, _, _, _ = gpu_chunks(ag, t, [x], [None], False, False)
+        assert st == 0
+        for cls in (np.isnan, np.isposinf, np.isneginf, np.isfinite):
+            bad = np.flatnonzero(cls(got) != cls(want))
+            assert bad.size == 0, (TYPE_NAME[t], spot, cls.__name__, bad[:5])
+        first = min(spot)
+        exact = np.cumsum(x[:first].astype(np.longdouble))
+        scale = np.cumsum(np.abs(x[:first]).astype(np.longdouble))
+        assert (np.abs(got[:first].astype(np.longdouble) - exact) <= 64 * eps * scale).all(), (TYPE_NAME[t], spot)
+
+
+@gpu
 def test_gpu_streaming_and_general_kernels_share_one_sequence(ag, cpu):
     """Chunks without a bitmap (16-byte aligned: the streaming kernel) and chunks with one (the general
     kernel) alternate inside one sequence; once a null was met (no skip) a later bitmap-free chunk is

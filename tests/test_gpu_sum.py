@@ -89,8 +89,10 @@ def test_f64_reference_order_mode_bit_exact_on_general_data(ag, cpu, ref, n):
 def test_f64_general_data_accuracy(ag, cpu, n, dist):
     """Dataset G, SURVEY §8d acceptance: the GPU sum is within 1 ULP of the exactly rounded sum (math.fsum) and no
     farther from the reference-order result than the reference is from exact (+1 ULP).  The kernel carries the
-    rounding error of every addition (TwoSum), so this holds whatever the condition number — "cancelling" is N(0,1)
-    data followed by its own negation plus a small tail (sum|x| / |sum x| ~ 1e9)."""
+    rounding error of every addition (TwoSum, summed in floating point: Sum2), so |res - S| <= 2 eps |S| +
+    gamma_n^2 sum|x|; 1 ULP holds while gamma_n^2 sum|x| is small against eps |S|, which covers these families —
+    "cancelling" is N(0,1) data followed by its own negation plus a small tail (sum|x| / |sum x| ~ 1e9).  Worse
+    conditioned data, where only the bound holds, and non-finite inputs are in test_gpu_sum_special.py."""
     rng = np.random.default_rng(0x94378165)
     if dist == "normal":
         x = rng.standard_normal(n)
@@ -112,7 +114,8 @@ def test_f64_general_data_accuracy(ag, cpu, n, dist):
 def test_f64_dataset_g_100m_rows_reports_ulp(ag, cpu, record_property):
     """BASELINE config size, dataset G (N(0,1), seed 0x94378165): report the ULP distance of the GPU sum to the exactly
     rounded sum and to the reference-order (AVX2) result, and of the reference to exact (SURVEY §8d asks for the
-    numbers); accept on <= 1 ULP from exact.  The reference-order mode must reproduce the AVX2 bits at this size too."""
+    numbers); accept on <= 1 ULP from exact, which the Sum2 bound (2 eps |S| + gamma_n^2 sum|x|) gives for N(0,1) data
+    even at 100M rows.  The reference-order mode must reproduce the AVX2 bits at this size too."""
     n = 100_000_000
     x = np.random.default_rng(0x94378165).standard_normal(n)
     exact = math.fsum(x)

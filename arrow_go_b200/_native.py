@@ -49,6 +49,24 @@ class PqPage(C.Structure):
     _fields_ = [("data", C.c_int64), ("len", C.c_int64), ("num_values", C.c_int64), ("out", C.c_int64)]
 
 
+class DictChunk(C.Structure):
+    """ag_dict_chunk: one chunk of a dictionary_encode call (values in, int32 indices out)."""
+    _fields_ = [("values", C.c_void_p), ("validity", C.c_void_p), ("offset", C.c_int64), ("length", C.c_int64),
+                ("indices", C.c_void_p), ("indices_validity", C.c_void_p)]
+
+
+def dict_chunk_table(chunks):
+    """[(values, validity, offset, length, indices, indices_validity), ...] -> ctypes array of ag_dict_chunk."""
+    arr = (DictChunk * max(len(chunks), 1))()
+    for k, c in enumerate(chunks):
+        for name, v in zip(("values", "validity", "offset", "length", "indices", "indices_validity"), c):
+            setattr(arr[k], name, v)
+    return arr
+
+
+NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1
+TYPE_DICTIONARY = 29
+
 PQ_LEVELS_V2_RLE, PQ_LEVELS_V1_RLE, PQ_LEVELS_BIT_PACKED = 0, 1, 2
 # include/arrowgpu.h AG_PQ_ENC_* (parquet.thrift Encoding values)
 PQ_ENC_PLAIN, PQ_ENC_PLAIN_DICTIONARY, PQ_ENC_DELTA_LENGTH_BYTE_ARRAY, PQ_ENC_DELTA_BYTE_ARRAY, PQ_ENC_RLE_DICTIONARY = 0, 2, 6, 7, 8
@@ -205,6 +223,8 @@ _SIGS = {
     "ag_is_in_dev": [_i, _p, _p, _i64, _i64, _p, _p, _i64, _i64, _i, _p, _p, _p, _p],
     "ag_unique": [_i, _p, _p, _i64, _i64, _p, _p, _pi64, _pi64],
     "ag_unique_dev": [_i, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p],
+    "ag_dictionary_encode": [_i, _p, _i64, _i, _p, _p, _p],
+    "ag_dictionary_encode_dev": [_i, _p, _i64, _i, _p, _p, _p, _p],
     "ag_sort_indices": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64],
     "ag_sort_indices_dev": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64, _p],
     "ag_parquet_unpack32": [_p, _p, _i64, _i, _pi64],
@@ -279,8 +299,12 @@ DEVICE_CPU, DEVICE_CUDA, DEVICE_CUDA_HOST, DEVICE_CUDA_MANAGED = 1, 2, 3, 13
 _SIGS.update({
     "ag_schema_format_to_type": [C.c_char_p, C.POINTER(_i)],
     "ag_device_array_describe": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), C.POINTER(ArrayView)],
+    "ag_dictionary_device_array_describe": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), C.POINTER(ArrayView), C.POINTER(ArrayView)],
     "ag_export_device_array": [_i, _i64, _i64, _i64, _p, _p, RELEASE_BUFFERS_FN, _p, _p, C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema)],
     "ag_import_device_array": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), _p, C.POINTER(ArrayView)],
+    "ag_export_dictionary_device_array": [_i, _i64, _i64, _i64, _p, _p, _i64, _i64, _i64, _p, _p, RELEASE_BUFFERS_FN, _p, _p,
+                                          C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema)],
+    "ag_import_dictionary_device_array": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), _p, C.POINTER(ArrayView), C.POINTER(ArrayView)],
 })
 
 _SPECIAL = {

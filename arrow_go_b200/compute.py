@@ -26,7 +26,9 @@ NA, BOOL, UINT8, INT8, UINT16, INT16, UINT32, INT32, UINT64, INT64, FLOAT16, FLO
 NP_OF = {UINT8: np.uint8, INT8: np.int8, UINT16: np.uint16, INT16: np.int16, UINT32: np.uint32, INT32: np.int32,
          UINT64: np.uint64, INT64: np.int64, FLOAT32: np.float32, FLOAT64: np.float64}
 TYPE_OF_NP = {np.dtype(v): k for k, v in NP_OF.items()}
+DICTIONARY = 29   # Dictionary<int32, T>
 DROP_NULLS, EMIT_NULLS = 0, 1
+NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1   # DictionaryEncodeOptions.NullEncoding
 KIND_SCALAR, KIND_ARRAY, KIND_CHUNKED = 1, 2, 3
 
 
@@ -66,6 +68,9 @@ def lib():
             getattr(h, nm).argtypes = [p]
             getattr(h, nm).restype = i64
         h.agx_chunk.argtypes = [p, i, pp]
+        h.agx_value_type.argtypes = [p]
+        h.agx_dictionary_indices.argtypes = [p, pp]
+        h.agx_dictionary_values.argtypes = [p, pp]
         h.agx_array_to_host.argtypes = [p, p, p, C.POINTER(i64)]
         h.agx_call_function.argtypes = [C.c_char_p, i, i, pp, i, pp]
         h.agx_arith.argtypes = [i, i, p, p, pp]
@@ -119,6 +124,28 @@ class Datum:
     def __len__(self):
         return int(lib().agx_len(self._h))
 
+    # ---- dictionary datums (Dictionary<int32, T>) ----
+    @property
+    def value_type(self):
+        """T of a Dictionary<int32, T> datum; the type itself for any other datum."""
+        return lib().agx_value_type(self._h)
+
+    def indices(self):
+        """The int32 indices of a dictionary datum (an array, or a chunked array of the same chunks)."""
+        out = C.c_void_p()
+        _check(lib().agx_dictionary_indices(self._h, C.byref(out)))
+        d = Datum(out)
+        d._keep = self
+        return d
+
+    def dictionary(self):
+        """The dictionary values of a dictionary datum (one array, shared by every chunk)."""
+        out = C.c_void_p()
+        _check(lib().agx_dictionary_values(self._h, C.byref(out)))
+        d = Datum(out)
+        d._keep = self
+        return d
+
     # ---- arrays ----
     @property
     def offset(self):
@@ -163,6 +190,10 @@ class Datum:
         return vals, valid, int(nulls.value)
 
     def to_pylist(self):
+        if self.type == DICTIONARY:   # decoded: the dictionary value of every index, None for a null index
+            dictionary = self.dictionary().to_pylist()
+            idx, valid, _ = self.indices().to_numpy()
+            return [(dictionary[i] if ok else None) for i, ok in zip(idx.tolist(), valid)]
         vals, valid, _ = self.to_numpy()
         return [(v.item() if ok else None) for v, ok in zip(vals, valid)]
 
@@ -227,10 +258,10 @@ def Chunked(chunks, type_id):
 
 def CallFunction(name, args, options=None):
     """compute.CallFunction(ctx, name, opts, args...) — options: None, ("arithmetic", no_check_overflow),
-    ("filter", null_selection) or ("take", bounds_check)."""
+    ("filter", null_selection), ("take", bounds_check) or ("dictionary_encode", null_encoding)."""
     kind, val = 0, 0
     if options is not None:
-        kind = {"arithmetic": 1, "filter": 2, "take": 3}[options[0]]
+        kind = {"arithmetic": 1, "filter": 2, "take": 3, "dictionary_encode": 4}[options[0]]
         val = int(options[1])
     arr = (C.c_void_p * max(len(args), 1))(*[a._h for a in args])
     out = C.c_void_p()
@@ -322,6 +353,13 @@ def Unique(values):
     out = C.c_void_p()
     _check(lib().agx_unique(values._h, C.byref(out)))
     return Datum(out)
+
+
+def DictionaryEncode(values, null_encoding=NULL_ENCODING_MASK):
+    """compute.DictionaryEncode(ctx, DictionaryEncodeOptions{NullEncoding}, values) (arrow/compute/vector_hash.go:105-121):
+    Dictionary<int32, T> with the distinct values in order of first appearance; a chunked input gets one dictionary
+    shared by its (non-empty) chunks."""
+    return CallFunction("dictionary_encode", [values], ("dictionary_encode", null_encoding))
 
 
 def IsIn(values, value_set, null_behavior=NULL_MATCH):

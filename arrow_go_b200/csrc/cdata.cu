@@ -19,6 +19,7 @@ struct ExportState {
   bool have_event;
   void (*release_buffers)(void*);
   void* opaque;
+  struct ArrowArray* dictionary;   // a dictionary array's child (heap), released and freed with the parent
 };
 
 void release_exported_array(struct ArrowArray* a) {
@@ -27,6 +28,10 @@ void release_exported_array(struct ArrowArray* a) {
   if (st) {
     if (st->have_event) cudaEventDestroy(st->event);
     if (st->release_buffers) st->release_buffers(st->opaque);
+    if (st->dictionary) {
+      if (st->dictionary->release) st->dictionary->release(st->dictionary);   // unless the consumer moved it out
+      free(st->dictionary);
+    }
     free(st);
   }
   a->release = nullptr;  // the ABI's "released" marker
@@ -36,6 +41,17 @@ void release_exported_array(struct ArrowArray* a) {
 void release_exported_schema(struct ArrowSchema* s) {
   if (!s || !s->release) return;
   s->release = nullptr;  // format / name point at static strings: nothing to free
+}
+
+// a dictionary schema owns its value schema (heap)
+void release_dictionary_schema(struct ArrowSchema* s) {
+  if (!s || !s->release) return;
+  if (s->dictionary) {
+    if (s->dictionary->release) s->dictionary->release(s->dictionary);
+    free(s->dictionary);
+    s->dictionary = nullptr;
+  }
+  s->release = nullptr;
 }
 
 }  // namespace
@@ -94,6 +110,25 @@ extern "C" ag_status ag_device_array_describe(const struct ArrowDeviceArray* in,
   return AG_OK;
 }
 
+// One level of dictionary: the parent's buffers are the indices (format "i"), the dictionary child a primitive array on
+// the parent's device.  Both are described by ag_device_array_describe on shallow copies without the dictionary link.
+extern "C" ag_status ag_dictionary_device_array_describe(const struct ArrowDeviceArray* in, const struct ArrowSchema* schema,
+                                                         ag_array_view* indices, ag_array_view* dictionary) {
+  if (!in || !schema || !indices || !dictionary) AG_FAIL(AG_ERR_INVALID, "cdata: NULL array / schema / view");
+  if (!in->array.dictionary || !schema->dictionary) AG_FAIL(AG_ERR_INVALID, "cdata: not a dictionary array");
+  if (!schema->format || strcmp(schema->format, "i") != 0)
+    AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "cdata: dictionary indices of format '%s' (only int32 'i')", schema->format ? schema->format : "");
+  struct ArrowDeviceArray parent = *in;
+  parent.array.dictionary = nullptr;
+  struct ArrowSchema parent_schema = *schema;
+  parent_schema.dictionary = nullptr;
+  AG_TRY(ag_device_array_describe(&parent, &parent_schema, indices));
+  struct ArrowDeviceArray child = *in;
+  child.array = *in->array.dictionary;
+  AG_TRY(ag_device_array_describe(&child, schema->dictionary, dictionary));
+  return AG_OK;
+}
+
 extern "C" ag_status ag_export_device_array(int type, int64_t length, int64_t null_count, int64_t offset,
                                             const void* d_validity, const void* d_values,
                                             void (*release_buffers)(void*), void* opaque, ag_stream_t produced_on,
@@ -147,9 +182,9 @@ extern "C" ag_status ag_export_device_array(int type, int64_t length, int64_t nu
   return AG_OK;
 }
 
-extern "C" ag_status ag_import_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on, ag_array_view* out) {
-  AG_TRY(ensure_init());
-  AG_TRY(ag_device_array_describe(in, schema, out));
+namespace {
+// the device checks and the wait of an import
+ag_status import_wait(const struct ArrowDeviceArray* in, ag_stream_t consume_on) {
   switch (in->device_type) {
     case ARROW_DEVICE_CUDA: {
       int dev = 0;
@@ -169,6 +204,59 @@ extern "C" ag_status ag_import_device_array(struct ArrowDeviceArray* in, const s
   if (in->sync_event) {
     cudaEvent_t ev = *static_cast<cudaEvent_t*>(in->sync_event);
     AG_CUDA_TRY(cudaStreamWaitEvent(resolve_stream(consume_on), ev, 0));
+  }
+  return AG_OK;
+}
+}  // namespace
+
+extern "C" ag_status ag_import_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on, ag_array_view* out) {
+  AG_TRY(ensure_init());
+  AG_TRY(ag_device_array_describe(in, schema, out));
+  return import_wait(in, consume_on);
+}
+
+extern "C" ag_status ag_import_dictionary_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on,
+                                                       ag_array_view* indices, ag_array_view* dictionary) {
+  AG_TRY(ensure_init());
+  AG_TRY(ag_dictionary_device_array_describe(in, schema, indices, dictionary));
+  return import_wait(in, consume_on);
+}
+
+extern "C" ag_status ag_export_dictionary_device_array(int value_type, int64_t length, int64_t null_count, int64_t offset,
+                                                       const void* d_index_validity, const int32_t* d_indices,
+                                                       int64_t dict_length, int64_t dict_null_count, int64_t dict_offset,
+                                                       const void* d_dict_validity, const void* d_dict_values,
+                                                       void (*release_buffers)(void*), void* opaque, ag_stream_t produced_on,
+                                                       struct ArrowDeviceArray* out, struct ArrowSchema* out_schema) {
+  AG_TRY(ensure_init());
+  if (!out) AG_FAIL(AG_ERR_INVALID, "cdata: NULL output");
+  const char* value_fmt = ag_type_to_schema_format(value_type);
+  if (!value_fmt) AG_FAIL(AG_ERR_TYPE, "cdata: unsupported dictionary value type id %d", value_type);
+  if (dict_length < 0 || dict_offset < 0) AG_FAIL(AG_ERR_INVALID, "cdata: negative dictionary length or offset");
+  if (dict_length > 0 && !d_dict_values) AG_FAIL(AG_ERR_INVALID, "cdata: NULL dictionary values buffer");
+  struct ArrowArray* child = static_cast<struct ArrowArray*>(calloc(1, sizeof(struct ArrowArray)));
+  struct ArrowSchema* child_schema = out_schema ? static_cast<struct ArrowSchema*>(calloc(1, sizeof(struct ArrowSchema))) : nullptr;
+  if (!child || (out_schema && !child_schema)) { free(child); free(child_schema); AG_FAIL(AG_ERR_OOM, "cdata: out of host memory"); }
+  // the child: a primitive export whose buffers the parent's release_buffers covers
+  struct ArrowDeviceArray tmp;
+  ag_status rc = ag_export_device_array(value_type, dict_length, dict_null_count, dict_offset, d_dict_validity, d_dict_values, nullptr, nullptr,
+                                        produced_on, &tmp, child_schema);
+  if (rc != AG_OK) { free(child); free(child_schema); return rc; }
+  *child = tmp.array;
+  // the parent: the int32 indices; its release runs release_buffers and then releases the child
+  rc = ag_export_device_array(AG_TYPE_INT32, length, null_count, offset, d_index_validity, d_indices, release_buffers, opaque, produced_on,
+                              out, out_schema);
+  if (rc != AG_OK) {
+    child->release(child);
+    free(child);
+    if (child_schema) { child_schema->release(child_schema); free(child_schema); }
+    return rc;
+  }
+  static_cast<ExportState*>(out->array.private_data)->dictionary = child;
+  out->array.dictionary = child;
+  if (out_schema) {
+    out_schema->dictionary = child_schema;
+    out_schema->release = release_dictionary_schema;
   }
   return AG_OK;
 }

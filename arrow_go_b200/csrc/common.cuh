@@ -124,6 +124,8 @@ ag_status is_in_dev(int bit_width, const void* vals, const uint8_t* valid, int64
                     int64_t set_off, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid, int64_t* d_null_count, cudaStream_t st);
 ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int64_t off, int64_t n, void* out, uint8_t* out_valid, int64_t capacity,
                      int64_t* d_out_len, cudaStream_t st);
+ag_status dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* dict,
+                                uint8_t* dict_valid, int64_t* d_counts, cudaStream_t st);
 // sort.cu
 ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int64_t voff, int64_t n, int order, int null_placement,
                            uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);

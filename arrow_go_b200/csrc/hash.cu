@@ -1,4 +1,4 @@
-// hash.cu — is_in and unique for fixed-width columns on sm_90a (SURVEY §8f rank 3).
+// hash.cu — is_in, unique and dictionary_encode for fixed-width columns on sm_90a (SURVEY §8f rank 3).
 //
 // Replaces, for 1/2/4/8-byte values, the memo-table kernels of the reference:
 //   is_in   arrow/compute/internal/kernels/scalar_set_lookup.go:112-413 (SetLookupState.Init builds a memo table of
@@ -6,7 +6,9 @@
 //           payload, -0.0 != +0.0; isInKernelExec :373-413 writes a data bit and a validity bit per row by the
 //           NullMatchingBehavior table restated in is_in_kernel below);
 //   unique  arrow/compute/internal/kernels/vector_hash.go (the distinct values in order of FIRST appearance, a null
-//           kept once at the position of its first appearance).
+//           kept once at the position of its first appearance);
+//   dictionary_encode  kernels/vector_hash.go:144-241 (int32 indices into the distinct values in order of first
+//           appearance over every chunk of a column; a null masked, or encoded as one entry where it first appears).
 // Both sit on the same open-addressing table: 16-byte slots {64-bit key = the value's bytes zero-extended, lowest row
 // that carried the key}, linear probing from an even slot (so a probe can always look at an aligned pair), load factor
 // <= 0.5, keys inserted with atomicCAS, first rows with atomicMin.  The first row is all `unique` needs: a row is
@@ -109,11 +111,12 @@ __device__ __forceinline__ int warp_cache_slot(unsigned long long key) {
   return (int)(((key ^ (key >> 32)) * 0x9E3779B97F4A7C15ull) >> 56);
 }
 
-// `run_if`: NULL, or a device word the kernel tests first (the full-size pass of `unique` runs only after an overflow)
+// `run_if`: NULL, or a device word the kernel tests first (the full-size pass of `unique` runs only after an overflow).
+// `row_base`: the row number of the first value (dictionary_encode numbers the rows of all chunks of a column in turn)
 template <typename V>
 __global__ void __launch_bounds__(kHThreads)
 hash_insert_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid, int64_t off, int64_t n, const HashTable t,
-                   const unsigned* __restrict__ run_if) {
+                   const unsigned* __restrict__ run_if, unsigned row_base) {
   __shared__ unsigned long long s_cache[kHWarps][kWarpCacheSlots];
   if (run_if && *run_if != 1u) return;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -141,7 +144,7 @@ hash_insert_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid
     }
 #pragma unroll
     for (int k = 0; k < kHUnroll; ++k) {
-      const unsigned row = (unsigned)(((w0 + k) << 5) + lane);
+      const unsigned row = row_base + (unsigned)(((w0 + k) << 5) + lane);
       const unsigned long long key = (unsigned long long)x[k];
       const int cs = warp_cache_slot(key);
       const bool ones = sizeof(V) == 8 && key == kEmptyKey;     // narrower values zero-extend: never all ones
@@ -293,20 +296,22 @@ is_in_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid, int6
   if (lane < kHUnroll && nulls && null_count) atomicAdd(null_count, nulls);
 }
 
-// unique: row i is kept iff it is the first row of its key (or the first null row).  `big` is the full-size table of an
-// overflowed call (slots == NULL when the call has only one table).
+// The complete table of a call: `big` (the full-size table; slots == NULL when the call has only one table) when the
+// small one overflowed, else the small one.
+__device__ __forceinline__ HashTable live_table(const HashTable& small_t, const HashTable& big_t) {
+  const bool use_big = big_t.slots && overflowed(small_t);
+  HashTable t = use_big ? big_t : small_t;
+  t.cap = kNoCap;
+  return t;
+}
+
+// unique: row i is kept iff it is the first row of its key (or the first null row).
 template <typename V>
 __global__ void __launch_bounds__(kHThreads)
 unique_mark_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid, int64_t off, int64_t n, const HashTable small_t,
                    const HashTable big_t, uint32_t* __restrict__ keep) {
   __shared__ unsigned long long s_cache[kHWarps][kWarpCacheSlots];
-  const bool use_big = big_t.slots && overflowed(small_t);
-  HashTable t;
-  t.slots = use_big ? big_t.slots : small_t.slots;
-  t.mask = use_big ? big_t.mask : small_t.mask;
-  t.shift = use_big ? big_t.shift : small_t.shift;
-  t.cap = kNoCap;
-  t.special = use_big ? big_t.special : small_t.special;
+  const HashTable t = live_table(small_t, big_t);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned long long* cache = s_cache[warp];
   for (int i = lane; i < kWarpCacheSlots; i += 32) cache[i] = kEmptyKey;
@@ -397,7 +402,7 @@ static ag_status is_in_t(const void* vals, const uint8_t* valid, int64_t off, in
     if (kSmall && cudaMemsetAsync(bits, 0, 8192, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break; }
     if (set_n > 0) {
       if constexpr (kSmall) set_bitmap_kernel<V><<<grid_for(set_n, kHThreads, 8), kHThreads, 0, st>>>(reinterpret_cast<const V*>(set), set_valid, set_off, set_n, bits, tm.t.special);
-      else hash_insert_kernel<V><<<grid_for(set_n, kHThreads * kHUnroll, 8), kHThreads, 0, st>>>(reinterpret_cast<const V*>(set), set_valid, set_off, set_n, tm.t, nullptr);
+      else hash_insert_kernel<V><<<grid_for(set_n, kHThreads * kHUnroll, 8), kHThreads, 0, st>>>(reinterpret_cast<const V*>(set), set_valid, set_off, set_n, tm.t, nullptr, 0u);
       if ((rc = check_launch("is_in set kernel")) != AG_OK) break;
     }
     if (d_null_count && cudaMemsetAsync(d_null_count, 0, 8, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break; }
@@ -457,12 +462,12 @@ static ag_status unique_t(int bit_width, const void* vals, const uint8_t* valid,
     if ((rc = dev_alloc_async((void**)&keep, (size_t)((n + 31) / 32) * 4 + 64, st)) != AG_OK) break;
     const V* v = reinterpret_cast<const V*>(vals);
     const int grid = grid_for(n, kHThreads * kHUnroll, 8);
-    hash_insert_kernel<V><<<grid, kHThreads, 0, st>>>(v, valid, off, n, small_t.t, nullptr);
+    hash_insert_kernel<V><<<grid, kHThreads, 0, st>>>(v, valid, off, n, small_t.t, nullptr, 0u);
     if ((rc = check_launch("hash_insert_kernel")) != AG_OK) break;
     if (two) {
       const unsigned* raised = small_t.t.special + 3;
       if ((rc = big_t.clear(st, raised)) != AG_OK) break;
-      hash_insert_kernel<V><<<grid, kHThreads, 0, st>>>(v, valid, off, n, big_t.t, raised);
+      hash_insert_kernel<V><<<grid, kHThreads, 0, st>>>(v, valid, off, n, big_t.t, raised, 0u);
       if ((rc = check_launch("hash_insert_kernel")) != AG_OK) break;
     }
     unique_mark_kernel<V><<<grid, kHThreads, 0, st>>>(v, valid, off, n, small_t.t, big_t.t, keep);
@@ -492,6 +497,236 @@ ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int6
   }, [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "unique: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width); });
 }
 
+// ---- dictionary_encode ----------------------------------------------------------------------------------------------
+// After `unique`'s inserts over every chunk (rows numbered across chunks), a key's dictionary index is the number of
+// first rows below its own first row: the rank of its bit in an n-bit bitmap of first rows.
+//   dict_first_bits_kernel  sets bit `first` of every live slot, of the all-ones key and (Encode) of the null;
+//   popcounts of the bitmap words -> cumulative_sum (scan.cu) -> inclusive word counts;
+//   dict_rank_kernel        writes each slot's rank into Slot::pad and the key into dict[rank], the ranks of the
+//                           all-ones key and of the null into special[4] / special[5], and the dictionary length;
+//   dict_index_kernel       probes the table for every row of a chunk: coalesced int32 indices, ballot validity.
+// special[4] / special[5] keep the clear's all-ones until the rank pass writes them.
+
+__global__ void __launch_bounds__(kHThreads)
+dict_first_bits_kernel(const HashTable small_t, const HashTable big_t, int encode_null, uint32_t* __restrict__ bits) {
+  const HashTable t = live_table(small_t, big_t);
+  const int64_t slots = (int64_t)t.mask + 1;
+  for (int64_t i = (int64_t)blockIdx.x * kHThreads + threadIdx.x; i < slots; i += (int64_t)gridDim.x * kHThreads) {
+    const ulonglong2 raw = __ldcs(reinterpret_cast<const ulonglong2*>(t.slots + i));
+    if (raw.x != kEmptyKey) { const unsigned f = (unsigned)raw.y; atomicOr(&bits[f >> 5], 1u << (f & 31)); }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const unsigned ones = t.special[0], null_row = t.special[1];
+    if (ones != kNoRow) atomicOr(&bits[ones >> 5], 1u << (ones & 31));
+    if (encode_null && null_row != kNoRow) atomicOr(&bits[null_row >> 5], 1u << (null_row & 31));
+  }
+}
+
+__global__ void __launch_bounds__(kHThreads)
+bit_word_popc_kernel(const uint32_t* __restrict__ bits, int64_t n_words, int* __restrict__ counts) {
+  for (int64_t i = (int64_t)blockIdx.x * kHThreads + threadIdx.x; i < n_words; i += (int64_t)gridDim.x * kHThreads) counts[i] = __popc(bits[i]);
+}
+
+// rank of row f (a set bit): the set bits below it
+__device__ __forceinline__ unsigned first_row_rank(const uint32_t* __restrict__ bits, const int* __restrict__ incl, unsigned f) {
+  return (unsigned)incl[f >> 5] - (unsigned)__popc(bits[f >> 5] >> (f & 31));
+}
+
+template <typename V>
+__global__ void __launch_bounds__(kHThreads)
+dict_rank_kernel(const HashTable small_t, const HashTable big_t, int encode_null, const uint32_t* __restrict__ bits,
+                 const int* __restrict__ incl, int64_t n_words, V* __restrict__ dict, uint8_t* __restrict__ dict_valid,
+                 int64_t* __restrict__ dict_len) {   // dict_len: {dictionary length, dictionary null count}, cleared
+  const HashTable t = live_table(small_t, big_t);
+  const int64_t slots = (int64_t)t.mask + 1;
+  for (int64_t i = (int64_t)blockIdx.x * kHThreads + threadIdx.x; i < slots; i += (int64_t)gridDim.x * kHThreads) {
+    const ulonglong2 raw = *reinterpret_cast<const ulonglong2*>(t.slots + i);
+    if (raw.x == kEmptyKey) continue;
+    const unsigned r = first_row_rank(bits, incl, (unsigned)raw.y);
+    t.slots[i].pad = r;
+    dict[r] = (V)raw.x;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const unsigned ones = t.special[0], null_row = t.special[1];
+    if (ones != kNoRow) { const unsigned r = first_row_rank(bits, incl, ones); t.special[4] = r; dict[r] = (V)kEmptyKey; }
+    if (encode_null && null_row != kNoRow) {
+      const unsigned r = first_row_rank(bits, incl, null_row);
+      t.special[5] = r;
+      dict[r] = V(0);
+      if (dict_valid) dict_valid[r >> 3] &= (uint8_t)~(1u << (r & 7));
+      dict_len[1] = 1;   // the dictionary's null count
+    }
+    dict_len[0] = incl[n_words - 1];
+  }
+}
+
+// the dictionary index of a key of the complete table
+__device__ __forceinline__ unsigned table_index(const HashTable& t, unsigned long long key) {
+  unsigned long long h = hash_slot(key, t.shift);
+  while (true) {
+    const ulonglong2 raw = *reinterpret_cast<const ulonglong2*>(t.slots + h);
+    if (raw.x == key) return (unsigned)(raw.y >> 32);   // Slot::pad
+    h = (h + 1) & t.mask;
+  }
+}
+
+// indices of one chunk; `out_valid` (Mask mode, chunk with a validity bitmap) gets one ballot word per 32 rows
+template <typename V>
+__global__ void __launch_bounds__(kHThreads)
+dict_index_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid, int64_t off, int64_t n, const HashTable small_t,
+                  const HashTable big_t, int encode_null, int32_t* __restrict__ out, uint32_t* __restrict__ out_valid,
+                  unsigned long long* __restrict__ null_count) {
+  const HashTable t = live_table(small_t, big_t);
+  const unsigned ones_index = t.special[4];
+  const unsigned null_index = encode_null ? t.special[5] : 0u;
+  const int lane = threadIdx.x & 31;
+  const int64_t n_words = (n + 31) >> 5;
+  const int64_t warp0 = ((int64_t)blockIdx.x * kHThreads + threadIdx.x) >> 5;
+  const int64_t warps = ((int64_t)gridDim.x * kHThreads) >> 5;
+  unsigned long long nulls = 0;
+  for (int64_t w0 = warp0 * kHUnroll; w0 < n_words; w0 += warps * kHUnroll) {
+    V x[kHUnroll];
+    int kind[kHUnroll];                                  // 0 nothing, 1 value, 2 null
+    if (!valid && ((w0 + kHUnroll) << 5) <= n) {         // interior, no nulls: unconditional loads
+      const V* __restrict__ p = vals + off + (w0 << 5) + lane;
+#pragma unroll
+      for (int k = 0; k < kHUnroll; ++k) { x[k] = __ldcs(p + 32 * k); kind[k] = 1; }
+    } else {
+#pragma unroll
+      for (int k = 0; k < kHUnroll; ++k) {
+        const int64_t i = ((w0 + k) << 5) + lane;
+        kind[k] = i < n ? ((valid && !bit_is_set(valid, off + i)) ? 2 : 1) : 0;
+        x[k] = kind[k] == 1 ? __ldcs(vals + off + i) : V(0);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kHUnroll; ++k) {
+      const int64_t w = w0 + k;
+      if (w >= n_words) break;   // warp-uniform
+      const int64_t i = (w << 5) + lane;
+      const unsigned long long key = (unsigned long long)x[k];
+      unsigned idx = null_index;
+      if (kind[k] == 1) idx = (sizeof(V) == 8 && key == kEmptyKey) ? ones_index : table_index(t, key);
+      if (kind[k]) __stcs(out + i, (int32_t)idx);
+      if (out_valid) {
+        const uint32_t vbits = __ballot_sync(0xffffffffu, kind[k] == 1);
+        if (lane == 0) {
+          const int64_t rem = n - (w << 5);
+          const uint32_t m = rem >= 32 ? 0xffffffffu : bit_range_mask(0, (int)rem);
+          out_valid[w] = vbits;
+          nulls += __popc(~vbits & m);
+        }
+      }
+    }
+  }
+  if (lane == 0 && nulls) atomicAdd(null_count, nulls);
+}
+
+template <typename V>
+static ag_status dictionary_encode_t(const ag_dict_chunk* chunks, int64_t n_chunks, int64_t total, int null_encoding, void* dict,
+                                     uint8_t* dict_valid, int64_t* d_counts, cudaStream_t st) {
+  const bool two = total > g_unique_small_rows.load(std::memory_order_relaxed);
+  const unsigned long long small_slots = (unsigned long long)g_unique_small_slots.load(std::memory_order_relaxed);
+  const int encode = null_encoding == AG_NULL_ENCODING_ENCODE;
+  const int64_t n_words = (total + 31) / 32;
+  TableMem small_t, big_t;
+  void* scratch = nullptr;
+  ag_status rc = AG_OK;
+  do {
+    if (two) rc = small_t.alloc(0, small_slots, (unsigned)(small_slots / 2), st);
+    else rc = small_t.alloc(total, 1024, kNoCap, st);
+    if (rc != AG_OK) break;
+    if ((rc = small_t.clear(st)) != AG_OK) break;
+    if (two && (rc = big_t.alloc(total, 1024, kNoCap, st)) != AG_OK) break;
+    // first-row bitmap | word popcounts | their inclusive scan | scan state, each region 256-byte aligned (the scan
+    // reads and writes whole vectors)
+    const size_t words_b = ((size_t)n_words * 4 + 255) & ~(size_t)255;
+    if ((rc = dev_alloc_async(&scratch, 3 * words_b + 64, st)) != AG_OK) break;
+    uint32_t* bits = static_cast<uint32_t*>(scratch);
+    int* counts = reinterpret_cast<int*>(static_cast<char*>(scratch) + words_b);
+    int* incl = reinterpret_cast<int*>(static_cast<char*>(scratch) + 2 * words_b);
+    void* scan_state = static_cast<char*>(scratch) + 3 * words_b;
+    if (cudaMemsetAsync(bits, 0, words_b, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break; }
+    if (encode && dict_valid && cudaMemsetAsync(dict_valid, 0xff, (size_t)((total + 7) / 8), st) != cudaSuccess) {
+      rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break;
+    }
+    // inserts: every chunk into the small table, then (only when it overflowed) every chunk into the full-size one
+    for (int pass = 0; pass < (two ? 2 : 1) && rc == AG_OK; ++pass) {
+      const unsigned* raised = pass ? small_t.t.special + 3 : nullptr;
+      if (pass && (rc = big_t.clear(st, raised)) != AG_OK) break;
+      int64_t row = 0;
+      for (int64_t c = 0; c < n_chunks; ++c) {
+        const ag_dict_chunk& ch = chunks[c];
+        if (ch.length == 0) continue;
+        hash_insert_kernel<V><<<grid_for(ch.length, kHThreads * kHUnroll, 8), kHThreads, 0, st>>>(
+            reinterpret_cast<const V*>(ch.values), ch.validity, ch.offset, ch.length, pass ? big_t.t : small_t.t, raised, (unsigned)row);
+        if ((rc = check_launch("hash_insert_kernel")) != AG_OK) break;
+        row += ch.length;
+      }
+    }
+    if (rc != AG_OK) break;
+    // ranks; grids cover the largest table the call may have ended on
+    const int64_t max_slots = (int64_t)((two ? big_t.t.mask : small_t.t.mask) + 1);
+    const int slot_grid = grid_for(max_slots, kHThreads * 4, 8);
+    dict_first_bits_kernel<<<slot_grid, kHThreads, 0, st>>>(small_t.t, big_t.t, encode, bits);
+    if ((rc = check_launch("dict_first_bits_kernel")) != AG_OK) break;
+    bit_word_popc_kernel<<<grid_for(n_words, kHThreads * 4, 8), kHThreads, 0, st>>>(bits, n_words, counts);
+    if ((rc = check_launch("bit_word_popc_kernel")) != AG_OK) break;
+    if ((rc = cumulative_sum_state_init(scan_state, AG_TYPE_INT32, nullptr, st)) != AG_OK) break;
+    if ((rc = cumulative_sum_dev(AG_TYPE_INT32, counts, nullptr, 0, n_words, 0, 0, incl, nullptr, 0, scan_state, nullptr, st)) != AG_OK) break;
+    dict_rank_kernel<V><<<slot_grid, kHThreads, 0, st>>>(small_t.t, big_t.t, encode, bits, incl, n_words, reinterpret_cast<V*>(dict),
+                                                        encode ? dict_valid : nullptr, d_counts);
+    if ((rc = check_launch("dict_rank_kernel")) != AG_OK) break;
+    // indices
+    for (int64_t c = 0; c < n_chunks; ++c) {
+      const ag_dict_chunk& ch = chunks[c];
+      if (ch.length == 0) continue;
+      uint32_t* ov = (!encode && ch.validity) ? reinterpret_cast<uint32_t*>(ch.indices_validity) : nullptr;
+      dict_index_kernel<V><<<grid_for(ch.length, kHThreads * kHUnroll, 8), kHThreads, 0, st>>>(
+          reinterpret_cast<const V*>(ch.values), ch.validity, ch.offset, ch.length, small_t.t, big_t.t, encode, ch.indices, ov,
+          reinterpret_cast<unsigned long long*>(d_counts + 2 + c));
+      if ((rc = check_launch("dict_index_kernel")) != AG_OK) break;
+    }
+  } while (0);
+  if (scratch) cudaFreeAsync(scratch, st);
+  small_t.release(st);
+  big_t.release(st);
+  return rc;
+}
+
+ag_status dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* dict,
+                                uint8_t* dict_valid, int64_t* d_counts, cudaStream_t st) {
+  if (null_encoding != AG_NULL_ENCODING_MASK && null_encoding != AG_NULL_ENCODING_ENCODE)
+    AG_FAIL(AG_ERR_INVALID, "dictionary_encode: invalid null encoding %d", null_encoding);
+  if (n_chunks < 0 || (n_chunks > 0 && !chunks)) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: bad chunk table");
+  if (!d_counts) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: NULL counts");
+  if (bit_width != 8 && bit_width != 16 && bit_width != 32 && bit_width != 64)
+    AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "dictionary_encode: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width);
+  int64_t total = 0;
+  bool any_valid = false;
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_dict_chunk& ch = chunks[c];
+    if (ch.length < 0 || ch.offset < 0) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: negative length or offset", (long long)c);
+    if (ch.length == 0) continue;
+    if (!ch.values || !ch.indices) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: NULL values or indices", (long long)c);
+    if (null_encoding == AG_NULL_ENCODING_MASK && ch.validity && !ch.indices_validity)
+      AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: a chunk with a validity bitmap needs an index validity bitmap", (long long)c);
+    if (reinterpret_cast<uintptr_t>(ch.indices_validity) & 3)
+      AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: the index validity bitmap must be 4-byte aligned", (long long)c);
+    any_valid |= ch.validity != nullptr;
+    total += ch.length;
+    if (total >= (1ll << 31)) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "dictionary_encode: more than 2^31-1 rows per call");
+  }
+  if (total > 0 && !dict) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: NULL dictionary");
+  if (null_encoding == AG_NULL_ENCODING_ENCODE && any_valid && !dict_valid)
+    AG_FAIL(AG_ERR_INVALID, "dictionary_encode: encoding the nulls of an input with validity bitmaps needs a dictionary validity bitmap");
+  AG_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)(n_chunks + 2) * sizeof(int64_t), st));
+  if (total == 0) return AG_OK;
+  return visit_width(bit_width, [&](auto tag) {
+    return dictionary_encode_t<typename decltype(tag)::type>(chunks, n_chunks, total, null_encoding, dict, dict_valid, d_counts, st);
+  }, [] { return AG_OK; });   // the width was checked above
+}
+
 }  // namespace ag
 
 using namespace ag;
@@ -517,4 +752,10 @@ extern "C" ag_status ag_unique_dev(int bit_width, const void* d_vals, const uint
                                    uint8_t* d_out_valid, int64_t capacity, int64_t* d_out_len, ag_stream_t s) {
   AG_TRY(ensure_init());
   return unique_dev(bit_width, d_vals, d_valid, offset, n, d_out, d_out_valid, capacity, d_out_len, resolve_stream(s));
+}
+
+extern "C" ag_status ag_dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* d_dict,
+                                              uint8_t* d_dict_valid, int64_t* d_counts, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  return dictionary_encode_dev(bit_width, chunks, n_chunks, null_encoding, d_dict, d_dict_valid, d_counts, resolve_stream(s));
 }

@@ -783,4 +783,54 @@ ag_status ag_unique(int bit_width, const void* vals, const uint8_t* valid, int64
   return AG_OK;
 }
 
+ag_status ag_dictionary_encode(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* dict,
+                               uint8_t* dict_valid, int64_t* counts) {
+  AG_TRY(ensure_init());
+  if (!counts) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: NULL counts");
+  if (n_chunks < 0 || (n_chunks > 0 && !chunks)) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: bad chunk table");
+  if (bit_width != 8 && bit_width != 16 && bit_width != 32 && bit_width != 64)
+    AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "dictionary_encode: fixed-width values of 1/2/4/8 bytes only (got %d bits)", bit_width);
+  for (int64_t c = 0; c < n_chunks; ++c)
+    if (chunks[c].length < 0 || chunks[c].offset < 0) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: negative length or offset", (long long)c);
+  const int w = bit_width / 8;
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  // device copies of the chunks: values rebased to the validity's bit phase, outputs at offset 0
+  std::vector<ag_dict_chunk> dc((size_t)n_chunks);
+  int64_t total = 0;
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_dict_chunk& h = chunks[c];
+    ag_dict_chunk& d = dc[(size_t)c];
+    d = ag_dict_chunk{nullptr, nullptr, 0, h.length, nullptr, nullptr};
+    total += h.length;
+    if (h.length == 0) continue;
+    if (!h.values || !h.indices) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: chunk %lld: NULL values or indices", (long long)c);
+    uint8_t* dvalid;
+    AG_TRY(upload_column(t, h.values, h.validity, h.offset, h.length, w, &d.values, &dvalid, &d.offset));
+    d.validity = dvalid;
+    AG_TRY(t.alloc_t(&d.indices, (size_t)h.length * 4));
+    if (h.indices_validity) AG_TRY(t.alloc_t(&d.indices_validity, (size_t)((h.length + 31) / 32) * 4));
+  }
+  if (total > 0 && !dict) AG_FAIL(AG_ERR_INVALID, "dictionary_encode: NULL dictionary");
+  void* ddict = nullptr; uint8_t* ddv = nullptr; int64_t* dcounts;
+  if (total > 0) AG_TRY(t.alloc(&ddict, (size_t)total * w));
+  if (dict_valid && total > 0) AG_TRY(t.alloc_t(&ddv, (size_t)((total + 7) / 8)));
+  AG_TRY(t.alloc_t(&dcounts, (size_t)(n_chunks + 2) * 8));
+  AG_TRY(dictionary_encode_dev(bit_width, dc.data(), n_chunks, null_encoding, ddict, ddv, dcounts, cs));
+  AG_TRY(d2h(counts, dcounts, (size_t)(n_chunks + 2) * 8, cs));
+  AG_TRY(sync(cs));
+  const int64_t k = counts[0];
+  AG_TRY(d2h(dict, ddict, (size_t)k * w, cs));
+  if (ddv && null_encoding == AG_NULL_ENCODING_ENCODE) AG_TRY(d2h(dict_valid, ddv, (size_t)((k + 7) / 8), cs));
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_dict_chunk& h = chunks[c];
+    const ag_dict_chunk& d = dc[(size_t)c];
+    if (h.length == 0) continue;
+    AG_TRY(d2h(h.indices, d.indices, (size_t)h.length * 4, cs));
+    if (null_encoding == AG_NULL_ENCODING_MASK && h.validity && h.indices_validity)
+      AG_TRY(d2h(h.indices_validity, d.indices_validity, (size_t)((h.length + 7) / 8), cs));
+  }
+  return sync(cs);
+}
+
 }  // extern "C"

@@ -33,7 +33,8 @@ namespace arrowgpu {
 // ---- arrow.Type (arrow/datatype.go:36-72) -----------------------------------------------
 enum class Type : int {
   NA = 0, BOOL = 1, UINT8 = 2, INT8 = 3, UINT16 = 4, INT16 = 5, UINT32 = 6, INT32 = 7,
-  UINT64 = 8, INT64 = 9, FLOAT16 = 10, FLOAT32 = 11, FLOAT64 = 12
+  UINT64 = 8, INT64 = 9, FLOAT16 = 10, FLOAT32 = 11, FLOAT64 = 12,
+  DICTIONARY = 29  // Dictionary<int32, T> only: indices in buffers[1], the values in ArrayData::dictionary
 };
 int BitWidth(Type t);  // 1 for BOOL
 const char* TypeName(Type t);
@@ -83,7 +84,8 @@ struct ArrayData {
   int64_t length = 0;
   int64_t null_count = 0;  // kUnknownNullCount allowed
   int64_t offset = 0;
-  std::shared_ptr<Buffer> buffers[2];  // [0] validity bitmap (may be null), [1] values / boolean data
+  std::shared_ptr<Buffer> buffers[2];  // [0] validity bitmap (may be null), [1] values / boolean data / int32 indices
+  std::shared_ptr<ArrayData> dictionary;  // DICTIONARY: the dictionary values (a primitive array), shared by slices
   std::shared_ptr<ArrayData> Slice(int64_t off, int64_t len) const;  // array.NewSlice semantics
   // validity (LSB-first bitmap, `offset` applies) may be NULL; values must hold (offset+length) elements
   static Status FromHost(Type type, int64_t length, int64_t offset, const uint8_t* validity, const void* values,
@@ -101,6 +103,7 @@ struct ArrayData {
 
 struct ChunkedArray {  // arrow.Chunked (arrow/table.go:135-143)
   Type type = Type::NA;
+  Type value_type = Type::NA;  // DICTIONARY: the dictionary's value type (known even with zero chunks)
   std::vector<std::shared_ptr<ArrayData>> chunks;
   int64_t length = 0;
   int64_t NullN() const;
@@ -256,6 +259,11 @@ struct SortOptions : FunctionOptions {                        // :46-50 (single 
 };
 enum NullMatchingBehavior { NullMatchingMatch = 0, NullMatchingSkip = 1, NullMatchingEmitNull = 2, NullMatchingInconclusive = 3 };
 struct Datum;
+enum NullEncodingBehavior { NullEncodingMask = 0, NullEncodingEncode = 1 };  // kernels/vector_hash.go:144-160
+struct DictionaryEncodeOptions : FunctionOptions {                            // compute/vector_hash.go:105-121
+  NullEncodingBehavior NullEncoding = NullEncodingMask;
+  const char* TypeName() const override { return "DictionaryEncodeOptions"; }
+};
 struct SetLookupOptions : FunctionOptions {                   // compute/scalar_set_lookup.go (ValueSet, NullBehavior)
   std::shared_ptr<ArrayData> ValueSet;
   NullMatchingBehavior NullBehavior = NullMatchingMatch;
@@ -356,6 +364,9 @@ Status Take(const ExecCtx& ctx, const TakeOptions& opts, const Datum& values, co
 // compute.SortIndices (vector_sort.go:205-211), compute.Unique (vector_hash.go), compute.IsIn (scalar_set_lookup.go)
 Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortOptions& opts, Datum* out);
 Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out);
+// compute.DictionaryEncode (vector_hash.go:105-121): Dictionary<int32, T>; a chunked input gets ONE dictionary for all
+// chunks and loses its empty chunks; a dictionary input is returned as it is
+Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts, const Datum& values, Datum* out);
 Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& values, Datum* out);
 
 // ---- executor internals exposed for tests (exec_internals_test.go exercises the same pieces) ----

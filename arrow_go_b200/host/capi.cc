@@ -37,8 +37,14 @@ int agx_scalar(int type, int valid, const void* value, agx_datum** out) {
 int agx_chunked(int type, agx_datum** chunks, int n, agx_datum** out) {
   auto c = std::make_shared<ChunkedArray>();
   c->type = (Type)type;
+  if (c->type == Type::DICTIONARY) {   // the value type comes from the chunks' dictionaries
+    if (n == 0) return fail(Status::Invalid("chunked: a dictionary column without chunks has no value type"));
+    if (chunks[0]->d.kind == DatumKind::ARRAY && chunks[0]->d.array->dictionary) c->value_type = chunks[0]->d.array->dictionary->type;
+  }
   for (int i = 0; i < n; ++i) {
     if (chunks[i]->d.kind != DatumKind::ARRAY || chunks[i]->d.array->type != c->type) return fail(Status::Invalid("chunked: chunks must be arrays of the chunked type"));
+    if (c->type == Type::DICTIONARY && chunks[i]->d.array->dictionary->type != c->value_type)
+      return fail(Status::Invalid("chunked: dictionary chunks must share one value type"));
     c->chunks.push_back(chunks[i]->d.array);
     c->length += chunks[i]->d.array->length;
   }
@@ -58,6 +64,31 @@ int64_t agx_len(agx_datum* d) { return d->d.Len(); }
 int64_t agx_offset(agx_datum* d) { return d->d.kind == DatumKind::ARRAY ? d->d.array->offset : 0; }
 int agx_has_validity(agx_datum* d) { return d->d.kind == DatumKind::ARRAY && d->d.array->buffers[0] != nullptr; }
 int64_t agx_null_count_raw(agx_datum* d) { return d->d.kind == DatumKind::ARRAY ? d->d.array->null_count : 0; }
+// Dictionary datums: the value type, the int32 indices (same shape as the datum) and the shared dictionary
+int agx_value_type(agx_datum* d) {
+  if (d->d.kind == DatumKind::ARRAY && d->d.array->dictionary) return (int)d->d.array->dictionary->type;
+  if (d->d.kind == DatumKind::CHUNKED && d->d.chunked->type == Type::DICTIONARY) return (int)d->d.chunked->value_type;
+  return (int)d->d.type();
+}
+int agx_dictionary_indices(agx_datum* d, agx_datum** out) {
+  auto indices = [](const std::shared_ptr<ArrayData>& a) { auto r = std::make_shared<ArrayData>(*a); r->type = Type::INT32; r->dictionary = nullptr; return r; };
+  if (d->d.type() != Type::DICTIONARY) return fail(Status::TypeError("indices: not a dictionary datum"));
+  if (d->d.kind == DatumKind::ARRAY) { *out = new agx_datum{Datum(indices(d->d.array))}; return AG_OK; }
+  auto c = std::make_shared<ChunkedArray>(*d->d.chunked);
+  c->type = Type::INT32; c->value_type = Type::NA;
+  for (auto& ch : c->chunks) ch = indices(ch);
+  *out = new agx_datum{Datum(c)};
+  return AG_OK;
+}
+int agx_dictionary_values(agx_datum* d, agx_datum** out) {
+  if (d->d.type() != Type::DICTIONARY) return fail(Status::TypeError("dictionary: not a dictionary datum"));
+  std::shared_ptr<ArrayData> dict;
+  if (d->d.kind == DatumKind::ARRAY) dict = d->d.array->dictionary;
+  else if (!d->d.chunked->chunks.empty()) dict = d->d.chunked->chunks[0]->dictionary;
+  else { AGX_TRY(ArrayData::FromHost(d->d.chunked->value_type, 0, 0, nullptr, nullptr, 0, &dict)); }
+  *out = new agx_datum{Datum(dict)};
+  return AG_OK;
+}
 int agx_num_chunks(agx_datum* d) { return d->d.kind == DatumKind::CHUNKED ? (int)d->d.chunked->chunks.size() : 0; }
 int agx_chunk(agx_datum* d, int i, agx_datum** out) {
   if (d->d.kind != DatumKind::CHUNKED || i < 0 || i >= (int)d->d.chunked->chunks.size()) return fail(Status::Invalid("chunk: out of range"));
@@ -71,15 +102,16 @@ int agx_array_to_host(agx_datum* d, void* values, uint8_t* validity, int64_t* nu
 }
 
 // opt_kind: 0 none, 1 ArithmeticOptions{NoCheckOverflow=opt_value}, 2 FilterOptions{NullSelection=opt_value},
-//           3 TakeOptions{BoundsCheck=opt_value}
+//           3 TakeOptions{BoundsCheck=opt_value}, 4 DictionaryEncodeOptions{NullEncoding=opt_value}
 int agx_call_function(const char* name, int opt_kind, int opt_value, agx_datum** args, int nargs, agx_datum** out) {
   std::vector<Datum> a;
   for (int i = 0; i < nargs; ++i) a.push_back(args[i]->d);
-  ArithmeticOptions ao; FilterOptions fo; TakeOptions to;
+  ArithmeticOptions ao; FilterOptions fo; TakeOptions to; DictionaryEncodeOptions deo;
   const FunctionOptions* opts = nullptr;
   if (opt_kind == 1) { ao.NoCheckOverflow = opt_value != 0; opts = &ao; }
   if (opt_kind == 2) { fo.NullSelection = (NullSelectionBehavior)opt_value; opts = &fo; }
   if (opt_kind == 3) { to.BoundsCheck = opt_value != 0; opts = &to; }
+  if (opt_kind == 4) { deo.NullEncoding = (NullEncodingBehavior)opt_value; opts = &deo; }
   ExecCtx ctx;
   Datum r;
   AGX_TRY(CallFunction(ctx, name, opts, a, &r));

@@ -20,6 +20,7 @@ int BitWidth(Type t) {
   }
 }
 const char* TypeName(Type t) {
+  if (t == Type::DICTIONARY) return "dictionary";
   static const char* names[] = {"null", "bool", "uint8", "int8", "uint16", "int16", "uint32", "int32", "uint64", "int64", "float16", "float32", "float64"};
   const int i = (int)t;
   return (i >= 0 && i <= 12) ? names[i] : "unknown";
@@ -92,11 +93,21 @@ Status Buffer::ToHost(void* host, int64_t nbytes, int64_t byte_offset) const {
 
 // ---------------------------------------------------------------- ArrayData ---------------
 namespace {
-struct ExportedBuffers { std::shared_ptr<Buffer> b[2]; };
+struct ExportedBuffers { std::shared_ptr<Buffer> b[4]; };   // [2], [3]: a dictionary array's dictionary buffers
 void ReleaseExportedBuffers(void* opaque) { delete static_cast<ExportedBuffers*>(opaque); }
 }  // namespace
 
 Status ArrayData::ExportDevice(struct ArrowDeviceArray* out, struct ArrowSchema* out_schema) const {
+  if (type == Type::DICTIONARY) {
+    const ArrayData& d = *dictionary;
+    auto* keep = new ExportedBuffers{{buffers[0], buffers[1], d.buffers[0], d.buffers[1]}};
+    const int rc = ag_export_dictionary_device_array((int)d.type, length, null_count, offset, buffers[0] ? buffers[0]->data() : nullptr,
+                                                     (const int32_t*)buffers[1]->data(), d.length, d.null_count, d.offset,
+                                                     d.buffers[0] ? d.buffers[0]->data() : nullptr, d.buffers[1] ? d.buffers[1]->data() : nullptr,
+                                                     ReleaseExportedBuffers, keep, nullptr, out, out_schema);
+    if (rc != AG_OK) { delete keep; return Status::FromNative(rc); }
+    return Status::OK();
+  }
   auto* keep = new ExportedBuffers{{buffers[0], buffers[1]}};
   const int rc = ag_export_device_array((int)type, length, null_count, offset, buffers[0] ? buffers[0]->data() : nullptr,
                                         buffers[1] ? buffers[1]->data() : nullptr, ReleaseExportedBuffers, keep, nullptr, out, out_schema);
@@ -105,8 +116,14 @@ Status ArrayData::ExportDevice(struct ArrowDeviceArray* out, struct ArrowSchema*
 }
 
 Status ArrayData::ImportDevice(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, std::shared_ptr<ArrayData>* out) {
-  ag_array_view v;
-  NATIVE(ag_import_device_array(in, schema, nullptr, &v));
+  const bool dict = in && in->array.dictionary;
+  ag_array_view v, dv{};
+  if (dict) {
+    if (!schema) return Status::Invalid("import: a schema is required");
+    NATIVE(ag_import_dictionary_device_array(in, schema, nullptr, &v, &dv));
+  } else {
+    NATIVE(ag_import_device_array(in, schema, nullptr, &v));
+  }
   if (v.type == 0) return Status::Invalid("import: a schema is required");
   // move the struct: the importer owns it now (C Data Interface "moving an array")
   auto owned = std::make_shared<ArrowDeviceArray>(*in);
@@ -118,6 +135,15 @@ Status ArrayData::ImportDevice(struct ArrowDeviceArray* in, const struct ArrowSc
   if (v.validity) d->buffers[0] = Buffer::Wrap(v.validity, BytesForBits(n), [releaser] {});
   d->buffers[1] = Buffer::Wrap(v.values, DataBytes((Type)v.type, n), [releaser] {});
   if (!v.validity) d->null_count = 0;
+  if (dict) {   // the indices and the dictionary keep the parent alive; its release releases the dictionary
+    d->type = Type::DICTIONARY;
+    auto c = std::make_shared<ArrayData>();
+    c->type = (Type)dv.type; c->length = dv.length; c->offset = dv.offset; c->null_count = dv.validity ? dv.null_count : 0;
+    const int64_t m = dv.offset + dv.length;
+    if (dv.validity) c->buffers[0] = Buffer::Wrap(dv.validity, BytesForBits(m), [releaser] {});
+    c->buffers[1] = Buffer::Wrap(dv.values, DataBytes(c->type, m), [releaser] {});
+    d->dictionary = c;
+  }
   *out = d;
   return Status::OK();
 }
@@ -144,6 +170,7 @@ Status ArrayData::FromHost(Type type, int64_t length, int64_t offset, const uint
 }
 
 Status ArrayData::ToHost(void* values, uint8_t* validity, int64_t* null_count_out) const {
+  if (type == Type::DICTIONARY) return Status::TypeError("to_host: a dictionary array is read through its indices and dictionary");
   if (length == 0) { if (null_count_out) *null_count_out = 0; return Status::OK(); }
   const int w = BitWidth(type);
   if (values) {
@@ -716,6 +743,10 @@ Status CallFunction(const ExecCtx& ctx, const std::string& name, const FunctionO
   FunctionRegistry* reg = ctx.Registry ? ctx.Registry : GetFunctionRegistry();
   const Function* fn = reg->GetFunction(name);
   if (!fn) return Status::Make(AG_ERR_INVALID, "no function registered with name: " + name);  // arrow.ErrKey
+  // dictionary arrays reach the kernels only through dictionary_encode (its identity case)
+  if (name != "dictionary_encode")
+    for (auto& a : args)
+      if (a.kind != DatumKind::NONE && a.type() == Type::DICTIONARY) return Status::NotImplemented("function '" + name + "' has no kernel for dictionary arguments");
   return fn->Execute(ctx, opts, args, out);
 }
 
@@ -1501,6 +1532,12 @@ FunctionRegistry* GetFunctionRegistry() {
       if (args.size() != 1) return Status::Invalid("unique takes one argument");
       return Unique(ctx, args[0], out);
     }), false);
+    reg->AddFunction(std::make_shared<MetaFunction>("dictionary_encode", 1, [](const ExecCtx& ctx, const FunctionOptions* fo, const std::vector<Datum>& args, Datum* out) -> Status {
+      const auto* o = dynamic_cast<const DictionaryEncodeOptions*>(fo);
+      if (fo && !o) return Status::Invalid(std::string("dictionary_encode: expected DictionaryEncodeOptions, got ") + fo->TypeName());
+      if (args.size() != 1) return Status::Invalid("dictionary_encode takes one argument");
+      return DictionaryEncode(ctx, o ? *o : DictionaryEncodeOptions(), args[0], out);
+    }), false);
     reg->AddFunction(std::make_shared<MetaFunction>("is_in", 1, [](const ExecCtx& ctx, const FunctionOptions* fo, const std::vector<Datum>& args, Datum* out) -> Status {
       const auto* so = dynamic_cast<const SetLookupOptions*>(fo);
       if (!so) return Status::Invalid("is_in requires SetLookupOptions");
@@ -1674,6 +1711,65 @@ Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out) {
   int64_t k = 0;
   RETURN_NOT_OK(len->ToHost(&k, 8));
   return MakeOut(a->type, k, data, valid, has_valid ? kUnknownNullCount : 0, out);
+}
+
+Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts, const Datum& values, Datum* out) {
+  if (opts.NullEncoding != NullEncodingMask && opts.NullEncoding != NullEncodingEncode)
+    return Status::Invalid("dictionary_encode: invalid NullEncodingBehavior " + std::to_string((int)opts.NullEncoding));
+  if (values.type() == Type::DICTIONARY) { *out = values; return Status::OK(); }   // GetVectorHashKernels' identity kernel
+  if (values.kind != DatumKind::ARRAY && values.kind != DatumKind::CHUNKED) return Status::NotImplemented("dictionary_encode takes an array-like argument");
+  const Type t = values.type();
+  const int bw = BitWidth(t);
+  if (bw != 8 && bw != 16 && bw != 32 && bw != 64) return Status::NotImplemented(std::string("dictionary_encode: unsupported type ") + TypeName(t));
+  const std::vector<std::shared_ptr<ArrayData>> in = values.kind == DatumKind::ARRAY ? std::vector<std::shared_ptr<ArrayData>>{values.array} : values.chunked->chunks;
+  const bool encode = opts.NullEncoding == NullEncodingEncode;
+  int64_t total = 0;
+  for (auto& a : in) total += a->length;
+  if (total >= ((int64_t)1 << 31)) return Status::NotImplemented("dictionary_encode: more than 2^31-1 rows");
+  bool any_valid = false;
+  std::vector<ag_dict_chunk> desc(in.size());
+  std::vector<std::shared_ptr<Buffer>> idx(in.size()), idx_valid(in.size());
+  for (size_t c = 0; c < in.size(); ++c) {
+    const ArrayData& a = *in[c];
+    const bool has_valid = a.buffers[0] && a.null_count != 0;
+    any_valid |= has_valid;
+    RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(a.length, 1) * 4, &idx[c]));
+    if (has_valid && !encode) RETURN_NOT_OK(Buffer::Allocate(((a.length + 31) / 32) * 4, &idx_valid[c]));
+    desc[c] = ag_dict_chunk{a.buffers[1] ? a.buffers[1]->data() : nullptr, has_valid ? a.buffers[0]->data() : nullptr, a.offset, a.length,
+                            (int32_t*)idx[c]->data(), idx_valid[c] ? idx_valid[c]->data() : nullptr};
+  }
+  // the call's dictionary has room for every row; the result keeps a copy of its k values only
+  std::shared_ptr<Buffer> scratch, scratch_valid, counts;
+  RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(total, 1) * (bw / 8), &scratch));
+  if (encode && any_valid) RETURN_NOT_OK(Buffer::Allocate((total + 7) / 8, &scratch_valid));
+  RETURN_NOT_OK(Buffer::Allocate(((int64_t)in.size() + 2) * 8, &counts));
+  NATIVE(ag_dictionary_encode_dev(bw, desc.data(), (int64_t)desc.size(), (int)opts.NullEncoding, scratch->data(),
+                                  scratch_valid ? scratch_valid->data() : nullptr, (int64_t*)counts->data(), nullptr));
+  std::vector<int64_t> cnt(in.size() + 2);
+  RETURN_NOT_OK(counts->ToHost(cnt.data(), (int64_t)cnt.size() * 8));
+  auto dict = std::make_shared<ArrayData>();
+  dict->type = t; dict->length = cnt[0]; dict->null_count = cnt[1];
+  RETURN_NOT_OK(Buffer::Allocate(cnt[0] * (bw / 8), &dict->buffers[1]));
+  NATIVE(ag_copy_dev(dict->buffers[1]->data(), scratch->data(), (size_t)(cnt[0] * (bw / 8)), nullptr));
+  if (cnt[1] > 0) {
+    RETURN_NOT_OK(Buffer::Allocate((cnt[0] + 7) / 8, &dict->buffers[0]));
+    NATIVE(ag_copy_dev(dict->buffers[0]->data(), scratch_valid->data(), (size_t)((cnt[0] + 7) / 8), nullptr));
+  }
+  NATIVE(ag_stream_sync(nullptr));
+  auto make = [&](size_t c) {
+    auto d = std::make_shared<ArrayData>();
+    d->type = Type::DICTIONARY; d->length = in[c]->length; d->null_count = cnt[2 + c];
+    d->buffers[1] = idx[c];
+    if (d->null_count > 0) d->buffers[0] = idx_valid[c];
+    d->dictionary = dict;
+    return d;
+  };
+  if (values.kind == DatumKind::ARRAY) { *out = Datum(make(0)); return Status::OK(); }
+  auto res = std::make_shared<ChunkedArray>();
+  res->type = Type::DICTIONARY; res->value_type = t; res->length = total;
+  for (size_t c = 0; c < in.size(); ++c) if (in[c]->length > 0) res->chunks.push_back(make(c));   // WrapResults drops empty chunks
+  *out = Datum(res);
+  return Status::OK();
 }
 
 Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& values, Datum* out) {

@@ -167,6 +167,121 @@ func uniqueFunction() *compute.VectorFunction {
 	return fn
 }
 
+// ---- dictionary_encode (vector_hash.go:105-121, kernels/vector_hash.go:144-241) --------------------------------------
+//
+// Not chunk-wise: the dictionary is shared by every chunk and built over the whole column, so ExecChunked hands all
+// chunks to ONE ag_dictionary_encode call (rows numbered across chunks) instead of concatenating them.  Output:
+// Dictionary<int32, T>; empty chunks are dropped by the executor's WrapResults as in the reference.
+
+func dictEncodeNulls(ctx *exec.KernelCtx) (C.int, error) {
+	opts, ok := ctx.State.(kernels.DictionaryEncodeOptions)
+	if !ok {
+		return C.AG_NULL_ENCODING_MASK, nil // no options: Mask, the reference's default
+	}
+	switch opts.NullEncoding {
+	case kernels.NullEncodingMask:
+		return C.AG_NULL_ENCODING_MASK, nil
+	case kernels.NullEncodingEncode:
+		return C.AG_NULL_ENCODING_ENCODE, nil
+	}
+	return 0, fmt.Errorf("%w: invalid NullEncodingBehavior %d", arrow.ErrInvalid, opts.NullEncoding)
+}
+
+func dictEncodeSpans(ctx *exec.KernelCtx, ins []*exec.ArraySpan) ([]*exec.ExecResult, error) {
+	ne, err := dictEncodeNulls(ctx)
+	if err != nil {
+		return nil, err
+	}
+	valueType := ins[0].Type
+	bw := valueType.(arrow.FixedWidthDataType).BitWidth()
+	total := int64(0)
+	outs := make([]*exec.ExecResult, len(ins))
+	descs := make([]C.ag_dict_chunk, len(ins))
+	for i, in := range ins {
+		out := &exec.ExecResult{Type: &arrow.DictionaryType{IndexType: arrow.PrimitiveTypes.Int32, ValueType: valueType}}
+		preallocate(ctx, in.Len, 32, in.MayHaveNulls() && ne == C.AG_NULL_ENCODING_MASK, out)
+		descs[i] = C.ag_dict_chunk{values: base0(in.Buffers[1].Buf), validity: validityOf(in), offset: C.int64_t(in.Offset),
+			length: C.int64_t(in.Len), indices: (*C.int32_t)(base0(out.Buffers[1].Buf)), indices_validity: bitmap(out.Buffers[0].Buf)}
+		outs[i] = out
+		total += in.Len
+	}
+	// the call writes into scratch room for every row; the result keeps a copy of the dictionary's k values only
+	scratch := make([]byte, total*int64(bw/8)+8)
+	var scratchValid []byte
+	if ne == C.AG_NULL_ENCODING_ENCODE {
+		scratchValid = make([]byte, total/8+8)
+	}
+	counts := make([]C.int64_t, len(ins)+2)
+	var descPtr *C.ag_dict_chunk
+	if len(descs) > 0 {
+		descPtr = &descs[0]
+	}
+	if err := check(C.ag_dictionary_encode(C.int(bw), descPtr, C.int64_t(len(descs)), ne, base0(scratch),
+		bitmap(scratchValid), &counts[0])); err != nil {
+		return nil, err
+	}
+	k := int64(counts[0])
+	dict := &exec.ArraySpan{Type: valueType}
+	preallocate(ctx, k, bw, counts[1] != 0, dict)
+	copy(dict.Buffers[1].Buf, scratch[:k*int64(bw/8)])
+	if counts[1] != 0 {
+		copy(dict.Buffers[0].Buf, scratchValid[:(k+7)/8])
+	}
+	dict.Nulls = int64(counts[1])
+	for i, out := range outs {
+		out.Nulls = int64(counts[2+i])
+		if out.Nulls == 0 {
+			out.Buffers[0] = exec.BufferSpan{} // the indices' validity is present only when they hold nulls
+		}
+		out.SetDictionary(dict)
+	}
+	return outs, nil
+}
+
+func dictEncodeExec(ctx *exec.KernelCtx, batch *exec.ExecSpan, out *exec.ExecResult) error {
+	res, err := dictEncodeSpans(ctx, []*exec.ArraySpan{&batch.Values[0].Array})
+	if err != nil {
+		return err
+	}
+	*out = *res[0]
+	return nil
+}
+
+func dictEncodeChunked(ctx *exec.KernelCtx, cols []*arrow.Chunked, _ *exec.ExecResult) ([]*exec.ExecResult, error) {
+	chunks := cols[0].Chunks()
+	ins := make([]*exec.ArraySpan, len(chunks))
+	for i, c := range chunks {
+		ins[i] = &exec.ArraySpan{}
+		ins[i].SetMembers(c.Data())
+	}
+	if len(ins) == 0 {
+		return nil, nil
+	}
+	return dictEncodeSpans(ctx, ins)
+}
+
+func dictionaryEncodeFunction() *compute.VectorFunction {
+	fn := compute.NewVectorFunction("dictionary_encode", compute.Unary(), compute.EmptyFuncDoc)
+	for _, ty := range numericTypes {
+		outType := &arrow.DictionaryType{IndexType: arrow.PrimitiveTypes.Int32, ValueType: ty}
+		k := exec.NewVectorKernel([]exec.InputType{exec.NewExactInput(ty)}, exec.NewOutputType(outType), dictEncodeExec,
+			func(_ *exec.KernelCtx, args exec.KernelInitArgs) (exec.KernelState, error) {
+				if o, ok := args.Options.(*kernels.DictionaryEncodeOptions); ok {
+					return *o, nil
+				}
+				return nil, nil
+			})
+		k.CanExecuteChunkWise = false
+		k.ExecChunked = dictEncodeChunked
+		k.NullHandling = exec.NullComputedNoPrealloc
+		k.MemAlloc = exec.MemNoPrealloc
+		if err := fn.AddKernel(k); err != nil {
+			panic(err)
+		}
+	}
+	return fn
+}
+
 // ---- sort_indices (vector_sort.go:42-204, kernels.SortIndices vector_sort.go:385-481) -------------------------------
 //
 // A MetaFunction in the reference.  The GPU entry sorts ONE contiguous fixed-width column (stable, NaNs after the finite
@@ -221,10 +336,11 @@ func sortOneColumn(ctx context.Context, col arrow.ArrayData, key compute.SortKey
 	return &compute.ArrayDatum{Value: out}, nil
 }
 
-// registerLookupSort adds is_in, unique and sort_indices to a registry built by NewRegistry.
+// registerLookupSort adds is_in, unique, dictionary_encode and sort_indices to a registry built by NewRegistry.
 func registerLookupSort(reg, parent compute.FunctionRegistry) {
 	addScalar(reg, parent, isInFunction())
 	addVector(reg, parent, uniqueFunction())
+	addVector(reg, parent, dictionaryEncodeFunction()) // other types (and dictionary inputs) go to the parent's kernels
 	p, _ := parent.GetFunction("sort_indices")
 	reg.AddFunction(sortIndicesFunction(p), true)
 }

@@ -533,6 +533,42 @@ ag_status ag_unique_dev(int bit_width, const void* d_vals, const uint8_t* d_vali
 ag_status ag_unique_set_policy(int64_t small_rows, int64_t small_slots);
 
 /* ================================================================================= *
+ * dictionary_encode for fixed-width values of 1/2/4/8 bytes — the memo-table kernels of
+ *   compute/vector_hash.go:105-121 and kernels/vector_hash.go:144-241 (dictionaryEncodeAction):
+ *   output type Dictionary<int32, T> (outputDictionaryType), the dictionary = the distinct values in order of first
+ *   appearance over the WHOLE column, keys compared by raw bytes as in unique.  One call encodes every chunk of a
+ *   column into one shared dictionary; rows are numbered across the chunks in table order.
+ *   null_encoding (DictionaryEncodeOptions.NullEncoding):
+ *     AG_NULL_ENCODING_MASK (0)   a null row gets index 0 and a null index slot; the dictionary holds no null;
+ *     AG_NULL_ENCODING_ENCODE (1) the null is an ordinary dictionary entry where it first appears (value bytes 0,
+ *                                 validity bit clear); the indices have no nulls.   Anything else: AG_ERR_INVALID.
+ *   chunks: a HOST array of n_chunks descriptors.  `offset` is an element offset into values and validity; indices
+ *     (length int32) and indices_validity (4-byte aligned, ceil(length/32)*4 bytes) are written at offset 0.
+ *     indices_validity is written only in Mask mode for a chunk that has a validity bitmap (then it is required).
+ *   dict: capacity total rows of the value width; d_dict_valid: ceil(total/8) bytes, written only in Encode mode
+ *     (required there when any chunk has a validity bitmap): all ones but the null's bit.
+ *   counts (n_chunks + 2 int64): [0] dictionary length, [1] dictionary null count (0 or 1), [2 + c] the null count of
+ *     chunk c's indices.
+ *   More than 2^31-1 rows in all: AG_ERR_NOT_IMPLEMENTED.  ag_unique_set_policy applies to the table.
+ *   Host flavour: every pointer is a host pointer; dict / dict_valid receive only the dictionary's length.
+ * ================================================================================= */
+#define AG_TYPE_DICTIONARY         29 /* arrow.DICTIONARY (arrow/datatype.go) */
+#define AG_NULL_ENCODING_MASK       0
+#define AG_NULL_ENCODING_ENCODE     1
+typedef struct ag_dict_chunk {
+  const void* values;
+  const uint8_t* validity;   /* may be NULL */
+  int64_t offset;
+  int64_t length;
+  int32_t* indices;
+  uint8_t* indices_validity;
+} ag_dict_chunk;
+ag_status ag_dictionary_encode(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding,
+                               void* dict, uint8_t* dict_valid, int64_t* counts);
+ag_status ag_dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding,
+                                   void* d_dict, uint8_t* d_dict_valid, int64_t* d_counts, ag_stream_t s);
+
+/* ================================================================================= *
  * sort_indices, one fixed-width column (SURVEY 8f rank 3) — replaces kernels.SortIndices for a single
  *   key (vector_sort.go:385-481, vector_sort_internal.go:36-150,250-300): a STABLE permutation of
  *   0..n-1 as uint64 row indices,

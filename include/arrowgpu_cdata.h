@@ -117,6 +117,12 @@ const char* ag_type_to_schema_format(int type); /* NULL for unsupported ids */
  * struct — which is how the tests check the layout against another producer (pyarrow). */
 ag_status ag_device_array_describe(const struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_array_view* out);
 
+/* A Dictionary<int32, T> array (one level, arrow/cdata/cdata.go importer's dictionary case): schema format "i" with
+ * schema->dictionary set, array->dictionary set, the dictionary a primitive array on the same device.  Fills the view of
+ * the indices and of the dictionary values; ag_device_array_describe itself keeps refusing dictionary arrays. */
+ag_status ag_dictionary_device_array_describe(const struct ArrowDeviceArray* in, const struct ArrowSchema* schema,
+                                              ag_array_view* indices, ag_array_view* dictionary);
+
 /* Export device buffers as an ArrowDeviceArray{ARROW_DEVICE_CUDA, current device}.
  *   d_validity may be NULL.  An event is recorded on `produced_on` and published as sync_event so
  *   that the consumer orders itself after the kernels that produced the buffers.
@@ -135,6 +141,22 @@ ag_status ag_export_device_array(int type, int64_t length, int64_t null_count, i
  * last kernel that reads the buffers has completed.  ARROW_DEVICE_CPU is rejected with
  * AG_ERR_INVALID (upload it: ag_upload / ArrayData::FromHost). */
 ag_status ag_import_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on, ag_array_view* out);
+
+/* One level of dictionary (Dictionary<int32, T>, the layout of arrow/cdata's dictionary export: the parent is the int32
+ * indices with format "i", schema->dictionary / array->dictionary the value type's primitive array).
+ *   Export: the parent's release runs `release_buffers(opaque)` (which must cover the index AND the dictionary
+ *   buffers) and then releases the dictionary child; the schema's release frees the child schema.  Both share the
+ *   device and the sync_event of the parent.  ag_export_device_array keeps refusing AG_TYPE_DICTIONARY.
+ *   Import: ag_dictionary_device_array_describe plus the device checks and the wait of ag_import_device_array.
+ *   Ownership stays with `in`: releasing the parent releases the dictionary. */
+ag_status ag_export_dictionary_device_array(int value_type, int64_t length, int64_t null_count, int64_t offset,
+                                            const void* d_index_validity, const int32_t* d_indices,
+                                            int64_t dict_length, int64_t dict_null_count, int64_t dict_offset,
+                                            const void* d_dict_validity, const void* d_dict_values,
+                                            void (*release_buffers)(void* opaque), void* opaque, ag_stream_t produced_on,
+                                            struct ArrowDeviceArray* out, struct ArrowSchema* out_schema);
+ag_status ag_import_dictionary_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on,
+                                            ag_array_view* indices, ag_array_view* dictionary);
 
 #ifdef __cplusplus
 }

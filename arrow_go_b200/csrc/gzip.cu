@@ -11,7 +11,7 @@
 //      scratch at their output position (one kLzLit element per run), a length/distance pair becomes a kLzCopy element,
 //      a stored block one kLzSrc element over the compressed bytes.  Per member it records the output range and the
 //      stored CRC32 and ISIZE; per page the first decode event.
-//   2. gz_exec_kernel, one block per page: the executor shared with SNAPPY and ZSTD (lz_exec.cuh).
+//   2. lz_exec_kernel, one block per page: the executor shared with every codec (lz_exec.cu).
 //   3. gz_crc_kernel, one block per member: every thread CRCs a contiguous 64-byte slice with a table in shared memory;
 //      the slice CRCs combine in a tree (a warp by shuffles, then the warps), multiplying by x^(8·len) mod P with one
 //      constant per level.  A member whose CRC32 or ISIZE differs sets the page's lowest failing member by atomicMin.
@@ -23,6 +23,7 @@ namespace ag {
 
 namespace {
 
+constexpr const char* kFn = "gzip_decompress";  // message prefix
 constexpr int kWarps = 4;                 // pages per block of gz_inflate_kernel
 constexpr int kPrim = 10;                 // primary decode-table bits; longer codes decode canonically
 constexpr int kNameMax = 512;             // FNAME / FCOMMENT: at most kNameMax - 1 bytes before the NUL
@@ -40,7 +41,7 @@ struct GMember {                // one member with its trailer read; output offs
   uint32_t crc, isize;
 };
 
-struct GPage {                  // written by gz_inflate_kernel, read by gz_exec_kernel (LzExec::done) and the host
+struct GPage {                  // written by gz_inflate_kernel, read by lz_exec_kernel (LzExec::done) and the host
   int64_t written;              // output bytes before the first decode event, at most dst_len
   int64_t nelem;
   int64_t total;                // output bytes of the stream before the first decode event (may pass dst_len by one element)
@@ -454,11 +455,6 @@ gz_inflate_kernel(GArgs a) {
   }
 }
 
-__global__ void __launch_bounds__(kLzThreads)
-gz_exec_kernel(LzExec a) {
-  lz_exec_page(a, blockIdx.x);
-}
-
 // CRC32 of every recorded member's output.  The member is read as if left-padded with zeros to whole chunks: zeros
 // before the first byte leave a zero CRC register unchanged, so every slice is exactly kCrcSlice bytes and every tree
 // level multiplies by one constant.  crc32(M) = x^(8n)·0xFFFFFFFF + R(M) + 0xFFFFFFFF, R the register from zero.
@@ -512,50 +508,34 @@ gz_crc_kernel(GArgs a) {
 const char* const kEventText[] = {"",          "unexpected EOF", "",        "gzip: invalid header", "gzip: block type",
                                   "gzip: stored length", "gzip: code lengths", "gzip: huffman", "gzip: symbol", "gzip: distance"};
 
-// Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
-// `st` once to read the per-page outcomes back.  h_written (host, may be NULL) receives the bytes per page.
+// Decompresses a checked, non-empty batch of pages (pq_codec_dev_fn).
 ag_status gzip_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst, int64_t* d_written,
                    int64_t* h_written, cudaStream_t st) {
-  const char* fn = "gzip_decompress";
-  int64_t src_end, dst_end;
-  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
-  if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   // plan: pages | three prefix arrays [n+1].  Bounds from the table, per page (sl = src_len, dl = dst_len):
   //   literals   a literal is stored only at an output position below dl: dl bytes;
   //   elements   every element starts below dl at its own position, so at most dl.  Also: copies C <= dl / 3 + 1 (each
   //              produces >= 3 bytes, one may cross dl); a non-empty stored block S takes >= 5 bytes of its own (LEN,
   //              NLEN, a byte), S <= sl / 5; a literal run ends at a copy, a stored block or the end, so runs <= C + S + 1;
   //   members    a member takes >= 20 bytes (10 header, 2 for the shortest block, 8 trailer): sl / 20 + 1.
-  const int64_t n1 = n_pages + 1;
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed);
-  const size_t plan_bytes = pb + 3 * (size_t)n1 * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  memcpy(h.data(), pages, pb);
-  int64_t* base = reinterpret_cast<int64_t*>(h.data() + pb);
-  int64_t *lb = base, *eb = base + n1, *mb = base + 2 * n1;
-  lb[0] = eb[0] = mb[0] = 0;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const int64_t sl = pages[i].src_len, dl = pages[i].dst_len;
-    lb[i + 1] = lb[i] + dl;
-    eb[i + 1] = eb[i] + std::min(dl, 2 * (dl / 3 + 1) + 2 * (sl / 5) + 1);
-    mb[i + 1] = mb[i] + sl / 20 + 1;
-  }
+  const LzPlan<3> plan = lz_plan<3>(pages, n_pages, [](const ag_pq_compressed& g) {
+    const int64_t sl = g.src_len, dl = g.dst_len;
+    return std::array<int64_t, 3>{dl, std::min(dl, 2 * (dl / 3 + 1) + 2 * (sl / 5) + 1), sl / 20 + 1};
+  });
+  const int64_t n_lit = plan.total[0], n_elem = plan.total[1], n_mem = plan.total[2];
   Carve sc;
-  sc.take(plan_bytes);
-  const size_t o_st = sc.take((size_t)n_pages * sizeof(GPage)), o_mem = sc.take((size_t)mb[n_pages] * sizeof(GMember));
-  const size_t o_lit = sc.take((size_t)lb[n_pages]);
-  const size_t o_eo = sc.take((size_t)eb[n_pages] * 4), o_er = sc.take((size_t)eb[n_pages] * 4), o_ek = sc.take((size_t)eb[n_pages]);
+  sc.take(plan.bytes.size());
+  const size_t o_st = sc.take((size_t)n_pages * sizeof(GPage)), o_mem = sc.take((size_t)n_mem * sizeof(GMember));
+  const size_t o_lit = sc.take((size_t)n_lit);
+  const size_t o_eo = sc.take((size_t)n_elem * 4), o_er = sc.take((size_t)n_elem * 4), o_ek = sc.take((size_t)n_elem);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
   AG_TRY(t.alloc_t(&d, sc.size));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
-  const int64_t* dbase = reinterpret_cast<const int64_t*>(d + pb);
+  LzPlanDev<3> pl;
+  AG_TRY(lz_upload(plan, d, st, &pl));
   GArgs a;
-  a.pages = reinterpret_cast<const ag_pq_compressed*>(d);
-  a.lit_base = dbase; a.elem_base = dbase + n1; a.mem_base = dbase + 2 * n1;
+  a.pages = pl.pages;
+  a.lit_base = pl.base[0]; a.elem_base = pl.base[1]; a.mem_base = pl.base[2];
   a.n_pages = n_pages;
   a.src = src; a.dst = dst;
   a.st = reinterpret_cast<GPage*>(d + o_st);
@@ -572,30 +552,21 @@ ag_status gzip_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_
   x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = a.lit; x.lit_base = a.lit_base; x.dst = dst;
   x.done = reinterpret_cast<const int64_t*>(a.st); x.stride = sizeof(GPage) / 8;
   x.e_out = a.e_out; x.e_ref = a.e_ref; x.e_lit = a.e_lit;
-  gz_exec_kernel<<<(unsigned)n_pages, kLzThreads, 0, st>>>(x);
-  AG_TRY(check_launch("gz_exec_kernel"));
+  AG_TRY(lz_exec_launch(x, n_pages, st));
   gz_crc_kernel<<<dim3((unsigned)n_pages, kCrcSplit), kCrcThreads, 0, st>>>(a);
   AG_TRY(check_launch("gz_crc_kernel"));
-  std::vector<GPage> hs((size_t)n_pages);
-  AG_TRY(d2h(hs.data(), a.st, (size_t)n_pages * sizeof(GPage), st));
-  AG_TRY(sync(st));
-  if (h_written)
-    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
   // The first event in stream order: a member's checksum is checked at its trailer, before anything the walk met after
   // it, so a mismatch wins; then the walk's event; then a clean stream that is short of dst_len.
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const GPage& s = hs[i];
+  return lz_read_back(kFn, a.st, n_pages, h_written, st, [&](int64_t i, const GPage& s, char* buf, size_t n) {
     const int64_t dl = pages[i].dst_len;
     char what[96];
     if (s.ck_bad != INT32_MAX) snprintf(what, sizeof what, "gzip: invalid checksum");
     else if (s.event == kGExceed) snprintf(what, sizeof what, "codec: gzip: decoded data exceeds destination size %lld", (long long)dl);
     else if (s.event != kGOk) snprintf(what, sizeof what, "%s", kEventText[s.event]);
     else if (s.total < dl) snprintf(what, sizeof what, "%s", s.total == 0 ? "EOF" : "unexpected EOF");
-    else continue;
-    AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: could not decompress page: %s (%lld bytes written)", fn, (long long)i, what,
-            (long long)s.written);
-  }
-  return AG_OK;
+    else return;
+    snprintf(buf, n, "parquet: could not decompress page: %s", what);
+  });
 }
 
 }  // namespace
@@ -609,13 +580,13 @@ extern "C" {
 ag_status ag_parquet_gzip_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
                                          int64_t* d_written, ag_stream_t s) {
   AG_TRY(ensure_init());
-  return gzip_dev(d_src, pages, n_pages, d_dst, d_written, nullptr, resolve_stream(s));
+  return pq_decompress_dev(kFn, gzip_dev, d_src, pages, n_pages, d_dst, d_written, resolve_stream(s));
 }
 
 ag_status ag_parquet_gzip_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                      int64_t* written) {
   AG_TRY(ensure_init());
-  return pq_decompress_host("gzip_decompress", gzip_dev, src, pages, n_pages, dst, written);
+  return pq_decompress_host(kFn, gzip_dev, src, pages, n_pages, dst, written);
 }
 
 }  // extern "C"

@@ -14,7 +14,7 @@
 //      is validated here, so a failing page knows how many bytes its valid elements produce before anything executes.
 //      A sequence that leaves the window (an extension run longer than kExt, or literals that carry its offset past the
 //      window) ends the span: its thread finishes it from global memory and the next span starts after it.
-//   2. lz4_exec_kernel: the shared executor of lz_exec.cuh, unchanged (the 16-bit offsets fit e_ref).
+//   2. lz_exec_kernel: the shared executor of lz_exec.cu, unchanged (the 16-bit offsets fit e_ref).
 // Roofline.  compressed bytes read + decompressed bytes written.  This design also writes and reads 9 B per element
 // descriptor and reads each copied byte once more (from L2).
 #include <string.h>
@@ -34,10 +34,12 @@ constexpr int kLook = 2 * kExt + 3;         // bytes past a span a short sequenc
 constexpr unsigned long long kCntOne = 1ull << 48;   // parse scan: descriptor count in bits 48.., output bytes below
 constexpr unsigned long long kLenMask = kCntOne - 1;
 
+constexpr const char* kFn = "lz4_raw_decompress";    // message prefix
+
 enum Lz4Err : int { kL4Ok = 0, kL4Corrupt = 1, kL4Size = 2 };
 enum SeqState : int { kSqOk = 0, kSqBadLit = 1, kSqBadMatch = 2, kSqOut = 3 };
 
-struct Lz4Page {            // written by lz4_parse_kernel, read by lz4_exec_kernel and the host
+struct Lz4Page {            // written by lz4_parse_kernel, read by lz_exec_kernel and the host
   int64_t written;          // output bytes of the page's valid elements (LzExec::done)
   int64_t nelem;            // element descriptors written
   int64_t got;              // a clean stream's output bytes (kL4Size names them)
@@ -266,48 +268,30 @@ lz4_parse_kernel(Lz4Args a) {
   }
 }
 
-// one block per page: the page's output from its element descriptors (lz_exec.cuh)
-__global__ void __launch_bounds__(kLzThreads)
-lz4_exec_kernel(LzExec a) {
-  lz_exec_page(a, blockIdx.x);
-}
-
 }  // namespace
 
-// Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
-// `st` once to read the per-page error codes back.  h_written (host, may be NULL) receives the bytes per page.
+// Decompresses a checked, non-empty batch of pages (pq_codec_dev_fn).
 static ag_status lz4_raw_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst, int64_t* d_written,
                              int64_t* h_written, cudaStream_t st) {
-  const char* fn = "lz4_raw_decompress";
-  int64_t src_end, dst_end;
-  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
-  if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   // plan: pages | elem_base[n+1].  Every sequence but the last takes >= 3 compressed bytes and makes <= 2 elements;
   // every valid element produces >= 1 output byte.
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed);
-  const size_t plan_bytes = pb + (size_t)(n_pages + 1) * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  memcpy(h.data(), pages, pb);
-  int64_t* elem_base = reinterpret_cast<int64_t*>(h.data() + pb);
-  elem_base[0] = 0;
-  for (int64_t i = 0; i < n_pages; ++i)
-    elem_base[i + 1] = elem_base[i] + std::min(pages[i].dst_len, 2 * (pages[i].src_len / 3) + 2);
-  const int64_t n_elem = elem_base[n_pages];
-  const size_t st_bytes = (size_t)n_pages * sizeof(Lz4Page);
+  const LzPlan<1> plan = lz_plan<1>(pages, n_pages, [](const ag_pq_compressed& g) {
+    return std::array<int64_t, 1>{std::min(g.dst_len, 2 * (g.src_len / 3) + 2)};
+  });
+  const int64_t n_elem = plan.total[0];
   Carve sc;
-  sc.take(plan_bytes);
-  const size_t off_st = sc.take(st_bytes), off_out = sc.take((size_t)n_elem * 4), off_ref = sc.take((size_t)n_elem * 4);
+  sc.take(plan.bytes.size());
+  const size_t off_st = sc.take((size_t)n_pages * sizeof(Lz4Page)), off_out = sc.take((size_t)n_elem * 4), off_ref = sc.take((size_t)n_elem * 4);
   const size_t off_lit = sc.take((size_t)n_elem);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
   AG_TRY(t.alloc_t(&d, sc.size));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  LzPlanDev<1> pl;
+  AG_TRY(lz_upload(plan, d, st, &pl));
   Lz4Args a;
-  a.pages = reinterpret_cast<const ag_pq_compressed*>(d);
-  a.elem_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.pages = pl.pages;
+  a.elem_base = pl.base[0];
   a.src = src;
   a.dst = dst;
   a.st = reinterpret_cast<Lz4Page*>(d + off_st);
@@ -321,23 +305,11 @@ static ag_status lz4_raw_dev(const uint8_t* src, const ag_pq_compressed* pages, 
   x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = nullptr; x.lit_base = nullptr; x.dst = dst;
   x.done = reinterpret_cast<const int64_t*>(a.st); x.stride = sizeof(Lz4Page) / 8;
   x.e_out = a.e_out; x.e_ref = a.e_ref; x.e_lit = a.e_lit;
-  lz4_exec_kernel<<<(unsigned)n_pages, kLzThreads, 0, st>>>(x);
-  AG_TRY(check_launch("lz4_exec_kernel"));
-  std::vector<Lz4Page> hs((size_t)n_pages);
-  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
-  AG_TRY(sync(st));
-  if (h_written)
-    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    if (hs[i].err == kL4Size)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: metadata said %lld bytes uncompressed data page, got %lld bytes (0 bytes written)", fn,
-              (long long)i, (long long)pages[i].dst_len, (long long)hs[i].got);
-    if (hs[i].err == kL4Corrupt)
-      AG_FAIL(AG_ERR_INVALID,
-              "%s: page %lld: parquet: could not decompress page: lz4: invalid source or destination buffer too short (%lld bytes written)", fn,
-              (long long)i, (long long)hs[i].written);
-  }
-  return AG_OK;
+  AG_TRY(lz_exec_launch(x, n_pages, st));
+  return lz_read_back(kFn, a.st, n_pages, h_written, st, [&](int64_t i, const Lz4Page& s, char* buf, size_t n) {
+    if (s.err == kL4Size) size_text(buf, n, pages[i].dst_len, s.got);
+    else if (s.err == kL4Corrupt) snprintf(buf, n, "parquet: could not decompress page: lz4: invalid source or destination buffer too short");
+  });
 }
 
 }  // namespace ag
@@ -349,14 +321,13 @@ extern "C" {
 ag_status ag_parquet_lz4_raw_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
                                             int64_t* d_written, ag_stream_t s) {
   AG_TRY(ensure_init());
-  return lz4_raw_dev(d_src, pages, n_pages, d_dst, d_written, nullptr, resolve_stream(s));
+  return pq_decompress_dev(kFn, lz4_raw_dev, d_src, pages, n_pages, d_dst, d_written, resolve_stream(s));
 }
 
-// host flavour: stage the compressed bytes, decompress, copy back only the bytes each page wrote
 ag_status ag_parquet_lz4_raw_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                         int64_t* written) {
   AG_TRY(ensure_init());
-  return pq_decompress_host("lz4_raw_decompress", lz4_raw_dev, src, pages, n_pages, dst, written);
+  return pq_decompress_host(kFn, lz4_raw_dev, src, pages, n_pages, dst, written);
 }
 
 }  // extern "C"

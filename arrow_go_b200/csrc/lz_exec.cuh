@@ -2,24 +2,30 @@
 // the ABI.
 //
 //   pq_compressed_check   the argument checks of an ag_pq_compressed batch, AG_ERR_INVALID before any launch
-//   pq_decompress_host    the host-pointer flavour: stage src, run the device flavour, copy back only written bytes
-//   lz_exec_page          the executor: a page's output from element descriptors {first output byte, literal source /
-//                         copy offset, kind}, in 2048-byte batches with pointer jumping over in-batch sources
+//   pq_decompress_dev     the device flavour: the checks, then the codec
+//   pq_decompress_host    the host flavour: the checks, stage src, run the codec, copy back only written bytes
+//   lz_plan / lz_upload   the page table and the codec's per-page bounds as prefix arrays, in one upload
+//   lz_exec_launch        the executor (lz_exec.cu): a page's output from element descriptors {first output byte,
+//                         literal source / copy offset, kind}
+//   lz_read_back          the end of a call: per-page states back, one synchronisation, the lowest failing page
 #pragma once
 
+#include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <vector>
 
 #include "host_stage.cuh"
 
 namespace ag {
 
-// Argument checks shared by every codec and both flavours; every one is AG_ERR_INVALID before any launch.
+// Argument checks shared by every codec and both flavours; every one is AG_ERR_INVALID before any launch.  `src` and
+// `dst` are the compressed data and the output, in host or device memory; only whether they are NULL matters.
 // *src_end / *dst_end: the bytes of `src` / `dst` the batch spans.
-static inline ag_status pq_compressed_check(const char* fn, const ag_pq_compressed* pages, int64_t n_pages, int64_t* src_end,
-                                            int64_t* dst_end) {
+static inline ag_status pq_compressed_check(const char* fn, const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages,
+                                            const uint8_t* dst, int64_t* src_end, int64_t* dst_end) {
   *src_end = *dst_end = 0;
   if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
   if (n_pages == 0) return AG_OK;
@@ -41,22 +47,31 @@ static inline ag_status pq_compressed_check(const char* fn, const ag_pq_compress
       AG_FAIL(AG_ERR_INVALID, "%s: pages %lld and %lld: overlapping dst ranges", fn, (long long)x, (long long)y);
     }
   }
+  if (*src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
+  if (*dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   return AG_OK;
 }
 
-// The device flavour of a codec: decompresses into device `dst`, fills h_written (host, may be NULL) with the bytes per
-// page, synchronises `st` once.
+// A codec: decompresses a checked, non-empty batch into device `dst`.  `pages` is host memory; everything else is
+// device memory on `st`.  Fills h_written (host, may be NULL) with the bytes per page and synchronises `st` once.
 typedef ag_status (*pq_codec_dev_fn)(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                      int64_t* d_written, int64_t* h_written, cudaStream_t st);
 
-// host flavour: stage the compressed bytes, decompress, copy back only the bytes each page wrote
+// device flavour: check, decompress
+static inline ag_status pq_decompress_dev(const char* fn, pq_codec_dev_fn dev, const uint8_t* src, const ag_pq_compressed* pages,
+                                          int64_t n_pages, uint8_t* dst, int64_t* d_written, cudaStream_t st) {
+  int64_t src_end, dst_end;
+  AG_TRY(pq_compressed_check(fn, src, pages, n_pages, dst, &src_end, &dst_end));
+  if (n_pages == 0) return AG_OK;
+  return dev(src, pages, n_pages, dst, d_written, nullptr, st);
+}
+
+// host flavour: check, stage the compressed bytes, decompress, copy back only the bytes each page wrote
 static inline ag_status pq_decompress_host(const char* fn, pq_codec_dev_fn dev, const uint8_t* src, const ag_pq_compressed* pages,
                                            int64_t n_pages, uint8_t* dst, int64_t* written) {
   int64_t src_end, dst_end;
-  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
+  AG_TRY(pq_compressed_check(fn, src, pages, n_pages, dst, &src_end, &dst_end));
   if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
   Carve sc;
@@ -73,6 +88,71 @@ static inline ag_status pq_decompress_host(const char* fn, pq_codec_dev_fn dev, 
   for (int64_t i = 0; i < n_pages; ++i) AG_TRY(d2h(dst + pages[i].dst, d + o_dst + pages[i].dst, (size_t)w[i], cs));
   const ag_status rs = sync(cs);
   return rc != AG_OK ? rc : rs;
+}
+
+// The plan a codec's kernels read: pages | K prefix arrays [n_pages + 1], one per per-page bound (element
+// descriptors, literal bytes, ...).  total[k] is bound k over the batch, what the codec carves its scratch by.
+template <size_t K>
+struct LzPlan {
+  std::vector<uint8_t> bytes;
+  int64_t n_pages = 0;
+  std::array<int64_t, K> total{};
+};
+
+// Its device views after lz_upload: base[k] is prefix array k.
+template <size_t K>
+struct LzPlanDev {
+  const ag_pq_compressed* pages;
+  std::array<const int64_t*, K> base;
+};
+
+// Plans a checked batch; bounds(page) gives the K bounds of one page as a std::array<int64_t, K>.
+template <size_t K, typename Bounds>
+static inline LzPlan<K> lz_plan(const ag_pq_compressed* pages, int64_t n_pages, Bounds bounds) {
+  LzPlan<K> p;
+  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed), n1 = (size_t)n_pages + 1;
+  p.n_pages = n_pages;
+  p.bytes.assign(pb + K * n1 * 8, 0);
+  memcpy(p.bytes.data(), pages, pb);
+  int64_t* base = reinterpret_cast<int64_t*>(p.bytes.data() + pb);
+  for (int64_t i = 0; i < n_pages; ++i) {
+    const std::array<int64_t, K> b = bounds(pages[i]);
+    for (size_t k = 0; k < K; ++k) base[k * n1 + i + 1] = base[k * n1 + i] + b[k];
+  }
+  for (size_t k = 0; k < K; ++k) p.total[k] = base[k * n1 + n_pages];
+  return p;
+}
+
+// Uploads the plan to device memory `d` (p.bytes.size() bytes) and returns its device views.
+template <size_t K>
+static inline ag_status lz_upload(const LzPlan<K>& p, uint8_t* d, cudaStream_t st, LzPlanDev<K>* out) {
+  AG_TRY(h2d(d, p.bytes.data(), p.bytes.size(), st));
+  out->pages = reinterpret_cast<const ag_pq_compressed*>(d);
+  const int64_t* base = reinterpret_cast<const int64_t*>(d + (size_t)p.n_pages * sizeof(ag_pq_compressed));
+  for (size_t k = 0; k < K; ++k) out->base[k] = base + k * (size_t)(p.n_pages + 1);
+  return AG_OK;
+}
+
+// The end of a call: copies the per-page states back, synchronises `st` once, fills h_written (host, may be NULL) from
+// state.written, and fails on the lowest page that text(page, state, buf, size) writes a non-empty text for.
+template <typename S, typename Text>
+ag_status lz_read_back(const char* fn, const S* d_st, int64_t n_pages, int64_t* h_written, cudaStream_t st, Text text) {
+  std::vector<S> hs((size_t)n_pages);
+  AG_TRY(d2h(hs.data(), d_st, (size_t)n_pages * sizeof(S), st));
+  AG_TRY(sync(st));
+  if (h_written)
+    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
+  for (int64_t i = 0; i < n_pages; ++i) {
+    char msg[200] = "";
+    text(i, hs[i], msg, sizeof msg);
+    if (msg[0]) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: %s (%lld bytes written)", fn, (long long)i, msg, (long long)hs[i].written);
+  }
+  return AG_OK;
+}
+
+// The text of a stream whose own output size is not the page's dst_len.
+static inline void size_text(char* buf, size_t n, int64_t dst_len, int64_t got) {
+  snprintf(buf, n, "parquet: metadata said %lld bytes uncompressed data page, got %lld bytes", (long long)dst_len, (long long)got);
 }
 
 constexpr int kLzThreads = 256;
@@ -98,75 +178,7 @@ struct LzExec {
   const uint8_t* e_lit;       // LzKind
 };
 
-// One block (kLzThreads) writes page p's output in batches of kLzBatch bytes, in order.  Each element produces at
-// least one byte.  Byte j of a copy at `pos` with offset r is dst[pos - r + (j mod r)], so every output byte names
-// one source byte: a literal byte, an output byte before the batch (read back from dst, written by this block), or
-// an earlier byte of the same batch, which pointer jumping in shared memory resolves.
-__device__ __forceinline__ void lz_exec_page(const LzExec& a, int64_t p) {
-  __shared__ uint32_t s_out[kLzBatch + 1], s_ref[kLzBatch + 1];
-  __shared__ uint8_t s_lit[kLzBatch + 1];
-  __shared__ unsigned long long s_src[kLzBatch];
-  const int64_t written = a.done[p * a.stride], nelem = a.done[p * a.stride + 1];
-  if (written <= 0 || nelem <= 0) return;                        // block-uniform
-  const ag_pq_compressed pg = a.pages[p];
-  const uint8_t* in = a.src + pg.src;
-  const uint8_t* lit = a.lit ? a.lit + a.lit_base[p] : nullptr;
-  uint8_t* out = a.dst + pg.dst;
-  const int64_t eb = a.elem_base[p];
-  const int tid = threadIdx.x;
-  int64_t e0 = 0;                                                // the element holding the batch's first byte
-  for (int64_t B = 0; B < written; B += kLzBatch) {
-    const int nb = (int)(written - B < kLzBatch ? written - B : kLzBatch);
-    // elements e0 .. e0 + nl - 1 hold every byte of [B, B + kLzBatch] (each element produces at least one byte)
-    const int nl = (int)(nelem - e0 < kLzBatch + 1 ? nelem - e0 : kLzBatch + 1);
-    for (int k = tid; k < nl; k += kLzThreads) {
-      s_out[k] = a.e_out[eb + e0 + k];
-      s_ref[k] = a.e_ref[eb + e0 + k];
-      s_lit[k] = a.e_lit[eb + e0 + k];
-    }
-    __syncthreads();
-    auto holder = [&](uint32_t pos) {                            // last loaded element starting at or before pos
-      int lo = 0, hi = nl - 1;
-      while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (s_out[mid] <= pos) lo = mid; else hi = mid - 1;
-      }
-      return lo;
-    };
-    for (int b = tid; b < nb; b += kLzThreads) {
-      const uint32_t pos = (uint32_t)(B + b);
-      const int e = holder(pos);
-      const uint32_t j = pos - s_out[e], r = s_ref[e];
-      unsigned long long s;
-      if (s_lit[e]) {
-        s = (s_lit[e] == kLzSrc ? kFromSrc : kFromLit) | (unsigned long long)(r + j);
-      } else {
-        const uint32_t q = s_out[e] - r + (j < r ? j : j % r);
-        s = (int64_t)q < B ? kFromDst | q : (unsigned long long)((int64_t)q - B);
-      }
-      s_src[b] = s;
-    }
-    __syncthreads();
-    while (true) {                                               // pointer jumping to a byte outside the batch
-      bool pend = false;
-      for (int b = tid; b < nb; b += kLzThreads) {
-        const unsigned long long v = s_src[b];
-        if (v < kFromLit) {
-          const unsigned long long w = s_src[v];
-          s_src[b] = w;
-          pend |= w < kFromLit;
-        }
-      }
-      if (!__syncthreads_or(pend)) break;
-    }
-    for (int b = tid; b < nb; b += kLzThreads) {
-      const unsigned long long v = s_src[b];
-      // dst bytes before the batch were written by this block before the last barrier: a plain (coherent) load
-      out[B + b] = (v & kFromSrc) ? __ldg(in + (v & kLzPosMask)) : (v & kFromLit) ? lit[v & kLzPosMask] : out[v & kLzPosMask];
-    }
-    e0 += holder((uint32_t)(B + kLzBatch < written ? B + kLzBatch : written - 1));
-    __syncthreads();
-  }
-}
+// Launches lz_exec_kernel, one block per page, on `st`.
+ag_status lz_exec_launch(const LzExec& x, int64_t n_pages, cudaStream_t st);
 
 }  // namespace ag

@@ -13,7 +13,7 @@
 //      written as a 9-byte descriptor {output position, literal source / copy offset, literal flag}, so a failing page
 //      knows how many bytes its valid elements produce before anything is executed.  A literal longer than the window
 //      moves the next span (and window) past it without loading it.
-//   2. snappy_exec_kernel (lz_exec.cuh, shared with ZSTD): walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
+//   2. lz_exec_kernel (lz_exec.cu, shared with every codec): walks the page's output in 2048-byte batches.  Byte j of a copy at `pos` is
 //      dst[pos - off + (j mod off)], so every output byte names one source byte: a compressed byte (literals), an
 //      output byte before the batch (read back from dst, which the same block wrote, L2-resident), or an earlier byte
 //      of the same batch.  Pointer jumping in shared memory resolves the last kind, so overlapping copies and copies of
@@ -37,9 +37,11 @@ constexpr unsigned long long kCntOne = 1ull << 48;   // parse scan: element coun
 constexpr unsigned long long kLenMask = kCntOne - 1;
 constexpr unsigned long long kLenClamp = 1ull << 33; // any longer element is corrupt (dst_len <= 2^32-1)
 
+constexpr const char* kFn = "snappy_decompress";     // message prefix
+
 enum SnapErr : int { kSnOk = 0, kSnCorrupt = 1, kSnSize = 2 };
 
-struct SnapPage {           // written by snappy_parse_kernel, read by snappy_exec_kernel and the host
+struct SnapPage {           // written by snappy_parse_kernel, read by lz_exec_kernel and the host
   int64_t written;          // output bytes of the page's valid elements (LzExec::done)
   int64_t nelem;            // element descriptors written
   int64_t preamble;         // the stream's uncompressed length (kSnSize names it)
@@ -212,46 +214,29 @@ snappy_parse_kernel(SnapArgs a) {
   }
 }
 
-// one block per page: the page's output from its element descriptors (lz_exec.cuh)
-__global__ void __launch_bounds__(kLzThreads)
-snappy_exec_kernel(LzExec a) {
-  lz_exec_page(a, blockIdx.x);
-}
-
 }  // namespace
 
-// Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
-// `st` once to read the per-page error codes back.  h_written (host, may be NULL) receives the bytes per page.
+// Decompresses a checked, non-empty batch of pages (pq_codec_dev_fn).
 static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst, int64_t* d_written,
                             int64_t* h_written, cudaStream_t st) {
-  const char* fn = "snappy_decompress";
-  int64_t src_end, dst_end;
-  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
-  if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   // plan: pages | elem_base[n+1].  A valid element takes >= 2 compressed bytes and produces >= 1 output byte.
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed);
-  const size_t plan_bytes = pb + (size_t)(n_pages + 1) * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  memcpy(h.data(), pages, pb);
-  int64_t* elem_base = reinterpret_cast<int64_t*>(h.data() + pb);
-  elem_base[0] = 0;
-  for (int64_t i = 0; i < n_pages; ++i) elem_base[i + 1] = elem_base[i] + std::min(pages[i].src_len / 2, pages[i].dst_len);
-  const int64_t n_elem = elem_base[n_pages];
-  const size_t st_bytes = (size_t)n_pages * sizeof(SnapPage);
+  const LzPlan<1> plan = lz_plan<1>(pages, n_pages, [](const ag_pq_compressed& g) {
+    return std::array<int64_t, 1>{std::min(g.src_len / 2, g.dst_len)};
+  });
+  const int64_t n_elem = plan.total[0];
   Carve sc;
-  sc.take(plan_bytes);
-  const size_t off_st = sc.take(st_bytes), off_out = sc.take((size_t)n_elem * 4), off_ref = sc.take((size_t)n_elem * 4);
+  sc.take(plan.bytes.size());
+  const size_t off_st = sc.take((size_t)n_pages * sizeof(SnapPage)), off_out = sc.take((size_t)n_elem * 4), off_ref = sc.take((size_t)n_elem * 4);
   const size_t off_lit = sc.take((size_t)n_elem);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
   AG_TRY(t.alloc_t(&d, sc.size));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
+  LzPlanDev<1> pl;
+  AG_TRY(lz_upload(plan, d, st, &pl));
   SnapArgs a;
-  a.pages = reinterpret_cast<const ag_pq_compressed*>(d);
-  a.elem_base = reinterpret_cast<const int64_t*>(d + pb);
+  a.pages = pl.pages;
+  a.elem_base = pl.base[0];
   a.src = src;
   a.dst = dst;
   a.st = reinterpret_cast<SnapPage*>(d + off_st);
@@ -265,22 +250,11 @@ static ag_status snappy_dev(const uint8_t* src, const ag_pq_compressed* pages, i
   x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = nullptr; x.lit_base = nullptr; x.dst = dst;
   x.done = reinterpret_cast<const int64_t*>(a.st); x.stride = sizeof(SnapPage) / 8;
   x.e_out = a.e_out; x.e_ref = a.e_ref; x.e_lit = a.e_lit;
-  snappy_exec_kernel<<<(unsigned)n_pages, kLzThreads, 0, st>>>(x);
-  AG_TRY(check_launch("snappy_exec_kernel"));
-  std::vector<SnapPage> hs((size_t)n_pages);
-  AG_TRY(d2h(hs.data(), a.st, st_bytes, st));
-  AG_TRY(sync(st));
-  if (h_written)
-    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    if (hs[i].err == kSnSize)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: metadata said %lld bytes uncompressed data page, got %lld bytes (0 bytes written)", fn,
-              (long long)i, (long long)pages[i].dst_len, (long long)hs[i].preamble);
-    if (hs[i].err == kSnCorrupt)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: could not decompress page: snappy: corrupt input (%lld bytes written)", fn,
-              (long long)i, (long long)hs[i].written);
-  }
-  return AG_OK;
+  AG_TRY(lz_exec_launch(x, n_pages, st));
+  return lz_read_back(kFn, a.st, n_pages, h_written, st, [&](int64_t i, const SnapPage& s, char* buf, size_t n) {
+    if (s.err == kSnSize) size_text(buf, n, pages[i].dst_len, s.preamble);
+    else if (s.err == kSnCorrupt) snprintf(buf, n, "parquet: could not decompress page: snappy: corrupt input");
+  });
 }
 
 }  // namespace ag
@@ -292,14 +266,13 @@ extern "C" {
 ag_status ag_parquet_snappy_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
                                            int64_t* d_written, ag_stream_t s) {
   AG_TRY(ensure_init());
-  return snappy_dev(d_src, pages, n_pages, d_dst, d_written, nullptr, resolve_stream(s));
+  return pq_decompress_dev(kFn, snappy_dev, d_src, pages, n_pages, d_dst, d_written, resolve_stream(s));
 }
 
-// host flavour: stage the compressed bytes, decompress, copy back only the bytes each page wrote
 ag_status ag_parquet_snappy_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                        int64_t* written) {
   AG_TRY(ensure_init());
-  return pq_decompress_host("snappy_decompress", snappy_dev, src, pages, n_pages, dst, written);
+  return pq_decompress_host(kFn, snappy_dev, src, pages, n_pages, dst, written);
 }
 
 }  // extern "C"

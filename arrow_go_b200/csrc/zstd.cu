@@ -15,7 +15,7 @@
 //      the descriptions in effect), then one lane decodes the (literal length, match length, offset value) triples.
 //   4. zstd_resolve_kernel, one thread per page: repeat offsets in order within each frame, the offset / literal /
 //      block / content-size checks, the first failing zstd block, and the execute elements.
-//   5. zstd_exec_kernel, one block per page: the executor shared with SNAPPY (lz_exec.cuh).
+//   5. lz_exec_kernel, one block per page: the executor shared with every codec (lz_exec.cu).
 //   6. zstd_xxh64_kernel, one warp per checksummed frame: XXH64 of the frame's output (4 lanes, one per accumulator).
 // Roofline.  compressed bytes read + decompressed bytes written.  This design also writes and reads 12 B per sequence,
 // 9 B per element (2 per sequence), the Huffman literals once more, and reads each copied byte once more (from L2).
@@ -25,6 +25,7 @@ namespace ag {
 
 namespace {
 
+constexpr const char* kFn = "zstd_decompress";  // message prefix
 constexpr uint32_t kMagic = 0xFD2FB528u;
 constexpr uint32_t kBlockMax = 1u << 17;
 constexpr int kWarps = 4;              // warps per thread block of the literals / sequences kernels
@@ -66,7 +67,7 @@ struct ZFrame {
   int64_t out0, out1;         // set by resolve: the frame's output range in the page
 };
 
-struct ZPage {                // written by the kernels, read by zstd_exec_kernel (LzExec::done) and the host
+struct ZPage {                // written by the kernels, read by lz_exec_kernel (LzExec::done) and the host
   int64_t written;
   int64_t nelem;
   int64_t got;                // kZErrSize: the size the frames give
@@ -808,11 +809,6 @@ zstd_resolve_kernel(ZArgs a) {
   if (a.d_written) a.d_written[p] = ps.written;
 }
 
-__global__ void __launch_bounds__(kLzThreads)
-zstd_exec_kernel(LzExec a) {
-  lz_exec_page(a, blockIdx.x);
-}
-
 // ------------------------------------------------------------------------------------------------------------- xxh64
 constexpr unsigned long long kP1 = 11400714785074694791ull, kP2 = 14029467366897019727ull, kP3 = 1609587929392839161ull,
                              kP4 = 9650029242287828579ull, kP5 = 2870177450012600261ull;
@@ -877,50 +873,32 @@ zstd_xxh64_kernel(ZArgs a) {
 const char* const kCheckName[] = {"", "truncated", "bad magic", "frame header", "dictionary", "block type", "block size", "literals",
                                   "huffman", "fse", "sequences", "offset", "content size", "page size"};
 
-// Decompresses a batch of pages.  `pages` is host memory; everything else is device memory on `st`.  Synchronises
-// `st` once to read the per-page outcomes back.  h_written (host, may be NULL) receives the bytes per page.
+// Decompresses a checked, non-empty batch of pages (pq_codec_dev_fn).
 ag_status zstd_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst, int64_t* d_written,
                    int64_t* h_written, cudaStream_t st) {
-  const char* fn = "zstd_decompress";
-  int64_t src_end, dst_end;
-  AG_TRY(pq_compressed_check(fn, pages, n_pages, &src_end, &dst_end));
-  if (n_pages == 0) return AG_OK;
-  if (src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
-  if (dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   // plan: pages | five prefix arrays [n+1].  Bounds from the table: a zstd block takes >= 3 compressed bytes, a frame
   // >= 8; a sequence produces >= 3 output bytes; literals are output bytes; an element produces >= 1 output byte and
   // there are at most 2 per sequence and 2 per zstd block.
-  const int64_t n1 = n_pages + 1;
-  const size_t pb = (size_t)n_pages * sizeof(ag_pq_compressed);
-  const size_t plan_bytes = pb + 5 * (size_t)n1 * 8;
-  std::vector<uint8_t> h(plan_bytes);
-  memcpy(h.data(), pages, pb);
-  int64_t* base = reinterpret_cast<int64_t*>(h.data() + pb);
-  int64_t *bb = base, *fb = base + n1, *lb = base + 2 * n1, *sq = base + 3 * n1, *eb = base + 4 * n1;
-  bb[0] = fb[0] = lb[0] = sq[0] = eb[0] = 0;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const int64_t sl = pages[i].src_len, dl = pages[i].dst_len;
-    bb[i + 1] = bb[i] + sl / 3;
-    fb[i + 1] = fb[i] + sl / 8;
-    lb[i + 1] = lb[i] + dl;
-    sq[i + 1] = sq[i] + dl / 3;
-    eb[i + 1] = eb[i] + std::min(dl, 2 * (dl / 3) + 2 * (sl / 3));
-  }
+  const LzPlan<5> plan = lz_plan<5>(pages, n_pages, [](const ag_pq_compressed& g) {
+    const int64_t sl = g.src_len, dl = g.dst_len;
+    return std::array<int64_t, 5>{sl / 3, sl / 8, dl, dl / 3, std::min(dl, 2 * (dl / 3) + 2 * (sl / 3))};
+  });
+  const int64_t n_blk = plan.total[0], n_frame = plan.total[1], n_lit = plan.total[2], n_seq = plan.total[3], n_elem = plan.total[4];
   Carve sc;
-  sc.take(plan_bytes);
-  const size_t o_st = sc.take((size_t)n_pages * sizeof(ZPage)), o_blk = sc.take((size_t)bb[n_pages] * sizeof(ZBlk));
-  const size_t o_fr = sc.take((size_t)fb[n_pages] * sizeof(ZFrame)), o_lit = sc.take((size_t)lb[n_pages]);
-  const size_t o_ll = sc.take((size_t)sq[n_pages] * 4), o_ml = sc.take((size_t)sq[n_pages] * 4), o_of = sc.take((size_t)sq[n_pages] * 4);
-  const size_t o_eo = sc.take((size_t)eb[n_pages] * 4), o_er = sc.take((size_t)eb[n_pages] * 4), o_ek = sc.take((size_t)eb[n_pages]);
+  sc.take(plan.bytes.size());
+  const size_t o_st = sc.take((size_t)n_pages * sizeof(ZPage)), o_blk = sc.take((size_t)n_blk * sizeof(ZBlk));
+  const size_t o_fr = sc.take((size_t)n_frame * sizeof(ZFrame)), o_lit = sc.take((size_t)n_lit);
+  const size_t o_ll = sc.take((size_t)n_seq * 4), o_ml = sc.take((size_t)n_seq * 4), o_of = sc.take((size_t)n_seq * 4);
+  const size_t o_eo = sc.take((size_t)n_elem * 4), o_er = sc.take((size_t)n_elem * 4), o_ek = sc.take((size_t)n_elem);
   // this call synchronises `st` anyway, so its device scratch may live in a Temps
   Temps t(st);
   uint8_t* d;
   AG_TRY(t.alloc_t(&d, sc.size));
-  AG_TRY(h2d(d, h.data(), plan_bytes, st));
-  const int64_t* dbase = reinterpret_cast<const int64_t*>(d + pb);
+  LzPlanDev<5> pl;
+  AG_TRY(lz_upload(plan, d, st, &pl));
   ZArgs a;
-  a.pages = reinterpret_cast<const ag_pq_compressed*>(d);
-  a.blk_base = dbase; a.frame_base = dbase + n1; a.lit_base = dbase + 2 * n1; a.seq_base = dbase + 3 * n1; a.elem_base = dbase + 4 * n1;
+  a.pages = pl.pages;
+  a.blk_base = pl.base[0]; a.frame_base = pl.base[1]; a.lit_base = pl.base[2]; a.seq_base = pl.base[3]; a.elem_base = pl.base[4];
   a.src = src; a.dst = dst;
   a.st = reinterpret_cast<ZPage*>(d + o_st);
   a.blk = reinterpret_cast<ZBlk*>(d + o_blk);
@@ -942,28 +920,14 @@ ag_status zstd_dev(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_
   x.pages = a.pages; x.elem_base = a.elem_base; x.src = src; x.lit = a.lit; x.lit_base = a.lit_base; x.dst = dst;
   x.done = reinterpret_cast<const int64_t*>(a.st); x.stride = sizeof(ZPage) / 8;
   x.e_out = a.e_out; x.e_ref = a.e_ref; x.e_lit = a.e_lit;
-  zstd_exec_kernel<<<(unsigned)n_pages, kLzThreads, 0, st>>>(x);
-  AG_TRY(check_launch("zstd_exec_kernel"));
+  AG_TRY(lz_exec_launch(x, n_pages, st));
   zstd_xxh64_kernel<<<split, 32 * kWarps, 0, st>>>(a);
   AG_TRY(check_launch("zstd_xxh64_kernel"));
-  std::vector<ZPage> hs((size_t)n_pages);
-  AG_TRY(d2h(hs.data(), a.st, (size_t)n_pages * sizeof(ZPage), st));
-  AG_TRY(sync(st));
-  if (h_written)
-    for (int64_t i = 0; i < n_pages; ++i) h_written[i] = hs[i].written;
-  for (int64_t i = 0; i < n_pages; ++i) {
-    const ZPage& s = hs[i];
-    if (s.err == kZErrSize)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: metadata said %lld bytes uncompressed data page, got %lld bytes (0 bytes written)", fn,
-              (long long)i, (long long)pages[i].dst_len, (long long)s.got);
-    if (s.ck_bad != INT32_MAX)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: could not decompress page: zstd: checksum mismatch (%lld bytes written)", fn,
-              (long long)i, (long long)s.written);
-    if (s.err == kZErrCorrupt)
-      AG_FAIL(AG_ERR_INVALID, "%s: page %lld: parquet: could not decompress page: zstd: %s (%lld bytes written)", fn, (long long)i,
-              kCheckName[s.check], (long long)s.written);
-  }
-  return AG_OK;
+  return lz_read_back(kFn, a.st, n_pages, h_written, st, [&](int64_t i, const ZPage& s, char* buf, size_t n) {
+    if (s.err == kZErrSize) size_text(buf, n, pages[i].dst_len, s.got);
+    else if (s.ck_bad != INT32_MAX) snprintf(buf, n, "parquet: could not decompress page: zstd: checksum mismatch");
+    else if (s.err == kZErrCorrupt) snprintf(buf, n, "parquet: could not decompress page: zstd: %s", kCheckName[s.check]);
+  });
 }
 
 }  // namespace
@@ -977,13 +941,13 @@ extern "C" {
 ag_status ag_parquet_zstd_decompress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
                                          int64_t* d_written, ag_stream_t s) {
   AG_TRY(ensure_init());
-  return zstd_dev(d_src, pages, n_pages, d_dst, d_written, nullptr, resolve_stream(s));
+  return pq_decompress_dev(kFn, zstd_dev, d_src, pages, n_pages, d_dst, d_written, resolve_stream(s));
 }
 
 ag_status ag_parquet_zstd_decompress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
                                      int64_t* written) {
   AG_TRY(ensure_init());
-  return pq_decompress_host("zstd_decompress", zstd_dev, src, pages, n_pages, dst, written);
+  return pq_decompress_host(kFn, zstd_dev, src, pages, n_pages, dst, written);
 }
 
 }  // extern "C"

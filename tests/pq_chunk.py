@@ -29,7 +29,7 @@ def _groups(pages):
 def read_chunk_dev(ag, plan, offset_width=8, host_values=False):
     """The column reader flow on the device -> (values, validity):
        1. upload the chunk as it sits in the file;
-       2. one ag_parquet_{snappy,zstd}_decompress_dev call, or device copies of the pages that are not compressed,
+       2. one ag_parquet_{snappy,zstd,gzip,lz4_raw}_decompress_dev call, or device copies of the pages that are not compressed,
           every page body at its 8-byte aligned offset of one buffer `dst` (checked against host_decompress);
        3. an optional column's levels -> ag_parquet_def_levels_to_bitmap_dev -> the validity bitmap;
        4. the values, by physical type, width and encoding.
@@ -39,7 +39,8 @@ def read_chunk_dev(ag, plan, offset_width=8, host_values=False):
     dchunk = Dev(P.as_array(plan["chunk"]))
     ddst = Dev(nbytes=plan["n_dst"])
     if plan["comp"]:
-        fn = {"SNAPPY": "ag_parquet_snappy_decompress_dev", "ZSTD": "ag_parquet_zstd_decompress_dev"}[plan["codec"]]
+        fn = {"SNAPPY": "ag_parquet_snappy_decompress_dev", "ZSTD": "ag_parquet_zstd_decompress_dev",
+              "GZIP": "ag_parquet_gzip_decompress_dev", "LZ4": "ag_parquet_lz4_raw_decompress_dev"}[plan["codec"]]
         dw = Dev(np.full(len(plan["comp"]), -1, np.int64))
         ag.call(fn, dchunk.ptr, N.compressed_table(plan["comp"]), len(plan["comp"]), ddst.ptr, dw.ptr, None)
     for s, d, k in plan["copies"]:

@@ -159,12 +159,14 @@ def chunk_plan(path, column=0):
 
 
 def host_decompress(plan):
-    """the decompressed buffer `dst` built on the host with pyarrow"""
+    """the decompressed buffer `dst` built on the host with pyarrow (a Parquet "LZ4" chunk is LZ4_RAW, pyarrow's
+    "lz4_raw"; its "lz4" is the frame format)"""
     import pyarrow as pa
+    codec = {"LZ4": "lz4_raw"}.get(plan["codec"], plan["codec"].lower())
     out = bytearray(plan["n_dst"])
     for s, sl, d, dl in plan["comp"]:
         if dl:
-            out[d:d + dl] = pa.decompress(plan["chunk"][s:s + sl], decompressed_size=dl, codec=plan["codec"].lower(), asbytes=True)
+            out[d:d + dl] = pa.decompress(plan["chunk"][s:s + sl], decompressed_size=dl, codec=codec, asbytes=True)
     for s, d, n in plan["copies"]:
         out[d:d + n] = plan["chunk"][s:s + n]
     return bytes(out)

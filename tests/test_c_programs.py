@@ -14,6 +14,8 @@ PROGRAMS = [
     ("pq_delta_smoke", "pq_delta_smoke ok"),        # ag_parquet_delta_decode
     ("pq_snappy_smoke", "pq_snappy_smoke ok"),      # ag_parquet_snappy_decompress
     ("pq_zstd_smoke", "pq_zstd_smoke ok"),          # ag_parquet_zstd_decompress
+    ("pq_gzip_smoke", "pq_gzip_smoke ok"),          # ag_parquet_gzip_decompress
+    ("pq_lz4_smoke", "pq_lz4_smoke ok"),            # ag_parquet_lz4_raw_decompress
     ("pq_bytearray_smoke", "pq_bytearray_smoke ok"),  # ag_parquet_byte_array_decode
     ("pq_fixed_smoke", "pq_fixed_smoke ok"),        # ag_parquet_bool_decode and ag_parquet_fixed_decode
 ]

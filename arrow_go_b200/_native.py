@@ -66,6 +66,7 @@ def dict_chunk_table(chunks):
 
 NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1
 TYPE_DICTIONARY = 29
+TYPE_RUN_END_ENCODED = 38
 
 PQ_LEVELS_V2_RLE, PQ_LEVELS_V1_RLE, PQ_LEVELS_BIT_PACKED = 0, 1, 2
 # include/arrowgpu.h AG_PQ_ENC_* (parquet.thrift Encoding values)
@@ -225,6 +226,12 @@ _SIGS = {
     "ag_unique_dev": [_i, _p, _p, _i64, _i64, _p, _p, _i64, _p, _p],
     "ag_dictionary_encode": [_i, _p, _i64, _i, _p, _p, _p],
     "ag_dictionary_encode_dev": [_i, _p, _i64, _i, _p, _p, _p, _p],
+    "ag_run_end_count": [_i, _p, _p, _i64, _i64, _p],
+    "ag_run_end_count_dev": [_i, _p, _p, _i64, _i64, _p, _p],
+    "ag_run_end_encode": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _p],
+    "ag_run_end_encode_dev": [_i, _i, _p, _p, _i64, _i64, _p, _p, _p, _i64, _p, _p],
+    "ag_run_end_decode": [_i, _i, _p, _i64, _p, _p, _i64, _i64, _i64, _p, _p, _p],
+    "ag_run_end_decode_dev": [_i, _i, _p, _i64, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, _p],
     "ag_sort_indices": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64],
     "ag_sort_indices_dev": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64, _p],
     "ag_parquet_unpack32": [_p, _p, _i64, _i, _pi64],
@@ -305,6 +312,12 @@ _SIGS.update({
     "ag_export_dictionary_device_array": [_i, _i64, _i64, _i64, _p, _p, _i64, _i64, _i64, _p, _p, RELEASE_BUFFERS_FN, _p, _p,
                                           C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema)],
     "ag_import_dictionary_device_array": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), _p, C.POINTER(ArrayView), C.POINTER(ArrayView)],
+    "ag_run_end_encoded_device_array_describe": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), C.POINTER(ArrayView),
+                                                 C.POINTER(ArrayView), C.POINTER(ArrayView)],
+    "ag_export_run_end_encoded_device_array": [_i, _i, _i64, _i64, _i64, _p, _i64, _i64, _i64, _p, _p, RELEASE_BUFFERS_FN, _p, _p,
+                                               C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema)],
+    "ag_import_run_end_encoded_device_array": [C.POINTER(ArrowDeviceArray), C.POINTER(ArrowSchema), _p, C.POINTER(ArrayView),
+                                               C.POINTER(ArrayView), C.POINTER(ArrayView)],
 })
 
 _SPECIAL = {

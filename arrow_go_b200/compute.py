@@ -27,6 +27,7 @@ NP_OF = {UINT8: np.uint8, INT8: np.int8, UINT16: np.uint16, INT16: np.int16, UIN
          UINT64: np.uint64, INT64: np.int64, FLOAT32: np.float32, FLOAT64: np.float64}
 TYPE_OF_NP = {np.dtype(v): k for k, v in NP_OF.items()}
 DICTIONARY = 29   # Dictionary<int32, T>
+RUN_END_ENCODED = 38   # RunEndEncoded<int16|int32|int64, T>
 DROP_NULLS, EMIT_NULLS = 0, 1
 NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1   # DictionaryEncodeOptions.NullEncoding
 KIND_SCALAR, KIND_ARRAY, KIND_CHUNKED = 1, 2, 3
@@ -71,6 +72,8 @@ def lib():
         h.agx_value_type.argtypes = [p]
         h.agx_dictionary_indices.argtypes = [p, pp]
         h.agx_dictionary_values.argtypes = [p, pp]
+        h.agx_run_end_type.argtypes = [p]
+        h.agx_run_end_child.argtypes = [p, i, pp]
         h.agx_array_to_host.argtypes = [p, p, p, C.POINTER(i64)]
         h.agx_call_function.argtypes = [C.c_char_p, i, i, pp, i, pp]
         h.agx_arith.argtypes = [i, i, p, p, pp]
@@ -146,6 +149,27 @@ class Datum:
         d._keep = self
         return d
 
+    # ---- run-end encoded datums (RunEndEncoded<R, T>) ----
+    @property
+    def run_end_type(self):
+        """R of a run-end encoded datum; 0 for any other datum."""
+        return lib().agx_run_end_type(self._h)
+
+    def _run_end_child(self, which):
+        out = C.c_void_p()
+        _check(lib().agx_run_end_child(self._h, which, C.byref(out)))
+        d = Datum(out)
+        d._keep = self
+        return d
+
+    def run_ends(self):
+        """The run ends of a run-end encoded array (the whole child: a slice changes only the parent's offset / length)."""
+        return self._run_end_child(0)
+
+    def values(self):
+        """The values of each run of a run-end encoded array (the whole child)."""
+        return self._run_end_child(1)
+
     # ---- arrays ----
     @property
     def offset(self):
@@ -190,6 +214,13 @@ class Datum:
         return vals, valid, int(nulls.value)
 
     def to_pylist(self):
+        if self.type == RUN_END_ENCODED:   # expanded: the value of the run that covers each row of the slice
+            if self.kind == KIND_CHUNKED:
+                return [v for c in self.chunks() for v in c.to_pylist()]
+            ends = self.run_ends().to_numpy()[0].astype(np.int64)
+            vals = self.values().to_pylist()
+            rows = np.arange(self.offset, self.offset + len(self), dtype=np.int64)
+            return [vals[p] for p in np.searchsorted(ends, rows, side="right").tolist()]
         if self.type == DICTIONARY:   # decoded: the dictionary value of every index, None for a null index
             dictionary = self.dictionary().to_pylist()
             idx, valid, _ = self.indices().to_numpy()
@@ -258,10 +289,11 @@ def Chunked(chunks, type_id):
 
 def CallFunction(name, args, options=None):
     """compute.CallFunction(ctx, name, opts, args...) — options: None, ("arithmetic", no_check_overflow),
-    ("filter", null_selection), ("take", bounds_check) or ("dictionary_encode", null_encoding)."""
+    ("filter", null_selection), ("take", bounds_check), ("dictionary_encode", null_encoding) or
+    ("run_end_encode", run_end_type)."""
     kind, val = 0, 0
     if options is not None:
-        kind = {"arithmetic": 1, "filter": 2, "take": 3, "dictionary_encode": 4}[options[0]]
+        kind = {"arithmetic": 1, "filter": 2, "take": 3, "dictionary_encode": 4, "run_end_encode": 5}[options[0]]
         val = int(options[1])
     arr = (C.c_void_p * max(len(args), 1))(*[a._h for a in args])
     out = C.c_void_p()
@@ -360,6 +392,18 @@ def DictionaryEncode(values, null_encoding=NULL_ENCODING_MASK):
     Dictionary<int32, T> with the distinct values in order of first appearance; a chunked input gets one dictionary
     shared by its (non-empty) chunks."""
     return CallFunction("dictionary_encode", [values], ("dictionary_encode", null_encoding))
+
+
+def RunEndEncode(values, run_end_type):
+    """compute.RunEndEncode(ctx, RunEndEncodeOptions{RunEndType}, values) (arrow/compute/vector_run_ends.go:64-66):
+    RunEndEncoded<run_end_type, T>; run_end_type is INT16, INT32 or INT64.  A chunked input is encoded chunk by chunk."""
+    return CallFunction("run_end_encode", [values], ("run_end_encode", run_end_type))
+
+
+def RunEndDecode(values):
+    """compute.RunEndDecode(ctx, values) (arrow/compute/vector_run_ends.go:78-80): the plain array of a run-end encoded
+    one, chunk by chunk."""
+    return CallFunction("run_end_decode", [values])
 
 
 def IsIn(values, value_set, null_behavior=NULL_MATCH):

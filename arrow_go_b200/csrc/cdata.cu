@@ -20,6 +20,7 @@ struct ExportState {
   void (*release_buffers)(void*);
   void* opaque;
   struct ArrowArray* dictionary;   // a dictionary array's child (heap), released and freed with the parent
+  struct ArrowArray* children[2];  // a run-end encoded array's run_ends and values (heap), released and freed with it
 };
 
 void release_exported_array(struct ArrowArray* a) {
@@ -31,6 +32,11 @@ void release_exported_array(struct ArrowArray* a) {
     if (st->dictionary) {
       if (st->dictionary->release) st->dictionary->release(st->dictionary);   // unless the consumer moved it out
       free(st->dictionary);
+    }
+    for (struct ArrowArray* c : st->children) {
+      if (!c) continue;
+      if (c->release) c->release(c);   // unless the consumer moved it out
+      free(c);
     }
     free(st);
   }
@@ -52,6 +58,27 @@ void release_dictionary_schema(struct ArrowSchema* s) {
     s->dictionary = nullptr;
   }
   s->release = nullptr;
+}
+
+// a run-end encoded schema owns its two child schemas and their pointer array (heap)
+void release_run_end_schema(struct ArrowSchema* s) {
+  if (!s || !s->release) return;
+  for (int64_t k = 0; k < s->n_children; ++k) {
+    struct ArrowSchema* c = s->children[k];
+    if (c->release) c->release(c);
+    free(c);
+  }
+  free(s->children);
+  s->children = nullptr;
+  s->release = nullptr;
+}
+
+int run_end_type_of(const char* format) {
+  if (!format) return 0;
+  if (strcmp(format, "s") == 0) return AG_TYPE_INT16;
+  if (strcmp(format, "i") == 0) return AG_TYPE_INT32;
+  if (strcmp(format, "l") == 0) return AG_TYPE_INT64;
+  return 0;
 }
 
 }  // namespace
@@ -257,6 +284,111 @@ extern "C" ag_status ag_export_dictionary_device_array(int value_type, int64_t l
   if (out_schema) {
     out_schema->dictionary = child_schema;
     out_schema->release = release_dictionary_schema;
+  }
+  return AG_OK;
+}
+
+// Run-end encoded: a "+r" parent without buffers and two children, run_ends and values, each described by
+// ag_device_array_describe on a shallow copy of the parent's device array.
+extern "C" ag_status ag_run_end_encoded_device_array_describe(const struct ArrowDeviceArray* in, const struct ArrowSchema* schema,
+                                                              ag_array_view* parent, ag_array_view* run_ends, ag_array_view* values) {
+  if (!in || !schema || !parent || !run_ends || !values) AG_FAIL(AG_ERR_INVALID, "cdata: NULL array / schema / view");
+  const struct ArrowArray& a = in->array;
+  if (!a.release || !schema->release) AG_FAIL(AG_ERR_INVALID, "cdata: array or schema was already released");
+  if (!schema->format || strcmp(schema->format, "+r") != 0) AG_FAIL(AG_ERR_INVALID, "cdata: not a run-end encoded array (format '%s')", schema->format ? schema->format : "");
+  if (a.n_children != 2 || schema->n_children != 2 || !a.children || !schema->children)
+    AG_FAIL(AG_ERR_INVALID, "cdata: a run-end encoded array has two children (run_ends, values)");
+  if (a.n_buffers != 0 || a.dictionary) AG_FAIL(AG_ERR_INVALID, "cdata: a run-end encoded parent has no buffers and no dictionary");
+  if (a.length < 0 || a.offset < 0) AG_FAIL(AG_ERR_INVALID, "cdata: negative length or offset");
+  if (a.null_count > 0) AG_FAIL(AG_ERR_INVALID, "cdata: a run-end encoded parent has no nulls of its own");
+  const int rt = run_end_type_of(schema->children[0]->format);
+  if (!rt) AG_FAIL(AG_ERR_INVALID, "cdata: run_ends of format '%s' (int16 's', int32 'i' or int64 'l')",
+                   schema->children[0]->format ? schema->children[0]->format : "");
+  struct ArrowDeviceArray child = *in;
+  child.array = *a.children[0];
+  AG_TRY(ag_device_array_describe(&child, schema->children[0], run_ends));
+  if (run_ends->null_count > 0) AG_FAIL(AG_ERR_INVALID, "cdata: run_ends must not contain nulls");
+  child.array = *a.children[1];
+  AG_TRY(ag_device_array_describe(&child, schema->children[1], values));
+  if (values->length < run_ends->length) AG_FAIL(AG_ERR_INVALID, "cdata: the values child is shorter than run_ends");
+  memset(parent, 0, sizeof(*parent));
+  parent->type = AG_TYPE_RUN_END_ENCODED;
+  parent->length = a.length;
+  parent->offset = a.offset;
+  parent->device_type = in->device_type;
+  parent->device_id = in->device_id;
+  return AG_OK;
+}
+
+extern "C" ag_status ag_import_run_end_encoded_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on,
+                                                            ag_array_view* parent, ag_array_view* run_ends, ag_array_view* values) {
+  AG_TRY(ensure_init());
+  AG_TRY(ag_run_end_encoded_device_array_describe(in, schema, parent, run_ends, values));
+  return import_wait(in, consume_on);
+}
+
+extern "C" ag_status ag_export_run_end_encoded_device_array(int value_type, int run_end_type, int64_t length, int64_t offset,
+                                                            int64_t n_runs, const void* d_run_ends,
+                                                            int64_t values_length, int64_t values_null_count, int64_t values_offset,
+                                                            const void* d_values_validity, const void* d_values,
+                                                            void (*release_buffers)(void*), void* opaque, ag_stream_t produced_on,
+                                                            struct ArrowDeviceArray* out, struct ArrowSchema* out_schema) {
+  AG_TRY(ensure_init());
+  if (!out) AG_FAIL(AG_ERR_INVALID, "cdata: NULL output");
+  if (!ag_type_to_schema_format(value_type)) AG_FAIL(AG_ERR_TYPE, "cdata: unsupported run-end encoded value type id %d", value_type);
+  if (run_end_type != AG_TYPE_INT16 && run_end_type != AG_TYPE_INT32 && run_end_type != AG_TYPE_INT64)
+    AG_FAIL(AG_ERR_INVALID, "cdata: bad run end type %d", run_end_type);
+  if (length < 0 || offset < 0 || n_runs < 0 || values_length < 0 || values_offset < 0) AG_FAIL(AG_ERR_INVALID, "cdata: negative length or offset");
+  struct ArrowArray* kids[2] = {nullptr, nullptr};
+  struct ArrowSchema* kid_schemas[2] = {nullptr, nullptr};
+  struct ArrowSchema** schema_children = nullptr;
+  auto cleanup = [&] {
+    for (int k = 0; k < 2; ++k) {
+      if (kids[k]) { if (kids[k]->release) kids[k]->release(kids[k]); free(kids[k]); }
+      if (kid_schemas[k]) { if (kid_schemas[k]->release) kid_schemas[k]->release(kid_schemas[k]); free(kid_schemas[k]); }
+    }
+    free(schema_children);
+  };
+  for (int k = 0; k < 2; ++k) {
+    kids[k] = static_cast<struct ArrowArray*>(calloc(1, sizeof(struct ArrowArray)));
+    if (out_schema) kid_schemas[k] = static_cast<struct ArrowSchema*>(calloc(1, sizeof(struct ArrowSchema)));
+    if (!kids[k] || (out_schema && !kid_schemas[k])) { cleanup(); AG_FAIL(AG_ERR_OOM, "cdata: out of host memory"); }
+  }
+  if (out_schema) {
+    schema_children = static_cast<struct ArrowSchema**>(calloc(2, sizeof(struct ArrowSchema*)));
+    if (!schema_children) { cleanup(); AG_FAIL(AG_ERR_OOM, "cdata: out of host memory"); }
+  }
+  // the children: primitive exports whose buffers the parent's release_buffers covers
+  struct ArrowDeviceArray tmp;
+  ag_status rc = ag_export_device_array(run_end_type, n_runs, 0, 0, nullptr, d_run_ends, nullptr, nullptr, produced_on, &tmp, kid_schemas[0]);
+  if (rc != AG_OK) { cleanup(); return rc; }
+  *kids[0] = tmp.array;
+  rc = ag_export_device_array(value_type, values_length, values_null_count, values_offset, d_values_validity, d_values, nullptr, nullptr,
+                              produced_on, &tmp, kid_schemas[1]);
+  if (rc != AG_OK) { cleanup(); return rc; }
+  *kids[1] = tmp.array;
+  // the parent: an empty primitive export turned into "+r" without buffers; its release runs release_buffers, then the
+  // children
+  rc = ag_export_device_array(value_type, 0, 0, 0, nullptr, nullptr, release_buffers, opaque, produced_on, out, out_schema);
+  if (rc != AG_OK) { cleanup(); return rc; }
+  ExportState* st = static_cast<ExportState*>(out->array.private_data);
+  out->array.length = length;
+  out->array.offset = offset;
+  st->children[0] = kids[0];
+  st->children[1] = kids[1];
+  out->array.n_buffers = 0;
+  out->array.n_children = 2;
+  out->array.children = st->children;
+  if (out_schema) {
+    kid_schemas[0]->name = "run_ends";
+    kid_schemas[0]->flags = 0;   // run ends are never null
+    kid_schemas[1]->name = "values";
+    schema_children[0] = kid_schemas[0];
+    schema_children[1] = kid_schemas[1];
+    out_schema->format = "+r";
+    out_schema->n_children = 2;
+    out_schema->children = schema_children;
+    out_schema->release = release_run_end_schema;
   }
   return AG_OK;
 }

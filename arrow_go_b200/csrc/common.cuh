@@ -126,6 +126,13 @@ ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int6
                      int64_t* d_out_len, cudaStream_t st);
 ag_status dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* dict,
                                 uint8_t* dict_valid, int64_t* d_counts, cudaStream_t st);
+// run_end.cu
+ag_status run_end_count_dev(int type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, int64_t* d_counts, cudaStream_t st);
+ag_status run_end_encode_dev(int type, int run_end_type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n,
+                             void* run_ends, void* out, uint8_t* out_valid, int64_t capacity, int64_t* d_counts, cudaStream_t st);
+ag_status run_end_decode_dev(int type, int run_end_type, const void* run_ends, int64_t n_runs, const void* vals, const uint8_t* valid,
+                             int64_t values_offset, int64_t offset, int64_t length, void* out, uint8_t* out_valid,
+                             int64_t* d_null_count, int64_t* d_error_word, cudaStream_t st);
 // sort.cu
 ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int64_t voff, int64_t n, int order, int null_placement,
                            uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);

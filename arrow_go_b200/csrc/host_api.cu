@@ -833,4 +833,107 @@ ag_status ag_dictionary_encode(int bit_width, const ag_dict_chunk* chunks, int64
   return sync(cs);
 }
 
+// Stage a values column for the run-end kernels: rows [off, off+n) of `vals` (a bitmap for BOOL) and `valid`, on the
+// device with the same row phase; *d_off is the offset that addresses row 0 of the copies.
+static ag_status upload_values(Temps& t, int type, const void* vals, const uint8_t* valid, int64_t off, int64_t n,
+                               const void** d_vals, uint8_t** d_valid, int64_t* d_off) {
+  if (type == AG_TYPE_BOOL) {
+    uint8_t* dv;
+    AG_TRY(upload_bitmap(t, static_cast<const uint8_t*>(vals), off, n, &dv, d_off));
+    *d_vals = dv;
+    int64_t phase;
+    return upload_bitmap(t, valid, off, n, d_valid, &phase);
+  }
+  if (type_width(type) == 0) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "run_end: type id %d (boolean and the 10 numeric types only)", type);
+  return upload_column(t, vals, valid, off, n, type_width(type), d_vals, d_valid, d_off);
+}
+static int run_end_width(int run_end_type) {
+  return run_end_type == AG_TYPE_INT16 ? 2 : (run_end_type == AG_TYPE_INT32 ? 4 : (run_end_type == AG_TYPE_INT64 ? 8 : 0));
+}
+static size_t value_bytes(int type, int64_t n) { return (size_t)(type == AG_TYPE_BOOL ? (n + 7) / 8 : n * type_width(type)); }
+static size_t word_bytes(int64_t nbits) { return (size_t)((nbits + 31) / 32) * 4; }
+
+ag_status ag_run_end_count(int type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, int64_t* counts) {
+  AG_TRY(ensure_init());
+  if (!counts) AG_FAIL(AG_ERR_INVALID, "run_end_count: NULL counts");
+  counts[0] = counts[1] = 0;
+  if (n < 0 || offset < 0) AG_FAIL(AG_ERR_INVALID, "run_end_count: negative length or offset");
+  if (n == 0) return AG_OK;
+  if (!vals) AG_FAIL(AG_ERR_INVALID, "run_end_count: NULL values");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const void* dv; uint8_t* dvv; int64_t ov; int64_t* dc;
+  AG_TRY(upload_values(t, type, vals, valid, offset, n, &dv, &dvv, &ov));
+  AG_TRY(t.alloc_t(&dc, 16));
+  AG_TRY(run_end_count_dev(type, dv, dvv, ov, n, dc, cs));
+  AG_TRY(d2h(counts, dc, 16, cs));
+  return sync(cs);
+}
+
+ag_status ag_run_end_encode(int type, int run_end_type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n,
+                            void* run_ends, void* out, uint8_t* out_valid, int64_t capacity, int64_t* counts) {
+  AG_TRY(ensure_init());
+  if (!counts) AG_FAIL(AG_ERR_INVALID, "run_end_encode: NULL counts");
+  counts[0] = counts[1] = 0;
+  const int rw = run_end_width(run_end_type);
+  if (rw == 0) AG_FAIL(AG_ERR_INVALID, "run_end_encode: bad run end type %d", run_end_type);
+  if (n < 0 || offset < 0 || capacity < 0) AG_FAIL(AG_ERR_INVALID, "run_end_encode: negative length, offset or capacity");
+  if (capacity > 0 && (!run_ends || !out)) AG_FAIL(AG_ERR_INVALID, "run_end_encode: NULL run_ends / values output");
+  if (valid && capacity > 0 && !out_valid) AG_FAIL(AG_ERR_INVALID, "run_end_encode: an input with a validity bitmap needs an output validity bitmap");
+  if (n > 0 && !vals) AG_FAIL(AG_ERR_INVALID, "run_end_encode: NULL values");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const void* dv = nullptr; uint8_t* dvv = nullptr; int64_t ov = 0; int64_t* dc;
+  void *dre, *dout; uint8_t* dov = nullptr;
+  if (n > 0) AG_TRY(upload_values(t, type, vals, valid, offset, n, &dv, &dvv, &ov));
+  AG_TRY(t.alloc(&dre, (size_t)capacity * rw));
+  AG_TRY(t.alloc(&dout, type == AG_TYPE_BOOL ? word_bytes(capacity) : value_bytes(type, capacity)));
+  if (valid) AG_TRY(t.alloc_t(&dov, word_bytes(capacity)));
+  AG_TRY(t.alloc_t(&dc, 16));
+  AG_TRY(run_end_encode_dev(type, run_end_type, dv, dvv, ov, n, dre, dout, dov, capacity, dc, cs));
+  AG_TRY(d2h(counts, dc, 16, cs));
+  AG_TRY(sync(cs));
+  const int64_t runs = counts[0] < capacity ? counts[0] : capacity;
+  AG_TRY(d2h(run_ends, dre, (size_t)runs * rw, cs));
+  AG_TRY(d2h(out, dout, value_bytes(type, runs), cs));
+  if (dov) AG_TRY(d2h(out_valid, dov, (size_t)((runs + 7) / 8), cs));
+  return sync(cs);
+}
+
+ag_status ag_run_end_decode(int type, int run_end_type, const void* run_ends, int64_t n_runs, const void* vals, const uint8_t* valid,
+                            int64_t values_offset, int64_t offset, int64_t length, void* out, uint8_t* out_valid, int64_t* null_count) {
+  AG_TRY(ensure_init());
+  if (null_count) *null_count = 0;
+  const int rw = run_end_width(run_end_type);
+  if (rw == 0) AG_FAIL(AG_ERR_INVALID, "run_end_decode: bad run end type %d", run_end_type);
+  if (n_runs < 0 || values_offset < 0 || offset < 0 || length < 0) AG_FAIL(AG_ERR_INVALID, "run_end_decode: negative length or offset");
+  if (length == 0) return AG_OK;
+  if (!run_ends && n_runs > 0) AG_FAIL(AG_ERR_INVALID, "run_end_decode: NULL run_ends");
+  if (!vals || !out) AG_FAIL(AG_ERR_INVALID, "run_end_decode: NULL values / output");
+  if (valid && !out_valid) AG_FAIL(AG_ERR_INVALID, "run_end_decode: a values child with a validity bitmap needs an output validity bitmap");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  void *dre, *dout; const void* dv = nullptr; uint8_t *dvv = nullptr, *dov = nullptr; int64_t ov = 0; int64_t* dw;
+  AG_TRY(t.alloc(&dre, (size_t)n_runs * rw));
+  AG_TRY(h2d(dre, run_ends, (size_t)n_runs * rw, cs));
+  if (n_runs > 0) AG_TRY(upload_values(t, type, vals, valid, values_offset, n_runs, &dv, &dvv, &ov));
+  else { void* z; AG_TRY(t.alloc(&z, 8)); dv = z; }
+  if (valid && !dvv) AG_TRY(t.alloc_t(&dvv, 8));
+  AG_TRY(t.alloc(&dout, type == AG_TYPE_BOOL ? word_bytes(length) : value_bytes(type, length)));
+  if (valid) AG_TRY(t.alloc_t(&dov, word_bytes(length)));
+  AG_TRY(t.alloc_t(&dw, 16));
+  AG_TRY(error_word_reset(dw + 1, cs));
+  AG_TRY(run_end_decode_dev(type, run_end_type, dre, n_runs, dv, dvv, ov, offset, length, dout, dov, dw, dw + 1, cs));
+  int64_t h[2];
+  AG_TRY(d2h(h, dw, 16, cs));
+  AG_TRY(sync(cs));
+  if (h[1] != AG_NO_ERROR_POS)
+    AG_FAIL(AG_ERR_INVALID, "run_end_decode: malformed run ends at run %lld (they must increase strictly and reach offset+length)", (long long)h[1]);
+  AG_TRY(d2h(out, dout, value_bytes(type, length), cs));
+  if (dov) AG_TRY(d2h(out_valid, dov, (size_t)((length + 7) / 8), cs));
+  AG_TRY(sync(cs));
+  if (null_count) *null_count = h[0];
+  return AG_OK;
+}
+
 }  // extern "C"

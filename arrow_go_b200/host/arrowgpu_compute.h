@@ -34,7 +34,8 @@ namespace arrowgpu {
 enum class Type : int {
   NA = 0, BOOL = 1, UINT8 = 2, INT8 = 3, UINT16 = 4, INT16 = 5, UINT32 = 6, INT32 = 7,
   UINT64 = 8, INT64 = 9, FLOAT16 = 10, FLOAT32 = 11, FLOAT64 = 12,
-  DICTIONARY = 29  // Dictionary<int32, T> only: indices in buffers[1], the values in ArrayData::dictionary
+  DICTIONARY = 29,  // Dictionary<int32, T> only: indices in buffers[1], the values in ArrayData::dictionary
+  RUN_END_ENCODED = 38  // no buffers: the children ArrayData::run_ends (int16/32/64) and ArrayData::values
 };
 int BitWidth(Type t);  // 1 for BOOL
 const char* TypeName(Type t);
@@ -86,6 +87,8 @@ struct ArrayData {
   int64_t offset = 0;
   std::shared_ptr<Buffer> buffers[2];  // [0] validity bitmap (may be null), [1] values / boolean data / int32 indices
   std::shared_ptr<ArrayData> dictionary;  // DICTIONARY: the dictionary values (a primitive array), shared by slices
+  // RUN_END_ENCODED: the run ends and the values of each run, shared by slices (a slice changes only offset / length)
+  std::shared_ptr<ArrayData> run_ends, values;
   std::shared_ptr<ArrayData> Slice(int64_t off, int64_t len) const;  // array.NewSlice semantics
   // validity (LSB-first bitmap, `offset` applies) may be NULL; values must hold (offset+length) elements
   static Status FromHost(Type type, int64_t length, int64_t offset, const uint8_t* validity, const void* values,
@@ -103,7 +106,8 @@ struct ArrayData {
 
 struct ChunkedArray {  // arrow.Chunked (arrow/table.go:135-143)
   Type type = Type::NA;
-  Type value_type = Type::NA;  // DICTIONARY: the dictionary's value type (known even with zero chunks)
+  Type value_type = Type::NA;  // DICTIONARY / RUN_END_ENCODED: the value type (known even with zero chunks)
+  Type run_end_type = Type::NA;  // RUN_END_ENCODED: the run ends' type
   std::vector<std::shared_ptr<ArrayData>> chunks;
   int64_t length = 0;
   int64_t NullN() const;
@@ -264,6 +268,10 @@ struct DictionaryEncodeOptions : FunctionOptions {                            //
   NullEncodingBehavior NullEncoding = NullEncodingMask;
   const char* TypeName() const override { return "DictionaryEncodeOptions"; }
 };
+struct RunEndEncodeOptions : FunctionOptions {                                // compute/vector_run_ends.go:43 (kernels.RunEndEncodeState)
+  Type RunEndType = Type::INT32;   // INT16, INT32 or INT64
+  const char* TypeName() const override { return "RunEndEncodeOptions"; }
+};
 struct SetLookupOptions : FunctionOptions {                   // compute/scalar_set_lookup.go (ValueSet, NullBehavior)
   std::shared_ptr<ArrayData> ValueSet;
   NullMatchingBehavior NullBehavior = NullMatchingMatch;
@@ -368,6 +376,10 @@ Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out);
 // chunks and loses its empty chunks; a dictionary input is returned as it is
 Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts, const Datum& values, Datum* out);
 Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& values, Datum* out);
+// compute.RunEndEncode / RunEndDecode (vector_run_ends.go:64-73), BOOL and the numeric types; chunkwise: runs never
+// cross a chunk boundary
+Status RunEndEncode(const ExecCtx& ctx, const RunEndEncodeOptions& opts, const Datum& values, Datum* out);
+Status RunEndDecode(const ExecCtx& ctx, const Datum& values, Datum* out);
 
 // ---- executor internals exposed for tests (exec_internals_test.go exercises the same pieces) ----
 struct SpanPiece { int64_t pos; int64_t len; std::vector<int> chunk_index; std::vector<int64_t> chunk_pos; };

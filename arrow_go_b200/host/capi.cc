@@ -41,10 +41,17 @@ int agx_chunked(int type, agx_datum** chunks, int n, agx_datum** out) {
     if (n == 0) return fail(Status::Invalid("chunked: a dictionary column without chunks has no value type"));
     if (chunks[0]->d.kind == DatumKind::ARRAY && chunks[0]->d.array->dictionary) c->value_type = chunks[0]->d.array->dictionary->type;
   }
+  if (c->type == Type::RUN_END_ENCODED) {   // the value and run-end types come from the chunks' children
+    if (n == 0) return fail(Status::Invalid("chunked: a run-end encoded column without chunks has no value type"));
+    const auto& a0 = chunks[0]->d.array;
+    if (chunks[0]->d.kind == DatumKind::ARRAY && a0->values) { c->value_type = a0->values->type; c->run_end_type = a0->run_ends->type; }
+  }
   for (int i = 0; i < n; ++i) {
     if (chunks[i]->d.kind != DatumKind::ARRAY || chunks[i]->d.array->type != c->type) return fail(Status::Invalid("chunked: chunks must be arrays of the chunked type"));
     if (c->type == Type::DICTIONARY && chunks[i]->d.array->dictionary->type != c->value_type)
       return fail(Status::Invalid("chunked: dictionary chunks must share one value type"));
+    if (c->type == Type::RUN_END_ENCODED && (chunks[i]->d.array->values->type != c->value_type || chunks[i]->d.array->run_ends->type != c->run_end_type))
+      return fail(Status::Invalid("chunked: run-end encoded chunks must share one value type and one run-end type"));
     c->chunks.push_back(chunks[i]->d.array);
     c->length += chunks[i]->d.array->length;
   }
@@ -68,7 +75,20 @@ int64_t agx_null_count_raw(agx_datum* d) { return d->d.kind == DatumKind::ARRAY 
 int agx_value_type(agx_datum* d) {
   if (d->d.kind == DatumKind::ARRAY && d->d.array->dictionary) return (int)d->d.array->dictionary->type;
   if (d->d.kind == DatumKind::CHUNKED && d->d.chunked->type == Type::DICTIONARY) return (int)d->d.chunked->value_type;
+  if (d->d.kind == DatumKind::ARRAY && d->d.array->values) return (int)d->d.array->values->type;
+  if (d->d.kind == DatumKind::CHUNKED && d->d.chunked->type == Type::RUN_END_ENCODED) return (int)d->d.chunked->value_type;
   return (int)d->d.type();
+}
+// Run-end encoded arrays: the run-end type and the two children (shared with the datum, whatever its offset)
+int agx_run_end_type(agx_datum* d) {
+  if (d->d.kind == DatumKind::ARRAY && d->d.array->run_ends) return (int)d->d.array->run_ends->type;
+  if (d->d.kind == DatumKind::CHUNKED && d->d.chunked->type == Type::RUN_END_ENCODED) return (int)d->d.chunked->run_end_type;
+  return 0;
+}
+int agx_run_end_child(agx_datum* d, int which, agx_datum** out) {
+  if (d->d.kind != DatumKind::ARRAY || d->d.array->type != Type::RUN_END_ENCODED) return fail(Status::TypeError("run ends / values: not a run-end encoded array"));
+  *out = new agx_datum{Datum(which == 0 ? d->d.array->run_ends : d->d.array->values)};
+  return AG_OK;
 }
 int agx_dictionary_indices(agx_datum* d, agx_datum** out) {
   auto indices = [](const std::shared_ptr<ArrayData>& a) { auto r = std::make_shared<ArrayData>(*a); r->type = Type::INT32; r->dictionary = nullptr; return r; };
@@ -102,16 +122,18 @@ int agx_array_to_host(agx_datum* d, void* values, uint8_t* validity, int64_t* nu
 }
 
 // opt_kind: 0 none, 1 ArithmeticOptions{NoCheckOverflow=opt_value}, 2 FilterOptions{NullSelection=opt_value},
-//           3 TakeOptions{BoundsCheck=opt_value}, 4 DictionaryEncodeOptions{NullEncoding=opt_value}
+//           3 TakeOptions{BoundsCheck=opt_value}, 4 DictionaryEncodeOptions{NullEncoding=opt_value},
+//           5 RunEndEncodeOptions{RunEndType=opt_value}
 int agx_call_function(const char* name, int opt_kind, int opt_value, agx_datum** args, int nargs, agx_datum** out) {
   std::vector<Datum> a;
   for (int i = 0; i < nargs; ++i) a.push_back(args[i]->d);
-  ArithmeticOptions ao; FilterOptions fo; TakeOptions to; DictionaryEncodeOptions deo;
+  ArithmeticOptions ao; FilterOptions fo; TakeOptions to; DictionaryEncodeOptions deo; RunEndEncodeOptions reo;
   const FunctionOptions* opts = nullptr;
   if (opt_kind == 1) { ao.NoCheckOverflow = opt_value != 0; opts = &ao; }
   if (opt_kind == 2) { fo.NullSelection = (NullSelectionBehavior)opt_value; opts = &fo; }
   if (opt_kind == 3) { to.BoundsCheck = opt_value != 0; opts = &to; }
   if (opt_kind == 4) { deo.NullEncoding = (NullEncodingBehavior)opt_value; opts = &deo; }
+  if (opt_kind == 5) { reo.RunEndType = (Type)opt_value; opts = &reo; }
   ExecCtx ctx;
   Datum r;
   AGX_TRY(CallFunction(ctx, name, opts, a, &r));

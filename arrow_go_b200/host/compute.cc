@@ -21,6 +21,7 @@ int BitWidth(Type t) {
 }
 const char* TypeName(Type t) {
   if (t == Type::DICTIONARY) return "dictionary";
+  if (t == Type::RUN_END_ENCODED) return "run_end_encoded";
   static const char* names[] = {"null", "bool", "uint8", "int8", "uint16", "int16", "uint32", "int32", "uint64", "int64", "float16", "float32", "float64"};
   const int i = (int)t;
   return (i >= 0 && i <= 12) ? names[i] : "unknown";
@@ -98,6 +99,16 @@ void ReleaseExportedBuffers(void* opaque) { delete static_cast<ExportedBuffers*>
 }  // namespace
 
 Status ArrayData::ExportDevice(struct ArrowDeviceArray* out, struct ArrowSchema* out_schema) const {
+  if (type == Type::RUN_END_ENCODED) {
+    const ArrayData &r = *run_ends, &v = *values;
+    auto* keep = new ExportedBuffers{{r.buffers[1], v.buffers[0], v.buffers[1]}};
+    const int rc = ag_export_run_end_encoded_device_array((int)v.type, (int)r.type, length, offset, r.length,
+                                                          r.buffers[1] ? r.buffers[1]->data() + r.offset * (BitWidth(r.type) / 8) : nullptr,
+                                                          v.length, v.null_count, v.offset, v.buffers[0] ? v.buffers[0]->data() : nullptr,
+                                                          v.buffers[1] ? v.buffers[1]->data() : nullptr, ReleaseExportedBuffers, keep, nullptr, out, out_schema);
+    if (rc != AG_OK) { delete keep; return Status::FromNative(rc); }
+    return Status::OK();
+  }
   if (type == Type::DICTIONARY) {
     const ArrayData& d = *dictionary;
     auto* keep = new ExportedBuffers{{buffers[0], buffers[1], d.buffers[0], d.buffers[1]}};
@@ -116,6 +127,28 @@ Status ArrayData::ExportDevice(struct ArrowDeviceArray* out, struct ArrowSchema*
 }
 
 Status ArrayData::ImportDevice(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, std::shared_ptr<ArrayData>* out) {
+  if (in && schema && schema->format && strcmp(schema->format, "+r") == 0) {
+    ag_array_view pv, rv, vv;
+    NATIVE(ag_import_run_end_encoded_device_array(in, schema, nullptr, &pv, &rv, &vv));
+    // move the struct: the importer owns it now; the children keep the parent alive, its release releases them
+    auto owned = std::make_shared<ArrowDeviceArray>(*in);
+    in->array.release = nullptr;
+    auto releaser = std::shared_ptr<void>(nullptr, [owned](void*) { if (owned->array.release) owned->array.release(&owned->array); });
+    auto child = [&](const ag_array_view& v) {
+      auto c = std::make_shared<ArrayData>();
+      c->type = (Type)v.type; c->length = v.length; c->offset = v.offset; c->null_count = v.validity ? v.null_count : 0;
+      const int64_t m = v.offset + v.length;
+      if (v.validity) c->buffers[0] = Buffer::Wrap(v.validity, BytesForBits(m), [releaser] {});
+      c->buffers[1] = Buffer::Wrap(v.values, DataBytes(c->type, m), [releaser] {});
+      return c;
+    };
+    auto d = std::make_shared<ArrayData>();
+    d->type = Type::RUN_END_ENCODED; d->length = pv.length; d->offset = pv.offset; d->null_count = 0;
+    d->run_ends = child(rv);
+    d->values = child(vv);
+    *out = d;
+    return Status::OK();
+  }
   const bool dict = in && in->array.dictionary;
   ag_array_view v, dv{};
   if (dict) {
@@ -171,6 +204,7 @@ Status ArrayData::FromHost(Type type, int64_t length, int64_t offset, const uint
 
 Status ArrayData::ToHost(void* values, uint8_t* validity, int64_t* null_count_out) const {
   if (type == Type::DICTIONARY) return Status::TypeError("to_host: a dictionary array is read through its indices and dictionary");
+  if (type == Type::RUN_END_ENCODED) return Status::TypeError("to_host: a run-end encoded array is read through its run ends and values");
   if (length == 0) { if (null_count_out) *null_count_out = 0; return Status::OK(); }
   const int w = BitWidth(type);
   if (values) {
@@ -743,10 +777,13 @@ Status CallFunction(const ExecCtx& ctx, const std::string& name, const FunctionO
   FunctionRegistry* reg = ctx.Registry ? ctx.Registry : GetFunctionRegistry();
   const Function* fn = reg->GetFunction(name);
   if (!fn) return Status::Make(AG_ERR_INVALID, "no function registered with name: " + name);  // arrow.ErrKey
-  // dictionary arrays reach the kernels only through dictionary_encode (its identity case)
-  if (name != "dictionary_encode")
-    for (auto& a : args)
-      if (a.kind != DatumKind::NONE && a.type() == Type::DICTIONARY) return Status::NotImplemented("function '" + name + "' has no kernel for dictionary arguments");
+  // dictionary arrays reach the kernels only through dictionary_encode (its identity case), run-end encoded arrays only
+  // through run_end_decode
+  for (auto& a : args) {
+    if (a.kind == DatumKind::NONE) continue;
+    if (name != "dictionary_encode" && a.type() == Type::DICTIONARY) return Status::NotImplemented("function '" + name + "' has no kernel for dictionary arguments");
+    if (name != "run_end_decode" && a.type() == Type::RUN_END_ENCODED) return Status::NotImplemented("function '" + name + "' has no kernel for run-end encoded arguments");
+  }
   return fn->Execute(ctx, opts, args, out);
 }
 
@@ -1538,6 +1575,18 @@ FunctionRegistry* GetFunctionRegistry() {
       if (args.size() != 1) return Status::Invalid("dictionary_encode takes one argument");
       return DictionaryEncode(ctx, o ? *o : DictionaryEncodeOptions(), args[0], out);
     }), false);
+    // vector_run_ends.go:46-61: chunkwise, so runs never cross a chunk boundary
+    reg->AddFunction(std::make_shared<MetaFunction>("run_end_encode", 1, [](const ExecCtx& ctx, const FunctionOptions* fo, const std::vector<Datum>& args, Datum* out) -> Status {
+      if (!fo) return Status::Invalid("function 'run_end_encode' cannot be called without options");   // functions.go:163-167
+      const auto* o = dynamic_cast<const RunEndEncodeOptions*>(fo);
+      if (!o) return Status::Invalid(std::string("run_end_encode: expected RunEndEncodeOptions, got ") + fo->TypeName());
+      if (args.size() != 1) return Status::Invalid("run_end_encode takes one argument");
+      return RunEndEncode(ctx, *o, args[0], out);
+    }), false);
+    reg->AddFunction(std::make_shared<MetaFunction>("run_end_decode", 1, [](const ExecCtx& ctx, const FunctionOptions*, const std::vector<Datum>& args, Datum* out) -> Status {
+      if (args.size() != 1) return Status::Invalid("run_end_decode takes one argument");
+      return RunEndDecode(ctx, args[0], out);
+    }), false);
     reg->AddFunction(std::make_shared<MetaFunction>("is_in", 1, [](const ExecCtx& ctx, const FunctionOptions* fo, const std::vector<Datum>& args, Datum* out) -> Status {
       const auto* so = dynamic_cast<const SetLookupOptions*>(fo);
       if (!so) return Status::Invalid("is_in requires SetLookupOptions");
@@ -1791,6 +1840,132 @@ Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& value
   int64_t nulls = 0;
   RETURN_NOT_OK(cnt->ToHost(&nulls, 8));
   return MakeOut(Type::BOOL, a->length, data, nulls ? valid : nullptr, nulls, out);
+}
+
+// ---- run_end_encode / run_end_decode ------------------------------------------------------------------------------
+namespace {
+// The arrays a chunkwise vector kernel runs on: the executor's spans of one argument (iterateExecSpans), so a chunked
+// input loses its empty chunks and a chunked input without rows gives one empty span (nullptr when it has no chunks).
+Status ChunkwiseSpans(const Datum& values, std::vector<std::shared_ptr<ArrayData>>* spans) {
+  if (values.kind == DatumKind::ARRAY) { spans->push_back(values.array); return Status::OK(); }
+  std::vector<std::vector<int64_t>> lens(1);
+  for (auto& c : values.chunked->chunks) lens[0].push_back(c->length);
+  std::vector<SpanPiece> pieces;
+  RETURN_NOT_OK(IterateExecSpans(lens, {true}, INT64_MAX, &pieces));
+  for (auto& p : pieces) spans->push_back(values.chunked->chunks[p.chunk_index[0]]->Slice(p.chunk_pos[0], p.len));
+  if (pieces.empty()) spans->push_back(values.chunked->chunks.empty() ? nullptr : values.chunked->chunks[0]->Slice(0, 0));
+  return Status::OK();
+}
+int64_t RunEndMax(Type t) { return t == Type::INT16 ? INT16_MAX : (t == Type::INT32 ? INT32_MAX : INT64_MAX); }
+const void* ElementPtr(const ArrayData& a) { return a.buffers[1] ? a.buffers[1]->data() + a.offset * (BitWidth(a.type) / 8) : nullptr; }
+int64_t BitmapWordBytes(int64_t nbits) { return ((nbits + 31) / 32) * 4; }
+
+// CountNumberOfRuns, one 16-byte read-back, exact allocation, WriteEncodedRuns (vector_run_end_encode.go:531-565)
+Status EncodeOne(Type rt, const ArrayData& a, std::shared_ptr<ArrayData>* out) {
+  const Type t = a.type;
+  const bool has_valid = a.buffers[0] != nullptr;
+  const uint8_t* valid = has_valid ? a.buffers[0]->data() : nullptr;
+  const void* vals = a.buffers[1] ? a.buffers[1]->data() : nullptr;   // row 0 at a.offset, a bit offset for BOOL
+  std::shared_ptr<Buffer> counts;
+  RETURN_NOT_OK(Buffer::Allocate(16, &counts));
+  NATIVE(ag_run_end_count_dev((int)t, vals, valid, a.offset, a.length, (int64_t*)counts->data(), nullptr));
+  int64_t cnt[2] = {0, 0};
+  RETURN_NOT_OK(counts->ToHost(cnt, 16));
+  const int64_t runs = cnt[0];
+  auto re = std::make_shared<ArrayData>();
+  re->type = rt; re->length = runs;
+  RETURN_NOT_OK(Buffer::Allocate(runs * (BitWidth(rt) / 8), &re->buffers[1]));
+  auto v = std::make_shared<ArrayData>();
+  v->type = t; v->length = runs; v->null_count = has_valid ? cnt[1] : 0;
+  RETURN_NOT_OK(Buffer::Allocate(t == Type::BOOL ? BitmapWordBytes(runs) : runs * (BitWidth(t) / 8), &v->buffers[1]));
+  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(runs), &v->buffers[0]));
+  NATIVE(ag_run_end_encode_dev((int)t, (int)rt, vals, valid, a.offset, a.length, re->buffers[1]->data(), v->buffers[1]->data(),
+                               has_valid ? v->buffers[0]->data() : nullptr, runs, (int64_t*)counts->data(), nullptr));
+  NATIVE(ag_stream_sync(nullptr));
+  auto d = std::make_shared<ArrayData>();
+  d->type = Type::RUN_END_ENCODED; d->length = a.length; d->null_count = 0;
+  d->run_ends = re;
+  d->values = v;
+  *out = d;
+  return Status::OK();
+}
+
+Status DecodeOne(const ArrayData& a, std::shared_ptr<ArrayData>* out) {
+  const ArrayData &re = *a.run_ends, &v = *a.values;
+  if (v.length < re.length) return Status::Invalid("run_end_decode: the values child is shorter than run_ends");
+  const Type t = v.type;
+  const bool has_valid = v.buffers[0] != nullptr;
+  auto d = std::make_shared<ArrayData>();
+  d->type = t; d->length = a.length;
+  RETURN_NOT_OK(Buffer::Allocate(t == Type::BOOL ? BitmapWordBytes(a.length) : a.length * (BitWidth(t) / 8), &d->buffers[1]));
+  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(a.length), &d->buffers[0]));
+  std::shared_ptr<Buffer> words;   // [0] null count, [1] error word
+  RETURN_NOT_OK(Buffer::Allocate(16, &words));
+  int64_t* w = (int64_t*)words->data();
+  NATIVE(ag_error_word_reset_dev(w + 1, nullptr));
+  NATIVE(ag_run_end_decode_dev((int)t, (int)re.type, ElementPtr(re), re.length, v.buffers[1] ? v.buffers[1]->data() : nullptr,
+                               has_valid ? v.buffers[0]->data() : nullptr, v.offset, a.offset, a.length, d->buffers[1]->data(),
+                               has_valid ? d->buffers[0]->data() : nullptr, w, w + 1, nullptr));
+  int64_t h[2];
+  RETURN_NOT_OK(words->ToHost(h, 16));
+  if (h[1] != AG_NO_ERROR_POS)
+    return Status::Invalid("run_end_decode: malformed run ends at run " + std::to_string(h[1]) + " (they must increase strictly and reach offset+length)");
+  d->null_count = has_valid ? h[0] : 0;
+  if (!has_valid) d->buffers[0] = nullptr;
+  *out = d;
+  return Status::OK();
+}
+
+bool RunEndValueType(Type t) { return t == Type::BOOL || IsNumeric(t); }
+}  // namespace
+
+Status RunEndEncode(const ExecCtx& ctx, const RunEndEncodeOptions& opts, const Datum& values, Datum* out) {
+  const Type rt = opts.RunEndType;
+  if (rt != Type::INT16 && rt != Type::INT32 && rt != Type::INT64) return Status::Invalid(std::string("bad run end type ") + TypeName(rt));
+  if (values.kind != DatumKind::ARRAY && values.kind != DatumKind::CHUNKED) return Status::NotImplemented("run_end_encode takes an array-like argument");
+  const Type t = values.type();
+  if (!RunEndValueType(t)) return Status::NotImplemented(std::string("run_end_encode: unsupported type ") + TypeName(t));
+  std::vector<std::shared_ptr<ArrayData>> spans;
+  RETURN_NOT_OK(ChunkwiseSpans(values, &spans));
+  std::vector<std::shared_ptr<ArrayData>> res;
+  for (auto a : spans) {
+    if (!a) { a = std::make_shared<ArrayData>(); a->type = t; }   // a chunked input without chunks
+    if (a->length > RunEndMax(rt))   // validateRunEndType (vector_run_end_encode.go:437-444)
+      return Status::Invalid("cannot run-end encode arrays with more elements than the run end type can hold: " + std::to_string(RunEndMax(rt)));
+    std::shared_ptr<ArrayData> r;
+    RETURN_NOT_OK(EncodeOne(rt, *a, &r));
+    res.push_back(r);
+  }
+  if (values.kind == DatumKind::ARRAY) { *out = Datum(res[0]); return Status::OK(); }
+  auto c = std::make_shared<ChunkedArray>();
+  c->type = Type::RUN_END_ENCODED; c->value_type = t; c->run_end_type = rt; c->chunks = res;
+  for (auto& r : res) c->length += r->length;
+  *out = Datum(c);
+  return Status::OK();
+}
+
+Status RunEndDecode(const ExecCtx& ctx, const Datum& values, Datum* out) {
+  if (values.kind != DatumKind::ARRAY && values.kind != DatumKind::CHUNKED) return Status::NotImplemented("run_end_decode takes an array-like argument");
+  if (values.type() != Type::RUN_END_ENCODED)
+    return Status::NotImplemented(std::string("function 'run_end_decode' has no kernel matching input types (") + TypeName(values.type()) + ")");
+  std::vector<std::shared_ptr<ArrayData>> spans;
+  RETURN_NOT_OK(ChunkwiseSpans(values, &spans));
+  std::vector<std::shared_ptr<ArrayData>> res;
+  for (auto& a : spans) {
+    std::shared_ptr<ArrayData> r;
+    if (!a) {   // a chunked input without chunks
+      RETURN_NOT_OK(ArrayData::FromHost(values.chunked->value_type, 0, 0, nullptr, nullptr, 0, &r));
+    } else {
+      RETURN_NOT_OK(DecodeOne(*a, &r));
+    }
+    res.push_back(r);
+  }
+  if (values.kind == DatumKind::ARRAY) { *out = Datum(res[0]); return Status::OK(); }
+  auto c = std::make_shared<ChunkedArray>();
+  c->type = values.chunked->value_type; c->chunks = res;
+  for (auto& r : res) c->length += r->length;
+  *out = Datum(c);
+  return Status::OK();
 }
 
 Status Filter(const ExecCtx& ctx, const Datum& values, const Datum& filter, const FilterOptions& opts, Datum* out) {

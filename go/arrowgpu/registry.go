@@ -214,6 +214,7 @@ func NewRegistry() compute.FunctionRegistry {
 	addVector(reg, parent, filterFn)
 	addVector(reg, parent, takeFn)
 	registerLookupSort(reg, parent) // is_in, unique, sort_indices (lookup_sort.go)
+	registerRunEnds(reg, parent)    // run_end_encode, run_end_decode (run_ends.go)
 	return reg
 }
 

@@ -569,6 +569,46 @@ ag_status ag_dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, i
                                    void* d_dict, uint8_t* d_dict_valid, int64_t* d_counts, ag_stream_t s);
 
 /* ================================================================================= *
+ * run_end_encode / run_end_decode for BOOL and the 10 numeric types — the fixed-width and boolean loops of
+ *   kernels/vector_run_end_encode.go: CountNumberOfRuns (:114-141) + WriteEncodedRuns (:86-112), and
+ *   decodeBool / decodeFixedWidth ExpandAllRuns (:591-719).  Run-end types: AG_TYPE_INT16 / INT32 / INT64; any other
+ *   run_end_type is AG_ERR_INVALID "bad run end type" (:567-578).
+ * Encode of rows [offset, offset+n) of `vals` (BOOL: an LSB-first bitmap) with optional `valid` (same offset):
+ *   rows i-1 and i share a run iff their validity bits are equal AND their values compare equal with the type's ==,
+ *   the payload under a null included (:96-105): float NaN rows each start a run, +0.0 and -0.0 share one.
+ *   Run r: run_ends[r] = the first row of run r+1 (n for the last run), out[r] = the value (BOOL: bit r) of its first
+ *   row, out_valid bit r = that row's validity.  out_valid is written only when `valid` is given (then required).
+ *   counts (2 int64): [0] runs, [1] null runs — the true totals even when they exceed `capacity`; runs past
+ *   `capacity` are not written.  n > the run-end type's maximum: AG_ERR_INVALID "cannot run-end encode arrays with
+ *   more elements than the run end type can hold: <max>" (validateRunEndType :437-444); n == 0: no runs, no error.
+ *   Device flavour: out_valid (and a BOOL out) are 4-byte aligned bitmaps of ceil(capacity/32) words, bit 0 = run 0.
+ * Decode of the logical slice [offset, offset+length) of a run-end encoded array (run_ends: n_runs entries; the values
+ *   child `vals` / `valid` at element offset values_offset, at least values_offset + n_runs elements):
+ *   out row j = the value and validity of the run p with run_ends[p-1] <= offset+j < run_ends[p]; the last run is
+ *   clipped at offset+length.  out is written at offset 0 (BOOL and out_valid: ceil(length/32) 4-byte aligned words,
+ *   bits past length cleared); out_valid is written only when `valid` is given (then required).
+ *   Malformed run ends — not strictly increasing over the runs that cover the slice, or a last run end below
+ *   offset+length — are AG_ERR_INVALID (host flavour) / lower *d_error_word (device flavour; reset it with
+ *   ag_error_word_reset_dev, it is only lowered, to the index of a malformed run end or to n_runs).  Whatever the
+ *   input, no read leaves run_ends[0..n_runs) and the values child, and no write leaves the words of [0, length).
+ *   The reference does neither: it walks every run to the end of run_ends (:673).
+ * Host flavours: every pointer is a host pointer; *null_count (may be NULL) receives the output's null count.
+ * ================================================================================= */
+#define AG_TYPE_RUN_END_ENCODED    38 /* arrow.RUN_END_ENCODED (arrow/datatype.go) */
+ag_status ag_run_end_count(int type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, int64_t* counts);
+ag_status ag_run_end_count_dev(int type, const void* d_vals, const uint8_t* d_valid, int64_t offset, int64_t n, int64_t* d_counts,
+                               ag_stream_t s);
+ag_status ag_run_end_encode(int type, int run_end_type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n,
+                            void* run_ends, void* out, uint8_t* out_valid, int64_t capacity, int64_t* counts);
+ag_status ag_run_end_encode_dev(int type, int run_end_type, const void* d_vals, const uint8_t* d_valid, int64_t offset, int64_t n,
+                                void* d_run_ends, void* d_out, uint8_t* d_out_valid, int64_t capacity, int64_t* d_counts, ag_stream_t s);
+ag_status ag_run_end_decode(int type, int run_end_type, const void* run_ends, int64_t n_runs, const void* vals, const uint8_t* valid,
+                            int64_t values_offset, int64_t offset, int64_t length, void* out, uint8_t* out_valid, int64_t* null_count);
+ag_status ag_run_end_decode_dev(int type, int run_end_type, const void* d_run_ends, int64_t n_runs, const void* d_vals,
+                                const uint8_t* d_valid, int64_t values_offset, int64_t offset, int64_t length, void* d_out,
+                                uint8_t* d_out_valid, int64_t* d_null_count, int64_t* d_error_word, ag_stream_t s);
+
+/* ================================================================================= *
  * sort_indices, one fixed-width column (SURVEY 8f rank 3) — replaces kernels.SortIndices for a single
  *   key (vector_sort.go:385-481, vector_sort_internal.go:36-150,250-300): a STABLE permutation of
  *   0..n-1 as uint64 row indices,

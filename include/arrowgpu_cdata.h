@@ -158,6 +158,26 @@ ag_status ag_export_dictionary_device_array(int value_type, int64_t length, int6
 ag_status ag_import_dictionary_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on,
                                             ag_array_view* indices, ag_array_view* dictionary);
 
+/* A run-end encoded array (the layout pyarrow and arrow/cdata export for arrow.RUN_END_ENCODED): the parent has format
+ * "+r", no buffers, null_count 0 and carries the logical offset and length; its two children are "run_ends" (format
+ * "s" / "i" / "l", non-nullable) and "values" (a primitive array).  All three live on one device.
+ *   Describe: fills the parent's view (type AG_TYPE_RUN_END_ENCODED, length, offset; no buffers) and the views of the
+ *   two children; ag_device_array_describe itself keeps refusing run-end encoded arrays.
+ *   Export: the parent's release runs `release_buffers(opaque)` (which must cover the run-end AND the values buffers)
+ *   and then releases each child a consumer has not moved out; the schema's release frees the child schemas.  The
+ *   children share the device of the parent.  ag_export_device_array keeps refusing AG_TYPE_RUN_END_ENCODED.
+ *   Import: describe plus the device checks and the wait of ag_import_device_array.  Ownership stays with `in`. */
+ag_status ag_run_end_encoded_device_array_describe(const struct ArrowDeviceArray* in, const struct ArrowSchema* schema,
+                                                   ag_array_view* parent, ag_array_view* run_ends, ag_array_view* values);
+ag_status ag_export_run_end_encoded_device_array(int value_type, int run_end_type, int64_t length, int64_t offset,
+                                                 int64_t n_runs, const void* d_run_ends,
+                                                 int64_t values_length, int64_t values_null_count, int64_t values_offset,
+                                                 const void* d_values_validity, const void* d_values,
+                                                 void (*release_buffers)(void* opaque), void* opaque, ag_stream_t produced_on,
+                                                 struct ArrowDeviceArray* out, struct ArrowSchema* out_schema);
+ag_status ag_import_run_end_encoded_device_array(struct ArrowDeviceArray* in, const struct ArrowSchema* schema, ag_stream_t consume_on,
+                                                 ag_array_view* parent, ag_array_view* run_ends, ag_array_view* values);
+
 #ifdef __cplusplus
 }
 #endif

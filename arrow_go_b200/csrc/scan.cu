@@ -12,10 +12,11 @@
 // updates, so a chunked column is a chain of launches on one stream with no host round trip.
 //
 // Roofline: HBM, 2 x sizeof(T) algorithmic bytes per row (read once, write once).
-// Algorithm: single-pass scan with decoupled look-back over 32 KB tiles.
-//   * a block = 8 warps; warp w of a tile owns a contiguous 4 KB segment and reads it as 8 rows of
-//     32 16-byte vectors (fully coalesced); the prefix inside a segment is 8 warp scans over the
-//     vector totals, carried row to row — no shared-memory transpose, no strided access;
+// Algorithm: single-pass scan with decoupled look-back over 32 KB tiles, one kernel for every call
+// (cumsum_stream_kernel below: checked or not, with or without a validity bitmap, any element-aligned operands).
+//   * warp w of a tile owns a contiguous 4 KB segment, loaded coalesced and transposed through
+//     swizzled shared memory so that each lane owns 128 contiguous bytes: one local scan and ONE warp
+//     scan per tile;
 //   * tile status, three levels: every tile publishes its AGGREGATE; the last tile of a group of 128
 //     publishes the GROUP aggregate (it needs only its own group's tile aggregates, so it never waits
 //     on earlier groups); the last tile of a super-group of 32 groups publishes the INCLUSIVE prefix.
@@ -28,9 +29,9 @@
 //     flag/value pair to guard against (a 64-bit accumulator is split over 32-bit payloads);
 //   * static tile order + cooperative launch (one resident wave): a tile only ever waits on lower
 //     tiles, which resident blocks reach in increasing order.
-// Integers accumulate in an exact 96-bit value (64-bit wrap + carry count): the wrapped low word is
-// the unchecked result, and the checked flavour compares the exact running sum with the type's
-// range per element.  Floats accumulate in their own type; results are bit-exact with the
+// Unchecked integers accumulate modulo 2^64, which is all the wrapped result needs; the checked flavour
+// accumulates an exact 96-bit value (64-bit wrap + carry count) and compares the running sum with the
+// type's range per element.  Floats accumulate in their own type; results are bit-exact with the
 // reference's left-to-right loop whenever every partial sum is exactly representable, and differ by
 // rounding of the same order as the reference's own otherwise (DESIGN.md).
 #include "common.cuh"
@@ -184,7 +185,6 @@ struct Pol<T, true> {  // float / double: accumulate in the value type
   }
 };
 
-__device__ __forceinline__ unsigned long long ld_word(const unsigned long long* p) { return *reinterpret_cast<const volatile unsigned long long*>(p); }
 __device__ __forceinline__ void st_word(unsigned long long* p, unsigned v) { *reinterpret_cast<volatile unsigned long long*>(p) = kScFlag | v; }
 
 struct CumsumParams {
@@ -194,353 +194,23 @@ struct CumsumParams {
   int64_t voff;
   int64_t n;
   int skip_nulls;
-  int checked;
   const long long* first_null;   // device: first null row of this call (n when none); NULL when valid == NULL
   CumsumState* state;
   long long* first_bad;          // may be NULL when !checked
   uint8_t* out_valid;            // may be NULL (then there are no nulls anywhere in the sequence)
   int64_t ooff;
-  unsigned long long* agg;       // [n_tiles][K]
-  unsigned long long* gagg;      // [n_groups][K]   aggregate of a whole group
-  unsigned long long* sincl;     // [n_super][K]    inclusive prefix at the end of a super-group
+  unsigned long long* agg;       // [n_tiles][S]    S = StatusEntry<K>::kStride words per entry
+  unsigned long long* gagg;      // [n_groups][S]   aggregate of a whole group
+  unsigned long long* sincl;     // [n_super][S]    inclusive prefix at the end of a super-group
   int64_t n_tiles;
 };
 
-// Wait for K flagged words and return the value they carry.
-template <typename P>
-__device__ __forceinline__ typename P::A poll_value(const unsigned long long* words) {
-  unsigned w[3] = {0u, 0u, 0u};
-#pragma unroll
-  for (int k = 0; k < P::K; ++k) {
-    unsigned long long s;
-    do { s = ld_word(words + k); } while (!(s & kScFlag));
-    w[k] = (unsigned)s;
-  }
-  return P::from_words(w);
-}
-
-// The look-back of one tile, executed by a whole warp.  Returns the tile's exclusive prefix (all lanes)
-// after publishing whatever this tile owes the others (its group aggregate, the super-group prefix).
-template <typename P>
-__device__ __forceinline__ typename P::A scan_lookback(const CumsumParams& p, int64_t tile, typename P::A tile_total,
-                                                       typename P::A start, int lane) {
-  using A = typename P::A;
-    const int64_t g = tile / kScGroup;
-    const int qpos = (int)(tile - g * kScGroup);
-    // Everything this tile needs from earlier tiles, fetched as ONE batch of independent polls
-    // (re-issued only for words whose flag is not up yet): slots 0..3 = aggregates of the earlier
-    // tiles of this group (four per lane), slot 4 = aggregates of the earlier groups of this
-    // super-group (one per lane), slot 5 = the previous super-group's inclusive prefix.
-    const int64_t sg = g / kScSuper;
-    const int gq = (int)(g - sg * kScSuper);
-    constexpr int kSlots = kScGroup / 32 + 2;
-    const unsigned long long* src[kSlots];
-    unsigned need = 0;
-#pragma unroll
-    for (int r = 0; r < kScGroup / 32; ++r) {
-      const int pos = r * 32 + lane;
-      src[r] = p.agg + (g * kScGroup + pos) * P::K;
-      if (pos < qpos) need |= ((1u << P::K) - 1u) << (r * P::K);
-    }
-    src[kSlots - 2] = p.gagg + (sg * kScSuper + lane) * P::K;
-    if (lane < gq) need |= ((1u << P::K) - 1u) << ((kSlots - 2) * P::K);
-    src[kSlots - 1] = p.sincl + (sg > 0 ? sg - 1 : 0) * P::K;
-    if (sg > 0) need |= ((1u << P::K) - 1u) << ((kSlots - 1) * P::K);
-    unsigned val[kSlots][3];
-#pragma unroll
-    for (int r = 0; r < kSlots; ++r) { val[r][0] = 0u; val[r][1] = 0u; val[r][2] = 0u; }
-    unsigned got = 0;
-    constexpr unsigned kAggMask = (1u << ((kScGroup / 32) * P::K)) - 1u;
-    bool folded = false;
-    A part = P::zero();
-    while (true) {  // warp-uniform loop: the fold below uses shuffles
-      unsigned long long sw[kSlots][3];
-#pragma unroll
-      for (int r = 0; r < kSlots; ++r)
-#pragma unroll
-        for (int k = 0; k < P::K; ++k)
-          sw[r][k] = (((need & ~got) >> (r * P::K + k)) & 1u) ? ld_word(src[r] + k) : 0ull;
-#pragma unroll
-      for (int r = 0; r < kSlots; ++r)
-#pragma unroll
-        for (int k = 0; k < P::K; ++k)
-          if (sw[r][k] & kScFlag) { val[r][k] = (unsigned)sw[r][k]; got |= 1u << (r * P::K + k); }
-      if (!folded && __all_sync(0xffffffffu, ((got ^ need) & kAggMask) == 0u)) {
-        // tile aggregates are in: fold them in a fixed order (lower tiles on the left) and, for the
-        // last tile of a group, publish the group aggregate WITHOUT waiting for anything older
-        folded = true;
-#pragma unroll
-        for (int r = 0; r < kScGroup / 32; ++r) {
-          A a = (r * 32 + lane < qpos) ? P::from_words(val[r]) : P::zero();
-#pragma unroll
-          for (int d = 1; d < 32; d <<= 1) {
-            const A up = P::shfl_up(a, d);
-            if (lane >= d) a = P::add(up, a);
-          }
-          part = P::add(part, P::shfl(a, 31));
-        }
-        if (qpos == kScGroup - 1 && lane == 0) {
-          unsigned wg[3] = {0u, 0u, 0u};
-          P::to_words(P::add(part, tile_total), wg);
-#pragma unroll
-          for (int k = 0; k < P::K; ++k) st_word(p.gagg + g * P::K + k, wg[k]);
-        }
-      }
-      if (__all_sync(0xffffffffu, got == need)) break;
-    }
-    A gpart = (lane < gq) ? P::from_words(val[kSlots - 2]) : P::zero();
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const A up = P::shfl_up(gpart, d);
-      if (lane >= d) gpart = P::add(up, gpart);
-    }
-    gpart = P::shfl(gpart, 31);
-    const A base = (sg > 0) ? P::from_words(val[kSlots - 1]) : start;
-    const A excl = P::add(P::add(base, gpart), part);
-    if (lane == 0 && qpos == kScGroup - 1 && gq == kScSuper - 1) {
-      unsigned wi[3] = {0u, 0u, 0u};
-      P::to_words(P::add(excl, tile_total), wi);
-#pragma unroll
-      for (int k = 0; k < P::K; ++k) st_word(p.sincl + sg * P::K + k, wi[k]);
-    }
-    return excl;
-}
-
-template <typename T, bool kVec, bool kHasValid, bool kChecked>
-__global__ void __launch_bounds__(kScThreads, 2)
-cumsum_kernel(const CumsumParams p) {
-  using P = typename PolSel<T, kChecked>::type;
-  using A = typename P::A;
-  constexpr int N = 16 / sizeof(T);            // elements per 16-byte vector
-  constexpr int kTileRows = kScTileBytes / sizeof(T);
-  constexpr int kSegRows = kTileRows / kScWarps;  // rows of one warp segment
-  constexpr int E = kScRows * N;                  // rows owned by one lane (128 contiguous bytes)
-  __shared__ uint4 s_tile[kScThreads * kScRows];  // 32 KB: the tile, transposed warp by warp
-  __shared__ unsigned long long s_warp_lo[kScWarps];
-  __shared__ int s_warp_hi[kScWarps];
-  __shared__ unsigned long long s_excl_lo;
-  __shared__ int s_excl_hi;
-  __shared__ CumsumState s_state;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const T* __restrict__ in = reinterpret_cast<const T*>(p.in);
-  T* __restrict__ out = reinterpret_cast<T*>(p.out);
-
-  // every block reads the carried state BEFORE it publishes anything; the last tile rewrites the state
-  // only after all earlier tiles have published, i.e. after every block has passed this point
-  if (threadIdx.x == 0) s_state = *p.state;
-  __syncthreads();
-  const bool dead = !p.skip_nulls && s_state.encountered_null != 0;  // a previous chunk hit a null
-  int64_t limit = p.n;                                               // rows >= limit are null
-  if (dead) limit = 0;
-  else if (kHasValid && !p.skip_nulls) limit = *p.first_null;
-  const A start = P::from_state(s_state);
-  long long my_bad = AG_NO_ERROR_POS;
-  const int64_t vlo = p.voff >> 3, vhi = (p.voff + p.n + 7) >> 3;   // byte range of the validity bitmap
-
-  // Coalesced tile load: row k of a warp's 4 KB segment is 32 consecutive 16-byte vectors.  The
-  // loads of tile t+G are issued while tile t is still waiting on its look-back and being written
-  // out, so HBM stays busy across the only serial part of the algorithm.
-  uint4 q[kScRows];
-  auto load_tile = [&](int64_t tile) {
-    const int64_t r0 = tile * kTileRows + (int64_t)warp * kSegRows;
-#pragma unroll
-    for (int k = 0; k < kScRows; ++k) {
-      const int64_t e0 = r0 + ((int64_t)k * 32 + lane) * N;
-      if (kVec && e0 + N <= p.n) {
-        q[k] = __ldcs(reinterpret_cast<const uint4*>(in + e0));
-      } else {
-        __align__(16) T tmp[N];
-#pragma unroll
-        for (int j = 0; j < N; ++j) tmp[j] = (e0 + j < p.n) ? in[e0 + j] : T(0);
-        q[k] = *reinterpret_cast<const uint4*>(tmp);
-      }
-    }
-  };
-  if ((int64_t)blockIdx.x < p.n_tiles) load_tile(blockIdx.x);
-
-  for (int64_t tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-    const int64_t row0 = tile * kTileRows + (int64_t)warp * kSegRows;  // first row of this warp's segment
-    // ---- load (coalesced): row k of the warp's 4 KB segment is 32 consecutive 16-byte vectors -----
-    // and transpose through shared memory so that lane l OWNS the 128 contiguous bytes l of the
-    // segment.  Vector vi = k*32 + lane belongs to owner vi>>3, chunk vi&7; it is parked at
-    // chunk ^ (owner & 7) of the owner's 128-byte row: both the striped writes and the blocked reads
-    // touch every bank once per quarter warp.
-    uint4* seg = s_tile + warp * (kScRows * 32);
-#pragma unroll
-    for (int k = 0; k < kScRows; ++k) {  // q[] was loaded one tile ahead (see the prefetch below)
-      const int vi = k * 32 + lane;
-      const int owner = vi >> 3, c = vi & 7;
-      seg[owner * 8 + (c ^ (owner & 7))] = q[k];
-    }
-    __syncwarp();
-    uint4 raw[kScRows];  // this lane's E = 8*N consecutive elements, still packed
-#pragma unroll
-    for (int c = 0; c < kScRows; ++c) raw[c] = seg[lane * 8 + (c ^ (lane & 7))];
-    const int64_t t0 = row0 + (int64_t)lane * E;  // first row owned by this lane
-    // validity of the E rows, 32 at a time; rows at or past `limit` (and past n) contribute nothing
-    unsigned vbits[(E + 31) / 32];
-#pragma unroll
-    for (int w = 0; w < (E + 31) / 32; ++w) {
-      const int64_t e0 = t0 + w * 32;
-      unsigned m = 0xffffffffu;
-      if (kHasValid) m = (e0 < p.n) ? bitmap_load32(p.valid, p.voff + e0, vlo, vhi) : 0u;
-      const int64_t room = limit - e0;
-      if (room < 32) m &= (room <= 0) ? 0u : ((1u << (int)room) - 1u);
-      if (E < 32) m &= (1u << (E & 31)) - 1u;
-      vbits[w] = m;
-    }
-    // ---- lane total, ONE warp scan, segment total ---------------------------------------------
-    // all E rows valid (the common case): no per-element bit tests — the kernel is issue-bound, not
-    // byte-bound (ncu: 7800 warp instructions per 32 KB tile at IPC 1.6)
-    bool dense = true;
-#pragma unroll
-    for (int w = 0; w < (E + 31) / 32; ++w) dense = dense && vbits[w] == ((E >= 32) ? 0xffffffffu : ((1u << (E & 31)) - 1u));
-    A tot = P::zero();
-    if (dense) {
-#pragma unroll
-      for (int i = 0; i < E; ++i) tot = P::add_elem(tot, reinterpret_cast<const T*>(raw)[i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < E; ++i)
-        if ((vbits[i >> 5] >> (i & 31)) & 1u) tot = P::add_elem(tot, reinterpret_cast<const T*>(raw)[i]);
-    }
-    A incl = tot;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const A up = P::shfl_up(incl, d);
-      if (lane >= d) incl = P::add(up, incl);
-    }
-    A lane_excl = P::shfl_up(incl, 1);
-    if (lane == 0) lane_excl = P::zero();
-    const A carry = P::shfl(incl, 31);
-    // ---- block: exclusive offsets of the 8 warp segments, tile total ----------------------------
-    {
-      unsigned w[3] = {0u, 0u, 0u};
-      P::to_words(carry, w);
-      if (lane == 0) { s_warp_lo[warp] = (unsigned long long)w[0] | ((unsigned long long)w[1] << 32); s_warp_hi[warp] = (int)w[2]; }
-    }
-    __syncthreads();
-    A warp_excl = P::zero(), tile_total = P::zero();
-#pragma unroll
-    for (int wi = 0; wi < kScWarps; ++wi) {
-      const unsigned w[3] = {(unsigned)s_warp_lo[wi], (unsigned)(s_warp_lo[wi] >> 32), (unsigned)s_warp_hi[wi]};
-      const A t = P::from_words(w);
-      if (wi == warp) warp_excl = tile_total;
-      tile_total = P::add(tile_total, t);
-    }
-    // ---- look-back (warp 0): publish the aggregate, gather the exclusive prefix of the tile -----
-    if (warp == 0 && lane == 0) {
-      unsigned w[3] = {0u, 0u, 0u};
-      P::to_words(tile_total, w);
-#pragma unroll
-      for (int k = 0; k < P::K; ++k) st_word(p.agg + tile * P::K + k, w[k]);
-    }
-    if (tile + gridDim.x < p.n_tiles) load_tile(tile + gridDim.x);  // prefetch: in flight during the wait below
-    // Unchecked flavours: the running sums RELATIVE to the tile start need nothing from other tiles, so
-    // warps 1..7 compute them while warp 0 is in the look-back; after the barrier only the tile's
-    // exclusive prefix is added.  (Checked integers keep the exact 96-bit pass after the barrier.)
-    auto local_pass = [&]() {
-      A run = P::add(warp_excl, lane_excl);
-      T* o = reinterpret_cast<T*>(raw);  // results replace the inputs in place
-      if (dense) {
-#pragma unroll
-        for (int i = 0; i < E; ++i) { run = P::add_elem(run, o[i]); o[i] = P::value(run); }
-      } else {
-#pragma unroll
-        for (int i = 0; i < E; ++i) {
-          if ((vbits[i >> 5] >> (i & 31)) & 1u) { run = P::add_elem(run, o[i]); o[i] = P::value(run); }
-          else o[i] = T(0);
-        }
-      }
-    };
-    if (!kChecked && warp != 0) local_pass();
-    if (warp == 0) {
-      const A excl = scan_lookback<P>(p, tile, tile_total, start, lane);
-      if (lane == 0) {
-        unsigned w[3] = {0u, 0u, 0u};
-        P::to_words(excl, w);
-        s_excl_lo = (unsigned long long)w[0] | ((unsigned long long)w[1] << 32);
-        s_excl_hi = (int)w[2];
-        const A incl = P::add(excl, tile_total);
-        if (tile == p.n_tiles - 1) {  // carry to the next chunk (null_count was advanced by cumsum_validity_kernel)
-          CumsumState ns = s_state;
-          P::to_state(incl, &ns);
-          if (kHasValid && *p.first_null < p.n) ns.encountered_null = 1;
-          *p.state = ns;
-        }
-      }
-    }
-    __syncthreads();
-    A tile_excl;
-    {
-      const unsigned w[3] = {(unsigned)s_excl_lo, (unsigned)(s_excl_lo >> 32), (unsigned)s_excl_hi};
-      tile_excl = P::from_words(w);
-    }
-    // ---- running sums of the valid slots (0 in null slots), back through shared memory, store --
-    if constexpr (kChecked) {
-      A run = P::add(P::add(tile_excl, warp_excl), lane_excl);
-      T* o = reinterpret_cast<T*>(raw);
-#pragma unroll
-      for (int i = 0; i < E; ++i) {
-        if ((vbits[i >> 5] >> (i & 31)) & 1u) {
-          run = P::add_elem(run, o[i]);
-          o[i] = P::value(run);
-          if (P::out_of_range(run) && t0 + i < my_bad) my_bad = t0 + i;
-        } else {
-          o[i] = T(0);
-        }
-      }
-    } else {
-      if (warp == 0) local_pass();
-      const T off = P::value(tile_excl);  // integers: the sum modulo 2^w; floats: the prefix itself
-      T* o = reinterpret_cast<T*>(raw);
-      if (dense) {
-#pragma unroll
-        for (int i = 0; i < E; ++i) o[i] = P::offset_add(off, o[i]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < E; ++i)
-          if ((vbits[i >> 5] >> (i & 31)) & 1u) o[i] = P::offset_add(off, o[i]);
-      }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < kScRows; ++c) seg[lane * 8 + (c ^ (lane & 7))] = raw[c];
-    __syncwarp();
-#pragma unroll
-    for (int k = 0; k < kScRows; ++k) {
-      const int vi = k * 32 + lane;
-      const int64_t e0 = row0 + (int64_t)vi * N;
-      if (e0 >= p.n) continue;
-      const int owner = vi >> 3, c = vi & 7;
-      const uint4 q = seg[owner * 8 + (c ^ (owner & 7))];
-      if (kVec && e0 + N <= p.n) {
-        __stcs(reinterpret_cast<uint4*>(out + e0), q);
-      } else {
-        const T* o = reinterpret_cast<const T*>(&q);
-#pragma unroll
-        for (int j = 0; j < N; ++j) if (e0 + j < p.n) out[e0 + j] = o[j];
-      }
-    }
-    __syncthreads();  // s_warp_* / s_excl_* are rewritten by the next tile
-  }
-  if (kChecked) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, d);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.first_bad, my_bad);
-  }
-}
-
-// ---- streaming flavour: no validity bitmap, unchecked, 16-byte aligned operands ------------------
-// Profiled on the block-synchronous shape (general kernel above, and a first streaming kernel with the same
-// schedule): most warp samples sit at the barrier behind the
-// look-back and warp 0 spends 92 % of its time inside it (half waiting for flags of tiles that other
-// blocks are reducing at the same moment, half in ~600 dependent instructions of one warp) — every
-// resident block is in the same phase, so nothing on the SM covers that wait, which took longer than the
-// tile's HBM time.  This kernel takes the look-back off the critical path:
+// ---- the scan kernel ------------------------------------------------------------------------------
+// Profiled on a block-synchronous shape (one warp of each block doing the look-back between two block barriers):
+// most warp samples sit at the barrier behind the look-back and that warp spends 92 % of its time inside it (half
+// waiting for flags of tiles that other blocks are reducing at the same moment, half in ~600 dependent instructions
+// of one warp) — every resident block is in the same phase, so nothing on the SM covers that wait, which took longer
+// than the tile's HBM time.  This kernel takes the look-back off the critical path:
 //   * a block = 8 compute warps + 1 LOOK-BACK warp.  In iteration j the compute warps reduce tile j
 //     and finalize tile j-1 while the look-back warp resolves the prefix of tile j-1 (whose aggregate,
 //     and those of its predecessors in other blocks, were published an iteration ago: the polls hit);
@@ -548,11 +218,11 @@ cumsum_kernel(const CumsumParams p) {
 //   * tiles arrive by cp.async (16 bytes per thread, no staging registers) straight into the SWIZZLED
 //     position of a 3-stage shared-memory ring (loading / being reduced / waiting for its prefix); a
 //     warp only ever touches its own 4 KB segment of a stage, so the ring needs __syncwarp only;
-//   * the look-back reads a whole 16-byte status entry per load, issues all its polls as one batch
+//   * the look-back reads a whole status entry per load, issues all its polls as one batch
 //     and folds them with interleaved warp scans: ~1 L2 round trip + ~150 instructions;
 //   * interior tiles run a branch-free body (base pointer + immediate offsets).
-// Same tiles, same status words, same fold order as cumsum_kernel: results are bit-identical to it
-// (floats included), so the two kernels can be mixed inside one chunked sequence.
+// Operands that are only element-aligned (Arrow slices, later chunks of a chunked output) take block-uniform side
+// paths in the load and store stages; the aligned path is unchanged by them.
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
@@ -564,13 +234,36 @@ template <int kB>
 __device__ __forceinline__ void cp_async_small_zfill(uint32_t dst, const void* src, int bytes) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], %2, %3;" ::"r"(dst), "l"(src), "n"(kB), "r"(bytes) : "memory");
 }
+// A 16-byte vector stored to an address aligned only to its lowest set bit `mis & -mis` (>= sizeof(T)), in the widest
+// pieces that alignment allows
+template <typename W>
+__device__ __forceinline__ void st_pieces_as(unsigned char* dst, const uint4& v) {
+  const W* s = reinterpret_cast<const W*>(&v);
+#pragma unroll
+  for (int q = 0; q < 16 / (int)sizeof(W); ++q) __stcs(reinterpret_cast<W*>(dst) + q, s[q]);
+}
+template <typename T>
+__device__ __forceinline__ void st_pieces(unsigned char* dst, const uint4& v, int mis) {
+  if (sizeof(T) >= 8 || (mis & 7) == 0) st_pieces_as<unsigned long long>(dst, v);
+  else if (sizeof(T) >= 4 || (mis & 3) == 0) st_pieces_as<unsigned>(dst, v);
+  else if (sizeof(T) >= 2 || (mis & 1) == 0) st_pieces_as<unsigned short>(dst, v);
+  else st_pieces_as<unsigned char>(dst, v);
+}
+// a shared-memory read the compiler must not reuse from before the atomic that announced it
+template <typename A> __device__ __forceinline__ A ld_shared_volatile(const A& a) { return *reinterpret_cast<const volatile A*>(&a); }
+__device__ __forceinline__ AccX ld_shared_volatile(const AccX& a) {
+  const volatile AccX& v = a;
+  return AccX{v.lo, v.hi};
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int kPending> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(kPending) : "memory"); }
 
-// One status entry = K flagged 64-bit words, fetched with ONE volatile load (K = 2: 128 bits; every word carries its own
-// flag, so it does not matter whether the two halves are observed at the same instant).
+// One status entry = K flagged 64-bit words, fetched with one volatile load per 16 bytes (every word carries its own
+// flag, so it does not matter whether the words are observed at the same instant).  kStride words apart, so that every
+// entry of a multi-word accumulator starts on a 16-byte boundary.
 template <int K> struct StatusEntry;
 template <> struct StatusEntry<1> {
+  static constexpr int kStride = 1;
   unsigned long long w0;
   __device__ __forceinline__ void load(const unsigned long long* p) { asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(w0) : "l"(p) : "memory"); }
   __device__ __forceinline__ bool ready() const { return (w0 & kScFlag) != 0; }
@@ -578,6 +271,7 @@ template <> struct StatusEntry<1> {
   __device__ __forceinline__ void set_ready_zero() { w0 = kScFlag; }
 };
 template <> struct StatusEntry<2> {
+  static constexpr int kStride = 2;
   unsigned long long w0, w1;
   __device__ __forceinline__ void load(const unsigned long long* p) {
     asm volatile("ld.volatile.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(p) : "memory");
@@ -586,23 +280,35 @@ template <> struct StatusEntry<2> {
   __device__ __forceinline__ void words(unsigned (&w)[3]) const { w[0] = (unsigned)w0; w[1] = (unsigned)w1; w[2] = 0u; }
   __device__ __forceinline__ void set_ready_zero() { w0 = kScFlag; w1 = kScFlag; }
 };
+template <> struct StatusEntry<3> {  // the exact 96-bit integer sum: 32 bytes, the fourth word is never written
+  static constexpr int kStride = 4;
+  unsigned long long w0, w1, w2, w3;
+  __device__ __forceinline__ void load(const unsigned long long* p) {
+    asm volatile("ld.volatile.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(p) : "memory");
+    asm volatile("ld.volatile.global.v2.u64 {%0, %1}, [%2];" : "=l"(w2), "=l"(w3) : "l"(p + 2) : "memory");
+  }
+  __device__ __forceinline__ bool ready() const { return ((w0 & w1 & w2) & kScFlag) != 0; }
+  __device__ __forceinline__ void words(unsigned (&w)[3]) const { w[0] = (unsigned)w0; w[1] = (unsigned)w1; w[2] = (unsigned)w2; }
+  __device__ __forceinline__ void set_ready_zero() { w0 = kScFlag; w1 = kScFlag; w2 = kScFlag; }
+};
 
-// scan_lookback with the same three levels, the same words and the same fold order, built for latency: whole entries per
-// load, every poll of a level in one batch, the four tile-aggregate scans interleaved.  Entries must be 16-byte aligned.
+// The look-back of one tile, executed by a whole warp.  Returns the tile's exclusive prefix (all lanes) after publishing
+// whatever this tile owes the others (its group aggregate, the super-group prefix).  Built for latency: whole entries
+// per load, every poll of a level in one batch, the four tile-aggregate scans interleaved.
 template <typename P>
-__device__ __forceinline__ typename P::A scan_lookback_lean(const CumsumParams& p, int64_t tile, typename P::A tile_total,
-                                                            typename P::A start, int lane) {
+__device__ __forceinline__ typename P::A cumsum_lookback(const CumsumParams& p, int64_t tile, typename P::A tile_total,
+                                                         typename P::A start, int lane) {
   using A = typename P::A;
   constexpr int K = P::K;
-  static_assert(K <= 2, "lean look-back: float / double / wrapped 64-bit accumulators");
+  constexpr int S = StatusEntry<K>::kStride;
   constexpr int R = kScGroup / 32;
   const int64_t g = tile / kScGroup;
   const int qpos = (int)(tile - g * kScGroup);
   const int64_t sg = g / kScSuper;
   const int gq = (int)(g - sg * kScSuper);
-  const unsigned long long* a_src = p.agg + (g * kScGroup + lane) * K;
-  const unsigned long long* g_src = p.gagg + (sg * kScSuper + lane) * K;
-  const unsigned long long* s_src = p.sincl + (sg > 0 ? sg - 1 : 0) * K;
+  const unsigned long long* a_src = p.agg + (g * kScGroup + lane) * S;
+  const unsigned long long* g_src = p.gagg + (sg * kScSuper + lane) * S;
+  const unsigned long long* s_src = p.sincl + (sg > 0 ? sg - 1 : 0) * S;
   StatusEntry<K> ea[R], eg, es;
   bool need_a[R];
 #pragma unroll
@@ -610,7 +316,7 @@ __device__ __forceinline__ typename P::A scan_lookback_lean(const CumsumParams& 
   const bool need_g = lane < gq, need_s = sg > 0;
   // first batch: everything at once (one L2 round trip when all flags are up, the common case)
 #pragma unroll
-  for (int r = 0; r < R; ++r) { if (need_a[r]) ea[r].load(a_src + r * 32 * K); else ea[r].set_ready_zero(); }
+  for (int r = 0; r < R; ++r) { if (need_a[r]) ea[r].load(a_src + r * 32 * S); else ea[r].set_ready_zero(); }
   if (need_g) eg.load(g_src); else eg.set_ready_zero();
   if (need_s) es.load(s_src); else es.set_ready_zero();
   while (true) {
@@ -619,7 +325,7 @@ __device__ __forceinline__ typename P::A scan_lookback_lean(const CumsumParams& 
     for (int r = 0; r < R; ++r) ok = ok && ea[r].ready();
     if (__all_sync(0xffffffffu, ok)) break;
 #pragma unroll
-    for (int r = 0; r < R; ++r) if (need_a[r] && !ea[r].ready()) ea[r].load(a_src + r * 32 * K);
+    for (int r = 0; r < R; ++r) if (need_a[r] && !ea[r].ready()) ea[r].load(a_src + r * 32 * S);
   }
   A x[R];
 #pragma unroll
@@ -643,7 +349,7 @@ __device__ __forceinline__ typename P::A scan_lookback_lean(const CumsumParams& 
     unsigned wg[3] = {0u, 0u, 0u};
     P::to_words(P::add(part, tile_total), wg);
 #pragma unroll
-    for (int k = 0; k < K; ++k) st_word(p.gagg + g * K + k, wg[k]);
+    for (int k = 0; k < K; ++k) st_word(p.gagg + g * S + k, wg[k]);
   }
   while (!__all_sync(0xffffffffu, eg.ready() && es.ready())) {
     if (need_g && !eg.ready()) eg.load(g_src);
@@ -665,7 +371,7 @@ __device__ __forceinline__ typename P::A scan_lookback_lean(const CumsumParams& 
     unsigned wi[3] = {0u, 0u, 0u};
     P::to_words(P::add(excl, tile_total), wi);
 #pragma unroll
-    for (int k = 0; k < K; ++k) st_word(p.sincl + sg * K + k, wi[k]);
+    for (int k = 0; k < K; ++k) st_word(p.sincl + sg * S + k, wi[k]);
   }
   return excl;
 }
@@ -674,11 +380,14 @@ constexpr int kScStreamThreads = kScThreads + 32;  // 8 compute warps + the look
 constexpr int kScStreamStages = 3;
 constexpr int kScStreamBlocksPerSm = 2;            // 2 x (3 x 32 KB) of the SM's 227 KB
 
-template <typename T, bool kHasValid>
+// kChecked (integers only): the exact 96-bit running sum, compared with T's range at every valid row; the lowest row
+// that leaves it goes to first_bad
+template <typename T, bool kHasValid, bool kChecked>
 __global__ void __launch_bounds__(kScStreamThreads, kScStreamBlocksPerSm)
 cumsum_stream_kernel(const CumsumParams p) {
-  using P = typename PolSel<T, false>::type;
+  using P = typename PolSel<T, kChecked>::type;
   using A = typename P::A;
+  constexpr int S = StatusEntry<P::K>::kStride;
   constexpr int N = 16 / sizeof(T);
   constexpr int E = kScRows * N;                  // rows owned by one lane (128 contiguous bytes)
   constexpr int kTileRows = kScTileBytes / sizeof(T);
@@ -695,16 +404,21 @@ cumsum_stream_kernel(const CumsumParams p) {
   const unsigned char* __restrict__ in = reinterpret_cast<const unsigned char*>(p.in);
   unsigned char* __restrict__ out = reinterpret_cast<unsigned char*>(p.out);
   const int64_t n_bytes = p.n * (int64_t)sizeof(T);
+  const int out_mis = (int)(reinterpret_cast<uintptr_t>(out) & 15);  // 0, or a multiple of sizeof(T) (block-uniform)
+  auto store16 = [&](int64_t g, const uint4& v) {  // bytes [g, g + 16) of the output, all inside it
+    if (out_mis) st_pieces<T>(out + g, v, out_mis);
+    else __stcs(reinterpret_cast<uint4*>(out + g), v);
+  };
 
   if (threadIdx.x == 0) s_state = *p.state;
   __syncthreads();
   const A start = P::from_state(s_state);
   if (!p.skip_nulls && s_state.encountered_null != 0) {
     // an earlier chunk of the sequence met a null: every slot of this call is null (value 0) and the
-    // carried state stays as it is (cumsum_kernel's limit = 0 case)
+    // carried state stays as it is
     const uint4 z = make_uint4(0u, 0u, 0u, 0u);
     for (int64_t b = ((int64_t)blockIdx.x * kScStreamThreads + threadIdx.x) * 16; b < n_bytes; b += (int64_t)gridDim.x * kScStreamThreads * 16) {
-      if (b + 16 <= n_bytes) __stcs(reinterpret_cast<uint4*>(out + b), z);
+      if (b + 16 <= n_bytes) store16(b, z);
       else for (int64_t j = b; j < n_bytes; ++j) out[j] = 0;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { CumsumState ns = s_state; P::to_state(start, &ns); *p.state = ns; }
@@ -712,7 +426,7 @@ cumsum_stream_kernel(const CumsumParams p) {
   }
 
   // validity of the E rows a lane owns, 32 at a time: rows at or past `limit` (the first null when nulls are not
-  // skipped) and past n contribute nothing — cumsum_kernel's rule.  Returns whether every row counts (the common case).
+  // skipped) and past n contribute nothing.  Returns whether every row counts (the common case).
   int64_t limit = p.n;
   if (kHasValid && !p.skip_nulls) limit = *p.first_null;
   const int64_t vlo = p.voff >> 3, vhi = (p.voff + p.n + 7) >> 3;
@@ -743,11 +457,23 @@ cumsum_stream_kernel(const CumsumParams p) {
   const uint32_t blk_row = (uint32_t)lane * 128u;
   const uint32_t blk_x = (uint32_t)(lane & 7) << 4;
 
-  const int in_mis = (int)(reinterpret_cast<uintptr_t>(in) & 15);   // 0, or a multiple of sizeof(T) >= 4 (block-uniform)
+  const int in_mis = (int)(reinterpret_cast<uintptr_t>(in) & 15);   // 0, or a multiple of sizeof(T) (block-uniform)
   auto prefetch = [&](int64_t tile, int stage) {
     const uint32_t dst0 = ring + (uint32_t)stage * kScTileBytes + seg_off;
     const int64_t g0 = tile * kScTileBytes + seg_off + (int64_t)lane * 16;
-    if (in_mis) {
+    if (sizeof(T) < 4 && (in_mis & 3)) {
+      // 1- / 2-byte elements below 4-byte alignment: cp.async has no piece that small, so plain loads fill the same
+      // slots (the __syncwarp after cp_async_wait orders these stores too: a warp only touches its own segment)
+      const T* src = reinterpret_cast<const T*>(in);
+#pragma unroll 4  // fully unrolled, the 16-bit kernels' loads in flight raise their register count by ~15
+      for (int k = 0; k < kScRows; ++k) {
+        const int64_t e = (g0 + k * 512) / (int64_t)sizeof(T);
+        __align__(16) T v[N];
+#pragma unroll
+        for (int i = 0; i < N; ++i) v[i] = e + i < p.n ? src[e + i] : T(0);
+        *reinterpret_cast<uint4*>(s_ring + (dst0 - ring) + (str_even ^ ((k & 1) << 6)) + k * 512) = *reinterpret_cast<const uint4*>(v);
+      }
+    } else if (in_mis) {
       // element-aligned input: the 16-byte slots of the ring are filled by two 8-byte or four 4-byte copies
 #pragma unroll
       for (int k = 0; k < kScRows; ++k) {
@@ -787,6 +513,7 @@ cumsum_stream_kernel(const CumsumParams p) {
   const int64_t mine = ((int64_t)blockIdx.x < p.n_tiles) ? (p.n_tiles - blockIdx.x + G - 1) / G : 0;  // tiles of this block
   if (!looker) { if (mine > 0) prefetch(blockIdx.x, 0); cp_async_commit(); }
   A lane_excl_cur = P::zero(), warp_excl_cur = P::zero();
+  long long my_bad = AG_NO_ERROR_POS;  // checked: lowest row of this lane whose running sum left T's range
   // validity words of the rows this lane owns: fetched once per tile, in its reduction, and carried to its finalization
   // one iteration later; `dense` is made warp-uniform so a warp runs ONE of the two loops, not both under divergence
   unsigned vb_cur[VW], vb_prev[VW];
@@ -838,11 +565,11 @@ cumsum_stream_kernel(const CumsumParams p) {
             s_arrived[br] = 0u;
             A tile_total = P::zero();
 #pragma unroll
-            for (int wi = 0; wi < kScWarps; ++wi) tile_total = P::add(tile_total, reinterpret_cast<volatile A*>(s_warp[br])[wi]);
+            for (int wi = 0; wi < kScWarps; ++wi) tile_total = P::add(tile_total, ld_shared_volatile(s_warp[br][wi]));
             unsigned w[3] = {0u, 0u, 0u};
             P::to_words(tile_total, w);
 #pragma unroll
-            for (int k = 0; k < P::K; ++k) st_word(p.agg + tile_r * P::K + k, w[k]);
+            for (int k = 0; k < P::K; ++k) st_word(p.agg + tile_r * S + k, w[k]);
           }
         }
       }
@@ -850,7 +577,7 @@ cumsum_stream_kernel(const CumsumParams p) {
       A tile_total = P::zero();
 #pragma unroll
       for (int wi = 0; wi < kScWarps; ++wi) tile_total = P::add(tile_total, s_warp[bf][wi]);
-      const A excl = scan_lookback_lean<P>(p, tile_f, tile_total, start, lane);
+      const A excl = cumsum_lookback<P>(p, tile_f, tile_total, start, lane);
       if (lane == 0) {
         s_excl[bf] = excl;
         if (tile_f == p.n_tiles - 1) {
@@ -878,23 +605,39 @@ cumsum_stream_kernel(const CumsumParams p) {
 #pragma unroll
         for (int c = 0; c < kScRows; ++c) raw[c] = *reinterpret_cast<const uint4*>(seg + blk_row + (((uint32_t)c << 4) ^ blk_x));
         T* o = reinterpret_cast<T*>(raw);
-        A run = P::add(warp_excl_cur, lane_excl_cur);
-        const T off = P::value(s_excl[bf]);
-        if (dense_prev) {
-#pragma unroll
-          for (int i = 0; i < E; ++i) { run = P::add_elem(run, o[i]); o[i] = P::offset_add(off, P::value(run)); }
-        } else {
+        if constexpr (kChecked) {
+          // the exact running sum from the tile's prefix on: every valid row is range-checked
+          A run = P::add(P::add(s_excl[bf], warp_excl_cur), lane_excl_cur);
+          const int64_t t0 = tile_f * kTileRows + (int64_t)warp * kSegRows + (int64_t)lane * E;
 #pragma unroll
           for (int i = 0; i < E; ++i) {
-            if ((vb_prev[i >> 5] >> (i & 31)) & 1u) { run = P::add_elem(run, o[i]); o[i] = P::offset_add(off, P::value(run)); }
-            else o[i] = T(0);
+            if (dense_prev || ((vb_prev[i >> 5] >> (i & 31)) & 1u)) {
+              run = P::add_elem(run, o[i]);
+              o[i] = P::value(run);
+              if (P::out_of_range(run) && t0 + i < my_bad) my_bad = t0 + i;
+            } else {
+              o[i] = T(0);
+            }
+          }
+        } else {
+          A run = P::add(warp_excl_cur, lane_excl_cur);
+          const T off = P::value(s_excl[bf]);
+          if (dense_prev) {
+#pragma unroll
+            for (int i = 0; i < E; ++i) { run = P::add_elem(run, o[i]); o[i] = P::offset_add(off, P::value(run)); }
+          } else {
+#pragma unroll
+            for (int i = 0; i < E; ++i) {
+              if ((vb_prev[i >> 5] >> (i & 31)) & 1u) { run = P::add_elem(run, o[i]); o[i] = P::offset_add(off, P::value(run)); }
+              else o[i] = T(0);
+            }
           }
         }
 #pragma unroll
         for (int c = 0; c < kScRows; ++c) *reinterpret_cast<uint4*>(seg + blk_row + (((uint32_t)c << 4) ^ blk_x)) = raw[c];
         __syncwarp();
         const int64_t g0 = tile_f * kScTileBytes + seg_off + (int64_t)lane * 16;
-        if (g0 - (int64_t)lane * 16 + 4096 <= n_bytes) {
+        if (!out_mis && g0 - (int64_t)lane * 16 + 4096 <= n_bytes) {
 #pragma unroll
           for (int k = 0; k < kScRows; ++k)
             __stcs(reinterpret_cast<uint4*>(out + g0 + k * 512), *reinterpret_cast<const uint4*>(seg + (str_even ^ ((k & 1) << 6)) + k * 512));
@@ -903,7 +646,7 @@ cumsum_stream_kernel(const CumsumParams p) {
           for (int k = 0; k < kScRows; ++k) {
             const int64_t g = g0 + k * 512;
             const uint4 v = *reinterpret_cast<const uint4*>(seg + (str_even ^ ((k & 1) << 6)) + k * 512);
-            if (g + 16 <= n_bytes) __stcs(reinterpret_cast<uint4*>(out + g), v);
+            if (g + 16 <= n_bytes) store16(g, v);
             else {
               const unsigned char* vb = reinterpret_cast<const unsigned char*>(&v);
               for (int q = 0; q < 16; ++q) if (g + q < n_bytes) out[g + q] = vb[q];
@@ -920,6 +663,14 @@ cumsum_stream_kernel(const CumsumParams p) {
     }
     st_f = st_r;
     st_r = st_r + 1 == kScStreamStages ? 0 : st_r + 1;
+  }
+  if (kChecked) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, d);
+      my_bad = o < my_bad ? o : my_bad;
+    }
+    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.first_bad, my_bad);
   }
 }
 
@@ -948,7 +699,7 @@ __global__ void set_i64_kernel(long long* p, long long v) { *p = v; }
 // Output validity of one call, one thread per aligned 32-bit output word:
 //   SkipNulls: the input validity;  otherwise: valid up to the first null, null from there on
 //   (vector_cumulative.go:277-289), everything null once an earlier chunk met a null.
-// Runs BEFORE cumsum_kernel on the same stream (it needs the state as the call found it) and adds
+// Runs BEFORE cumsum_stream_kernel on the same stream (it needs the state as the call found it) and adds
 // the number of null slots it wrote to state->null_count.
 __global__ void __launch_bounds__(256)
 cumsum_validity_kernel(const uint8_t* __restrict__ valid, int64_t voff, int64_t n, int skip_nulls, const long long* first_null,
@@ -977,9 +728,9 @@ cumsum_validity_kernel(const uint8_t* __restrict__ valid, int64_t voff, int64_t 
   if ((threadIdx.x & 31) == 0 && nulls) atomicAdd(reinterpret_cast<unsigned long long*>(&state->null_count), (unsigned long long)nulls);
 }
 
-template <typename T>
+template <typename T, bool kChecked>
 ag_status launch_cumsum(CumsumParams& p, cudaStream_t st) {
-  constexpr int kStatusK = 3;  // sized for the widest accumulator (exact 96-bit)
+  constexpr int S = StatusEntry<PolSel<T, kChecked>::type::K>::kStride;  // words per status entry
   constexpr int kTileRows = kScTileBytes / sizeof(T);
   Workspace* ws;
   AG_TRY(get_workspace(st, &ws));
@@ -987,13 +738,11 @@ ag_status launch_cumsum(CumsumParams& p, cudaStream_t st) {
   p.n_tiles = (p.n + kTileRows - 1) / kTileRows;
   const int64_t n_groups = (p.n_tiles + kScGroup - 1) / kScGroup;
   const int64_t n_super = (n_groups + kScSuper - 1) / kScSuper;
-  // every level starts on a 16-byte boundary (the streaming kernel fetches whole entries with 128-bit loads)
-  const size_t agg_words = ((size_t)p.n_tiles * kStatusK + 1) & ~(size_t)1, gagg_words = ((size_t)n_groups * kStatusK + 1) & ~(size_t)1;
-  const size_t words = agg_words + gagg_words + (size_t)n_super * kStatusK;
+  const size_t words = (size_t)(p.n_tiles + n_groups + n_super) * S;
   AG_TRY(ensure_tile_status(ws, words, st));
   p.agg = ws->tile_status;
-  p.gagg = p.agg + agg_words;
-  p.sincl = p.gagg + gagg_words;
+  p.gagg = p.agg + p.n_tiles * S;
+  p.sincl = p.gagg + n_groups * S;
   AG_CUDA_TRY(cudaMemsetAsync(ws->tile_status, 0, words * sizeof(unsigned long long), st));
   if (p.valid) {
     long long* fn = reinterpret_cast<long long*>(ws->scalars) + 8;  // slot 8 of the per-stream scalars
@@ -1012,38 +761,18 @@ ag_status launch_cumsum(CumsumParams& p, cudaStream_t st) {
     cumsum_validity_kernel<<<grid_for(n_words, 256, 8), 256, 0, st>>>(p.valid, p.voff, p.n, p.skip_nulls, p.first_null, p.state, words, shift, n_words);
     AG_TRY(check_launch("cumsum_validity_kernel"));
   }
-  // the streaming kernel wants a 16-byte aligned OUTPUT; an input that is only element-aligned (a slice) is fetched in
-  // 4- / 8-byte pieces, which needs elements of at least 4 bytes
-  const bool vec = ((reinterpret_cast<uintptr_t>(p.in) & 15) == 0 || sizeof(T) >= 4) && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
-  void* args[] = {(void*)&p};
-  const void* fn;
-  const bool chk = p.checked && !IsFp<T>::v;  // floats: the checked adder is the plain one
-  if (vec && !chk) {
-    constexpr int kRing = kScStreamStages * kScTileBytes;
-    static std::atomic<unsigned> attr_set{0u};  // per instantiation, one bit per device
-    const void* sfn = p.valid ? (const void*)cumsum_stream_kernel<T, true> : (const void*)cumsum_stream_kernel<T, false>;
-    static std::atomic<unsigned> attr_set_v{0u};
-    AG_TRY(ensure_dynamic_smem(sfn, kRing, p.valid ? &attr_set_v : &attr_set));
-    int per_sm = 0;
-    AG_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sfn, kScStreamThreads, kRing));
-    if (per_sm < 1) per_sm = 1;
-    const int64_t cap = (int64_t)sm_count() * per_sm;
-    const int grid = (int)(p.n_tiles < cap ? p.n_tiles : cap);
-    AG_CUDA_TRY(cudaLaunchCooperativeKernel(sfn, dim3(grid), dim3(kScStreamThreads), args, kRing, st));
-    return check_launch("cumsum_stream_kernel");
-  }
-  if (chk) {
-    if (vec) fn = p.valid ? (const void*)cumsum_kernel<T, true, true, !IsFp<T>::v> : (const void*)cumsum_kernel<T, true, false, !IsFp<T>::v>;
-    else fn = p.valid ? (const void*)cumsum_kernel<T, false, true, !IsFp<T>::v> : (const void*)cumsum_kernel<T, false, false, !IsFp<T>::v>;
-  } else {
-    if (vec) fn = p.valid ? (const void*)cumsum_kernel<T, true, true, false> : (const void*)cumsum_kernel<T, true, false, false>;
-    else fn = p.valid ? (const void*)cumsum_kernel<T, false, true, false> : (const void*)cumsum_kernel<T, false, false, false>;
-  }
-  const int per_sm = blocks_per_sm(fn, kScThreads);
+  constexpr int kRing = kScStreamStages * kScTileBytes;
+  static std::atomic<unsigned> attr_set{0u}, attr_set_v{0u};  // per instantiation, one bit per device
+  const void* fn = p.valid ? (const void*)cumsum_stream_kernel<T, true, kChecked> : (const void*)cumsum_stream_kernel<T, false, kChecked>;
+  AG_TRY(ensure_dynamic_smem(fn, kRing, p.valid ? &attr_set_v : &attr_set));
+  int per_sm = 0;
+  AG_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kScStreamThreads, kRing));
+  if (per_sm < 1) per_sm = 1;
   const int64_t cap = (int64_t)sm_count() * per_sm;
   const int grid = (int)(p.n_tiles < cap ? p.n_tiles : cap);
-  AG_CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kScThreads), args, 0, st));
-  return check_launch("cumsum_kernel");
+  void* args[] = {(void*)&p};
+  AG_CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kScStreamThreads), args, kRing, st));
+  return check_launch("cumsum_stream_kernel");
 }
 
 __global__ void cumsum_state_init_kernel(CumsumState* s, unsigned long long lo, long long hi) {
@@ -1063,11 +792,16 @@ ag_status cumulative_sum_dev(int type, const void* in, const uint8_t* valid, int
   if (valid && !out_valid) AG_FAIL(AG_ERR_INVALID, "cumulative_sum: an input with a validity bitmap needs an output validity bitmap");
   CumsumParams p{};
   p.out_valid = out_valid; p.ooff = ooff;
-  p.in = in; p.out = out; p.valid = valid; p.voff = voff; p.n = n; p.skip_nulls = skip_nulls; p.checked = checked;
+  p.in = in; p.out = out; p.valid = valid; p.voff = voff; p.n = n; p.skip_nulls = skip_nulls;
   p.first_null = nullptr; p.state = static_cast<CumsumState*>(d_state); p.first_bad = (long long*)d_first_bad;
   // the type id was validated above; anything else would run as float64
-  return visit_type(type, [&](auto tag) { return launch_cumsum<typename decltype(tag)::type>(p, st); },
-                    [&] { return launch_cumsum<double>(p, st); });
+  return visit_type(type, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if constexpr (!IsFp<T>::v) {  // floats: the checked adder is the plain one
+      if (checked) return launch_cumsum<T, true>(p, st);
+    }
+    return launch_cumsum<T, false>(p, st);
+  }, [&] { return launch_cumsum<double, false>(p, st); });
 }
 
 ag_status cumulative_sum_state_init(void* d_state, int type, const void* start_host, cudaStream_t st) {

@@ -120,7 +120,8 @@ def test_oracle_matches_numpy_model_integers(cpu, t):
 gpu = pytest.mark.gpu
 
 
-def gpu_chunks(ag, t, chunks, valids, skip, checked, start=None, via="dev"):
+def gpu_chunks(ag, t, chunks, valids, skip, checked, start=None, via="dev", in_off=0, out_off=0):
+    """in_off / out_off (dev only): the input and output pointers are that many elements past an aligned allocation."""
     total = sum(len(c) for c in chunks)
     isz = np.dtype(NP_OF[t]).itemsize
     if via == "host":
@@ -141,22 +142,22 @@ def gpu_chunks(ag, t, chunks, valids, skip, checked, start=None, via="dev"):
     ag.call("ag_cumulative_sum_state_init_dev", state.ptr, t, ptr(sv) if sv is not None else None, None)
     bad = Dev(np.zeros(1, dtype=np.int64))
     ag.call("ag_error_word_reset_dev", bad.ptr, None)
-    dout = Dev(np.zeros(total + 8, dtype=NP_OF[t]))
+    dout = Dev(np.zeros(out_off + total + 8, dtype=NP_OF[t]))
     any_nulls = any(v is not None for v in valids)
     dov = Dev(np.zeros((total + 7) // 8 + 8, dtype=np.uint8)) if any_nulls else None
     keep, pos = [], 0
     for x, v in zip(chunks, valids):
         n = len(x)
-        dx = Dev(x if n else np.zeros(1, dtype=NP_OF[t]))
+        dx = Dev(np.concatenate([np.zeros(in_off, dtype=NP_OF[t]), x]) if n + in_off else np.zeros(1, dtype=NP_OF[t]))
         dv = Dev(pack_bits(v, offset=3)) if v is not None else None
         keep += [dx, dv]
-        ag.call("ag_cumulative_sum_dev", t, dx.ptr, dv.ptr if dv else None, 3, n, int(skip), int(checked),
-                dout.ptr + pos * isz, dov.ptr if dov else None, pos, state.ptr, bad.ptr, None)
+        ag.call("ag_cumulative_sum_dev", t, dx.ptr + in_off * isz, dv.ptr if dv else None, 3, n, int(skip), int(checked),
+                dout.ptr + (out_off + pos) * isz, dov.ptr if dov else None, pos, state.ptr, bad.ptr, None)
         pos += n
     ag.call("ag_stream_sync", None)
     b = int(bad.get()[0])
     stt = state.get()
-    out = dout.get()[:total]
+    out = dout.get()[out_off:out_off + total]
     valid = unpack_bits(dov.get(), 0, total).astype(bool) if dov else np.ones(total, dtype=bool)
     return (N.AG_ERR_INVALID if (checked and b != NO_POS) else 0), out, valid, int(stt[3]), b
 
@@ -216,6 +217,9 @@ def test_gpu_checked_overflow_row(ag, cpu, t):
         wst, wout, _, _, wbad = oracle_chunks(cpu, t, [x], [None], False, True)
         st, out, _, _, bad = gpu_chunks(ag, t, [x], [None], False, True)
         assert (st != 0) == (wst != 0) and (wst == 0 or bad == wbad), (TYPE_NAME[t], n, pos, bad, wbad)
+        # the same from a slice (input 1 element past a 16-byte boundary) into an output 3 elements past one
+        st, out, _, _, bad = gpu_chunks(ag, t, [x], [None], False, True, in_off=1, out_off=3)
+        assert (st != 0) == (wst != 0) and (wst == 0 or bad == wbad), (TYPE_NAME[t], n, pos, bad, wbad, "sliced")
         # a null in front of the offender (no skip) hides it: the sequence is dead before the overflow
         valid = np.ones(n, dtype=bool)
         valid[0] = False
@@ -227,14 +231,16 @@ def test_gpu_checked_overflow_row(ag, cpu, t):
 @gpu
 @pytest.mark.parametrize("t", [N.INT64, N.FLOAT64, N.INT32], ids=lambda t: TYPE_NAME[t])
 def test_gpu_large_crosses_super_group(ag, cpu, t):
-    """> 4096 tiles (128 MB of input): the third look-back level (inclusive prefix per super-group)."""
+    """> 4096 tiles (128 MB of input): the third look-back level (inclusive prefix per super-group); checked int64 runs
+    it with three-word status entries."""
     rng = np.random.default_rng(4242)
     n = 4100 * (32768 // np.dtype(NP_OF[t]).itemsize) + 77
     x = rng.integers(-3, 4, n).astype(NP_OF[t])
     for valid in (None, rng.random(n) > 0.001):
-        wst, wout, wv, wn, _ = oracle_chunks(cpu, t, [x], [valid], True, False, 11)
-        st, out, v, nulls, _ = gpu_chunks(ag, t, [x], [valid], True, False, 11)
-        assert st == 0 and np.array_equal(v, wv) and out.tobytes() == wout.tobytes() and nulls == wn
+        for checked in ((False, True) if t == N.INT64 else (False,)):
+            wst, wout, wv, wn, _ = oracle_chunks(cpu, t, [x], [valid], True, checked, 11)
+            st, out, v, nulls, _ = gpu_chunks(ag, t, [x], [valid], True, checked, 11)
+            assert st == wst == 0 and np.array_equal(v, wv) and out.tobytes() == wout.tobytes() and nulls == wn, checked
 
 
 @gpu
@@ -310,10 +316,9 @@ def test_gpu_nonfinite_prefix_classes(ag, cpu, t):
 
 
 @gpu
-def test_gpu_streaming_and_general_kernels_share_one_sequence(ag, cpu):
-    """Chunks without a bitmap (16-byte aligned: the streaming kernel) and chunks with one (the general
-    kernel) alternate inside one sequence; once a null was met (no skip) a later bitmap-free chunk is
-    all null and leaves the carried value alone."""
+def test_gpu_chunks_with_and_without_bitmap_share_one_sequence(ag, cpu):
+    """Chunks without a bitmap and chunks with one alternate inside one sequence; once a null was met (no skip) a
+    later bitmap-free chunk is all null and leaves the carried value alone."""
     rng = np.random.default_rng(78)
     for t in (N.INT64, N.INT16, N.FLOAT64, N.FLOAT32):
         cuts = [0, 4096 * 16, 4096 * 16 + 48_000, 300_000 + 16, 300_000 + 16 + 70_000 + 32, 500_000]
@@ -330,9 +335,11 @@ def test_gpu_streaming_and_general_kernels_share_one_sequence(ag, cpu):
 
 @gpu
 def test_gpu_element_aligned_input_streams(ag, cpu):
-    """An Arrow slice: the values pointer is only element-aligned (8 / 4 bytes off a 16-byte boundary), the output is
-    aligned.  4- and 8-byte types go through the streaming kernel's 4- / 8-byte cp.async pieces, 1- / 2-byte types through
-    the general kernel; with and without a validity bitmap, lengths around the 32 KB tile edges."""
+    """An Arrow slice: the values pointer is only element-aligned (1, 2 or 3 elements past a 16-byte boundary).  4- and
+    8-byte types are fetched in 4- / 8-byte cp.async pieces, 1- / 2-byte types below 4-byte alignment by plain loads
+    (the others in 4-byte pieces).  Each input runs three ways: into an aligned output, into an output just as far past
+    a 16-byte boundary (stored in pieces), and checked (status, first failing row and values equal the oracle's); with
+    and without a validity bitmap, lengths around the 32 KB tile edges."""
     rng = np.random.default_rng(79)
     for t in (N.INT64, N.FLOAT64, N.INT32, N.FLOAT32, N.UINT32, N.INT16, N.UINT8):
         dt = NP_OF[t]; isz = np.dtype(dt).itemsize
@@ -342,19 +349,26 @@ def test_gpu_element_aligned_input_streams(ag, cpu):
                 x = base[off_elems:off_elems + n]
                 for p_null, skip in ((0.0, False), (0.05, True), (0.05, False)):
                     valid = rng.random(n) >= p_null if p_null else None
-                    wst, wout, wv, wn, _ = oracle_chunks(cpu, t, [x], [valid], skip, False, 2)
-                    # device call on a pointer off_elems elements past an aligned allocation
-                    dbase = Dev(base)
-                    state = Dev(np.zeros(4, dtype=np.int64)); sv = np.array([2], dtype=dt)
-                    ag.call("ag_cumulative_sum_state_init_dev", state.ptr, t, ptr(sv), None)
-                    bad = Dev(np.zeros(1, dtype=np.int64)); ag.call("ag_error_word_reset_dev", bad.ptr, None)
-                    dout = Dev(np.zeros(n + 8, dtype=dt))
-                    dv = Dev(pack_bits(valid, offset=3)) if valid is not None else None
-                    dov = Dev(np.zeros((n + 7) // 8 + 8, dtype=np.uint8)) if valid is not None else None
-                    ag.call("ag_cumulative_sum_dev", t, dbase.ptr + off_elems * isz, dv.ptr if dv else None, 3, n, int(skip), 0,
-                            dout.ptr, dov.ptr if dov else None, 0, state.ptr, bad.ptr, None)
-                    ag.call("ag_stream_sync", None)
-                    out = dout.get()[:n]
-                    assert out.tobytes() == wout.tobytes(), (TYPE_NAME[t], off_elems, n, p_null, skip)
-                    if valid is not None:
-                        assert np.array_equal(unpack_bits(dov.get(), 0, n).astype(bool), wv) and int(state.get()[3]) == wn
+                    for out_off, checked in ((0, False), (off_elems, False), (0, True)):
+                        wst, wout, wv, wn, wbad = oracle_chunks(cpu, t, [x], [valid], skip, checked, 2)
+                        # device call on a pointer off_elems elements past an aligned allocation
+                        dbase = Dev(base)
+                        state = Dev(np.zeros(4, dtype=np.int64)); sv = np.array([2], dtype=dt)
+                        ag.call("ag_cumulative_sum_state_init_dev", state.ptr, t, ptr(sv), None)
+                        bad = Dev(np.zeros(1, dtype=np.int64)); ag.call("ag_error_word_reset_dev", bad.ptr, None)
+                        dout = Dev(np.zeros(out_off + n + 8, dtype=dt))
+                        dv = Dev(pack_bits(valid, offset=3)) if valid is not None else None
+                        dov = Dev(np.zeros((n + 7) // 8 + 8, dtype=np.uint8)) if valid is not None else None
+                        ag.call("ag_cumulative_sum_dev", t, dbase.ptr + off_elems * isz, dv.ptr if dv else None, 3, n, int(skip),
+                                int(checked), dout.ptr + out_off * isz, dov.ptr if dov else None, 0, state.ptr, bad.ptr, None)
+                        ag.call("ag_stream_sync", None)
+                        where = (TYPE_NAME[t], off_elems, n, p_null, skip, out_off, checked)
+                        got_bad = int(bad.get()[0])
+                        if wst != 0:  # a checked narrow type whose running sum leaves its range
+                            assert got_bad == wbad, where
+                            continue
+                        assert got_bad == NO_POS, where
+                        out = dout.get()[out_off:out_off + n]
+                        assert out.tobytes() == wout.tobytes(), where
+                        if valid is not None:
+                            assert np.array_equal(unpack_bits(dov.get(), 0, n).astype(bool), wv) and int(state.get()[3]) == wn, where

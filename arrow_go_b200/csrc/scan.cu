@@ -31,9 +31,13 @@
 //     tiles, which resident blocks reach in increasing order.
 // Unchecked integers accumulate modulo 2^64, which is all the wrapped result needs; the checked flavour
 // accumulates an exact 96-bit value (64-bit wrap + carry count) and compares the running sum with the
-// type's range per element.  Floats accumulate in their own type; results are bit-exact with the
-// reference's left-to-right loop whenever every partial sum is exactly representable, and differ by
-// rounding of the same order as the reference's own otherwise (DESIGN.md).
+// type's range per element.  Floats accumulate in their own type from -0.0 (the identity of IEEE addition);
+// outputs and carried state are bit-exact with tests/cumsum_float_ref.py, the step-by-step model of this
+// fold order, on any input; bit-exact with the reference's left-to-right loop, signed zeros included,
+// whenever every partial sum is exactly representable; within the summation bound of the fold's depth
+// otherwise.  The carried state is the last tile's excl + tile_total, which can differ by rounding from
+// the last output slot (excl + ((warp_excl + lane_excl) + x...)); the reference's state is its last output
+// (DESIGN.md).
 #include "common.cuh"
 
 #include <limits>
@@ -157,7 +161,9 @@ template <typename T>
 struct Pol<T, true> {  // float / double: accumulate in the value type
   using A = T;
   static constexpr int K = sizeof(T) == 8 ? 2 : 1;
-  static __device__ __forceinline__ A zero() { return T(0); }
+  // -0.0 is the identity of IEEE addition (+0.0 is not: -0.0 + +0.0 = +0.0), so the padded lanes, entries and
+  // accumulators that start from it leave every sum's bits alone, the sign of a zero included
+  static __device__ __forceinline__ A zero() { return T(-0.0); }
   static __device__ __forceinline__ A add(A a, A b) {
     if constexpr (sizeof(T) == 8) return __dadd_rn(a, b); else return __fadd_rn(a, b);
   }
@@ -663,6 +669,26 @@ cumsum_stream_kernel(const CumsumParams p) {
     }
     st_f = st_r;
     st_r = st_r + 1 == kScStreamStages ? 0 : st_r + 1;
+  }
+  if constexpr (IsFp<T>::v && !kHasValid) {
+    // Without a bitmap the last tile's rows past n arrive zero-filled and enter its lane totals as +0.0, which is not
+    // the identity of the fold.  They come after every real row, so no output sees them; only the carried state
+    // excl + tile_total can: it reads +0.0 where the real rows give -0.0 + -0.0.  That happens exactly when excl and
+    // the last output (excl + the real rows' fold) are both -0.0, so the owner of row n - 1 puts the sign back here,
+    // once per call, after the looker's state store (ordered by the last iteration's barrier).
+    const int64_t last = p.n - 1, tile = last / kTileRows;
+    const int64_t local = last - tile * kTileRows;
+    if (p.n % kTileRows != 0 && tile % G == blockIdx.x && !looker && warp == local / kSegRows && lane == (local % kSegRows) / E) {
+      const int i = (int)(local % E);
+      const unsigned char* seg = s_ring + ((mine - 1) % kScStreamStages) * kScTileBytes + seg_off;
+      const T out_last = *reinterpret_cast<const T*>(seg + blk_row + (((uint32_t)(i / N) << 4) ^ blk_x) + (i % N) * sizeof(T));
+      const T excl = s_excl[(mine - 1) & 1];
+      if (out_last == T(0) && signbit(out_last) && excl == T(0) && signbit(excl)) {
+        CumsumState ns = *p.state;
+        P::to_state(T(-0.0), &ns);
+        *p.state = ns;
+      }
+    }
   }
   if (kChecked) {
 #pragma unroll

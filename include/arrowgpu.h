@@ -352,8 +352,11 @@ ag_status ag_cast_numeric_checked_dev(int itype, int otype, const void* d_in, co
  *   it.  `checked`: AG_ERR_INVALID "overflow" at the first running sum outside the type's range
  *   (integers only; floats never fail), lowest failing row in *first_bad.
  *   Integers: bit-exact.  Floats: single-pass parallel scan with a fixed (data- and n-determined)
- *   association — bit-exact with the reference's left-to-right loop whenever every partial sum
- *   is exactly representable, otherwise within the usual summation error bound (DESIGN.md).
+ *   association, bit-exact with its model tests/cumsum_float_ref.py on any input — bit-exact with
+ *   the reference's left-to-right loop whenever every partial sum is exactly representable (signed
+ *   zeros included), otherwise within the summation error bound of that association (DESIGN.md).
+ *   The state carried to the next chunk is the last tile's exclusive prefix + tile total, which may
+ *   differ from the last output slot by rounding (the reference carries its last output).
  *
  *   Device flavour: the running value and the encountered-null flag live in a 32-byte device
  *   block (ag_cumsum_state) so that the chunks of a chunked column are a chain of launches on

@@ -139,3 +139,37 @@ def checksum64(words):
 
 def dev_scalar_i64(value=0):
     return Dev(np.array([value], dtype=np.int64))
+
+
+class CumsumOracleState(C.Structure):
+    """oracle/cpu_ref.c ref_cumsum_state: the running value in the type's own bytes + the encountered-null flag."""
+    _fields_ = [("cur", C.c_uint8 * 8), ("encountered_null", C.c_int64)]
+
+
+def oracle_cumsum(cpu, chunks, valids=None, skip=False, start=None, voff=3):
+    """ref_cumulative_sum over the chunks of one sequence (unchecked): (values, output validity, null count, final
+    running value).  start None is zero."""
+    dt = np.asarray(chunks[0]).dtype
+    t = {v: k for k, v in NP_OF.items()}[dt.type]
+    valids = valids if valids is not None else [None] * len(chunks)
+    st = CumsumOracleState()
+    raw = np.array([0 if start is None else start], dtype=dt).tobytes()
+    for i, b in enumerate(raw):
+        st.cur[i] = b
+    total = sum(len(c) for c in chunks)
+    out = np.zeros(total, dtype=dt)
+    ovalid = np.zeros((total + 7) // 8 + 1, dtype=np.uint8)
+    pos = nulls = 0
+    for x, v in zip(chunks, valids):
+        x = np.ascontiguousarray(x, dtype=dt)
+        bm = pack_bits(v, offset=voff) if v is not None else None
+        o = np.zeros(len(x), dtype=dt)
+        nn, bad = C.c_int64(0), C.c_int64(0)
+        rc = cpu.ref_cumulative_sum(t, ptr(x), ptr(bm), voff, len(x), int(skip), 0, ptr(o), ptr(ovalid), pos,
+                                    C.byref(st), C.byref(nn), C.byref(bad))
+        assert rc == 0
+        out[pos:pos + len(x)] = o
+        nulls += nn.value
+        pos += len(x)
+    cur = np.frombuffer(bytes(st.cur)[:dt.itemsize], dtype=dt)[0]
+    return out, unpack_bits(ovalid, 0, total).astype(bool), nulls, cur

@@ -3,9 +3,12 @@
 CPU part: the restatement (oracle/cpu_ref.c:ref_cumulative_sum) against the literal vectors of
 arrow/compute/vector_cumulative_test.go (tests/golden/cumulative_sum.json) and against an
 independent numpy model.  GPU part: the single-pass CUDA scan through the C ABI vs the oracle:
-bit-exact for integers and for floats whose partial sums are exactly representable; for general
-floats the deviation from the reference's left-to-right loop is bounded and, because the scan's
-association is fixed, identical from run to run."""
+bit-exact for integers and for floats whose partial sums are exactly representable (signed zeros
+included); for general floats the deviation from the reference's left-to-right loop is bounded and,
+because the scan's association is fixed, identical from run to run.  Float outputs and the carried
+state are bit-exact with tests/cumsum_float_ref.py on any input (tests/test_gpu_cumsum_float.py);
+that state is the last tile's excl + tile_total and may differ from the last output by rounding,
+unlike the reference's."""
 import ctypes as C
 import json
 import os

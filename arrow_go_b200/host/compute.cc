@@ -1052,8 +1052,14 @@ std::string Int128ToString(__int128 v) {
   return neg ? "-" + r : r;
 }
 
+const char* CastFunctionName(Type t);
+
 Status CastNumericExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out) {
-  const auto* opts = static_cast<const CastOptions*>(ctx->state);
+  // cast_<type> called by name carries whatever options the caller passed (functions.go:163-167 refuses none)
+  const auto* fo = static_cast<const FunctionOptions*>(ctx->state);   // the executor's state is the call's options
+  const auto* opts = dynamic_cast<const CastOptions*>(fo);
+  if (!fo) return Status::Invalid(std::string("function '") + CastFunctionName(out->type) + "' cannot be called without options");
+  if (!opts) return Status::Invalid(std::string(CastFunctionName(out->type)) + ": expected CastOptions, got " + fo->TypeName());
   const ArraySpan& in = batch.values[0].array;
   if (batch.len == 0) return Status::OK();
   NATIVE(ag_cast_numeric_checked_dev((int)in.type, (int)out->type, ValuesPtr(in), in.buffers[0].buf, in.offset, ValuesPtr(out), batch.len,
@@ -1202,7 +1208,11 @@ Status CumulativeSpans(bool checked, const CumulativeOptions* opts, Type t, cons
   bool needs_validity = false;
   for (auto& in : inputs) { total += in.len; needs_validity = needs_validity || (in.buffers[0].buf != nullptr && in.nulls != 0); }
   out->type = t; out->len = total; out->offset = 0; out->nulls = 0;
-  if (total == 0) return Status::OK();
+  if (total == 0) {   // no rows, but the start value is still checked: initCumulativeSum runs for every call (:119-144)
+    bool has_start;
+    uint8_t raw[8];
+    return CumulativeStart(opts, t, &has_start, raw);
+  }
   CumsumRun run;
   RETURN_NOT_OK(run.Init(t, opts));
   std::shared_ptr<Buffer> data, validity;

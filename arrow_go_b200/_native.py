@@ -64,6 +64,32 @@ def dict_chunk_table(chunks):
     return arr
 
 
+class SortChunk(C.Structure):
+    """ag_sort_chunk: one chunk of a sort key column."""
+    _fields_ = [("vals", C.c_void_p), ("valid", C.c_void_p), ("offset", C.c_int64), ("length", C.c_int64)]
+
+
+class SortKey(C.Structure):
+    """ag_sort_key: one key of a multi-key sort_indices call (type, order, null placement, chunks)."""
+    _fields_ = [("type", C.c_int), ("order", C.c_int), ("null_placement", C.c_int), ("nchunks", C.c_int),
+                ("chunks", C.POINTER(SortChunk))]
+
+
+def sort_key_table(keys):
+    """[(type, order, null_placement, [(vals, valid, offset, length), ...]), ...] -> ctypes array of ag_sort_key.
+    The chunk arrays are kept alive on the returned array (`_chunks`)."""
+    arr = (SortKey * max(len(keys), 1))()
+    arr._chunks = []
+    for k, (ty, order, placement, chunks) in enumerate(keys):
+        ch = (SortChunk * max(len(chunks), 1))()
+        for c, (v, ok, off, ln) in enumerate(chunks):
+            ch[c].vals, ch[c].valid, ch[c].offset, ch[c].length = v, ok, off, ln
+        arr._chunks.append(ch)
+        arr[k].type, arr[k].order, arr[k].null_placement, arr[k].nchunks = ty, order, placement, len(chunks)
+        arr[k].chunks = C.cast(ch, C.POINTER(SortChunk))
+    return arr
+
+
 NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1
 TYPE_DICTIONARY = 29
 TYPE_RUN_END_ENCODED = 38
@@ -234,6 +260,8 @@ _SIGS = {
     "ag_run_end_decode_dev": [_i, _i, _p, _i64, _p, _p, _i64, _i64, _i64, _p, _p, _p, _p, _p],
     "ag_sort_indices": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64],
     "ag_sort_indices_dev": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64, _p],
+    "ag_sort_indices_keys": [_i, _p, _i64, _p],
+    "ag_sort_indices_keys_dev": [_i, _p, _i64, _p, _p],
     "ag_parquet_unpack32": [_p, _p, _i64, _i, _pi64],
     "ag_parquet_unpack32_dev": [_p, _p, _i64, _i, _pi64, _p],
     "ag_parquet_bytes_to_bools": [_p, _i64, _p, _i64],

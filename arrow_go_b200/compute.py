@@ -30,7 +30,7 @@ DICTIONARY = 29   # Dictionary<int32, T>
 RUN_END_ENCODED = 38   # RunEndEncoded<int16|int32|int64, T>
 DROP_NULLS, EMIT_NULLS = 0, 1
 NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1   # DictionaryEncodeOptions.NullEncoding
-KIND_SCALAR, KIND_ARRAY, KIND_CHUNKED = 1, 2, 3
+KIND_SCALAR, KIND_ARRAY, KIND_CHUNKED, KIND_RECORD, KIND_TABLE = 1, 2, 3, 4, 5
 
 
 class ArrowError(RuntimeError):
@@ -93,6 +93,9 @@ def lib():
         h.agx_sort_indices.argtypes = [p, i, i, pp]
         h.agx_unique.argtypes = [p, pp]
         h.agx_is_in.argtypes = [p, p, i, pp]
+        h.agx_record_batch.argtypes = [i64, pp, i, pp]
+        h.agx_table.argtypes = [i64, pp, i, pp]
+        h.agx_sort_indices_keys.argtypes = [p, C.POINTER(i), C.POINTER(i), C.POINTER(i), i, pp]
         _lib = h
     return _lib
 
@@ -287,6 +290,31 @@ def Chunked(chunks, type_id):
     return d
 
 
+def RecordBatch(columns, num_rows=None):
+    """array.NewRecordBatch: array datums of num_rows rows each (default: the first column's length)."""
+    if num_rows is None:
+        num_rows = len(columns[0]) if columns else 0
+    arr = (C.c_void_p * max(len(columns), 1))(*[c._h for c in columns])
+    out = C.c_void_p()
+    _check(lib().agx_record_batch(num_rows, arr, len(columns), C.byref(out)))
+    d = Datum(out)
+    d._keep = columns
+    return d
+
+
+def Table(columns, num_rows=None):
+    """array.NewTable: chunked datums of num_rows rows each (an array datum becomes a one-chunk column)."""
+    cols = [Chunked([c], c.type) if c.kind == KIND_ARRAY else c for c in columns]
+    if num_rows is None:
+        num_rows = len(cols[0]) if cols else 0
+    arr = (C.c_void_p * max(len(cols), 1))(*[c._h for c in cols])
+    out = C.c_void_p()
+    _check(lib().agx_table(num_rows, arr, len(cols), C.byref(out)))
+    d = Datum(out)
+    d._keep = cols
+    return d
+
+
 def CallFunction(name, args, options=None):
     """compute.CallFunction(ctx, name, opts, args...) — options: None, ("arithmetic", no_check_overflow),
     ("filter", null_selection), ("take", bounds_check), ("dictionary_encode", null_encoding) or
@@ -373,10 +401,18 @@ NULLS_AT_END, NULLS_AT_START = 0, 1
 NULL_MATCH, NULL_SKIP, NULL_EMIT_NULL, NULL_INCONCLUSIVE = 0, 1, 2, 3
 
 
-def SortIndices(values, order=ASCENDING, null_placement=NULLS_AT_END):
-    """compute.SortIndices(ctx, input, SortOptions): uint64 row indices (arrow/compute/vector_sort.go:205-211)."""
+def SortIndices(values, order=ASCENDING, null_placement=NULLS_AT_END, keys=None):
+    """compute.SortIndices(ctx, input, SortOptions): uint64 row indices (arrow/compute/vector_sort.go:205-211).
+    keys=[(column, order, null_placement), ...] sorts with SortKeys instead: arrays and chunked arrays by the first key
+    (column ignored), record batches and tables lexicographically by every key; order and null_placement are then
+    unused.  keys=None keeps the single-key SortOptions call."""
     out = C.c_void_p()
-    _check(lib().agx_sort_indices(values._h, int(order), int(null_placement), C.byref(out)))
+    if keys is None:
+        _check(lib().agx_sort_indices(values._h, int(order), int(null_placement), C.byref(out)))
+        return Datum(out)
+    n = len(keys)
+    cols, orders, places = ((C.c_int * max(n, 1))(*[int(k[i]) for k in keys]) for i in range(3))
+    _check(lib().agx_sort_indices_keys(values._h, cols, orders, places, n, C.byref(out)))
     return Datum(out)
 
 

@@ -136,6 +136,9 @@ ag_status run_end_decode_dev(int type, int run_end_type, const void* run_ends, i
 // sort.cu
 ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int64_t voff, int64_t n, int order, int null_placement,
                            uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);
+// argument checks of sort_indices_keys_dev (no device work)
+ag_status sort_indices_keys_check(int nkeys, const ag_sort_key* keys, int64_t n);
+ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out, cudaStream_t st);
 // take.cu
 ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, int64_t vlen, int idx_width, int idx_signed,
                              const void* idx, const uint8_t* ivalid, int64_t ioff, int64_t n, int bounds_check, void* out, uint8_t* out_valid,

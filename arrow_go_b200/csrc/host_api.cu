@@ -724,6 +724,43 @@ ag_status ag_sort_indices(int type, const void* vals, const uint8_t* valid, int6
   return sync(cs);
 }
 
+ag_status ag_sort_indices_keys(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* out) {
+  AG_TRY(ensure_init());
+  AG_TRY(sort_indices_keys_check(nkeys, keys, n));
+  if (n == 0) return AG_OK;
+  if (!out) AG_FAIL(AG_ERR_INVALID, "sort_indices: NULL output");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  std::vector<ag_sort_key> dkeys(keys, keys + nkeys);
+  std::vector<std::vector<ag_sort_chunk>> dchunks(nkeys);
+  for (int j = 0; j < nkeys; ++j) {
+    for (int c = 0; c < keys[j].nchunks; ++c) {
+      const ag_sort_chunk& ch = keys[j].chunks[c];
+      ag_sort_chunk d{nullptr, nullptr, 0, ch.length};
+      if (ch.length > 0) {
+        uint8_t* dvalid;
+        if (keys[j].type == AG_TYPE_BOOL) {
+          uint8_t* dv;
+          AG_TRY(upload_bitmap(t, (const uint8_t*)ch.vals, ch.offset, ch.length, &dv, &d.offset));
+          d.vals = dv;
+          int64_t phase;
+          AG_TRY(upload_bitmap(t, ch.valid, ch.offset, ch.length, &dvalid, &phase));
+        } else {
+          AG_TRY(upload_column(t, ch.vals, ch.valid, ch.offset, ch.length, type_width(keys[j].type), &d.vals, &dvalid, &d.offset));
+        }
+        d.valid = dvalid;
+      }
+      dchunks[j].push_back(d);
+    }
+    dkeys[j].chunks = dchunks[j].data();
+  }
+  uint64_t* dout;
+  AG_TRY(t.alloc_t(&dout, (size_t)n * 8));
+  AG_TRY(sort_indices_keys_dev(nkeys, dkeys.data(), n, dout, cs));
+  AG_TRY(d2h(out, dout, (size_t)n * 8, cs));
+  return sync(cs);
+}
+
 ag_status ag_is_in(int bit_width, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, const void* set_vals,
                    const uint8_t* set_valid, int64_t set_offset, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid,
                    int64_t* out_nulls) {

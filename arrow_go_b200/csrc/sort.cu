@@ -29,6 +29,7 @@
 #include "common.cuh"
 
 #include <string.h>
+#include <algorithm>
 #include <type_traits>
 #include <vector>
 
@@ -358,24 +359,33 @@ sort_class_scatter_kernel(const SortSource src, const SortXform xf, const unsign
 }
 
 // ---------------------------------------------------------------- K2: digit passes
-// kFromSource: the pass reads the column itself (no NaN / null rows: pair i is (key(vals[i]), i)), otherwise the pair
-// buffers of the previous pass.  T is only used with kFromSource.
-template <typename T, typename K, bool kFromSource>
-__device__ __forceinline__ K pass_key(const SortSource& src, const SortXform& xf, const K* __restrict__ keys, int64_t lo, int64_t i) {
-  if constexpr (kFromSource) {
+// Where a pass reads its (key, row) pairs:
+//   kPairs       the pair buffers of the previous pass;
+//   kFromSource  the column itself (no NaN / null rows: pair i is (key(vals[i]), i));
+//   kFromWords   a packed key word of the multi-key sort, in row order: pair i is (words[i], i);
+//   kGather      the next packed key word, through the permutation so far: pair i is (words[row_i], row_i) with row_i
+//                from the pair buffers of the previous pass (an 8-byte random read per row).
+// T is only used with kFromSource.
+constexpr int kPairs = 0, kFromSource = 1, kFromWords = 2, kGather = 3;
+template <typename T, typename K, int kMode>
+__device__ __forceinline__ K pass_key(const SortSource& src, const SortXform& xf, const K* __restrict__ keys, const unsigned* __restrict__ idx,
+                                      int64_t lo, int64_t i) {
+  if constexpr (kMode == kFromSource) {
     int cls;
     const K k = sort_key<T, K>(__ldcs(reinterpret_cast<const T*>(src.vals) + src.voff + i), src.descending, &cls);
     return (K)((k - (K)xf.kmin) >> xf.tz);
+  } else if constexpr (kMode == kGather) {
+    return __ldg(keys + __ldcs(idx + lo + i));
   } else {
     return __ldcs(keys + lo + i);
   }
 }
 
 // tot[256]: per-bin totals of the pass (zeroed by the host), accumulated per block and flushed once
-template <typename T, typename K, bool kFromSource>
+template <typename T, typename K, int kMode>
 __global__ void __launch_bounds__(kSoThreads)
-sort_digit_hist_kernel(const SortSource src, const SortXform xf, const K* __restrict__ keys, int64_t lo, int64_t n, int shift,
-                       unsigned* __restrict__ tile_hist, int64_t ntiles, unsigned* __restrict__ tot) {
+sort_digit_hist_kernel(const SortSource src, const SortXform xf, const K* __restrict__ keys, const unsigned* __restrict__ idx, int64_t lo, int64_t n,
+                       int shift, unsigned* __restrict__ tile_hist, int64_t ntiles, unsigned* __restrict__ tot) {
   __shared__ unsigned s_h[kSoBins];
   unsigned acc = 0;                      // thread b < 256: rows of digit b in this block's tiles
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -385,7 +395,7 @@ sort_digit_hist_kernel(const SortSource src, const SortXform xf, const K* __rest
 #pragma unroll
     for (int e = 0; e < kSoPerThread; ++e) {      // every load of the tile in flight before the first atomic
       const int64_t i = tile * kSoTile + e * kSoThreads + threadIdx.x;
-      kk[e] = i < n ? pass_key<T, K, kFromSource>(src, xf, keys, lo, i) : (K)0;
+      kk[e] = i < n ? pass_key<T, K, kMode>(src, xf, keys, idx, lo, i) : (K)0;
     }
 #pragma unroll
     for (int e = 0; e < kSoPerThread; ++e) {
@@ -408,7 +418,7 @@ sort_digit_hist_kernel(const SortSource src, const SortXform xf, const K* __rest
 // are consecutive there AND consecutive in the destination, so the global writes are contiguous runs issued by
 // neighbouring lanes instead of 16 isolated 8-byte stores per bin.
 // kLast: the final pass writes the uint64 row indices into `out64` (positions are absolute) and drops the keys.
-template <typename T, typename K, bool kFromSource, bool kLast>
+template <typename T, typename K, int kMode, bool kLast>
 __global__ void __launch_bounds__(kSoThreads, 2)     // 64 registers: two 512-thread blocks per SM (71 in one variant left one)
 sort_digit_scatter_kernel(const SortSource src, const SortXform xf, const K* __restrict__ keys_in, const unsigned* __restrict__ idx_in, int64_t lo,
                           int64_t n, int shift, const unsigned* __restrict__ tile_off, int64_t ntiles, K* __restrict__ keys_out,
@@ -438,8 +448,13 @@ sort_digit_scatter_kernel(const SortSource src, const SortXform xf, const K* __r
       live[e] = kFull || i < n;
       key[e] = 0; idx[e] = 0; digits[e] = 0;
       if (live[e]) {
-        key[e] = pass_key<T, K, kFromSource>(src, xf, keys_in, lo, i);
-        idx[e] = kFromSource ? (unsigned)i : __ldcs(idx_in + lo + i);
+        if constexpr (kMode == kGather) {
+          idx[e] = __ldcs(idx_in + lo + i);
+          key[e] = __ldg(keys_in + idx[e]);
+        } else {
+          key[e] = pass_key<T, K, kMode>(src, xf, keys_in, idx_in, lo, i);
+          idx[e] = (kMode == kFromSource || kMode == kFromWords) ? (unsigned)i : __ldcs(idx_in + lo + i);
+        }
         digits[e] = (int)((key[e] >> shift) & 0xff);
       }
     }
@@ -501,17 +516,17 @@ sort_iota_kernel(int64_t n, unsigned long long* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * kSoThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kSoThreads) out[i] = (unsigned long long)i;
 }
 
-template <typename T, typename K, bool kFromSource>
+template <typename T, typename K, int kMode>
 static ag_status launch_digit_pass(const SortSource& src, const SortXform& xf, const K* keys_in, const unsigned* idx_in, int64_t lo, int64_t fn, int shift,
                                    unsigned* tile_hist, unsigned* seg_sums, unsigned* tot, K* keys_out, unsigned* idx_out, unsigned long long* out64,
                                    bool last, cudaStream_t st) {
   constexpr size_t kScatterSmem = (sizeof(K) + 4) * (size_t)kSoTile + (size_t)kSoWarps * 256 * 4;
   static std::atomic<unsigned> attr_a{0u}, attr_b{0u};   // per instantiation, one bit per device
-  AG_TRY(ensure_dynamic_smem((const void*)sort_digit_scatter_kernel<T, K, kFromSource, false>, (int)kScatterSmem, &attr_a));
-  AG_TRY(ensure_dynamic_smem((const void*)sort_digit_scatter_kernel<T, K, kFromSource, true>, (int)kScatterSmem, &attr_b));
+  AG_TRY(ensure_dynamic_smem((const void*)sort_digit_scatter_kernel<T, K, kMode, false>, (int)kScatterSmem, &attr_a));
+  AG_TRY(ensure_dynamic_smem((const void*)sort_digit_scatter_kernel<T, K, kMode, true>, (int)kScatterSmem, &attr_b));
   const int64_t ftiles = (fn + kSoTile - 1) / kSoTile;
   const int fgrid = grid_for(fn, kSoTile, 8);
-  sort_digit_hist_kernel<T, K, kFromSource><<<fgrid, kSoThreads, 0, st>>>(src, xf, keys_in, lo, fn, shift, tile_hist, ftiles, tot);
+  sort_digit_hist_kernel<T, K, kMode><<<fgrid, kSoThreads, 0, st>>>(src, xf, keys_in, idx_in, lo, fn, shift, tile_hist, ftiles, tot);
   AG_TRY(check_launch("sort_digit_hist_kernel"));
   int64_t nseg = 2 * (int64_t)sm_count();
   if (nseg > ftiles) nseg = ftiles;
@@ -522,9 +537,9 @@ static ag_status launch_digit_pass(const SortSource& src, const SortXform& xf, c
   sort_digit_apply_kernel<<<(int)nseg, kSoSegThreads, 0, st>>>(tile_hist, ftiles, tps, seg_sums, tot);
   AG_TRY(check_launch("sort_digit_apply_kernel"));
   if (last)
-    sort_digit_scatter_kernel<T, K, kFromSource, true><<<fgrid, kSoThreads, kScatterSmem, st>>>(src, xf, keys_in, idx_in, lo, fn, shift, tile_hist, ftiles, keys_out, idx_out, out64);
+    sort_digit_scatter_kernel<T, K, kMode, true><<<fgrid, kSoThreads, kScatterSmem, st>>>(src, xf, keys_in, idx_in, lo, fn, shift, tile_hist, ftiles, keys_out, idx_out, out64);
   else
-    sort_digit_scatter_kernel<T, K, kFromSource, false><<<fgrid, kSoThreads, kScatterSmem, st>>>(src, xf, keys_in, idx_in, lo, fn, shift, tile_hist, ftiles, keys_out, idx_out, out64);
+    sort_digit_scatter_kernel<T, K, kMode, false><<<fgrid, kSoThreads, kScatterSmem, st>>>(src, xf, keys_in, idx_in, lo, fn, shift, tile_hist, ftiles, keys_out, idx_out, out64);
   return check_launch("sort_digit_scatter_kernel");
 }
 
@@ -594,9 +609,9 @@ static ag_status sort_indices_t(const SortSource& src, unsigned long long* d_out
     for (int d = 0; d < nd; ++d) {
       const bool last = d == nd - 1;
       if (d == 0 && !classes)
-        rc = launch_digit_pass<T, K, true>(src, xf, nullptr, nullptr, 0, fn, 0, tile_hist, d_seg, d_tot, keys[0], idx[0], d_out, last, st);
+        rc = launch_digit_pass<T, K, kFromSource>(src, xf, nullptr, nullptr, 0, fn, 0, tile_hist, d_seg, d_tot, keys[0], idx[0], d_out, last, st);
       else
-        rc = launch_digit_pass<K, K, false>(src, xf, keys[cur], idx[cur], fin_lo, fn, 8 * d, tile_hist, d_seg, d_tot + (size_t)d * 256, keys[cur ^ 1], idx[cur ^ 1], d_out, last, st);
+        rc = launch_digit_pass<K, K, kPairs>(src, xf, keys[cur], idx[cur], fin_lo, fn, 8 * d, tile_hist, d_seg, d_tot + (size_t)d * 256, keys[cur ^ 1], idx[cur ^ 1], d_out, last, st);
       if (rc != AG_OK) break;
       if (!(d == 0 && !classes)) cur ^= 1;     // a source pass writes buffer 0
     }
@@ -636,6 +651,368 @@ ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int
   }, [&] { AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: unsupported type id %d (fixed-width numeric columns only)", type); });
 }
 
+// ================================================================ several keys over chunked columns
+// The keys of a row are packed into one B-bit integer whose ascending order is the lexicographic order of the keys, and
+// the digit passes above sort that integer.  Key j contributes, most significant key first, the field
+//     class code (0..2 bits) | value (vbits)
+// class code: the row's class among {finite, NaN, null} numbered in placement order over the classes the column holds
+// (one class: no bits); value: (key' - min key') >> tz for finite rows (the transform of the single-key sort), 0 for
+// NaN and null rows, so that those tie on the key and fall through to the next one.
+//   P0  one launch (blockIdx.y = key): min / max / OR / AND of key' over the finite rows, NaN and null rows of every key
+//       -> one read-back so the host can size the fields;
+//   P1  one launch: every row's packed key, written once as W = ceil(B/64) uint64 words (one uint32 word if B <= 32);
+//   P2+ the digit passes, least significant digit of word 0 first; the first pass of every later word gathers that word
+//       through the permutation so far (kGather), the last pass writes the uint64 row indices.
+// Rows are numbered across chunks.  Both kernels walk a span table: the row ranges inside which every key column stays
+// in one chunk (cut wherever a chunk of any key ends, like IterateExecSpans); a tile of 4096 rows never crosses a span
+// and blocks find their span by binary search over the spans' first tiles, so a table of many small chunks is still
+// one launch per kernel.
+struct SkChunk { const void* vals; const uint8_t* valid; int64_t offset; int64_t row0; };   // row0: first row of the chunk
+struct SkSpan { int64_t row0; int64_t len; int64_t first_tile; };
+struct SkKey {
+  int type, descending;
+  int cls_bits, vbits, tz;
+  int code[3];                  // class code of finite / NaN / null rows
+  unsigned long long kmin;
+};
+constexpr int kSkStats = 8;     // per key: [0] min, [1] max, [2] OR, [3] AND of key' (finite rows), [4] NaN rows, [5] null rows
+
+// key' of element li (offset included) of a chunk; *cls = 0 finite, 1 NaN, 2 null.  BOOL: the data bit.
+__device__ __forceinline__ unsigned long long sk_load(int type, const SkChunk& c, int64_t li, int descending, int* cls) {
+  using U = unsigned long long;
+  U k = 0;
+  *cls = 0;
+  switch (type) {
+    case AG_TYPE_BOOL: k = (U)bit_is_set(reinterpret_cast<const uint8_t*>(c.vals), li) ^ (U)(descending != 0); break;
+    case AG_TYPE_UINT8: k = sort_key<uint8_t, U>(reinterpret_cast<const uint8_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_INT8: k = sort_key<int8_t, U>(reinterpret_cast<const int8_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_UINT16: k = sort_key<uint16_t, U>(reinterpret_cast<const uint16_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_INT16: k = sort_key<int16_t, U>(reinterpret_cast<const int16_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_UINT32: k = sort_key<uint32_t, U>(reinterpret_cast<const uint32_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_INT32: k = sort_key<int32_t, U>(reinterpret_cast<const int32_t*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_UINT64: k = sort_key<U, U>(reinterpret_cast<const U*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_INT64: k = sort_key<long long, U>(reinterpret_cast<const long long*>(c.vals)[li], descending, cls); break;
+    case AG_TYPE_FLOAT32: k = sort_key<float, U>(reinterpret_cast<const float*>(c.vals)[li], descending, cls); break;
+    default: k = sort_key<double, U>(reinterpret_cast<const double*>(c.vals)[li], descending, cls); break;
+  }
+  if (c.valid && !bit_is_set(c.valid, li)) *cls = 2;
+  return k;
+}
+
+// the span of a tile: the last span whose first tile is <= tile
+__device__ __forceinline__ int sk_span_of(const SkSpan* __restrict__ spans, int nspans, int64_t tile) {
+  int lo = 0, hi = nspans - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (spans[mid].first_tile <= tile) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// P0.  span_chunk[s * nkeys + j]: the chunk (index into `chunks`) of key j over span s.
+__global__ void __launch_bounds__(kSoThreads)
+sort_keys_prep_kernel(const SkKey* __restrict__ keys, const SkChunk* __restrict__ chunks, const SkSpan* __restrict__ spans,
+                      const int* __restrict__ span_chunk, int nspans, int nkeys, int64_t ntiles, unsigned long long* __restrict__ stats) {
+  const int j = blockIdx.y;
+  const int type = keys[j].type, descending = keys[j].descending;
+  unsigned long long mn = ~0ull, mx = 0, vor = 0, vand = ~0ull;
+  unsigned n_nan = 0, n_null = 0;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int s = sk_span_of(spans, nspans, tile);
+    const SkSpan sp = spans[s];
+    const SkChunk c = chunks[span_chunk[(int64_t)s * nkeys + j]];
+    const int64_t r0 = sp.row0 + (tile - sp.first_tile) * kSoTile;
+    const int64_t len = min((int64_t)kSoTile, sp.row0 + sp.len - r0);
+    const int64_t base = c.offset + (r0 - c.row0);
+#pragma unroll
+    for (int e = 0; e < kSoPerThread; ++e) {
+      const int64_t i = e * kSoThreads + threadIdx.x;
+      if (i < len) {
+        int cls;
+        const unsigned long long k = sk_load(type, c, base + i, descending, &cls);
+        if (cls == 0) { mn = k < mn ? k : mn; mx = k > mx ? k : mx; vor |= k; vand &= k; }
+        n_nan += cls == 1;
+        n_null += cls == 2;
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) {
+    const unsigned long long omn = __shfl_xor_sync(0xffffffffu, mn, m), omx = __shfl_xor_sync(0xffffffffu, mx, m);
+    mn = omn < mn ? omn : mn; mx = omx > mx ? omx : mx;
+    vor |= __shfl_xor_sync(0xffffffffu, vor, m);
+    vand &= __shfl_xor_sync(0xffffffffu, vand, m);
+    n_nan += __shfl_xor_sync(0xffffffffu, n_nan, m);
+    n_null += __shfl_xor_sync(0xffffffffu, n_null, m);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    unsigned long long* st = stats + (int64_t)j * kSkStats;
+    if (mn <= mx) {
+      atomicMin(&st[0], mn);
+      atomicMax(&st[1], mx);
+      atomicOr(&st[2], vor);
+      atomicAnd(&st[3], vand);
+    }
+    if (n_nan) atomicAdd(&st[4], (unsigned long long)n_nan);
+    if (n_null) atomicAdd(&st[5], (unsigned long long)n_null);
+  }
+}
+
+// P1.  Word w of row r is words[w * n + r]; fields are emitted from the least significant key up.
+template <typename W>
+__global__ void __launch_bounds__(kSoThreads, 2)
+sort_keys_pack_kernel(const SkKey* __restrict__ keys, const SkChunk* __restrict__ chunks, const SkSpan* __restrict__ spans,
+                      const int* __restrict__ span_chunk, int nspans, int nkeys, int64_t ntiles, int64_t n, W* __restrict__ words) {
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int s = sk_span_of(spans, nspans, tile);
+    const SkSpan sp = spans[s];
+    const int64_t r0 = sp.row0 + (tile - sp.first_tile) * kSoTile;
+    const int64_t len = min((int64_t)kSoTile, sp.row0 + sp.len - r0);
+    for (int e = 0; e < kSoPerThread; ++e) {
+      const int64_t i = e * kSoThreads + threadIdx.x;
+      if (i >= len) break;
+      const int64_t r = r0 + i;
+      unsigned long long cur = 0;
+      int sh = 0;
+      W* out = words + r;
+      // OR `width` (<= 64) bits of v in at bit `sh` of the current word; store each word once, when it is full
+      auto emit = [&](unsigned long long v, int width) {
+        if (width == 0) return;
+        cur |= v << sh;
+        if (sh + width >= 64) {
+          *out = (W)cur;
+          out += n;
+          cur = sh ? v >> (64 - sh) : 0ull;
+          sh = sh + width - 64;
+        } else {
+          sh += width;
+        }
+      };
+      for (int j = nkeys - 1; j >= 0; --j) {
+        const SkKey kd = keys[j];
+        if (kd.cls_bits + kd.vbits == 0) continue;
+        const SkChunk c = chunks[span_chunk[(int64_t)s * nkeys + j]];
+        int cls;
+        const unsigned long long k = sk_load(kd.type, c, c.offset + (r - c.row0), kd.descending, &cls);
+        emit(cls ? 0ull : (k - kd.kmin) >> kd.tz, kd.vbits);
+        emit((unsigned long long)(cls == 0 ? kd.code[0] : cls == 1 ? kd.code[1] : kd.code[2]), kd.cls_bits);
+      }
+      if (sh) *out = (W)cur;
+    }
+  }
+}
+
+namespace {
+struct SkPlan {
+  std::vector<SkKey> keys;
+  std::vector<SkChunk> chunks;
+  std::vector<SkSpan> spans;
+  std::vector<int> span_chunk;
+  int64_t ntiles = 0;
+};
+
+// Chunk table and span table of the keys (host only).  Empty chunks never own a span.
+static void sk_build_tables(int nkeys, const ag_sort_key* keys, int64_t n, SkPlan* p) {
+  std::vector<int> base(nkeys);
+  std::vector<int64_t> cuts;
+  for (int j = 0; j < nkeys; ++j) {
+    base[j] = (int)p->chunks.size();
+    int64_t row = 0;
+    for (int c = 0; c < keys[j].nchunks; ++c) {
+      const ag_sort_chunk& ch = keys[j].chunks[c];
+      p->chunks.push_back(SkChunk{ch.vals, ch.valid, ch.offset, row});
+      row += ch.length;
+      cuts.push_back(row);
+    }
+  }
+  std::sort(cuts.begin(), cuts.end());
+  cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
+  std::vector<int> at(nkeys, 0);   // current chunk of each key
+  int64_t row0 = 0;
+  for (int64_t cut : cuts) {
+    if (cut <= row0) continue;
+    const int64_t len = cut - row0;
+    p->spans.push_back(SkSpan{row0, len, p->ntiles});
+    p->ntiles += (len + kSoTile - 1) / kSoTile;
+    for (int j = 0; j < nkeys; ++j) {
+      while (keys[j].chunks[at[j]].length == 0 || p->chunks[base[j] + at[j]].row0 + keys[j].chunks[at[j]].length <= row0) ++at[j];
+      p->span_chunk.push_back(base[j] + at[j]);
+    }
+    row0 = cut;
+  }
+  (void)n;
+}
+
+static int bit_length(unsigned long long v) { int b = 0; while (v) { ++b; v >>= 1; } return b; }
+}  // namespace
+
+// The digit passes over the packed words.  K = uint32 when the key fits 32 bits (one word), else uint64.
+template <typename K>
+static ag_status sk_digit_passes(const K* words, int64_t n, int bits, char* body, size_t words_bytes, unsigned* d_tot, unsigned* d_seg,
+                                 unsigned long long* d_out, cudaStream_t st) {
+  const size_t key_bytes = ((size_t)n * sizeof(K) + 255) & ~(size_t)255;
+  const size_t idx_bytes = ((size_t)n * 4 + 255) & ~(size_t)255;
+  K* keys[2] = {reinterpret_cast<K*>(body + words_bytes), reinterpret_cast<K*>(body + words_bytes + key_bytes)};
+  unsigned* idx[2] = {reinterpret_cast<unsigned*>(body + words_bytes + 2 * key_bytes), reinterpret_cast<unsigned*>(body + words_bytes + 2 * key_bytes + idx_bytes)};
+  unsigned* tile_hist = reinterpret_cast<unsigned*>(body + words_bytes + 2 * key_bytes + 2 * idx_bytes);
+  const SortSource none{nullptr, nullptr, 0, n, 0, 0};
+  const SortXform xf{0, 0};
+  const int nwords = (bits + 8 * (int)sizeof(K) - 1) / (8 * (int)sizeof(K));
+  int pass = 0, cur = 0;
+  const int npasses = [&] { int t = 0; for (int w = 0; w < nwords; ++w) t += (std::min(bits - 64 * w, 8 * (int)sizeof(K)) + 7) / 8; return t; }();
+  for (int w = 0; w < nwords; ++w) {
+    const K* word = words + (size_t)w * n;
+    const int nd = (std::min(bits - 64 * w, 8 * (int)sizeof(K)) + 7) / 8;
+    for (int d = 0; d < nd; ++d, ++pass) {
+      const bool last = pass == npasses - 1;
+      unsigned* tot = d_tot + (size_t)pass * 256;
+      if (pass == 0) {
+        AG_TRY((launch_digit_pass<K, K, kFromWords>(none, xf, word, nullptr, 0, n, 0, tile_hist, d_seg, tot, keys[0], idx[0], d_out, last, st)));
+        continue;     // the first pass writes buffer 0
+      }
+      if constexpr (sizeof(K) == 8) {   // a 32-bit key is one word: nothing to gather
+        if (d == 0) {
+          AG_TRY((launch_digit_pass<K, K, kGather>(none, xf, word, idx[cur], 0, n, 0, tile_hist, d_seg, tot, keys[cur ^ 1], idx[cur ^ 1], d_out, last, st)));
+          cur ^= 1;
+          continue;
+        }
+      }
+      AG_TRY((launch_digit_pass<K, K, kPairs>(none, xf, keys[cur], idx[cur], 0, n, 8 * d, tile_hist, d_seg, tot, keys[cur ^ 1], idx[cur ^ 1], d_out, last, st)));
+      cur ^= 1;
+    }
+  }
+  return AG_OK;
+}
+
+ag_status sort_indices_keys_check(int nkeys, const ag_sort_key* keys, int64_t n) {
+  if (nkeys < 1 || !keys) AG_FAIL(AG_ERR_INVALID, "sort_indices: must provide at least one sort key");
+  if (n < 0) AG_FAIL(AG_ERR_INVALID, "sort_indices: negative length");
+  for (int j = 0; j < nkeys; ++j) {
+    const ag_sort_key& k = keys[j];
+    if (k.order != 0 && k.order != 1) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: order must be 0 (ascending) or 1 (descending)", j);
+    if (k.null_placement != 0 && k.null_placement != 1) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: null placement must be 0 (at end) or 1 (at start)", j);
+    if (k.nchunks < 0 || (k.nchunks > 0 && !k.chunks)) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: bad chunk list", j);
+    int64_t rows = 0;
+    for (int c = 0; c < k.nchunks; ++c) {
+      const ag_sort_chunk& ch = k.chunks[c];
+      if (ch.offset < 0 || ch.length < 0) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: negative chunk offset or length", j);
+      if (ch.length > 0 && !ch.vals) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: NULL chunk values", j);
+      rows += ch.length;
+    }
+    if (rows != n) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: chunk row count %lld does not match column length %lld", j, (long long)rows, (long long)n);
+    if (k.type != AG_TYPE_BOOL && type_width(k.type) == 0)
+      AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: sort key %d: unsupported type id %d (boolean and numeric columns only)", j, k.type);
+  }
+  if (n >= (1ll << 32)) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: more than 2^32-1 rows per call");
+  return AG_OK;
+}
+
+ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out, cudaStream_t st) {
+  AG_TRY(sort_indices_keys_check(nkeys, keys, n));
+  if (n == 0) return AG_OK;
+  if (!d_out) AG_FAIL(AG_ERR_INVALID, "sort_indices: NULL output");
+
+  SkPlan p;
+  sk_build_tables(nkeys, keys, n, &p);
+  for (int j = 0; j < nkeys; ++j) {
+    SkKey k{};
+    k.type = keys[j].type;
+    k.descending = keys[j].order;
+    p.keys.push_back(k);
+  }
+  // head: statistics | key plans | chunks | spans | span chunks; freed on every return path
+  const size_t o_keys = ((size_t)nkeys * kSkStats * 8 + 255) & ~(size_t)255;
+  const size_t o_chunks = o_keys + (((size_t)nkeys * sizeof(SkKey) + 255) & ~(size_t)255);
+  const size_t o_spans = o_chunks + ((p.chunks.size() * sizeof(SkChunk) + 255) & ~(size_t)255);
+  const size_t o_sc = o_spans + ((p.spans.size() * sizeof(SkSpan) + 255) & ~(size_t)255);
+  const size_t head_bytes = o_sc + p.span_chunk.size() * sizeof(int);
+  std::vector<unsigned long long> h(head_bytes / 8 + 1, 0);   // staged as one host image, one copy
+  char* hb = reinterpret_cast<char*>(h.data());
+  for (int j = 0; j < nkeys; ++j) { h[j * kSkStats + 0] = ~0ull; h[j * kSkStats + 3] = ~0ull; }
+  memcpy(hb + o_chunks, p.chunks.data(), p.chunks.size() * sizeof(SkChunk));
+  memcpy(hb + o_spans, p.spans.data(), p.spans.size() * sizeof(SkSpan));
+  memcpy(hb + o_sc, p.span_chunk.data(), p.span_chunk.size() * sizeof(int));
+  void* head = nullptr;
+  void* body = nullptr;
+  AG_TRY(dev_alloc_async(&head, head_bytes, st));
+  char* hd = reinterpret_cast<char*>(head);
+  unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(hd);
+  SkKey* d_keys = reinterpret_cast<SkKey*>(hd + o_keys);
+  const SkChunk* d_chunks = reinterpret_cast<const SkChunk*>(hd + o_chunks);
+  const SkSpan* d_spans = reinterpret_cast<const SkSpan*>(hd + o_spans);
+  const int* d_sc = reinterpret_cast<const int*>(hd + o_sc);
+  const int nspans = (int)p.spans.size();
+  unsigned long long* out = reinterpret_cast<unsigned long long*>(d_out);
+  ag_status rc = AG_OK;
+  do {
+    memcpy(hb + o_keys, p.keys.data(), (size_t)nkeys * sizeof(SkKey));
+    if (cudaMemcpyAsync(head, hb, head_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "sort key tables", __FILE__, __LINE__); break; }
+    // ---- P0: statistics of every key, one read-back
+    const dim3 pgrid((unsigned)grid_for(n, kSoTile, std::max(1, 8 / nkeys)), (unsigned)nkeys);
+    sort_keys_prep_kernel<<<pgrid, kSoThreads, 0, st>>>(d_keys, d_chunks, d_spans, d_sc, nspans, nkeys, p.ntiles, d_stats);
+    if ((rc = check_launch("sort_keys_prep_kernel")) != AG_OK) break;
+    std::vector<unsigned long long> hs((size_t)nkeys * kSkStats);
+    if (cudaMemcpyAsync(hs.data(), d_stats, hs.size() * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "statistics read-back", __FILE__, __LINE__); break; }
+    // ---- plan: the field of every key
+    int bits = 0;
+    for (int j = 0; j < nkeys; ++j) {
+      SkKey& k = p.keys[j];
+      const unsigned long long* s = &hs[(size_t)j * kSkStats];
+      const unsigned long long n_nan = s[4], n_null = s[5], n_fin = (unsigned long long)n - n_nan - n_null;
+      // classes in placement order (NullsAtEnd: finite, NaN, null; NullsAtStart: null, NaN, finite), absent ones skipped
+      const int order[3] = {keys[j].null_placement ? 2 : 0, 1, keys[j].null_placement ? 0 : 2};
+      const unsigned long long count[3] = {n_fin, n_nan, n_null};
+      int present = 0;
+      for (int c : order) if (count[c]) k.code[c] = present++;
+      k.cls_bits = present == 3 ? 2 : present == 2 ? 1 : 0;
+      if (n_fin > 1 && s[1] > s[0]) {
+        k.kmin = s[0];
+        const unsigned long long varying = s[2] ^ s[3];
+        while (!((varying >> k.tz) & 1ull)) ++k.tz;
+        k.vbits = bit_length((s[1] - s[0]) >> k.tz);
+      }
+      bits += k.cls_bits + k.vbits;
+    }
+    if (bits == 0) {   // every row ties on every key
+      sort_iota_kernel<<<grid_for(n, kSoThreads * 8, 8), kSoThreads, 0, st>>>(n, out);
+      rc = check_launch("sort_iota_kernel");
+      break;
+    }
+    memcpy(hb + o_keys, p.keys.data(), (size_t)nkeys * sizeof(SkKey));
+    if (cudaMemcpyAsync(d_keys, hb + o_keys, (size_t)nkeys * sizeof(SkKey), cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "sort key plans", __FILE__, __LINE__); break; }
+    // body: totals of every pass | segment sums | packed words | pairs x2 | indices x2 | tile histograms
+    const bool narrow = bits <= 32;
+    const size_t kw = narrow ? 4 : 8;
+    const int nwords = narrow ? 1 : (bits + 63) / 64;
+    const int npasses_max = nwords * 8;
+    const size_t tot_bytes = ((size_t)npasses_max * 256 * 4 + 255) & ~(size_t)255;
+    const size_t seg_bytes = ((size_t)2 * sm_count() * 256 * 4 + 255) & ~(size_t)255;
+    const size_t words_bytes = ((size_t)nwords * n * kw + 255) & ~(size_t)255;
+    const size_t pair_bytes = 2 * (((size_t)n * kw + 255) & ~(size_t)255) + 2 * (((size_t)n * 4 + 255) & ~(size_t)255);
+    const int64_t ntiles = (n + kSoTile - 1) / kSoTile;
+    const size_t th_bytes = (size_t)256 * ntiles * 4;
+    if ((rc = dev_alloc_async(&body, tot_bytes + seg_bytes + words_bytes + pair_bytes + th_bytes, st)) != AG_OK) break;
+    char* bd = reinterpret_cast<char*>(body);
+    unsigned* d_tot = reinterpret_cast<unsigned*>(bd);
+    unsigned* d_seg = reinterpret_cast<unsigned*>(bd + tot_bytes);
+    char* wbase = bd + tot_bytes + seg_bytes;
+    if (cudaMemsetAsync(d_tot, 0, tot_bytes, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "pass totals", __FILE__, __LINE__); break; }
+    // ---- P1: pack
+    const int grid = grid_for(p.ntiles * kSoTile, kSoTile, 8);
+    if (narrow) sort_keys_pack_kernel<uint32_t><<<grid, kSoThreads, 0, st>>>(d_keys, d_chunks, d_spans, d_sc, nspans, nkeys, p.ntiles, n, reinterpret_cast<uint32_t*>(wbase));
+    else sort_keys_pack_kernel<unsigned long long><<<grid, kSoThreads, 0, st>>>(d_keys, d_chunks, d_spans, d_sc, nspans, nkeys, p.ntiles, n, reinterpret_cast<unsigned long long*>(wbase));
+    if ((rc = check_launch("sort_keys_pack_kernel")) != AG_OK) break;
+    // ---- P2+: digit passes
+    if (narrow) rc = sk_digit_passes<uint32_t>(reinterpret_cast<const uint32_t*>(wbase), n, bits, wbase, words_bytes, d_tot, d_seg, out, st);
+    else rc = sk_digit_passes<unsigned long long>(reinterpret_cast<const unsigned long long*>(wbase), n, bits, wbase, words_bytes, d_tot, d_seg, out, st);
+  } while (0);
+  const ag_status frc_body = body ? dev_free_async(body, st) : AG_OK;
+  const ag_status frc = dev_free_async(head, st);
+  if (rc != AG_OK) return rc;
+  return frc_body != AG_OK ? frc_body : frc;
+}
+
 }  // namespace ag
 
 using namespace ag;
@@ -644,4 +1021,9 @@ extern "C" ag_status ag_sort_indices_dev(int type, const void* d_vals, const uin
                                          int null_placement, uint64_t* d_out, int64_t* null_count, int64_t* nan_count, ag_stream_t s) {
   AG_TRY(ensure_init());
   return sort_indices_dev(type, d_vals, d_valid, offset, n, order, null_placement, d_out, null_count, nan_count, resolve_stream(s));
+}
+
+extern "C" ag_status ag_sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  return sort_indices_keys_dev(nkeys, keys, n, d_out, resolve_stream(s));
 }

@@ -113,6 +113,14 @@ struct ChunkedArray {  // arrow.Chunked (arrow/table.go:135-143)
   int64_t NullN() const;
 };
 
+// arrow.RecordBatch (arrow/record.go) and arrow.Table (arrow/table.go) as the columns they hold.  ipc::FileReader reads
+// into the same RecordBatch, so a batch it returns can be passed to any function that takes one.
+struct RecordBatch { int64_t num_rows = 0; std::vector<std::shared_ptr<ArrayData>> columns; };
+struct Table { int64_t num_rows = 0; std::vector<std::shared_ptr<ChunkedArray>> columns; };
+// Check that every column holds num_rows rows (array.NewRecordBatch / array.NewTable), ErrInvalid otherwise.
+Status MakeRecordBatch(int64_t num_rows, std::vector<std::shared_ptr<ArrayData>> columns, std::shared_ptr<RecordBatch>* out);
+Status MakeTable(int64_t num_rows, std::vector<std::shared_ptr<ChunkedArray>> columns, std::shared_ptr<Table>* out);
+
 struct Scalar {  // scalar.PrimitiveScalar: Data() is the raw little-endian value
   Type type = Type::NA;
   bool valid = false;
@@ -121,19 +129,24 @@ struct Scalar {  // scalar.PrimitiveScalar: Data() is the raw little-endian valu
 
 namespace compute {
 
-enum class DatumKind { NONE, SCALAR, ARRAY, CHUNKED };  // datum.go KindScalar/KindArray/KindChunked
+// datum.go KindScalar/KindArray/KindChunked/KindRecord/KindTable (RECORD and TABLE after CHUNKED: the values before stay)
+enum class DatumKind { NONE, SCALAR, ARRAY, CHUNKED, RECORD, TABLE };
 
 struct Datum {
   DatumKind kind = DatumKind::NONE;
   std::shared_ptr<Scalar> scalar;
   std::shared_ptr<ArrayData> array;
   std::shared_ptr<ChunkedArray> chunked;
+  std::shared_ptr<RecordBatch> record;
+  std::shared_ptr<Table> table;
   Datum() = default;
   explicit Datum(std::shared_ptr<ArrayData> a) : kind(DatumKind::ARRAY), array(std::move(a)) {}
   explicit Datum(std::shared_ptr<ChunkedArray> c) : kind(DatumKind::CHUNKED), chunked(std::move(c)) {}
   explicit Datum(std::shared_ptr<Scalar> s) : kind(DatumKind::SCALAR), scalar(std::move(s)) {}
-  Type type() const;
-  int64_t Len() const;  // -1 for scalars (datum.go: scalars have no length)
+  explicit Datum(std::shared_ptr<RecordBatch> r) : kind(DatumKind::RECORD), record(std::move(r)) {}
+  explicit Datum(std::shared_ptr<Table> t) : kind(DatumKind::TABLE), table(std::move(t)) {}
+  Type type() const;    // NA for record batches and tables
+  int64_t Len() const;  // -1 for scalars (datum.go: scalars have no length); the row count of a record batch or table
 };
 
 }  // namespace compute
@@ -272,6 +285,15 @@ struct RunEndEncodeOptions : FunctionOptions {                                //
   Type RunEndType = Type::INT32;   // INT16, INT32 or INT64
   const char* TypeName() const override { return "RunEndEncodeOptions"; }
 };
+struct SortKey {                                              // kernels/vector_sort.go:56-61
+  int ColumnIndex = 0;
+  SortOrder Order = Ascending;
+  NullPlacement Placement = NullsAtEnd;
+};
+struct SortKeys : FunctionOptions {                           // compute.SortOptions, vector_sort.go:94-98
+  std::vector<SortKey> Keys;
+  const char* TypeName() const override { return "SortKeys"; }
+};
 struct SetLookupOptions : FunctionOptions {                   // compute/scalar_set_lookup.go (ValueSet, NullBehavior)
   std::shared_ptr<ArrayData> ValueSet;
   NullMatchingBehavior NullBehavior = NullMatchingMatch;
@@ -371,6 +393,12 @@ Status Filter(const ExecCtx& ctx, const Datum& values, const Datum& filter, cons
 Status Take(const ExecCtx& ctx, const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out);
 // compute.SortIndices (vector_sort.go:205-211), compute.Unique (vector_hash.go), compute.IsIn (scalar_set_lookup.go)
 Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortOptions& opts, Datum* out);
+// With SortKeys (sortIndicesImpl, vector_sort.go:117-200): arrays and chunked arrays use the first key (ColumnIndex
+// ignored), record batches and tables sort lexicographically by every key; BOOL and numeric key columns.
+Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortKeys& keys, Datum* out);
+// vector_sort.go:240-271
+Status SortIndicesRecordBatch(const ExecCtx& ctx, const std::shared_ptr<RecordBatch>& batch, const std::vector<SortKey>& keys, Datum* out);
+Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, const std::vector<SortKey>& keys, Datum* out);
 Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out);
 // compute.DictionaryEncode (vector_hash.go:105-121): Dictionary<int32, T>; a chunked input gets ONE dictionary for all
 // chunks and loses its empty chunks; a dictionary input is returned as it is
@@ -412,7 +440,7 @@ namespace ipc {
 struct Field { std::string name; Type type = Type::NA; bool nullable = false; };   // arrow.Field of a numeric / boolean column
 // Where a column's buffers sit inside its record batch body (offsets relative to the body; -1 = no buffer).
 struct ColumnLayout { int64_t length, null_count, validity_offset, validity_length, data_offset, data_length; };
-struct RecordBatch { int64_t num_rows = 0; std::vector<std::shared_ptr<ArrayData>> columns; };
+using arrowgpu::RecordBatch;
 
 class FileReader {
  public:

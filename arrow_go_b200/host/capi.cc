@@ -92,7 +92,8 @@ int agx_run_end_child(agx_datum* d, int which, agx_datum** out) {
 }
 int agx_dictionary_indices(agx_datum* d, agx_datum** out) {
   auto indices = [](const std::shared_ptr<ArrayData>& a) { auto r = std::make_shared<ArrayData>(*a); r->type = Type::INT32; r->dictionary = nullptr; return r; };
-  if (d->d.type() != Type::DICTIONARY) return fail(Status::TypeError("indices: not a dictionary datum"));
+  if ((d->d.kind != DatumKind::ARRAY && d->d.kind != DatumKind::CHUNKED) || d->d.type() != Type::DICTIONARY)
+    return fail(Status::TypeError("indices: not a dictionary array or chunked array"));
   if (d->d.kind == DatumKind::ARRAY) { *out = new agx_datum{Datum(indices(d->d.array))}; return AG_OK; }
   auto c = std::make_shared<ChunkedArray>(*d->d.chunked);
   c->type = Type::INT32; c->value_type = Type::NA;
@@ -101,7 +102,8 @@ int agx_dictionary_indices(agx_datum* d, agx_datum** out) {
   return AG_OK;
 }
 int agx_dictionary_values(agx_datum* d, agx_datum** out) {
-  if (d->d.type() != Type::DICTIONARY) return fail(Status::TypeError("dictionary: not a dictionary datum"));
+  if ((d->d.kind != DatumKind::ARRAY && d->d.kind != DatumKind::CHUNKED) || d->d.type() != Type::DICTIONARY)
+    return fail(Status::TypeError("dictionary: not a dictionary array or chunked array"));
   std::shared_ptr<ArrayData> dict;
   if (d->d.kind == DatumKind::ARRAY) dict = d->d.array->dictionary;
   else if (!d->d.chunked->chunks.empty()) dict = d->d.chunked->chunks[0]->dictionary;
@@ -169,6 +171,38 @@ int agx_cast(agx_datum* d, int to_type, int allow_int_overflow, int allow_float_
 // compute.SortIndices(SortOptions{Order, NullPlacement}) / compute.Unique / compute.IsIn(SetLookupOptions{ValueSet, NullBehavior})
 int agx_sort_indices(agx_datum* d, int order, int null_placement, agx_datum** out) {
   SortOptions o; o.Order = (SortOrder)order; o.Placement = (NullPlacement)null_placement;
+  ExecCtx ctx; Datum res;
+  AGX_TRY(CallFunction(ctx, "sort_indices", &o, {d->d}, &res));
+  *out = new agx_datum{res};
+  return AG_OK;
+}
+// array.NewRecordBatch over array datums / array.NewTable over chunked datums (every column num_rows rows)
+int agx_record_batch(int64_t num_rows, agx_datum** cols, int ncols, agx_datum** out) {
+  std::vector<std::shared_ptr<ArrayData>> c;
+  for (int i = 0; i < ncols; ++i) {
+    if (cols[i]->d.kind != DatumKind::ARRAY) return fail(Status::Invalid("record batch: columns must be arrays"));
+    c.push_back(cols[i]->d.array);
+  }
+  std::shared_ptr<RecordBatch> r;
+  AGX_TRY(MakeRecordBatch(num_rows, std::move(c), &r));
+  *out = new agx_datum{Datum(r)};
+  return AG_OK;
+}
+int agx_table(int64_t num_rows, agx_datum** cols, int ncols, agx_datum** out) {
+  std::vector<std::shared_ptr<ChunkedArray>> c;
+  for (int i = 0; i < ncols; ++i) {
+    if (cols[i]->d.kind != DatumKind::CHUNKED) return fail(Status::Invalid("table: columns must be chunked arrays"));
+    c.push_back(cols[i]->d.chunked);
+  }
+  std::shared_ptr<Table> t;
+  AGX_TRY(MakeTable(num_rows, std::move(c), &t));
+  *out = new agx_datum{Datum(t)};
+  return AG_OK;
+}
+// compute.SortIndices(SortKeys{{column[i], order[i], null_placement[i]}...}); nkeys may be 0 (an error of the function)
+int agx_sort_indices_keys(agx_datum* d, const int* columns, const int* orders, const int* null_placements, int nkeys, agx_datum** out) {
+  SortKeys o;
+  for (int i = 0; i < nkeys; ++i) o.Keys.push_back(SortKey{columns[i], (SortOrder)orders[i], (NullPlacement)null_placements[i]});
   ExecCtx ctx; Datum res;
   AGX_TRY(CallFunction(ctx, "sort_indices", &o, {d->d}, &res));
   *out = new agx_datum{res};

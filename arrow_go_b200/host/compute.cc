@@ -248,6 +248,29 @@ int64_t ChunkedArray::NullN() const {
   return n;
 }
 
+Status MakeRecordBatch(int64_t num_rows, std::vector<std::shared_ptr<ArrayData>> columns, std::shared_ptr<RecordBatch>* out) {
+  if (num_rows < 0) return Status::Invalid("record batch: negative row count");
+  for (size_t i = 0; i < columns.size(); ++i)
+    if (!columns[i] || columns[i]->length != num_rows)
+      return Status::Invalid("arrow/array: mismatch number of rows in column " + std::to_string(i) + ": got=" +
+                             std::to_string(columns[i] ? columns[i]->length : -1) + ", want=" + std::to_string(num_rows));
+  auto r = std::make_shared<RecordBatch>();
+  r->num_rows = num_rows; r->columns = std::move(columns);
+  *out = r;
+  return Status::OK();
+}
+Status MakeTable(int64_t num_rows, std::vector<std::shared_ptr<ChunkedArray>> columns, std::shared_ptr<Table>* out) {
+  if (num_rows < 0) return Status::Invalid("table: negative row count");
+  for (size_t i = 0; i < columns.size(); ++i)
+    if (!columns[i] || columns[i]->length != num_rows)
+      return Status::Invalid("arrow/array: column " + std::to_string(i) + " expected length " + std::to_string(num_rows) + " but got length " +
+                             std::to_string(columns[i] ? columns[i]->length : -1));
+  auto t = std::make_shared<Table>();
+  t->num_rows = num_rows; t->columns = std::move(columns);
+  *out = t;
+  return Status::OK();
+}
+
 namespace compute {
 Type Datum::type() const {
   switch (kind) {
@@ -261,6 +284,8 @@ int64_t Datum::Len() const {
   switch (kind) {
     case DatumKind::ARRAY: return array->length;
     case DatumKind::CHUNKED: return chunked->length;
+    case DatumKind::RECORD: return record->num_rows;
+    case DatumKind::TABLE: return table->num_rows;
     default: return -1;
   }
 }
@@ -781,6 +806,9 @@ Status CallFunction(const ExecCtx& ctx, const std::string& name, const FunctionO
   // through run_end_decode
   for (auto& a : args) {
     if (a.kind == DatumKind::NONE) continue;
+    // only sort_indices takes whole record batches and tables; the kernels of every other function take columns
+    if (name != "sort_indices" && (a.kind == DatumKind::RECORD || a.kind == DatumKind::TABLE))
+      return Status::NotImplemented("function '" + name + "' has no kernel for record batch or table arguments");
     if (name != "dictionary_encode" && a.type() == Type::DICTIONARY) return Status::NotImplemented("function '" + name + "' has no kernel for dictionary arguments");
     if (name != "run_end_decode" && a.type() == Type::RUN_END_ENCODED) return Status::NotImplemented("function '" + name + "' has no kernel for run-end encoded arguments");
   }
@@ -1573,6 +1601,9 @@ FunctionRegistry* GetFunctionRegistry() {
     reg->AddFunction(std::make_shared<MetaFunction>("sort_indices", 1, [](const ExecCtx& ctx, const FunctionOptions* fo, const std::vector<Datum>& args, Datum* out) -> Status {
       const auto* so = dynamic_cast<const SortOptions*>(fo);
       if (args.size() != 1) return Status::Invalid("sort_indices takes one argument");
+      if (const auto* sk = dynamic_cast<const SortKeys*>(fo)) return SortIndices(ctx, args[0], *sk, out);
+      if (args[0].kind == DatumKind::RECORD || args[0].kind == DatumKind::TABLE)
+        return Status::Invalid("sort_indices: record batches and tables are sorted with SortKeys options");
       return SortIndices(ctx, args[0], so ? *so : SortOptions(), out);
     }), false);
     reg->AddFunction(std::make_shared<MetaFunction>("unique", 1, [](const ExecCtx& ctx, const FunctionOptions*, const std::vector<Datum>& args, Datum* out) -> Status {
@@ -1753,6 +1784,69 @@ Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortOptions& op
   NATIVE(ag_sort_indices_dev((int)a->type, a->buffers[1] ? a->buffers[1]->data() : nullptr, valid, a->offset, a->length, (int)opts.Order, (int)opts.Placement,
                              (uint64_t*)idx->data(), &nulls, &nans, nullptr));
   return MakeOut(Type::UINT64, a->length, idx, nullptr, 0, out);
+}
+
+// sortIndicesImpl (vector_sort.go:117-200) + the column checks of kernels.SortIndices (internal/kernels/vector_sort.go:390-416):
+// the key columns go to the device as chunk lists, whatever their chunking.
+Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortKeys& opts, Datum* out) {
+  if (opts.Keys.empty()) return Status::Invalid("must provide at least one sort key");
+  std::vector<std::pair<Type, std::vector<std::shared_ptr<ArrayData>>>> cols;   // (type, chunks) per key
+  std::vector<SortKey> keys = opts.Keys;
+  int64_t n = 0;
+  switch (input.kind) {
+    case DatumKind::ARRAY:      // one column: the first key only, ColumnIndex ignored
+      cols.push_back({input.array->type, {input.array}});
+      keys.resize(1);
+      n = input.array->length;
+      break;
+    case DatumKind::CHUNKED:
+      cols.push_back({input.chunked->type, input.chunked->chunks});
+      keys.resize(1);
+      n = input.chunked->length;
+      break;
+    case DatumKind::RECORD:
+    case DatumKind::TABLE: {
+      const bool rec = input.kind == DatumKind::RECORD;
+      const int64_t ncols = rec ? (int64_t)input.record->columns.size() : (int64_t)input.table->columns.size();
+      for (size_t i = 0; i < keys.size(); ++i) {
+        const int c = keys[i].ColumnIndex;
+        if (c < 0 || c >= ncols) return Status::Invalid("sort key " + std::to_string(i) + " has invalid column index " + std::to_string(c));
+        if (rec) cols.push_back({input.record->columns[c]->type, {input.record->columns[c]}});
+        else cols.push_back({input.table->columns[c]->type, input.table->columns[c]->chunks});
+      }
+      n = rec ? input.record->num_rows : input.table->num_rows;
+      break;
+    }
+    default:
+      return Status::NotImplemented("unsupported type for sort_indices operation");
+  }
+  for (auto& c : cols)
+    if (c.first != Type::BOOL && !IsInteger(c.first) && !IsFloating(c.first))
+      return Status::NotImplemented(std::string("sorting not supported for type ") + TypeName(c.first));
+  std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
+  std::vector<ag_sort_key> desc(cols.size());
+  for (size_t i = 0; i < cols.size(); ++i) {
+    for (auto& a : cols[i].second) {
+      const uint8_t* valid = (a->buffers[0] && a->null_count != 0) ? a->buffers[0]->data() : nullptr;
+      chunks[i].push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, valid, a->offset, a->length});
+    }
+    desc[i] = ag_sort_key{(int)cols[i].first, (int)keys[i].Order, (int)keys[i].Placement, (int)chunks[i].size(), chunks[i].data()};
+  }
+  std::shared_ptr<Buffer> idx;
+  RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(n, 1) * 8, &idx));
+  NATIVE(ag_sort_indices_keys_dev((int)desc.size(), desc.data(), n, (uint64_t*)idx->data(), nullptr));
+  return MakeOut(Type::UINT64, n, idx, nullptr, 0, out);
+}
+
+Status SortIndicesRecordBatch(const ExecCtx& ctx, const std::shared_ptr<RecordBatch>& batch, const std::vector<SortKey>& keys, Datum* out) {
+  if (keys.empty()) return Status::Invalid("at least one sort key is required");
+  SortKeys o; o.Keys = keys;
+  return CallFunction(ctx, "sort_indices", &o, {Datum(batch)}, out);
+}
+Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, const std::vector<SortKey>& keys, Datum* out) {
+  if (keys.empty()) return Status::Invalid("at least one sort key is required");
+  SortKeys o; o.Keys = keys;
+  return CallFunction(ctx, "sort_indices", &o, {Datum(table)}, out);
 }
 
 Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out) {

@@ -1,6 +1,7 @@
 package arrowgpu
 
 /*
+#include <stdlib.h>
 #include "arrowgpu.h"
 */
 import "C"
@@ -8,6 +9,8 @@ import "C"
 import (
 	"context"
 	"fmt"
+	"runtime"
+	"unsafe"
 
 	"github.com/apache/arrow-go/v18/arrow"
 	"github.com/apache/arrow-go/v18/arrow/array"
@@ -284,16 +287,20 @@ func dictionaryEncodeFunction() *compute.VectorFunction {
 
 // ---- sort_indices (vector_sort.go:42-204, kernels.SortIndices vector_sort.go:385-481) -------------------------------
 //
-// A MetaFunction in the reference.  The GPU entry sorts ONE contiguous fixed-width column (stable, NaNs after the finite
-// values, nulls per NullPlacement); chunked inputs, record batches, tables and multi-key sorts go to the parent's
-// implementation, like every other shape this package does not cover.
+// A MetaFunction in the reference.  Every input whose key columns are numeric or boolean goes to ag_sort_indices_keys:
+// an array or chunked array by its first key (ColumnIndex ignored, vector_sort.go:130-152), a record batch or table by
+// every key, whatever the chunking of its columns.  The device order places NaN next to the nulls on every path
+// (DESIGN §2).  Other key types, invalid column indices (so the parent reports them) and calls without SortOptions go
+// to the parent's implementation.
 
 func sortIndicesFunction(parent compute.Function) *compute.MetaFunction {
 	return compute.NewMetaFunction("sort_indices", compute.Unary(), compute.EmptyFuncDoc,
 		func(ctx context.Context, opts compute.FunctionOptions, args ...compute.Datum) (compute.Datum, error) {
 			keys, isKeys := opts.(compute.SortOptions)
-			if in, ok := args[0].(*compute.ArrayDatum); ok && isKeys && len(keys) >= 1 && isNumeric(in.Type()) {
-				return sortOneColumn(ctx, in.Value, keys[0]) // a bare array uses the first key only (vector_sort.go:138-142)
+			if isKeys && len(keys) >= 1 {
+				if cols, ks, n, ok := sortKeyColumns(args[0], keys); ok {
+					return sortKeyed(ctx, cols, ks, n)
+				}
 			}
 			if parent == nil {
 				return nil, fmt.Errorf("%w: unsupported type for sort_indices operation: %s", arrow.ErrNotImplemented, args[0])
@@ -311,27 +318,103 @@ func isNumeric(dt arrow.DataType) bool {
 	return false
 }
 
-func sortOneColumn(ctx context.Context, col arrow.ArrayData, key compute.SortKey) (compute.Datum, error) {
-	n := col.Len()
+func isSortable(dt arrow.DataType) bool { return dt.ID() == arrow.BOOL || isNumeric(dt) }
+
+// sortColumn is one key column: its type and the data of its chunks.
+type sortColumn struct {
+	dt     arrow.DataType
+	chunks []arrow.ArrayData
+}
+
+// sortKeyColumns resolves the chunks of every key column; ok is false when the device cannot take the call.  Only
+// arrow.ArrayData is kept: the datum owns it for the duration of the call.
+func sortKeyColumns(d compute.Datum, keys compute.SortOptions) (cols []sortColumn, ks []compute.SortKey, n int64, ok bool) {
+	chunksOf := func(c *arrow.Chunked) sortColumn {
+		col := sortColumn{dt: c.DataType()}
+		for _, ch := range c.Chunks() {
+			col.chunks = append(col.chunks, ch.Data())
+		}
+		return col
+	}
+	switch in := d.(type) {
+	case *compute.ArrayDatum:
+		return []sortColumn{{in.Value.DataType(), []arrow.ArrayData{in.Value}}}, keys[:1], int64(in.Value.Len()), isSortable(in.Value.DataType())
+	case *compute.ChunkedDatum:
+		return []sortColumn{chunksOf(in.Value)}, keys[:1], int64(in.Value.Len()), isSortable(in.Value.DataType())
+	case *compute.RecordDatum:
+		batch := in.Value
+		for _, k := range keys {
+			if k.ColumnIndex < 0 || int64(k.ColumnIndex) >= batch.NumCols() || !isSortable(batch.Column(k.ColumnIndex).DataType()) {
+				return nil, nil, 0, false
+			}
+			col := batch.Column(k.ColumnIndex)
+			cols = append(cols, sortColumn{col.DataType(), []arrow.ArrayData{col.Data()}})
+		}
+		return cols, keys, batch.NumRows(), true
+	case *compute.TableDatum:
+		tbl := in.Value
+		for _, k := range keys {
+			if k.ColumnIndex < 0 || int64(k.ColumnIndex) >= tbl.NumCols() || !isSortable(tbl.Column(k.ColumnIndex).DataType()) {
+				return nil, nil, 0, false
+			}
+			cols = append(cols, chunksOf(tbl.Column(k.ColumnIndex).Data()))
+		}
+		return cols, keys, tbl.NumRows(), true
+	}
+	return nil, nil, 0, false
+}
+
+func sortKeyed(ctx context.Context, cols []sortColumn, keys []compute.SortKey, n int64) (compute.Datum, error) {
+	// The key and chunk descriptors live in C memory.  The buffers they point at may be Go memory (a Go allocator's
+	// arrays), so they stay pinned until the call returns (cgo pointer rules); Pin does nothing for C memory.
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	total := 0
+	for _, col := range cols {
+		total += len(col.chunks)
+	}
+	descs := unsafe.Slice((*C.ag_sort_key)(C.malloc(C.size_t(len(cols))*C.size_t(unsafe.Sizeof(C.ag_sort_key{})))), len(cols))
+	defer C.free(unsafe.Pointer(&descs[0]))
+	chunkMem := (*C.ag_sort_chunk)(C.malloc(C.size_t(max(total, 1)) * C.size_t(unsafe.Sizeof(C.ag_sort_chunk{}))))
+	defer C.free(unsafe.Pointer(chunkMem))
+	chunks := unsafe.Slice(chunkMem, max(total, 1))
+	next := 0
+	for i, col := range cols {
+		first := next
+		for _, data := range col.chunks {
+			var vals []byte
+			if data.Len() > 0 {
+				vals = data.Buffers()[1].Bytes()
+			}
+			var valid *C.uint8_t
+			if data.NullN() != 0 && data.Buffers()[0] != nil {
+				valid = bitmap(data.Buffers()[0].Bytes())
+			}
+			if p := base0(vals); p != nil {
+				pin.Pin(p)
+			}
+			if valid != nil {
+				pin.Pin(valid)
+			}
+			chunks[next] = C.ag_sort_chunk{vals: base0(vals), valid: valid, offset: C.int64_t(data.Offset()), length: C.int64_t(data.Len())}
+			next++
+		}
+		var firstChunk *C.ag_sort_chunk // a column without chunks (no rows) has none to point at
+		if next > first {
+			firstChunk = &chunks[first]
+		}
+		// arrow.Type ids are the AG_TYPE_* ids; SortOrder / NullPlacement are 0 / 1 on both sides (kernels/vector_sort.go:34-46)
+		descs[i] = C.ag_sort_key{_type: C.int(col.dt.ID()), order: C.int(keys[i].Order), null_placement: C.int(keys[i].NullPlacement),
+			nchunks: C.int(next - first), chunks: firstChunk}
+	}
 	buf := memory.NewResizableBuffer(exec.GetAllocator(ctx))
-	buf.Resize(n * 8)
-	var vals []byte
-	if n > 0 {
-		vals = col.Buffers()[1].Bytes()
-	}
-	var valid *C.uint8_t
-	if col.NullN() != 0 && col.Buffers()[0] != nil {
-		valid = bitmap(col.Buffers()[0].Bytes())
-	}
-	var nulls, nans C.int64_t
-	// arrow.Type ids are the AG_TYPE_* ids; SortOrder / NullPlacement are 0 / 1 on both sides (kernels/vector_sort.go:34-46)
-	err := check(C.ag_sort_indices(C.int(col.DataType().ID()), base0(vals), valid, C.int64_t(col.Offset()), C.int64_t(n),
-		C.int(key.Order), C.int(key.NullPlacement), (*C.uint64_t)(base0(buf.Bytes())), &nulls, &nans))
+	buf.Resize(int(n) * 8)
+	err := check(C.ag_sort_indices_keys(C.int(len(descs)), &descs[0], C.int64_t(n), (*C.uint64_t)(base0(buf.Bytes()))))
 	if err != nil {
 		buf.Release()
 		return nil, err
 	}
-	out := array.NewData(arrow.PrimitiveTypes.Uint64, n, []*memory.Buffer{nil, buf}, nil, 0, 0)
+	out := array.NewData(arrow.PrimitiveTypes.Uint64, int(n), []*memory.Buffer{nil, buf}, nil, 0, 0)
 	buf.Release() // NewData retained it
 	return &compute.ArrayDatum{Value: out}, nil
 }

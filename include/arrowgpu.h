@@ -628,6 +628,32 @@ ag_status ag_sort_indices_dev(int type, const void* d_vals, const uint8_t* d_val
                               int null_placement, uint64_t* d_out_indices, int64_t* null_count, int64_t* nan_count, ag_stream_t s);
 
 /* ================================================================================= *
+ * sort_indices over several keys, each key column split into chunks — replaces kernels.SortIndices for
+ *   record batches, tables and chunked arrays whose key columns are BOOL or one of the 10 numeric types
+ *   (arrow/compute/vector_sort.go:30-52,117-200, internal/kernels/vector_sort.go:390-481): a STABLE
+ *   lexicographic permutation of 0..n-1 as uint64, rows numbered across chunks.  For each key, first to last:
+ *     null_placement 0 (NullsAtEnd)  : [finite in key order | NaN | null]
+ *     null_placement 1 (NullsAtStart): [null | NaN | finite in key order]
+ *   and ties on a key (NaN and null rows included) are ordered by the next key; ties on every key keep row
+ *   order.  -0.0 == +0.0, descending reverses only the finite values, false < true.  This is the partition
+ *   rule of radixRecordBatchSortRange (vector_sort_internal.go:170-206) on every input; the reference's chunk
+ *   merges and its tail comparator above 8 keys place NaN by order instead (vector_sort_support.go:120-137),
+ *   see DESIGN §2.
+ *   keys[j]: the column of key j as `nchunks` chunks of `length` rows each (values and validity at element
+ *   `offset`; BOOL values are an LSB-first bitmap); every key's chunk lengths sum to n, chunk boundaries may
+ *   differ between keys.  The ag_sort_key and ag_sort_chunk arrays are host memory in both flavours; `vals`
+ *   and `valid` are host pointers in the host flavour and device pointers in the device flavour.
+ *   nkeys < 1, order / null_placement other than 0 / 1, negative offsets or lengths, or chunk lengths that
+ *   do not sum to n: AG_ERR_INVALID (vector_sort.go:164-170,390-404); another key type, or n >= 2^32:
+ *   AG_ERR_NOT_IMPLEMENTED.  The device flavour synchronises the stream once (the per-key statistics
+ *   read-back that sizes the packed key).
+ * ================================================================================= */
+typedef struct { const void* vals; const uint8_t* valid; int64_t offset; int64_t length; } ag_sort_chunk;
+typedef struct { int type; int order; int null_placement; int nchunks; const ag_sort_chunk* chunks; } ag_sort_key;
+ag_status ag_sort_indices_keys(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* out_indices);
+ag_status ag_sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out_indices, ag_stream_t s);
+
+/* ================================================================================= *
  * Parquet decode primitives (SURVEY 8f rank 4: the feeder side) — the SIMD leaf loops arrow-go links under
  *   parquet/internal, so pages can be decoded into device-resident Arrow buffers.
  *   ag_parquet_unpack32 ↔ unpack32_avx2 (parquet/internal/utils/_lib/bit_packing_avx2.c:1772): values of

@@ -90,6 +90,27 @@ def sort_key_table(keys):
     return arr
 
 
+class TakeColumn(C.Structure):
+    """ag_take_column: one column of a take_columns call (type, chunks, output values and validity)."""
+    _fields_ = [("type", C.c_int), ("nchunks", C.c_int), ("chunks", C.POINTER(SortChunk)), ("out", C.c_void_p),
+                ("out_valid", C.c_void_p)]
+
+
+def take_column_table(cols):
+    """[(type, [(vals, valid, offset, length), ...], out, out_valid), ...] -> ctypes array of ag_take_column.
+    The chunk arrays are kept alive on the returned array (`_chunks`)."""
+    arr = (TakeColumn * max(len(cols), 1))()
+    arr._chunks = []
+    for k, (ty, chunks, out, out_valid) in enumerate(cols):
+        ch = (SortChunk * max(len(chunks), 1))()
+        for c, (v, ok, off, ln) in enumerate(chunks):
+            ch[c].vals, ch[c].valid, ch[c].offset, ch[c].length = v, ok, off, ln
+        arr._chunks.append(ch)
+        arr[k].type, arr[k].nchunks, arr[k].out, arr[k].out_valid = ty, len(chunks), out, out_valid
+        arr[k].chunks = C.cast(ch, C.POINTER(SortChunk))
+    return arr
+
+
 NULL_ENCODING_MASK, NULL_ENCODING_ENCODE = 0, 1
 TYPE_DICTIONARY = 29
 TYPE_RUN_END_ENCODED = 38
@@ -262,6 +283,8 @@ _SIGS = {
     "ag_sort_indices_dev": [_i, _p, _p, _i64, _i64, _i, _i, _p, _pi64, _pi64, _p],
     "ag_sort_indices_keys": [_i, _p, _i64, _p],
     "ag_sort_indices_keys_dev": [_i, _p, _i64, _p, _p],
+    "ag_take_columns": [_i, _p, _i64, _i, _i, _p, _p, _i64, _i64, _i, _pi64, _pi64],
+    "ag_take_columns_dev": [_i, _p, _i64, _i, _i, _p, _p, _i64, _i64, _i, _p, _p],
     "ag_parquet_unpack32": [_p, _p, _i64, _i, _pi64],
     "ag_parquet_unpack32_dev": [_p, _p, _i64, _i, _pi64, _p],
     "ag_parquet_bytes_to_bools": [_p, _i64, _p, _i64],

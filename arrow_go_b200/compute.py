@@ -96,6 +96,11 @@ def lib():
         h.agx_record_batch.argtypes = [i64, pp, i, pp]
         h.agx_table.argtypes = [i64, pp, i, pp]
         h.agx_sort_indices_keys.argtypes = [p, C.POINTER(i), C.POINTER(i), C.POINTER(i), i, pp]
+        h.agx_num_columns.argtypes = [p]
+        h.agx_column.argtypes = [p, i, pp]
+        h.agx_filter_record_batch.argtypes = [p, p, i, pp]
+        h.agx_filter_table.argtypes = [p, p, i, pp]
+        h.agx_sort.argtypes = [p, C.POINTER(i), C.POINTER(i), C.POINTER(i), i, pp]
         _lib = h
     return _lib
 
@@ -193,6 +198,17 @@ class Datum:
             out = C.c_void_p()
             _check(lib().agx_chunk(self._h, k, C.byref(out)))
             res.append(Datum(out))
+        return res
+
+    def columns(self):
+        """The columns of a record batch (array datums) or a table (chunked datums); [] for any other datum."""
+        res = []
+        for k in range(lib().agx_num_columns(self._h)):
+            out = C.c_void_p()
+            _check(lib().agx_column(self._h, k, C.byref(out)))
+            d = Datum(out)
+            d._keep = self
+            res.append(d)
         return res
 
     def to_numpy(self):
@@ -393,7 +409,24 @@ def Filter(values, mask, null_selection=DROP_NULLS):
 
 
 def Take(values, indices, bounds_check=True):
+    """compute.Take: arrays, chunked arrays, record batches and tables (every column of a record batch or table is
+    gathered by one device launch per index chunk)."""
     return CallFunction("take", [values, indices], ("take", bounds_check))
+
+
+def FilterRecordBatch(batch, mask, null_selection=DROP_NULLS):
+    """compute.FilterRecordBatch(ctx, batch, mask, FilterOptions{NullSelection}) (arrow/compute/selection.go:679-722)."""
+    out = C.c_void_p()
+    _check(lib().agx_filter_record_batch(batch._h, mask._h, int(null_selection), C.byref(out)))
+    return Datum(out)
+
+
+def FilterTable(table, mask, null_selection=DROP_NULLS):
+    """compute.FilterTable(ctx, table, mask, FilterOptions{NullSelection}) (arrow/compute/selection.go:724-800); the mask
+    is an array or a chunked array."""
+    out = C.c_void_p()
+    _check(lib().agx_filter_table(table._h, mask._h, int(null_selection), C.byref(out)))
+    return Datum(out)
 
 
 ASCENDING, DESCENDING = 0, 1
@@ -413,6 +446,16 @@ def SortIndices(values, order=ASCENDING, null_placement=NULLS_AT_END, keys=None)
     n = len(keys)
     cols, orders, places = ((C.c_int * max(n, 1))(*[int(k[i]) for k in keys]) for i in range(3))
     _check(lib().agx_sort_indices_keys(values._h, cols, orders, places, n, C.byref(out)))
+    return Datum(out)
+
+
+def Sort(values, keys):
+    """compute.Sort(ctx, input, SortKeys) (arrow/compute/vector_sort.go:65-81): sort_indices by keys=[(column, order,
+    null_placement), ...] (as in SortIndices) followed by Take, for arrays, chunked arrays, record batches and tables."""
+    out = C.c_void_p()
+    n = len(keys)
+    cols, orders, places = ((C.c_int * max(n, 1))(*[int(k[i]) for k in keys]) for i in range(3))
+    _check(lib().agx_sort(values._h, cols, orders, places, n, C.byref(out)))
     return Datum(out)
 
 

@@ -143,6 +143,10 @@ ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, u
 ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, int64_t vlen, int idx_width, int idx_signed,
                              const void* idx, const uint8_t* ivalid, int64_t ioff, int64_t n, int bounds_check, void* out, uint8_t* out_valid,
                              int64_t* d_bad_pos, cudaStream_t st);
+// take_columns.cu: descriptor checks (no device work) and the gather
+ag_status take_columns_check(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int64_t idx_offset, int64_t n);
+ag_status take_columns_dev(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int idx_signed, const void* idx,
+                           const uint8_t* idx_valid, int64_t idx_offset, int64_t n, int bounds_check, int64_t* d_bad_pos, cudaStream_t st);
 
 // ---------------------------------------------------------------- cross-GPU exchange (comm.cu, reduce.cu) ----
 struct alignas(32) MailSlot { unsigned long long flag; unsigned long long pad; unsigned long long s; unsigned long long c; };

@@ -761,6 +761,78 @@ ag_status ag_sort_indices_keys(int nkeys, const ag_sort_key* keys, int64_t n, ui
   return sync(cs);
 }
 
+ag_status ag_take_columns(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int idx_signed, const void* idx,
+                          const uint8_t* idx_valid, int64_t idx_offset, int64_t n, int bounds_check, int64_t* bad_pos, int64_t* bad_index) {
+  AG_TRY(ensure_init());
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  AG_TRY(take_columns_check(ncols, cols, nrows, idx_width, idx_offset, n));
+  if (n == 0) return AG_OK;
+  if (!idx) AG_FAIL(AG_ERR_INVALID, "take_columns: NULL indices");
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const size_t words = (size_t)((n + 31) / 32) * 4;
+  std::vector<ag_take_column> dcols(cols, cols + ncols);
+  std::vector<std::vector<ag_sort_chunk>> dchunks(ncols);
+  for (int j = 0; j < ncols; ++j) {
+    const bool is_bool = cols[j].type == AG_TYPE_BOOL;
+    for (int c = 0; c < cols[j].nchunks; ++c) {
+      const ag_sort_chunk& ch = cols[j].chunks[c];
+      ag_sort_chunk d{nullptr, nullptr, 0, ch.length};
+      if (ch.length > 0) {
+        uint8_t* dvalid;
+        if (is_bool) {
+          uint8_t* dv;
+          AG_TRY(upload_bitmap(t, (const uint8_t*)ch.vals, ch.offset, ch.length, &dv, &d.offset));
+          d.vals = dv;
+          int64_t phase;
+          AG_TRY(upload_bitmap(t, ch.valid, ch.offset, ch.length, &dvalid, &phase));
+        } else {
+          AG_TRY(upload_column(t, ch.vals, ch.valid, ch.offset, ch.length, type_width(cols[j].type), &d.vals, &dvalid, &d.offset));
+        }
+        d.valid = dvalid;
+      }
+      dchunks[j].push_back(d);
+    }
+    dcols[j].chunks = dchunks[j].data();
+    AG_TRY(t.alloc(&dcols[j].out, is_bool ? words : (size_t)n * type_width(cols[j].type)));
+    dcols[j].out_valid = nullptr;
+    if (cols[j].out_valid) AG_TRY(t.alloc_t(&dcols[j].out_valid, words));
+  }
+  const int iw = idx_width / 8;
+  void* di;
+  uint8_t* div;
+  int64_t oiv;
+  int64_t* d_word;
+  AG_TRY(t.alloc(&di, (size_t)n * iw));
+  AG_TRY(h2d(di, idx, (size_t)n * iw, cs));
+  AG_TRY(upload_bitmap(t, idx_valid, idx_offset, n, &div, &oiv));
+  AG_TRY(t.alloc_t(&d_word, sizeof(int64_t)));
+  AG_TRY(error_word_reset(d_word, cs));
+  AG_TRY(take_columns_dev(ncols, dcols.data(), nrows, idx_width, idx_signed, di, div, oiv, n, bounds_check, d_word, cs));
+  int64_t bad = AG_NO_ERROR_POS;
+  AG_TRY(d2h(&bad, d_word, sizeof(int64_t), cs));
+  AG_TRY(sync(cs));
+  if (bad != AG_NO_ERROR_POS) {
+    if (bad_pos) *bad_pos = bad;
+    int64_t v = 0;
+    switch (idx_width) {
+      case 8: v = idx_signed ? (int64_t)((const int8_t*)idx)[bad] : (int64_t)((const uint8_t*)idx)[bad]; break;
+      case 16: v = idx_signed ? (int64_t)((const int16_t*)idx)[bad] : (int64_t)((const uint16_t*)idx)[bad]; break;
+      case 32: v = idx_signed ? (int64_t)((const int32_t*)idx)[bad] : (int64_t)((const uint32_t*)idx)[bad]; break;
+      default: v = ((const int64_t*)idx)[bad]; break;
+    }
+    if (bad_index) *bad_index = v;
+    if (idx_width == 64 && !idx_signed) AG_FAIL(AG_ERR_INDEX, "%llu out of bounds", (unsigned long long)v);
+    AG_FAIL(AG_ERR_INDEX, "%lld out of bounds", (long long)v);  // helpers.go:951
+  }
+  for (int j = 0; j < ncols; ++j) {
+    const bool is_bool = cols[j].type == AG_TYPE_BOOL;
+    AG_TRY(d2h(cols[j].out, dcols[j].out, is_bool ? (size_t)((n + 7) / 8) : (size_t)n * type_width(cols[j].type), cs));
+    if (cols[j].out_valid) AG_TRY(d2h(cols[j].out_valid, dcols[j].out_valid, (size_t)((n + 7) / 8), cs));
+  }
+  return sync(cs);
+}
+
 ag_status ag_is_in(int bit_width, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, const void* set_vals,
                    const uint8_t* set_valid, int64_t set_offset, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid,
                    int64_t* out_nulls) {

@@ -388,7 +388,8 @@ Status Multiply(const ExecCtx& ctx, const ArithmeticOptions& opts, const Datum& 
 // vector_cumulative.go:96-102
 Status CumulativeSum(const ExecCtx& ctx, const CumulativeOptions& opts, const Datum& values, Datum* out);
 Status CumulativeSumChecked(const ExecCtx& ctx, const CumulativeOptions& opts, const Datum& values, Datum* out);
-// selection.go:657 / :304
+// selection.go:657 / :304.  Take also takes record batches and tables (takeRecordImpl / takeTableImpl): every column is
+// gathered by one ag_take_columns_dev launch per index chunk.
 Status Filter(const ExecCtx& ctx, const Datum& values, const Datum& filter, const FilterOptions& opts, Datum* out);
 Status Take(const ExecCtx& ctx, const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out);
 // compute.SortIndices (vector_sort.go:205-211), compute.Unique (vector_hash.go), compute.IsIn (scalar_set_lookup.go)
@@ -399,6 +400,14 @@ Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortKeys& keys,
 // vector_sort.go:240-271
 Status SortIndicesRecordBatch(const ExecCtx& ctx, const std::shared_ptr<RecordBatch>& batch, const std::vector<SortKey>& keys, Datum* out);
 Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, const std::vector<SortKey>& keys, Datum* out);
+// selection.go:679-800.  CallFunction("filter") does not take record batches or tables (it answers ErrNotImplemented);
+// these two do.  Every column is gathered by ag_take_columns_dev; boolean and numeric columns only.
+Status FilterRecordBatch(const ExecCtx& ctx, const std::shared_ptr<RecordBatch>& batch, const std::shared_ptr<ArrayData>& filter,
+                         const FilterOptions& opts, std::shared_ptr<RecordBatch>* out);
+Status FilterTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, const Datum& filter, const FilterOptions& opts, std::shared_ptr<Table>* out);
+// compute.Sort (vector_sort.go:65-81): SortIndices(keys) then Take with default TakeOptions, for arrays, chunked arrays,
+// record batches and tables.  A host function only: no "sort" name is registered.
+Status Sort(const ExecCtx& ctx, const Datum& input, const SortKeys& keys, Datum* out);
 Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out);
 // compute.DictionaryEncode (vector_hash.go:105-121): Dictionary<int32, T>; a chunked input gets ONE dictionary for all
 // chunks and loses its empty chunks; a dictionary input is returned as it is

@@ -208,6 +208,45 @@ int agx_sort_indices_keys(agx_datum* d, const int* columns, const int* orders, c
   *out = new agx_datum{res};
   return AG_OK;
 }
+// The columns of a record batch (arrays) or a table (chunked arrays); Datum chunks stay [] for both
+int agx_num_columns(agx_datum* d) {
+  if (d->d.kind == DatumKind::RECORD) return (int)d->d.record->columns.size();
+  if (d->d.kind == DatumKind::TABLE) return (int)d->d.table->columns.size();
+  return 0;
+}
+int agx_column(agx_datum* d, int i, agx_datum** out) {
+  if (d->d.kind != DatumKind::RECORD && d->d.kind != DatumKind::TABLE) return fail(Status::Invalid("column: not a record batch or table"));
+  if (i < 0 || i >= agx_num_columns(d)) return fail(Status::Invalid("column: out of range"));
+  *out = d->d.kind == DatumKind::RECORD ? new agx_datum{Datum(d->d.record->columns[i])} : new agx_datum{Datum(d->d.table->columns[i])};
+  return AG_OK;
+}
+// compute.FilterRecordBatch / FilterTable with FilterOptions{NullSelection} (selection.go:679-800)
+int agx_filter_record_batch(agx_datum* d, agx_datum* filter, int null_selection, agx_datum** out) {
+  if (d->d.kind != DatumKind::RECORD) return fail(Status::Invalid("filter_record_batch: not a record batch"));
+  if (filter->d.kind != DatumKind::ARRAY) return fail(Status::Invalid("filter_record_batch: the filter must be an array"));
+  FilterOptions o; o.NullSelection = (NullSelectionBehavior)null_selection;
+  ExecCtx ctx; std::shared_ptr<RecordBatch> r;
+  AGX_TRY(FilterRecordBatch(ctx, d->d.record, filter->d.array, o, &r));
+  *out = new agx_datum{Datum(r)};
+  return AG_OK;
+}
+int agx_filter_table(agx_datum* d, agx_datum* filter, int null_selection, agx_datum** out) {
+  if (d->d.kind != DatumKind::TABLE) return fail(Status::Invalid("filter_table: not a table"));
+  FilterOptions o; o.NullSelection = (NullSelectionBehavior)null_selection;
+  ExecCtx ctx; std::shared_ptr<Table> r;
+  AGX_TRY(FilterTable(ctx, d->d.table, filter->d, o, &r));
+  *out = new agx_datum{Datum(r)};
+  return AG_OK;
+}
+// compute.Sort(SortKeys{{column[i], order[i], null_placement[i]}...}) (vector_sort.go:65-81)
+int agx_sort(agx_datum* d, const int* columns, const int* orders, const int* null_placements, int nkeys, agx_datum** out) {
+  SortKeys o;
+  for (int i = 0; i < nkeys; ++i) o.Keys.push_back(SortKey{columns[i], (SortOrder)orders[i], (NullPlacement)null_placements[i]});
+  ExecCtx ctx; Datum res;
+  AGX_TRY(Sort(ctx, d->d, o, &res));
+  *out = new agx_datum{res};
+  return AG_OK;
+}
 int agx_unique(agx_datum* d, agx_datum** out) {
   ExecCtx ctx; Datum res;
   AGX_TRY(CallFunction(ctx, "unique", nullptr, {d->d}, &res));

@@ -806,8 +806,9 @@ Status CallFunction(const ExecCtx& ctx, const std::string& name, const FunctionO
   // through run_end_decode
   for (auto& a : args) {
     if (a.kind == DatumKind::NONE) continue;
-    // only sort_indices takes whole record batches and tables; the kernels of every other function take columns
-    if (name != "sort_indices" && (a.kind == DatumKind::RECORD || a.kind == DatumKind::TABLE))
+    // only sort_indices and take take whole record batches and tables; the kernels of every other function take
+    // columns.  "filter" keeps refusing them: FilterRecordBatch / FilterTable filter a record batch or table.
+    if (name != "sort_indices" && name != "take" && (a.kind == DatumKind::RECORD || a.kind == DatumKind::TABLE))
       return Status::NotImplemented("function '" + name + "' has no kernel for record batch or table arguments");
     if (name != "dictionary_encode" && a.type() == Type::DICTIONARY) return Status::NotImplemented("function '" + name + "' has no kernel for dictionary arguments");
     if (name != "run_end_decode" && a.type() == Type::RUN_END_ENCODED) return Status::NotImplemented("function '" + name + "' has no kernel for run-end encoded arguments");
@@ -1476,6 +1477,7 @@ std::shared_ptr<ScalarFunction> MakeBool(const std::string& name, exec::ArrayKer
 }
 
 Status ConcatenateChunks(const ChunkedArray& c, std::shared_ptr<ArrayData>* out);
+Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out);
 
 }  // namespace
 
@@ -1673,6 +1675,8 @@ FunctionRegistry* GetFunctionRegistry() {
       // takeMetaFunc, selection.go:93-114 -> takeArrayImpl :206-244 / takeChunkedImpl :246-300
       if (args.size() != 2) return Status::Invalid("take takes 2 arguments");
       if (args[1].kind != DatumKind::ARRAY && args[1].kind != DatumKind::CHUNKED) return Status::NotImplemented("unsupported types for take operation");
+      if (args[0].kind == DatumKind::RECORD || args[0].kind == DatumKind::TABLE)   // takeRecordImpl / takeTableImpl
+        return TakeRecordOrTable(dynamic_cast<const TakeOptions*>(opts) ? *dynamic_cast<const TakeOptions*>(opts) : TakeOptions(), args[0], args[1], out);
       Datum values = args[0];
       const bool values_chunked = values.kind == DatumKind::CHUNKED;
       if (values_chunked) {  // ChunkedPrimitiveTake resolves chunks per index; on the device we gather from one table
@@ -1847,6 +1851,259 @@ Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table,
   if (keys.empty()) return Status::Invalid("at least one sort key is required");
   SortKeys o; o.Keys = keys;
   return CallFunction(ctx, "sort_indices", &o, {Datum(table)}, out);
+}
+
+// ---- take / filter / sort on record batches and tables ---------------------------------------------------------------
+// Every column of a record batch or table is gathered by one ag_take_columns_dev launch per index chunk (per filter span
+// for FilterTable), never one launch per column.  Arrays and chunked arrays keep the "take" meta function's own path.
+namespace {
+bool SelectionType(Type t) { return t == Type::BOOL || IsNumeric(t); }
+bool MayHaveNulls(const ArrayData& a) { return a.buffers[0] != nullptr && a.null_count != 0; }
+bool MayHaveNulls(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
+  for (auto& c : chunks) if (MayHaveNulls(*c)) return true;
+  return false;
+}
+
+// One column of a selection: its type and chunks (a record batch column is one chunk).
+struct SelColumn { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
+
+Status SelColumns(const Datum& values, std::vector<SelColumn>* cols, int64_t* nrows) {
+  if (values.kind == DatumKind::RECORD) {
+    for (auto& c : values.record->columns) cols->push_back(SelColumn{c->type, {c}});
+    *nrows = values.record->num_rows;
+  } else {
+    for (auto& c : values.table->columns) cols->push_back(SelColumn{c->type, c->chunks});
+    *nrows = values.table->num_rows;
+  }
+  for (size_t i = 0; i < cols->size(); ++i)
+    if (!SelectionType((*cols)[i].type))
+      return Status::NotImplemented("take: column " + std::to_string(i) + " has unsupported type " + TypeName((*cols)[i].type) +
+                                    " (boolean and numeric columns only)");
+  return Status::OK();
+}
+
+// The output of one column for `n` rows (preallocateData, vector_selection.go:83-93): values at offset 0, a validity
+// bitmap exactly when `nullable`.
+std::shared_ptr<ArrayData> SelOutput(Type t, int64_t n, bool nullable, Status* st) {
+  auto d = std::make_shared<ArrayData>();
+  d->type = t; d->length = n; d->offset = 0; d->null_count = nullable ? kUnknownNullCount : 0;
+  *st = Buffer::Allocate(t == Type::BOOL ? ((n + 31) / 32) * 4 : n * (BitWidth(t) / 8), &d->buffers[1]);
+  if (st->ok() && nullable) *st = Buffer::Allocate(((n + 31) / 32) * 4, &d->buffers[0]);
+  return d;
+}
+
+// One launch: gather rows [0, idx.length) of `idx` from every column.  `chunks[c]` are the chunks column c is read from
+// (their lengths sum to nrows); outs[c] receives the result.
+Status GatherColumns(const std::vector<SelColumn>& cols, const std::vector<std::vector<ag_sort_chunk>>& chunks, int64_t nrows, const ArrayData& idx,
+                     bool bounds, int64_t* d_bad, const std::vector<std::shared_ptr<ArrayData>>& outs) {
+  std::vector<ag_take_column> desc(cols.size());
+  for (size_t c = 0; c < cols.size(); ++c)
+    desc[c] = ag_take_column{(int)cols[c].type, (int)chunks[c].size(), chunks[c].data(), outs[c]->buffers[1]->data(),
+                             outs[c]->buffers[0] ? outs[c]->buffers[0]->data() : nullptr};
+  const int iw = BitWidth(idx.type);
+  const uint8_t* ivalid = MayHaveNulls(idx) ? idx.buffers[0]->data() : nullptr;
+  const void* iptr = idx.buffers[1] ? idx.buffers[1]->data() + idx.offset * (iw / 8) : nullptr;
+  NATIVE(ag_take_columns_dev((int)desc.size(), desc.data(), nrows, iw, IsSignedInteger(idx.type), iptr, ivalid, idx.offset, idx.length,
+                             bounds ? 1 : 0, d_bad, nullptr));
+  return Status::OK();
+}
+
+std::vector<ag_sort_chunk> ChunkDescs(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
+  std::vector<ag_sort_chunk> d;
+  for (auto& a : chunks)
+    d.push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, MayHaveNulls(*a) ? a->buffers[0]->data() : nullptr, a->offset, a->length});
+  return d;
+}
+
+// "%d out of bounds" with the index at row `bad` of `idx` (helpers.go:951), as PrimitiveTakeExec reports it
+Status BoundsError(const ArrayData& idx, int64_t bad) {
+  const int iw = BitWidth(idx.type) / 8;
+  uint8_t raw[8] = {0};
+  RETURN_NOT_OK(idx.buffers[1]->ToHost(raw, iw, (idx.offset + bad) * iw));
+  if (IsSignedInteger(idx.type)) {
+    long long v = 0;
+    switch (iw) { case 1: v = (int8_t)raw[0]; break; case 2: { int16_t t; memcpy(&t, raw, 2); v = t; break; }
+                  case 4: { int32_t t; memcpy(&t, raw, 4); v = t; break; } default: memcpy(&v, raw, 8); }
+    return Status::IndexError(std::to_string(v) + " out of bounds");
+  }
+  unsigned long long uv = 0;
+  memcpy(&uv, raw, 8);
+  return Status::IndexError(std::to_string(uv) + " out of bounds");
+}
+
+// takeRecordImpl (selection.go:160-204) and takeTableImpl -> takeChunkedImpl -> ChunkedPrimitiveTake (:117-158, 246-300,
+// kernels/vector_selection.go:1194-1228): a record batch takes by the concatenated indices and gives arrays of
+// len(indices) rows; a table gives every column one chunk per index chunk (an array index: one chunk).
+Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out) {
+  std::vector<SelColumn> cols;
+  int64_t nrows = 0;
+  RETURN_NOT_OK(SelColumns(values, &cols, &nrows));
+  const Type it = indices.type();
+  if (!IsInteger(it)) return Status::Invalid("invalid index type for bounds checking");   // helpers.go:978
+  std::vector<std::shared_ptr<ArrayData>> idx;
+  if (indices.kind == DatumKind::ARRAY) {
+    idx.push_back(indices.array);
+  } else if (values.kind == DatumKind::RECORD) {   // chunked indices are concatenated first (:163-171)
+    std::shared_ptr<ArrayData> cat;
+    RETURN_NOT_OK(ConcatenateChunks(*indices.chunked, &cat));
+    idx.push_back(cat);
+  } else {
+    idx = indices.chunked->chunks;
+  }
+  std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
+  for (size_t c = 0; c < cols.size(); ++c) chunks[c] = ChunkDescs(cols[c].chunks);
+  const bool idx_nullable = MayHaveNulls(idx);
+  std::shared_ptr<Buffer> words;
+  RETURN_NOT_OK(Buffer::Allocate(8 * std::max<int64_t>((int64_t)idx.size(), 1), &words));
+  int64_t* d_bad = (int64_t*)words->data();
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> res(cols.size());
+  // the reference takes column by column, so without columns nothing is gathered or bounds-checked
+  const size_t launches = cols.empty() ? 0 : idx.size();
+  for (size_t k = 0; k < launches; ++k) {
+    std::vector<std::shared_ptr<ArrayData>> outs(cols.size());
+    for (size_t c = 0; c < cols.size(); ++c) {
+      Status st;
+      outs[c] = SelOutput(cols[c].type, idx[k]->length, idx_nullable || MayHaveNulls(cols[c].chunks), &st);
+      RETURN_NOT_OK(st);
+      res[c].push_back(outs[c]);
+    }
+    if (opts.BoundsCheck) NATIVE(ag_error_word_reset_dev(d_bad + k, nullptr));
+    RETURN_NOT_OK(GatherColumns(cols, chunks, nrows, *idx[k], opts.BoundsCheck, opts.BoundsCheck ? d_bad + k : nullptr, outs));
+  }
+  if (opts.BoundsCheck && launches > 0) {   // checkIndexBoundsChunked: the first offending row in index order
+    std::vector<int64_t> bad(launches);
+    RETURN_NOT_OK(words->ToHost(bad.data(), 8 * (int64_t)launches));
+    for (size_t k = 0; k < launches; ++k)
+      if (bad[k] != AG_NO_ERROR_POS) return BoundsError(*idx[k], bad[k]);
+  }
+  int64_t out_rows = 0;
+  for (auto& a : idx) out_rows += a->length;
+  if (values.kind == DatumKind::RECORD) {
+    std::vector<std::shared_ptr<ArrayData>> arrs;
+    for (auto& r : res) arrs.push_back(r[0]);
+    std::shared_ptr<RecordBatch> rb;
+    RETURN_NOT_OK(MakeRecordBatch(out_rows, std::move(arrs), &rb));
+    *out = Datum(rb);
+    return Status::OK();
+  }
+  std::vector<std::shared_ptr<ChunkedArray>> ccols;
+  for (size_t c = 0; c < cols.size(); ++c) {
+    auto ch = std::make_shared<ChunkedArray>();
+    ch->type = cols[c].type; ch->chunks = res[c]; ch->length = out_rows;
+    ccols.push_back(ch);
+  }
+  std::shared_ptr<Table> tb;   // array.NewTable(schema, cols, -1): a table without columns has no rows
+  RETURN_NOT_OK(MakeTable(cols.empty() ? 0 : out_rows, std::move(ccols), &tb));
+  *out = Datum(tb);
+  return Status::OK();
+}
+
+// GetTakeIndices (kernels/vector_selection.go:102-236) of each mask span, with one read-back for all their lengths:
+// uint32 row indices relative to the span, validity only when EmitNulls meets a null mask slot.
+Status MaskSpansToIndices(const std::vector<std::shared_ptr<ArrayData>>& masks, NullSelectionBehavior sel, std::vector<std::shared_ptr<ArrayData>>* out) {
+  const size_t ns = masks.size();
+  std::shared_ptr<Buffer> lens;
+  RETURN_NOT_OK(Buffer::Allocate(16 * std::max<int64_t>((int64_t)ns, 1), &lens));
+  int64_t* d_len = (int64_t*)lens->data();
+  for (size_t k = 0; k < ns; ++k) {
+    const ArrayData& m = *masks[k];
+    if (m.length > (int64_t)UINT32_MAX) return Status::NotImplemented("filter: more than 2^32-1 rows in one chunk");
+    NATIVE(ag_filter_output_size_dev(m.buffers[1]->data(), MayHaveNulls(m) ? m.buffers[0]->data() : nullptr, m.offset, m.length, (int)sel,
+                                     d_len + 2 * k, nullptr));
+  }
+  std::vector<int64_t> h(2 * std::max<size_t>(ns, 1));
+  RETURN_NOT_OK(lens->ToHost(h.data(), 16 * (int64_t)ns));
+  for (size_t k = 0; k < ns; ++k) {
+    const ArrayData& m = *masks[k];
+    const int64_t len = h[2 * k];
+    const bool nullable = sel == EmitNulls && MayHaveNulls(m);
+    auto d = std::make_shared<ArrayData>();
+    d->type = Type::UINT32; d->length = len; d->offset = 0; d->null_count = nullable ? kUnknownNullCount : 0;
+    RETURN_NOT_OK(Buffer::Allocate(len * 4, &d->buffers[1]));
+    if (nullable) RETURN_NOT_OK(Buffer::Allocate(((len + 31) / 32) * 4, &d->buffers[0]));
+    if (len > 0)
+      NATIVE(ag_take_indices_dev(32, m.buffers[1]->data(), MayHaveNulls(m) ? m.buffers[0]->data() : nullptr, m.offset, m.length, (int)sel,
+                                 d->buffers[1]->data(), nullable ? d->buffers[0]->data() : nullptr, len, d_len + 2 * k + 1, nullptr));
+    out->push_back(d);
+  }
+  return Status::OK();
+}
+}  // namespace
+
+// FilterRecordBatch (selection.go:679-722): the mask becomes indices once, every column is gathered without a bounds check
+Status FilterRecordBatch(const ExecCtx& ctx, const std::shared_ptr<RecordBatch>& batch, const std::shared_ptr<ArrayData>& filter,
+                         const FilterOptions& opts, std::shared_ptr<RecordBatch>* out) {
+  if (!filter || batch->num_rows != filter->length) return Status::Invalid("filter inputs must all be the same length");
+  if (filter->type != Type::BOOL) return Status::NotImplemented("filter argument must be boolean type");
+  std::vector<std::shared_ptr<ArrayData>> idx;
+  RETURN_NOT_OK(MaskSpansToIndices({filter}, opts.NullSelection, &idx));
+  TakeOptions to; to.BoundsCheck = false;
+  Datum r;
+  RETURN_NOT_OK(TakeRecordOrTable(to, Datum(batch), Datum(idx[0]), &r));
+  *out = r.record;
+  return Status::OK();
+}
+
+// FilterTable (selection.go:724-800): columns and filter are cut at every chunk boundary of any of them (the walk of
+// RechunkArraysConsistently, which IterateExecSpans does); each span's mask becomes indices once and all columns are
+// gathered from that span in one launch.  A span that selects no row gives no chunk; a zero-row table comes back as it is.
+Status FilterTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, const Datum& filter, const FilterOptions& opts, std::shared_ptr<Table>* out) {
+  if (table->num_rows != filter.Len()) return Status::Invalid("filter inputs must all be the same length");
+  if (table->num_rows == 0) { *out = table; return Status::OK(); }
+  if (filter.kind != DatumKind::ARRAY && filter.kind != DatumKind::CHUNKED) return Status::NotImplemented("filter should be array-like");
+  if (filter.type() != Type::BOOL) return Status::NotImplemented("filter argument must be boolean type");
+  std::vector<SelColumn> cols;
+  int64_t nrows = 0;
+  RETURN_NOT_OK(SelColumns(Datum(table), &cols, &nrows));
+  const std::vector<std::shared_ptr<ArrayData>> fchunks = filter.kind == DatumKind::ARRAY ? std::vector<std::shared_ptr<ArrayData>>{filter.array} : filter.chunked->chunks;
+  std::vector<std::vector<int64_t>> lens(cols.size() + 1);
+  for (size_t c = 0; c < cols.size(); ++c) for (auto& a : cols[c].chunks) lens[c].push_back(a->length);
+  for (auto& a : fchunks) lens.back().push_back(a->length);
+  std::vector<SpanPiece> pieces;
+  RETURN_NOT_OK(IterateExecSpans(lens, std::vector<bool>(lens.size(), true), INT64_MAX, &pieces));
+  std::vector<std::shared_ptr<ArrayData>> masks;
+  for (auto& p : pieces) masks.push_back(fchunks[p.chunk_index.back()]->Slice(p.chunk_pos.back(), p.len));
+  std::vector<std::shared_ptr<ArrayData>> idx;
+  RETURN_NOT_OK(MaskSpansToIndices(masks, opts.NullSelection, &idx));
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> res(cols.size());
+  int64_t out_rows = 0;
+  for (size_t k = 0; k < pieces.size(); ++k) {
+    if (idx[k]->length == 0) continue;
+    const SpanPiece& p = pieces[k];
+    std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
+    std::vector<std::shared_ptr<ArrayData>> outs(cols.size());
+    for (size_t c = 0; c < cols.size(); ++c) {
+      const auto& src = cols[c].chunks[p.chunk_index[c]];
+      chunks[c] = ChunkDescs({src->Slice(p.chunk_pos[c], p.len)});
+      Status st;
+      outs[c] = SelOutput(cols[c].type, idx[k]->length, MayHaveNulls(*idx[k]) || MayHaveNulls(*src), &st);
+      RETURN_NOT_OK(st);
+      res[c].push_back(outs[c]);
+    }
+    RETURN_NOT_OK(GatherColumns(cols, chunks, p.len, *idx[k], false, nullptr, outs));
+    out_rows += idx[k]->length;
+  }
+  std::vector<std::shared_ptr<ChunkedArray>> ccols;
+  for (size_t c = 0; c < cols.size(); ++c) {
+    auto ch = std::make_shared<ChunkedArray>();
+    ch->type = cols[c].type; ch->chunks = res[c]; ch->length = out_rows;
+    ccols.push_back(ch);
+  }
+  return MakeTable(out_rows, std::move(ccols), out);
+}
+
+// compute.Sort (vector_sort.go:65-81): sort_indices by `keys`, then take with default TakeOptions.  A chunked array is
+// taken as a one-column table (one gather over its chunks) and comes back as a one-chunk chunked array.
+Status Sort(const ExecCtx& ctx, const Datum& input, const SortKeys& keys, Datum* out) {
+  Datum idx;
+  RETURN_NOT_OK(SortIndices(ctx, input, keys, &idx));
+  if (input.kind != DatumKind::CHUNKED) return Take(ctx, TakeOptions(), input, idx, out);
+  std::shared_ptr<Table> t;
+  RETURN_NOT_OK(MakeTable(input.chunked->length, {input.chunked}, &t));
+  Datum r;
+  RETURN_NOT_OK(Take(ctx, TakeOptions(), Datum(t), idx, &r));
+  *out = Datum(r.table->columns[0]);
+  return Status::OK();
 }
 
 Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out) {

@@ -215,6 +215,7 @@ func NewRegistry() compute.FunctionRegistry {
 	addVector(reg, parent, takeFn)
 	registerLookupSort(reg, parent) // is_in, unique, sort_indices (lookup_sort.go)
 	registerRunEnds(reg, parent)    // run_end_encode, run_end_decode (run_ends.go)
+	registerSelection(reg, parent)  // take on record batches and tables (selection.go)
 	return reg
 }
 

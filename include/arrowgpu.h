@@ -654,6 +654,35 @@ ag_status ag_sort_indices_keys(int nkeys, const ag_sort_key* keys, int64_t n, ui
 ag_status ag_sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out_indices, ag_stream_t s);
 
 /* ================================================================================= *
+ * Take over several columns at once — the per-column takes of takeRecordImpl / takeTableImpl and of
+ *   FilterRecordBatch / FilterTable (arrow/compute/selection.go:117-204,679-800) in one launch: every column is
+ *   gathered by the same n indices, with the rules of ag_take_primitive:
+ *     out[i] = the column's row idx[i], rows numbered across its chunks (ag_sort_chunk: values and validity at element
+ *       `offset`, BOOL values an LSB-first bitmap); out_valid[i] = idx_valid[idx_offset+i] & the row's validity; value
+ *       0 where out_valid is clear.
+ *   cols[j]: type BOOL or one of the 10 numeric types, any mix; nchunks chunks whose lengths sum to nrows (empty and
+ *   sliced chunks allowed, columns may be chunked differently).  out (BOOL: a bitmap) and out_valid are written at
+ *   offset 0.  out_valid may be NULL only when neither the column nor the indices have a validity bitmap.
+ *   idx: n indices of idx_width bits (8/16/32/64) starting at element 0, signed when idx_signed; idx_valid (may be
+ *   NULL) at bit idx_offset.  Only valid index slots are bounds-checked; negative (signed) or >= nrows is out of
+ *   bounds.  With bounds_check: AG_ERR_INDEX "%d out of bounds" with the index of the lowest offending row in
+ *   *bad_pos / *bad_index (host flavour), or that row lowered into *d_bad_pos (device flavour; reset it with
+ *   ag_error_word_reset_dev).
+ *   The ag_take_column and ag_sort_chunk arrays are host memory in both flavours; every other pointer is a host
+ *   pointer in the host flavour (out / out_valid receive ceil(n/8) bytes of bitmap) and a device pointer in the
+ *   device flavour (out_valid, and a BOOL out, 4-byte aligned, ceil(n/32) words).
+ *   Negative offsets or lengths, or chunk lengths that do not sum to nrows: AG_ERR_INVALID; another column type:
+ *   AG_ERR_NOT_IMPLEMENTED naming the column.  Both are checked before any device work.
+ * ================================================================================= */
+typedef struct { int type; int nchunks; const ag_sort_chunk* chunks; void* out; uint8_t* out_valid; } ag_take_column;
+ag_status ag_take_columns(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int idx_signed, const void* idx,
+                          const uint8_t* idx_valid, int64_t idx_offset, int64_t n, int bounds_check, int64_t* bad_pos,
+                          int64_t* bad_index);
+ag_status ag_take_columns_dev(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int idx_signed,
+                              const void* d_idx, const uint8_t* d_idx_valid, int64_t idx_offset, int64_t n, int bounds_check,
+                              int64_t* d_bad_pos, ag_stream_t s);
+
+/* ================================================================================= *
  * Parquet decode primitives (SURVEY 8f rank 4: the feeder side) — the SIMD leaf loops arrow-go links under
  *   parquet/internal, so pages can be decoded into device-resident Arrow buffers.
  *   ag_parquet_unpack32 ↔ unpack32_avx2 (parquet/internal/utils/_lib/bit_packing_avx2.c:1772): values of

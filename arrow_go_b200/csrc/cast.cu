@@ -171,14 +171,7 @@ cast_vec_kernel(const I* __restrict__ in, O* __restrict__ out, int64_t n,
       }
     }
   }
-  if constexpr (kCheck != 0) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, d);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(first_bad, my_bad);
-  }
+  if constexpr (kCheck != 0) lower_error_row(my_bad, first_bad);
 }
 
 // Element-aligned operands (odd element offsets): one element per thread, still coalesced.
@@ -196,14 +189,7 @@ cast_scalar_kernel(const I* __restrict__ in, O* __restrict__ out, int64_t n,
       if (cast_fails<I, O, kCheck>(v, o, lo, hi) && (!valid || bit_is_set(valid, voff + i)) && row_base + i < my_bad) my_bad = row_base + i;
     }
   }
-  if constexpr (kCheck != 0) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, d);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(first_bad, my_bad);
-  }
+  if constexpr (kCheck != 0) lower_error_row(my_bad, first_bad);
 }
 
 template <typename I, typename O, int kCheck>

@@ -138,6 +138,9 @@ ag_status sort_indices_dev(int type, const void* vals, const uint8_t* valid, int
                            uint64_t* d_out, int64_t* nulls_out, int64_t* nans_out, cudaStream_t st);
 // argument checks of sort_indices_keys_dev (no device work)
 ag_status sort_indices_keys_check(int nkeys, const ag_sort_key* keys, int64_t n);
+// One column's chunk list against its row count: the list, each chunk's offset, length and values, the sum of the
+// lengths.  Messages start with "<who> <j>: "; the row-count one ends with "does not match <rows_name> <nrows>".
+ag_status check_chunk_list(const char* who, int j, int nchunks, const ag_sort_chunk* chunks, int64_t nrows, const char* rows_name);
 ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, uint64_t* d_out, cudaStream_t st);
 // take.cu
 ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vvalid, int64_t voff, int64_t vlen, int idx_width, int idx_signed,
@@ -335,6 +338,49 @@ __device__ __forceinline__ void bitmap_store32_masked(uint32_t* wp, uint32_t val
 
 __device__ __forceinline__ bool bit_is_set(const uint8_t* __restrict__ bits, int64_t i) {
   return (bits[i >> 3] >> (i & 7)) & 1;
+}
+
+// Lower the warp's lowest failing row into the error word: a shuffle-xor minimum, then one atomicMin from lane 0 when
+// some lane saw a failure.  Every lane of the warp calls it.
+__device__ __forceinline__ void lower_error_row(long long my_bad, long long* word) {
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) {
+    const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
+    my_bad = o < my_bad ? o : my_bad;
+  }
+  if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(word, my_bad);
+}
+
+// Take's bounds rule for a valid index slot (I: the unsigned type of the index width): out of bounds when the index is
+// negative (a signed index type with the sign bit set) or, read as unsigned, >= rows.  take_partition_kernel computes
+// the same rule as one unsigned compare against min(rows, 2^(bits-1)) for signed indices.  The operands are references
+// so that the kernels keep their register counts: by value, take_kernel needs up to 11 more registers.
+// take_columns_kernel spells the rule out: through this helper nvcc reorders its gathers.
+template <typename I>
+__device__ __forceinline__ bool take_index_oob(const I& ix, const unsigned long long& rows, const int& idx_signed) {
+  constexpr I kSignBit = (I)((I)1 << (sizeof(I) * 8 - 1));
+  return (idx_signed && (ix & kSignBit)) || (unsigned long long)ix >= rows;
+}
+
+// Lane 0 stores word w (a warp's ballot) of an output bitmap of n bits: whole inside the bitmap, masked to the bits
+// below n in the last word, not at all past it.
+__device__ __forceinline__ void store_valid_word(uint32_t* out_valid, int64_t w, uint32_t bits, int64_t n, int lane) {
+  const int64_t rem = n - (w << 5);
+  if (lane == 0 && rem > 0) {
+    if (rem >= 32) out_valid[w] = bits;
+    else bitmap_store32_masked(out_valid + w, bits, bit_range_mask(0, (int)rem));
+  }
+}
+
+// The same for a boolean output: the data word and, when out_valid is set, the validity word, under one mask.
+__device__ __forceinline__ void store_bool_words(uint32_t* out, uint32_t* out_valid, int64_t w, uint32_t dbits, uint32_t vbits,
+                                                 int64_t n, int lane) {
+  const int64_t rem = n - (w << 5);
+  if (lane == 0 && rem > 0) {
+    const uint32_t m = rem >= 32 ? 0xffffffffu : bit_range_mask(0, (int)rem);
+    bitmap_store32_masked(out + w, dbits, m);
+    if (out_valid) bitmap_store32_masked(out_valid + w, vbits, m);
+  }
 }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser

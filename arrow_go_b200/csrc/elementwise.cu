@@ -630,13 +630,7 @@ checked_kernel(const ST* __restrict__ l, const uint8_t* __restrict__ lvalid, int
     }
     if (i < n) out[i] = o;
   }
-  // lowest failing row: warp min, then one atomicMin per warp that saw a failure
-#pragma unroll
-  for (int m = 16; m >= 1; m >>= 1) {
-    const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-    my_bad = o < my_bad ? o : my_bad;
-  }
-  if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(first_bad, my_bad);
+  lower_error_row(my_bad, first_bad);
 }
 
 
@@ -734,12 +728,7 @@ checked_tile_kernel(const ST* __restrict__ l, const uint8_t* __restrict__ lvalid
       out[row] = o;
     }
   }
-#pragma unroll
-  for (int m = 16; m >= 1; m >>= 1) {
-    const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-    my_bad = o < my_bad ? o : my_bad;
-  }
-  if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(first_bad, my_bad);
+  lower_error_row(my_bad, first_bad);
 }
 
 template <typename ST, typename Op, bool kNotNull>
@@ -828,12 +817,7 @@ unary_checked_kernel(const ST* __restrict__ in, ST* __restrict__ out, int64_t n,
     if (v == tmin && (long long)i < my_bad) my_bad = (long long)i;
     out[i] = kAbs ? UAbs::apply<ST, ST>(v) : UNeg::apply<ST, ST>(v);
   }
-#pragma unroll
-  for (int m = 16; m >= 1; m >>= 1) {
-    const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-    my_bad = o < my_bad ? o : my_bad;
-  }
-  if ((threadIdx.x & 31) == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(first_bad, my_bad);
+  lower_error_row(my_bad, first_bad);
 }
 
 template <typename ST>

@@ -35,6 +35,39 @@ static ag_status upload_column(Temps& t, const void* vals, const uint8_t* valid,
   return AG_OK;
 }
 
+// Stage one chunk of a BOOL or numeric column: a BOOL bitmap keeps its bit phase (upload_bitmap), other values are
+// rebased as upload_column does; d->offset addresses row 0 of the copies.  An empty chunk stages nothing.
+static ag_status upload_chunk(Temps& t, int type, const ag_sort_chunk& h, ag_sort_chunk* d) {
+  *d = ag_sort_chunk{nullptr, nullptr, 0, h.length};
+  if (h.length <= 0) return AG_OK;
+  uint8_t* dvalid;
+  if (type == AG_TYPE_BOOL) {
+    uint8_t* dv;
+    AG_TRY(upload_bitmap(t, static_cast<const uint8_t*>(h.vals), h.offset, h.length, &dv, &d->offset));
+    d->vals = dv;
+    int64_t phase;
+    AG_TRY(upload_bitmap(t, h.valid, h.offset, h.length, &dvalid, &phase));
+  } else {
+    AG_TRY(upload_column(t, h.vals, h.valid, h.offset, h.length, type_width(type), &d->vals, &dvalid, &d->offset));
+  }
+  d->valid = dvalid;
+  return AG_OK;
+}
+
+// AG_ERR_INDEX naming the host index at the lowest offending row `bad` (helpers.go:951), also stored in *bad_index.
+static ag_status index_bounds_error(const void* idx, int idx_width, int idx_signed, int64_t bad, int64_t* bad_index) {
+  int64_t v = 0;
+  switch (idx_width) {
+    case 8: v = idx_signed ? (int64_t)((const int8_t*)idx)[bad] : (int64_t)((const uint8_t*)idx)[bad]; break;
+    case 16: v = idx_signed ? (int64_t)((const int16_t*)idx)[bad] : (int64_t)((const uint16_t*)idx)[bad]; break;
+    case 32: v = idx_signed ? (int64_t)((const int32_t*)idx)[bad] : (int64_t)((const uint32_t*)idx)[bad]; break;
+    default: v = ((const int64_t*)idx)[bad]; break;
+  }
+  if (bad_index) *bad_index = v;
+  if (idx_width == 64 && !idx_signed) AG_FAIL(AG_ERR_INDEX, "%llu out of bounds", (unsigned long long)v);
+  AG_FAIL(AG_ERR_INDEX, "%lld out of bounds", (long long)v);
+}
+
 // Finish a call whose output has `len` rows: copy the output validity back when the caller passed a bitmap, set *nulls
 // to its clear bits when asked (d_count: one device int64 of scratch), and synchronise the stream.
 static ag_status fetch_validity(uint8_t* out_valid, const uint8_t* d_valid, int64_t len, int64_t* nulls, int64_t* d_count,
@@ -689,16 +722,7 @@ ag_status ag_take_primitive(int bit_width, const void* vals, const uint8_t* vval
   AG_TRY(sync(cs));
   if (bad != AG_NO_ERROR_POS) {
     if (bad_pos) *bad_pos = bad;
-    int64_t v = 0;
-    switch (idx_width) {
-      case 8: v = idx_signed ? (int64_t)((const int8_t*)idx)[bad] : (int64_t)((const uint8_t*)idx)[bad]; break;
-      case 16: v = idx_signed ? (int64_t)((const int16_t*)idx)[bad] : (int64_t)((const uint16_t*)idx)[bad]; break;
-      case 32: v = idx_signed ? (int64_t)((const int32_t*)idx)[bad] : (int64_t)((const uint32_t*)idx)[bad]; break;
-      default: v = ((const int64_t*)idx)[bad]; break;
-    }
-    if (bad_index) *bad_index = v;
-    if (idx_width == 64 && !idx_signed) AG_FAIL(AG_ERR_INDEX, "%llu out of bounds", (unsigned long long)v);
-    AG_FAIL(AG_ERR_INDEX, "%lld out of bounds", (long long)v);  // helpers.go:951
+    return index_bounds_error(idx, idx_width, idx_signed, bad, bad_index);
   }
   AG_TRY(d2h(out, dout, is_bool ? (size_t)((n + 7) / 8) : (size_t)n * w, cs));
   return fetch_validity(out_valid, dov, n, out_nulls, d_word + 1, cs);
@@ -734,24 +758,8 @@ ag_status ag_sort_indices_keys(int nkeys, const ag_sort_key* keys, int64_t n, ui
   std::vector<ag_sort_key> dkeys(keys, keys + nkeys);
   std::vector<std::vector<ag_sort_chunk>> dchunks(nkeys);
   for (int j = 0; j < nkeys; ++j) {
-    for (int c = 0; c < keys[j].nchunks; ++c) {
-      const ag_sort_chunk& ch = keys[j].chunks[c];
-      ag_sort_chunk d{nullptr, nullptr, 0, ch.length};
-      if (ch.length > 0) {
-        uint8_t* dvalid;
-        if (keys[j].type == AG_TYPE_BOOL) {
-          uint8_t* dv;
-          AG_TRY(upload_bitmap(t, (const uint8_t*)ch.vals, ch.offset, ch.length, &dv, &d.offset));
-          d.vals = dv;
-          int64_t phase;
-          AG_TRY(upload_bitmap(t, ch.valid, ch.offset, ch.length, &dvalid, &phase));
-        } else {
-          AG_TRY(upload_column(t, ch.vals, ch.valid, ch.offset, ch.length, type_width(keys[j].type), &d.vals, &dvalid, &d.offset));
-        }
-        d.valid = dvalid;
-      }
-      dchunks[j].push_back(d);
-    }
+    dchunks[j].resize(keys[j].nchunks);
+    for (int c = 0; c < keys[j].nchunks; ++c) AG_TRY(upload_chunk(t, keys[j].type, keys[j].chunks[c], &dchunks[j][c]));
     dkeys[j].chunks = dchunks[j].data();
   }
   uint64_t* dout;
@@ -774,27 +782,10 @@ ag_status ag_take_columns(int ncols, const ag_take_column* cols, int64_t nrows, 
   std::vector<ag_take_column> dcols(cols, cols + ncols);
   std::vector<std::vector<ag_sort_chunk>> dchunks(ncols);
   for (int j = 0; j < ncols; ++j) {
-    const bool is_bool = cols[j].type == AG_TYPE_BOOL;
-    for (int c = 0; c < cols[j].nchunks; ++c) {
-      const ag_sort_chunk& ch = cols[j].chunks[c];
-      ag_sort_chunk d{nullptr, nullptr, 0, ch.length};
-      if (ch.length > 0) {
-        uint8_t* dvalid;
-        if (is_bool) {
-          uint8_t* dv;
-          AG_TRY(upload_bitmap(t, (const uint8_t*)ch.vals, ch.offset, ch.length, &dv, &d.offset));
-          d.vals = dv;
-          int64_t phase;
-          AG_TRY(upload_bitmap(t, ch.valid, ch.offset, ch.length, &dvalid, &phase));
-        } else {
-          AG_TRY(upload_column(t, ch.vals, ch.valid, ch.offset, ch.length, type_width(cols[j].type), &d.vals, &dvalid, &d.offset));
-        }
-        d.valid = dvalid;
-      }
-      dchunks[j].push_back(d);
-    }
+    dchunks[j].resize(cols[j].nchunks);
+    for (int c = 0; c < cols[j].nchunks; ++c) AG_TRY(upload_chunk(t, cols[j].type, cols[j].chunks[c], &dchunks[j][c]));
     dcols[j].chunks = dchunks[j].data();
-    AG_TRY(t.alloc(&dcols[j].out, is_bool ? words : (size_t)n * type_width(cols[j].type)));
+    AG_TRY(t.alloc(&dcols[j].out, cols[j].type == AG_TYPE_BOOL ? words : (size_t)n * type_width(cols[j].type)));
     dcols[j].out_valid = nullptr;
     if (cols[j].out_valid) AG_TRY(t.alloc_t(&dcols[j].out_valid, words));
   }
@@ -814,16 +805,7 @@ ag_status ag_take_columns(int ncols, const ag_take_column* cols, int64_t nrows, 
   AG_TRY(sync(cs));
   if (bad != AG_NO_ERROR_POS) {
     if (bad_pos) *bad_pos = bad;
-    int64_t v = 0;
-    switch (idx_width) {
-      case 8: v = idx_signed ? (int64_t)((const int8_t*)idx)[bad] : (int64_t)((const uint8_t*)idx)[bad]; break;
-      case 16: v = idx_signed ? (int64_t)((const int16_t*)idx)[bad] : (int64_t)((const uint16_t*)idx)[bad]; break;
-      case 32: v = idx_signed ? (int64_t)((const int32_t*)idx)[bad] : (int64_t)((const uint32_t*)idx)[bad]; break;
-      default: v = ((const int64_t*)idx)[bad]; break;
-    }
-    if (bad_index) *bad_index = v;
-    if (idx_width == 64 && !idx_signed) AG_FAIL(AG_ERR_INDEX, "%llu out of bounds", (unsigned long long)v);
-    AG_FAIL(AG_ERR_INDEX, "%lld out of bounds", (long long)v);  // helpers.go:951
+    return index_bounds_error(idx, idx_width, idx_signed, bad, bad_index);
   }
   for (int j = 0; j < ncols; ++j) {
     const bool is_bool = cols[j].type == AG_TYPE_BOOL;
@@ -942,19 +924,11 @@ ag_status ag_dictionary_encode(int bit_width, const ag_dict_chunk* chunks, int64
   return sync(cs);
 }
 
-// Stage a values column for the run-end kernels: rows [off, off+n) of `vals` (a bitmap for BOOL) and `valid`, on the
-// device with the same row phase; *d_off is the offset that addresses row 0 of the copies.
-static ag_status upload_values(Temps& t, int type, const void* vals, const uint8_t* valid, int64_t off, int64_t n,
-                               const void** d_vals, uint8_t** d_valid, int64_t* d_off) {
-  if (type == AG_TYPE_BOOL) {
-    uint8_t* dv;
-    AG_TRY(upload_bitmap(t, static_cast<const uint8_t*>(vals), off, n, &dv, d_off));
-    *d_vals = dv;
-    int64_t phase;
-    return upload_bitmap(t, valid, off, n, d_valid, &phase);
-  }
-  if (type_width(type) == 0) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "run_end: type id %d (boolean and the 10 numeric types only)", type);
-  return upload_column(t, vals, valid, off, n, type_width(type), d_vals, d_valid, d_off);
+// Stage a values column for the run-end kernels: rows [off, off+n) of `vals` (a bitmap for BOOL) and `valid`
+// (upload_chunk).
+static ag_status upload_values(Temps& t, int type, const void* vals, const uint8_t* valid, int64_t off, int64_t n, ag_sort_chunk* d) {
+  if (type != AG_TYPE_BOOL && type_width(type) == 0) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "run_end: type id %d (boolean and the 10 numeric types only)", type);
+  return upload_chunk(t, type, ag_sort_chunk{vals, valid, off, n}, d);
 }
 static int run_end_width(int run_end_type) {
   return run_end_type == AG_TYPE_INT16 ? 2 : (run_end_type == AG_TYPE_INT32 ? 4 : (run_end_type == AG_TYPE_INT64 ? 8 : 0));
@@ -971,10 +945,10 @@ ag_status ag_run_end_count(int type, const void* vals, const uint8_t* valid, int
   if (!vals) AG_FAIL(AG_ERR_INVALID, "run_end_count: NULL values");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  const void* dv; uint8_t* dvv; int64_t ov; int64_t* dc;
-  AG_TRY(upload_values(t, type, vals, valid, offset, n, &dv, &dvv, &ov));
+  ag_sort_chunk v; int64_t* dc;
+  AG_TRY(upload_values(t, type, vals, valid, offset, n, &v));
   AG_TRY(t.alloc_t(&dc, 16));
-  AG_TRY(run_end_count_dev(type, dv, dvv, ov, n, dc, cs));
+  AG_TRY(run_end_count_dev(type, v.vals, v.valid, v.offset, n, dc, cs));
   AG_TRY(d2h(counts, dc, 16, cs));
   return sync(cs);
 }
@@ -992,14 +966,14 @@ ag_status ag_run_end_encode(int type, int run_end_type, const void* vals, const 
   if (n > 0 && !vals) AG_FAIL(AG_ERR_INVALID, "run_end_encode: NULL values");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  const void* dv = nullptr; uint8_t* dvv = nullptr; int64_t ov = 0; int64_t* dc;
+  ag_sort_chunk v{}; int64_t* dc;
   void *dre, *dout; uint8_t* dov = nullptr;
-  if (n > 0) AG_TRY(upload_values(t, type, vals, valid, offset, n, &dv, &dvv, &ov));
+  if (n > 0) AG_TRY(upload_values(t, type, vals, valid, offset, n, &v));
   AG_TRY(t.alloc(&dre, (size_t)capacity * rw));
   AG_TRY(t.alloc(&dout, type == AG_TYPE_BOOL ? word_bytes(capacity) : value_bytes(type, capacity)));
   if (valid) AG_TRY(t.alloc_t(&dov, word_bytes(capacity)));
   AG_TRY(t.alloc_t(&dc, 16));
-  AG_TRY(run_end_encode_dev(type, run_end_type, dv, dvv, ov, n, dre, dout, dov, capacity, dc, cs));
+  AG_TRY(run_end_encode_dev(type, run_end_type, v.vals, v.valid, v.offset, n, dre, dout, dov, capacity, dc, cs));
   AG_TRY(d2h(counts, dc, 16, cs));
   AG_TRY(sync(cs));
   const int64_t runs = counts[0] < capacity ? counts[0] : capacity;
@@ -1022,17 +996,17 @@ ag_status ag_run_end_decode(int type, int run_end_type, const void* run_ends, in
   if (valid && !out_valid) AG_FAIL(AG_ERR_INVALID, "run_end_decode: a values child with a validity bitmap needs an output validity bitmap");
   CallStream cs; AG_TRY(cs.acquire());
   Temps t(cs);
-  void *dre, *dout; const void* dv = nullptr; uint8_t *dvv = nullptr, *dov = nullptr; int64_t ov = 0; int64_t* dw;
+  void *dre, *dout, *z; ag_sort_chunk v{}; uint8_t *zv, *dov = nullptr; int64_t* dw;
   AG_TRY(t.alloc(&dre, (size_t)n_runs * rw));
   AG_TRY(h2d(dre, run_ends, (size_t)n_runs * rw, cs));
-  if (n_runs > 0) AG_TRY(upload_values(t, type, vals, valid, values_offset, n_runs, &dv, &dvv, &ov));
-  else { void* z; AG_TRY(t.alloc(&z, 8)); dv = z; }
-  if (valid && !dvv) AG_TRY(t.alloc_t(&dvv, 8));
+  if (n_runs > 0) AG_TRY(upload_values(t, type, vals, valid, values_offset, n_runs, &v));
+  else { AG_TRY(t.alloc(&z, 8)); v.vals = z; }
+  if (valid && !v.valid) { AG_TRY(t.alloc_t(&zv, 8)); v.valid = zv; }
   AG_TRY(t.alloc(&dout, type == AG_TYPE_BOOL ? word_bytes(length) : value_bytes(type, length)));
   if (valid) AG_TRY(t.alloc_t(&dov, word_bytes(length)));
   AG_TRY(t.alloc_t(&dw, 16));
   AG_TRY(error_word_reset(dw + 1, cs));
-  AG_TRY(run_end_decode_dev(type, run_end_type, dre, n_runs, dv, dvv, ov, offset, length, dout, dov, dw, dw + 1, cs));
+  AG_TRY(run_end_decode_dev(type, run_end_type, dre, n_runs, v.vals, v.valid, v.offset, offset, length, dout, dov, dw, dw + 1, cs));
   int64_t h[2];
   AG_TRY(d2h(h, dw, 16, cs));
   AG_TRY(sync(cs));

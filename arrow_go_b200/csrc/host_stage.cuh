@@ -16,6 +16,8 @@
 // asynchronous *_dev paths keep their scratch stream-ordered.
 #pragma once
 
+#include <string.h>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -59,6 +61,31 @@ static inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 struct Carve {
   size_t size = 0;
   size_t take(size_t nbytes) { const size_t r = size; size = align256(size + nbytes); return r; }
+};
+
+// Host tables of a *_dev call packed into one device image: add() copies a table into the next 256-byte aligned region
+// and returns its offset, upload() makes one allocation and one H2D copy, at<T>(offset) is the table on the device.
+// The image is freed (stream-ordered, after the work that reads it) when it goes out of scope.
+struct TableImage {
+  cudaStream_t st;
+  Carve carve;
+  std::vector<unsigned char> host;
+  void* dev = nullptr;
+  explicit TableImage(cudaStream_t s) : st(s) {}
+  ~TableImage() { dev_free_async(dev, st); }
+  template <typename T> size_t add(const std::vector<T>& v) {
+    static_assert(std::is_trivially_copyable<T>::value, "tables are copied as bytes");
+    const size_t off = carve.take(v.size() * sizeof(T));
+    host.resize(carve.size);
+    if (!v.empty()) memcpy(host.data() + off, v.data(), v.size() * sizeof(T));
+    return off;
+  }
+  ag_status upload(const char* what) {
+    AG_TRY(dev_alloc_async(&dev, carve.size, st));
+    const cudaError_t e = cudaMemcpyAsync(dev, host.data(), carve.size, cudaMemcpyHostToDevice, st);
+    return e == cudaSuccess ? AG_OK : cuda_fail(e, what, __FILE__, __LINE__);
+  }
+  template <typename T> T* at(size_t off) const { return reinterpret_cast<T*>(static_cast<char*>(dev) + off); }
 };
 
 // Upload the bytes of a bitmap range [off, off+n) to a device temp; the device copy keeps the

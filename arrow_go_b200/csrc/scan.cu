@@ -690,14 +690,7 @@ cumsum_stream_kernel(const CumsumParams p) {
       }
     }
   }
-  if (kChecked) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, d);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.first_bad, my_bad);
-  }
+  if (kChecked) lower_error_row(my_bad, p.first_bad);
 }
 
 // first 0 bit of validity[voff, voff+n): one thread per 32 rows, atomicMin into *first_null (pre-set to n)
@@ -705,19 +698,14 @@ __global__ void __launch_bounds__(256)
 first_null_kernel(const uint8_t* __restrict__ valid, int64_t voff, int64_t n, long long* first_null) {
   const int64_t vlo = voff >> 3, vhi = (voff + n + 7) >> 3;
   const int64_t n_words = (n + 31) >> 5;
-  long long mine = n;
+  long long mine = AG_NO_ERROR_POS;
   for (int64_t w = (int64_t)blockIdx.x * 256 + threadIdx.x; w < n_words; w += (int64_t)gridDim.x * 256) {
     uint32_t bits = bitmap_load32(valid, voff + w * 32, vlo, vhi);
     const int64_t room = n - w * 32;
     if (room < 32) bits |= ~((1u << (int)room) - 1u);  // rows past n count as valid
     if (bits != 0xffffffffu) { const long long r = w * 32 + (__ffs(~bits) - 1); if (r < mine) mine = r; break; }  // rows only grow with w
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    const long long o = __shfl_xor_sync(0xffffffffu, mine, d);
-    mine = o < mine ? o : mine;
-  }
-  if ((threadIdx.x & 31) == 0 && mine < n) atomicMin(first_null, mine);
+  lower_error_row(mine, first_null);
 }
 
 __global__ void set_i64_kernel(long long* p, long long v) { *p = v; }

@@ -26,9 +26,8 @@
 // Roofline: HBM; per digit pass 8 (histogram read) + 12 + 12 bytes/row for 64-bit keys (first pass from the source:
 // 8 + 8 + 12; last pass: 8 + 12 + 8); the gathers are never random (pairs move with their rows).  The API is synchronous
 // in one spot: the 40-byte read-back after K0.
-#include "common.cuh"
+#include "host_stage.cuh"
 
-#include <string.h>
 #include <algorithm>
 #include <type_traits>
 #include <vector>
@@ -884,6 +883,20 @@ static ag_status sk_digit_passes(const K* words, int64_t n, int bits, char* body
   return AG_OK;
 }
 
+ag_status check_chunk_list(const char* who, int j, int nchunks, const ag_sort_chunk* chunks, int64_t nrows, const char* rows_name) {
+  if (nchunks < 0 || (nchunks > 0 && !chunks)) AG_FAIL(AG_ERR_INVALID, "%s %d: bad chunk list", who, j);
+  int64_t rows = 0;
+  for (int c = 0; c < nchunks; ++c) {
+    const ag_sort_chunk& ch = chunks[c];
+    if (ch.offset < 0 || ch.length < 0) AG_FAIL(AG_ERR_INVALID, "%s %d: negative chunk offset or length", who, j);
+    if (ch.length > 0 && !ch.vals) AG_FAIL(AG_ERR_INVALID, "%s %d: NULL chunk values", who, j);
+    rows += ch.length;
+  }
+  if (rows != nrows)
+    AG_FAIL(AG_ERR_INVALID, "%s %d: chunk row count %lld does not match %s %lld", who, j, (long long)rows, rows_name, (long long)nrows);
+  return AG_OK;
+}
+
 ag_status sort_indices_keys_check(int nkeys, const ag_sort_key* keys, int64_t n) {
   if (nkeys < 1 || !keys) AG_FAIL(AG_ERR_INVALID, "sort_indices: must provide at least one sort key");
   if (n < 0) AG_FAIL(AG_ERR_INVALID, "sort_indices: negative length");
@@ -891,15 +904,7 @@ ag_status sort_indices_keys_check(int nkeys, const ag_sort_key* keys, int64_t n)
     const ag_sort_key& k = keys[j];
     if (k.order != 0 && k.order != 1) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: order must be 0 (ascending) or 1 (descending)", j);
     if (k.null_placement != 0 && k.null_placement != 1) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: null placement must be 0 (at end) or 1 (at start)", j);
-    if (k.nchunks < 0 || (k.nchunks > 0 && !k.chunks)) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: bad chunk list", j);
-    int64_t rows = 0;
-    for (int c = 0; c < k.nchunks; ++c) {
-      const ag_sort_chunk& ch = k.chunks[c];
-      if (ch.offset < 0 || ch.length < 0) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: negative chunk offset or length", j);
-      if (ch.length > 0 && !ch.vals) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: NULL chunk values", j);
-      rows += ch.length;
-    }
-    if (rows != n) AG_FAIL(AG_ERR_INVALID, "sort_indices: sort key %d: chunk row count %lld does not match column length %lld", j, (long long)rows, (long long)n);
+    AG_TRY(check_chunk_list("sort_indices: sort key", j, k.nchunks, k.chunks, n, "column length"));
     if (k.type != AG_TYPE_BOOL && type_width(k.type) == 0)
       AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "sort_indices: sort key %d: unsupported type id %d (boolean and numeric columns only)", j, k.type);
   }
@@ -920,33 +925,23 @@ ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, u
     k.descending = keys[j].order;
     p.keys.push_back(k);
   }
-  // head: statistics | key plans | chunks | spans | span chunks; freed on every return path
-  const size_t o_keys = ((size_t)nkeys * kSkStats * 8 + 255) & ~(size_t)255;
-  const size_t o_chunks = o_keys + (((size_t)nkeys * sizeof(SkKey) + 255) & ~(size_t)255);
-  const size_t o_spans = o_chunks + ((p.chunks.size() * sizeof(SkChunk) + 255) & ~(size_t)255);
-  const size_t o_sc = o_spans + ((p.spans.size() * sizeof(SkSpan) + 255) & ~(size_t)255);
-  const size_t head_bytes = o_sc + p.span_chunk.size() * sizeof(int);
-  std::vector<unsigned long long> h(head_bytes / 8 + 1, 0);   // staged as one host image, one copy
-  char* hb = reinterpret_cast<char*>(h.data());
-  for (int j = 0; j < nkeys; ++j) { h[j * kSkStats + 0] = ~0ull; h[j * kSkStats + 3] = ~0ull; }
-  memcpy(hb + o_chunks, p.chunks.data(), p.chunks.size() * sizeof(SkChunk));
-  memcpy(hb + o_spans, p.spans.data(), p.spans.size() * sizeof(SkSpan));
-  memcpy(hb + o_sc, p.span_chunk.data(), p.span_chunk.size() * sizeof(int));
-  void* head = nullptr;
-  void* body = nullptr;
-  AG_TRY(dev_alloc_async(&head, head_bytes, st));
-  char* hd = reinterpret_cast<char*>(head);
-  unsigned long long* d_stats = reinterpret_cast<unsigned long long*>(hd);
-  SkKey* d_keys = reinterpret_cast<SkKey*>(hd + o_keys);
-  const SkChunk* d_chunks = reinterpret_cast<const SkChunk*>(hd + o_chunks);
-  const SkSpan* d_spans = reinterpret_cast<const SkSpan*>(hd + o_spans);
-  const int* d_sc = reinterpret_cast<const int*>(hd + o_sc);
+  // head: statistics | key plans | chunks | spans | span chunks
+  std::vector<unsigned long long> stats((size_t)nkeys * kSkStats, 0);
+  for (int j = 0; j < nkeys; ++j) { stats[j * kSkStats + 0] = ~0ull; stats[j * kSkStats + 3] = ~0ull; }
+  TableImage head(st);
+  const size_t o_stats = head.add(stats), o_keys = head.add(p.keys), o_chunks = head.add(p.chunks), o_spans = head.add(p.spans),
+               o_sc = head.add(p.span_chunk);
+  AG_TRY(head.upload("sort key tables"));
+  unsigned long long* d_stats = head.at<unsigned long long>(o_stats);
+  SkKey* d_keys = head.at<SkKey>(o_keys);
+  const SkChunk* d_chunks = head.at<const SkChunk>(o_chunks);
+  const SkSpan* d_spans = head.at<const SkSpan>(o_spans);
+  const int* d_sc = head.at<const int>(o_sc);
   const int nspans = (int)p.spans.size();
   unsigned long long* out = reinterpret_cast<unsigned long long*>(d_out);
+  void* body = nullptr;
   ag_status rc = AG_OK;
   do {
-    memcpy(hb + o_keys, p.keys.data(), (size_t)nkeys * sizeof(SkKey));
-    if (cudaMemcpyAsync(head, hb, head_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "sort key tables", __FILE__, __LINE__); break; }
     // ---- P0: statistics of every key, one read-back
     const dim3 pgrid((unsigned)grid_for(n, kSoTile, std::max(1, 8 / nkeys)), (unsigned)nkeys);
     sort_keys_prep_kernel<<<pgrid, kSoThreads, 0, st>>>(d_keys, d_chunks, d_spans, d_sc, nspans, nkeys, p.ntiles, d_stats);
@@ -979,8 +974,7 @@ ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, u
       rc = check_launch("sort_iota_kernel");
       break;
     }
-    memcpy(hb + o_keys, p.keys.data(), (size_t)nkeys * sizeof(SkKey));
-    if (cudaMemcpyAsync(d_keys, hb + o_keys, (size_t)nkeys * sizeof(SkKey), cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "sort key plans", __FILE__, __LINE__); break; }
+    if (cudaMemcpyAsync(d_keys, p.keys.data(), (size_t)nkeys * sizeof(SkKey), cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "sort key plans", __FILE__, __LINE__); break; }
     // body: totals of every pass | segment sums | packed words | pairs x2 | indices x2 | tile histograms
     const bool narrow = bits <= 32;
     const size_t kw = narrow ? 4 : 8;
@@ -1007,10 +1001,8 @@ ag_status sort_indices_keys_dev(int nkeys, const ag_sort_key* keys, int64_t n, u
     if (narrow) rc = sk_digit_passes<uint32_t>(reinterpret_cast<const uint32_t*>(wbase), n, bits, wbase, words_bytes, d_tot, d_seg, out, st);
     else rc = sk_digit_passes<unsigned long long>(reinterpret_cast<const unsigned long long*>(wbase), n, bits, wbase, words_bytes, d_tot, d_seg, out, st);
   } while (0);
-  const ag_status frc_body = body ? dev_free_async(body, st) : AG_OK;
-  const ag_status frc = dev_free_async(head, st);
-  if (rc != AG_OK) return rc;
-  return frc_body != AG_OK ? frc_body : frc;
+  const ag_status frc = dev_free_async(body, st);
+  return rc != AG_OK ? rc : frc;
 }
 
 }  // namespace ag

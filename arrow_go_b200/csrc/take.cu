@@ -71,7 +71,6 @@ take_kernel(const TakeParams p) {
   const V* __restrict__ vals = reinterpret_cast<const V*>(p.vals) + p.voff;
   const I* __restrict__ idx = reinterpret_cast<const I*>(p.idx);
   V* __restrict__ out = reinterpret_cast<V*>(p.out);
-  constexpr I kSignBit = (I)((I)1 << (sizeof(I) * 8 - 1));
   const int lane = threadIdx.x & 31;
   const int64_t step = (int64_t)gridDim.x * kTkThreads * kTkUnroll;
   long long my_bad = AG_NO_ERROR_POS;
@@ -94,9 +93,7 @@ take_kernel(const TakeParams p) {
     for (int k = 0; k < kTkUnroll; ++k) {
       v[k] = V(0);
       if (ok[k]) {
-        const bool neg = p.idx_signed && (ix[k] & kSignBit);
-        const bool oob = neg || (unsigned long long)ix[k] >= p.vlen;
-        if (oob) {
+        if (take_index_oob(ix[k], p.vlen, p.idx_signed)) {
           ok[k] = false;  // never dereference; with bounds_check the whole call fails anyway
           if (p.bounds_check) {
             const long long i = base + k * kTkThreads + threadIdx.x;
@@ -114,23 +111,11 @@ take_kernel(const TakeParams p) {
       if (i < p.n) __stcs(out + i, v[k]);
       if (p.out_valid) {
         const int64_t w = (base + k * kTkThreads + (threadIdx.x & ~31)) >> 5;  // warp-uniform
-        const uint32_t bits = __ballot_sync(0xffffffffu, ok[k]);
-        const int64_t rem = p.n - (w << 5);
-        if (lane == 0 && rem > 0) {
-          if (rem >= 32) p.out_valid[w] = bits;
-          else bitmap_store32_masked(p.out_valid + w, bits, bit_range_mask(0, (int)rem));
-        }
+        store_valid_word(p.out_valid, w, __ballot_sync(0xffffffffu, ok[k]), p.n, lane);
       }
     }
   }
-  if (p.bounds_check) {
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.bad_pos, my_bad);
-  }
+  if (p.bounds_check) lower_error_row(my_bad, p.bad_pos);
 }
 
 // booleanTakeImpl (vector_selection.go:990-1074): out bit i = values bit [voff + idx[i]]; same
@@ -141,7 +126,6 @@ take_bool_kernel(const TakeParams p) {
   const uint8_t* __restrict__ vals = reinterpret_cast<const uint8_t*>(p.vals);
   const I* __restrict__ idx = reinterpret_cast<const I*>(p.idx);
   uint32_t* __restrict__ out = reinterpret_cast<uint32_t*>(p.out);
-  constexpr I kSignBit = (I)((I)1 << (sizeof(I) * 8 - 1));
   const int lane = threadIdx.x & 31;
   const int64_t step = (int64_t)gridDim.x * kTkThreads;
   long long my_bad = AG_NO_ERROR_POS;
@@ -152,8 +136,7 @@ take_bool_kernel(const TakeParams p) {
       const I ix = idx[i];
       if (p.ivalid) ok = bit_is_set(p.ivalid, p.ioff + i);
       if (ok) {
-        const bool oob = (p.idx_signed && (ix & kSignBit)) || (unsigned long long)ix >= p.vlen;
-        if (oob) {
+        if (take_index_oob(ix, p.vlen, p.idx_signed)) {
           ok = false;
           if (p.bounds_check && (long long)i < my_bad) my_bad = (long long)i;
         } else {
@@ -165,21 +148,9 @@ take_bool_kernel(const TakeParams p) {
     const int64_t w = (base + (threadIdx.x & ~31)) >> 5;
     const uint32_t dbits = __ballot_sync(0xffffffffu, bit);
     const uint32_t vbits = __ballot_sync(0xffffffffu, ok);
-    const int64_t rem = p.n - (w << 5);
-    if (lane == 0 && rem > 0) {
-      const uint32_t m = rem >= 32 ? 0xffffffffu : bit_range_mask(0, (int)rem);
-      bitmap_store32_masked(out + w, dbits, m);
-      if (p.out_valid) bitmap_store32_masked(p.out_valid + w, vbits, m);
-    }
+    store_bool_words(out, p.out_valid, w, dbits, vbits, p.n, lane);
   }
-  if (p.bounds_check) {
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.bad_pos, my_bad);
-  }
+  if (p.bounds_check) lower_error_row(my_bad, p.bad_pos);
 }
 
 static ag_status launch_take_bool(int idx_width, const TakeParams& p, cudaStream_t st) {
@@ -398,15 +369,7 @@ take_partition_kernel(const TakeParams p, const TakeWindowPlan w, uint32_t* __re
     else partition_tile<I, kValid, false>(p, w, sh, idx, tile, limit, sorted, perm, off, bad_local);
     if (bad_local != 0xffffffffu && tile * kWinTile + bad_local < my_bad) my_bad = tile * kWinTile + bad_local;
   }
-  if (p.bounds_check) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.bad_pos, my_bad);
-  }
+  if (p.bounds_check) lower_error_row(my_bad, p.bad_pos);
 }
 
 // off[tile][slot] -> offT[slot][tile] (pass A writes one contiguous row per tile, pass B reads one contiguous run of

@@ -17,7 +17,7 @@
 //
 // Bytes per output row: the index (1-8 B) once, then per column one gathered value (a 32 B sector for random indices
 // into a column larger than L2), one value write and one validity bit.
-#include "common.cuh"
+#include "host_stage.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -85,12 +85,7 @@ __device__ __forceinline__ void tc_gather(const TcParams& p, const TcColumn& col
     if (i < p.n) __stcs(out + i, v[k]);
     if (col.out_valid) {
       const int64_t w = (base + k * kTcThreads + (threadIdx.x & ~31)) >> 5;   // warp-uniform
-      const uint32_t bits = __ballot_sync(0xffffffffu, ok[k]);
-      const int64_t rem = p.n - (w << 5);
-      if (lane == 0 && rem > 0) {
-        if (rem >= 32) col.out_valid[w] = bits;
-        else bitmap_store32_masked(col.out_valid + w, bits, bit_range_mask(0, (int)rem));
-      }
+      store_valid_word(col.out_valid, w, __ballot_sync(0xffffffffu, ok[k]), p.n, lane);
     }
   }
 }
@@ -115,12 +110,7 @@ __device__ __forceinline__ void tc_gather_bool(const TcParams& p, const TcColumn
     const int64_t w = (base + k * kTcThreads + (threadIdx.x & ~31)) >> 5;
     const uint32_t dbits = __ballot_sync(0xffffffffu, bit[k]);
     const uint32_t vbits = __ballot_sync(0xffffffffu, ok[k]);
-    const int64_t rem = p.n - (w << 5);
-    if (lane == 0 && rem > 0) {
-      const uint32_t m = rem >= 32 ? 0xffffffffu : bit_range_mask(0, (int)rem);
-      bitmap_store32_masked(out + w, dbits, m);
-      if (col.out_valid) bitmap_store32_masked(col.out_valid + w, vbits, m);
-    }
+    store_bool_words(out, col.out_valid, w, dbits, vbits, p.n, lane);
   }
 }
 
@@ -151,7 +141,7 @@ take_columns_kernel(const TcParams p) {
         const I ix = __ldcs(idx + i);
         live[k] = !p.ivalid || bit_is_set(p.ivalid, p.ioff + i);
         if (live[k]) {
-          const bool oob = (p.idx_signed && (ix & kSignBit)) || (unsigned long long)ix >= p.nrows;
+          const bool oob = (p.idx_signed && (ix & kSignBit)) || (unsigned long long)ix >= p.nrows;   // take_index_oob
           if (oob) {
             live[k] = false;   // never dereferenced; with bounds_check the whole call fails anyway
             if (p.bounds_check && i < my_bad) my_bad = i;
@@ -185,14 +175,7 @@ take_columns_kernel(const TcParams p) {
       }
     }
   }
-  if (p.bounds_check) {
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      const long long o = __shfl_xor_sync(0xffffffffu, my_bad, m);
-      my_bad = o < my_bad ? o : my_bad;
-    }
-    if (lane == 0 && my_bad != AG_NO_ERROR_POS) atomicMin(p.bad_pos, my_bad);
-  }
+  if (p.bounds_check) lower_error_row(my_bad, p.bad_pos);
 }
 
 static int tc_bits(int type) { return type == AG_TYPE_BOOL ? 1 : type_width(type) * 8; }
@@ -205,16 +188,7 @@ ag_status take_columns_check(int ncols, const ag_take_column* cols, int64_t nrow
     const ag_take_column& c = cols[j];
     if (c.type != AG_TYPE_BOOL && type_width(c.type) == 0)
       AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "take_columns: column %d: unsupported type id %d (boolean and numeric columns only)", j, c.type);
-    if (c.nchunks < 0 || (c.nchunks > 0 && !c.chunks)) AG_FAIL(AG_ERR_INVALID, "take_columns: column %d: bad chunk list", j);
-    int64_t rows = 0;
-    for (int k = 0; k < c.nchunks; ++k) {
-      const ag_sort_chunk& ch = c.chunks[k];
-      if (ch.offset < 0 || ch.length < 0) AG_FAIL(AG_ERR_INVALID, "take_columns: column %d: negative chunk offset or length", j);
-      if (ch.length > 0 && !ch.vals) AG_FAIL(AG_ERR_INVALID, "take_columns: column %d: NULL chunk values", j);
-      rows += ch.length;
-    }
-    if (rows != nrows)
-      AG_FAIL(AG_ERR_INVALID, "take_columns: column %d: chunk row count %lld does not match row count %lld", j, (long long)rows, (long long)nrows);
+    AG_TRY(check_chunk_list("take_columns: column", j, c.nchunks, c.chunks, nrows, "row count"));
     if (n > 0 && !c.out) AG_FAIL(AG_ERR_INVALID, "take_columns: column %d: NULL output", j);
   }
   return AG_OK;
@@ -265,27 +239,15 @@ ag_status take_columns_dev(int ncols, const ag_take_column* cols, int64_t nrows,
   }
   std::stable_sort(tcols.begin(), tcols.end(), [](const TcColumn& a, const TcColumn& b) { return a.layout < b.layout; });
   if (starts.size() > (size_t)INT32_MAX || chunks.size() > (size_t)INT32_MAX) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "take_columns: too many chunks");
-  // one device image: columns | layouts | chunks | starts
-  auto align256 = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t o_lay = align256(tcols.size() * sizeof(TcColumn));
-  const size_t o_ch = o_lay + align256(layouts.size() * sizeof(TcLayout));
-  const size_t o_st = o_ch + align256(chunks.size() * sizeof(TcChunk));
-  const size_t bytes = o_st + starts.size() * sizeof(int64_t) + 8;
-  std::vector<unsigned long long> h(bytes / 8 + 1, 0);
-  char* hb = reinterpret_cast<char*>(h.data());
-  if (!tcols.empty()) memcpy(hb, tcols.data(), tcols.size() * sizeof(TcColumn));
-  if (!layouts.empty()) memcpy(hb + o_lay, layouts.data(), layouts.size() * sizeof(TcLayout));
-  if (!chunks.empty()) memcpy(hb + o_ch, chunks.data(), chunks.size() * sizeof(TcChunk));
-  if (!starts.empty()) memcpy(hb + o_st, starts.data(), starts.size() * sizeof(int64_t));
-  void* head = nullptr;
-  AG_TRY(dev_alloc_async(&head, bytes, st));
-  char* hd = reinterpret_cast<char*>(head);
+  TableImage img(st);
+  const size_t o_col = img.add(tcols), o_lay = img.add(layouts), o_ch = img.add(chunks), o_st = img.add(starts);
+  AG_TRY(img.upload("take_columns tables"));
   TcParams p{};
-  p.cols = reinterpret_cast<const TcColumn*>(hd);
+  p.cols = img.at<const TcColumn>(o_col);
   p.ncols = (int)tcols.size();
-  p.layouts = reinterpret_cast<const TcLayout*>(hd + o_lay);
-  p.chunks = reinterpret_cast<const TcChunk*>(hd + o_ch);
-  p.starts = reinterpret_cast<const int64_t*>(hd + o_st);
+  p.layouts = img.at<const TcLayout>(o_lay);
+  p.chunks = img.at<const TcChunk>(o_ch);
+  p.starts = img.at<const int64_t>(o_st);
   p.nstarts = (int)starts.size();
   p.starts_in_smem = p.nstarts <= kTcSmemStarts;
   p.nrows = (unsigned long long)nrows;
@@ -293,19 +255,12 @@ ag_status take_columns_dev(int ncols, const ag_take_column* cols, int64_t nrows,
   p.idx_signed = idx_signed; p.bounds_check = bounds_check;
   p.bad_pos = reinterpret_cast<long long*>(d_bad_pos);
   const size_t smem = p.starts_in_smem ? (size_t)p.nstarts * sizeof(int64_t) : 0;
-  ag_status rc = AG_OK;
-  if (cudaMemcpyAsync(head, hb, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-    rc = cuda_fail(cudaGetLastError(), "take_columns tables", __FILE__, __LINE__);
-  } else {
-    const int64_t need = (n + kTcThreads * kTcUnroll - 1) / (kTcThreads * kTcUnroll);
-    rc = visit_width(idx_width, [&](auto tag) {
-      const auto kernel = take_columns_kernel<typename decltype(tag)::type>;
-      kernel<<<grid_one_wave(kernel, kTcThreads, need), kTcThreads, smem, st>>>(p);
-      return check_launch("take_columns_kernel");
-    }, [&] { AG_FAIL(AG_ERR_INDEX, "take_columns: invalid indices byte width"); });
-  }
-  const ag_status frc = dev_free_async(head, st);
-  return rc != AG_OK ? rc : frc;
+  const int64_t need = (n + kTcThreads * kTcUnroll - 1) / (kTcThreads * kTcUnroll);
+  return visit_width(idx_width, [&](auto tag) {
+    const auto kernel = take_columns_kernel<typename decltype(tag)::type>;
+    kernel<<<grid_one_wave(kernel, kTcThreads, need), kTcThreads, smem, st>>>(p);
+    return check_launch("take_columns_kernel");
+  }, [&] { AG_FAIL(AG_ERR_INDEX, "take_columns: invalid indices byte width"); });
 }
 
 }  // namespace ag

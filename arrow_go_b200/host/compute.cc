@@ -828,6 +828,37 @@ inline const uint8_t* ValuesPtr(const ArraySpan& a) {  // exec.GetSpanValues: Bu
 }
 inline uint8_t* ValuesPtr(ExecResult* a) { return a->buffers[1].buf + a->offset * (BitWidth(a->type) / 8); }
 
+// The validity bitmap a kernel reads, or nullptr when the array has none or no nulls.
+const uint8_t* ValidityOrNull(const ArrayData& a) { return a.buffers[0] && a.null_count != 0 ? a.buffers[0]->data() : nullptr; }
+bool MayHaveNulls(const ArrayData& a) { return ValidityOrNull(a) != nullptr; }
+bool MayHaveNulls(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
+  for (auto& c : chunks) if (MayHaveNulls(*c)) return true;
+  return false;
+}
+
+// The chunk list of a column for ag_sort_indices_keys_dev / ag_take_columns_dev.
+std::vector<ag_sort_chunk> ChunkDescs(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
+  std::vector<ag_sort_chunk> d;
+  for (auto& a : chunks) d.push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, ValidityOrNull(*a), a->offset, a->length});
+  return d;
+}
+
+// The IndexError naming the index at row `row` of the `type` indices starting at element `offset` of `buf` (helpers.go:951).
+Status IndexOutOfBounds(const Buffer& buf, Type type, int64_t offset, int64_t row) {
+  const int iw = BitWidth(type) / 8;
+  uint8_t raw[8] = {0};
+  RETURN_NOT_OK(buf.ToHost(raw, iw, (offset + row) * iw));
+  if (IsSignedInteger(type)) {
+    long long v = 0;
+    switch (iw) { case 1: v = (int8_t)raw[0]; break; case 2: { int16_t t; memcpy(&t, raw, 2); v = t; break; }
+                  case 4: { int32_t t; memcpy(&t, raw, 4); v = t; break; } default: memcpy(&v, raw, 8); }
+    return Status::IndexError(std::to_string(v) + " out of bounds");
+  }
+  unsigned long long uv = 0;
+  memcpy(&uv, raw, 8);
+  return Status::IndexError(std::to_string(uv) + " out of bounds");
+}
+
 const std::vector<Type>& kNumericTypesForCast() {
   static const std::vector<Type> v = {Type::UINT8, Type::INT8, Type::UINT16, Type::INT16, Type::UINT32, Type::INT32,
                                       Type::UINT64, Type::INT64, Type::FLOAT32, Type::FLOAT64};
@@ -1332,19 +1363,7 @@ Status PrimitiveTakeExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out)
   if (bounds) {
     int64_t bad = 0;
     RETURN_NOT_OK(word->ToHost(&bad, 8));
-    if (bad != AG_NO_ERROR_POS) {
-      // "%d out of bounds" with the offending index value (helpers.go:951)
-      uint8_t raw[8] = {0};
-      RETURN_NOT_OK(indices.buffers[1].owner->ToHost(raw, iw / 8, (indices.offset + bad) * (iw / 8)));
-      long long v = 0; unsigned long long uv = 0;
-      memcpy(&uv, raw, 8);
-      if (IsSignedInteger(indices.type)) {
-        switch (iw) { case 8: v = (int8_t)raw[0]; break; case 16: { int16_t t; memcpy(&t, raw, 2); v = t; break; }
-                      case 32: { int32_t t; memcpy(&t, raw, 4); v = t; break; } default: memcpy(&v, raw, 8); }
-        return Status::IndexError(std::to_string(v) + " out of bounds");
-      }
-      return Status::IndexError(std::to_string(uv) + " out of bounds");
-    }
+    if (bad != AG_NO_ERROR_POS) return IndexOutOfBounds(*indices.buffers[1].owner, indices.type, indices.offset, bad);
   }
   return Status::OK();
 }
@@ -1717,14 +1736,13 @@ Status ConcatenateChunks(const ChunkedArray& c, std::shared_ptr<ArrayData>* out)
   const int w = BitWidth(c.type) / 8;
   if (w == 0) return Status::NotImplemented("concatenate of boolean chunks");
   RETURN_NOT_OK(Buffer::Allocate(c.length * w, &d->buffers[1]));
-  bool any_nulls = false;
-  for (auto& ch : c.chunks) any_nulls = any_nulls || (ch->buffers[0] && ch->null_count != 0);
+  const bool any_nulls = MayHaveNulls(c.chunks);
   if (any_nulls) RETURN_NOT_OK(Buffer::Allocate((c.length + 7) / 8, &d->buffers[0]));
   int64_t pos = 0;
   for (auto& ch : c.chunks) {
     NATIVE(ag_copy_dev(d->buffers[1]->data() + pos * w, ch->buffers[1]->data() + ch->offset * w, (size_t)(ch->length * w), nullptr));
     if (any_nulls) {
-      if (ch->buffers[0] && ch->null_count != 0) NATIVE(ag_bitmap_copy_dev(ch->buffers[0]->data(), ch->offset, ch->length, d->buffers[0]->data(), pos, nullptr));
+      if (MayHaveNulls(*ch)) NATIVE(ag_bitmap_copy_dev(ch->buffers[0]->data(), ch->offset, ch->length, d->buffers[0]->data(), pos, nullptr));
       else NATIVE(ag_bitmap_set_dev(d->buffers[0]->data(), pos, ch->length, 1, nullptr));
     }
     pos += ch->length;
@@ -1784,8 +1802,7 @@ Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortOptions& op
   std::shared_ptr<Buffer> idx;
   RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(a->length, 1) * 8, &idx));
   int64_t nulls = 0, nans = 0;
-  const uint8_t* valid = (a->buffers[0] && a->null_count != 0) ? a->buffers[0]->data() : nullptr;
-  NATIVE(ag_sort_indices_dev((int)a->type, a->buffers[1] ? a->buffers[1]->data() : nullptr, valid, a->offset, a->length, (int)opts.Order, (int)opts.Placement,
+  NATIVE(ag_sort_indices_dev((int)a->type, a->buffers[1] ? a->buffers[1]->data() : nullptr, ValidityOrNull(*a), a->offset, a->length, (int)opts.Order, (int)opts.Placement,
                              (uint64_t*)idx->data(), &nulls, &nans, nullptr));
   return MakeOut(Type::UINT64, a->length, idx, nullptr, 0, out);
 }
@@ -1830,10 +1847,7 @@ Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortKeys& opts,
   std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
   std::vector<ag_sort_key> desc(cols.size());
   for (size_t i = 0; i < cols.size(); ++i) {
-    for (auto& a : cols[i].second) {
-      const uint8_t* valid = (a->buffers[0] && a->null_count != 0) ? a->buffers[0]->data() : nullptr;
-      chunks[i].push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, valid, a->offset, a->length});
-    }
+    chunks[i] = ChunkDescs(cols[i].second);
     desc[i] = ag_sort_key{(int)cols[i].first, (int)keys[i].Order, (int)keys[i].Placement, (int)chunks[i].size(), chunks[i].data()};
   }
   std::shared_ptr<Buffer> idx;
@@ -1858,11 +1872,6 @@ Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table,
 // for FilterTable), never one launch per column.  Arrays and chunked arrays keep the "take" meta function's own path.
 namespace {
 bool SelectionType(Type t) { return t == Type::BOOL || IsNumeric(t); }
-bool MayHaveNulls(const ArrayData& a) { return a.buffers[0] != nullptr && a.null_count != 0; }
-bool MayHaveNulls(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
-  for (auto& c : chunks) if (MayHaveNulls(*c)) return true;
-  return false;
-}
 
 // One column of a selection: its type and chunks (a record batch column is one chunk).
 struct SelColumn { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
@@ -1901,34 +1910,10 @@ Status GatherColumns(const std::vector<SelColumn>& cols, const std::vector<std::
     desc[c] = ag_take_column{(int)cols[c].type, (int)chunks[c].size(), chunks[c].data(), outs[c]->buffers[1]->data(),
                              outs[c]->buffers[0] ? outs[c]->buffers[0]->data() : nullptr};
   const int iw = BitWidth(idx.type);
-  const uint8_t* ivalid = MayHaveNulls(idx) ? idx.buffers[0]->data() : nullptr;
   const void* iptr = idx.buffers[1] ? idx.buffers[1]->data() + idx.offset * (iw / 8) : nullptr;
-  NATIVE(ag_take_columns_dev((int)desc.size(), desc.data(), nrows, iw, IsSignedInteger(idx.type), iptr, ivalid, idx.offset, idx.length,
+  NATIVE(ag_take_columns_dev((int)desc.size(), desc.data(), nrows, iw, IsSignedInteger(idx.type), iptr, ValidityOrNull(idx), idx.offset, idx.length,
                              bounds ? 1 : 0, d_bad, nullptr));
   return Status::OK();
-}
-
-std::vector<ag_sort_chunk> ChunkDescs(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
-  std::vector<ag_sort_chunk> d;
-  for (auto& a : chunks)
-    d.push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, MayHaveNulls(*a) ? a->buffers[0]->data() : nullptr, a->offset, a->length});
-  return d;
-}
-
-// "%d out of bounds" with the index at row `bad` of `idx` (helpers.go:951), as PrimitiveTakeExec reports it
-Status BoundsError(const ArrayData& idx, int64_t bad) {
-  const int iw = BitWidth(idx.type) / 8;
-  uint8_t raw[8] = {0};
-  RETURN_NOT_OK(idx.buffers[1]->ToHost(raw, iw, (idx.offset + bad) * iw));
-  if (IsSignedInteger(idx.type)) {
-    long long v = 0;
-    switch (iw) { case 1: v = (int8_t)raw[0]; break; case 2: { int16_t t; memcpy(&t, raw, 2); v = t; break; }
-                  case 4: { int32_t t; memcpy(&t, raw, 4); v = t; break; } default: memcpy(&v, raw, 8); }
-    return Status::IndexError(std::to_string(v) + " out of bounds");
-  }
-  unsigned long long uv = 0;
-  memcpy(&uv, raw, 8);
-  return Status::IndexError(std::to_string(uv) + " out of bounds");
 }
 
 // takeRecordImpl (selection.go:160-204) and takeTableImpl -> takeChunkedImpl -> ChunkedPrimitiveTake (:117-158, 246-300,
@@ -1974,7 +1959,7 @@ Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Dat
     std::vector<int64_t> bad(launches);
     RETURN_NOT_OK(words->ToHost(bad.data(), 8 * (int64_t)launches));
     for (size_t k = 0; k < launches; ++k)
-      if (bad[k] != AG_NO_ERROR_POS) return BoundsError(*idx[k], bad[k]);
+      if (bad[k] != AG_NO_ERROR_POS) return IndexOutOfBounds(*idx[k]->buffers[1], idx[k]->type, idx[k]->offset, bad[k]);
   }
   int64_t out_rows = 0;
   for (auto& a : idx) out_rows += a->length;
@@ -2008,7 +1993,7 @@ Status MaskSpansToIndices(const std::vector<std::shared_ptr<ArrayData>>& masks, 
   for (size_t k = 0; k < ns; ++k) {
     const ArrayData& m = *masks[k];
     if (m.length > (int64_t)UINT32_MAX) return Status::NotImplemented("filter: more than 2^32-1 rows in one chunk");
-    NATIVE(ag_filter_output_size_dev(m.buffers[1]->data(), MayHaveNulls(m) ? m.buffers[0]->data() : nullptr, m.offset, m.length, (int)sel,
+    NATIVE(ag_filter_output_size_dev(m.buffers[1]->data(), ValidityOrNull(m), m.offset, m.length, (int)sel,
                                      d_len + 2 * k, nullptr));
   }
   std::vector<int64_t> h(2 * std::max<size_t>(ns, 1));
@@ -2022,7 +2007,7 @@ Status MaskSpansToIndices(const std::vector<std::shared_ptr<ArrayData>>& masks, 
     RETURN_NOT_OK(Buffer::Allocate(len * 4, &d->buffers[1]));
     if (nullable) RETURN_NOT_OK(Buffer::Allocate(((len + 31) / 32) * 4, &d->buffers[0]));
     if (len > 0)
-      NATIVE(ag_take_indices_dev(32, m.buffers[1]->data(), MayHaveNulls(m) ? m.buffers[0]->data() : nullptr, m.offset, m.length, (int)sel,
+      NATIVE(ag_take_indices_dev(32, m.buffers[1]->data(), ValidityOrNull(m), m.offset, m.length, (int)sel,
                                  d->buffers[1]->data(), nullable ? d->buffers[0]->data() : nullptr, len, d_len + 2 * k + 1, nullptr));
     out->push_back(d);
   }
@@ -2195,8 +2180,8 @@ Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& value
   RETURN_NOT_OK(Buffer::Allocate(bm, &data));
   RETURN_NOT_OK(Buffer::Allocate(bm, &valid));
   RETURN_NOT_OK(Buffer::Allocate(8, &cnt));
-  NATIVE(ag_is_in_dev(bw, a->buffers[1] ? a->buffers[1]->data() : nullptr, (a->buffers[0] && a->null_count != 0) ? a->buffers[0]->data() : nullptr, a->offset, a->length,
-                      s.buffers[1] ? s.buffers[1]->data() : nullptr, (s.buffers[0] && s.null_count != 0) ? s.buffers[0]->data() : nullptr, s.offset, s.length,
+  NATIVE(ag_is_in_dev(bw, a->buffers[1] ? a->buffers[1]->data() : nullptr, ValidityOrNull(*a), a->offset, a->length,
+                      s.buffers[1] ? s.buffers[1]->data() : nullptr, ValidityOrNull(s), s.offset, s.length,
                       (int)opts.NullBehavior, data->data(), valid->data(), (int64_t*)cnt->data(), nullptr));
   int64_t nulls = 0;
   RETURN_NOT_OK(cnt->ToHost(&nulls, 8));

@@ -285,6 +285,8 @@ _SIGS = {
     "ag_sort_indices_keys_dev": [_i, _p, _i64, _p, _p],
     "ag_take_columns": [_i, _p, _i64, _i, _i, _p, _p, _i64, _i64, _i, _pi64, _pi64],
     "ag_take_columns_dev": [_i, _p, _i64, _i, _i, _p, _p, _i64, _i64, _i, _p, _p],
+    "ag_eval_program": [_p, _i64, _p, _p, _p, _pi64],
+    "ag_eval_program_dev": [_p, _i64, _p, _p, _p, _p, _p],
     "ag_parquet_unpack32": [_p, _p, _i64, _i, _pi64],
     "ag_parquet_unpack32_dev": [_p, _p, _i64, _i, _pi64, _p],
     "ag_parquet_bytes_to_bools": [_p, _i64, _p, _i64],

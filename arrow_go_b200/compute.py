@@ -101,6 +101,14 @@ def lib():
         h.agx_filter_record_batch.argtypes = [p, p, i, pp]
         h.agx_filter_table.argtypes = [p, p, i, pp]
         h.agx_sort.argtypes = [p, C.POINTER(i), C.POINTER(i), C.POINTER(i), i, pp]
+        h.agx_expr_field.argtypes = [i, pp]
+        h.agx_expr_literal.argtypes = [p, pp]
+        h.agx_expr_call.argtypes = [C.c_char_p, i, i, pp, i, pp]
+        h.agx_expr_cast.argtypes = [p, i, i, i, pp]
+        h.agx_expr_is_in.argtypes = [p, p, i, pp]
+        h.agx_expr_free.argtypes = [p]
+        h.agx_expr_free.restype = None
+        h.agx_execute_scalar_expression.argtypes = [p, p, pp]
         _lib = h
     return _lib
 
@@ -331,14 +339,20 @@ def Table(columns, num_rows=None):
     return d
 
 
+def _options(options):
+    if options is None:
+        return 0, 0
+    if options[0] == "cast":   # ("cast", (to_type, allow_int_overflow, allow_float_truncate))
+        to, ai, af = options[1]
+        return 6, int(to) | (0x100 if ai else 0) | (0x200 if af else 0)
+    return {"arithmetic": 1, "filter": 2, "take": 3, "dictionary_encode": 4, "run_end_encode": 5}[options[0]], int(options[1])
+
+
 def CallFunction(name, args, options=None):
     """compute.CallFunction(ctx, name, opts, args...) — options: None, ("arithmetic", no_check_overflow),
-    ("filter", null_selection), ("take", bounds_check), ("dictionary_encode", null_encoding) or
-    ("run_end_encode", run_end_type)."""
-    kind, val = 0, 0
-    if options is not None:
-        kind = {"arithmetic": 1, "filter": 2, "take": 3, "dictionary_encode": 4, "run_end_encode": 5}[options[0]]
-        val = int(options[1])
+    ("filter", null_selection), ("take", bounds_check), ("dictionary_encode", null_encoding),
+    ("run_end_encode", run_end_type) or ("cast", (to_type, allow_int_overflow, allow_float_truncate))."""
+    kind, val = _options(options)
     arr = (C.c_void_p * max(len(args), 1))(*[a._h for a in args])
     out = C.c_void_p()
     _check(lib().agx_call_function(name.encode(), kind, val, arr, len(args), C.byref(out)))
@@ -489,6 +503,64 @@ def IsIn(values, value_set, null_behavior=NULL_MATCH):
     """compute.IsIn(ctx, SetOptions{ValueSet, NullBehavior}, values) (arrow/compute/scalar_set_lookup.go)."""
     out = C.c_void_p()
     _check(lib().agx_is_in(values._h, value_set._h, int(null_behavior), C.byref(out)))
+    return Datum(out)
+
+
+class Expression:
+    """A handle on an expression tree (arrow/compute/expression.go); build it with Field, Literal, Call and CastExpr."""
+
+    def __init__(self, handle, keep=()):
+        self._h = handle
+        self._keep = keep
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().agx_expr_free(self._h)
+        except Exception:
+            pass
+
+
+def _expr(fn, *args, keep=()):
+    out = C.c_void_p()
+    _check(fn(*args, C.byref(out)))
+    return Expression(out, keep)
+
+
+def Field(index):
+    """compute.NewFieldRef by column index: column `index` of the record batch or table."""
+    return _expr(lib().agx_expr_field, int(index))
+
+
+def Literal(value, type_id):
+    """compute.NewLiteral: a scalar of `type_id`; value None is a null literal."""
+    s = Scalar(value, type_id)
+    return _expr(lib().agx_expr_literal, s._h, keep=(s,))
+
+
+def Call(name, args, options=None):
+    """compute.NewCall(name, args, options): options as in CallFunction."""
+    kind, val = _options(options)
+    arr = (C.c_void_p * max(len(args), 1))(*[a._h for a in args])
+    return _expr(lib().agx_expr_call, name.encode(), kind, val, arr, len(args), keep=tuple(args))
+
+
+def CastExpr(arg, to_type, allow_int_overflow=False, allow_float_truncate=False):
+    """compute.Cast: a "cast" call with CastOptions{ToType, AllowIntOverflow, AllowFloatTruncate}."""
+    return _expr(lib().agx_expr_cast, arg._h, int(to_type), int(allow_int_overflow), int(allow_float_truncate), keep=(arg,))
+
+
+def IsInExpr(arg, value_set, null_behavior=NULL_MATCH):
+    """An is_in call with SetLookupOptions{ValueSet: value_set (an Array), NullBehavior}."""
+    return _expr(lib().agx_expr_is_in, arg._h, value_set._h, int(null_behavior), keep=(arg, value_set))
+
+
+def ExecuteScalarExpression(expr, batch_or_table):
+    """compute.ExecuteScalarExpression (arrow/compute/exprs/exec.go:440-456): the tree evaluated over a record batch (an
+    array) or a table (a chunked array), as one fused device program; the result and any error are those of calling
+    CallFunction node by node."""
+    out = C.c_void_p()
+    _check(lib().agx_execute_scalar_expression(expr._h, batch_or_table._h, C.byref(out)))
     return Datum(out)
 
 

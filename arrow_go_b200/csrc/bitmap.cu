@@ -12,49 +12,16 @@
 // operand: one thread per ALIGNED 32-bit output word, inputs fetched as two aligned words +
 // funnel shift, edge words merged byte-wise so no byte outside [offset, offset+n) is written.
 #include "common.cuh"
+#include "elem_ops.cuh"
 
 namespace ag {
 
 constexpr int kBmThreads = 256;
 
-enum WordOp {
-  W_AND = 0, W_OR, W_XOR, W_ANDNOT, W_XNOR,   // == AG_BITOP_*
-  W_COPY, W_INVERT, W_SET0, W_SET1,
-  // Kleene: inputs (lvalid, ldata, rvalid, rdata)
-  W_KAND_V, W_KAND_D, W_KOR_V, W_KOR_D, W_KANDNOT_V, W_KANDNOT_D,
-};
-
 struct BitmapArg {
   const uint8_t* p;   // may be NULL => all ones
   int64_t off;        // bit offset of element 0
 };
-
-template <int kOp>
-__device__ __forceinline__ uint32_t word_op(uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  switch (kOp) {
-    case W_AND: return a & b;
-    case W_OR: return a | b;
-    case W_XOR: return a ^ b;
-    case W_ANDNOT: return a & ~b;
-    case W_XNOR: return ~(a ^ b);
-    case W_COPY: return a;
-    case W_INVERT: return ~a;
-    case W_SET0: return 0u;
-    case W_SET1: return 0xffffffffu;
-    default: break;
-  }
-  // Kleene (scalar_boolean.go:42-46): a=lvalid b=ldata c=rvalid d=rdata
-  const uint32_t lt = a & b, lf = a & ~b, rt = c & d, rf = c & ~d;
-  switch (kOp) {
-    case W_KAND_V: return lf | rf | (lt & rt);
-    case W_KAND_D: return lt & rt;
-    case W_KOR_V: return lt | rt | (lf & rf);
-    case W_KOR_D: return lt | rt;
-    case W_KANDNOT_V: return lf | rt | (lt & rf);
-    case W_KANDNOT_D: return lt & rf;
-    default: return 0;
-  }
-}
 
 template <int kOp, int kNIn>
 __global__ void __launch_bounds__(kBmThreads)

@@ -18,6 +18,7 @@
 // type — the only inputs the reference's AVX2 body, SSE4 body and scalar tail agree on, and
 // the only ones a safe cast accepts — this is bit-exact with cast_type_numeric_*.
 #include "common.cuh"
+#include "elem_ops.cuh"
 
 namespace ag {
 
@@ -25,53 +26,6 @@ namespace {
 
 constexpr int kCastThreads = 256;
 constexpr int kCastUnroll = 8;
-
-template <typename T> struct IsFloat { static constexpr bool v = false; };
-template <> struct IsFloat<float> { static constexpr bool v = true; };
-template <> struct IsFloat<double> { static constexpr bool v = true; };
-template <typename T> struct IsSigned { static constexpr bool v = T(-1) < T(0); };
-
-__device__ __forceinline__ long long x86_cvtt(double v) {
-  // CVTTSD2SI r64: NaN and out-of-range give the "integer indefinite" value
-  if (!(v >= -9223372036854775808.0 && v < 9223372036854775808.0)) return (long long)0x8000000000000000ull;
-  return __double2ll_rz(v);
-}
-
-template <typename I, typename O>
-__device__ __forceinline__ O cast_one(I v) {
-  if constexpr (IsFloat<I>::v && !IsFloat<O>::v) {
-    const double d = (double)v;  // float -> double is exact
-    if constexpr (sizeof(O) == 8 && !IsSigned<O>::v) {
-      // Go / clang uint64 conversion: values >= 2^63 go through (x - 2^63) with the top bit set
-      if (d >= 9223372036854775808.0) return (O)((unsigned long long)x86_cvtt(d - 9223372036854775808.0) ^ 0x8000000000000000ull);
-      return (O)(unsigned long long)x86_cvtt(d);
-    } else {
-      return (O)x86_cvtt(d);  // wrap-truncation to the output width
-    }
-  } else if constexpr (!IsFloat<I>::v && IsFloat<O>::v) {
-    if constexpr (sizeof(O) == 4) {
-      if constexpr (IsSigned<I>::v) return __ll2float_rn((long long)v);
-      else return __ull2float_rn((unsigned long long)v);
-    } else {
-      if constexpr (IsSigned<I>::v) return __ll2double_rn((long long)v);
-      else return __ull2double_rn((unsigned long long)v);
-    }
-  } else if constexpr (IsFloat<I>::v && IsFloat<O>::v) {
-    if constexpr (sizeof(I) == 8 && sizeof(O) == 4) return __double2float_rn(v);
-    else return (O)v;
-  } else {
-    return (O)v;  // integer -> integer: sign/zero extension or truncation
-  }
-}
-
-// kCheck: 0 none, 1 integer input in [lo, hi] (intsInRange), 2 float -> int round trip
-// (wasTrunc: OutT -> InT conversion of the result differs from the input; NaN always differs).
-template <typename I, typename O, int kCheck>
-__device__ __forceinline__ bool cast_fails(I in, O out, I lo, I hi) {
-  if constexpr (kCheck == 1) return in < lo || in > hi;
-  else if constexpr (kCheck == 2) return cast_one<O, I>(out) != in;
-  else return false;
-}
 
 template <int kBytes> struct RawVec;
 template <> struct RawVec<1> { using type = uint8_t; };
@@ -205,39 +159,6 @@ ag_status launch_cast(const void* in, void* out, int64_t n, const uint8_t* valid
     cast_scalar_kernel<I, O, kCheck><<<grid, kCastThreads, 0, st>>>((const I*)in, (O*)out, n, valid, voff, lo, hi, (long long*)first_bad, row_base);
   }
   return check_launch("cast_kernel");
-}
-
-template <typename T> struct Lim;
-#define AG_LIM(T, LO, HI) template <> struct Lim<T> { static constexpr T lo = LO; static constexpr T hi = HI; };
-AG_LIM(uint8_t, 0, 0xff) AG_LIM(int8_t, -128, 127) AG_LIM(uint16_t, 0, 0xffff) AG_LIM(int16_t, -32768, 32767)
-AG_LIM(uint32_t, 0, 0xffffffffu) AG_LIM(int32_t, (-2147483647 - 1), 2147483647)
-AG_LIM(unsigned long long, 0, 0xffffffffffffffffull) AG_LIM(long long, (-9223372036854775807ll - 1), 9223372036854775807ll)
-#undef AG_LIM
-
-// Safe bounds of an integer input type I for target O, in I's own domain
-// (getSafeMinMaxSigned / Unsigned, helpers.go:496-543) and for float targets
-// (checkIntToFloatTrunc, numeric_cast.go:698-729).  Returns false when every I fits.
-template <typename I, typename O>
-bool safe_bounds(I* lo, I* hi) {
-  if constexpr (IsFloat<O>::v) {
-    constexpr int mant = sizeof(O) == 4 ? 24 : 53;
-    if (sizeof(I) * 8 <= (size_t)mant) return false;  // int8/16 always; int32/uint32 -> float64
-    const I lim = (I)((unsigned long long)1 << mant);
-    *hi = lim;
-    *lo = IsSigned<I>::v ? (I)(0 - lim) : (I)0;
-    return true;
-  } else {
-    I l = Lim<I>::lo, h = Lim<I>::hi;
-    if constexpr (IsSigned<I>::v) {
-      if constexpr (IsSigned<O>::v) { if (sizeof(I) > sizeof(O)) { l = (I)Lim<O>::lo; h = (I)Lim<O>::hi; } }
-      else { l = 0; if (sizeof(I) > sizeof(O)) h = (I)Lim<O>::hi; }
-    } else {
-      if constexpr (IsSigned<O>::v) { if (sizeof(I) >= sizeof(O)) h = (I)Lim<O>::hi; }
-      else { if (sizeof(I) > sizeof(O)) h = (I)Lim<O>::hi; }
-    }
-    *lo = l; *hi = h;
-    return !(l == Lim<I>::lo && h == Lim<I>::hi);  // intsInRange's early return, helpers.go:581-583
-  }
 }
 
 template <typename I, typename O>

@@ -150,6 +150,10 @@ ag_status take_primitive_dev(int bit_width, const void* vals, const uint8_t* vva
 ag_status take_columns_check(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int64_t idx_offset, int64_t n);
 ag_status take_columns_dev(int ncols, const ag_take_column* cols, int64_t nrows, int idx_width, int idx_signed, const void* idx,
                            const uint8_t* idx_valid, int64_t idx_offset, int64_t n, int bounds_check, int64_t* d_bad_pos, cudaStream_t st);
+// expr.cu: the checks of the program and its spans (no device work), and the checks followed by one launch
+ag_status eval_program_check(const ag_expr_program* prog, int64_t n_spans, const ag_sort_chunk* spans);
+ag_status eval_program_dev(const ag_expr_program* prog, int64_t n_spans, const ag_sort_chunk* spans, void* out, uint8_t* out_valid,
+                           int64_t* d_error_word, cudaStream_t st);
 
 // ---------------------------------------------------------------- cross-GPU exchange (comm.cu, reduce.cu) ----
 struct alignas(32) MailSlot { unsigned long long flag; unsigned long long pad; unsigned long long s; unsigned long long c; };

@@ -17,6 +17,7 @@
 // straddle the ends of the range are merged byte-wise (bitmap_store32_masked), so bytes the
 // reference would not touch are not touched.
 #include "common.cuh"
+#include "elem_ops.cuh"
 
 #include <type_traits>
 
@@ -25,11 +26,6 @@ namespace ag {
 constexpr int kCmpThreads = 256;
 constexpr int kCmpFastBatch = 16;  // interior tiles: loads in flight per lane before the votes
 constexpr int kCmpBatch = 8;   // loads in flight per lane before the votes (16 -> 90 regs, 2 blocks/SM: measured slower)
-
-struct CmpEq { template <typename T> static __device__ __forceinline__ bool apply(T a, T b) { return a == b; } };
-struct CmpNe { template <typename T> static __device__ __forceinline__ bool apply(T a, T b) { return a != b; } };
-struct CmpGt { template <typename T> static __device__ __forceinline__ bool apply(T a, T b) { return a > b; } };
-struct CmpGe { template <typename T> static __device__ __forceinline__ bool apply(T a, T b) { return a >= b; } };
 
 template <typename T, typename Cmp, int kShape>
 __global__ void __launch_bounds__(kCmpThreads)

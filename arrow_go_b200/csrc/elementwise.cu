@@ -17,6 +17,7 @@
 // slices, Appendix D of SURVEY.md) keep the 128-bit accesses: the tile aligns on its output and
 // funnel-shifts the inputs (shift_combine below); same arithmetic, same bits.
 #include "common.cuh"
+#include "elem_ops.cuh"
 
 #include <stdlib.h>
 #include <type_traits>
@@ -27,30 +28,6 @@ namespace ag {
 constexpr int kEwThreads = 256;
 constexpr int kEwUnroll = 4;
 constexpr int kEwBlocksPerSM = 8;
-
-// ---------------------------------------------------------------- functors ---------
-// Integers run on their storage type (visit_storage_type), so int8/uint8 ... int64/uint64 share kernels.
-struct OpAdd { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { return (T)(a + b); } };
-struct OpSub { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { return (T)(a - b); } };
-struct OpMul {
-  template <typename T> static __device__ __forceinline__ T apply(T a, T b) {
-    if constexpr (std::is_floating_point<T>::value) return a * b;
-    else if constexpr (sizeof(T) == 8) return (T)(a * b);
-    else return (T)((uint32_t)a * (uint32_t)b);
-  }
-};
-// explicit round-to-nearest intrinsics: no FMA contraction, no reassociation
-// bitwiseKernelOp (scalar_arithmetic.go:191-243): the reference runs BitmapAnd/Or/Xor over the value buffers, i.e. the
-// plain bitwise op on every slot; integer types only (the float instantiations are never dispatched).
-struct OpBitAnd { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { if constexpr (std::is_integral<T>::value) return (T)(a & b); else return a; } };
-struct OpBitOr { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { if constexpr (std::is_integral<T>::value) return (T)(a | b); else return a; } };
-struct OpBitXor { template <typename T> static __device__ __forceinline__ T apply(T a, T b) { if constexpr (std::is_integral<T>::value) return (T)(a ^ b); else return a; } };
-template <> __device__ __forceinline__ double OpAdd::apply<double>(double a, double b) { return __dadd_rn(a, b); }
-template <> __device__ __forceinline__ float OpAdd::apply<float>(float a, float b) { return __fadd_rn(a, b); }
-template <> __device__ __forceinline__ double OpSub::apply<double>(double a, double b) { return __dsub_rn(a, b); }
-template <> __device__ __forceinline__ float OpSub::apply<float>(float a, float b) { return __fsub_rn(a, b); }
-template <> __device__ __forceinline__ double OpMul::apply<double>(double a, double b) { return __dmul_rn(a, b); }
-template <> __device__ __forceinline__ float OpMul::apply<float>(float a, float b) { return __fmul_rn(a, b); }
 
 template <typename T, int N> struct alignas(16) Vec { T v[N]; };
 
@@ -359,48 +336,6 @@ ag_status arith_binary_spans_dev(int type, int8_t op, int shape, const ag_span3*
 }
 
 // ---------------------------------------------------------------- unary ------------
-// AbsoluteValue base_arithmetic.cc:160-176 (floats: clear the sign bit; signed ints:
-// (x + mask) ^ mask), Negate :194-205, NegateChecked :207-219 (unsigned -> 0), Sign :221-234.
-struct UAbs {
-  template <typename TO, typename T> static __device__ __forceinline__ TO apply(T x) {
-    if constexpr (std::is_same<T, float>::value) return __uint_as_float(__float_as_uint(x) & 0x7fffffffu);
-    else if constexpr (std::is_same<T, double>::value) return __longlong_as_double(__double_as_longlong(x) & 0x7fffffffffffffffll);
-    else if constexpr (std::is_unsigned<T>::value) return x;
-    else {
-      using U = typename std::make_unsigned<T>::type;
-      const U mask = (U)(x >> (sizeof(T) * 8 - 1));
-      return (T)(((U)x + mask) ^ mask);
-    }
-  }
-};
-struct UNeg {
-  template <typename TO, typename T> static __device__ __forceinline__ TO apply(T x) {
-    if constexpr (std::is_same<T, float>::value) return __uint_as_float(__float_as_uint(x) ^ 0x80000000u);
-    else if constexpr (std::is_same<T, double>::value) return __longlong_as_double(__double_as_longlong(x) ^ (long long)0x8000000000000000ull);
-    else { using U = typename std::make_unsigned<T>::type; return (T)((U)0 - (U)x); }
-  }
-};
-struct UNegChecked {  // identical to UNeg except unsigned -> 0 (base_arithmetic.cc:213-214)
-  template <typename TO, typename T> static __device__ __forceinline__ TO apply(T x) {
-    if constexpr (std::is_unsigned<T>::value) return 0;
-    else return UNeg::apply<TO, T>(x);
-  }
-};
-struct UBitNot {  // bitwiseNot, scalar_arithmetic.go:257-259 (integer types; floats are refused before the launch)
-  template <typename TO, typename T> static __device__ __forceinline__ TO apply(T x) {
-    if constexpr (std::is_integral<T>::value) return (TO)(T)~x; else return (TO)x;
-  }
-};
-struct USign {
-  template <typename TO, typename T> static __device__ __forceinline__ TO apply(T x) {
-    // NaN: the reference's shipped AVX2/SSE4 objects lost the isnan() test of base_arithmetic.cc:224
-    // to -funsafe-math-optimizations (kernels/Makefile:23-27): sign(NaN) = +-1 by sign bit.
-    if constexpr (std::is_floating_point<T>::value) return (TO)((x == 0) ? T(0) : (signbit(x) ? T(-1) : T(1)));
-    else if constexpr (std::is_unsigned<T>::value) return (TO)(x > 0 ? 1 : 0);
-    else return (TO)(x > 0 ? 1 : (x ? -1 : 0));
-  }
-};
-
 // Same shape as binary_spans_kernel: tiles of 32 KB that start on the output's first 16-byte boundary; a warp owns 128
 // consecutive vectors of a tile (4 x 16-byte loads in flight per lane); kShift adds the shuffle / funnel-shift read of an
 // input that is not 16-byte aligned where the output is (an Arrow slice).
@@ -521,81 +456,6 @@ ag_status arith_unary_diff_dev(int itype, int otype, int8_t op, const void* in, 
 }
 
 // ---------------------------------------------------------------- checked ----------
-// base_arithmetic.go:249-278: carry = ((a&b) | ((a|b) &^ out)) >> shiftBy, "carry > 0", with
-// shiftBy = bits-1 (unsigned) or bits-2 (signed) evaluated in the operand type (arithmetic
-// shift for signed).  We restate the formula bit for bit, including what it does for signed
-// operands (it flags a carry into the sign bit that is not carried out).
-template <typename ST> struct ChkAdd {
-  static __device__ __forceinline__ ST apply(ST a, ST b, bool& bad) {
-    using U = typename std::make_unsigned<ST>::type;
-    constexpr int shift_by = (int)sizeof(ST) * 8 - 1 - (std::is_signed<ST>::value ? 1 : 0);
-    const ST o = (ST)((U)a + (U)b);
-    const ST c = (ST)((ST)((ST)(a & b) | ((ST)(a | b) & (ST)~o)) >> shift_by);
-    bad = c > 0;
-    return o;
-  }
-};
-template <typename ST> struct ChkSub {
-  static __device__ __forceinline__ ST apply(ST a, ST b, bool& bad) {
-    using U = typename std::make_unsigned<ST>::type;
-    constexpr int shift_by = (int)sizeof(ST) * 8 - 1 - (std::is_signed<ST>::value ? 1 : 0);
-    const ST o = (ST)((U)a - (U)b);
-    const ST c = (ST)((ST)((ST)((ST)~a & b) | ((ST)~(ST)(a ^ b) & o)) >> shift_by);
-    bad = c > 0;
-    return o;
-  }
-};
-// mulWithOverflow base_arithmetic.go:84-108 (division-based test; an overflowing slot yields 0)
-template <typename ST> struct ChkMul {
-  static __device__ __forceinline__ ST apply(ST a, ST b, bool& bad) {
-    using U = typename std::make_unsigned<ST>::type;
-    constexpr ST tmax = std::is_signed<ST>::value ? (ST)(((U)1 << (sizeof(ST) * 8 - 1)) - 1) : (ST)~(U)0;
-    constexpr ST tmin = std::is_signed<ST>::value ? (ST)((U)1 << (sizeof(ST) * 8 - 1)) : (ST)0;
-    bool ovf = false;
-    if (a > 0) { if (b > 0) { ovf = a > (ST)(tmax / b); } else { ovf = b < (ST)(tmin / a); } }
-    else if (b > 0) { ovf = a < (ST)(tmin / b); }
-    else { ovf = (a != 0) && (b < (ST)(tmax / a)); }
-    bad = ovf;
-    return ovf ? (ST)0 : (ST)((U)a * (U)b);
-  }
-};
-// Div / DivChecked base_arithmetic.go:154-161,287-294: b == 0 -> error (value 0); Go's
-// MinInt / -1 wraps to MinInt.
-template <typename ST> struct ChkDiv {
-  static __device__ __forceinline__ ST apply(ST a, ST b, bool& bad) {
-    using U = typename std::make_unsigned<ST>::type;
-    bad = (b == 0);
-    if (b == 0) return 0;
-    if constexpr (std::is_signed<ST>::value) {
-      constexpr ST tmin = (ST)((U)1 << (sizeof(ST) * 8 - 1));
-      if (a == tmin && b == (ST)-1) return a;
-    }
-    return (ST)(a / b);
-  }
-};
-
-// shiftKernelSignedImpl / UnsignedImpl (scalar_arithmetic.go:293-379): an amount outside [0, maxShift) leaves lhs as it
-// is and, in the checked flavour, fails the call; maxShift = bits - 1 for SIGNED types, bits for unsigned.
-template <typename ST, bool kLeft, bool kChecked> struct ChkShift {
-  static __device__ __forceinline__ ST apply(ST a, ST b, bool& bad) {
-    using U = typename std::make_unsigned<ST>::type;
-    constexpr int max_shift = (int)sizeof(ST) * 8 - (std::is_signed<ST>::value ? 1 : 0);
-    const bool invalid = (std::is_signed<ST>::value && b < 0) || (unsigned long long)b >= (unsigned long long)max_shift;
-    bad = kChecked && invalid;
-    if (invalid) return a;
-    if (kLeft) return (ST)((U)a << (int)b);
-    return (ST)(a >> (int)b);
-  }
-};
-// floating point Div / DivChecked (base_arithmetic.go:386-397): IEEE quotient; the checked op fails on a zero divisor
-template <typename FT, bool kChecked> struct ChkFDiv {
-  static __device__ __forceinline__ FT apply(FT a, FT b, bool& bad) {
-    bad = kChecked && b == FT(0);
-    if (bad) return FT(0);
-    if constexpr (sizeof(FT) == 8) return __ddiv_rn(a, b); else return __fdiv_rn(a, b);
-  }
-};
-
 // kNotNull: ScalarBinaryNotNull slot semantics (null slots written as 0, not computed);
 // otherwise ScalarBinary (every slot computed — MUL_CHECKED, base_arithmetic.go:279-286).
 template <typename ST, typename Op, int kShape, bool kNotNull, bool kHasValid>

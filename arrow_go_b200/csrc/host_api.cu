@@ -815,6 +815,47 @@ ag_status ag_take_columns(int ncols, const ag_take_column* cols, int64_t nrows, 
   return sync(cs);
 }
 
+// The program's spans staged chunk by chunk (upload_chunk); the output is fetched only when no row failed.
+ag_status ag_eval_program(const ag_expr_program* prog, int64_t n_spans, const ag_sort_chunk* spans, void* out, uint8_t* out_valid,
+                          int64_t* first_bad) {
+  AG_TRY(ensure_init());
+  if (first_bad) *first_bad = AG_NO_ERROR_POS;
+  AG_TRY(eval_program_check(prog, n_spans, spans));
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  const int nc = prog->n_cols;
+  std::vector<ag_sort_chunk> dspans((size_t)(n_spans * nc));
+  int64_t rows = 0;
+  for (int64_t i = 0; i < n_spans && nc > 0; ++i) {
+    rows += spans[i * nc].length > 0 ? spans[i * nc].length : 0;
+    for (int j = 0; j < nc; ++j) {
+      AG_TRY(upload_chunk(t, prog->col_types[j], spans[i * nc + j], &dspans[i * nc + j]));
+    }
+  }
+  const size_t words = (size_t)((rows + 31) / 32) * 4;
+  void* dout = nullptr;
+  uint8_t* dvalid = nullptr;
+  int64_t* d_word;
+  AG_TRY(t.alloc(&dout, (size_t)rows * 8));   // room for any output type
+  if (out_valid) AG_TRY(t.alloc_t(&dvalid, words));
+  AG_TRY(t.alloc_t(&d_word, sizeof(int64_t)));
+  AG_TRY(error_word_reset(d_word, cs));
+  AG_TRY(eval_program_dev(prog, n_spans, dspans.data(), dout, dvalid, d_word, cs));
+  if (rows == 0) return sync(cs);
+  int64_t bad = AG_NO_ERROR_POS;
+  AG_TRY(d2h(&bad, d_word, sizeof(int64_t), cs));
+  AG_TRY(sync(cs));
+  if (bad != AG_NO_ERROR_POS) {
+    if (first_bad) *first_bad = bad;
+    AG_FAIL(AG_ERR_INVALID, "expression failed at row %lld", (long long)bad);
+  }
+  int out_type = AG_TYPE_NULL;   // a checked program's result type: out_type of the last instruction that wrote out_reg
+  for (int i = 0; i < prog->n_instr; ++i) if (prog->instr[i].dst == prog->out_reg) out_type = prog->instr[i].out_type;
+  AG_TRY(d2h(out, dout, out_type == AG_TYPE_BOOL ? (size_t)((rows + 7) / 8) : (size_t)rows * type_width(out_type), cs));
+  if (out_valid) AG_TRY(d2h(out_valid, dvalid, (size_t)((rows + 7) / 8), cs));
+  return sync(cs);
+}
+
 ag_status ag_is_in(int bit_width, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, const void* set_vals,
                    const uint8_t* set_valid, int64_t set_offset, int64_t set_n, int null_behavior, uint8_t* out_data, uint8_t* out_valid,
                    int64_t* out_nulls) {

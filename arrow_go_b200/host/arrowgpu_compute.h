@@ -222,6 +222,9 @@ struct ScalarKernel : Kernel {  // kernel.go:632-640
   BatchKernelExec exec_batch;
   bool can_fail = false;        // kernels that lower KernelCtx::error_word
   const char* fail_message = "";
+  // GPU-first extension: the op of the fused expression program (AG_EXPR_*, include/arrowgpu.h) that computes what
+  // `exec` computes in every slot, decided where the kernel is registered; -1 = none.
+  int expr_op = -1;
 };
 struct VectorKernel : Kernel {  // kernel.go:693-704
   bool can_execute_chunkwise = true;
@@ -417,6 +420,29 @@ Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& value
 // cross a chunk boundary
 Status RunEndEncode(const ExecCtx& ctx, const RunEndEncodeOptions& opts, const Datum& values, Datum* out);
 Status RunEndDecode(const ExecCtx& ctx, const Datum& values, Datum* out);
+
+// ---- scalar expressions (arrow/compute/expression.go:528,596-620; exprs/exec.go:542-700) ----
+// A field reference names a column of the record batch or table by index; a literal is a Scalar (may be null); a call
+// is a registered function name, its arguments and its options (ArithmeticOptions, or CastOptions for "cast" and the
+// cast_<type> functions).
+struct Expression {
+  enum class Kind { FIELD, LITERAL, CALL };
+  Kind kind = Kind::LITERAL;
+  int field = -1;
+  std::shared_ptr<Scalar> literal;
+  std::string name;
+  std::shared_ptr<FunctionOptions> options;
+  std::vector<std::shared_ptr<Expression>> args;
+};
+std::shared_ptr<Expression> FieldRef(int index);
+std::shared_ptr<Expression> Literal(std::shared_ptr<Scalar> value);
+std::shared_ptr<Expression> Call(std::string name, std::vector<std::shared_ptr<Expression>> args, std::shared_ptr<FunctionOptions> options = nullptr);
+std::shared_ptr<Expression> Cast(std::shared_ptr<Expression> arg, const CastOptions& opts);   // Call("cast", {arg}, opts)
+// The result of evaluating `expr` node by node with CallFunction in post-order, arguments left to right (an array
+// for a record batch, a chunked array for a table), error and message included.  The calls run as one fused device
+// program (ag_eval_program_dev); is_in is evaluated by CallFunction first and enters the program as a column.  When
+// the program reports a failure, the tree is evaluated node by node and that status is returned.
+Status ExecuteScalarExpression(const ExecCtx& ctx, const Expression& expr, const Datum& input, Datum* out);
 
 // ---- executor internals exposed for tests (exec_internals_test.go exercises the same pieces) ----
 struct SpanPiece { int64_t pos; int64_t len; std::vector<int> chunk_index; std::vector<int64_t> chunk_pos; };

@@ -125,17 +125,24 @@ int agx_array_to_host(agx_datum* d, void* values, uint8_t* validity, int64_t* nu
 
 // opt_kind: 0 none, 1 ArithmeticOptions{NoCheckOverflow=opt_value}, 2 FilterOptions{NullSelection=opt_value},
 //           3 TakeOptions{BoundsCheck=opt_value}, 4 DictionaryEncodeOptions{NullEncoding=opt_value},
-//           5 RunEndEncodeOptions{RunEndType=opt_value}
+//           5 RunEndEncodeOptions{RunEndType=opt_value},
+//           6 CastOptions{ToType = opt_value & 0xff, AllowIntOverflow = opt_value & 0x100, AllowFloatTruncate = opt_value & 0x200}
+static CastOptions CastOptionsOf(int v) {
+  CastOptions o; o.ToType = (Type)(v & 0xff); o.AllowIntOverflow = (v & 0x100) != 0; o.AllowFloatTruncate = (v & 0x200) != 0;
+  return o;
+}
 int agx_call_function(const char* name, int opt_kind, int opt_value, agx_datum** args, int nargs, agx_datum** out) {
   std::vector<Datum> a;
   for (int i = 0; i < nargs; ++i) a.push_back(args[i]->d);
   ArithmeticOptions ao; FilterOptions fo; TakeOptions to; DictionaryEncodeOptions deo; RunEndEncodeOptions reo;
+  CastOptions co = CastOptionsOf(opt_value);
   const FunctionOptions* opts = nullptr;
   if (opt_kind == 1) { ao.NoCheckOverflow = opt_value != 0; opts = &ao; }
   if (opt_kind == 2) { fo.NullSelection = (NullSelectionBehavior)opt_value; opts = &fo; }
   if (opt_kind == 3) { to.BoundsCheck = opt_value != 0; opts = &to; }
   if (opt_kind == 4) { deo.NullEncoding = (NullEncodingBehavior)opt_value; opts = &deo; }
   if (opt_kind == 5) { reo.RunEndType = (Type)opt_value; opts = &reo; }
+  if (opt_kind == 6) opts = &co;
   ExecCtx ctx;
   Datum r;
   AGX_TRY(CallFunction(ctx, name, opts, a, &r));
@@ -408,6 +415,49 @@ int agx_ipc_import_stream(struct ArrowDeviceArrayStream* stream, int* nfields, i
     rows[b] = batches[b].num_rows;
     for (size_t c = 0; c < schema.size(); ++c) cols[b * schema.size() + c] = new agx_datum{Datum(batches[b].columns[c])};
   }
+  return AG_OK;
+}
+
+// Expression trees (compute/expression.go: NewFieldRef, NewLiteral, NewCall, Cast) and ExecuteScalarExpression.
+// agx_expr_call takes the option encoding of agx_call_function; a handle stays valid after it is used as an argument.
+typedef struct agx_expr { std::shared_ptr<Expression> e; } agx_expr;
+int agx_expr_field(int index, agx_expr** out) { *out = new agx_expr{FieldRef(index)}; return AG_OK; }
+int agx_expr_literal(agx_datum* scalar, agx_expr** out) {
+  if (scalar->d.kind != DatumKind::SCALAR) return fail(Status::Invalid("expression literal: not a scalar"));
+  *out = new agx_expr{Literal(scalar->d.scalar)};
+  return AG_OK;
+}
+int agx_expr_call(const char* name, int opt_kind, int opt_value, agx_expr** args, int nargs, agx_expr** out) {
+  std::vector<std::shared_ptr<Expression>> a;
+  for (int i = 0; i < nargs; ++i) a.push_back(args[i]->e);
+  std::shared_ptr<FunctionOptions> opts;
+  if (opt_kind == 1) { auto o = std::make_shared<ArithmeticOptions>(); o->NoCheckOverflow = opt_value != 0; opts = o; }
+  if (opt_kind == 2) { auto o = std::make_shared<FilterOptions>(); o->NullSelection = (NullSelectionBehavior)opt_value; opts = o; }
+  if (opt_kind == 3) { auto o = std::make_shared<TakeOptions>(); o->BoundsCheck = opt_value != 0; opts = o; }
+  if (opt_kind == 4) { auto o = std::make_shared<DictionaryEncodeOptions>(); o->NullEncoding = (NullEncodingBehavior)opt_value; opts = o; }
+  if (opt_kind == 5) { auto o = std::make_shared<RunEndEncodeOptions>(); o->RunEndType = (Type)opt_value; opts = o; }
+  if (opt_kind == 6) opts = std::make_shared<CastOptions>(CastOptionsOf(opt_value));
+  *out = new agx_expr{Call(name, std::move(a), std::move(opts))};
+  return AG_OK;
+}
+int agx_expr_cast(agx_expr* arg, int to_type, int allow_int_overflow, int allow_float_truncate, agx_expr** out) {
+  CastOptions o; o.ToType = (Type)to_type; o.AllowIntOverflow = allow_int_overflow != 0; o.AllowFloatTruncate = allow_float_truncate != 0;
+  *out = new agx_expr{Cast(arg->e, o)};
+  return AG_OK;
+}
+// is_in(arg) with SetLookupOptions{ValueSet, NullBehavior}: CallFunction evaluates it, its result enters the program
+int agx_expr_is_in(agx_expr* arg, agx_datum* value_set, int null_behavior, agx_expr** out) {
+  if (value_set->d.kind != DatumKind::ARRAY) return fail(Status::Invalid("is_in: the value set must be an array"));
+  auto o = std::make_shared<SetLookupOptions>();
+  o->ValueSet = value_set->d.array; o->NullBehavior = (NullMatchingBehavior)null_behavior;
+  *out = new agx_expr{Call("is_in", {arg->e}, o)};
+  return AG_OK;
+}
+void agx_expr_free(agx_expr* e) { delete e; }
+int agx_execute_scalar_expression(agx_expr* expr, agx_datum* input, agx_datum** out) {
+  ExecCtx ctx; Datum r;
+  AGX_TRY(ExecuteScalarExpression(ctx, *expr->e, input->d, &r));
+  *out = new agx_datum{r};
   return AG_OK;
 }
 

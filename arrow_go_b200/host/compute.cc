@@ -5,6 +5,7 @@
 #include <string.h>
 #include <algorithm>
 #include <mutex>
+#include <tuple>
 
 namespace arrowgpu {
 
@@ -1171,6 +1172,7 @@ std::shared_ptr<ScalarFunction> MakeCastTo(Type to) {  // GetCastToInteger / Get
     k.in_types = {t};
     k.out_type = [to](const std::vector<Type>&) { return to; };
     k.exec = CastNumericExec;
+    k.expr_op = AG_EXPR_CAST;
     k.can_fail = true;  // the executor supplies the error word; CastNumericExec words the error itself
     k.fail_message = "cast failed";
     fn->AddKernel(std::move(k));
@@ -1368,6 +1370,42 @@ Status PrimitiveTakeExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out)
   return Status::OK();
 }
 
+// The expression-program op of a kernel, read from the device op its exec launches: the plain loops of
+// ag_arith_binary_dev / ag_arith_unary_same_dev (launch_binary, launch_unary_same_op: a *_CHECKED op there is the plain
+// loop) and the checked kernels of ag_arith_checked_dev / ag_arith_unary_checked_dev (launch_checked_op).
+int PlainExprOp(int8_t op) {
+  switch (op) {
+    case AG_OP_ADD: case AG_OP_ADD_CHECKED: return AG_EXPR_ADD;
+    case AG_OP_SUB: case AG_OP_SUB_CHECKED: return AG_EXPR_SUB;
+    case AG_OP_MUL: case AG_OP_MUL_CHECKED: return AG_EXPR_MUL;
+    case AG_OP_BIT_AND: return AG_EXPR_BIT_AND;
+    case AG_OP_BIT_OR: return AG_EXPR_BIT_OR;
+    case AG_OP_BIT_XOR: return AG_EXPR_BIT_XOR;
+    case AG_OP_ABS: case AG_OP_ABS_CHECKED: return AG_EXPR_ABS;
+    case AG_OP_NEGATE: return AG_EXPR_NEG;
+    case AG_OP_NEGATE_CHECKED: return AG_EXPR_NEG_UNSIGNED_ZERO;
+    case AG_OP_SIGN: return AG_EXPR_SIGN;
+    case AG_OP_BIT_NOT: return AG_EXPR_BIT_NOT;
+    default: return -1;
+  }
+}
+int CheckedExprOp(int8_t op) {
+  switch (op) {
+    case AG_OP_ADD_CHECKED: return AG_EXPR_ADD_CHECKED;
+    case AG_OP_SUB_CHECKED: return AG_EXPR_SUB_CHECKED;
+    case AG_OP_MUL_CHECKED: return AG_EXPR_MUL_CHECKED;
+    case AG_OP_DIV: return AG_EXPR_DIV;
+    case AG_OP_DIV_CHECKED: return AG_EXPR_DIV_CHECKED;
+    case AG_OP_SHIFT_LEFT: return AG_EXPR_SHL;
+    case AG_OP_SHIFT_RIGHT: return AG_EXPR_SHR;
+    case AG_OP_SHIFT_LEFT_CHECKED: return AG_EXPR_SHL_CHECKED;
+    case AG_OP_SHIFT_RIGHT_CHECKED: return AG_EXPR_SHR_CHECKED;
+    case AG_OP_ABS_CHECKED: return AG_EXPR_ABS_CHECKED;
+    case AG_OP_NEGATE_CHECKED: return AG_EXPR_NEG_CHECKED;
+    default: return -1;
+  }
+}
+
 Type FirstType(const std::vector<Type>& t) { return t[0]; }
 Type BoolType(const std::vector<Type>&) { return Type::BOOL; }
 
@@ -1383,10 +1421,12 @@ std::shared_ptr<ScalarFunction> MakeArithBinary(const std::string& name, int8_t 
     k.out_type = FirstType;
     if (checked && IsInteger(t)) {  // integral checked funcs use the NotNull versions (base_arithmetic_amd64.go:103-106)
       k.exec = ArithCheckedExec(checked_op);
+      k.expr_op = CheckedExprOp(checked_op);
       k.can_fail = true;
       k.fail_message = fail_msg;
     } else {
       k.exec = ArithBinaryExec(checked ? checked_op : unchecked_op);
+      k.expr_op = PlainExprOp(checked ? checked_op : unchecked_op);
       k.exec_batch = ArithBinaryBatchExec(checked ? checked_op : unchecked_op);
     }
     fn->AddKernel(std::move(k));
@@ -1404,6 +1444,7 @@ std::shared_ptr<ScalarFunction> MakeDivide(const std::string& name, bool checked
     k.in_types = {t, t};
     k.out_type = FirstType;
     k.exec = ArithCheckedExec(checked ? AG_OP_DIV_CHECKED : AG_OP_DIV);
+    k.expr_op = CheckedExprOp(checked ? AG_OP_DIV_CHECKED : AG_OP_DIV);
     k.can_fail = true;   // the NotNull entry point always takes an error word; the unchecked float op never raises it
     k.fail_message = "divide by zero";
     fn->AddKernel(std::move(k));
@@ -1424,6 +1465,7 @@ std::shared_ptr<ScalarFunction> MakeBitwiseBinary(const std::string& name, int8_
     k.out_type = FirstType;
     k.exec = ArithBinaryExec(op);
     k.exec_batch = ArithBinaryBatchExec(op);
+    k.expr_op = PlainExprOp(op);
     fn->AddKernel(std::move(k));
   }
   return fn;
@@ -1438,6 +1480,7 @@ std::shared_ptr<ScalarFunction> MakeShift(const std::string& name, int8_t op, bo
     k.in_types = {t, t};
     k.out_type = FirstType;
     k.exec = ArithCheckedExec(op);
+    k.expr_op = CheckedExprOp(op);
     k.can_fail = true;   // error word always supplied; only the checked ops raise it
     k.fail_message = "shift amount must be >= 0 and less than precision of type";
     fn->AddKernel(std::move(k));
@@ -1452,6 +1495,7 @@ std::shared_ptr<ScalarFunction> MakeArithUnary(const std::string& name, int8_t o
     k.in_types = {t};
     k.out_type = FirstType;
     k.exec = ArithUnaryExec(op);
+    k.expr_op = PlainExprOp(op);
     fn->AddKernel(std::move(k));
   }
   return fn;
@@ -1464,8 +1508,8 @@ std::shared_ptr<ScalarFunction> MakeArithUnaryChecked(const std::string& name, i
     exec::ScalarKernel k;
     k.in_types = {t};
     k.out_type = FirstType;
-    if (IsSignedInteger(t)) { k.exec = ArithUnaryCheckedExec(op); k.can_fail = true; k.fail_message = "overflow"; }
-    else k.exec = ArithUnaryExec(op);
+    if (IsSignedInteger(t)) { k.exec = ArithUnaryCheckedExec(op); k.expr_op = CheckedExprOp(op); k.can_fail = true; k.fail_message = "overflow"; }
+    else { k.exec = ArithUnaryExec(op); k.expr_op = PlainExprOp(op); }
     fn->AddKernel(std::move(k));
   }
   return fn;
@@ -1479,17 +1523,19 @@ std::shared_ptr<ScalarFunction> MakeCompare(const std::string& name, int cmp) { 
     k.in_types = {t, t};
     k.out_type = BoolType;
     k.exec = CompareExec(cmp);
+    k.expr_op = AG_EXPR_EQ + cmp;   // AG_CMP_EQ .. AG_CMP_LE in the order of AG_EXPR_EQ .. AG_EXPR_LE
     fn->AddKernel(std::move(k));
   }
   return fn;
 }
 
-std::shared_ptr<ScalarFunction> MakeBool(const std::string& name, exec::ArrayKernelExec ex, exec::NullHandling nh) {  // scalar_bool.go:123-140
+std::shared_ptr<ScalarFunction> MakeBool(const std::string& name, exec::ArrayKernelExec ex, exec::NullHandling nh, int expr_op) {  // scalar_bool.go:123-140
   auto fn = std::make_shared<ScalarFunction>(name, 2);
   exec::ScalarKernel k;
   k.in_types = {Type::BOOL, Type::BOOL};
   k.out_type = BoolType;
   k.exec = std::move(ex);
+  k.expr_op = expr_op;
   k.null_handling = nh;
   fn->AddKernel(std::move(k));
   return fn;
@@ -1532,6 +1578,7 @@ FunctionRegistry* GetFunctionRegistry() {
         k.in_types = {t};
         k.out_type = FirstType;
         k.exec = ArithUnaryExec(AG_OP_BIT_NOT);
+        k.expr_op = PlainExprOp(AG_OP_BIT_NOT);
         fn->AddKernel(std::move(k));
       }
       reg->AddFunction(fn, false);
@@ -1548,19 +1595,20 @@ FunctionRegistry* GetFunctionRegistry() {
     reg->AddFunction(MakeCompare("less", AG_CMP_LT), false);
     reg->AddFunction(MakeCompare("less_equal", AG_CMP_LE), false);
     // scalar_bool.go:123-140
-    reg->AddFunction(MakeBool("and", BoolBinaryExec(AG_BITOP_AND), exec::NullHandling::INTERSECTION), false);
-    reg->AddFunction(MakeBool("or", BoolBinaryExec(AG_BITOP_OR), exec::NullHandling::INTERSECTION), false);
-    reg->AddFunction(MakeBool("xor", BoolBinaryExec(AG_BITOP_XOR), exec::NullHandling::INTERSECTION), false);
-    reg->AddFunction(MakeBool("and_not", BoolBinaryExec(AG_BITOP_ANDNOT), exec::NullHandling::INTERSECTION), false);
-    reg->AddFunction(MakeBool("and_kleene", KleeneExec(AG_KLEENE_AND, AG_BITOP_AND), exec::NullHandling::COMPUTED_PREALLOC), false);
-    reg->AddFunction(MakeBool("or_kleene", KleeneExec(AG_KLEENE_OR, AG_BITOP_OR), exec::NullHandling::COMPUTED_PREALLOC), false);
-    reg->AddFunction(MakeBool("and_not_kleene", KleeneExec(AG_KLEENE_ANDNOT, AG_BITOP_ANDNOT), exec::NullHandling::COMPUTED_PREALLOC), false);
+    reg->AddFunction(MakeBool("and", BoolBinaryExec(AG_BITOP_AND), exec::NullHandling::INTERSECTION, AG_EXPR_AND), false);
+    reg->AddFunction(MakeBool("or", BoolBinaryExec(AG_BITOP_OR), exec::NullHandling::INTERSECTION, AG_EXPR_OR), false);
+    reg->AddFunction(MakeBool("xor", BoolBinaryExec(AG_BITOP_XOR), exec::NullHandling::INTERSECTION, AG_EXPR_XOR), false);
+    reg->AddFunction(MakeBool("and_not", BoolBinaryExec(AG_BITOP_ANDNOT), exec::NullHandling::INTERSECTION, AG_EXPR_AND_NOT), false);
+    reg->AddFunction(MakeBool("and_kleene", KleeneExec(AG_KLEENE_AND, AG_BITOP_AND), exec::NullHandling::COMPUTED_PREALLOC, AG_EXPR_KLEENE_AND), false);
+    reg->AddFunction(MakeBool("or_kleene", KleeneExec(AG_KLEENE_OR, AG_BITOP_OR), exec::NullHandling::COMPUTED_PREALLOC, AG_EXPR_KLEENE_OR), false);
+    reg->AddFunction(MakeBool("and_not_kleene", KleeneExec(AG_KLEENE_ANDNOT, AG_BITOP_ANDNOT), exec::NullHandling::COMPUTED_PREALLOC, AG_EXPR_KLEENE_AND_NOT), false);
     {
       auto fn = std::make_shared<ScalarFunction>("not", 1);
       exec::ScalarKernel k;
       k.in_types = {Type::BOOL};
       k.out_type = BoolType;
       k.exec = NotExec;
+      k.expr_op = AG_EXPR_NOT;
       k.null_handling = exec::NullHandling::COMPUTED_NO_PREALLOC;
       k.can_write_into_slices = false;
       fn->AddKernel(std::move(k));
@@ -1568,11 +1616,13 @@ FunctionRegistry* GetFunctionRegistry() {
     }
     // scalar_compare.go / scalar_comparisons.go:718-813: is_null, is_not_null, is_nan
     for (auto& spec : std::vector<std::pair<const char*, exec::ArrayKernelExec>>{{"is_null", IsNullExec}, {"is_not_null", IsNotNullExec}}) {
+      const int expr_op = spec.first == std::string("is_null") ? AG_EXPR_IS_NULL : AG_EXPR_IS_NOT_NULL;
       auto fn = std::make_shared<ScalarFunction>(spec.first, 1);
       exec::ScalarKernel k;
       k.any_input_type = true;
       k.out_type = BoolType;
       k.exec = spec.second;
+      k.expr_op = expr_op;
       k.null_handling = exec::NullHandling::COMPUTED_NO_PREALLOC;
       k.mem_alloc = exec::MemAlloc::NO_PREALLOC;
       k.can_write_into_slices = false;
@@ -1586,6 +1636,7 @@ FunctionRegistry* GetFunctionRegistry() {
         k.in_types = {t};
         k.out_type = BoolType;
         k.exec = IsNanExec;
+        k.expr_op = AG_EXPR_IS_NAN;
         k.null_handling = exec::NullHandling::OUTPUT_NOT_NULL;
         fn->AddKernel(std::move(k));
       }
@@ -2319,6 +2370,338 @@ Status Filter(const ExecCtx& ctx, const Datum& values, const Datum& filter, cons
 }
 Status Take(const ExecCtx& ctx, const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out) {
   return CallFunction(ctx, "take", &opts, {values, indices}, out);
+}
+
+// ---------------------------------------------------------------- scalar expressions ------
+std::shared_ptr<Expression> FieldRef(int index) {
+  auto e = std::make_shared<Expression>();
+  e->kind = Expression::Kind::FIELD; e->field = index;
+  return e;
+}
+std::shared_ptr<Expression> Literal(std::shared_ptr<Scalar> value) {
+  auto e = std::make_shared<Expression>();
+  e->kind = Expression::Kind::LITERAL; e->literal = std::move(value);
+  return e;
+}
+std::shared_ptr<Expression> Call(std::string name, std::vector<std::shared_ptr<Expression>> args, std::shared_ptr<FunctionOptions> options) {
+  auto e = std::make_shared<Expression>();
+  e->kind = Expression::Kind::CALL; e->name = std::move(name); e->args = std::move(args); e->options = std::move(options);
+  return e;
+}
+std::shared_ptr<Expression> Cast(std::shared_ptr<Expression> arg, const CastOptions& opts) {
+  return Call("cast", {std::move(arg)}, std::make_shared<CastOptions>(opts));
+}
+
+namespace {
+
+// executeScalarBatch (exprs/exec.go:542-700) over CallFunction: arguments left to right, then the call.  is_in and
+// cast are meta functions here but scalar functions in the reference, so they are called like one.
+Status EvalNodeByNode(const ExecCtx& ctx, const Expression& e, const Datum& input, Datum* out) {
+  switch (e.kind) {
+    case Expression::Kind::LITERAL:
+      if (!e.literal) return Status::Invalid("literal expression without a value");
+      *out = Datum(e.literal);
+      return Status::OK();
+    case Expression::Kind::FIELD: {
+      const int n = input.kind == DatumKind::RECORD ? (int)input.record->columns.size() : (int)input.table->columns.size();
+      if (e.field < 0 || e.field >= n)
+        return Status::Invalid("field index " + std::to_string(e.field) + " out of range: the input has " + std::to_string(n) + " columns");
+      *out = input.kind == DatumKind::RECORD ? Datum(input.record->columns[e.field]) : Datum(input.table->columns[e.field]);
+      return Status::OK();
+    }
+    case Expression::Kind::CALL: {
+      std::vector<Datum> args(e.args.size());
+      for (size_t i = 0; i < e.args.size(); ++i) {
+        if (!e.args[i]) return Status::Invalid("call '" + e.name + "': argument " + std::to_string(i) + " is not an expression");
+        RETURN_NOT_OK(EvalNodeByNode(ctx, *e.args[i], input, &args[i]));
+      }
+      FunctionRegistry* reg = ctx.Registry ? ctx.Registry : GetFunctionRegistry();
+      const Function* fn = reg->GetFunction(e.name);
+      if (fn && fn->Kind() != FuncKind::SCALAR && e.name != "cast" && e.name != "is_in")   // exec.go:625-627
+        return Status::Invalid("function '" + e.name + "' is not a scalar function");
+      return CallFunction(ctx, e.name, e.options.get(), args, out);
+    }
+  }
+  return Status::NotImplemented("unknown expression kind");
+}
+
+// An input column of a fused program: its chunks (one for a record batch column or an intermediate result).
+struct ExprColumn { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
+
+// A bound node: a column of `cols`, a literal, or a program op over bound arguments.
+struct BNode {
+  enum Kind { COL, LIT, OP } kind = LIT;
+  int col = -1;
+  std::shared_ptr<Scalar> lit;
+  int op = -1, flags = 0;
+  Type type = Type::NA, out = Type::NA;   // operand type, result type
+  std::vector<std::shared_ptr<BNode>> args;
+};
+using BPtr = std::shared_ptr<BNode>;
+
+bool ValueType(Type t) { return t == Type::BOOL || IsNumeric(t); }
+bool IsNullLiteral(const BPtr& n) { return n->kind == BNode::LIT && !n->lit->valid; }
+
+struct Binder {
+  const ExecCtx& ctx;
+  const Datum& input;
+  std::vector<ExprColumn>* cols;
+  std::map<int, int> field_col;   // field index -> its column in `cols`: a field named twice is read once
+
+  BPtr Leaf(int c) { auto n = std::make_shared<BNode>(); n->kind = BNode::COL; n->col = c; n->out = (*cols)[c].type; return n; }
+  BPtr Lit(std::shared_ptr<Scalar> s) { auto n = std::make_shared<BNode>(); n->kind = BNode::LIT; n->out = s->type; n->lit = std::move(s); return n; }
+  BPtr Op(int op, Type type, Type out, std::vector<BPtr> args, int flags = 0) {
+    auto n = std::make_shared<BNode>();
+    n->kind = BNode::OP; n->op = op; n->type = type; n->out = out; n->args = std::move(args); n->flags = flags;
+    return n;
+  }
+  static int CastFlags(const CastOptions& o) {
+    return (o.AllowIntOverflow ? AG_EXPR_ALLOW_INT_OVERFLOW : 0) | (o.AllowFloatTruncate ? AG_EXPR_ALLOW_FLOAT_TRUNCATE : 0);
+  }
+  // `arg` as type `to` under `o`: a literal is cast now through the cast meta function's scalar route (the node-by-node
+  // path casts it the same way), a column in the program.
+  bool CastTo(BPtr arg, Type to, const CastOptions& o, BPtr* out) {
+    if (arg->out == to) { *out = arg; return true; }
+    if (!IsNumeric(arg->out) || !IsNumeric(to)) return false;
+    if (arg->kind == BNode::LIT) {
+      Datum r;
+      if (!CastDatum(ctx, Datum(arg->lit), o, &r).ok()) return false;
+      *out = Lit(r.scalar);
+      return true;
+    }
+    *out = Op(AG_EXPR_CAST, arg->out, to, {arg}, CastFlags(o));
+    return true;
+  }
+
+  // false: the tree is not fused (it fails, or holds something the program does not run); node by node decides.
+  bool Bind(const Expression& e, BPtr* out) {
+    if (e.kind == Expression::Kind::LITERAL) {
+      if (!e.literal || !ValueType(e.literal->type)) return false;
+      *out = Lit(e.literal);
+      return true;
+    }
+    if (e.kind == Expression::Kind::FIELD) {
+      const int n = input.kind == DatumKind::RECORD ? (int)input.record->columns.size() : (int)input.table->columns.size();
+      if (e.field < 0 || e.field >= n) return false;
+      const auto seen = field_col.find(e.field);
+      if (seen != field_col.end()) { *out = Leaf(seen->second); return true; }
+      ExprColumn c;
+      if (input.kind == DatumKind::RECORD) { c.type = input.record->columns[e.field]->type; c.chunks = {input.record->columns[e.field]}; }
+      else { c.type = input.table->columns[e.field]->type; c.chunks = input.table->columns[e.field]->chunks; }
+      if (!ValueType(c.type)) return false;
+      cols->push_back(std::move(c));
+      field_col[e.field] = (int)cols->size() - 1;
+      *out = Leaf((int)cols->size() - 1);
+      return true;
+    }
+    std::vector<BPtr> args(e.args.size());
+    bool all_literal = true;
+    if (e.name == "is_in") {   // a meta function here: CallFunction runs it and its result is a column of the program
+      Datum r;
+      if (!EvalNodeByNode(ctx, e, input, &r).ok()) return false;
+      ExprColumn c;
+      c.type = r.type();
+      if (r.kind == DatumKind::ARRAY) c.chunks = {r.array};
+      else if (r.kind == DatumKind::CHUNKED) c.chunks = r.chunked->chunks;
+      else return false;
+      cols->push_back(std::move(c));
+      *out = Leaf((int)cols->size() - 1);
+      return true;
+    }
+    for (size_t i = 0; i < e.args.size(); ++i) {
+      if (!e.args[i] || !Bind(*e.args[i], &args[i])) return false;
+      all_literal = all_literal && args[i]->kind == BNode::LIT;
+    }
+    FunctionRegistry* reg = ctx.Registry ? ctx.Registry : GetFunctionRegistry();
+    if (e.name == "cast" && reg->GetFunction(e.name)) {   // the cast meta function: a literal is cast here, as it takes scalars
+      const auto* co = dynamic_cast<const CastOptions*>(e.options.get());
+      if (!co || co->ToType == Type::NA || args.size() != 1) return false;
+      return CastTo(args[0], co->ToType, *co, out);
+    }
+    if (all_literal) return false;   // scalar-only execution is refused by CallFunction
+    const Function* fn = reg->GetFunction(e.name);
+    if (!fn) return false;
+    if (fn->Kind() != FuncKind::SCALAR || (int)args.size() != fn->Arity()) return false;
+    const auto* sfn = static_cast<const ScalarFunction*>(fn);
+    std::vector<Type> types;
+    for (auto& a : args) types.push_back(a->out);
+    const exec::ScalarKernel* k = nullptr;
+    if (!sfn->DispatchBest(&types, &k).ok() || k->expr_op < 0) return false;
+    for (size_t i = 0; i < args.size(); ++i)   // the implicit safe casts of exec.go:101-121
+      if (!CastTo(args[i], types[i], SafeCastOptions(types[i]), &args[i])) return false;
+    const Type res = k->out_type(types);
+    int flags = 0;
+    if (k->expr_op == AG_EXPR_CAST) {   // cast_<type> by name: its options are the call's
+      const auto* co = dynamic_cast<const CastOptions*>(e.options.get());
+      if (!co) return false;
+      flags = CastFlags(*co);
+    }
+    // A null literal operand: the checked kernels write nothing (helpers.go:287) and the boolean kernels leave the data
+    // at 0, so the result is 0 and null in every row; the other operand still runs for its failures.
+    const int op = k->expr_op;
+    const bool empty_on_null = op == AG_EXPR_ADD_CHECKED || op == AG_EXPR_SUB_CHECKED || op == AG_EXPR_MUL_CHECKED || op == AG_EXPR_DIV ||
+                               op == AG_EXPR_DIV_CHECKED || (op >= AG_EXPR_SHL && op <= AG_EXPR_SHR_CHECKED) ||
+                               (op >= AG_EXPR_AND && op <= AG_EXPR_AND_NOT);
+    if (empty_on_null && args.size() == 2 && (IsNullLiteral(args[0]) || IsNullLiteral(args[1]))) {
+      *out = Op(AG_EXPR_NULL_OF, res, res, {IsNullLiteral(args[0]) ? args[1] : args[0]});
+      return true;
+    }
+    *out = Op(op, types.empty() ? res : types[0], res, args, flags);
+    return true;
+  }
+};
+
+// Sethi-Ullman label (registers the subtree needs), its distinct columns and its instruction count.
+struct Need { int regs = 1, nodes = 1; std::vector<int> cols; };
+Need Measure(const BPtr& n) {
+  Need r;
+  if (n->kind == BNode::COL) { r.cols = {n->col}; return r; }
+  if (n->kind == BNode::LIT) return r;
+  std::vector<Need> c;
+  for (auto& a : n->args) c.push_back(Measure(a));
+  r.nodes = 1;
+  for (auto& x : c) { r.nodes += x.nodes; r.cols.insert(r.cols.end(), x.cols.begin(), x.cols.end()); }
+  std::sort(r.cols.begin(), r.cols.end());
+  r.cols.erase(std::unique(r.cols.begin(), r.cols.end()), r.cols.end());
+  r.regs = c[0].regs;
+  if (c.size() == 2) r.regs = c[0].regs == c[1].regs ? c[0].regs + 1 : std::max(c[0].regs, c[1].regs);
+  return r;
+}
+bool Fits(const Need& n) { return n.regs <= AG_EXPR_MAX_REGS && (int)n.cols.size() <= AG_EXPR_MAX_COLS && n.nodes <= AG_EXPR_MAX_INSTR; }
+
+struct Emitter {
+  std::vector<ag_expr_instr> ins;
+  std::vector<int> col_slot;    // program column -> index into the bound columns
+  std::vector<int> free_regs;
+  int Alloc() { int r = free_regs.back(); free_regs.pop_back(); return r; }
+  int Slot(int c) {
+    for (size_t i = 0; i < col_slot.size(); ++i) if (col_slot[i] == c) return (int)i;
+    col_slot.push_back(c);
+    return (int)col_slot.size() - 1;
+  }
+  // Post-order; of two arguments the one that needs more registers goes first, and the result reuses its register.
+  int Gen(const BPtr& n) {
+    ag_expr_instr in{};
+    in.out_type = (int)n->out;
+    if (n->kind != BNode::OP) {
+      in.dst = Alloc();
+      in.type = (int)n->out;
+      if (n->kind == BNode::COL) { in.op = AG_EXPR_LOAD; in.a = Slot(n->col); }
+      else { in.op = AG_EXPR_CONST; in.flags = n->lit->valid ? 1 : 0; memcpy(&in.bits, n->lit->value, 8); }
+      ins.push_back(in);
+      return in.dst;
+    }
+    in.op = n->op; in.type = (int)n->type; in.flags = n->flags;
+    if (n->args.size() == 1) {
+      in.a = in.dst = Gen(n->args[0]);
+    } else {
+      const bool left_first = Measure(n->args[0]).regs >= Measure(n->args[1]).regs;
+      if (left_first) { in.a = Gen(n->args[0]); in.b = Gen(n->args[1]); }
+      else { in.b = Gen(n->args[1]); in.a = Gen(n->args[0]); }
+      in.dst = in.a;
+      free_regs.push_back(in.b);
+    }
+    ins.push_back(in);
+    return in.dst;
+  }
+};
+
+// One program over the rows of `cols`: spans from iterateExecSpans over the chunk layouts of the columns it reads,
+// one ag_eval_program_dev launch, the output as one array.  *failed: some op of the program failed.
+Status RunProgram(const BPtr& root, const std::vector<ExprColumn>& cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
+  Emitter em;
+  for (int r = AG_EXPR_MAX_REGS - 1; r >= 0; --r) em.free_regs.push_back(r);
+  ag_expr_program prog{};
+  prog.out_reg = em.Gen(root);
+  prog.n_instr = (int)em.ins.size();
+  prog.instr = em.ins.data();
+  std::vector<int32_t> col_types;
+  std::vector<std::vector<int64_t>> lens;
+  for (int c : em.col_slot) {
+    col_types.push_back((int32_t)cols[c].type);
+    std::vector<int64_t> l;
+    for (auto& ch : cols[c].chunks) l.push_back(ch->length);
+    lens.push_back(l);
+  }
+  prog.n_cols = (int)col_types.size();
+  prog.col_types = col_types.data();
+  std::vector<SpanPiece> pieces;
+  RETURN_NOT_OK(IterateExecSpans(lens, std::vector<bool>(lens.size(), true), INT64_MAX, &pieces));
+  std::vector<ag_sort_chunk> spans;
+  int64_t n_spans = 0;
+  for (auto& p : pieces) {
+    if (p.len == 0) continue;
+    for (size_t j = 0; j < em.col_slot.size(); ++j) {
+      const ArrayData& a = *cols[em.col_slot[j]].chunks[p.chunk_index[j]];
+      spans.push_back(ag_sort_chunk{a.buffers[1] ? a.buffers[1]->data() : nullptr, ValidityOrNull(a), a.offset + p.chunk_pos[j], p.len});
+    }
+    ++n_spans;
+  }
+  const Type out_type = root->out;
+  std::shared_ptr<Buffer> data, valid, word;
+  RETURN_NOT_OK(Buffer::Allocate(out_type == Type::BOOL ? ((nrows + 31) / 32) * 4 : nrows * (BitWidth(out_type) / 8), &data));
+  RETURN_NOT_OK(Buffer::Allocate(((nrows + 31) / 32) * 4, &valid));
+  RETURN_NOT_OK(Buffer::Allocate(8, &word));
+  NATIVE(ag_error_word_reset_dev((int64_t*)word->data(), nullptr));
+  NATIVE(ag_eval_program_dev(&prog, n_spans, spans.data(), data->data(), valid->data(), (int64_t*)word->data(), nullptr));
+  int64_t bad = AG_NO_ERROR_POS;
+  RETURN_NOT_OK(word->ToHost(&bad, 8));
+  *failed = bad != AG_NO_ERROR_POS;
+  auto a = std::make_shared<ArrayData>();
+  a->type = out_type; a->length = nrows; a->offset = 0; a->null_count = kUnknownNullCount;
+  a->buffers[0] = valid; a->buffers[1] = data;
+  *out = a;
+  return Status::OK();
+}
+
+// A tree that needs more registers, columns or instructions than one program holds: its largest subtree that does not
+// fit is evaluated first, as programs of its own, and enters the rest as a column.
+Status RunFused(BPtr root, std::vector<ExprColumn>* cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
+  while (!Fits(Measure(root))) {
+    // descend into an argument that does not fit; below a node whose arguments all fit, take its largest argument
+    BPtr* slot = &root;
+    for (bool fits = false; !fits;) {
+      BPtr* next = nullptr;
+      Need best;
+      for (auto& a : (*slot)->args) {
+        if (a->kind != BNode::OP) continue;
+        const Need m = Measure(a);
+        const bool better = !next || (Fits(best) && !Fits(m)) ||
+                            (Fits(best) == Fits(m) && std::make_tuple(m.regs, m.cols.size(), m.nodes) > std::make_tuple(best.regs, best.cols.size(), best.nodes));
+        if (better) { next = &a; best = m; }
+      }
+      slot = next;
+      fits = Fits(best);
+    }
+    std::shared_ptr<ArrayData> part;
+    RETURN_NOT_OK(RunProgram(*slot, *cols, nrows, &part, failed));
+    if (*failed) return Status::OK();
+    cols->push_back(ExprColumn{part->type, {part}});
+    auto leaf = std::make_shared<BNode>();
+    leaf->kind = BNode::COL; leaf->col = (int)cols->size() - 1; leaf->out = part->type;
+    *slot = leaf;
+  }
+  return RunProgram(root, *cols, nrows, out, failed);
+}
+
+}  // namespace
+
+Status ExecuteScalarExpression(const ExecCtx& ctx, const Expression& expr, const Datum& input, Datum* out) {
+  if (input.kind != DatumKind::RECORD && input.kind != DatumKind::TABLE)
+    return Status::Invalid("ExecuteScalarExpression takes a record batch or a table");
+  std::vector<ExprColumn> cols;
+  Binder b{ctx, input, &cols, {}};
+  BPtr root;
+  if (!b.Bind(expr, &root) || root->kind != BNode::OP) return EvalNodeByNode(ctx, expr, input, out);
+  std::shared_ptr<ArrayData> res;
+  bool failed = false;
+  RETURN_NOT_OK(RunFused(root, &cols, input.Len(), &res, &failed));
+  if (failed) return EvalNodeByNode(ctx, expr, input, out);   // its status, message included
+  if (input.kind == DatumKind::RECORD) { *out = Datum(res); return Status::OK(); }
+  auto c = std::make_shared<ChunkedArray>();
+  c->type = res->type; c->length = res->length; c->chunks = {res};
+  *out = Datum(c);
+  return Status::OK();
 }
 
 }  // namespace compute

@@ -683,6 +683,113 @@ ag_status ag_take_columns_dev(int ncols, const ag_take_column* cols, int64_t nro
                               int64_t* d_bad_pos, ag_stream_t s);
 
 /* ================================================================================= *
+ * Scalar expressions as one register program — the device half of ExecuteScalarExpression
+ * (arrow/compute/exprs/exec.go:542-700) over expression trees (arrow/compute/expression.go: NewLiteral, NewFieldRef,
+ * NewCall, Cast).  The host compiler (arrowgpu::compute::ExecuteScalarExpression) binds a tree through the registry,
+ * emits it in post-order with registers in Sethi-Ullman order, and runs it with one launch of expr_eval_kernel over
+ * every span of a record batch or table.
+ *
+ *   Registers hold one value per row (any of the 10 numeric types, or BOOL) and a validity bit per row.  Each op
+ *   computes what the single-op kernel of its registered function computes in EVERY slot, nulls included:
+ *     ADD SUB MUL BIT_AND BIT_OR BIT_XOR             ScalarBinary: every slot; validity = a & b
+ *     ADD_CHECKED SUB_CHECKED DIV DIV_CHECKED SHL SHR SHL_CHECKED SHR_CHECKED
+ *                                                    ScalarBinaryNotNull: computed where a and b are valid, 0 elsewhere;
+ *                                                    overflow / zero divisor (integers: both DIVs; floats: DIV_CHECKED) /
+ *                                                    shift out of range (the _CHECKED shifts) fails the program
+ *     MUL_CHECKED                                    every slot, fails on overflow in ANY slot (checked multiply)
+ *     ABS NEG NEG_UNSIGNED_ZERO SIGN BIT_NOT         every slot; validity = a
+ *     ABS_CHECKED NEG_CHECKED                        signed integers, every slot, MinInt fails
+ *     EQ NE GT GE LT LE                              BOOL result, every slot; validity = a & b
+ *     AND OR XOR AND_NOT / NOT                       BOOL, every slot; validity = a & b / a
+ *     KLEENE_AND KLEENE_OR KLEENE_AND_NOT            the Kleene truth tables of scalar_boolean.go:42-46
+ *     IS_NULL IS_NOT_NULL IS_NAN                     BOOL result, no nulls
+ *     CAST                                           type -> out_type; fails at a valid row as the checked cast does,
+ *                                                    unless `flags` allows int overflow / float truncation
+ *     LOAD                                           dst <- column a (type = the column's type)
+ *     CONST                                          dst <- `bits` (raw little-endian value) in every row, valid iff
+ *                                                    flags & 1
+ *     NULL_OF                                        dst <- out_type value 0, every row null (a is evaluated first and
+ *                                                    its failures count): a checked op with a null literal operand
+ *   `type` is the operand type, `out_type` the result type (CAST, NULL_OF: the target; other ops: what the op gives).
+ *
+ * ag_eval_program[_dev](prog, n_spans, spans, out, out_valid, error):
+ *   spans: HOST array of n_spans * prog->n_cols chunk descriptors, span i column j at [i * n_cols + j]; every column of
+ *   a span has the span's length, offsets are element offsets (bit offsets for BOOL values and every bitmap) and need
+ *   not be multiples of 8; a NULL validity pointer means no nulls.  Output rows start at 0 in span order: `out` holds
+ *   the values (BOOL: a bitmap), `out_valid` (may be NULL) the validity; output bitmaps are written in whole 32-bit
+ *   words and must be 4-byte aligned.  Device flavour: the span pointers are device pointers and *d_error_word
+ *   (reset with ag_error_word_reset_dev) is lowered to the lowest failing output row.  Host flavour: host pointers,
+ *   a failing program returns AG_ERR_INVALID "expression failed at row %lld" and stores the row in *first_bad (may
+ *   be NULL).  A malformed program — an unknown op, a register or column index out of range, operand types that do
+ *   not fit the op, more than AG_EXPR_MAX_* instructions or columns — is AG_ERR_INVALID before any launch.
+ * ================================================================================= */
+#define AG_EXPR_MAX_REGS   8
+#define AG_EXPR_MAX_COLS  16
+#define AG_EXPR_MAX_INSTR 128
+#define AG_EXPR_LOAD               0
+#define AG_EXPR_CONST              1
+#define AG_EXPR_NULL_OF            2
+#define AG_EXPR_ADD                3
+#define AG_EXPR_SUB                4
+#define AG_EXPR_MUL                5
+#define AG_EXPR_ADD_CHECKED        6
+#define AG_EXPR_SUB_CHECKED        7
+#define AG_EXPR_MUL_CHECKED        8
+#define AG_EXPR_DIV                9
+#define AG_EXPR_DIV_CHECKED       10
+#define AG_EXPR_BIT_AND           11
+#define AG_EXPR_BIT_OR            12
+#define AG_EXPR_BIT_XOR           13
+#define AG_EXPR_SHL               14
+#define AG_EXPR_SHR               15
+#define AG_EXPR_SHL_CHECKED       16
+#define AG_EXPR_SHR_CHECKED       17
+#define AG_EXPR_ABS               18
+#define AG_EXPR_NEG               19
+#define AG_EXPR_NEG_UNSIGNED_ZERO 20
+#define AG_EXPR_SIGN              21
+#define AG_EXPR_BIT_NOT           22
+#define AG_EXPR_ABS_CHECKED       23
+#define AG_EXPR_NEG_CHECKED       24
+#define AG_EXPR_EQ                25
+#define AG_EXPR_NE                26
+#define AG_EXPR_GT                27
+#define AG_EXPR_GE                28
+#define AG_EXPR_LT                29
+#define AG_EXPR_LE                30
+#define AG_EXPR_AND               31
+#define AG_EXPR_OR                32
+#define AG_EXPR_XOR               33
+#define AG_EXPR_AND_NOT           34
+#define AG_EXPR_KLEENE_AND        35
+#define AG_EXPR_KLEENE_OR         36
+#define AG_EXPR_KLEENE_AND_NOT    37
+#define AG_EXPR_NOT               38
+#define AG_EXPR_IS_NULL           39
+#define AG_EXPR_IS_NOT_NULL       40
+#define AG_EXPR_IS_NAN            41
+#define AG_EXPR_CAST              42
+#define AG_EXPR_ALLOW_INT_OVERFLOW   1 /* CAST flags */
+#define AG_EXPR_ALLOW_FLOAT_TRUNCATE 2
+typedef struct ag_expr_instr {
+  int32_t op, type, out_type;
+  int32_t dst, a, b;   /* registers; LOAD: a = column */
+  int32_t flags;       /* CONST: 1 = valid; CAST: AG_EXPR_ALLOW_* */
+  uint64_t bits;       /* CONST: the value */
+} ag_expr_instr;
+typedef struct ag_expr_program {
+  int32_t n_instr;
+  const ag_expr_instr* instr;  /* host memory */
+  int32_t n_cols;
+  const int32_t* col_types;    /* host memory: AG_TYPE_BOOL or a numeric type per column */
+  int32_t out_reg;
+} ag_expr_program;
+ag_status ag_eval_program(const ag_expr_program* prog, int64_t n_spans, const ag_sort_chunk* spans, void* out, uint8_t* out_valid,
+                          int64_t* first_bad);
+ag_status ag_eval_program_dev(const ag_expr_program* prog, int64_t n_spans, const ag_sort_chunk* spans, void* out,
+                              uint8_t* out_valid, int64_t* d_error_word, ag_stream_t s);
+
+/* ================================================================================= *
  * Parquet decode primitives (SURVEY 8f rank 4: the feeder side) — the SIMD leaf loops arrow-go links under
  *   parquet/internal, so pages can be decoded into device-resident Arrow buffers.
  *   ag_parquet_unpack32 ↔ unpack32_avx2 (parquet/internal/utils/_lib/bit_packing_avx2.c:1772): values of

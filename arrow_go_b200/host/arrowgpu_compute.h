@@ -148,6 +148,10 @@ struct Datum {
   Type type() const;    // NA for record batches and tables
   int64_t Len() const;  // -1 for scalars (datum.go: scalars have no length); the row count of a record batch or table
 };
+// The columns of a record batch or table: how many (0 for any other datum), and column i as it is held (an array for
+// a record batch, a chunked array for a table).  ColumnDatum does not check i.
+int NumColumns(const Datum& d);
+Datum ColumnDatum(const Datum& d, int i);
 
 }  // namespace compute
 
@@ -160,7 +164,6 @@ struct BufferSpan {  // exec/span.go:32-50
   uint8_t* buf = nullptr;  // DEVICE pointer
   int64_t len = 0;         // bytes
   std::shared_ptr<Buffer> owner;
-  bool self_alloc = false;
 };
 
 struct ArraySpan {  // exec/span.go:76-88

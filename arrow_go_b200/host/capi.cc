@@ -216,15 +216,11 @@ int agx_sort_indices_keys(agx_datum* d, const int* columns, const int* orders, c
   return AG_OK;
 }
 // The columns of a record batch (arrays) or a table (chunked arrays); Datum chunks stay [] for both
-int agx_num_columns(agx_datum* d) {
-  if (d->d.kind == DatumKind::RECORD) return (int)d->d.record->columns.size();
-  if (d->d.kind == DatumKind::TABLE) return (int)d->d.table->columns.size();
-  return 0;
-}
+int agx_num_columns(agx_datum* d) { return NumColumns(d->d); }
 int agx_column(agx_datum* d, int i, agx_datum** out) {
   if (d->d.kind != DatumKind::RECORD && d->d.kind != DatumKind::TABLE) return fail(Status::Invalid("column: not a record batch or table"));
-  if (i < 0 || i >= agx_num_columns(d)) return fail(Status::Invalid("column: out of range"));
-  *out = d->d.kind == DatumKind::RECORD ? new agx_datum{Datum(d->d.record->columns[i])} : new agx_datum{Datum(d->d.table->columns[i])};
+  if (i < 0 || i >= NumColumns(d->d)) return fail(Status::Invalid("column: out of range"));
+  *out = new agx_datum{ColumnDatum(d->d, i)};
   return AG_OK;
 }
 // compute.FilterRecordBatch / FilterTable with FilterOptions{NullSelection} (selection.go:679-800)

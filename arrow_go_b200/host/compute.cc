@@ -52,6 +52,10 @@ Status Status::FromNative(int c) {
 
 static inline int64_t BytesForBits(int64_t n) { return (n + 7) / 8; }
 static inline int64_t DataBytes(Type t, int64_t n) { return t == Type::BOOL ? BytesForBits(n) : n * (BitWidth(t) / 8); }
+// An n-bit bitmap rounded up to whole 32-bit words: what the kernels that store a word at a time write.
+static inline int64_t BitmapWordBytes(int64_t nbits) { return ((nbits + 31) / 32) * 4; }
+// Point a span buffer at all of `b`.
+static void SetBuffer(exec::BufferSpan* s, const std::shared_ptr<Buffer>& b) { s->buf = b->data(); s->len = b->size(); s->owner = b; }
 
 // ---------------------------------------------------------------- Buffer ------------------
 Buffer::~Buffer() {
@@ -249,6 +253,14 @@ int64_t ChunkedArray::NullN() const {
   return n;
 }
 
+// A chunked array of type `t` over `chunks`, its length their sum.
+static std::shared_ptr<ChunkedArray> MakeChunked(Type t, std::vector<std::shared_ptr<ArrayData>> chunks) {
+  auto c = std::make_shared<ChunkedArray>();
+  c->type = t; c->chunks = std::move(chunks);
+  for (auto& a : c->chunks) c->length += a->length;
+  return c;
+}
+
 Status MakeRecordBatch(int64_t num_rows, std::vector<std::shared_ptr<ArrayData>> columns, std::shared_ptr<RecordBatch>* out) {
   if (num_rows < 0) return Status::Invalid("record batch: negative row count");
   for (size_t i = 0; i < columns.size(); ++i)
@@ -290,6 +302,29 @@ int64_t Datum::Len() const {
     default: return -1;
   }
 }
+
+int NumColumns(const Datum& d) {
+  if (d.kind == DatumKind::RECORD) return (int)d.record->columns.size();
+  if (d.kind == DatumKind::TABLE) return (int)d.table->columns.size();
+  return 0;
+}
+Datum ColumnDatum(const Datum& d, int i) {
+  return d.kind == DatumKind::RECORD ? Datum(d.record->columns[i]) : Datum(d.table->columns[i]);
+}
+
+namespace {
+// The chunks of an array (the array itself) or of a chunked array.
+std::vector<std::shared_ptr<ArrayData>> ArrayChunks(const Datum& d) {
+  return d.kind == DatumKind::ARRAY ? std::vector<std::shared_ptr<ArrayData>>{d.array} : d.chunked->chunks;
+}
+
+// A column of a record batch or table as its type and chunks (a record batch column is one chunk).
+struct Column { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
+Column GetColumn(const Datum& d, int i) {
+  const Datum c = ColumnDatum(d, i);
+  return Column{c.type(), ArrayChunks(c)};
+}
+}  // namespace
 }  // namespace compute
 
 // ======================================================================================
@@ -301,11 +336,7 @@ void ArraySpan::SetMembers(const ArrayData& d) {
   type = d.type; len = d.length; nulls = d.null_count; offset = d.offset;
   for (int i = 0; i < 2; ++i) {
     buffers[i] = BufferSpan();
-    if (d.buffers[i]) {
-      buffers[i].buf = d.buffers[i]->data();
-      buffers[i].len = d.buffers[i]->size();
-      buffers[i].owner = d.buffers[i];
-    }
+    if (d.buffers[i]) SetBuffer(&buffers[i], d.buffers[i]);
   }
   if (!buffers[0].buf && type != Type::NA) nulls = 0;  // no validity bitmap => no nulls
 }
@@ -386,7 +417,7 @@ Status PropagateNulls(KernelCtx* ctx, const ExecSpan& batch, ArraySpan* out) {  
   auto alloc_bitmap = [&]() -> Status {
     std::shared_ptr<Buffer> buf;
     RETURN_NOT_OK(ctx->AllocateBitmap(out->len + out->offset, &buf));
-    out->buffers[0].buf = buf->data(); out->buffers[0].len = buf->size(); out->buffers[0].owner = buf; out->buffers[0].self_alloc = true;
+    SetBuffer(&out->buffers[0], buf);
     return Status::OK();
   };
   if (is_all_null) {
@@ -412,7 +443,7 @@ Status PropagateNulls(KernelCtx* ctx, const ExecSpan& batch, ArraySpan* out) {  
         NATIVE(ag_bitmap_copy_dev(arr->buffers[0].buf, arr->offset, arr->len, out->buffers[0].buf, out->offset, nullptr));
         return Status::OK();
       }
-      if (arr->offset == 0) { out->buffers[0] = arr->buffers[0]; out->buffers[0].self_alloc = false; return Status::OK(); }  // zero-copy share
+      if (arr->offset == 0) { out->buffers[0] = arr->buffers[0]; return Status::OK(); }  // zero-copy share
       // (the reference also zero-copies byte-aligned offsets with SliceBuffer; a device Buffer has no
       //  sub-buffer view here, so those are copied like the unaligned case — same bits)
       RETURN_NOT_OK(alloc_bitmap());
@@ -469,6 +500,17 @@ Status IterateExecSpans(const std::vector<std::vector<int64_t>>& lens, const std
   }
   return Status::OK();
 }
+
+namespace {
+// IterateExecSpans over the chunk lengths of each argument (no chunks for a scalar).
+Status ChunkSpans(const std::vector<std::vector<std::shared_ptr<ArrayData>>>& args, const std::vector<bool>& is_chunked,
+                  int64_t max_chunk_size, std::vector<SpanPiece>* out) {
+  std::vector<std::vector<int64_t>> lens(args.size());
+  for (size_t i = 0; i < args.size(); ++i)
+    for (auto& c : args[i]) lens[i].push_back(c->length);
+  return IterateExecSpans(lens, is_chunked, max_chunk_size, out);
+}
+}  // namespace
 
 // ---------------------------------------------------------------- registry ----------------
 Status FunctionRegistry::AddFunction(std::shared_ptr<Function> fn, bool allow_overwrite) {
@@ -571,6 +613,7 @@ struct ErrorWord {  // device int64 "first failing row", reset per call
   std::shared_ptr<Buffer> buf;
   Status Init() { RETURN_NOT_OK(Buffer::Allocate(8, &buf)); NATIVE(ag_error_word_reset_dev((int64_t*)buf->data(), nullptr)); return Status::OK(); }
   Status Read(int64_t* v) { return buf->ToHost(v, 8); }
+  int64_t* word() const { return (int64_t*)buf->data(); }
 };
 }  // namespace
 
@@ -593,19 +636,19 @@ Status ScalarFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
   const Type out_type = kernel->out_type(in_types);
 
   // span iteration metadata
-  std::vector<std::vector<int64_t>> lens(args.size());
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> chunks(args.size());
   std::vector<bool> is_chunked(args.size(), false);
   bool have_chunked = false, all_scalar = true;
   for (size_t i = 0; i < args.size(); ++i) {
-    if (args[i].kind == DatumKind::ARRAY) { lens[i] = {args[i].array->length}; all_scalar = false; }
-    else if (args[i].kind == DatumKind::CHUNKED) {
-      is_chunked[i] = true; have_chunked = true; all_scalar = false;
-      for (auto& c : args[i].chunked->chunks) lens[i].push_back(c->length);
-    }
+    if (args[i].kind != DatumKind::ARRAY && args[i].kind != DatumKind::CHUNKED) continue;
+    chunks[i] = ArrayChunks(args[i]);
+    is_chunked[i] = args[i].kind == DatumKind::CHUNKED;
+    have_chunked = have_chunked || is_chunked[i];
+    all_scalar = false;
   }
   if (all_scalar) return Status::NotImplemented("scalar-only execution (PromoteExecSpanScalars) is not part of the accelerated path");
   std::vector<SpanPiece> pieces;
-  RETURN_NOT_OK(IterateExecSpans(lens, is_chunked, ectx.ChunkSize, &pieces));
+  RETURN_NOT_OK(ChunkSpans(chunks, is_chunked, ectx.ChunkSize, &pieces));
   int64_t total = 0;
   for (size_t i = 0; i < args.size(); ++i) if (args[i].kind != DatumKind::SCALAR) { total = args[i].Len(); break; }
 
@@ -627,7 +670,7 @@ Status ScalarFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
   kctx.kernel = kernel;
   kctx.state = opts;
   ErrorWord err_word;
-  if (kernel->can_fail) { RETURN_NOT_OK(err_word.Init()); kctx.error_word = (int64_t*)err_word.buf->data(); }
+  if (kernel->can_fail) { RETURN_NOT_OK(err_word.Init()); kctx.error_word = err_word.word(); }
 
   auto prepare_output = [&](int64_t length, ArraySpan* o) -> Status {  // prepareOutput, executor.go:441-470
     *o = ArraySpan();
@@ -635,12 +678,12 @@ Status ScalarFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
     if (validity_prealloc) {
       std::shared_ptr<Buffer> b;
       RETURN_NOT_OK(kctx.AllocateBitmap(length, &b));
-      o->buffers[0].buf = b->data(); o->buffers[0].len = b->size(); o->buffers[0].owner = b; o->buffers[0].self_alloc = true;
+      SetBuffer(&o->buffers[0], b);
     }
     if (data_prealloc) {
       std::shared_ptr<Buffer> b;
       RETURN_NOT_OK(kctx.Allocate(DataBytes(out_type, length), &b));  // allocateDataBuffer, executor.go:155-163
-      o->buffers[1].buf = b->data(); o->buffers[1].len = b->size(); o->buffers[1].owner = b; o->buffers[1].self_alloc = true;
+      SetBuffer(&o->buffers[1], b);
     }
     if (kernel->null_handling == exec::NullHandling::OUTPUT_NOT_NULL || elide_validity) o->nulls = 0;
     return Status::OK();
@@ -717,10 +760,7 @@ Status ScalarFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
   }
   // emitResult :704-708 recounts nulls lazily; we leave them unknown (ToHost counts on demand)
   if (have_chunked) {  // WrapResults: Chunked if any input was chunked (executor.go:521-580)
-    auto c = std::make_shared<ChunkedArray>();
-    c->type = out_type; c->chunks = results;
-    for (auto& r : results) c->length += r->length;
-    *out = Datum(c);
+    *out = Datum(MakeChunked(out_type, results));
   } else {
     *out = Datum(results.empty() ? std::make_shared<ArrayData>() : results[0]);
   }
@@ -742,12 +782,13 @@ Status VectorFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
   kctx.kernel = kernel;
   kctx.state = opts;
   bool have_chunked = false;
-  std::vector<std::vector<int64_t>> lens(args.size());
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> chunks(args.size());
   std::vector<bool> is_chunked(args.size(), false);
   for (size_t i = 0; i < args.size(); ++i) {
     if (args[i].kind == DatumKind::SCALAR) return Status::NotImplemented("vector kernels take array-like arguments");
-    if (args[i].kind == DatumKind::ARRAY) lens[i] = {args[i].array->length};
-    else { is_chunked[i] = true; have_chunked = true; for (auto& c : args[i].chunked->chunks) lens[i].push_back(c->length); }
+    chunks[i] = ArrayChunks(args[i]);
+    is_chunked[i] = args[i].kind != DatumKind::ARRAY;
+    have_chunked = have_chunked || is_chunked[i];
   }
   std::vector<std::shared_ptr<ArrayData>> results;
   if (kernel->can_execute_chunkwise) {
@@ -755,7 +796,7 @@ Status VectorFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
     int64_t l0 = args[0].Len();
     for (auto& a : args) if (a.Len() != l0) return Status::Invalid("vector kernel arguments must all be the same length");
     std::vector<SpanPiece> pieces;
-    RETURN_NOT_OK(IterateExecSpans(lens, is_chunked, INT64_MAX, &pieces));
+    RETURN_NOT_OK(ChunkSpans(chunks, is_chunked, INT64_MAX, &pieces));
     if (pieces.empty()) { SpanPiece p; p.pos = 0; p.len = 0; p.chunk_index.assign(args.size(), 0); p.chunk_pos.assign(args.size(), 0); pieces.push_back(p); }
     for (auto& p : pieces) {
       ExecSpan span;
@@ -789,10 +830,7 @@ Status VectorFunction::Execute(const ExecCtx& ectx, const FunctionOptions* opts,
     results.push_back(o.MakeData());
   }
   if (have_chunked) {
-    auto c = std::make_shared<ChunkedArray>();
-    c->type = out_type; c->chunks = results;
-    for (auto& r : results) c->length += r->length;
-    *out = Datum(c);
+    *out = Datum(MakeChunked(out_type, results));
   } else {
     *out = Datum(results[0]);
   }
@@ -837,11 +875,26 @@ bool MayHaveNulls(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
   return false;
 }
 
+// Rows [pos, pos + len) of `a` as one chunk of a device chunk list.
+ag_sort_chunk ChunkDesc(const ArrayData& a, int64_t pos, int64_t len) {
+  return ag_sort_chunk{a.buffers[1] ? a.buffers[1]->data() : nullptr, ValidityOrNull(a), a.offset + pos, len};
+}
 // The chunk list of a column for ag_sort_indices_keys_dev / ag_take_columns_dev.
 std::vector<ag_sort_chunk> ChunkDescs(const std::vector<std::shared_ptr<ArrayData>>& chunks) {
   std::vector<ag_sort_chunk> d;
-  for (auto& a : chunks) d.push_back(ag_sort_chunk{a->buffers[1] ? a->buffers[1]->data() : nullptr, ValidityOrNull(*a), a->offset, a->length});
+  for (auto& a : chunks) d.push_back(ChunkDesc(*a, 0, a->length));
   return d;
+}
+
+// A new array of `n` rows of type `t` at offset 0 (preallocateData, vector_selection.go:83-93): the values (word-rounded
+// for BOOL) and, exactly when `nullable`, a word-rounded validity bitmap with an unknown null count.
+Status AllocateOutput(Type t, int64_t n, bool nullable, std::shared_ptr<ArrayData>* out) {
+  auto d = std::make_shared<ArrayData>();
+  d->type = t; d->length = n; d->offset = 0; d->null_count = nullable ? kUnknownNullCount : 0;
+  RETURN_NOT_OK(Buffer::Allocate(t == Type::BOOL ? BitmapWordBytes(n) : n * (BitWidth(t) / 8), &d->buffers[1]));
+  if (nullable) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(n), &d->buffers[0]));
+  *out = std::move(d);
+  return Status::OK();
 }
 
 // The IndexError naming the index at row `row` of the `type` indices starting at element `offset` of `buf` (helpers.go:951).
@@ -1064,7 +1117,7 @@ Status IsNullExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out) {
   if (in.buffers[0].buf) NATIVE(ag_bitmap_invert_dev(in.buffers[0].buf, in.offset, in.len, b->data(), 0, nullptr));
   out->type = Type::BOOL; out->len = in.len; out->offset = 0; out->nulls = 0;
   out->buffers[0] = exec::BufferSpan();
-  out->buffers[1].buf = b->data(); out->buffers[1].len = b->size(); out->buffers[1].owner = b; out->buffers[1].self_alloc = true;
+  SetBuffer(&out->buffers[1], b);
   return Status::OK();
 }
 Status IsNotNullExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out) {
@@ -1075,7 +1128,7 @@ Status IsNotNullExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out) {
   else NATIVE(ag_bitmap_set_dev(b->data(), 0, in.len, 1, nullptr));  // memory.Set(0xFF)
   out->type = Type::BOOL; out->len = in.len; out->offset = 0; out->nulls = 0;
   out->buffers[0] = exec::BufferSpan();
-  out->buffers[1].buf = b->data(); out->buffers[1].len = b->size(); out->buffers[1].owner = b; out->buffers[1].self_alloc = true;
+  SetBuffer(&out->buffers[1], b);
   return Status::OK();
 }
 // isNanKernelExec (scalar_comparisons.go:754-765): the NE kernel with the input on both sides;
@@ -1184,12 +1237,12 @@ Status NotExec(KernelCtx*, const ExecSpan& batch, ExecResult* out) {
   const ArraySpan& in = batch.values[0].array;
   NATIVE(ag_bitmap_invert_dev(in.buffers[1].buf, in.offset, in.len, out->buffers[1].buf, out->offset, nullptr));
   if (in.buffers[0].buf && in.nulls != 0) {
-    if (in.offset == out->offset) { out->buffers[0] = in.buffers[0]; out->buffers[0].self_alloc = false; }
+    if (in.offset == out->offset) out->buffers[0] = in.buffers[0];
     else {
       std::shared_ptr<Buffer> b;
       RETURN_NOT_OK(Buffer::Allocate((out->offset + out->len + 7) / 8, &b));
       NATIVE(ag_bitmap_copy_dev(in.buffers[0].buf, in.offset, in.len, b->data(), out->offset, nullptr));
-      out->buffers[0].buf = b->data(); out->buffers[0].len = b->size(); out->buffers[0].owner = b; out->buffers[0].self_alloc = true;
+      SetBuffer(&out->buffers[0], b);
     }
   }
   out->nulls = in.nulls;
@@ -1212,21 +1265,14 @@ Status PrimitiveFilterExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* ou
   NATIVE(ag_filter_output_size_dev(filter.buffers[1].buf, mvalid, filter.offset, filter.len, sel, (int64_t*)scal->data(), nullptr));
   int64_t out_len = 0;
   RETURN_NOT_OK(scal->ToHost(&out_len, 8));
-  out->nulls = (vn == 0 && (sel == DropNulls || fn == 0)) ? 0 : kUnknownNullCount;  // :464-468
   const bool allocate_validity = vn != 0 || fn != 0;                                  // :473
-  const int bw = BitWidth(values.type);
-  // preallocateData (:83-93)
-  out->type = values.type; out->len = out_len; out->offset = 0;
-  std::shared_ptr<Buffer> data, valid;
-  RETURN_NOT_OK(ctx->Allocate(bw == 1 ? ((out_len + 31) / 32) * 4 : out_len * (bw / 8), &data));
-  out->buffers[1].buf = data->data(); out->buffers[1].len = data->size(); out->buffers[1].owner = data; out->buffers[1].self_alloc = true;
-  if (allocate_validity) {
-    RETURN_NOT_OK(ctx->Allocate(((out_len + 31) / 32) * 4, &valid));
-    out->buffers[0].buf = valid->data(); out->buffers[0].len = valid->size(); out->buffers[0].owner = valid; out->buffers[0].self_alloc = true;
-  }
+  std::shared_ptr<ArrayData> res;
+  RETURN_NOT_OK(AllocateOutput(values.type, out_len, allocate_validity, &res));   // preallocateData (:83-93)
+  out->SetMembers(*res);
+  out->nulls = (vn == 0 && (sel == DropNulls || fn == 0)) ? 0 : kUnknownNullCount;  // :464-468
   if (values.len == 0) return Status::OK();
-  NATIVE(ag_filter_primitive_dev(bw, values.buffers[1].buf, vvalid, values.offset, filter.buffers[1].buf, mvalid, filter.offset, values.len, sel,
-                                 data->data(), allocate_validity ? valid->data() : nullptr, out_len, (int64_t*)scal->data() + 1, nullptr));
+  NATIVE(ag_filter_primitive_dev(BitWidth(values.type), values.buffers[1].buf, vvalid, values.offset, filter.buffers[1].buf, mvalid, filter.offset,
+                                 values.len, sel, out->buffers[1].buf, out->buffers[0].buf, out_len, (int64_t*)scal->data() + 1, nullptr));
   return Status::OK();
 }
 
@@ -1251,15 +1297,14 @@ Status CumulativeStart(const CumulativeOptions* opts, Type t, bool* has_start, u
 }
 
 struct CumsumRun {  // device state + error word shared by the chunks of one call
-  std::shared_ptr<Buffer> state, bad;
+  std::shared_ptr<Buffer> state;
+  ErrorWord bad;
   Status Init(Type t, const CumulativeOptions* opts) {
     bool has_start; uint8_t raw[8];
     RETURN_NOT_OK(CumulativeStart(opts, t, &has_start, raw));
     RETURN_NOT_OK(Buffer::Allocate(sizeof(ag_cumsum_state), &state));
-    RETURN_NOT_OK(Buffer::Allocate(8, &bad));
     NATIVE(ag_cumulative_sum_state_init_dev(state->data(), (int)t, has_start ? raw : nullptr, nullptr));
-    NATIVE(ag_error_word_reset_dev((int64_t*)bad->data(), nullptr));
-    return Status::OK();
+    return bad.Init();
   }
 };
 
@@ -1288,19 +1333,19 @@ Status CumulativeSpans(bool checked, const CumulativeOptions* opts, Type t, cons
     // preallocated PropagateNulls bitmaps) takes the no-nulls path like the reference (vector_cumulative.go:341-346)
     const uint8_t* in_valid = in.nulls != 0 ? in.buffers[0].buf : nullptr;
     NATIVE(ag_cumulative_sum_dev((int)t, ValuesPtr(in), in_valid, in.offset, in.len, opts && opts->SkipNulls ? 1 : 0, checked ? 1 : 0,
-                                 data->data() + pos * w, validity ? validity->data() : nullptr, pos, run.state->data(), (int64_t*)run.bad->data(), nullptr));
+                                 data->data() + pos * w, validity ? validity->data() : nullptr, pos, run.state->data(), run.bad.word(), nullptr));
     pos += in.len;
   }
   if (checked) {
     int64_t bad = 0;
-    RETURN_NOT_OK(run.bad->ToHost(&bad, 8));
+    RETURN_NOT_OK(run.bad.Read(&bad));
     if (bad != AG_NO_ERROR_POS) return Status::Invalid("overflow");  // errOverflow, base_arithmetic.go:137
   }
-  out->buffers[1].buf = data->data(); out->buffers[1].len = data->size(); out->buffers[1].owner = data;
+  SetBuffer(&out->buffers[1], data);
   if (validity) {
     ag_cumsum_state hs;
     RETURN_NOT_OK(run.state->ToHost(&hs, sizeof(hs)));
-    out->buffers[0].buf = validity->data(); out->buffers[0].len = validity->size(); out->buffers[0].owner = validity;
+    SetBuffer(&out->buffers[0], validity);
     out->nulls = hs.null_count;
   }
   return Status::OK();
@@ -1344,27 +1389,20 @@ Status PrimitiveTakeExec(KernelCtx* ctx, const ExecSpan& batch, ExecResult* out)
   int64_t vn = 0, in_ = 0;
   RETURN_NOT_OK(values.UpdateNullCount(&vn));
   RETURN_NOT_OK(indices.UpdateNullCount(&in_));
-  const int bw = BitWidth(values.type);
   const bool allocate_validity = vn != 0 || in_ != 0;  // :1175
-  out->type = values.type; out->len = indices.len; out->offset = 0;
-  std::shared_ptr<Buffer> data, valid, word;
-  RETURN_NOT_OK(ctx->Allocate(bw == 1 ? ((indices.len + 31) / 32) * 4 : indices.len * (bw / 8), &data));
-  out->buffers[1].buf = data->data(); out->buffers[1].len = data->size(); out->buffers[1].owner = data; out->buffers[1].self_alloc = true;
-  if (allocate_validity) {
-    RETURN_NOT_OK(ctx->Allocate(((indices.len + 31) / 32) * 4, &valid));
-    out->buffers[0].buf = valid->data(); out->buffers[0].len = valid->size(); out->buffers[0].owner = valid; out->buffers[0].self_alloc = true;
-  }
-  out->nulls = allocate_validity ? kUnknownNullCount : 0;
+  std::shared_ptr<ArrayData> res;
+  RETURN_NOT_OK(AllocateOutput(values.type, indices.len, allocate_validity, &res));
+  out->SetMembers(*res);
   if (indices.len == 0) return Status::OK();
-  RETURN_NOT_OK(Buffer::Allocate(8, &word));
-  NATIVE(ag_error_word_reset_dev((int64_t*)word->data(), nullptr));
+  ErrorWord word;
+  RETURN_NOT_OK(word.Init());
   const int iw = BitWidth(indices.type);
-  NATIVE(ag_take_primitive_dev(bw, values.buffers[1].buf, vn ? values.buffers[0].buf : nullptr, values.offset, values.len, iw, IsSignedInteger(indices.type),
-                               indices.buffers[1].buf + indices.offset * (iw / 8), in_ ? indices.buffers[0].buf : nullptr, indices.offset, indices.len,
-                               bounds ? 1 : 0, data->data(), allocate_validity ? valid->data() : nullptr, (int64_t*)word->data(), nullptr));
+  NATIVE(ag_take_primitive_dev(BitWidth(values.type), values.buffers[1].buf, vn ? values.buffers[0].buf : nullptr, values.offset, values.len, iw,
+                               IsSignedInteger(indices.type), indices.buffers[1].buf + indices.offset * (iw / 8), in_ ? indices.buffers[0].buf : nullptr,
+                               indices.offset, indices.len, bounds ? 1 : 0, out->buffers[1].buf, out->buffers[0].buf, word.word(), nullptr));
   if (bounds) {
     int64_t bad = 0;
-    RETURN_NOT_OK(word->ToHost(&bad, 8));
+    RETURN_NOT_OK(word.Read(&bad));
     if (bad != AG_NO_ERROR_POS) return IndexOutOfBounds(*indices.buffers[1].owner, indices.type, indices.offset, bad);
   }
   return Status::OK();
@@ -1759,21 +1797,16 @@ FunctionRegistry* GetFunctionRegistry() {
       if (args[1].kind == DatumKind::ARRAY) {
         Datum r;
         RETURN_NOT_OK(CallFunction(ctx, "array_take", opts, {values, args[1]}, &r));
-        if (!values_chunked) { *out = r; return Status::OK(); }
-        auto c = std::make_shared<ChunkedArray>();
-        c->type = r.array->type; c->chunks = {r.array}; c->length = r.array->length;
-        *out = Datum(c);
+        *out = values_chunked ? Datum(MakeChunked(r.array->type, {r.array})) : r;
         return Status::OK();
       }
-      auto c = std::make_shared<ChunkedArray>();
-      c->type = values.type();
+      std::vector<std::shared_ptr<ArrayData>> chunks;
       for (auto& chunk : args[1].chunked->chunks) {  // one array_take per index chunk (selection.go:221-234)
         Datum r;
         RETURN_NOT_OK(CallFunction(ctx, "array_take", opts, {values, Datum(chunk)}, &r));
-        c->chunks.push_back(r.array);
-        c->length += r.array->length;
+        chunks.push_back(r.array);
       }
-      *out = Datum(c);
+      *out = Datum(MakeChunked(values.type(), std::move(chunks)));
       return Status::OK();
     }), false);
   });
@@ -1862,44 +1895,36 @@ Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortOptions& op
 // the key columns go to the device as chunk lists, whatever their chunking.
 Status SortIndices(const ExecCtx& ctx, const Datum& input, const SortKeys& opts, Datum* out) {
   if (opts.Keys.empty()) return Status::Invalid("must provide at least one sort key");
-  std::vector<std::pair<Type, std::vector<std::shared_ptr<ArrayData>>>> cols;   // (type, chunks) per key
+  std::vector<Column> cols;   // one per key
   std::vector<SortKey> keys = opts.Keys;
-  int64_t n = 0;
   switch (input.kind) {
     case DatumKind::ARRAY:      // one column: the first key only, ColumnIndex ignored
-      cols.push_back({input.array->type, {input.array}});
-      keys.resize(1);
-      n = input.array->length;
-      break;
     case DatumKind::CHUNKED:
-      cols.push_back({input.chunked->type, input.chunked->chunks});
+      cols.push_back(Column{input.type(), ArrayChunks(input)});
       keys.resize(1);
-      n = input.chunked->length;
       break;
     case DatumKind::RECORD:
     case DatumKind::TABLE: {
-      const bool rec = input.kind == DatumKind::RECORD;
-      const int64_t ncols = rec ? (int64_t)input.record->columns.size() : (int64_t)input.table->columns.size();
+      const int ncols = NumColumns(input);
       for (size_t i = 0; i < keys.size(); ++i) {
         const int c = keys[i].ColumnIndex;
         if (c < 0 || c >= ncols) return Status::Invalid("sort key " + std::to_string(i) + " has invalid column index " + std::to_string(c));
-        if (rec) cols.push_back({input.record->columns[c]->type, {input.record->columns[c]}});
-        else cols.push_back({input.table->columns[c]->type, input.table->columns[c]->chunks});
+        cols.push_back(GetColumn(input, c));
       }
-      n = rec ? input.record->num_rows : input.table->num_rows;
       break;
     }
     default:
       return Status::NotImplemented("unsupported type for sort_indices operation");
   }
+  const int64_t n = input.Len();
   for (auto& c : cols)
-    if (c.first != Type::BOOL && !IsInteger(c.first) && !IsFloating(c.first))
-      return Status::NotImplemented(std::string("sorting not supported for type ") + TypeName(c.first));
+    if (c.type != Type::BOOL && !IsInteger(c.type) && !IsFloating(c.type))
+      return Status::NotImplemented(std::string("sorting not supported for type ") + TypeName(c.type));
   std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
   std::vector<ag_sort_key> desc(cols.size());
   for (size_t i = 0; i < cols.size(); ++i) {
-    chunks[i] = ChunkDescs(cols[i].second);
-    desc[i] = ag_sort_key{(int)cols[i].first, (int)keys[i].Order, (int)keys[i].Placement, (int)chunks[i].size(), chunks[i].data()};
+    chunks[i] = ChunkDescs(cols[i].chunks);
+    desc[i] = ag_sort_key{(int)cols[i].type, (int)keys[i].Order, (int)keys[i].Placement, (int)chunks[i].size(), chunks[i].data()};
   }
   std::shared_ptr<Buffer> idx;
   RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(n, 1) * 8, &idx));
@@ -1924,46 +1949,57 @@ Status SortIndicesTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table,
 namespace {
 bool SelectionType(Type t) { return t == Type::BOOL || IsNumeric(t); }
 
-// One column of a selection: its type and chunks (a record batch column is one chunk).
-struct SelColumn { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
-
-Status SelColumns(const Datum& values, std::vector<SelColumn>* cols, int64_t* nrows) {
-  if (values.kind == DatumKind::RECORD) {
-    for (auto& c : values.record->columns) cols->push_back(SelColumn{c->type, {c}});
-    *nrows = values.record->num_rows;
-  } else {
-    for (auto& c : values.table->columns) cols->push_back(SelColumn{c->type, c->chunks});
-    *nrows = values.table->num_rows;
-  }
-  for (size_t i = 0; i < cols->size(); ++i)
-    if (!SelectionType((*cols)[i].type))
-      return Status::NotImplemented("take: column " + std::to_string(i) + " has unsupported type " + TypeName((*cols)[i].type) +
+// The columns of a record batch or table; ErrNotImplemented for the first one of a type the gather does not take.
+Status SelColumns(const Datum& values, std::vector<Column>* cols) {
+  for (int i = 0; i < NumColumns(values); ++i) {
+    cols->push_back(GetColumn(values, i));
+    if (!SelectionType(cols->back().type))
+      return Status::NotImplemented("take: column " + std::to_string(i) + " has unsupported type " + TypeName(cols->back().type) +
                                     " (boolean and numeric columns only)");
+  }
   return Status::OK();
 }
 
-// The output of one column for `n` rows (preallocateData, vector_selection.go:83-93): values at offset 0, a validity
-// bitmap exactly when `nullable`.
-std::shared_ptr<ArrayData> SelOutput(Type t, int64_t n, bool nullable, Status* st) {
-  auto d = std::make_shared<ArrayData>();
-  d->type = t; d->length = n; d->offset = 0; d->null_count = nullable ? kUnknownNullCount : 0;
-  *st = Buffer::Allocate(t == Type::BOOL ? ((n + 31) / 32) * 4 : n * (BitWidth(t) / 8), &d->buffers[1]);
-  if (st->ok() && nullable) *st = Buffer::Allocate(((n + 31) / 32) * 4, &d->buffers[0]);
-  return d;
-}
-
-// One launch: gather rows [0, idx.length) of `idx` from every column.  `chunks[c]` are the chunks column c is read from
-// (their lengths sum to nrows); outs[c] receives the result.
-Status GatherColumns(const std::vector<SelColumn>& cols, const std::vector<std::vector<ag_sort_chunk>>& chunks, int64_t nrows, const ArrayData& idx,
-                     bool bounds, int64_t* d_bad, const std::vector<std::shared_ptr<ArrayData>>& outs) {
+// One ag_take_columns_dev launch: rows [0, idx.length) of `idx` from every column, read from `chunks[c]` (their lengths
+// sum to nrows), into a new output per column appended to (*res)[c].  An output has a validity bitmap when
+// `idx_nullable` or a chunk it reads may have nulls.  `d_bad`: the error word of a bounds-checked gather, reset here;
+// nullptr for no bounds check.
+Status GatherColumns(const std::vector<Column>& cols, const std::vector<std::vector<ag_sort_chunk>>& chunks, int64_t nrows, const ArrayData& idx,
+                     bool idx_nullable, int64_t* d_bad, std::vector<std::vector<std::shared_ptr<ArrayData>>>* res) {
   std::vector<ag_take_column> desc(cols.size());
-  for (size_t c = 0; c < cols.size(); ++c)
-    desc[c] = ag_take_column{(int)cols[c].type, (int)chunks[c].size(), chunks[c].data(), outs[c]->buffers[1]->data(),
-                             outs[c]->buffers[0] ? outs[c]->buffers[0]->data() : nullptr};
+  for (size_t c = 0; c < cols.size(); ++c) {
+    bool nullable = idx_nullable;
+    for (auto& ch : chunks[c]) nullable = nullable || ch.valid != nullptr;
+    std::shared_ptr<ArrayData> o;
+    RETURN_NOT_OK(AllocateOutput(cols[c].type, idx.length, nullable, &o));
+    (*res)[c].push_back(o);
+    desc[c] = ag_take_column{(int)cols[c].type, (int)chunks[c].size(), chunks[c].data(), o->buffers[1]->data(), o->buffers[0] ? o->buffers[0]->data() : nullptr};
+  }
+  if (d_bad) NATIVE(ag_error_word_reset_dev(d_bad, nullptr));
   const int iw = BitWidth(idx.type);
   const void* iptr = idx.buffers[1] ? idx.buffers[1]->data() + idx.offset * (iw / 8) : nullptr;
   NATIVE(ag_take_columns_dev((int)desc.size(), desc.data(), nrows, iw, IsSignedInteger(idx.type), iptr, ValidityOrNull(idx), idx.offset, idx.length,
-                             bounds ? 1 : 0, d_bad, nullptr));
+                             d_bad ? 1 : 0, d_bad, nullptr));
+  return Status::OK();
+}
+
+// The record batch (`kind` RECORD: the one output of each column) or table (each column's outputs as its chunks) of
+// `num_rows` rows that GatherColumns filled `res` for.
+Status MakeSelection(DatumKind kind, const std::vector<Column>& cols, const std::vector<std::vector<std::shared_ptr<ArrayData>>>& res, int64_t num_rows,
+                     Datum* out) {
+  if (kind == DatumKind::RECORD) {
+    std::vector<std::shared_ptr<ArrayData>> arrs;
+    for (auto& r : res) arrs.push_back(r[0]);
+    std::shared_ptr<RecordBatch> rb;
+    RETURN_NOT_OK(MakeRecordBatch(num_rows, std::move(arrs), &rb));
+    *out = Datum(rb);
+    return Status::OK();
+  }
+  std::vector<std::shared_ptr<ChunkedArray>> ccols;
+  for (size_t c = 0; c < cols.size(); ++c) ccols.push_back(MakeChunked(cols[c].type, res[c]));
+  std::shared_ptr<Table> tb;
+  RETURN_NOT_OK(MakeTable(num_rows, std::move(ccols), &tb));
+  *out = Datum(tb);
   return Status::OK();
 }
 
@@ -1971,20 +2007,17 @@ Status GatherColumns(const std::vector<SelColumn>& cols, const std::vector<std::
 // kernels/vector_selection.go:1194-1228): a record batch takes by the concatenated indices and gives arrays of
 // len(indices) rows; a table gives every column one chunk per index chunk (an array index: one chunk).
 Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Datum& indices, Datum* out) {
-  std::vector<SelColumn> cols;
-  int64_t nrows = 0;
-  RETURN_NOT_OK(SelColumns(values, &cols, &nrows));
+  std::vector<Column> cols;
+  RETURN_NOT_OK(SelColumns(values, &cols));
   const Type it = indices.type();
   if (!IsInteger(it)) return Status::Invalid("invalid index type for bounds checking");   // helpers.go:978
   std::vector<std::shared_ptr<ArrayData>> idx;
-  if (indices.kind == DatumKind::ARRAY) {
-    idx.push_back(indices.array);
-  } else if (values.kind == DatumKind::RECORD) {   // chunked indices are concatenated first (:163-171)
+  if (indices.kind == DatumKind::CHUNKED && values.kind == DatumKind::RECORD) {   // chunked indices are concatenated first (:163-171)
     std::shared_ptr<ArrayData> cat;
     RETURN_NOT_OK(ConcatenateChunks(*indices.chunked, &cat));
     idx.push_back(cat);
   } else {
-    idx = indices.chunked->chunks;
+    idx = ArrayChunks(indices);
   }
   std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
   for (size_t c = 0; c < cols.size(); ++c) chunks[c] = ChunkDescs(cols[c].chunks);
@@ -1995,17 +2028,8 @@ Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Dat
   std::vector<std::vector<std::shared_ptr<ArrayData>>> res(cols.size());
   // the reference takes column by column, so without columns nothing is gathered or bounds-checked
   const size_t launches = cols.empty() ? 0 : idx.size();
-  for (size_t k = 0; k < launches; ++k) {
-    std::vector<std::shared_ptr<ArrayData>> outs(cols.size());
-    for (size_t c = 0; c < cols.size(); ++c) {
-      Status st;
-      outs[c] = SelOutput(cols[c].type, idx[k]->length, idx_nullable || MayHaveNulls(cols[c].chunks), &st);
-      RETURN_NOT_OK(st);
-      res[c].push_back(outs[c]);
-    }
-    if (opts.BoundsCheck) NATIVE(ag_error_word_reset_dev(d_bad + k, nullptr));
-    RETURN_NOT_OK(GatherColumns(cols, chunks, nrows, *idx[k], opts.BoundsCheck, opts.BoundsCheck ? d_bad + k : nullptr, outs));
-  }
+  for (size_t k = 0; k < launches; ++k)
+    RETURN_NOT_OK(GatherColumns(cols, chunks, values.Len(), *idx[k], idx_nullable, opts.BoundsCheck ? d_bad + k : nullptr, &res));
   if (opts.BoundsCheck && launches > 0) {   // checkIndexBoundsChunked: the first offending row in index order
     std::vector<int64_t> bad(launches);
     RETURN_NOT_OK(words->ToHost(bad.data(), 8 * (int64_t)launches));
@@ -2014,24 +2038,8 @@ Status TakeRecordOrTable(const TakeOptions& opts, const Datum& values, const Dat
   }
   int64_t out_rows = 0;
   for (auto& a : idx) out_rows += a->length;
-  if (values.kind == DatumKind::RECORD) {
-    std::vector<std::shared_ptr<ArrayData>> arrs;
-    for (auto& r : res) arrs.push_back(r[0]);
-    std::shared_ptr<RecordBatch> rb;
-    RETURN_NOT_OK(MakeRecordBatch(out_rows, std::move(arrs), &rb));
-    *out = Datum(rb);
-    return Status::OK();
-  }
-  std::vector<std::shared_ptr<ChunkedArray>> ccols;
-  for (size_t c = 0; c < cols.size(); ++c) {
-    auto ch = std::make_shared<ChunkedArray>();
-    ch->type = cols[c].type; ch->chunks = res[c]; ch->length = out_rows;
-    ccols.push_back(ch);
-  }
-  std::shared_ptr<Table> tb;   // array.NewTable(schema, cols, -1): a table without columns has no rows
-  RETURN_NOT_OK(MakeTable(cols.empty() ? 0 : out_rows, std::move(ccols), &tb));
-  *out = Datum(tb);
-  return Status::OK();
+  // array.NewTable(schema, cols, -1): a table without columns has no rows
+  return MakeSelection(values.kind, cols, res, values.kind == DatumKind::TABLE && cols.empty() ? 0 : out_rows, out);
 }
 
 // GetTakeIndices (kernels/vector_selection.go:102-236) of each mask span, with one read-back for all their lengths:
@@ -2053,10 +2061,8 @@ Status MaskSpansToIndices(const std::vector<std::shared_ptr<ArrayData>>& masks, 
     const ArrayData& m = *masks[k];
     const int64_t len = h[2 * k];
     const bool nullable = sel == EmitNulls && MayHaveNulls(m);
-    auto d = std::make_shared<ArrayData>();
-    d->type = Type::UINT32; d->length = len; d->offset = 0; d->null_count = nullable ? kUnknownNullCount : 0;
-    RETURN_NOT_OK(Buffer::Allocate(len * 4, &d->buffers[1]));
-    if (nullable) RETURN_NOT_OK(Buffer::Allocate(((len + 31) / 32) * 4, &d->buffers[0]));
+    std::shared_ptr<ArrayData> d;
+    RETURN_NOT_OK(AllocateOutput(Type::UINT32, len, nullable, &d));
     if (len > 0)
       NATIVE(ag_take_indices_dev(32, m.buffers[1]->data(), ValidityOrNull(m), m.offset, m.length, (int)sel,
                                  d->buffers[1]->data(), nullable ? d->buffers[0]->data() : nullptr, len, d_len + 2 * k + 1, nullptr));
@@ -2088,15 +2094,14 @@ Status FilterTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, cons
   if (table->num_rows == 0) { *out = table; return Status::OK(); }
   if (filter.kind != DatumKind::ARRAY && filter.kind != DatumKind::CHUNKED) return Status::NotImplemented("filter should be array-like");
   if (filter.type() != Type::BOOL) return Status::NotImplemented("filter argument must be boolean type");
-  std::vector<SelColumn> cols;
-  int64_t nrows = 0;
-  RETURN_NOT_OK(SelColumns(Datum(table), &cols, &nrows));
-  const std::vector<std::shared_ptr<ArrayData>> fchunks = filter.kind == DatumKind::ARRAY ? std::vector<std::shared_ptr<ArrayData>>{filter.array} : filter.chunked->chunks;
-  std::vector<std::vector<int64_t>> lens(cols.size() + 1);
-  for (size_t c = 0; c < cols.size(); ++c) for (auto& a : cols[c].chunks) lens[c].push_back(a->length);
-  for (auto& a : fchunks) lens.back().push_back(a->length);
+  std::vector<Column> cols;
+  RETURN_NOT_OK(SelColumns(Datum(table), &cols));
+  const std::vector<std::shared_ptr<ArrayData>> fchunks = ArrayChunks(filter);
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> args;
+  for (auto& c : cols) args.push_back(c.chunks);
+  args.push_back(fchunks);
   std::vector<SpanPiece> pieces;
-  RETURN_NOT_OK(IterateExecSpans(lens, std::vector<bool>(lens.size(), true), INT64_MAX, &pieces));
+  RETURN_NOT_OK(ChunkSpans(args, std::vector<bool>(args.size(), true), INT64_MAX, &pieces));
   std::vector<std::shared_ptr<ArrayData>> masks;
   for (auto& p : pieces) masks.push_back(fchunks[p.chunk_index.back()]->Slice(p.chunk_pos.back(), p.len));
   std::vector<std::shared_ptr<ArrayData>> idx;
@@ -2107,25 +2112,14 @@ Status FilterTable(const ExecCtx& ctx, const std::shared_ptr<Table>& table, cons
     if (idx[k]->length == 0) continue;
     const SpanPiece& p = pieces[k];
     std::vector<std::vector<ag_sort_chunk>> chunks(cols.size());
-    std::vector<std::shared_ptr<ArrayData>> outs(cols.size());
-    for (size_t c = 0; c < cols.size(); ++c) {
-      const auto& src = cols[c].chunks[p.chunk_index[c]];
-      chunks[c] = ChunkDescs({src->Slice(p.chunk_pos[c], p.len)});
-      Status st;
-      outs[c] = SelOutput(cols[c].type, idx[k]->length, MayHaveNulls(*idx[k]) || MayHaveNulls(*src), &st);
-      RETURN_NOT_OK(st);
-      res[c].push_back(outs[c]);
-    }
-    RETURN_NOT_OK(GatherColumns(cols, chunks, p.len, *idx[k], false, nullptr, outs));
+    for (size_t c = 0; c < cols.size(); ++c) chunks[c] = {ChunkDesc(*cols[c].chunks[p.chunk_index[c]], p.chunk_pos[c], p.len)};
+    RETURN_NOT_OK(GatherColumns(cols, chunks, p.len, *idx[k], MayHaveNulls(*idx[k]), nullptr, &res));
     out_rows += idx[k]->length;
   }
-  std::vector<std::shared_ptr<ChunkedArray>> ccols;
-  for (size_t c = 0; c < cols.size(); ++c) {
-    auto ch = std::make_shared<ChunkedArray>();
-    ch->type = cols[c].type; ch->chunks = res[c]; ch->length = out_rows;
-    ccols.push_back(ch);
-  }
-  return MakeTable(out_rows, std::move(ccols), out);
+  Datum r;
+  RETURN_NOT_OK(MakeSelection(DatumKind::TABLE, cols, res, out_rows, &r));
+  *out = r.table;
+  return Status::OK();
 }
 
 // compute.Sort (vector_sort.go:65-81): sort_indices by `keys`, then take with default TakeOptions.  A chunked array is
@@ -2150,7 +2144,7 @@ Status Unique(const ExecCtx& ctx, const Datum& values, Datum* out) {
   const bool has_valid = a->buffers[0] && a->null_count != 0;
   std::shared_ptr<Buffer> data, valid, len;
   RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(a->length, 1) * (bw / 8), &data));
-  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(((a->length + 31) / 32) * 4 + 4, &valid));
+  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(a->length) + 4, &valid));
   RETURN_NOT_OK(Buffer::Allocate(16, &len));
   NATIVE(ag_unique_dev(bw, a->buffers[1] ? a->buffers[1]->data() : nullptr, has_valid ? a->buffers[0]->data() : nullptr, a->offset, a->length, data->data(),
                        has_valid ? valid->data() : nullptr, a->length, (int64_t*)len->data(), nullptr));
@@ -2167,7 +2161,7 @@ Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts,
   const Type t = values.type();
   const int bw = BitWidth(t);
   if (bw != 8 && bw != 16 && bw != 32 && bw != 64) return Status::NotImplemented(std::string("dictionary_encode: unsupported type ") + TypeName(t));
-  const std::vector<std::shared_ptr<ArrayData>> in = values.kind == DatumKind::ARRAY ? std::vector<std::shared_ptr<ArrayData>>{values.array} : values.chunked->chunks;
+  const std::vector<std::shared_ptr<ArrayData>> in = ArrayChunks(values);
   const bool encode = opts.NullEncoding == NullEncodingEncode;
   int64_t total = 0;
   for (auto& a : in) total += a->length;
@@ -2180,7 +2174,7 @@ Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts,
     const bool has_valid = a.buffers[0] && a.null_count != 0;
     any_valid |= has_valid;
     RETURN_NOT_OK(Buffer::Allocate(std::max<int64_t>(a.length, 1) * 4, &idx[c]));
-    if (has_valid && !encode) RETURN_NOT_OK(Buffer::Allocate(((a.length + 31) / 32) * 4, &idx_valid[c]));
+    if (has_valid && !encode) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(a.length), &idx_valid[c]));
     desc[c] = ag_dict_chunk{a.buffers[1] ? a.buffers[1]->data() : nullptr, has_valid ? a.buffers[0]->data() : nullptr, a.offset, a.length,
                             (int32_t*)idx[c]->data(), idx_valid[c] ? idx_valid[c]->data() : nullptr};
   }
@@ -2211,9 +2205,10 @@ Status DictionaryEncode(const ExecCtx& ctx, const DictionaryEncodeOptions& opts,
     return d;
   };
   if (values.kind == DatumKind::ARRAY) { *out = Datum(make(0)); return Status::OK(); }
-  auto res = std::make_shared<ChunkedArray>();
-  res->type = Type::DICTIONARY; res->value_type = t; res->length = total;
-  for (size_t c = 0; c < in.size(); ++c) if (in[c]->length > 0) res->chunks.push_back(make(c));   // WrapResults drops empty chunks
+  std::vector<std::shared_ptr<ArrayData>> chunks;
+  for (size_t c = 0; c < in.size(); ++c) if (in[c]->length > 0) chunks.push_back(make(c));   // WrapResults drops empty chunks
+  auto res = MakeChunked(Type::DICTIONARY, std::move(chunks));
+  res->value_type = t;
   *out = Datum(res);
   return Status::OK();
 }
@@ -2227,7 +2222,7 @@ Status IsIn(const ExecCtx& ctx, const SetLookupOptions& opts, const Datum& value
   if (bw != 8 && bw != 16 && bw != 32 && bw != 64) return Status::Invalid(std::string("unsupported type ") + TypeName(a->type) + " for is_in function");
   const ArrayData& s = *opts.ValueSet;
   std::shared_ptr<Buffer> data, valid, cnt;
-  const int64_t bm = ((a->length + 31) / 32) * 4 + 4;
+  const int64_t bm = BitmapWordBytes(a->length) + 4;
   RETURN_NOT_OK(Buffer::Allocate(bm, &data));
   RETURN_NOT_OK(Buffer::Allocate(bm, &valid));
   RETURN_NOT_OK(Buffer::Allocate(8, &cnt));
@@ -2244,18 +2239,15 @@ namespace {
 // The arrays a chunkwise vector kernel runs on: the executor's spans of one argument (iterateExecSpans), so a chunked
 // input loses its empty chunks and a chunked input without rows gives one empty span (nullptr when it has no chunks).
 Status ChunkwiseSpans(const Datum& values, std::vector<std::shared_ptr<ArrayData>>* spans) {
-  if (values.kind == DatumKind::ARRAY) { spans->push_back(values.array); return Status::OK(); }
-  std::vector<std::vector<int64_t>> lens(1);
-  for (auto& c : values.chunked->chunks) lens[0].push_back(c->length);
+  const std::vector<std::shared_ptr<ArrayData>> chunks = ArrayChunks(values);
   std::vector<SpanPiece> pieces;
-  RETURN_NOT_OK(IterateExecSpans(lens, {true}, INT64_MAX, &pieces));
-  for (auto& p : pieces) spans->push_back(values.chunked->chunks[p.chunk_index[0]]->Slice(p.chunk_pos[0], p.len));
-  if (pieces.empty()) spans->push_back(values.chunked->chunks.empty() ? nullptr : values.chunked->chunks[0]->Slice(0, 0));
+  RETURN_NOT_OK(ChunkSpans({chunks}, {true}, INT64_MAX, &pieces));
+  for (auto& p : pieces) spans->push_back(chunks[p.chunk_index[0]]->Slice(p.chunk_pos[0], p.len));
+  if (pieces.empty()) spans->push_back(chunks.empty() ? nullptr : chunks[0]->Slice(0, 0));
   return Status::OK();
 }
 int64_t RunEndMax(Type t) { return t == Type::INT16 ? INT16_MAX : (t == Type::INT32 ? INT32_MAX : INT64_MAX); }
 const void* ElementPtr(const ArrayData& a) { return a.buffers[1] ? a.buffers[1]->data() + a.offset * (BitWidth(a.type) / 8) : nullptr; }
-int64_t BitmapWordBytes(int64_t nbits) { return ((nbits + 31) / 32) * 4; }
 
 // CountNumberOfRuns, one 16-byte read-back, exact allocation, WriteEncodedRuns (vector_run_end_encode.go:531-565)
 Status EncodeOne(Type rt, const ArrayData& a, std::shared_ptr<ArrayData>* out) {
@@ -2269,13 +2261,10 @@ Status EncodeOne(Type rt, const ArrayData& a, std::shared_ptr<ArrayData>* out) {
   int64_t cnt[2] = {0, 0};
   RETURN_NOT_OK(counts->ToHost(cnt, 16));
   const int64_t runs = cnt[0];
-  auto re = std::make_shared<ArrayData>();
-  re->type = rt; re->length = runs;
-  RETURN_NOT_OK(Buffer::Allocate(runs * (BitWidth(rt) / 8), &re->buffers[1]));
-  auto v = std::make_shared<ArrayData>();
-  v->type = t; v->length = runs; v->null_count = has_valid ? cnt[1] : 0;
-  RETURN_NOT_OK(Buffer::Allocate(t == Type::BOOL ? BitmapWordBytes(runs) : runs * (BitWidth(t) / 8), &v->buffers[1]));
-  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(runs), &v->buffers[0]));
+  std::shared_ptr<ArrayData> re, v;
+  RETURN_NOT_OK(AllocateOutput(rt, runs, false, &re));
+  RETURN_NOT_OK(AllocateOutput(t, runs, has_valid, &v));
+  v->null_count = has_valid ? cnt[1] : 0;
   NATIVE(ag_run_end_encode_dev((int)t, (int)rt, vals, valid, a.offset, a.length, re->buffers[1]->data(), v->buffers[1]->data(),
                                has_valid ? v->buffers[0]->data() : nullptr, runs, (int64_t*)counts->data(), nullptr));
   NATIVE(ag_stream_sync(nullptr));
@@ -2292,10 +2281,8 @@ Status DecodeOne(const ArrayData& a, std::shared_ptr<ArrayData>* out) {
   if (v.length < re.length) return Status::Invalid("run_end_decode: the values child is shorter than run_ends");
   const Type t = v.type;
   const bool has_valid = v.buffers[0] != nullptr;
-  auto d = std::make_shared<ArrayData>();
-  d->type = t; d->length = a.length;
-  RETURN_NOT_OK(Buffer::Allocate(t == Type::BOOL ? BitmapWordBytes(a.length) : a.length * (BitWidth(t) / 8), &d->buffers[1]));
-  if (has_valid) RETURN_NOT_OK(Buffer::Allocate(BitmapWordBytes(a.length), &d->buffers[0]));
+  std::shared_ptr<ArrayData> d;
+  RETURN_NOT_OK(AllocateOutput(t, a.length, has_valid, &d));
   std::shared_ptr<Buffer> words;   // [0] null count, [1] error word
   RETURN_NOT_OK(Buffer::Allocate(16, &words));
   int64_t* w = (int64_t*)words->data();
@@ -2308,7 +2295,6 @@ Status DecodeOne(const ArrayData& a, std::shared_ptr<ArrayData>* out) {
   if (h[1] != AG_NO_ERROR_POS)
     return Status::Invalid("run_end_decode: malformed run ends at run " + std::to_string(h[1]) + " (they must increase strictly and reach offset+length)");
   d->null_count = has_valid ? h[0] : 0;
-  if (!has_valid) d->buffers[0] = nullptr;
   *out = d;
   return Status::OK();
 }
@@ -2334,9 +2320,8 @@ Status RunEndEncode(const ExecCtx& ctx, const RunEndEncodeOptions& opts, const D
     res.push_back(r);
   }
   if (values.kind == DatumKind::ARRAY) { *out = Datum(res[0]); return Status::OK(); }
-  auto c = std::make_shared<ChunkedArray>();
-  c->type = Type::RUN_END_ENCODED; c->value_type = t; c->run_end_type = rt; c->chunks = res;
-  for (auto& r : res) c->length += r->length;
+  auto c = MakeChunked(Type::RUN_END_ENCODED, std::move(res));
+  c->value_type = t; c->run_end_type = rt;
   *out = Datum(c);
   return Status::OK();
 }
@@ -2358,10 +2343,7 @@ Status RunEndDecode(const ExecCtx& ctx, const Datum& values, Datum* out) {
     res.push_back(r);
   }
   if (values.kind == DatumKind::ARRAY) { *out = Datum(res[0]); return Status::OK(); }
-  auto c = std::make_shared<ChunkedArray>();
-  c->type = values.chunked->value_type; c->chunks = res;
-  for (auto& r : res) c->length += r->length;
-  *out = Datum(c);
+  *out = Datum(MakeChunked(values.chunked->value_type, std::move(res)));
   return Status::OK();
 }
 
@@ -2403,10 +2385,10 @@ Status EvalNodeByNode(const ExecCtx& ctx, const Expression& e, const Datum& inpu
       *out = Datum(e.literal);
       return Status::OK();
     case Expression::Kind::FIELD: {
-      const int n = input.kind == DatumKind::RECORD ? (int)input.record->columns.size() : (int)input.table->columns.size();
+      const int n = NumColumns(input);
       if (e.field < 0 || e.field >= n)
         return Status::Invalid("field index " + std::to_string(e.field) + " out of range: the input has " + std::to_string(n) + " columns");
-      *out = input.kind == DatumKind::RECORD ? Datum(input.record->columns[e.field]) : Datum(input.table->columns[e.field]);
+      *out = ColumnDatum(input, e.field);
       return Status::OK();
     }
     case Expression::Kind::CALL: {
@@ -2425,10 +2407,8 @@ Status EvalNodeByNode(const ExecCtx& ctx, const Expression& e, const Datum& inpu
   return Status::NotImplemented("unknown expression kind");
 }
 
-// An input column of a fused program: its chunks (one for a record batch column or an intermediate result).
-struct ExprColumn { Type type; std::vector<std::shared_ptr<ArrayData>> chunks; };
-
-// A bound node: a column of `cols`, a literal, or a program op over bound arguments.
+// A bound node: a column of `cols` (an input column, an is_in result or an intermediate result), a literal, or a program op
+// over bound arguments.
 struct BNode {
   enum Kind { COL, LIT, OP } kind = LIT;
   int col = -1;
@@ -2445,7 +2425,7 @@ bool IsNullLiteral(const BPtr& n) { return n->kind == BNode::LIT && !n->lit->val
 struct Binder {
   const ExecCtx& ctx;
   const Datum& input;
-  std::vector<ExprColumn>* cols;
+  std::vector<Column>* cols;
   std::map<int, int> field_col;   // field index -> its column in `cols`: a field named twice is read once
 
   BPtr Leaf(int c) { auto n = std::make_shared<BNode>(); n->kind = BNode::COL; n->col = c; n->out = (*cols)[c].type; return n; }
@@ -2481,13 +2461,10 @@ struct Binder {
       return true;
     }
     if (e.kind == Expression::Kind::FIELD) {
-      const int n = input.kind == DatumKind::RECORD ? (int)input.record->columns.size() : (int)input.table->columns.size();
-      if (e.field < 0 || e.field >= n) return false;
+      if (e.field < 0 || e.field >= NumColumns(input)) return false;
       const auto seen = field_col.find(e.field);
       if (seen != field_col.end()) { *out = Leaf(seen->second); return true; }
-      ExprColumn c;
-      if (input.kind == DatumKind::RECORD) { c.type = input.record->columns[e.field]->type; c.chunks = {input.record->columns[e.field]}; }
-      else { c.type = input.table->columns[e.field]->type; c.chunks = input.table->columns[e.field]->chunks; }
+      Column c = GetColumn(input, e.field);
       if (!ValueType(c.type)) return false;
       cols->push_back(std::move(c));
       field_col[e.field] = (int)cols->size() - 1;
@@ -2498,13 +2475,8 @@ struct Binder {
     bool all_literal = true;
     if (e.name == "is_in") {   // a meta function here: CallFunction runs it and its result is a column of the program
       Datum r;
-      if (!EvalNodeByNode(ctx, e, input, &r).ok()) return false;
-      ExprColumn c;
-      c.type = r.type();
-      if (r.kind == DatumKind::ARRAY) c.chunks = {r.array};
-      else if (r.kind == DatumKind::CHUNKED) c.chunks = r.chunked->chunks;
-      else return false;
-      cols->push_back(std::move(c));
+      if (!EvalNodeByNode(ctx, e, input, &r).ok() || (r.kind != DatumKind::ARRAY && r.kind != DatumKind::CHUNKED)) return false;
+      cols->push_back(Column{r.type(), ArrayChunks(r)});
       *out = Leaf((int)cols->size() - 1);
       return true;
     }
@@ -2608,7 +2580,7 @@ struct Emitter {
 
 // One program over the rows of `cols`: spans from iterateExecSpans over the chunk layouts of the columns it reads,
 // one ag_eval_program_dev launch, the output as one array.  *failed: some op of the program failed.
-Status RunProgram(const BPtr& root, const std::vector<ExprColumn>& cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
+Status RunProgram(const BPtr& root, const std::vector<Column>& cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
   Emitter em;
   for (int r = AG_EXPR_MAX_REGS - 1; r >= 0; --r) em.free_regs.push_back(r);
   ag_expr_program prog{};
@@ -2616,47 +2588,37 @@ Status RunProgram(const BPtr& root, const std::vector<ExprColumn>& cols, int64_t
   prog.n_instr = (int)em.ins.size();
   prog.instr = em.ins.data();
   std::vector<int32_t> col_types;
-  std::vector<std::vector<int64_t>> lens;
+  std::vector<std::vector<std::shared_ptr<ArrayData>>> chunks;
   for (int c : em.col_slot) {
     col_types.push_back((int32_t)cols[c].type);
-    std::vector<int64_t> l;
-    for (auto& ch : cols[c].chunks) l.push_back(ch->length);
-    lens.push_back(l);
+    chunks.push_back(cols[c].chunks);
   }
   prog.n_cols = (int)col_types.size();
   prog.col_types = col_types.data();
   std::vector<SpanPiece> pieces;
-  RETURN_NOT_OK(IterateExecSpans(lens, std::vector<bool>(lens.size(), true), INT64_MAX, &pieces));
+  RETURN_NOT_OK(ChunkSpans(chunks, std::vector<bool>(chunks.size(), true), INT64_MAX, &pieces));
   std::vector<ag_sort_chunk> spans;
   int64_t n_spans = 0;
   for (auto& p : pieces) {
     if (p.len == 0) continue;
-    for (size_t j = 0; j < em.col_slot.size(); ++j) {
-      const ArrayData& a = *cols[em.col_slot[j]].chunks[p.chunk_index[j]];
-      spans.push_back(ag_sort_chunk{a.buffers[1] ? a.buffers[1]->data() : nullptr, ValidityOrNull(a), a.offset + p.chunk_pos[j], p.len});
-    }
+    for (size_t j = 0; j < chunks.size(); ++j) spans.push_back(ChunkDesc(*chunks[j][p.chunk_index[j]], p.chunk_pos[j], p.len));
     ++n_spans;
   }
-  const Type out_type = root->out;
-  std::shared_ptr<Buffer> data, valid, word;
-  RETURN_NOT_OK(Buffer::Allocate(out_type == Type::BOOL ? ((nrows + 31) / 32) * 4 : nrows * (BitWidth(out_type) / 8), &data));
-  RETURN_NOT_OK(Buffer::Allocate(((nrows + 31) / 32) * 4, &valid));
-  RETURN_NOT_OK(Buffer::Allocate(8, &word));
-  NATIVE(ag_error_word_reset_dev((int64_t*)word->data(), nullptr));
-  NATIVE(ag_eval_program_dev(&prog, n_spans, spans.data(), data->data(), valid->data(), (int64_t*)word->data(), nullptr));
+  std::shared_ptr<ArrayData> a;
+  RETURN_NOT_OK(AllocateOutput(root->out, nrows, true, &a));
+  ErrorWord word;
+  RETURN_NOT_OK(word.Init());
+  NATIVE(ag_eval_program_dev(&prog, n_spans, spans.data(), a->buffers[1]->data(), a->buffers[0]->data(), word.word(), nullptr));
   int64_t bad = AG_NO_ERROR_POS;
-  RETURN_NOT_OK(word->ToHost(&bad, 8));
+  RETURN_NOT_OK(word.Read(&bad));
   *failed = bad != AG_NO_ERROR_POS;
-  auto a = std::make_shared<ArrayData>();
-  a->type = out_type; a->length = nrows; a->offset = 0; a->null_count = kUnknownNullCount;
-  a->buffers[0] = valid; a->buffers[1] = data;
   *out = a;
   return Status::OK();
 }
 
 // A tree that needs more registers, columns or instructions than one program holds: its largest subtree that does not
 // fit is evaluated first, as programs of its own, and enters the rest as a column.
-Status RunFused(BPtr root, std::vector<ExprColumn>* cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
+Status RunFused(BPtr root, std::vector<Column>* cols, int64_t nrows, std::shared_ptr<ArrayData>* out, bool* failed) {
   while (!Fits(Measure(root))) {
     // descend into an argument that does not fit; below a node whose arguments all fit, take its largest argument
     BPtr* slot = &root;
@@ -2676,7 +2638,7 @@ Status RunFused(BPtr root, std::vector<ExprColumn>* cols, int64_t nrows, std::sh
     std::shared_ptr<ArrayData> part;
     RETURN_NOT_OK(RunProgram(*slot, *cols, nrows, &part, failed));
     if (*failed) return Status::OK();
-    cols->push_back(ExprColumn{part->type, {part}});
+    cols->push_back(Column{part->type, {part}});
     auto leaf = std::make_shared<BNode>();
     leaf->kind = BNode::COL; leaf->col = (int)cols->size() - 1; leaf->out = part->type;
     *slot = leaf;
@@ -2689,7 +2651,7 @@ Status RunFused(BPtr root, std::vector<ExprColumn>* cols, int64_t nrows, std::sh
 Status ExecuteScalarExpression(const ExecCtx& ctx, const Expression& expr, const Datum& input, Datum* out) {
   if (input.kind != DatumKind::RECORD && input.kind != DatumKind::TABLE)
     return Status::Invalid("ExecuteScalarExpression takes a record batch or a table");
-  std::vector<ExprColumn> cols;
+  std::vector<Column> cols;
   Binder b{ctx, input, &cols, {}};
   BPtr root;
   if (!b.Bind(expr, &root) || root->kind != BNode::OP) return EvalNodeByNode(ctx, expr, input, out);
@@ -2697,10 +2659,7 @@ Status ExecuteScalarExpression(const ExecCtx& ctx, const Expression& expr, const
   bool failed = false;
   RETURN_NOT_OK(RunFused(root, &cols, input.Len(), &res, &failed));
   if (failed) return EvalNodeByNode(ctx, expr, input, out);   // its status, message included
-  if (input.kind == DatumKind::RECORD) { *out = Datum(res); return Status::OK(); }
-  auto c = std::make_shared<ChunkedArray>();
-  c->type = res->type; c->length = res->length; c->chunks = {res};
-  *out = Datum(c);
+  *out = input.kind == DatumKind::RECORD ? Datum(res) : Datum(MakeChunked(res->type, {res}));
   return Status::OK();
 }
 

@@ -131,6 +131,24 @@ def page_table(pages):
     return arr
 
 
+# include/arrowgpu.h AG_PQ_RLE_* (page encoders: stream form, input kind)
+PQ_RLE_BARE, PQ_RLE_LEN4, PQ_RLE_WIDTH = 0, 1, 2
+PQ_RLE_IN_U32, PQ_RLE_IN_I16, PQ_RLE_IN_BITMAP = 0, 1, 2
+
+
+class PqEncPage(C.Structure):
+    """ag_pq_enc_page: one page of a batched encode (input element offset, values, output byte offset, capacity)."""
+    _fields_ = [("in_", C.c_int64), ("num_values", C.c_int64), ("out", C.c_int64), ("capacity", C.c_int64)]
+
+
+def enc_page_table(pages):
+    """[(in, num_values, out, capacity), ...] -> ctypes array of ag_pq_enc_page."""
+    arr = (PqEncPage * max(len(pages), 1))()
+    for k, (i, nv, o, cap) in enumerate(pages):
+        arr[k].in_, arr[k].num_values, arr[k].out, arr[k].capacity = i, nv, o, cap
+    return arr
+
+
 class PqCompressed(C.Structure):
     """ag_pq_compressed: one compressed Parquet page of a batched decompression (byte offsets and lengths)."""
     _fields_ = [("src", C.c_int64), ("src_len", C.c_int64), ("dst", C.c_int64), ("dst_len", C.c_int64)]
@@ -307,6 +325,12 @@ _SIGS = {
     "ag_parquet_bool_decode_dev": [_i, _p, _p, _i64, _p, _p, _p, _p],
     "ag_parquet_fixed_decode": [_i, _i, _i, _p, _p, _i64, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_fixed_decode_dev": [_i, _i, _i, _p, _p, _i64, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_rle_max_size": [_i, _i, _i64, _pi64],
+    "ag_parquet_rle_encode": [_i, _i, _i, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_rle_encode_dev": [_i, _i, _i, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_delta_max_size": [_i, _i, _i, _i64, _pi64],
+    "ag_parquet_delta_encode": [_i, _i, _i, _p, _p, _i64, _p, _p],
+    "ag_parquet_delta_encode_dev": [_i, _i, _i, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_zstd_decompress": [_p, _p, _i64, _p, _p],

@@ -913,6 +913,67 @@ ag_status ag_parquet_delta_decode_dev(int value_width, const uint8_t* d_data, co
                                       const uint8_t* d_valid, void* d_out, int64_t* d_decoded, ag_stream_t s);
 
 /* ================================================================================= *
+ * Page encoders: the value sections of data pages, as arrow-go's writer produces them, from device-resident values.
+ *   Batch-of-pages calls in the shape of the decoders: `pages` is a HOST array in both flavours,
+ *     in          element offset of the page's first value in `values` (bit offset for bitmap input)
+ *     num_values  values to encode, 0 .. 2^31-1
+ *     out         byte offset of the page's section in `out`
+ *     capacity    bytes available there: at least the call's *_max_size bound for num_values (AG_ERR_INVALID
+ *                 naming the page otherwise, before any launch)
+ *   Pages may come in any order, share or skip input, and their sections need not be contiguous.  lengths[i] (may be
+ *   NULL) receives the bytes page i wrote, prefix included.  Inputs are dense: dictionary indices and DELTA values are
+ *   the valid values in order (compact a spaced column with ag_filter_primitive_dev and its validity as the mask).
+ *   The device flavours synchronise `s` once (d_lengths and *d_bad_pos are device memory); host flavours stage the
+ *   input the pages reach and copy back each page's written bytes.  Without a usable GPU every entry point returns
+ *   AG_ERR_CUDA.
+ *
+ *   ag_parquet_rle_encode: the RLE/bit-packed hybrid stream of RleEncoder.Put / Flush (parquet/internal/utils/
+ *     rle.go:314-445), byte for byte: repeated runs of >= 8 caught on the group alignment, literal runs of at most
+ *     63 groups, a zero-padded last group.  Used by LevelEncoder (encoding/levels.go:77-169), dictEncoder.WriteIndices
+ *     (encoding/encoder.go:293-302) and RleBooleanEncoder (encoding/boolean_encoder.go:185-).
+ *     form  AG_PQ_RLE_BARE  the stream alone                        (data page v2 levels)
+ *           AG_PQ_RLE_LEN4  4-byte little-endian length, the stream  (data page v1 levels, BOOLEAN RLE pages)
+ *           AG_PQ_RLE_WIDTH 1 bit-width byte, the stream             (RLE_DICTIONARY / PLAIN_DICTIONARY data pages)
+ *     input AG_PQ_RLE_IN_U32    uint32 dictionary indices, bit width 0..32
+ *           AG_PQ_RLE_IN_I16    int16 levels, bit width 0..16
+ *           AG_PQ_RLE_IN_BITMAP bits, bit width 1: definition levels of a flat optional column from its validity
+ *                               bitmap, or BOOLEAN values
+ *     A value wider than the bit width (a negative level included) is AG_ERR_INVALID naming the page, with the lowest
+ *     offending element offset (into `values`) in *bad_pos; *bad_pos is AG_NO_ERROR_POS otherwise (may be NULL).  The
+ *     reference's BitWriter.WriteValue does not mask and corrupts the neighbouring values (utils/bit_writer.go:115-130).
+ *   ag_parquet_rle_max_size: MaxRLEBufferSize + MinRLEBufferSize (rle.go:36-51) plus the form's prefix.
+ *   ag_parquet_delta_encode: deltaBitPackEncoder.Put / FlushValues (encoding/delta_bit_packing.go:338,362-494), byte
+ *     for byte, with the block shape as a parameter (the reference fixes 128 values in 4 miniblocks; pyarrow writes
+ *     INT64 pages with 256/4).  value_width 4 (INT32) or 8 (INT64), `values` aligned to it; deltas wrap at that
+ *     width; the width bytes of absent miniblocks of the last block are 0 and the last miniblock is padded with zeros.
+ *     A block size that is not a positive multiple of 128, a miniblock count that does not divide it, or values per
+ *     miniblock that are not a multiple of 32 is AG_ERR_INVALID (the shapes deltaBitPackDecoder.SetData refuses).
+ *   ag_parquet_delta_max_size: 40 header bytes, then per block of deltas 10 + miniblocks + block_size * value_width.
+ * ================================================================================= */
+typedef struct ag_pq_enc_page {
+  int64_t in;
+  int64_t num_values;
+  int64_t out;
+  int64_t capacity;
+} ag_pq_enc_page;
+#define AG_PQ_RLE_BARE      0
+#define AG_PQ_RLE_LEN4      1
+#define AG_PQ_RLE_WIDTH     2
+#define AG_PQ_RLE_IN_U32    0
+#define AG_PQ_RLE_IN_I16    1
+#define AG_PQ_RLE_IN_BITMAP 2
+ag_status ag_parquet_rle_max_size(int bit_width, int form, int64_t num_values, int64_t* size);
+ag_status ag_parquet_rle_encode(int bit_width, int form, int input, const void* values, const ag_pq_enc_page* pages,
+                                int64_t n_pages, uint8_t* out, int64_t* lengths, int64_t* bad_pos);
+ag_status ag_parquet_rle_encode_dev(int bit_width, int form, int input, const void* d_values, const ag_pq_enc_page* pages,
+                                    int64_t n_pages, uint8_t* d_out, int64_t* d_lengths, int64_t* d_bad_pos, ag_stream_t s);
+ag_status ag_parquet_delta_max_size(int value_width, int block_size, int miniblocks, int64_t num_values, int64_t* size);
+ag_status ag_parquet_delta_encode(int value_width, int block_size, int miniblocks, const void* values, const ag_pq_enc_page* pages,
+                                  int64_t n_pages, uint8_t* out, int64_t* lengths);
+ag_status ag_parquet_delta_encode_dev(int value_width, int block_size, int miniblocks, const void* d_values, const ag_pq_enc_page* pages,
+                                      int64_t n_pages, uint8_t* d_out, int64_t* d_lengths, ag_stream_t s);
+
+/* ================================================================================= *
  * BYTE_ARRAY pages into an Arrow Binary / String (offset_width 4, int32 offsets) or LargeBinary / LargeString
  *   (offset_width 8) array: `offsets` plus one data buffer, as arrow-go's byteArrayRecordReader builds with
  *   array.BinaryBuilder (parquet/file/record_reader.go:902-1030).  The same batch-of-pages contract as

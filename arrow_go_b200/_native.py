@@ -339,6 +339,9 @@ _SIGS = {
     "ag_parquet_gzip_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_lz4_raw_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_lz4_raw_decompress_dev": [_p, _p, _i64, _p, _p, _p],
+    "ag_parquet_snappy_max_size": [_i64, _pi64],
+    "ag_parquet_snappy_compress": [_p, _p, _i64, _p, _p],
+    "ag_parquet_snappy_compress_dev": [_p, _p, _i64, _p, _p, _p],
     # parity helpers
     "ag_checksum64_dev": [_p, _sz, _p, _p],
     "ag_generate_dev": [_i, _u64, _i64, _i64, _p, _sz, _p],

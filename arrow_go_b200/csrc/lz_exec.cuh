@@ -1,6 +1,7 @@
 // lz_exec.cuh — what the Parquet page decompressors (snappy.cu, zstd.cu, gzip.cu, lz4.cu) share.  Internal, not part of
 // the ABI.
 //
+//   pq_dst_overlap_check  overlapping dst ranges of an ag_pq_compressed batch (the SNAPPY compressor checks it too)
 //   pq_compressed_check   the argument checks of an ag_pq_compressed batch, AG_ERR_INVALID before any launch
 //   pq_decompress_dev     the device flavour: the checks, then the codec
 //   pq_decompress_host    the host flavour: the checks, stage src, run the codec, copy back only written bytes
@@ -21,6 +22,23 @@
 
 namespace ag {
 
+// AG_ERR_INVALID naming the two lowest pages whose [dst, dst + dst_len) ranges overlap (empty ranges overlap nothing).
+// Shared with the compressor (snappy_encode.cu), where dst_len is the capacity.
+static inline ag_status pq_dst_overlap_check(const char* fn, const ag_pq_compressed* pages, int64_t n_pages) {
+  std::vector<int64_t> order;
+  for (int64_t i = 0; i < n_pages; ++i)
+    if (pages[i].dst_len > 0) order.push_back(i);
+  std::sort(order.begin(), order.end(), [&](int64_t x, int64_t y) { return pages[x].dst < pages[y].dst || (pages[x].dst == pages[y].dst && x < y); });
+  for (size_t k = 1; k < order.size(); ++k) {
+    const ag_pq_compressed &u = pages[order[k - 1]], &v = pages[order[k]];
+    if (v.dst < u.dst + u.dst_len) {
+      const int64_t x = std::min(order[k - 1], order[k]), y = std::max(order[k - 1], order[k]);
+      AG_FAIL(AG_ERR_INVALID, "%s: pages %lld and %lld: overlapping dst ranges", fn, (long long)x, (long long)y);
+    }
+  }
+  return AG_OK;
+}
+
 // Argument checks shared by every codec and both flavours; every one is AG_ERR_INVALID before any launch.  `src` and
 // `dst` are the compressed data and the output, in host or device memory; only whether they are NULL matters.
 // *src_end / *dst_end: the bytes of `src` / `dst` the batch spans.
@@ -30,23 +48,14 @@ static inline ag_status pq_compressed_check(const char* fn, const uint8_t* src, 
   if (n_pages < 0) AG_FAIL(AG_ERR_INVALID, "%s: negative page count", fn);
   if (n_pages == 0) return AG_OK;
   if (!pages) AG_FAIL(AG_ERR_INVALID, "%s: NULL page table", fn);
-  std::vector<int64_t> order;
   for (int64_t i = 0; i < n_pages; ++i) {
     const ag_pq_compressed& g = pages[i];
     if (g.src < 0 || g.src_len < 0 || g.dst < 0 || g.dst_len < 0 || g.src_len > 0xffffffffLL || g.dst_len > 0xffffffffLL)
       AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative field or more than 2^32-1 bytes", fn, (long long)i);
     *src_end = std::max(*src_end, g.src + g.src_len);
     *dst_end = std::max(*dst_end, g.dst + g.dst_len);
-    if (g.dst_len > 0) order.push_back(i);
   }
-  std::sort(order.begin(), order.end(), [&](int64_t x, int64_t y) { return pages[x].dst < pages[y].dst || (pages[x].dst == pages[y].dst && x < y); });
-  for (size_t k = 1; k < order.size(); ++k) {
-    const ag_pq_compressed &u = pages[order[k - 1]], &v = pages[order[k]];
-    if (v.dst < u.dst + u.dst_len) {
-      const int64_t x = std::min(order[k - 1], order[k]), y = std::max(order[k - 1], order[k]);
-      AG_FAIL(AG_ERR_INVALID, "%s: pages %lld and %lld: overlapping dst ranges", fn, (long long)x, (long long)y);
-    }
-  }
+  AG_TRY(pq_dst_overlap_check(fn, pages, n_pages));
   if (*src_end > 0 && !src) AG_FAIL(AG_ERR_INVALID, "%s: NULL compressed data", fn);
   if (*dst_end > 0 && !dst) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
   return AG_OK;

@@ -1326,6 +1326,49 @@ ag_status ag_parquet_lz4_raw_decompress_dev(const uint8_t* d_src, const ag_pq_co
                                             int64_t* d_written, ag_stream_t s);
 
 /* ================================================================================= *
+ * SNAPPY page compression — the decompressors' batch shape read the other way round, so that pages encoded on the
+ *   device are compressed there too.  serializedPageWriter.Compress (parquet/file/page_writer.go:229-233) sizes a
+ *   buffer with CompressBound and calls EncodeLevel; for SNAPPY that is snappyCodec (parquet/compress/snappy.go:27-33,
+ *   51-53), github.com/klauspost/compress's snappy.Encode with the bound 32 + n + n/6.
+ *     src      byte offset of the page's uncompressed bytes in `src`
+ *     src_len  their count, at most 2^32-1
+ *     dst      byte offset of the page's stream in `dst`
+ *     dst_len  the capacity there, at least ag_parquet_snappy_max_size(src_len)
+ *   `pages` is a HOST array in both flavours; pages may come in any order and may share or skip input.  written (may
+ *   be NULL) receives each stream's length, preamble included.  No byte outside [dst, dst + written) of any page is
+ *   written.  `src` and `dst` must not overlap (not checked).
+ *   Argument checks, AG_ERR_INVALID naming the page before any launch: a negative field, src_len above 2^32-1, a
+ *   capacity below the bound, and dst ranges [dst, dst + dst_len) that overlap.  Once they pass no data-dependent error
+ *   exists, so the device flavour does not synchronise `s`: d_written is a device array written in stream order, and
+ *   the call's tables and scratch (about the input's size) are stream-ordered allocations.  The host flavour stages `src` through device
+ *   memory and copies back only the written bytes.  Without a usable GPU both return AG_ERR_CUDA.
+ *   Format: raw Snappy, one parse stated exactly (tests/snappy_encode_model.py):
+ *     - the preamble uvarint(src_len); a page shorter than 4 bytes is the preamble and one literal (an empty page is
+ *       the single byte 0x00);
+ *     - 64 KiB fragments (the last may be shorter), each encoded on its own: an empty hash table, copies only within
+ *       the fragment (offsets 1..65535), its trailing bytes flushed as a literal;
+ *     - the candidate positions p of a fragment [s, e) are those with p + 4 <= e, walked in windows of 32 from a
+ *       cursor.  For each p in order: h(p) = ((load32le(p) * 0x1E35A7BD) mod 2^32) >> 20; its candidate q is the
+ *       latest position inserted with that hash (earlier positions of the window count); p is then inserted.  The
+ *       first p whose q holds the same 4 bytes starts a match, and the rest of the window is neither looked up nor
+ *       inserted.  The match extends while p + L < e and src[q + L] == src[p + L]; the bytes since the last match end
+ *       go out as a literal, then the copy, and the cursor moves to p + L.  A window without a match moves the cursor
+ *       past its last position;
+ *     - golang/snappy's element forms: a literal header holds length-1 in the tag below 60, else tag 60..63 and the
+ *       minimal 1..4 length bytes.  A copy of L bytes: 64-byte copies (2-byte offset) while L >= 68, a 60-byte copy
+ *       if L > 64 remains, then the 1-byte-offset form when L < 12 and offset < 2048, else the 2-byte-offset form.
+ *   Differences from the reference (DESIGN §2): klauspost/compress's source is not in the reference tree, so its bytes
+ *   are not pinned.  The streams here are valid raw Snappy within the same bound, and their size is close to a
+ *   production encoder's.
+ *   ag_parquet_snappy_max_size: 32 + n + n/6; n < 0 or n > 2^32-1 is AG_ERR_INVALID.  It needs no GPU.
+ * ================================================================================= */
+ag_status ag_parquet_snappy_max_size(int64_t n, int64_t* size);
+ag_status ag_parquet_snappy_compress(const uint8_t* src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* dst,
+                                     int64_t* written);
+ag_status ag_parquet_snappy_compress_dev(const uint8_t* d_src, const ag_pq_compressed* pages, int64_t n_pages, uint8_t* d_dst,
+                                         int64_t* d_written, ag_stream_t s);
+
+/* ================================================================================= *
  * Parity helpers for inputs too large to bring back to the host (SURVEY §8d):
  * order-sensitive 64-bit checksum  sum_i mix64(i) * word_i  (mod 2^64)  over a buffer
  * viewed as little-endian uint64 words (n_words = nbytes/8), and a counter-based

@@ -331,6 +331,9 @@ _SIGS = {
     "ag_parquet_delta_max_size": [_i, _i, _i, _i64, _pi64],
     "ag_parquet_delta_encode": [_i, _i, _i, _p, _p, _i64, _p, _p],
     "ag_parquet_delta_encode_dev": [_i, _i, _i, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_byte_array_max_size": [_i, _i64, _i64, _pi64],
+    "ag_parquet_byte_array_encode": [_i, _i, _p, _p, _p, _p, _i64, _p, _p, _p],
+    "ag_parquet_byte_array_encode_dev": [_i, _i, _p, _p, _p, _p, _i64, _p, _p, _p, _p],
     "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_zstd_decompress": [_p, _p, _i64, _p, _p],

@@ -25,10 +25,16 @@
 // block's min delta, each miniblock's width (deltas wrap at the physical width), the block's size, a scan of the 8
 // warps' sizes, then the header and bit-packed miniblocks.  Values are read from global memory (L1 / L2 serve the
 // repeats); HBM traffic: values read once plus encoded bytes written once.
+//
+// BYTE_ARRAY (PLAIN, DELTA_LENGTH_BYTE_ARRAY, DELTA_BYTE_ARRAY) from Arrow offsets, data and validity, over 1024-slot
+// tiles of every page: ba_check_kernel (offsets and validity only: slot errors, per-tile sums) and tile_sum_scan_kernel,
+// then the call's one synchronisation reads the per-page error words; ba_last_scan_kernel (DELTA: each tile's previous
+// valid slot) and ba_dense_kernel (dense lengths, DELTA prefixes)
+// feeds delta_encode_kernel<int32_t> through device page tables; ba_bytes_kernel writes each section in aligned 16-byte
+// pieces.  BaCall below describes the order.
 #include <climits>
 
-#include "host_stage.cuh"
-#include "pq_window.cuh"
+#include "pq_decode.cuh"
 
 namespace ag {
 
@@ -406,7 +412,7 @@ int64_t rle_bound(int bw, int form, int64_t n) {
 }
 
 // header (4 varints of at most 10 bytes each) + per block: min delta (10) + width bytes + every miniblock at full width
-int64_t delta_bound(int width, int block, int mini, int64_t n) {
+__host__ __device__ int64_t delta_bound(int width, int block, int mini, int64_t n) {
   const int64_t nblk = n > 1 ? (n - 2) / block + 1 : 0;
   return 40 + nblk * (10 + mini + (int64_t)block * width);
 }
@@ -534,6 +540,458 @@ ag_status encode_host(const ag_pq_enc_page* pages, int64_t n_pages, const void* 
   return sync(cs);
 }
 
+// ------------------------------------------------------------------------------- BYTE_ARRAY value sections ----
+constexpr int kBaTile = 1024;                       // slots per tile of every BYTE_ARRAY pass
+constexpr int kBaItems = kBaTile / kPqThreads;      // 4 consecutive slots per thread
+constexpr unsigned long long kBaOk = ~0ull;         // error word of a page that passes
+constexpr unsigned long long kBaCap = ~0ull - 1;    // capacity below the bound; every slot error is lower
+enum BaErr { kBaNegFirst = 0, kBaDecreasing = 1, kBaTooLong = 2 };   // slot errors: word = slot * 4 + kind
+
+using u128 = unsigned __int128;
+
+struct BaArgs {
+  const ag_pq_enc_page* pages;
+  const int64_t* tile_base;       // [n_pages + 1]: first tile of every page
+  const int64_t* sum_base;        // [n_pages + 1]: tile_base[p] + p, page p's entries in cnt / bytes
+  int64_t n_pages, n_tiles;
+  const void* offsets;
+  const uint8_t* data;
+  const uint8_t* valid;           // NULL: every slot valid
+  int enc;
+  unsigned long long* err;        // [n_pages] lowest slot error word, kBaCap, or kBaOk
+  unsigned long long* cnt;        // per tile valid values, then (scanned) the page's before the tile; the page's
+                                  // entry after its tiles holds its total
+  unsigned long long* bytes;      // the same for the section bytes (DELTA: suffix bytes, written by the dense pass)
+  long long* last;                // [n_tiles] the tile's last valid slot, -1 if none (DELTA: then the page's, up to
+                                  // and including the tile)
+  int64_t* dense;                 // [n_pages + 1] the page's first dense value; [n_pages] all of them
+  int32_t* lens;                  // dense: lengths (DELTA_LENGTH) or suffix lengths (DELTA)
+  int32_t* pre;                   // dense: prefix lengths (DELTA)
+  ag_pq_enc_page* tab;            // [2 * n_pages] the length streams' pages (DELTA: prefixes, then suffixes)
+  int64_t* slen;                  // [2 * n_pages] bytes of those streams
+  int64_t* sec;                   // [n_pages] the byte section's offset from the page's out
+  uint8_t* out;
+  int64_t* lengths;               // may be NULL
+};
+
+__host__ __device__ __forceinline__ int64_t ba_bound(int enc, int64_t n, int64_t span) {
+  if (enc == AG_PQ_ENC_PLAIN) return 4 * n + span;
+  return (enc == AG_PQ_ENC_DELTA_BYTE_ARRAY ? 2 : 1) * delta_bound(4, 128, 4, n) + span;
+}
+
+template <typename O>
+__device__ __forceinline__ int64_t off_at(const void* o, int64_t i) { return (int64_t) static_cast<const O*>(o)[i]; }
+
+__device__ __forceinline__ u128 ld16(const uint8_t* p) {
+  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
+  return (u128)v.x | (u128)v.y << 32 | (u128)v.z << 64 | (u128)v.w << 96;
+}
+
+// bytes p[0, k), 1 <= k <= 16, in the low bytes: one or two aligned 16-byte loads shifted into place, touching only
+// the aligned words that hold those bytes
+__device__ __forceinline__ u128 window(const uint8_t* p, int k) {
+  const int sh = (int)(reinterpret_cast<uintptr_t>(p) & 15);
+  const uint8_t* a = p - sh;
+  u128 w = ld16(a) >> (8 * sh);
+  if (sh + k > 16) w |= ld16(a + 16) << (8 * (16 - sh));
+  return k == 16 ? w : w & (((u128)1 << (8 * k)) - 1);
+}
+
+// the length of the common prefix of x[0, m) and y[0, m), 16 bytes per step
+__device__ __forceinline__ int64_t common_prefix(const uint8_t* x, const uint8_t* y, int64_t m) {
+  for (int64_t k = 0; k < m; k += 16) {
+    const int c = m - k < 16 ? (int)(m - k) : 16;
+    const u128 d = window(x + k, c) ^ window(y + k, c);
+    if (d) {
+      const unsigned long long lo = (unsigned long long)d;
+      return k + (lo ? __ffsll((long long)lo) - 1 : 64 + __ffsll((long long)(d >> 64)) - 1) / 8;
+    }
+  }
+  return m;
+}
+
+// the tile of block `t`: its page, the page's slot of the thread's first item, the offsets of the thread's items and
+// their validity (false past the page)
+struct BaSlots {
+  int64_t p, j0;
+  ag_pq_enc_page pg;
+  int64_t o[kBaItems + 1];
+  bool v[kBaItems];
+};
+
+template <typename O>
+__device__ __forceinline__ void ba_slots(const BaArgs& a, int64_t t, BaSlots& s) {
+  s.p = find_page(a.tile_base, a.n_pages, t);
+  s.pg = a.pages[s.p];
+  s.j0 = (t - a.tile_base[s.p]) * kBaTile + threadIdx.x * kBaItems;
+#pragma unroll
+  for (int q = 0; q <= kBaItems; ++q) {
+    const int64_t j = s.j0 + q;
+    s.o[q] = j <= s.pg.num_values ? off_at<O>(a.offsets, s.pg.in + j) : 0;
+    if (q < kBaItems) s.v[q] = j < s.pg.num_values && (!a.valid || bit_is_set(a.valid, s.pg.in + j));
+  }
+}
+
+// Checking pass: one thread per page for the capacity (from the page's offsets span), one block per tile for the
+// slot errors and the tile's valid count, section bytes (PLAIN, DELTA_LENGTH) and last valid slot.  Reads offsets and
+// validity only.
+template <typename O>
+__global__ void __launch_bounds__(kPqThreads)
+ba_check_kernel(BaArgs a) {
+  __shared__ long long wl[kPqThreads / 32];
+  for (int64_t p = (int64_t)blockIdx.x * kPqThreads + threadIdx.x; p < a.n_pages; p += (int64_t)gridDim.x * kPqThreads) {
+    const ag_pq_enc_page pg = a.pages[p];
+    const int64_t span = pg.num_values ? off_at<O>(a.offsets, pg.in + pg.num_values) - off_at<O>(a.offsets, pg.in) : 0;
+    if (pg.capacity < ba_bound(a.enc, pg.num_values, span)) atomicMin(a.err + p, kBaCap);
+  }
+  if (blockIdx.x >= a.n_tiles) return;
+  const int64_t t = blockIdx.x;
+  BaSlots s;
+  ba_slots<O>(a, t, s);
+  long long c = 0, b = 0, lst = -1;
+  unsigned long long bad = kBaOk;
+#pragma unroll
+  for (int q = 0; q < kBaItems; ++q) {
+    const int64_t j = s.j0 + q;
+    if (j >= s.pg.num_values) break;
+    const unsigned long long w = (unsigned long long)(s.pg.in + j) * 4;
+    const int64_t len = s.o[q + 1] - s.o[q];
+    if (j == 0 && s.o[0] < 0) bad = min(bad, w + kBaNegFirst);
+    if (len < 0) bad = min(bad, w + kBaDecreasing);
+    else if (s.v[q] && len > INT_MAX) bad = min(bad, w + kBaTooLong);
+    if (s.v[q]) {
+      ++c;
+      b += len + (a.enc == AG_PQ_ENC_PLAIN ? 4 : 0);
+      lst = s.pg.in + j;
+    }
+  }
+  if (bad != kBaOk) atomicMin(a.err + s.p, bad);
+  auto lsum = [](long long x, long long y) { return x + y; };
+  auto lmax = [](long long x, long long y) { return x > y ? x : y; };
+  long long ctot, btot, ltot;
+  block_scan_op<false>(c, 0ll, lsum, wl, &ctot);
+  block_scan_op<false>(b, 0ll, lsum, wl, &btot);
+  block_scan_op<false>(lst, -1ll, lmax, wl, &ltot);
+  if (threadIdx.x == 0) {
+    a.cnt[t + s.p] = (unsigned long long)ctot;
+    if (a.enc != AG_PQ_ENC_DELTA_BYTE_ARRAY) a.bytes[t + s.p] = (unsigned long long)btot;
+    a.last[t] = ltot;
+  }
+}
+
+// one block: every page's first dense value and the length streams' page tables (input at the page's dense base,
+// num_values its valid count, output at its out)
+__global__ void __launch_bounds__(kPqThreads)
+ba_tables_kernel(BaArgs a) {
+  __shared__ long long ws[kPqThreads / 32];
+  for (int64_t p = threadIdx.x; p < a.n_pages; p += kPqThreads) a.dense[p] = (int64_t)a.cnt[a.sum_base[p + 1] - 1];
+  __syncthreads();
+  const int64_t total = segment_excl_scan(a.dense, 0, a.n_pages, ws);
+  __syncthreads();
+  if (threadIdx.x == 0) a.dense[a.n_pages] = total;
+  for (int64_t p = threadIdx.x; p < a.n_pages; p += kPqThreads) {
+    const ag_pq_enc_page pg = a.pages[p];
+    const ag_pq_enc_page t{a.dense[p], (int64_t)a.cnt[a.sum_base[p + 1] - 1], pg.out, pg.capacity};
+    a.tab[p] = t;
+    a.tab[a.n_pages + p] = t;
+  }
+}
+
+// DELTA, one block per page: each tile's last valid slot -> the page's last valid slot at or before the tile (a max-scan
+// over the page's tiles), so that a tile after a run of all-null tiles finds its previous value in one load
+__global__ void __launch_bounds__(kPqThreads)
+ba_last_scan_kernel(const int64_t* tile_base, long long* last) {
+  __shared__ long long wl[kPqThreads / 32];
+  auto lmax = [](long long x, long long y) { return x > y ? x : y; };
+  const int64_t t1 = tile_base[blockIdx.x + 1];
+  long long run = -1;
+  for (int64_t t = tile_base[blockIdx.x]; t < t1; t += kPqThreads) {
+    const int64_t i = t + threadIdx.x;
+    const long long x = i < t1 ? last[i] : -1ll;
+    long long tot;
+    const long long ex = block_scan_op<false>(x, -1ll, lmax, wl, &tot);
+    if (i < t1) last[i] = lmax(lmax(run, ex), x);
+    run = lmax(run, tot);
+  }
+}
+
+// DELTA_LENGTH / DELTA: the valid values' lengths as dense int32; DELTA: prefix lengths against the previous valid
+// value of the page (across a tile edge, the page's last valid slot before the tile, from ba_last_scan_kernel) and
+// suffix lengths, and the tile's suffix bytes
+template <typename O, bool DBA>
+__global__ void __launch_bounds__(kPqThreads)
+ba_dense_kernel(BaArgs a) {
+  __shared__ long long wl[kPqThreads / 32];
+  const int64_t t = blockIdx.x;
+  BaSlots s;
+  ba_slots<O>(a, t, s);
+  auto lsum = [](long long x, long long y) { return x + y; };
+  auto lmax = [](long long x, long long y) { return x > y ? x : y; };
+  long long c = 0, lst = -1, tot;
+#pragma unroll
+  for (int q = 0; q < kBaItems; ++q)
+    if (s.v[q]) { ++c; lst = s.pg.in + s.j0 + q; }
+  int64_t r = a.dense[s.p] + (int64_t)a.cnt[t + s.p] + block_scan_op<false>(c, 0ll, lsum, wl, &tot);
+  long long prev = -1;
+  if (DBA) prev = lmax(block_scan_op<false>(lst, -1ll, lmax, wl, &tot), t > a.tile_base[s.p] ? a.last[t - 1] : -1ll);
+  long long sb = 0;
+#pragma unroll
+  for (int q = 0; q < kBaItems; ++q) {
+    if (!s.v[q]) continue;
+    const int64_t len = s.o[q + 1] - s.o[q];
+    int64_t pl = 0;
+    if (DBA) {
+      if (prev >= 0) {
+        const int64_t p0 = off_at<O>(a.offsets, prev), plen = off_at<O>(a.offsets, prev + 1) - p0;
+        pl = common_prefix(a.data + p0, a.data + s.o[q], plen < len ? plen : len);
+      }
+      a.pre[r] = (int32_t)pl;
+      prev = s.pg.in + s.j0 + q;
+    }
+    a.lens[r++] = (int32_t)(len - pl);
+    sb += len - pl;
+  }
+  if (DBA) {
+    block_scan_op<false>(sb, 0ll, lsum, wl, &tot);
+    if (threadIdx.x == 0) a.bytes[t + s.p] = (unsigned long long)tot;
+  }
+}
+
+// DELTA: the suffix-length stream starts where the prefix stream ends
+__global__ void ba_link_kernel(BaArgs a) {
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < a.n_pages; p += (int64_t)gridDim.x * blockDim.x)
+    a.tab[a.n_pages + p].out = a.tab[p].out + a.slen[p];
+}
+
+// every page: its byte section's offset after its length streams, and the bytes it wrote
+__global__ void ba_finish_kernel(BaArgs a, int streams) {
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < a.n_pages; p += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t sec = (streams > 0 ? a.slen[p] : 0) + (streams > 1 ? a.slen[a.n_pages + p] : 0);
+    a.sec[p] = sec;
+    if (a.lengths) a.lengths[p] = sec + (int64_t)a.bytes[a.sum_base[p + 1] - 1];
+  }
+}
+
+// Byte pass, one block per tile: each slot's section bytes (PLAIN: 4-byte length and value; DELTA_LENGTH: value;
+// DELTA: suffix) are placed by a scan into shared memory, then threads fill the tile's section in 16-byte pieces
+// aligned in `out`: a binary search finds the slot under a piece's first byte, the piece is assembled in a register
+// from 16-byte loads shifted into place, and stored whole (pieces cut by the tile's ends: byte by byte).
+template <typename O, int ENC>
+__global__ void __launch_bounds__(kPqThreads)
+ba_bytes_kernel(BaArgs a) {
+  __shared__ long long wl[kPqThreads / 32];
+  __shared__ int64_t soff[kBaTile + 1];   // tile slot -> its first byte, relative to the tile's
+  __shared__ int64_t ssrc[kBaTile];       // tile slot -> its first data byte placed
+  const int64_t t = blockIdx.x;
+  const int tid = threadIdx.x;
+  BaSlots s;
+  ba_slots<O>(a, t, s);
+  auto lsum = [](long long x, long long y) { return x + y; };
+  long long tot;
+  int64_t r = 0;
+  if (ENC == AG_PQ_ENC_DELTA_BYTE_ARRAY) {
+    long long c = 0;
+#pragma unroll
+    for (int q = 0; q < kBaItems; ++q) c += s.v[q];
+    r = a.dense[s.p] + (int64_t)a.cnt[t + s.p] + block_scan_op<false>(c, 0ll, lsum, wl, &tot);
+  }
+  int64_t z[kBaItems];
+  long long sum = 0;
+#pragma unroll
+  for (int q = 0; q < kBaItems; ++q) {
+    z[q] = 0;
+    int64_t src = s.o[q];
+    if (s.v[q]) {
+      z[q] = s.o[q + 1] - s.o[q];
+      if (ENC == AG_PQ_ENC_PLAIN) z[q] += 4;
+      if (ENC == AG_PQ_ENC_DELTA_BYTE_ARRAY) { const int32_t pl = a.pre[r++]; z[q] -= pl; src += pl; }
+    }
+    ssrc[tid * kBaItems + q] = src;
+    sum += z[q];
+  }
+  long long run = block_scan_op<false>(sum, 0ll, lsum, wl, &tot);
+#pragma unroll
+  for (int q = 0; q < kBaItems; ++q) { soff[tid * kBaItems + q] = run; run += z[q]; }
+  if (tid == 0) soff[kBaTile] = tot;
+  __syncthreads();
+
+  uint8_t* const lo_p = a.out + s.pg.out + a.sec[s.p] + (int64_t)a.bytes[t + s.p];
+  const uintptr_t lo_a = reinterpret_cast<uintptr_t>(lo_p), hi_a = lo_a + (uintptr_t)tot;
+  for (uintptr_t P = (lo_a & ~(uintptr_t)15) + 16 * (uintptr_t)tid; P < hi_a; P += 16 * kPqThreads) {
+    const uintptr_t lo = P > lo_a ? P : lo_a, hi = P + 16 < hi_a ? P + 16 : hi_a;
+    int64_t b = (int64_t)(lo - lo_a);
+    int l = 0, h = kBaTile - 1;                     // the last slot starting at or before b holds b
+    while (l < h) {
+      const int m = (l + h + 1) >> 1;
+      if (soff[m] <= b) l = m; else h = m - 1;
+    }
+    u128 acc = 0;
+    const int dend = (int)(hi - P);
+    for (int d = (int)(lo - P), k; d < dend; d += k, b += k) {
+      int64_t w = b - soff[l];
+      while (w >= soff[l + 1] - soff[l]) { ++l; w = b - soff[l]; }   // past the slot's bytes, and empty slots
+      const int64_t left = soff[l + 1] - soff[l] - w;
+      u128 part;
+      if (ENC == AG_PQ_ENC_PLAIN && w < 4) {
+        k = (int)(4 - w < dend - d ? 4 - w : dend - d);
+        const unsigned long long hdr = (unsigned long long)(uint32_t)(soff[l + 1] - soff[l] - 4) >> (8 * w);
+        part = (u128)(hdr & ((1ull << (8 * k)) - 1));
+      } else {
+        k = (int)(left < dend - d ? left : dend - d);
+        part = window(a.data + ssrc[l] + (ENC == AG_PQ_ENC_PLAIN ? w - 4 : w), k);
+      }
+      acc |= part << (8 * d);
+    }
+    uint8_t* const dst = reinterpret_cast<uint8_t*>(P);
+    if (lo == P && hi == P + 16) {
+      *reinterpret_cast<uint4*>(dst) = make_uint4((uint32_t)acc, (uint32_t)(acc >> 32), (uint32_t)(acc >> 64), (uint32_t)(acc >> 96));
+    } else {
+      for (int d = (int)(lo - P); d < dend; ++d) dst[d] = (uint8_t)(acc >> (8 * d));
+    }
+  }
+}
+
+ag_status check_ba_args(const char* fn, int enc, int ow) {
+  if (enc != AG_PQ_ENC_PLAIN && enc != AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY && enc != AG_PQ_ENC_DELTA_BYTE_ARRAY)
+    AG_FAIL(AG_ERR_INVALID, "%s: encoding %d is not PLAIN, DELTA_LENGTH_BYTE_ARRAY or DELTA_BYTE_ARRAY", fn, enc);
+  if (ow != 4 && ow != 8) AG_FAIL(AG_ERR_INVALID, "%s: offset_width must be 4 or 8, got %d", fn, ow);
+  return AG_OK;
+}
+
+// The host checks of a call: arguments, the page table, and the buffers the pages reach.  *in_end: the slots they reach.
+ag_status check_ba_call(const char* fn, int enc, int ow, const void* offsets, const uint8_t* data, const ag_pq_enc_page* pages,
+                        int64_t n_pages, const uint8_t* out, int64_t* in_end, int64_t* out_end) {
+  AG_TRY(check_ba_args(fn, enc, ow));
+  AG_TRY(check_pages(fn, pages, n_pages, [](int64_t) { return (int64_t)0; }, in_end, out_end));
+  if (*in_end > 0 && !offsets) AG_FAIL(AG_ERR_INVALID, "%s: NULL offsets", fn);
+  if (*in_end > 0 && !data) AG_FAIL(AG_ERR_INVALID, "%s: NULL data", fn);
+  if (*out_end > 0 && !out) AG_FAIL(AG_ERR_INVALID, "%s: NULL output", fn);
+  return AG_OK;
+}
+
+// One checked call in two steps: check() runs the checking pass and synchronises `st` once to read the per-page error
+// words; encode() then enqueues the rest without synchronising.  Scratch and tables are stream-ordered.
+struct BaCall {
+  const char* fn;
+  int enc, ow;
+  const ag_pq_enc_page* pages;
+  int64_t n_pages;
+  cudaStream_t st;
+  TableImage img;
+  void* scratch = nullptr;
+  void* vals = nullptr;
+  BaArgs a{};
+  int64_t total = 0;   // valid values of all pages (DELTA_LENGTH, DELTA)
+  BaCall(const char* f, int e, int w, const ag_pq_enc_page* p, int64_t n, cudaStream_t s)
+      : fn(f), enc(e), ow(w), pages(p), n_pages(n), st(s), img(s) {}
+  ~BaCall() { dev_free_async(vals, st); dev_free_async(scratch, st); }
+
+  ag_status check(const void* d_off, const uint8_t* d_valid, int64_t* d_bad_pos, int64_t* h_bad) {
+    std::vector<int64_t> tb((size_t)n_pages + 1, 0), sb((size_t)n_pages + 1, 0);
+    for (int64_t i = 0; i < n_pages; ++i) {
+      tb[(size_t)i + 1] = tb[(size_t)i] + (pages[i].num_values + kBaTile - 1) / kBaTile;
+      sb[(size_t)i + 1] = tb[(size_t)i + 1] + i + 1;
+    }
+    const int64_t n_tiles = tb[(size_t)n_pages];
+    if (n_tiles > 0x7fffffff) AG_FAIL(AG_ERR_INVALID, "%s: more than 2^31-1 tiles of %d slots", fn, kBaTile);
+    const size_t o_pages = img.add(std::vector<ag_pq_enc_page>(pages, pages + n_pages));
+    const size_t o_tb = img.add(tb), o_sb = img.add(sb);
+    const size_t o_err = img.add(std::vector<unsigned long long>((size_t)n_pages, kBaOk));
+    AG_TRY(img.upload(fn));
+    Carve sc;
+    const size_t o_cnt = sc.take((size_t)(n_tiles + n_pages) * 8), o_bytes = sc.take((size_t)(n_tiles + n_pages) * 8);
+    const size_t o_last = sc.take((size_t)n_tiles * 8), o_dense = sc.take((size_t)(n_pages + 1) * 8);
+    const size_t o_tab = sc.take((size_t)n_pages * 2 * sizeof(ag_pq_enc_page)), o_slen = sc.take((size_t)n_pages * 16);
+    const size_t o_sec = sc.take((size_t)n_pages * 8);
+    AG_TRY(dev_alloc_async(&scratch, sc.size, st));
+    uint8_t* d = static_cast<uint8_t*>(scratch);
+    AG_CUDA_TRY(cudaMemsetAsync(d, 0, o_last, st));   // cnt and bytes: the pages' total entries start at 0
+    a = BaArgs{img.at<ag_pq_enc_page>(o_pages), img.at<int64_t>(o_tb), img.at<int64_t>(o_sb), n_pages, n_tiles, d_off,
+               nullptr, d_valid, enc, img.at<unsigned long long>(o_err), reinterpret_cast<unsigned long long*>(d + o_cnt),
+               reinterpret_cast<unsigned long long*>(d + o_bytes), reinterpret_cast<long long*>(d + o_last),
+               reinterpret_cast<int64_t*>(d + o_dense), nullptr, nullptr, reinterpret_cast<ag_pq_enc_page*>(d + o_tab),
+               reinterpret_cast<int64_t*>(d + o_slen), reinterpret_cast<int64_t*>(d + o_sec), nullptr, nullptr};
+    const unsigned grid = (unsigned)std::max<int64_t>(n_tiles, (n_pages + kPqThreads - 1) / kPqThreads);
+    if (ow == 4) ba_check_kernel<int32_t><<<grid, kPqThreads, 0, st>>>(a);
+    else ba_check_kernel<int64_t><<<grid, kPqThreads, 0, st>>>(a);
+    AG_TRY(check_launch("ba_check_kernel"));
+    tile_sum_scan_kernel<<<(unsigned)n_pages, kPqThreads, 0, st>>>(a.sum_base, a.cnt);
+    AG_TRY(check_launch("tile_sum_scan_kernel"));
+    if (enc != AG_PQ_ENC_DELTA_BYTE_ARRAY) {
+      tile_sum_scan_kernel<<<(unsigned)n_pages, kPqThreads, 0, st>>>(a.sum_base, a.bytes);
+      AG_TRY(check_launch("tile_sum_scan_kernel"));
+    }
+    if (enc != AG_PQ_ENC_PLAIN) {
+      ba_tables_kernel<<<1, kPqThreads, 0, st>>>(a);
+      AG_TRY(check_launch("ba_tables_kernel"));
+      AG_TRY(d2h(&total, a.dense + n_pages, 8, st));
+    }
+    std::vector<unsigned long long> err((size_t)n_pages);
+    AG_TRY(d2h(err.data(), a.err, (size_t)n_pages * 8, st));
+    AG_TRY(sync(st));
+    int64_t page = -1;
+    for (int64_t i = 0; i < n_pages && page < 0; ++i) if (err[(size_t)i] != kBaOk) page = i;
+    const unsigned long long w = page < 0 ? kBaOk : err[(size_t)page];
+    const int64_t bad = page < 0 || w == kBaCap ? (int64_t)AG_NO_ERROR_POS : (int64_t)(w >> 2);
+    if (h_bad) *h_bad = bad;
+    if (d_bad_pos) AG_TRY(h2d(d_bad_pos, &bad, 8, st));
+    if (page < 0) return AG_OK;
+    const long long pl = (long long)page, sl = (long long)bad;
+    if (w == kBaCap) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: capacity %lld below the bound for its %lld values and their bytes", fn, pl,
+                             (long long)pages[page].capacity, (long long)pages[page].num_values);
+    if ((w & 3) == kBaNegFirst) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative offset at slot %lld", fn, pl, sl);
+    if ((w & 3) == kBaDecreasing) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: offsets decrease after slot %lld", fn, pl, sl);
+    AG_FAIL(AG_ERR_INVALID, "%s: page %lld: value at slot %lld longer than 2^31-1 bytes", fn, pl, sl);
+  }
+
+  ag_status encode(const uint8_t* d_data, uint8_t* d_out, int64_t* d_lengths) {
+    a.data = d_data;
+    a.out = d_out;
+    a.lengths = d_lengths;
+    const bool dba = enc == AG_PQ_ENC_DELTA_BYTE_ARRAY;
+    const unsigned nt = (unsigned)a.n_tiles, np = (unsigned)n_pages, ng = (unsigned)((n_pages + kPqThreads - 1) / kPqThreads);
+    if (enc != AG_PQ_ENC_PLAIN) {
+      AG_TRY(dev_alloc_async(&vals, (size_t)total * (dba ? 8 : 4) + 16, st));
+      a.lens = static_cast<int32_t*>(vals);
+      a.pre = a.lens + total;
+      if (nt && dba) {
+        ba_last_scan_kernel<<<np, kPqThreads, 0, st>>>(a.tile_base, a.last);
+        AG_TRY(check_launch("ba_last_scan_kernel"));
+      }
+      if (nt) {
+        if (ow == 4) dba ? ba_dense_kernel<int32_t, true><<<nt, kPqThreads, 0, st>>>(a) : ba_dense_kernel<int32_t, false><<<nt, kPqThreads, 0, st>>>(a);
+        else dba ? ba_dense_kernel<int64_t, true><<<nt, kPqThreads, 0, st>>>(a) : ba_dense_kernel<int64_t, false><<<nt, kPqThreads, 0, st>>>(a);
+        AG_TRY(check_launch("ba_dense_kernel"));
+      }
+      if (dba) {
+        tile_sum_scan_kernel<<<np, kPqThreads, 0, st>>>(a.sum_base, a.bytes);
+        AG_TRY(check_launch("tile_sum_scan_kernel"));
+      }
+      delta_encode_kernel<int32_t><<<np, kPqThreads, 0, st>>>(DeltaEncArgs{a.tab, dba ? a.pre : a.lens, d_out, a.slen, 128, 4});
+      AG_TRY(check_launch("delta_encode_kernel"));
+      if (dba) {
+        ba_link_kernel<<<ng, kPqThreads, 0, st>>>(a);
+        AG_TRY(check_launch("ba_link_kernel"));
+        delta_encode_kernel<int32_t><<<np, kPqThreads, 0, st>>>(DeltaEncArgs{a.tab + n_pages, a.lens, d_out, a.slen + n_pages, 128, 4});
+        AG_TRY(check_launch("delta_encode_kernel"));
+      }
+    }
+    ba_finish_kernel<<<ng, kPqThreads, 0, st>>>(a, enc == AG_PQ_ENC_PLAIN ? 0 : dba ? 2 : 1);
+    AG_TRY(check_launch("ba_finish_kernel"));
+    if (!nt) return AG_OK;
+    if (ow == 4) {
+      if (enc == AG_PQ_ENC_PLAIN) ba_bytes_kernel<int32_t, AG_PQ_ENC_PLAIN><<<nt, kPqThreads, 0, st>>>(a);
+      else if (dba) ba_bytes_kernel<int32_t, AG_PQ_ENC_DELTA_BYTE_ARRAY><<<nt, kPqThreads, 0, st>>>(a);
+      else ba_bytes_kernel<int32_t, AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY><<<nt, kPqThreads, 0, st>>>(a);
+    } else {
+      if (enc == AG_PQ_ENC_PLAIN) ba_bytes_kernel<int64_t, AG_PQ_ENC_PLAIN><<<nt, kPqThreads, 0, st>>>(a);
+      else if (dba) ba_bytes_kernel<int64_t, AG_PQ_ENC_DELTA_BYTE_ARRAY><<<nt, kPqThreads, 0, st>>>(a);
+      else ba_bytes_kernel<int64_t, AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY><<<nt, kPqThreads, 0, st>>>(a);
+    }
+    return check_launch("ba_bytes_kernel");
+  }
+};
+
 }  // namespace
 
 }  // namespace ag
@@ -598,6 +1056,79 @@ ag_status ag_parquet_delta_encode(int value_width, int block_size, int miniblock
   return encode_host(pages, n_pages, values, in_end * value_width, out_end, out, lengths, [&](const uint8_t* dv, uint8_t* dout, int64_t* dlen, cudaStream_t st) {
     return delta_encode_dev(value_width, block_size, miniblocks, dv, pages, n_pages, dout, dlen, st);
   });
+}
+
+ag_status ag_parquet_byte_array_max_size(int encoding, int64_t num_values, int64_t value_bytes, int64_t* size) {
+  AG_TRY(check_ba_args("byte_array_max_size", encoding, 4));
+  if (num_values < 0 || num_values > 0x7fffffff) AG_FAIL(AG_ERR_INVALID, "byte_array_max_size: num_values %lld outside 0..2^31-1", (long long)num_values);
+  if (value_bytes < 0 || value_bytes > (1ll << 62)) AG_FAIL(AG_ERR_INVALID, "byte_array_max_size: value_bytes %lld outside 0..2^62", (long long)value_bytes);
+  if (!size) AG_FAIL(AG_ERR_INVALID, "byte_array_max_size: NULL size");
+  *size = ba_bound(encoding, num_values, value_bytes);
+  return AG_OK;
+}
+
+ag_status ag_parquet_byte_array_encode_dev(int encoding, int offset_width, const void* d_offsets, const uint8_t* d_data,
+                                           const uint8_t* d_valid, const ag_pq_enc_page* pages, int64_t n_pages, uint8_t* d_out,
+                                           int64_t* d_lengths, int64_t* d_bad_pos, ag_stream_t s) {
+  AG_TRY(ensure_init());
+  const char* fn = "byte_array_encode";
+  int64_t in_end, out_end;
+  AG_TRY(check_ba_call(fn, encoding, offset_width, d_offsets, d_data, pages, n_pages, d_out, &in_end, &out_end));
+  const cudaStream_t st = resolve_stream(s);
+  if (n_pages == 0) {
+    static const int64_t kNoPos = AG_NO_ERROR_POS;
+    return d_bad_pos ? h2d(d_bad_pos, &kNoPos, 8, st) : AG_OK;
+  }
+  BaCall c(fn, encoding, offset_width, pages, n_pages, st);
+  AG_TRY(c.check(d_offsets, d_valid, d_bad_pos, nullptr));
+  return c.encode(d_data, d_out, d_lengths);
+}
+
+ag_status ag_parquet_byte_array_encode(int encoding, int offset_width, const void* offsets, const uint8_t* data, const uint8_t* valid,
+                                       const ag_pq_enc_page* pages, int64_t n_pages, uint8_t* out, int64_t* lengths, int64_t* bad_pos) {
+  AG_TRY(ensure_init());
+  const char* fn = "byte_array_encode";
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  int64_t in_end, out_end;
+  AG_TRY(check_ba_call(fn, encoding, offset_width, offsets, data, pages, n_pages, out, &in_end, &out_end));
+  if (n_pages == 0) return AG_OK;
+  // Stage the slots the pages reach, [s0, in_end) with s0 a multiple of 8 so the validity bytes keep their bit phase.
+  // Staged buffers are addressed through pointers moved back by their first element, so the kernels see the caller's
+  // slot and data indices.
+  int64_t s0 = in_end;
+  for (int64_t i = 0; i < n_pages; ++i) if (pages[i].num_values) s0 = std::min(s0, pages[i].in);
+  s0 &= ~(int64_t)7;
+  const int64_t n_off = in_end > 0 ? in_end - s0 + 1 : 0, n_vb = valid && in_end > 0 ? (in_end - s0 + 7) / 8 : 0;
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  Carve sc;
+  const size_t o_off = sc.take((size_t)(n_off * offset_width)), o_vb = sc.take((size_t)n_vb);
+  const size_t o_out = sc.take((size_t)out_end), o_len = sc.take((size_t)n_pages * 8);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, sc.size));
+  AG_TRY(h2d(d + o_off, static_cast<const uint8_t*>(offsets) + s0 * offset_width, (size_t)(n_off * offset_width), cs));
+  AG_TRY(h2d(d + o_vb, valid + s0 / 8, (size_t)n_vb, cs));
+  int64_t* d_len = reinterpret_cast<int64_t*>(d + o_len);
+  BaCall c(fn, encoding, offset_width, pages, n_pages, cs);
+  AG_TRY(c.check(d + o_off - s0 * offset_width, valid ? d + o_vb - s0 / 8 : nullptr, nullptr, bad_pos));
+  // the checks passed, so every page's bytes lie between its first and last offsets
+  auto off = [&](int64_t i) {
+    return offset_width == 4 ? (int64_t) static_cast<const int32_t*>(offsets)[i] : static_cast<const int64_t*>(offsets)[i];
+  };
+  int64_t lo = INT64_MAX, hi = 0;
+  for (int64_t i = 0; i < n_pages; ++i)
+    if (pages[i].num_values) { lo = std::min(lo, off(pages[i].in)); hi = std::max(hi, off(pages[i].in + pages[i].num_values)); }
+  if (hi < lo) lo = hi;
+  uint8_t* dd;
+  AG_TRY(t.alloc_t(&dd, (size_t)(hi - lo)));
+  AG_TRY(h2d(dd, data + lo, (size_t)(hi - lo), cs));
+  AG_TRY(c.encode(dd - lo, d + o_out, d_len));
+  std::vector<int64_t> len((size_t)n_pages);
+  AG_TRY(d2h(len.data(), d_len, (size_t)n_pages * 8, cs));
+  AG_TRY(sync(cs));
+  for (int64_t i = 0; i < n_pages; ++i) AG_TRY(d2h(out + pages[i].out, d + o_out + pages[i].out, (size_t)len[(size_t)i], cs));
+  if (lengths) memcpy(lengths, len.data(), (size_t)n_pages * 8);
+  return sync(cs);
 }
 
 }  // extern "C"

@@ -1041,6 +1041,55 @@ ag_status ag_parquet_byte_array_decode_dev(int encoding, int offset_width, const
                                            int64_t* total, int64_t* d_decoded, int64_t* d_bad_pos, ag_stream_t s);
 
 /* ================================================================================= *
+ * BYTE_ARRAY page encoders: the value sections of data pages from an Arrow Binary / String (offset_width 4) or
+ *   LargeBinary / LargeString (offset_width 8) array, as arrow-go's writer produces them.  The page encoders' batch
+ *   contract (ag_pq_enc_page, a HOST array in both flavours), except that the input is spaced: slot i is bit i of
+ *   `valid` (NULL: every slot valid) and the bytes data[offsets[i] .. offsets[i+1]); a null slot is skipped whatever
+ *   its length.  pg.in is the page's first slot, pg.num_values its slots (nulls included, 0 .. 2^31-1); a slice is a
+ *   page table, so there is no offset argument.  Pages may come in any order, share or skip slots, and their sections
+ *   need not be contiguous.  lengths[i] (may be NULL) receives the bytes page i wrote.
+ *     AG_PQ_ENC_PLAIN: PlainByteArrayEncoder.Put / PutSpaced (parquet/internal/encoding/byte_array_encoder.go:41-89):
+ *       each valid value as a 4-byte little-endian length and its bytes.  Also the dictionary page of a string
+ *       dictionary, with valid = NULL.
+ *     AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY: DeltaLengthByteArrayEncoder (delta_length_byte_array.go:44-96): the lengths as
+ *       a DELTA_BINARY_PACKED INT32 stream, then the values' bytes back to back.
+ *     AG_PQ_ENC_DELTA_BYTE_ARRAY: DeltaByteArrayEncoder (delta_byte_array.go:56-149): the lengths of the prefixes each
+ *       valid value shares with the previous valid value of the page as a DELTA_BINARY_PACKED INT32 stream, then the
+ *       suffixes as a DELTA_LENGTH_BYTE_ARRAY section.
+ *     The length streams use the reference's block shape, 128 values in 4 miniblocks (delta_bit_packing.go:338-339),
+ *     byte for byte as ag_parquet_delta_encode writes them.
+ *   ag_parquet_byte_array_max_size: with value_bytes = offsets[in + n] - offsets[in] (0 .. 2^62), PLAIN 4n + value_bytes,
+ *     DELTA_LENGTH_BYTE_ARRAY delta(n) + value_bytes, DELTA_BYTE_ARRAY 2 delta(n) + value_bytes, where delta(n) is
+ *     ag_parquet_delta_max_size(4, 128, 4, n).  It needs no GPU.
+ *   Checks, every one AG_ERR_INVALID before any output byte is written:
+ *     on the host: an unknown encoding or offset width, a page-table error of the page encoders (negative field,
+ *       num_values past 2^31-1), and NULL offsets, data or output that a page reaches;
+ *     on the device, by one pass over the offsets and validity the pages reach (never `data`), naming the lowest
+ *       failing page: a capacity below the page's bound; then, for the slot errors, with the page's lowest offending
+ *       slot in *bad_pos: a negative offsets[in], offsets that decrease inside the page, a valid value longer than
+ *       2^31-1 bytes.  A page with a slot error is reported for it rather than for its capacity.  *bad_pos is
+ *       AG_NO_ERROR_POS otherwise (may be NULL).
+ *   The device flavour synchronises `s` once, after the checking pass, and leaves the encode stream-ordered: no error
+ *   depends on the data after it.  d_lengths and *d_bad_pos are device memory; *d_bad_pos is written once the checking
+ *   pass has run.  The kernels read d_data in whole aligned 16-byte words, so they may read up to 15 bytes before
+ *   the first and after the last data byte a page reaches, never outside the aligned 16-byte words holding those bytes:
+ *   d_data must be readable there, as a cudaMalloc allocation (256-byte aligned) or a padded Arrow buffer (64 bytes)
+ *   is.  The host flavour stages the offsets and validity the pages reach, then the data bytes they reach, and copies
+ *   back each page's written bytes.  Without a usable GPU both flavours return AG_ERR_CUDA.
+ *   Differences from the reference (DESIGN §2):
+ *     - DELTA_BYTE_ARRAY: every page starts fresh (its first valid value has prefix 0), as parquet-cpp writes it; the
+ *       reference carries the previous page's last value into the next page, which its own decoder refuses;
+ *     - a valid value longer than 2^31-1 bytes is refused; the reference writes uint32(len) unchecked.
+ * ================================================================================= */
+ag_status ag_parquet_byte_array_max_size(int encoding, int64_t num_values, int64_t value_bytes, int64_t* size);
+ag_status ag_parquet_byte_array_encode(int encoding, int offset_width, const void* offsets, const uint8_t* data,
+                                       const uint8_t* valid, const ag_pq_enc_page* pages, int64_t n_pages,
+                                       uint8_t* out, int64_t* lengths, int64_t* bad_pos);
+ag_status ag_parquet_byte_array_encode_dev(int encoding, int offset_width, const void* d_offsets, const uint8_t* d_data,
+                                           const uint8_t* d_valid, const ag_pq_enc_page* pages, int64_t n_pages,
+                                           uint8_t* d_out, int64_t* d_lengths, int64_t* d_bad_pos, ag_stream_t s);
+
+/* ================================================================================= *
  * BOOLEAN, INT32 / INT64 / FLOAT / DOUBLE, INT96 and FIXED_LEN_BYTE_ARRAY pages — the same batch-of-pages contract as
  *   ag_parquet_dict_decode: a host page table, pages in any order, valid == NULL for dense output, pg.out is both the
  *   slot and the bit offset in `valid`, decoded[i] counts page i's slots, and the device flavour synchronises `s`

@@ -149,6 +149,21 @@ def enc_page_table(pages):
     return arr
 
 
+class PqBaChunk(C.Structure):
+    """ag_pq_ba_chunk: one Arrow binary chunk of a BYTE_ARRAY dictionary call (offsets, data, validity in; first out)."""
+    _fields_ = [("offsets", C.c_void_p), ("data", C.c_void_p), ("valid", C.c_void_p), ("offset", C.c_int64),
+                ("length", C.c_int64), ("first", C.c_void_p)]
+
+
+def ba_chunk_table(chunks):
+    """[(offsets, data, valid, offset, length, first), ...] -> ctypes array of ag_pq_ba_chunk."""
+    arr = (PqBaChunk * max(len(chunks), 1))()
+    for k, c in enumerate(chunks):
+        for name, v in zip(("offsets", "data", "valid", "offset", "length", "first"), c):
+            setattr(arr[k], name, v)
+    return arr
+
+
 class PqCompressed(C.Structure):
     """ag_pq_compressed: one compressed Parquet page of a batched decompression (byte offsets and lengths)."""
     _fields_ = [("src", C.c_int64), ("src_len", C.c_int64), ("dst", C.c_int64), ("dst_len", C.c_int64)]
@@ -334,6 +349,8 @@ _SIGS = {
     "ag_parquet_byte_array_max_size": [_i, _i64, _i64, _pi64],
     "ag_parquet_byte_array_encode": [_i, _i, _p, _p, _p, _p, _i64, _p, _p, _p],
     "ag_parquet_byte_array_encode_dev": [_i, _i, _p, _p, _p, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_byte_array_dict_encode": [_i, _p, _i64, _p, _i64, _p, _p, _p, _p],
+    "ag_parquet_byte_array_dict_encode_dev": [_i, _p, _i64, _p, _i64, _p, _p, _p, _p, _p],
     "ag_parquet_snappy_decompress": [_p, _p, _i64, _p, _p],
     "ag_parquet_snappy_decompress_dev": [_p, _p, _i64, _p, _p, _p],
     "ag_parquet_zstd_decompress": [_p, _p, _i64, _p, _p],

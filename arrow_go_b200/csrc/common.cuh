@@ -126,6 +126,21 @@ ag_status unique_dev(int bit_width, const void* vals, const uint8_t* valid, int6
                      int64_t* d_out_len, cudaStream_t st);
 ag_status dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int64_t n_chunks, int null_encoding, void* dict,
                                 uint8_t* dict_valid, int64_t* d_counts, cudaStream_t st);
+// A BYTE_ARRAY dictionary call after pq_encode.cu's checking pass, which counts the valid slots of every kBaTile-slot
+// tile of every chunk.  Device tables.
+constexpr int kBaTile = 1024;              // slots per tile of every BYTE_ARRAY pass
+struct BaDictPlan {
+  int ow;                                  // offset width, 4 or 8
+  const ag_pq_ba_chunk* chunks;            // [n_chunks] (set by ba_dict_encode_dev from h_chunks)
+  const int64_t* row_base;                 // [n_chunks + 1] the first slot of every chunk in the call's numbering (ditto)
+  const int64_t* tile_base;                // [n_chunks + 1] the first tile of every chunk
+  const unsigned long long* tile_cnt;      // tile t of chunk c, at [t + c]: the chunk's valid slots before the tile
+  const int64_t* dense;                    // [n_chunks] the call's valid slots before every chunk
+  int64_t n_chunks, n_tiles, slots, valid;
+};
+// the dictionary kernels of ag_parquet_byte_array_dict_encode_dev; h_chunks and marks are host arrays
+ag_status ba_dict_encode_dev(BaDictPlan p, const ag_pq_ba_chunk* h_chunks, const int64_t* marks, int64_t n_marks, uint32_t* indices,
+                             int64_t* mark_counts, int64_t* counts, cudaStream_t st);
 // run_end.cu
 ag_status run_end_count_dev(int type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n, int64_t* d_counts, cudaStream_t st);
 ag_status run_end_encode_dev(int type, int run_end_type, const void* vals, const uint8_t* valid, int64_t offset, int64_t n,
@@ -385,6 +400,33 @@ __device__ __forceinline__ void store_bool_words(uint32_t* out, uint32_t* out_va
     bitmap_store32_masked(out + w, dbits, m);
     if (out_valid) bitmap_store32_masked(out_valid + w, vbits, m);
   }
+}
+
+// last page p with base[p] <= tile (pages with no tiles share their base with the next page)
+__device__ __forceinline__ int64_t find_page(const int64_t* base, int64_t n_pages, int64_t tile) {
+  int64_t lo = 0, hi = n_pages - 1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (base[mid] <= tile) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+using u128 = unsigned __int128;
+
+__device__ __forceinline__ u128 ld16(const uint8_t* p) {
+  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
+  return (u128)v.x | (u128)v.y << 32 | (u128)v.z << 64 | (u128)v.w << 96;
+}
+
+// bytes p[0, k), 1 <= k <= 16, in the low bytes: one or two aligned 16-byte loads shifted into place, touching only
+// the aligned words that hold those bytes
+__device__ __forceinline__ u128 window(const uint8_t* p, int k) {
+  const int sh = (int)(reinterpret_cast<uintptr_t>(p) & 15);
+  const uint8_t* a = p - sh;
+  u128 w = ld16(a) >> (8 * sh);
+  if (sh + k > 16) w |= ld16(a + 16) << (8 * (16 - sh));
+  return k == 16 ? w : w & (((u128)1 << (8 * k)) - 1);
 }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser

@@ -25,7 +25,7 @@
 //           a key met at a lower row of the same warp cannot be a first appearance, so low-cardinality columns
 //           (the usual dictionary-encoding case) hardly touch the table at all.
 // Roofline: HBM, 8 B/row read once per pass (is_in: one pass; unique: insert + mark + compaction).
-#include "common.cuh"
+#include "host_stage.cuh"
 
 namespace ag {
 
@@ -66,6 +66,30 @@ __device__ __forceinline__ void lower_row(unsigned* p, unsigned seen, unsigned r
   if (seen > row) atomicMin(p, row);
 }
 
+// after each probe step of an insert: true when the insert should give up.  A capped table can fill up completely
+// while the inserts that were in flight when the cap was crossed finish.
+__device__ __forceinline__ bool probe_gives_up(const HashTable& t, unsigned& probes) {
+  if (t.cap == kNoCap || ((++probes & 7u) != 0u)) return false;
+  if (overflowed(t)) return true;
+  // a probe this long at load factor <= 1/2 means the table has filled up behind the counter (the lanes that
+  // created the last keys report them only after their warp step, and a lane spinning here would keep its own
+  // warp from ever reporting): raise the word from here
+  if (probes >= 1024u) { *reinterpret_cast<volatile unsigned*>(&t.special[3]) = 1u; return true; }
+  return false;
+}
+
+// distinct keys so far, one atomic per warp step (a column of all-distinct values would otherwise put 2M atomics on
+// one word before the cap stops it: 2.9 ms); raises the overflow word past the cap.  special[2] is cleared to
+// 0xffffffff = count - 1.  Every lane of the warp calls it.
+__device__ __forceinline__ void count_made(const HashTable& t, bool made, int lane) {
+  if (t.cap == kNoCap) return;
+  const unsigned m = __ballot_sync(0xffffffffu, made);
+  if (lane == 0 && m) {
+    const unsigned c = (unsigned)__popc(m);
+    if (atomicAdd(&t.special[2], c) + 1u + c > t.cap) *reinterpret_cast<volatile unsigned*>(&t.special[3]) = 1u;
+  }
+}
+
 // returns true when this call created the key's slot
 __device__ __forceinline__ bool table_insert(const HashTable& t, unsigned long long key, unsigned row) {
   unsigned long long h = hash_slot(key, t.shift);
@@ -83,14 +107,7 @@ __device__ __forceinline__ bool table_insert(const HashTable& t, unsigned long l
     }
     if (cur == key) { lower_row(&s->first, seen, row); return made; }
     h = (h + 1) & t.mask;
-    // a capped table can fill up completely while the inserts that were in flight when the cap was crossed finish
-    if (t.cap != kNoCap && ((++probes & 7u) == 0u)) {
-      if (overflowed(t)) return false;
-      // a probe this long at load factor <= 1/2 means the table has filled up behind the counter (the lanes that
-      // created the last keys report them only after their warp step, and a lane spinning here would keep its own
-      // warp from ever reporting): raise the word from here
-      if (probes >= 1024u) { *reinterpret_cast<volatile unsigned*>(&t.special[3]) = 1u; return false; }
-    }
+    if (probe_gives_up(t, probes)) return false;
   }
 }
 // lowest row that carried `key`, kNoRow when absent (the table is complete: plain cached loads)
@@ -155,15 +172,7 @@ hash_insert_kernel(const V* __restrict__ vals, const uint8_t* __restrict__ valid
       bool made = false;
       if (go) { made = table_insert(t, key, row); atomicExch(&cache[cs], key); }   // several lanes may share a slot: one whole key wins
       __syncwarp();
-      if (t.cap != kNoCap) {
-        // distinct keys so far, one atomic per warp step (a column of all-distinct values would otherwise put 2M
-        // atomics on one word before the cap stops it: 2.9 ms).  special[2] is cleared to 0xffffffff = count - 1.
-        const unsigned m = __ballot_sync(0xffffffffu, made);
-        if (lane == 0 && m) {
-          const unsigned c = (unsigned)__popc(m);
-          if (atomicAdd(&t.special[2], c) + 1u + c > t.cap) *reinterpret_cast<volatile unsigned*>(&t.special[3]) = 1u;
-        }
-      }
+      count_made(t, made, lane);
     }
   }
 }
@@ -544,7 +553,7 @@ dict_rank_kernel(const HashTable small_t, const HashTable big_t, int encode_null
     if (raw.x == kEmptyKey) continue;
     const unsigned r = first_row_rank(bits, incl, (unsigned)raw.y);
     t.slots[i].pad = r;
-    dict[r] = (V)raw.x;
+    if (dict) dict[r] = (V)raw.x;   // NULL: ranks only (byte-array keys are hashes)
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     const unsigned ones = t.special[0], null_row = t.special[1];
@@ -725,6 +734,363 @@ ag_status dictionary_encode_dev(int bit_width, const ag_dict_chunk* chunks, int6
   return visit_width(bit_width, [&](auto tag) {
     return dictionary_encode_t<typename decltype(tag)::type>(chunks, n_chunks, total, null_encoding, dict, dict_valid, d_counts, st);
   }, [] { return AG_OK; });   // the width was checked above
+}
+
+
+// ---- BYTE_ARRAY dictionaries (DictByteArrayEncoder) -----------------------------------------------------------------
+// The same table, ranks and two-table policy as dictionary_encode, over slots numbered across the chunks of a column
+// chunk.  A slot's key is a 64-bit hash of the value's bytes (never the all-ones pattern), and a key match counts only
+// once the bytes compare equal to the row in Slot::first: that field is only ever lowered to rows whose bytes matched,
+// so it always holds a row carrying the value.  Unequal values with equal hashes probe on.  The creator of a slot
+// publishes its row right after its key CAS, and a lane that finds the key before the row waits for it.
+//   ba_dict_insert_kernel   one 1024-slot tile of a chunk per block step (the checking pass's tiles, whose valid
+//                           counts give every valid slot its dense position); each warp walks 4 steps of 32 slots in
+//                           slot order.  Values up to kBaWarpLen bytes are hashed and compared by their lane, longer ones
+//                           by the whole warp, one at a time.  The hash sums one mix per 16-byte piece, so both ways
+//                           give the same key.  A per-warp cache of values met at lower slots {hash, bytes, table slot}
+//                           answers repeats without touching the table (hits are confirmed by comparing bytes).  Every
+//                           valid slot records its table slot at its dense position (4 B per valid value), so the index
+//                           pass does not hash again.
+//   dict_first_bits_kernel, bit_word_popc_kernel, cumulative_sum, dict_rank_kernel (ranks only): as dictionary_encode.
+//   ba_dict_word_bytes_kernel  len + 4 of the first rows of every bitmap word; its scan and the word-count scan
+//                           answer the marks (ba_dict_marks_kernel: the scans at the mark's word, plus the partial word).
+//                           Scanning per word keeps the scan's length known on the host (the entry count is not).
+//   ba_dict_index_kernel    the rank of every valid slot's table slot, coalesced uint32 at its dense position.
+//   ba_dict_first_kernel    per chunk: the first-row bitmap rebased to the chunk's slot numbering, whole words.
+// Bytes: offsets and validity read by the checking pass and again by the insert pass, data read once (repeats from the
+// cache, L1 or L2), 4 B per valid slot written and read back, indices written, bitmaps ~1 bit per slot.
+
+constexpr int kBaWarpLen = 256;        // longer values are hashed and compared by a whole warp
+constexpr int kBaCacheSlots = 128;     // per warp
+static_assert(kBaTile == kHThreads * kHUnroll, "a warp's 4 steps of 32 slots cover its share of a tile");
+
+struct BaCache {
+  unsigned long long key[kBaCacheSlots];   // kEmptyKey: free
+  const uint8_t* ptr[kBaCacheSlots];
+  uint2 len_slot[kBaCacheSlots];           // {value length, table slot}
+};
+
+// the bytes of global slot `row`
+template <typename O>
+__device__ __forceinline__ const uint8_t* ba_value(const BaDictPlan& p, unsigned row, int64_t& len) {
+  const int64_t c = find_page(p.row_base, p.n_chunks, row);
+  const ag_pq_ba_chunk& ch = p.chunks[c];
+  const O* o = static_cast<const O*>(ch.offsets) + ch.offset + ((int64_t)row - p.row_base[c]);
+  const int64_t o0 = (int64_t)o[0];
+  len = (int64_t)o[1] - o0;
+  return ch.data + o0;
+}
+
+// piece k of a value: its bytes [16k, 16k + 16), zero-padded past the value's end
+__device__ __forceinline__ unsigned long long piece_mix(const uint8_t* p, int64_t len, int64_t k) {
+  const u128 w = window(p + 16 * k, len - 16 * k < 16 ? (int)(len - 16 * k) : 16);
+  return mix64((unsigned long long)w ^ mix64((unsigned long long)(w >> 64) + (unsigned long long)k * 0x9E3779B97F4A7C15ull));
+}
+__device__ __forceinline__ unsigned long long finish_hash(unsigned long long sum, int64_t len) {
+  const unsigned long long h = mix64(sum ^ (unsigned long long)len);
+  return h == kEmptyKey ? 0ull : h;
+}
+__device__ __forceinline__ unsigned long long thread_hash(const uint8_t* p, int64_t len) {
+  unsigned long long s = 0;
+  for (int64_t k = 0; 16 * k < len; ++k) s += piece_mix(p, len, k);
+  return finish_hash(s, len);
+}
+__device__ __forceinline__ unsigned long long warp_hash(const uint8_t* p, int64_t len, int lane) {
+  unsigned long long s = 0;
+  for (int64_t k = lane; 16 * k < len; k += 32) s += piece_mix(p, len, k);
+#pragma unroll
+  for (int m = 16; m; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+  return finish_hash(s, len);
+}
+__device__ __forceinline__ bool thread_equal(const uint8_t* x, const uint8_t* y, int64_t len) {
+  if (x == y) return true;
+  for (int64_t k = 0; k < len; k += 16) {
+    const int c = len - k < 16 ? (int)(len - k) : 16;
+    if (window(x + k, c) != window(y + k, c)) return false;
+  }
+  return true;
+}
+__device__ __forceinline__ bool warp_equal(const uint8_t* x, const uint8_t* y, int64_t len, int lane) {
+  bool ne = false;
+  if (x != y)
+    for (int64_t k = 16 * lane; k < len && !ne; k += 512) {
+      const int c = len - k < 16 ? (int)(len - k) : 16;
+      ne = window(x + k, c) != window(y + k, c);
+    }
+  return !__any_sync(0xffffffffu, ne);
+}
+
+// The table slot of value v (len bytes) at global slot `row`, -1 when a capped table gives up.  WARP: every lane of
+// the warp calls it with the same arguments; lane 0 makes the atomic updates.
+template <bool WARP, typename O>
+__device__ __forceinline__ long long ba_table_insert(const HashTable& t, const BaDictPlan& p, unsigned long long key, unsigned row,
+                                                    const uint8_t* v, int64_t len, bool& made, int lane) {
+  unsigned long long h = hash_slot(key, t.shift);
+  unsigned probes = 0;
+  made = false;
+  while (true) {
+    Slot* s = t.slots + h;
+    const ulonglong2 raw = __ldcg(reinterpret_cast<const ulonglong2*>(s));
+    unsigned long long cur = raw.x;
+    unsigned seen = (unsigned)raw.y;
+    if (cur == kEmptyKey) {
+      if (!WARP || lane == 0) {
+        cur = atomicCAS(&s->key, kEmptyKey, key);
+        if (cur == kEmptyKey) atomicExch(&s->first, row);   // publish the row before anything else
+      }
+      if (WARP) cur = __shfl_sync(0xffffffffu, cur, 0);
+      if (cur == kEmptyKey) { made = true; return (long long)h; }
+      seen = kNoRow;
+    }
+    if (cur == key) {
+      while (seen == kNoRow) seen = *reinterpret_cast<volatile unsigned*>(&s->first);   // its creator is publishing it
+      if (WARP) seen = __shfl_sync(0xffffffffu, seen, 0);
+      int64_t flen;
+      const uint8_t* f = ba_value<O>(p, seen, flen);
+      if (flen == len && (WARP ? warp_equal(f, v, len, lane) : thread_equal(f, v, len))) {
+        if (!WARP || lane == 0) lower_row(&s->first, seen, row);
+        return (long long)h;
+      }
+    }
+    h = (h + 1) & t.mask;
+    bool stop = probe_gives_up(t, probes);
+    if (WARP) stop = __shfl_sync(0xffffffffu, stop, 0);
+    if (stop) return -1;
+  }
+}
+
+// `run_if`: NULL, or the small table's overflow word (the full-size pass)
+template <typename O>
+__global__ void __launch_bounds__(kHThreads, 3)
+ba_dict_insert_kernel(const BaDictPlan p, uint32_t* __restrict__ ref, const HashTable t, const unsigned* __restrict__ run_if) {
+  __shared__ BaCache s_cache[kHWarps];
+  __shared__ unsigned s_cnt[kHWarps];
+  if (run_if && *run_if != 1u) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned lt = (1u << lane) - 1u;
+  BaCache& cache = s_cache[warp];
+  for (int i = lane; i < kBaCacheSlots; i += 32) cache.key[i] = kEmptyKey;
+  __syncwarp();
+  for (int64_t tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    if (__syncthreads_or(t.cap != kNoCap && overflowed(t))) return;   // the small table is being abandoned
+    const int64_t c = find_page(p.tile_base, p.n_chunks, tile);
+    const ag_pq_ba_chunk ch = p.chunks[c];
+    const O* offs = static_cast<const O*>(ch.offsets) + ch.offset;
+    const int64_t j0 = (tile - p.tile_base[c]) * kBaTile + warp * (32 * kHUnroll);   // the warp's first slot in the chunk
+    auto valid_at = [&](int64_t j) { return j < ch.length && (!ch.valid || bit_is_set(ch.valid, ch.offset + j)); };
+    unsigned cnt = 0;
+#pragma unroll
+    for (int k = 0; k < kHUnroll; ++k) cnt += __popc(__ballot_sync(0xffffffffu, valid_at(j0 + 32 * k + lane)));
+    if (lane == 0) s_cnt[warp] = cnt;
+    __syncthreads();   // s_cnt is written again only after the next step's barrier
+    int64_t d = p.dense[c] + (int64_t)p.tile_cnt[tile + c];
+    for (int w = 0; w < warp; ++w) d += s_cnt[w];
+    const unsigned row0 = (unsigned)(p.row_base[c] + j0);
+#pragma unroll 1
+    for (int k = 0; k < kHUnroll; ++k) {
+      const int64_t j = j0 + 32 * k + lane;
+      const bool v = valid_at(j);
+      const unsigned vb = __ballot_sync(0xffffffffu, v);
+      const unsigned row = row0 + 32 * k + lane;
+      const int64_t o0 = v ? (int64_t)offs[j] : 0;
+      const uint8_t* ptr = ch.data + o0;
+      const int64_t len = v ? (int64_t)offs[j + 1] - o0 : 0;
+      unsigned long long key = 0;
+      long long slot = -1;
+      bool hit = false, made = false;
+      int cs = 0;
+      if (v && len <= kBaWarpLen) {
+        key = thread_hash(ptr, len);
+        cs = warp_cache_slot(key) & (kBaCacheSlots - 1);
+        hit = cache.key[cs] == key && cache.len_slot[cs].x == (unsigned)len && thread_equal(cache.ptr[cs], ptr, len);
+        if (hit) slot = cache.len_slot[cs].y;
+      }
+      for (unsigned m = __ballot_sync(0xffffffffu, v && len > kBaWarpLen); m; m &= m - 1) {   // long values, one at a time
+        const int src = __ffs(m) - 1;
+        const uint8_t* q = reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(ptr), src));
+        const int64_t ql = __shfl_sync(0xffffffffu, len, src);
+        const unsigned long long qk = warp_hash(q, ql, lane);
+        const int qs = warp_cache_slot(qk) & (kBaCacheSlots - 1);
+        long long qslot = -1;
+        bool qmade = false;
+        const bool qhit = cache.key[qs] == qk && cache.len_slot[qs].x == (unsigned)ql && warp_equal(cache.ptr[qs], q, ql, lane);
+        if (qhit) qslot = cache.len_slot[qs].y;
+        else qslot = ba_table_insert<true, O>(t, p, qk, row0 + 32 * k + src, q, ql, qmade, lane);
+        if (lane == src) { key = qk; cs = qs; hit = qhit; slot = qslot; made = qmade; }
+      }
+      __syncwarp();
+      if (v && len <= kBaWarpLen && !hit) slot = ba_table_insert<false, O>(t, p, key, row, ptr, len, made, lane);
+      __syncwarp();
+      // the cache keeps one of the values that went to the table per cache slot (lanes may share a slot)
+      const bool go = v && !hit && slot >= 0;
+      const unsigned same = __match_any_sync(0xffffffffu, go ? cs : kBaCacheSlots + lane);
+      if (go && lane == __ffs(same) - 1) {
+        cache.key[cs] = key;
+        cache.ptr[cs] = ptr;
+        cache.len_slot[cs] = make_uint2((unsigned)len, (unsigned)slot);
+      }
+      if (v && slot >= 0) ref[d + __popc(vb & lt)] = (uint32_t)slot;
+      d += __popc(vb);
+      __syncwarp();   // the cache writes are seen by the next step
+      count_made(t, made, lane);
+    }
+  }
+}
+
+// len + 4 of the first rows of every word of the first-row bitmap
+template <typename O>
+__global__ void __launch_bounds__(kHThreads)
+ba_dict_word_bytes_kernel(const BaDictPlan p, const uint32_t* __restrict__ bits, int64_t n_words, long long* __restrict__ wbytes) {
+  for (int64_t i = (int64_t)blockIdx.x * kHThreads + threadIdx.x; i < n_words; i += (int64_t)gridDim.x * kHThreads) {
+    long long s = 0;
+    for (uint32_t b = bits[i]; b; b &= b - 1) {
+      int64_t len;
+      ba_value<O>(p, (unsigned)(i * 32 + __ffs(b) - 1), len);
+      s += len + 4;
+    }
+    wbytes[i] = s;
+  }
+}
+
+// incl / wscan: inclusive scans of the bitmap words' entries and bytes
+template <typename O>
+__global__ void __launch_bounds__(kHThreads)
+ba_dict_marks_kernel(const BaDictPlan p, const uint32_t* __restrict__ bits, const int* __restrict__ incl,
+                     const long long* __restrict__ wscan, int64_t n_words, const int64_t* __restrict__ marks, int64_t n_marks,
+                     int64_t* __restrict__ mark_counts, int64_t* __restrict__ counts) {
+  for (int64_t j = (int64_t)blockIdx.x * kHThreads + threadIdx.x; j < n_marks; j += (int64_t)gridDim.x * kHThreads) {
+    const int64_t m = marks[j], w = m >> 5;
+    long long e = w ? incl[w - 1] : 0, s = w ? wscan[w - 1] : 0;
+    if (m & 31) {
+      for (uint32_t b = bits[w] & ((1u << (m & 31)) - 1u); b; b &= b - 1) {
+        int64_t len;
+        ba_value<O>(p, (unsigned)(w * 32 + __ffs(b) - 1), len);
+        ++e;
+        s += len + 4;
+      }
+    }
+    mark_counts[2 * j] = e;
+    mark_counts[2 * j + 1] = s;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    counts[0] = incl[n_words - 1];
+    counts[1] = wscan[n_words - 1] - 4ll * incl[n_words - 1];
+    counts[2] = p.valid;
+  }
+}
+
+__global__ void __launch_bounds__(kHThreads)
+ba_dict_index_kernel(const HashTable small_t, const HashTable big_t, const uint32_t* __restrict__ ref, int64_t n, uint32_t* __restrict__ out) {
+  const HashTable t = live_table(small_t, big_t);
+  for (int64_t i = (int64_t)blockIdx.x * kHThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kHThreads)
+    __stcs(out + i, t.slots[__ldcs(ref + i)].pad);
+}
+
+// words [offset / 32, ceil((offset + length) / 32)) of a chunk's `first`: global bit row + i - offset at chunk slot i
+__global__ void __launch_bounds__(kHThreads)
+ba_dict_first_kernel(const uint32_t* __restrict__ bits, int64_t n_words, int64_t row, int64_t offset, int64_t length, uint32_t* __restrict__ first) {
+  const int64_t w0 = offset >> 5, w1 = (offset + length + 31) >> 5;
+  auto word = [&](int64_t i) { return i >= 0 && i < n_words ? bits[i] : 0u; };
+  for (int64_t w = w0 + (int64_t)blockIdx.x * kHThreads + threadIdx.x; w < w1; w += (int64_t)gridDim.x * kHThreads) {
+    const int64_t g = row + (w << 5) - offset;        // global slot of the word's bit 0 (negative before the chunk)
+    const uint32_t x = __funnelshift_r(word(g >> 5), word((g >> 5) + 1), (int)(g & 31));
+    const int64_t a = offset - (w << 5), b = offset + length - (w << 5);
+    first[w] = x & bit_range_mask(a > 0 ? (int)a : 0, b < 32 ? (int)b : 32);
+  }
+}
+
+template <typename O>
+static ag_status ba_dict_encode_t(BaDictPlan p, const ag_pq_ba_chunk* h_chunks, const int64_t* marks, int64_t n_marks, uint32_t* indices,
+                                  int64_t* mark_counts, int64_t* counts, cudaStream_t st) {
+  const int64_t total = p.slots;
+  const bool two = total > g_unique_small_rows.load(std::memory_order_relaxed);
+  const unsigned long long small_slots = (unsigned long long)g_unique_small_slots.load(std::memory_order_relaxed);
+  const int64_t n_words = (total + 31) / 32;
+  TableMem small_t, big_t;
+  TableImage img(st);
+  void* scratch = nullptr;
+  ag_status rc = AG_OK;
+  do {
+    std::vector<int64_t> rb((size_t)p.n_chunks + 1, 0);
+    for (int64_t c = 0; c < p.n_chunks; ++c) rb[(size_t)c + 1] = rb[(size_t)c] + h_chunks[c].length;
+    const size_t o_rb = img.add(rb), o_marks = img.add(std::vector<int64_t>(marks, marks + n_marks));
+    const size_t o_ch = img.add(std::vector<ag_pq_ba_chunk>(h_chunks, h_chunks + p.n_chunks));
+    if ((rc = img.upload("byte_array_dict_encode")) != AG_OK) break;
+    p.row_base = img.at<int64_t>(o_rb);
+    p.chunks = img.at<ag_pq_ba_chunk>(o_ch);
+    if (two) rc = small_t.alloc(0, small_slots, (unsigned)(small_slots / 2), st);
+    else rc = small_t.alloc(p.valid, 1024, kNoCap, st);
+    if (rc != AG_OK) break;
+    if ((rc = small_t.clear(st)) != AG_OK) break;
+    if (two && (rc = big_t.alloc(p.valid, 1024, kNoCap, st)) != AG_OK) break;
+    // first-row bitmap | word popcounts | their scan | scan state | word bytes | their scan | scan state | table slots
+    Carve sc;
+    const size_t o_bits = sc.take((size_t)n_words * 4), o_cnt = sc.take((size_t)n_words * 4), o_incl = sc.take((size_t)n_words * 4);
+    const size_t o_st = sc.take(64), o_wb = sc.take((size_t)n_words * 8), o_ws = sc.take((size_t)n_words * 8), o_st2 = sc.take(64);
+    const size_t o_ref = sc.take((size_t)p.valid * 4);
+    if ((rc = dev_alloc_async(&scratch, sc.size, st)) != AG_OK) break;
+    char* d = static_cast<char*>(scratch);
+    uint32_t* bits = reinterpret_cast<uint32_t*>(d + o_bits);
+    int* wcnt = reinterpret_cast<int*>(d + o_cnt);
+    int* incl = reinterpret_cast<int*>(d + o_incl);
+    long long* wb = reinterpret_cast<long long*>(d + o_wb);
+    long long* ws = reinterpret_cast<long long*>(d + o_ws);
+    uint32_t* ref = reinterpret_cast<uint32_t*>(d + o_ref);
+    if (cudaMemsetAsync(bits, 0, (size_t)n_words * 4, st) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "memset", __FILE__, __LINE__); break; }
+    // inserts: every chunk into the small table, then (only when it overflowed) every chunk into the full-size one
+    const int grid = grid_one_wave(ba_dict_insert_kernel<O>, kHThreads, p.n_tiles);
+    for (int pass = 0; pass < (two ? 2 : 1) && rc == AG_OK; ++pass) {
+      const unsigned* raised = pass ? small_t.t.special + 3 : nullptr;
+      if (pass && (rc = big_t.clear(st, raised)) != AG_OK) break;
+      ba_dict_insert_kernel<O><<<grid, kHThreads, 0, st>>>(p, ref, pass ? big_t.t : small_t.t, raised);
+      rc = check_launch("ba_dict_insert_kernel");
+    }
+    if (rc != AG_OK) break;
+    const int64_t max_slots = (int64_t)((two ? big_t.t.mask : small_t.t.mask) + 1);
+    const int slot_grid = grid_for(max_slots, kHThreads * 4, 8), word_grid = grid_for(n_words, kHThreads * 4, 8);
+    dict_first_bits_kernel<<<slot_grid, kHThreads, 0, st>>>(small_t.t, big_t.t, 0, bits);
+    if ((rc = check_launch("dict_first_bits_kernel")) != AG_OK) break;
+    bit_word_popc_kernel<<<word_grid, kHThreads, 0, st>>>(bits, n_words, wcnt);
+    if ((rc = check_launch("bit_word_popc_kernel")) != AG_OK) break;
+    if ((rc = cumulative_sum_state_init(d + o_st, AG_TYPE_INT32, nullptr, st)) != AG_OK) break;
+    if ((rc = cumulative_sum_dev(AG_TYPE_INT32, wcnt, nullptr, 0, n_words, 0, 0, incl, nullptr, 0, d + o_st, nullptr, st)) != AG_OK) break;
+    dict_rank_kernel<unsigned long long><<<slot_grid, kHThreads, 0, st>>>(small_t.t, big_t.t, 0, bits, incl, n_words, nullptr, nullptr, counts);
+    if ((rc = check_launch("dict_rank_kernel")) != AG_OK) break;
+    ba_dict_word_bytes_kernel<O><<<word_grid, kHThreads, 0, st>>>(p, bits, n_words, wb);
+    if ((rc = check_launch("ba_dict_word_bytes_kernel")) != AG_OK) break;
+    if ((rc = cumulative_sum_state_init(d + o_st2, AG_TYPE_INT64, nullptr, st)) != AG_OK) break;
+    if ((rc = cumulative_sum_dev(AG_TYPE_INT64, wb, nullptr, 0, n_words, 0, 0, ws, nullptr, 0, d + o_st2, nullptr, st)) != AG_OK) break;
+    ba_dict_marks_kernel<O><<<grid_for(n_marks, kHThreads, 8), kHThreads, 0, st>>>(p, bits, incl, ws, n_words, img.at<int64_t>(o_marks),
+                                                                                   n_marks, mark_counts, counts);
+    if ((rc = check_launch("ba_dict_marks_kernel")) != AG_OK) break;
+    if (p.valid > 0) {
+      ba_dict_index_kernel<<<grid_for(p.valid, kHThreads * 4, 8), kHThreads, 0, st>>>(small_t.t, big_t.t, ref, p.valid, indices);
+      if ((rc = check_launch("ba_dict_index_kernel")) != AG_OK) break;
+    }
+    for (int64_t c = 0; c < p.n_chunks && rc == AG_OK; ++c) {
+      const ag_pq_ba_chunk& ch = h_chunks[c];
+      if (ch.length == 0) continue;
+      const int64_t words = (ch.offset + ch.length + 31) / 32 - ch.offset / 32;
+      ba_dict_first_kernel<<<grid_for(words, kHThreads, 8), kHThreads, 0, st>>>(bits, n_words, rb[(size_t)c], ch.offset, ch.length,
+                                                                                reinterpret_cast<uint32_t*>(ch.first));
+      rc = check_launch("ba_dict_first_kernel");
+    }
+  } while (0);
+  if (scratch) cudaFreeAsync(scratch, st);
+  small_t.release(st);
+  big_t.release(st);
+  return rc;
+}
+
+ag_status ba_dict_encode_dev(BaDictPlan p, const ag_pq_ba_chunk* h_chunks, const int64_t* marks, int64_t n_marks, uint32_t* indices,
+                             int64_t* mark_counts, int64_t* counts, cudaStream_t st) {
+  if (p.slots == 0) {   // every mark is 0
+    AG_CUDA_TRY(cudaMemsetAsync(counts, 0, 3 * sizeof(int64_t), st));
+    if (n_marks) AG_CUDA_TRY(cudaMemsetAsync(mark_counts, 0, (size_t)n_marks * 2 * sizeof(int64_t), st));
+    return AG_OK;
+  }
+  return p.ow == 4 ? ba_dict_encode_t<int32_t>(p, h_chunks, marks, n_marks, indices, mark_counts, counts, st)
+                   : ba_dict_encode_t<int64_t>(p, h_chunks, marks, n_marks, indices, mark_counts, counts, st);
 }
 
 }  // namespace ag

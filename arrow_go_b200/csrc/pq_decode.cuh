@@ -111,16 +111,6 @@ struct PqArgs {
   void* out;
 };
 
-__device__ __forceinline__ int64_t find_page(const int64_t* base, int64_t n_pages, int64_t tile) {
-  // last page p with base[p] <= tile (pages with no tiles share their base with the next page)
-  int64_t lo = 0, hi = n_pages - 1;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi + 1) >> 1;
-    if (base[mid] <= tile) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // valid bits per tile of every page: one warp per tile, 32 windows of 32 bits
 __global__ void __launch_bounds__(kRleThreads)
 pq_tile_count_kernel(PqArgs a) {

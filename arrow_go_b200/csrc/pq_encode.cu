@@ -541,13 +541,10 @@ ag_status encode_host(const ag_pq_enc_page* pages, int64_t n_pages, const void* 
 }
 
 // ------------------------------------------------------------------------------- BYTE_ARRAY value sections ----
-constexpr int kBaTile = 1024;                       // slots per tile of every BYTE_ARRAY pass
 constexpr int kBaItems = kBaTile / kPqThreads;      // 4 consecutive slots per thread
 constexpr unsigned long long kBaOk = ~0ull;         // error word of a page that passes
 constexpr unsigned long long kBaCap = ~0ull - 1;    // capacity below the bound; every slot error is lower
 enum BaErr { kBaNegFirst = 0, kBaDecreasing = 1, kBaTooLong = 2 };   // slot errors: word = slot * 4 + kind
-
-using u128 = unsigned __int128;
 
 struct BaArgs {
   const ag_pq_enc_page* pages;
@@ -572,6 +569,7 @@ struct BaArgs {
   int64_t* sec;                   // [n_pages] the byte section's offset from the page's out
   uint8_t* out;
   int64_t* lengths;               // may be NULL
+  const ag_pq_ba_chunk* chunks;   // NULL, or per page its own offsets and validity (a dictionary call's chunks)
 };
 
 __host__ __device__ __forceinline__ int64_t ba_bound(int enc, int64_t n, int64_t span) {
@@ -581,21 +579,6 @@ __host__ __device__ __forceinline__ int64_t ba_bound(int enc, int64_t n, int64_t
 
 template <typename O>
 __device__ __forceinline__ int64_t off_at(const void* o, int64_t i) { return (int64_t) static_cast<const O*>(o)[i]; }
-
-__device__ __forceinline__ u128 ld16(const uint8_t* p) {
-  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
-  return (u128)v.x | (u128)v.y << 32 | (u128)v.z << 64 | (u128)v.w << 96;
-}
-
-// bytes p[0, k), 1 <= k <= 16, in the low bytes: one or two aligned 16-byte loads shifted into place, touching only
-// the aligned words that hold those bytes
-__device__ __forceinline__ u128 window(const uint8_t* p, int k) {
-  const int sh = (int)(reinterpret_cast<uintptr_t>(p) & 15);
-  const uint8_t* a = p - sh;
-  u128 w = ld16(a) >> (8 * sh);
-  if (sh + k > 16) w |= ld16(a + 16) << (8 * (16 - sh));
-  return k == 16 ? w : w & (((u128)1 << (8 * k)) - 1);
-}
 
 // the length of the common prefix of x[0, m) and y[0, m), 16 bytes per step
 __device__ __forceinline__ int64_t common_prefix(const uint8_t* x, const uint8_t* y, int64_t m) {
@@ -611,7 +594,7 @@ __device__ __forceinline__ int64_t common_prefix(const uint8_t* x, const uint8_t
 }
 
 // the tile of block `t`: its page, the page's slot of the thread's first item, the offsets of the thread's items and
-// their validity (false past the page)
+// their validity (false past the page).  `offsets` / `valid`: the page's arrays.
 struct BaSlots {
   int64_t p, j0;
   ag_pq_enc_page pg;
@@ -620,15 +603,15 @@ struct BaSlots {
 };
 
 template <typename O>
-__device__ __forceinline__ void ba_slots(const BaArgs& a, int64_t t, BaSlots& s) {
+__device__ __forceinline__ void ba_slots(const BaArgs& a, int64_t t, BaSlots& s, const void* offsets, const uint8_t* valid) {
   s.p = find_page(a.tile_base, a.n_pages, t);
   s.pg = a.pages[s.p];
   s.j0 = (t - a.tile_base[s.p]) * kBaTile + threadIdx.x * kBaItems;
 #pragma unroll
   for (int q = 0; q <= kBaItems; ++q) {
     const int64_t j = s.j0 + q;
-    s.o[q] = j <= s.pg.num_values ? off_at<O>(a.offsets, s.pg.in + j) : 0;
-    if (q < kBaItems) s.v[q] = j < s.pg.num_values && (!a.valid || bit_is_set(a.valid, s.pg.in + j));
+    s.o[q] = j <= s.pg.num_values ? off_at<O>(offsets, s.pg.in + j) : 0;
+    if (q < kBaItems) s.v[q] = j < s.pg.num_values && (!valid || bit_is_set(valid, s.pg.in + j));
   }
 }
 
@@ -641,13 +624,19 @@ ba_check_kernel(BaArgs a) {
   __shared__ long long wl[kPqThreads / 32];
   for (int64_t p = (int64_t)blockIdx.x * kPqThreads + threadIdx.x; p < a.n_pages; p += (int64_t)gridDim.x * kPqThreads) {
     const ag_pq_enc_page pg = a.pages[p];
-    const int64_t span = pg.num_values ? off_at<O>(a.offsets, pg.in + pg.num_values) - off_at<O>(a.offsets, pg.in) : 0;
+    const void* o = a.chunks ? a.chunks[p].offsets : a.offsets;
+    const int64_t span = pg.num_values ? off_at<O>(o, pg.in + pg.num_values) - off_at<O>(o, pg.in) : 0;
     if (pg.capacity < ba_bound(a.enc, pg.num_values, span)) atomicMin(a.err + p, kBaCap);
   }
   if (blockIdx.x >= a.n_tiles) return;
   const int64_t t = blockIdx.x;
   BaSlots s;
-  ba_slots<O>(a, t, s);
+  if (a.chunks) {
+    const ag_pq_ba_chunk& ch = a.chunks[find_page(a.tile_base, a.n_pages, t)];
+    ba_slots<O>(a, t, s, ch.offsets, ch.valid);
+  } else {
+    ba_slots<O>(a, t, s, a.offsets, a.valid);
+  }
   long long c = 0, b = 0, lst = -1;
   unsigned long long bad = kBaOk;
 #pragma unroll
@@ -724,7 +713,7 @@ ba_dense_kernel(BaArgs a) {
   __shared__ long long wl[kPqThreads / 32];
   const int64_t t = blockIdx.x;
   BaSlots s;
-  ba_slots<O>(a, t, s);
+  ba_slots<O>(a, t, s, a.offsets, a.valid);
   auto lsum = [](long long x, long long y) { return x + y; };
   auto lmax = [](long long x, long long y) { return x > y ? x : y; };
   long long c = 0, lst = -1, tot;
@@ -785,7 +774,7 @@ ba_bytes_kernel(BaArgs a) {
   const int64_t t = blockIdx.x;
   const int tid = threadIdx.x;
   BaSlots s;
-  ba_slots<O>(a, t, s);
+  ba_slots<O>(a, t, s, a.offsets, a.valid);
   auto lsum = [](long long x, long long y) { return x + y; };
   long long tot;
   int64_t r = 0;
@@ -886,7 +875,9 @@ struct BaCall {
       : fn(f), enc(e), ow(w), pages(p), n_pages(n), st(s), img(s) {}
   ~BaCall() { dev_free_async(vals, st); dev_free_async(scratch, st); }
 
-  ag_status check(const void* d_off, const uint8_t* d_valid, int64_t* d_bad_pos, int64_t* h_bad) {
+  // chunks: NULL, or a HOST array of one dictionary chunk per page, which then brings its own offsets and validity;
+  // errors name the chunk and give the slot in the call's numbering across the chunks
+  ag_status check(const void* d_off, const uint8_t* d_valid, int64_t* d_bad_pos, int64_t* h_bad, const ag_pq_ba_chunk* chunks = nullptr) {
     std::vector<int64_t> tb((size_t)n_pages + 1, 0), sb((size_t)n_pages + 1, 0);
     for (int64_t i = 0; i < n_pages; ++i) {
       tb[(size_t)i + 1] = tb[(size_t)i] + (pages[i].num_values + kBaTile - 1) / kBaTile;
@@ -897,6 +888,7 @@ struct BaCall {
     const size_t o_pages = img.add(std::vector<ag_pq_enc_page>(pages, pages + n_pages));
     const size_t o_tb = img.add(tb), o_sb = img.add(sb);
     const size_t o_err = img.add(std::vector<unsigned long long>((size_t)n_pages, kBaOk));
+    const size_t o_chunks = chunks ? img.add(std::vector<ag_pq_ba_chunk>(chunks, chunks + n_pages)) : 0;
     AG_TRY(img.upload(fn));
     Carve sc;
     const size_t o_cnt = sc.take((size_t)(n_tiles + n_pages) * 8), o_bytes = sc.take((size_t)(n_tiles + n_pages) * 8);
@@ -910,7 +902,8 @@ struct BaCall {
                nullptr, d_valid, enc, img.at<unsigned long long>(o_err), reinterpret_cast<unsigned long long*>(d + o_cnt),
                reinterpret_cast<unsigned long long*>(d + o_bytes), reinterpret_cast<long long*>(d + o_last),
                reinterpret_cast<int64_t*>(d + o_dense), nullptr, nullptr, reinterpret_cast<ag_pq_enc_page*>(d + o_tab),
-               reinterpret_cast<int64_t*>(d + o_slen), reinterpret_cast<int64_t*>(d + o_sec), nullptr, nullptr};
+               reinterpret_cast<int64_t*>(d + o_slen), reinterpret_cast<int64_t*>(d + o_sec), nullptr, nullptr,
+               chunks ? img.at<ag_pq_ba_chunk>(o_chunks) : nullptr};
     const unsigned grid = (unsigned)std::max<int64_t>(n_tiles, (n_pages + kPqThreads - 1) / kPqThreads);
     if (ow == 4) ba_check_kernel<int32_t><<<grid, kPqThreads, 0, st>>>(a);
     else ba_check_kernel<int64_t><<<grid, kPqThreads, 0, st>>>(a);
@@ -932,16 +925,21 @@ struct BaCall {
     int64_t page = -1;
     for (int64_t i = 0; i < n_pages && page < 0; ++i) if (err[(size_t)i] != kBaOk) page = i;
     const unsigned long long w = page < 0 ? kBaOk : err[(size_t)page];
-    const int64_t bad = page < 0 || w == kBaCap ? (int64_t)AG_NO_ERROR_POS : (int64_t)(w >> 2);
+    int64_t bad = page < 0 || w == kBaCap ? (int64_t)AG_NO_ERROR_POS : (int64_t)(w >> 2);
+    if (chunks && bad != (int64_t)AG_NO_ERROR_POS) {
+      bad -= chunks[page].offset;
+      for (int64_t c = 0; c < page; ++c) bad += chunks[c].length;
+    }
     if (h_bad) *h_bad = bad;
     if (d_bad_pos) AG_TRY(h2d(d_bad_pos, &bad, 8, st));
     if (page < 0) return AG_OK;
+    const char* unit = chunks ? "chunk" : "page";
     const long long pl = (long long)page, sl = (long long)bad;
     if (w == kBaCap) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: capacity %lld below the bound for its %lld values and their bytes", fn, pl,
                              (long long)pages[page].capacity, (long long)pages[page].num_values);
-    if ((w & 3) == kBaNegFirst) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: negative offset at slot %lld", fn, pl, sl);
-    if ((w & 3) == kBaDecreasing) AG_FAIL(AG_ERR_INVALID, "%s: page %lld: offsets decrease after slot %lld", fn, pl, sl);
-    AG_FAIL(AG_ERR_INVALID, "%s: page %lld: value at slot %lld longer than 2^31-1 bytes", fn, pl, sl);
+    if ((w & 3) == kBaNegFirst) AG_FAIL(AG_ERR_INVALID, "%s: %s %lld: negative offset at slot %lld", fn, unit, pl, sl);
+    if ((w & 3) == kBaDecreasing) AG_FAIL(AG_ERR_INVALID, "%s: %s %lld: offsets decrease after slot %lld", fn, unit, pl, sl);
+    AG_FAIL(AG_ERR_INVALID, "%s: %s %lld: value at slot %lld longer than 2^31-1 bytes", fn, unit, pl, sl);
   }
 
   ag_status encode(const uint8_t* d_data, uint8_t* d_out, int64_t* d_lengths) {
@@ -991,6 +989,57 @@ struct BaCall {
     return check_launch("ba_bytes_kernel");
   }
 };
+
+// ------------------------------------------------------------------------------- BYTE_ARRAY dictionaries ----
+// The host checks of a dictionary call (before the device is touched); *slots: the call's slots.
+ag_status check_ba_dict_call(const char* fn, int ow, const ag_pq_ba_chunk* chunks, int64_t n_chunks, const int64_t* marks, int64_t n_marks,
+                             const void* indices, const int64_t* mark_counts, const int64_t* counts, int64_t* slots) {
+  if (ow != 4 && ow != 8) AG_FAIL(AG_ERR_INVALID, "%s: offset_width must be 4 or 8, got %d", fn, ow);
+  if (n_chunks < 0 || (n_chunks > 0 && !chunks)) AG_FAIL(AG_ERR_INVALID, "%s: bad chunk table", fn);
+  int64_t total = 0;
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_pq_ba_chunk& ch = chunks[c];
+    if (ch.offset < 0 || ch.length < 0) AG_FAIL(AG_ERR_INVALID, "%s: chunk %lld: negative offset or length", fn, (long long)c);
+    if (ch.length == 0) continue;
+    if (!ch.offsets || !ch.data || !ch.first) AG_FAIL(AG_ERR_INVALID, "%s: chunk %lld: NULL offsets, data or first bitmap", fn, (long long)c);
+    if (reinterpret_cast<uintptr_t>(ch.first) & 3) AG_FAIL(AG_ERR_INVALID, "%s: chunk %lld: the first bitmap must be 4-byte aligned", fn, (long long)c);
+    if (ch.length > INT_MAX - total) AG_FAIL(AG_ERR_NOT_IMPLEMENTED, "%s: more than 2^31-1 slots per call", fn);
+    total += ch.length;
+  }
+  if (n_marks < 0 || (n_marks > 0 && (!marks || !mark_counts))) AG_FAIL(AG_ERR_INVALID, "%s: bad mark table", fn);
+  for (int64_t j = 0; j < n_marks; ++j)
+    if (marks[j] < 0 || marks[j] > total)
+      AG_FAIL(AG_ERR_INVALID, "%s: mark %lld at slot %lld outside 0..%lld", fn, (long long)j, (long long)marks[j], (long long)total);
+  if (!counts) AG_FAIL(AG_ERR_INVALID, "%s: NULL counts", fn);
+  if (total > 0 && !indices) AG_FAIL(AG_ERR_INVALID, "%s: NULL indices", fn);
+  *slots = total;
+  return AG_OK;
+}
+
+// One dictionary call over device chunks: the checking pass over every chunk as a page of its own arrays (one
+// synchronisation; it never reads `data`), then `checked` (which may still fill in the chunks' data), then hash.cu's
+// dictionary kernels.
+template <typename Checked>
+ag_status ba_dict_call(const char* fn, int ow, const ag_pq_ba_chunk* chunks, int64_t n_chunks, int64_t slots, const int64_t* marks,
+                       int64_t n_marks, uint32_t* indices, int64_t* mark_counts, int64_t* counts, int64_t* d_bad_pos, int64_t* h_bad,
+                       cudaStream_t st, Checked checked) {
+  if (slots == 0) {
+    if (h_bad) *h_bad = AG_NO_ERROR_POS;
+    static const int64_t kNoPos = AG_NO_ERROR_POS;
+    if (d_bad_pos) AG_TRY(h2d(d_bad_pos, &kNoPos, 8, st));
+    AG_TRY(checked((int64_t)0));
+    return ba_dict_encode_dev(BaDictPlan{ow, nullptr, nullptr, nullptr, nullptr, nullptr, n_chunks, 0, 0, 0}, chunks, marks, n_marks,
+                              indices, mark_counts, counts, st);
+  }
+  std::vector<ag_pq_enc_page> pages((size_t)n_chunks);
+  for (int64_t c = 0; c < n_chunks; ++c) pages[(size_t)c] = ag_pq_enc_page{chunks[c].offset, chunks[c].length, 0, INT64_MAX};
+  // DELTA_LENGTH_BYTE_ARRAY: the checking pass that also finds every page's (chunk's) first dense slot
+  BaCall c(fn, AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY, ow, pages.data(), n_chunks, st);
+  AG_TRY(c.check(nullptr, nullptr, d_bad_pos, h_bad, chunks));
+  AG_TRY(checked(c.total));
+  const BaDictPlan p{ow, nullptr, nullptr, c.a.tile_base, c.a.cnt, c.a.dense, n_chunks, c.a.n_tiles, slots, c.total};
+  return ba_dict_encode_dev(p, chunks, marks, n_marks, indices, mark_counts, counts, st);
+}
 
 }  // namespace
 
@@ -1128,6 +1177,83 @@ ag_status ag_parquet_byte_array_encode(int encoding, int offset_width, const voi
   AG_TRY(sync(cs));
   for (int64_t i = 0; i < n_pages; ++i) AG_TRY(d2h(out + pages[i].out, d + o_out + pages[i].out, (size_t)len[(size_t)i], cs));
   if (lengths) memcpy(lengths, len.data(), (size_t)n_pages * 8);
+  return sync(cs);
+}
+
+ag_status ag_parquet_byte_array_dict_encode_dev(int offset_width, const ag_pq_ba_chunk* chunks, int64_t n_chunks, const int64_t* marks,
+                                                int64_t n_marks, uint32_t* d_indices, int64_t* d_mark_counts, int64_t* d_counts,
+                                                int64_t* d_bad_pos, ag_stream_t s) {
+  const char* fn = "byte_array_dict_encode";
+  int64_t slots;
+  AG_TRY(check_ba_dict_call(fn, offset_width, chunks, n_chunks, marks, n_marks, d_indices, d_mark_counts, d_counts, &slots));
+  AG_TRY(ensure_init());
+  return ba_dict_call(fn, offset_width, chunks, n_chunks, slots, marks, n_marks, d_indices, d_mark_counts, d_counts, d_bad_pos, nullptr,
+                      resolve_stream(s), [](int64_t) { return AG_OK; });
+}
+
+ag_status ag_parquet_byte_array_dict_encode(int offset_width, const ag_pq_ba_chunk* chunks, int64_t n_chunks, const int64_t* marks,
+                                            int64_t n_marks, uint32_t* indices, int64_t* mark_counts, int64_t* counts, int64_t* bad_pos) {
+  const char* fn = "byte_array_dict_encode";
+  if (bad_pos) *bad_pos = AG_NO_ERROR_POS;
+  int64_t slots;
+  AG_TRY(check_ba_dict_call(fn, offset_width, chunks, n_chunks, marks, n_marks, indices, mark_counts, counts, &slots));
+  AG_TRY(ensure_init());
+  CallStream cs; AG_TRY(cs.acquire());
+  Temps t(cs);
+  // Each chunk's offsets, validity bytes, first words and (once the checking pass has passed) data are staged at
+  // pointers moved back by their first element, so the kernels see the chunk's own slot numbering.  The data staged is
+  // [offsets[offset], offsets[offset + length]), which holds every value once the offsets are checked.
+  const int ow = offset_width;
+  std::vector<ag_pq_ba_chunk> dc((size_t)n_chunks);
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_pq_ba_chunk& ch = chunks[c];
+    ag_pq_ba_chunk& d = dc[(size_t)c];
+    d = ch;
+    if (ch.length == 0) continue;
+    const int64_t v0 = ch.offset >> 3, nv = ch.valid ? ((ch.offset + ch.length + 7) >> 3) - v0 : 0;
+    const int64_t f0 = ch.offset >> 5, nf = ((ch.offset + ch.length + 31) >> 5) - f0;
+    uint8_t *o, *v = nullptr, *f;
+    AG_TRY(t.alloc_t(&o, (size_t)(ch.length + 1) * ow));
+    AG_TRY(h2d(o, static_cast<const uint8_t*>(ch.offsets) + ch.offset * ow, (size_t)(ch.length + 1) * ow, cs));
+    if (ch.valid) { AG_TRY(t.alloc_t(&v, (size_t)nv)); AG_TRY(h2d(v, ch.valid + v0, (size_t)nv, cs)); }
+    AG_TRY(t.alloc_t(&f, (size_t)nf * 4));
+    d.offsets = o - ch.offset * ow;
+    d.valid = ch.valid ? v - v0 : nullptr;
+    d.data = nullptr;
+    d.first = f - f0 * 4;
+  }
+  Carve sc;
+  const size_t o_idx = sc.take((size_t)slots * 4), o_mc = sc.take((size_t)n_marks * 16), o_cnt = sc.take(24);
+  uint8_t* d;
+  AG_TRY(t.alloc_t(&d, sc.size));
+  int64_t valid = 0;
+  auto stage_data = [&](int64_t nv) {
+    valid = nv;
+    for (int64_t c = 0; c < n_chunks; ++c) {
+      const ag_pq_ba_chunk& ch = chunks[c];
+      if (ch.length == 0) continue;
+      auto off = [&](int64_t i) {
+        return ow == 4 ? (int64_t) static_cast<const int32_t*>(ch.offsets)[i] : static_cast<const int64_t*>(ch.offsets)[i];
+      };
+      const int64_t lo = off(ch.offset), hi = off(ch.offset + ch.length);
+      uint8_t* dd;
+      AG_TRY(t.alloc_t(&dd, (size_t)(hi - lo)));
+      AG_TRY(h2d(dd, ch.data + lo, (size_t)(hi - lo), cs));
+      dc[(size_t)c].data = dd - lo;
+    }
+    return AG_OK;
+  };
+  AG_TRY(ba_dict_call(fn, ow, dc.data(), n_chunks, slots, marks, n_marks, reinterpret_cast<uint32_t*>(d + o_idx),
+                      reinterpret_cast<int64_t*>(d + o_mc), reinterpret_cast<int64_t*>(d + o_cnt), nullptr, bad_pos, cs, stage_data));
+  AG_TRY(d2h(indices, d + o_idx, (size_t)valid * 4, cs));
+  AG_TRY(d2h(mark_counts, d + o_mc, (size_t)n_marks * 16, cs));
+  AG_TRY(d2h(counts, d + o_cnt, 24, cs));
+  for (int64_t c = 0; c < n_chunks; ++c) {
+    const ag_pq_ba_chunk& ch = chunks[c];
+    if (ch.length == 0) continue;
+    const int64_t f0 = ch.offset >> 5, nf = ((ch.offset + ch.length + 31) >> 5) - f0;
+    AG_TRY(d2h(ch.first + f0 * 4, dc[(size_t)c].first + f0 * 4, (size_t)nf * 4, cs));
+  }
   return sync(cs);
 }
 

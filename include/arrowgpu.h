@@ -1050,7 +1050,8 @@ ag_status ag_parquet_byte_array_decode_dev(int encoding, int offset_width, const
  *   need not be contiguous.  lengths[i] (may be NULL) receives the bytes page i wrote.
  *     AG_PQ_ENC_PLAIN: PlainByteArrayEncoder.Put / PutSpaced (parquet/internal/encoding/byte_array_encoder.go:41-89):
  *       each valid value as a 4-byte little-endian length and its bytes.  Also the dictionary page of a string
- *       dictionary, with valid = NULL.
+ *       dictionary: with valid = NULL over the entries, or over a column's slots with valid = the `first` bitmap of
+ *       ag_parquet_byte_array_dict_encode.
  *     AG_PQ_ENC_DELTA_LENGTH_BYTE_ARRAY: DeltaLengthByteArrayEncoder (delta_length_byte_array.go:44-96): the lengths as
  *       a DELTA_BINARY_PACKED INT32 stream, then the values' bytes back to back.
  *     AG_PQ_ENC_DELTA_BYTE_ARRAY: DeltaByteArrayEncoder (delta_byte_array.go:56-149): the lengths of the prefixes each
@@ -1088,6 +1089,60 @@ ag_status ag_parquet_byte_array_encode(int encoding, int offset_width, const voi
 ag_status ag_parquet_byte_array_encode_dev(int encoding, int offset_width, const void* d_offsets, const uint8_t* d_data,
                                            const uint8_t* d_valid, const ag_pq_enc_page* pages, int64_t n_pages,
                                            uint8_t* d_out, int64_t* d_lengths, int64_t* d_bad_pos, ag_stream_t s);
+
+/* ================================================================================= *
+ * BYTE_ARRAY dictionaries: the memo table of DictByteArrayEncoder (parquet/internal/encoding/byte_array_encoder.go:
+ *   97-135, encoder.go:241-325) over a column chunk of Arrow Binary / String (offset_width 4) or LargeBinary /
+ *   LargeString (offset_width 8) arrays.  Every valid value is keyed on its raw bytes, so the dictionary's entries come in
+ *   order of first appearance; nulls are skipped.
+ *   chunks: a HOST array of n_chunks descriptors in table order, in both flavours.  Slot i of a chunk is bit i of
+ *     `valid` (NULL: every slot valid) and the bytes data[offsets[i] .. offsets[i+1]); the chunk holds slots
+ *     [offset, offset + length).  The slots of all chunks are numbered in turn ("global slots"), at most 2^31-1 of
+ *     them (more is AG_ERR_NOT_IMPLEMENTED), and share one dictionary.
+ *   Outputs:
+ *     indices      one uint32 per valid slot of all chunks, in order: entry k is the k-th distinct value.  This is the
+ *                  input of ag_parquet_rle_encode with AG_PQ_RLE_IN_U32.
+ *     chunk.first  bit i set iff slot i of the chunk is the first valid appearance of its value in the call, in the
+ *                  chunk's own slot numbering.  Written in whole aligned 32-bit words covering [offset, offset + length),
+ *                  with the bits outside those slots cleared: ceil((offset + length) / 32) * 4 bytes, 4-byte aligned.
+ *                  ag_parquet_byte_array_encode(AG_PQ_ENC_PLAIN) with valid = first over the chunk's slots writes the
+ *                  chunk's share of the dictionary page; over a one-chunk column, the whole page.
+ *     counts[3]    the dictionary's entries, the entries' value bytes (sum of len), and the valid slots.
+ *     mark_counts  for every global slot position marks[j] in [0, total slots] (a HOST array; may be NULL when n_marks
+ *                  is 0): [2j] the entries first seen at a slot below marks[j], [2j + 1] their dictEncodedSize (the sum
+ *                  of len + 4: the size of the PLAIN dictionary page).  The dictionary of any prefix of the slots is a
+ *                  prefix of the whole dictionary and the prefix's indices are unchanged, so marks at page ends give
+ *                  each page's index bit width (BitWidth() of the entries so far: 0 for none, 1 for one, else
+ *                  bits.Len32(entries - 1)) and marks at the writer's batch ends give its fallback cut.
+ *   Checks, every one before any output is written:
+ *     on the host, before the device is touched (AG_ERR_INVALID): an unknown offset width; a negative chunk offset or
+ *       length; NULL offsets, data or first of a non-empty chunk, or a first bitmap that is not 4-byte aligned; a mark
+ *       outside [0, total slots]; NULL indices (with slots), counts, or mark_counts (with marks);
+ *     on the device, by one pass over the offsets and validity (never `data`), as ag_parquet_byte_array_encode makes
+ *       them: a negative first offset of a chunk, offsets that decrease, a valid value longer than 2^31-1 bytes.  Each
+ *       is AG_ERR_INVALID naming the chunk, with the lowest offending global slot in *bad_pos (AG_NO_ERROR_POS
+ *       otherwise; may be NULL).
+ *   The device flavour synchronises `s` once, after that pass; the rest is stream-ordered.  d_indices, d_mark_counts,
+ *   d_counts and *d_bad_pos are device memory.  `data` is read in whole aligned 16-byte words under the rule of
+ *   ag_parquet_byte_array_encode.  ag_unique_set_policy applies to the table.  The host flavour stages what the chunks
+ *   reach and copies back indices, every first bitmap, counts and mark_counts.  Without a usable GPU both flavours
+ *   return AG_ERR_CUDA once the host checks pass.
+ * ================================================================================= */
+typedef struct ag_pq_ba_chunk {
+  const void*    offsets;   /* offset_width bytes each; slot i uses offsets[i], offsets[i+1] */
+  const uint8_t* data;
+  const uint8_t* valid;     /* may be NULL */
+  int64_t        offset;    /* first slot of the chunk */
+  int64_t        length;    /* slots */
+  uint8_t*       first;     /* out: first-appearance bitmap */
+} ag_pq_ba_chunk;
+ag_status ag_parquet_byte_array_dict_encode(int offset_width, const ag_pq_ba_chunk* chunks, int64_t n_chunks,
+                                            const int64_t* marks, int64_t n_marks, uint32_t* indices,
+                                            int64_t* mark_counts, int64_t* counts, int64_t* bad_pos);
+ag_status ag_parquet_byte_array_dict_encode_dev(int offset_width, const ag_pq_ba_chunk* chunks, int64_t n_chunks,
+                                                const int64_t* marks, int64_t n_marks, uint32_t* d_indices,
+                                                int64_t* d_mark_counts, int64_t* d_counts, int64_t* d_bad_pos,
+                                                ag_stream_t s);
 
 /* ================================================================================= *
  * BOOLEAN, INT32 / INT64 / FLOAT / DOUBLE, INT96 and FIXED_LEN_BYTE_ARRAY pages — the same batch-of-pages contract as
